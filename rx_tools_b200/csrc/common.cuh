@@ -1,5 +1,6 @@
 // common.cuh — shared helpers of librxb200.so (error plumbing, wrap-safe integer helpers).
 #pragma once
+#include <cuda.h>               // CUtensorMap (types only: the encoder is reached through cudaGetDriverEntryPoint)
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -90,6 +91,12 @@ __device__ __forceinline__ void bulk_load(void *dst, const void *src, uint32_t b
 {
 	asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
 	             ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
+}
+// tensor TMA: one box of a 2-D tensor map at element coordinates (c0, c1) -> shared, completion on the mbarrier
+__device__ __forceinline__ void tensor_load_2d(void *dst, const CUtensorMap *map, int c0, int c1, uint64_t *bar)
+{
+	asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
+	             ::"r"(smem_u32(dst)), "l"(map), "r"(c0), "r"(c1), "r"(smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity)
 {

@@ -30,6 +30,7 @@
 #include <stdlib.h>
 #include <new>
 #include <vector>
+#include <cudaTypedefs.h>        // PFN_cuTensorMapEncodeTiled
 #include "common.cuh"
 
 namespace rxb {
@@ -1751,11 +1752,14 @@ static fm_kernel_fn pick_back_kernel(int ws, int t)
 //   FE 0: per-thread segments (front_item)   FE 1: warp rows with the droop FIR (fm_rows.cuh)   FE 2: rows, no FIR
 #define BAR_FE 2
 #define SPLIT_BE_MAX 128
+// The row front end reads its input through `in_map` (fm_rows.cuh); the segment front end ignores it.
 template <int P, int SPEC, int FE, int TMAX, int MINB>
-__global__ void __launch_bounds__(TMAX, MINB) fm_split_kernel(const FmDev c, const FmCall k)
+__global__ void __launch_bounds__(TMAX, MINB) fm_split_kernel(const FmDev c, const FmCall k, const __grid_constant__ CUtensorMap in_map)
 {
-	extern __shared__ __align__(16) int16_t pcm_s[];       // [2][pcm_cap] PCM buffers, then the row exchange areas
+	// [2][pcm_cap] PCM buffers, then the row exchange areas, then (from the next 1024-byte boundary) the row input rings
+	extern __shared__ __align__(16) int16_t pcm_s[];
 	__shared__ __align__(8) uint64_t s_full[2], s_empty[2];
+	__shared__ __align__(8) uint64_t s_ring_bar[FE == 0 ? 1 : (TMAX / 32) * ROWS_STAGES];
 	__shared__ int s_ticket[2];
 	__shared__ int s_avg[SPLIT_BE_MAX], s_mrun[SPLIT_BE_MAX], s_start[SPLIT_BE_MAX];
 	__shared__ unsigned char s_ok[SPLIT_BE_MAX];
@@ -1766,10 +1770,22 @@ __global__ void __launch_bounds__(TMAX, MINB) fm_split_kernel(const FmDev c, con
 	if (tid == 0) {
 		mbar_init(&s_full[0], n_fe); mbar_init(&s_full[1], n_fe);
 		mbar_init(&s_empty[0], k.be_lanes); mbar_init(&s_empty[1], k.be_lanes);
+		if (FE != 0) {
+			for (int j = 0; j < k.fe_warps * ROWS_STAGES; j++) { mbar_init(&s_ring_bar[j], 1); }
+		}
 	}
 	__syncthreads();
 	const int total_work = k.n_ch * k.n_cta;
 	if (tid < n_fe) {
+		RowRing ring;
+		if (FE != 0) {
+			uint8_t *end = reinterpret_cast<uint8_t *>(pcm_s + 2 * (size_t)k.pcm_cap) + (size_t)k.fe_warps * k.xs_words * sizeof(uint32_t);
+			end += (0u - smem_u32(end)) & 1023u;
+			ring.map = &in_map;
+			ring.buf = end + (size_t)(tid >> 5) * ROWS_STAGES * ROW_BYTES;
+			ring.bar = s_ring_bar + (tid >> 5) * ROWS_STAGES;
+			ring.seq = 0;
+		}
 		for (int i = 0;; i++) {
 			const int b = i & 1;
 			if (i >= 2) { mbar_wait(&s_empty[b], (uint32_t)(((i >> 1) - 1) & 1)); }   // the back end is done with item i-2
@@ -1785,7 +1801,7 @@ __global__ void __launch_bounds__(TMAX, MINB) fm_split_kernel(const FmDev c, con
 			if constexpr (FE == 0) { front_item<P, SPEC>(c, k, it, tid, buf); }
 			else {
 				uint32_t *xs = reinterpret_cast<uint32_t *>(pcm_s + 2 * (size_t)k.pcm_cap) + (size_t)(tid >> 5) * k.xs_words;
-				front_rows<P, FE == 1>(c, k, it, tid >> 5, lane, buf, xs);
+				front_rows<P, FE == 1>(c, k, it, tid >> 5, lane, buf, xs, ring);
 			}
 			mbar_arrive(&s_full[b]);
 		}
@@ -1924,22 +1940,29 @@ static fm_kernel_fn pick_kernel_p(int P, int threads)
 #endif
 }
 
+typedef void (*fm_split_fn)(const FmDev, const FmCall, const CUtensorMap);
+
 // the split kernel with the row front end exists for the wbfm shape with 1..3 packed passes
 // CTA shape of the split kernel (overridable for A/B builds, tools/build_variants.sh): front-end warps, back-end lanes,
 // CTAs per SM the register budget is cut for
-// Two CTAs of 8 + 2 warps: longer items replay less per sample than with smaller CTAs, and one back-end warp per four
-// front-end warps keeps the front end from waiting for PCM buffers.  Not re-tuned on H100.
+// Three CTAs of 4 + 1 warps, ROWS_STAGES = 2.  Every front-end warp's input ring takes 8 KB of shared memory, so
+// fewer front-end warps per CTA leave longer items (less replay per sample).  fm2b (bench.py, 10 steps, two rounds
+// alternating the builds, one H100 80GB HBM3 SXM at a 700 W power limit, SM clock 1980 MHz), Msamples/s:
+//   4 + 1 warps x 3 CTAs 579 / 579    6 + 2 x 2 562 / 563    7 + 2 x 2 549 / 547    6 + 1 x 2 547 / 544
+//   5 + 1 x 3 522 / 516               before the ring (8 + 2 x 2, register loads) 388 / 387
+// and on a 400 W board of the same kind: 6 + 2 x 2 469 / 469, 16 + 4 x 1 416 / 414, 12 + 3 x 1 with 3 stages
+// 412 / 410, before the ring 362 / 364.  The P = 1 and P = 2 shapes share the choice and were not timed.
 #ifndef ROWS_FE_WARPS
-#define ROWS_FE_WARPS 8
+#define ROWS_FE_WARPS 4
 #endif
 #ifndef ROWS_BE_LANES
-#define ROWS_BE_LANES 64
+#define ROWS_BE_LANES 32
 #endif
 #ifndef ROWS_MINB
-#define ROWS_MINB 2
+#define ROWS_MINB 3
 #endif
 #define ROWS_TMAX (ROWS_FE_WARPS * 32 + ROWS_BE_LANES)
-static fm_kernel_fn pick_rows_kernel(int P, int fir_on)
+static fm_split_fn pick_rows_kernel(int P, int fir_on)
 {
 #ifdef RXB_QUICK
 	return (P == 3 && fir_on) ? fm_split_kernel<3, 1, 1, ROWS_TMAX, ROWS_MINB> : nullptr;
@@ -1960,7 +1983,7 @@ static fm_kernel_fn pick_rows_kernel(int P, int fir_on)
 #ifndef SEGS_BE_LANES
 #define SEGS_BE_LANES 128
 #endif
-static fm_kernel_fn pick_segs_kernel(int P, int D, int deemph)
+static fm_split_fn pick_segs_kernel(int P, int D, int deemph)
 {
 #ifdef RXB_QUICK
 	return nullptr;
@@ -2022,8 +2045,8 @@ struct rxb200_fm {
 	int tune_seg, tune_warm;
 	rxb200_fm_stats stats;
 	fm_kernel_fn kern;
-	fm_kernel_fn kern_rows;        // split kernel with the row front end (null: shape not covered)
-	fm_kernel_fn kern_segs;        // split kernel with the segment front end (null: shape not covered)
+	fm_split_fn kern_rows;         // split kernel with the row front end (null: shape not covered)
+	fm_split_fn kern_segs;         // split kernel with the segment front end (null: shape not covered)
 	fm_kernel_fn kern_front;       // stream path: front end alone (SPEC 4), PCM to global memory; fm_back_kernel follows
 	int16_t *d_pcm; size_t d_pcm_cap;   // its PCM scratch, int16 elements
 	size_t stream_min; int stream_piece, stream_win, stream_t, stream_warm_a;
@@ -2319,6 +2342,37 @@ static bool fm_rows_shape_ok(const rxb200_fm *h, size_t n_int16, size_t chunk_in
 	return chunk % ROW_LEN == 0 && n % ROW_LEN == 0 && n >= 16 * (size_t)ROW_LEN;
 }
 
+// The row front end's view of the input: [n_ch * n / 32] lines of 32 words (128 bytes), one box = one row
+// (32 lines), 128-byte swizzle (fm_rows.cuh).  cuTensorMapEncodeTiled comes from the driver at run time, so the
+// library has no link-time libcuda dependency.
+static int fm_rows_map(const int16_t *d_in, long long lines, CUtensorMap *map)
+{
+	static PFN_cuTensorMapEncodeTiled_v12000 encode = nullptr;
+	if (!encode) {
+		cudaDriverEntryPointQueryResult q;
+		if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", reinterpret_cast<void **>(&encode), cudaEnableDefault, &q) != cudaSuccess ||
+		    q != cudaDriverEntryPointSuccess || !encode) {
+			encode = nullptr;
+			set_error("the CUDA driver has no cuTensorMapEncodeTiled (the row front end needs it)");
+			return RXB200_EUNSUPPORTED;
+		}
+	}
+	// the box's line coordinate is a signed 32-bit int; the map's base address must be 16-byte aligned
+	if ((reinterpret_cast<uintptr_t>(d_in) & 15u) != 0 || lines < 32 || lines > 0x7fffffffLL) {
+		set_error("row front end: input at %p with %lld lines of 128 bytes cannot be mapped (16-byte alignment, at most 2^31 - 1 lines)",
+		          (const void *)d_in, lines);
+		return RXB200_EUNSUPPORTED;
+	}
+	const cuuint64_t dims[2] = {32, (cuuint64_t)lines};
+	const cuuint64_t strides[1] = {128};
+	const cuuint32_t box[2] = {32, 32}, estr[2] = {1, 1};
+	const CUresult r = encode(map, CU_TENSOR_MAP_DATA_TYPE_UINT32, 2, const_cast<int16_t *>(d_in), dims, strides, box, estr,
+	                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+	                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+	if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed (%d) for %lld lines at %p", (int)r, lines, (const void *)d_in); return RXB200_EUNSUPPORTED; }
+	return RXB200_OK;
+}
+
 static int fm_launch_rows(rxb200_fm *h, const int16_t *d_in, size_t n_int16, size_t chunk_int16, int16_t *d_out, size_t out_stride)
 {
 	const rxb200_fm_params &p = h->p;
@@ -2333,8 +2387,14 @@ static int fm_launch_rows(rxb200_fm *h, const int16_t *d_in, size_t n_int16, siz
 	const long long rows_margin = (margin_dec + row_pcm - 1) / row_pcm;
 	const int fe_warps = h->rows_fe_warps, be_lanes = h->rows_be_lanes;
 	const int threads = fe_warps * 32 + be_lanes;
+	CUtensorMap in_map;
+	{
+		const int rc = fm_rows_map(d_in, (long long)h->n_channels * (n / 32), &in_map);
+		if (rc != RXB200_OK) { return rc; }
+	}
 	const int xs_words = rows_xs_words(P);
-	const size_t xs_bytes = (size_t)fe_warps * xs_words * sizeof(uint32_t);
+	// exchange areas, then the input rings from the next 1024-byte boundary (up to 1008 bytes of padding)
+	const size_t xs_bytes = (size_t)fe_warps * xs_words * sizeof(uint32_t) + 1008 + (size_t)fe_warps * ROWS_STAGES * ROW_BYTES;
 	cudaFuncAttributes fa;
 	RXB_CUDA(cudaFuncGetAttributes(&fa, h->kern_rows));
 	// shared memory of one CTA when ROWS_MINB of them share an SM
@@ -2395,7 +2455,7 @@ static int fm_launch_rows(rxb200_fm *h, const int16_t *d_in, size_t n_int16, siz
 	if (blocks > total_work) { blocks = total_work; }
 	RXB_CUDA(cudaMemsetAsync(h->d_sync, 0, need_sync * sizeof(int), h->stream));
 	RXB_CUDA(cudaEventRecord(h->ev0, h->stream));
-	h->kern_rows<<<(unsigned)blocks, threads, smem, h->stream>>>(dv, k);
+	h->kern_rows<<<(unsigned)blocks, threads, smem, h->stream>>>(dv, k, in_map);
 	RXB_CUDA(cudaGetLastError());
 	RXB_CUDA(cudaEventRecord(h->ev1, h->stream));
 	h->cur ^= 1;
@@ -2457,7 +2517,9 @@ static int fm_launch_segs(rxb200_fm *h, const int16_t *d_in, size_t n_int16, siz
 	if (blocks > total_work) { blocks = total_work; }
 	RXB_CUDA(cudaMemsetAsync(h->d_sync, 0, need_sync * sizeof(int), h->stream));
 	RXB_CUDA(cudaEventRecord(h->ev0, h->stream));
-	h->kern_segs<<<(unsigned)blocks, T + be_lanes, smem, h->stream>>>(dv, k);
+	CUtensorMap no_map;                                  // the segment front end reads its input directly
+	memset(&no_map, 0, sizeof no_map);
+	h->kern_segs<<<(unsigned)blocks, T + be_lanes, smem, h->stream>>>(dv, k, no_map);
 	RXB_CUDA(cudaGetLastError());
 	RXB_CUDA(cudaEventRecord(h->ev1, h->stream));
 	h->cur ^= 1;

@@ -9,7 +9,12 @@
 // inputs of that level, nine for the droop FIR, one for the discriminator) is the neighbouring lane's tail,
 // handed over through a 1.8 KB per-warp exchange area in shared memory (lane 0 receives lane 31's tail of
 // the previous row).  Nothing is replayed per lane; a warp replays ONE row before its stretch (the chain's
-// memory is 128 samples) and the loads are whole 128-byte lines.
+// memory is 128 samples).
+//
+// Input: a row is 32 lines of 128 bytes, one per lane.  A per-lane 128-byte load spreads every warp-wide load
+// instruction over 32 lines, 16 bytes in each (Hopper has no 256-bit load); instead each front-end warp has a ring of
+// ROWS_STAGES row buffers in shared memory that a 2-D tensor copy (one box = one row, 128-byte swizzle) fills, and
+// lanes read their line back with conflict-free 128-bit shared loads.
 //
 // Per-chunk semantics stay literal (SURVEY F7, F8): a chunk is a whole number of rows, so only lane 0 of a
 // chunk's first row sees the boundary -- there every pass drops its pending odd sample (the history is taken
@@ -18,8 +23,9 @@
 
 #define ROW_LANE 32                    // input samples per lane per row
 #define ROW_LEN (32 * ROW_LANE)        // input samples per warp row
-#ifndef ROW_PF
-#define ROW_PF 3                       // L2 prefetch distance in rows
+#define ROW_BYTES (4 * ROW_LEN)        // one row of CS16 input
+#ifndef ROWS_STAGES
+#define ROWS_STAGES 2                  // row buffers per front-end warp
 #endif
 
 template <int P>
@@ -33,20 +39,31 @@ struct RowSmem {                       // word offsets inside a warp's exchange 
 	static constexpr int WORDS = FPRE + 4;
 };
 
-__device__ __forceinline__ void ldg256_row(const int16_t *p, uint32_t *v, uint32_t dep)
-{
-	asm volatile("ld.global.nc.L2::256B.v4.u32 {%0,%1,%2,%3}, [%8];\n\t"
-	             "ld.global.nc.L2::256B.v4.u32 {%4,%5,%6,%7}, [%8+16];"
-	             : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-	             : "l"(p), "r"(dep));
-}
+// A warp's input ring: stage s of the warp's ROWS_STAGES row buffers (1024-byte aligned, as the 128-byte swizzle
+// requires) and its mbarrier.  `line` = first 128-byte line of the row in the tensor map (channel ch, row r:
+// ch * n / 32 + 32 r); only lane 0 calls this.
+struct RowRing {
+	const CUtensorMap *map;
+	uint8_t *buf;                      // [ROWS_STAGES][ROW_BYTES]
+	uint64_t *bar;                     // [ROWS_STAGES]
+	uint32_t seq;                      // rows this warp has consumed so far: stage seq % S, phase (seq / S) & 1
+	__device__ __forceinline__ void issue(int stage, int line)
+	{
+		mbar_expect_tx(&bar[stage], ROW_BYTES);
+		tensor_load_2d(buf + stage * ROW_BYTES, map, 0, line, &bar[stage]);
+	}
+};
 
-// a lane's 32 samples of one row (128 bytes, one line) from p = the lane's first sample; `dep` only orders the loads
-// behind its producer
-__device__ __forceinline__ void row_load(const int16_t *p, uint32_t (&v)[ROW_LANE], uint32_t dep)
+// a lane's 32 samples of the current row from its stage.  The copy swizzles 16-byte chunk q of line l to chunk
+// q ^ (l & 7): eight consecutive lanes then read eight different bank groups.
+__device__ __forceinline__ void row_read(const uint8_t *stage, int lane, uint32_t (&v)[ROW_LANE])
 {
+	const uint8_t *line = stage + 128 * lane;
 #pragma unroll
-	for (int q = 0; q < ROW_LANE / 8; q++) { ldg256_row(p + 16 * q, &v[8 * q], dep); }
+	for (int q = 0; q < ROW_LANE / 4; q++) {
+		const uint4 w = *reinterpret_cast<const uint4 *>(line + 16 * (q ^ (lane & 7)));
+		v[4 * q] = w.x; v[4 * q + 1] = w.y; v[4 * q + 2] = w.z; v[4 * q + 3] = w.w;
+	}
 }
 
 // hand the level's tail (its last six inputs, oldest first) to the next lane and fetch the five inputs before this
@@ -102,15 +119,13 @@ __device__ __forceinline__ void droop9_words(const int (&c)[6], int fir_bias, ui
 	dq = wrap16(aq >> 15);
 }
 
-// One row of one lane.  v: the lane's 32 raw CS16 words (consumed by the scale, then refilled with the NEXT row, whose
-// loads are issued once level 0 is through -- from there on few registers are live, and the rest of the row's work
-// hides the latency).  par = parity of the row (which carry slot lane 31 writes); CS = the row starts a chunk;
+// One row of one lane, read from stage `stage` of the ring.  Once level 0 is through (its exchange has every lane's
+// inputs consumed) lane 0 refills the stage with the row ROWS_STAGES ahead, at `next_line` (< 0: none left).
+// par = parity of the row (which carry slot lane 31 writes); CS = the row starts a chunk;
 // rel = index of the lane's first PCM sample in the item's shared PCM buffer.
-// Returns a word that depends on the row's last results (the caller hangs the prefetched registers on it).
 template <int P, bool FIR, bool CS>
-__device__ __forceinline__ uint32_t row_body(const FmDev &c, uint32_t *xs, int par, int lane, bool store,
-                                             uint32_t (&v)[ROW_LANE], const int16_t *next_row, const int16_t *pf_row,
-                                             int16_t *pcm_s, int rel)
+__device__ __forceinline__ void row_body(const FmDev &c, uint32_t *xs, int par, int lane, bool store,
+                                         RowRing &ring, int stage, int next_line, int16_t *pcm_s, int rel)
 {
 	typedef RowSmem<P> RS;
 	constexpr int NV = RS::NV;
@@ -119,12 +134,15 @@ __device__ __forceinline__ uint32_t row_body(const FmDev &c, uint32_t *xs, int p
 		uint32_t y[ROW_LANE / 2];
 		{
 			uint32_t x[ROW_LANE];
+			{
+				uint32_t v[ROW_LANE];
+				row_read(ring.buf + stage * ROW_BYTES, lane, v);
 #pragma unroll
-			for (int j = 0; j < ROW_LANE; j++) { x[j] = scale_rot_pack(v[j], j, true); }
+				for (int j = 0; j < ROW_LANE; j++) { x[j] = scale_rot_pack(v[j], j, true); }
+			}
 			row_level<ROW_LANE, CS>(xs, RS::CARRY + (0 * 2 + par) * 8, RS::CARRY + (0 * 2 + (par ^ 1)) * 8, lane, x, y);
 		}
-		row_load(next_row, v, y[ROW_LANE / 2 - 1]);
-		asm volatile("prefetch.global.L2 [%0];" ::"l"(pf_row));      // rows further ahead: into L2, one line per lane
+		if (lane == 0 && next_line >= 0) { ring.issue(stage, next_line); }
 		if constexpr (P == 1) {
 #pragma unroll
 			for (int j = 0; j < NV; j++) { o[j] = y[j]; }
@@ -228,13 +246,12 @@ __device__ __forceinline__ uint32_t row_body(const FmDev &c, uint32_t *xs, int p
 			*reinterpret_cast<uint2 *>(dst + j) = w;
 		}
 	}
-	return wpk[NV / 2 - 1];
 }
 
 // The rows [r0, r1) of one work item that this warp owns (rows are counted from the start of the channel's call).
 template <int P, bool FIR>
 __device__ __forceinline__ void front_rows(const FmDev &c, const FmCall &k, const Item &it, int warp, int lane,
-                                           int16_t *pcm_s, uint32_t *xs)
+                                           int16_t *pcm_s, uint32_t *xs, RowRing &ring)
 {
 	typedef RowSmem<P> RS;
 	constexpr int NV = RS::NV;
@@ -271,38 +288,29 @@ __device__ __forceinline__ void front_rows(const FmDev &c, const FmCall &k, cons
 	}
 	__syncwarp();
 	int r = r0 == 0 ? 0 : r0 - 1;                   // one replayed row makes every filter exact (the chain remembers 16 << P samples)
-	// the lane's sample pointer walks row by row; rows_left counts the loop; to_cs counts down to the next chunk start
-	const int16_t *p = k.in + 2 * ((size_t)it.ch * (size_t)k.n + (size_t)r * ROW_LEN + (size_t)(ROW_LANE * lane));
-	const int16_t *p_last = k.in + 2 * ((size_t)it.ch * (size_t)k.n + (size_t)(rows_total - 1) * ROW_LEN + (size_t)(ROW_LANE * lane));
+	// line walks the rows' tensor-map coordinates; rows_left counts the loop; to_cs counts down to the next chunk start.
+	// Every row this warp copies it also consumes, so the ring is empty between items.
+	constexpr int S = ROWS_STAGES;
+	const int line0 = it.ch * (int)(k.n / 32) + 32 * r;
 	int to_cs = r % rpc;                            // 0: this row starts a chunk
 	int rel = (int)((((long long)r * ROW_LEN) >> P) - it.m_lo) + NV * lane;
 	int skip = r0 - r;                              // rows whose PCM is not stored (the replayed one)
 	int rows_left = r1 - r;
-	uint32_t v[ROW_LANE];
-	row_load(p, v, 0u);
-	for (; rows_left > 0; rows_left--) {
-		const int16_t *pn = rows_left > 1 ? p + 2 * ROW_LEN : p;            // the last row re-reads itself (never used)
-		const int16_t *pf = p + 2 * ROW_LEN * ROW_PF <= p_last ? p + 2 * ROW_LEN * ROW_PF : p_last;
+	if (lane == 0) {
+		for (int i = 0; i < S && i < rows_left; i++) { ring.issue((int)((ring.seq + i) % S), line0 + 32 * i); }
+	}
+	for (int i = 0; rows_left > 0; rows_left--, i++) {
+		const int stage = (int)(ring.seq % S);
+		mbar_wait(&ring.bar[stage], (ring.seq / S) & 1u);
+		const int next_line = rows_left > S ? line0 + 32 * (i + S) : -1;
 		// a chunk's first row is its own instantiation (warp-uniform branch): the common rows carry no trace of it
-		uint32_t token;
-		if (to_cs == 0) { token = row_body<P, FIR, true>(c, xs, par, lane, skip <= 0, v, pn, pf, pcm_s, rel); }
-		else { token = row_body<P, FIR, false>(c, xs, par, lane, skip <= 0, v, pn, pf, pcm_s, rel); }
+		if (to_cs == 0) { row_body<P, FIR, true>(c, xs, par, lane, skip <= 0, ring, stage, next_line, pcm_s, rel); }
+		else { row_body<P, FIR, false>(c, xs, par, lane, skip <= 0, ring, stage, next_line, pcm_s, rel); }
+		ring.seq++;
 		par ^= 1;
-		p = pn;
 		rel += ROW_LEN >> P;
 		skip--;
 		if (++to_cs == rpc) { to_cs = 0; }
-		// keep the prefetched row in the registers it was loaded into until here: left alone, the compiler copies some
-		// of them right behind the loads and the warp then sits out the whole memory latency
-#ifndef ROW_NO_FENCE
-#pragma unroll
-		for (int q = 0; q < ROW_LANE; q += 8) {
-			asm volatile("" : "+r"(v[q]), "+r"(v[q + 1]), "+r"(v[q + 2]), "+r"(v[q + 3]), "+r"(v[q + 4]), "+r"(v[q + 5]), "+r"(v[q + 6]), "+r"(v[q + 7])
-			             : "r"(token));
-		}
-#else
-		(void)token;
-#endif
 	}
 	if (r1 == rows_total) {
 		// this warp saw the end of the stream: lane 31's tails are the next call's carry (same layout as front_store)
