@@ -78,7 +78,8 @@ struct FmCall {
 	const uint32_t *carry_in; // [n_ch][state_words]
 	uint32_t *carry_out;      // [n_ch][state_words]
 	int *ticket;              // work counter
-	int *pub;                 // [n_ch*n_cta][4]  flag, avg, lpr_acc, -
+	int *pub;                 // [n_ch*n_cta][4]  flag, avg, margin flag (row front end), -
+	int16_t *margin;          // row front end: [n_ch*n_cta][n_extra * row PCM] the margin hand-over (fm_rows.cuh)
 	int *fix_count;           // lanes that had to be re-run from a neighbour's state
 	// per-chunk scalars of the optional reduction stages, [n_ch][n_chunks]; null when the stage is off
 	const int *rdc;           // [..][2] dc_avgI, dc_avgQ subtracted in that chunk
@@ -1802,6 +1803,7 @@ __global__ void __launch_bounds__(TMAX, MINB) fm_split_kernel(const FmDev c, con
 			else {
 				uint32_t *xs = reinterpret_cast<uint32_t *>(pcm_s + 2 * (size_t)k.pcm_cap) + (size_t)(tid >> 5) * k.xs_words;
 				front_rows<P, FE == 1>(c, k, it, tid >> 5, lane, buf, xs, ring);
+				rows_publish<P>(k, it, work, buf, tid >> 5, lane);
 			}
 			mbar_arrive(&s_full[b]);
 		}
@@ -1813,6 +1815,7 @@ __global__ void __launch_bounds__(TMAX, MINB) fm_split_kernel(const FmDev c, con
 			const int work = s_ticket[b];
 			if (work >= total_work) { break; }
 			const Item it = make_item(c, k, work);
+			if constexpr (FE != 0) { rows_collect<P>(k, it, work, pcm_s + (size_t)b * k.pcm_cap, q, k.be_lanes); }
 			back_item<SPEC, FE == 0 ? PCM_PAD_SEG : PCM_PAD_ROWS>(c, k, it, work, q, k.be_lanes, pcm_s + (size_t)b * k.pcm_cap, s_avg, s_mrun, s_ok, s_start);
 			mbar_arrive(&s_empty[b]);
 		}
@@ -1945,21 +1948,25 @@ typedef void (*fm_split_fn)(const FmDev, const FmCall, const CUtensorMap);
 // the split kernel with the row front end exists for the wbfm shape with 1..3 packed passes
 // CTA shape of the split kernel (overridable for A/B builds, tools/build_variants.sh): front-end warps, back-end lanes,
 // CTAs per SM the register budget is cut for
-// Three CTAs of 4 + 1 warps, ROWS_STAGES = 2.  Every front-end warp's input ring takes 8 KB of shared memory, so
-// fewer front-end warps per CTA leave longer items (less replay per sample).  fm2b (bench.py, 10 steps, two rounds
-// alternating the builds, one H100 80GB HBM3 SXM at a 700 W power limit, SM clock 1980 MHz), Msamples/s:
+// Two CTAs of 7 + 1 warps, ROWS_STAGES = 2.  Every front-end warp's input ring takes 8 KB of shared memory.  While each
+// warp replayed a whole row before its stretch, fewer front-end warps (longer stretches) won: fm2b (bench.py, 10 steps,
+// two rounds alternating the builds, one H100 80GB HBM3 SXM at a 700 W power limit, SM clock 1980 MHz), Msamples/s:
 //   4 + 1 warps x 3 CTAs 579 / 579    6 + 2 x 2 562 / 563    7 + 2 x 2 549 / 547    6 + 1 x 2 547 / 544
 //   5 + 1 x 3 522 / 516               before the ring (8 + 2 x 2, register loads) 388 / 387
 // and on a 400 W board of the same kind: 6 + 2 x 2 469 / 469, 16 + 4 x 1 416 / 414, 12 + 3 x 1 with 3 stages
-// 412 / 410, before the ring 362 / 364.  The P = 1 and P = 2 shapes share the choice and were not timed.
+// 412 / 410, before the ring 362 / 364.  Since a warp's start state costs 1/8 row and the margin rows are handed over,
+// the sweep of the P = 3 kernel alone (same bench line, fm2b only, two rounds; H100 80GB HBM3 SXM, 400 W power limit,
+// SM clock 1530-1680 MHz inside the kernel by clock64 against %globaltimer):
+//   7 + 1 x 2 531 / 530    6 + 1 x 2 507 / 508    4 + 1 x 3 500 / 500    5 + 1 x 3 457 / 459
+// The P = 1 and P = 2 shapes share the choice and were not timed.
 #ifndef ROWS_FE_WARPS
-#define ROWS_FE_WARPS 4
+#define ROWS_FE_WARPS 7
 #endif
 #ifndef ROWS_BE_LANES
 #define ROWS_BE_LANES 32
 #endif
 #ifndef ROWS_MINB
-#define ROWS_MINB 3
+#define ROWS_MINB 2
 #endif
 #define ROWS_TMAX (ROWS_FE_WARPS * 32 + ROWS_BE_LANES)
 static fm_split_fn pick_rows_kernel(int P, int fir_on)
@@ -2036,6 +2043,7 @@ struct rxb200_fm {
 	uint32_t *d_carry[2];
 	int cur;                       // which carry buffer holds the current state
 	int *d_sync; size_t sync_cap;  // [0] ticket, [1] fix_count, [4..] pub[n_ch*n_cta][4]
+	int16_t *d_margin; size_t margin_cap;   // row front end: margin hand-over slots (int16 entries)
 	int *d_atan_lut;
 	int16_t *d_in; size_t d_in_cap;                // int16 elements
 	int16_t *d_out; size_t d_out_cap;
@@ -2254,7 +2262,7 @@ extern "C" void rxb200_fm_destroy(rxb200_fm *h)
 	if (!h) { return; }
 	cudaSetDevice(h->device);
 	if (h->stream) { cudaStreamSynchronize(h->stream); }
-	cudaFree(h->d_carry[0]); cudaFree(h->d_carry[1]); cudaFree(h->d_sync);
+	cudaFree(h->d_carry[0]); cudaFree(h->d_carry[1]); cudaFree(h->d_sync); cudaFree(h->d_margin);
 	cudaFree(h->d_atan_lut); cudaFree(h->d_in); cudaFree(h->d_out); cudaFree(h->d_pcm);
 	cudaFree(h->d_sums); cudaFree(h->d_rdc); cudaFree(h->d_sqz); cudaFree(h->d_adc); cudaFree(h->d_lens); cudaFree(h->d_levels);
 	delete h->h_lens;
@@ -2333,8 +2341,9 @@ static int fm_check_shape(const rxb200_fm *h, size_t n_int16, size_t chunk_int16
 static long long round_up_ll(long long v, long long g) { return ((v + g - 1) / g) * g; }
 
 // ---- launch of the split kernel with the row front end (fm_rows.cuh).  Geometry in ROWS of ROW_LEN input samples:
-// an item owns `rows_own` rows, its warps also produce the `rows_margin` rows before them (the back end's replay
-// window); the two PCM buffers and the warps' exchange areas share the CTA's dynamic shared memory.
+// an item owns `rows_own` rows; its PCM buffer also holds the `rows_margin` rows before them (the back end's replay
+// window), which the previous items of the channel hand over through global memory; the two PCM buffers and the
+// warps' exchange areas share the CTA's dynamic shared memory.
 static bool fm_rows_shape_ok(const rxb200_fm *h, size_t n_int16, size_t chunk_int16)
 {
 	if (!h->kern_rows) { return false; }
@@ -2414,21 +2423,23 @@ static int fm_launch_rows(rxb200_fm *h, const int16_t *d_in, size_t n_int16, siz
 		if (t < 1) { t = 1; }
 		if (t < rows_own) { rows_own = t; }
 	} else {
-		// whole waves of the resident CTAs: a slightly shorter item beats a ragged last wave
+		// Items go out in waves of the resident CTAs.  A warp spends on an item its even share of the rows plus the 1/8
+		// row of its start state (row_start_state), so the estimate for a length is waves x (ceil(rows / fe_warps) + 1/8):
+		// a slightly shorter item that splits evenly or fills the last wave beats the longest one that fits.  Lengths
+		// down to 60 % of that are tried; the longest of equal estimates wins.
 		const long long slots = (long long)h->n_sm * ROWS_MINB;
-		const long long items = (rows_total * h->n_channels + rows_own - 1) / rows_own;
-		if (items > slots) {
-			const long long waves = (items + slots - 1) / slots;
-			const long long t = (rows_total * h->n_channels + waves * slots - 1) / (waves * slots);
-			if (t >= 1 && t < rows_own && t * 10 >= rows_own * 6) { rows_own = t; }
+		const long long longest = rows_own;
+		double best = 0.0;
+		for (long long t = longest; t >= 1 && t * 10 >= longest * 6; t--) {
+			const long long items = (rows_total + t - 1) / t * h->n_channels;
+			const double est = (double)((items + slots - 1) / slots) * ((double)((t + fe_warps - 1) / fe_warps) + 0.125);
+			if (t == longest || est < best) { best = est; rows_own = t; }
 		}
 	}
 	if (rows_own > rows_total) { rows_own = rows_total; }
 	rows_item = rows_own + rows_margin;
 	const long long pcm_cap = cap_for(rows_item);
 	const size_t smem = 2 * (size_t)pcm_cap * sizeof(int16_t) + xs_bytes;
-	// (no last wave of quarter-size items to shorten the drain of the grid: the short items would pay the per-warp halo
-	// row and the margin rows on a quarter of the rows)
 	const long long n_cta = (rows_total + rows_own - 1) / rows_own;
 	RXB_CUDA(cudaFuncSetAttribute(h->kern_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
 	int per_sm = 1;
@@ -2441,9 +2452,16 @@ static int fm_launch_rows(rxb200_fm *h, const int16_t *d_in, size_t n_int16, siz
 		RXB_CUDA(cudaMalloc(&h->d_sync, need_sync * sizeof(int)));
 		h->sync_cap = need_sync;
 	}
+	const size_t need_margin = total_work * (size_t)rows_margin * (size_t)row_pcm;
+	if (need_margin > h->margin_cap) {
+		cudaFree(h->d_margin); h->d_margin = nullptr; h->margin_cap = 0;
+		RXB_CUDA(cudaMalloc(&h->d_margin, need_margin * sizeof(int16_t)));
+		h->margin_cap = need_margin;
+	}
 	FmCall k;
 	memset(&k, 0, sizeof k);
 	k.in = d_in; k.out = d_out; k.n = n; k.out_stride = (long long)out_stride; k.chunk = (int)(chunk_int16 / 2);
+	k.margin = h->d_margin;
 	k.n_ch = h->n_channels; k.Sf = ROW_LEN; k.halo = 0; k.n_extra = (int)rows_margin; k.n_own = (int)rows_own;
 	k.n_cta = (int)n_cta; k.W_dec = (int)W_dec; k.pcm_cap = (int)pcm_cap; k.direct_out = 0;
 	k.be_lanes = be_lanes; k.fe_warps = fe_warps; k.fe_threads = fe_warps * 32; k.xs_words = xs_words;

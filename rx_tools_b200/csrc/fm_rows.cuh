@@ -8,8 +8,13 @@
 // is evaluated level by level on the lane's block; what a level needs from BEFORE the block (the last five
 // inputs of that level, nine for the droop FIR, one for the discriminator) is the neighbouring lane's tail,
 // handed over through a 1.8 KB per-warp exchange area in shared memory (lane 0 receives lane 31's tail of
-// the previous row).  Nothing is replayed per lane; a warp replays ONE row before its stretch (the chain's
-// memory is 128 samples).
+// the previous row).  Nothing is replayed per lane; a warp rebuilds the state in front of its stretch from the last
+// 128 input samples of the row before it (row_start_state: the chain's memory is shorter than that).
+//
+// An item's back end also needs the PCM of the `n_extra` (rows_margin) rows before the item's own rows.  Those rows
+// belong to the previous items of the channel: each item's front end publishes the PCM of its last n_extra rows to a
+// per-item slot in global memory (rows_publish), and the back end copies it from there (rows_collect), so no row is
+// computed twice.
 //
 // Input: a row is 32 lines of 128 bytes, one per lane.  A per-lane 128-byte load spreads every warp-wide load
 // instruction over 32 lines, 16 bytes in each (Hopper has no 256-bit load); instead each front-end warp has a ring of
@@ -124,7 +129,7 @@ __device__ __forceinline__ void droop9_words(const int (&c)[6], int fir_bias, ui
 // par = parity of the row (which carry slot lane 31 writes); CS = the row starts a chunk;
 // rel = index of the lane's first PCM sample in the item's shared PCM buffer.
 template <int P, bool FIR, bool CS>
-__device__ __forceinline__ void row_body(const FmDev &c, uint32_t *xs, int par, int lane, bool store,
+__device__ __forceinline__ void row_body(const FmDev &c, uint32_t *xs, int par, int lane,
                                          RowRing &ring, int stage, int next_line, int16_t *pcm_s, int rel)
 {
 	typedef RowSmem<P> RS;
@@ -237,18 +242,87 @@ __device__ __forceinline__ void row_body(const FmDev &c, uint32_t *xs, int par, 
 		for (int j = 0; j < NV; j += 2) { wpk[j / 2] = ((uint32_t)pcm[j] & 0xffffu) | ((uint32_t)pcm[j + 1] << 16); }
 	}
 #endif
-	if (store) {
-		int16_t *dst = pcm_s + pcm_phys<PCM_PAD_ROWS>(rel);
+	int16_t *dst = pcm_s + pcm_phys<PCM_PAD_ROWS>(rel);
 #pragma unroll
-		for (int j = 0; j < NV; j += 4) {
-			uint2 w;
-			w.x = wpk[j / 2]; w.y = wpk[j / 2 + 1];
-			*reinterpret_cast<uint2 *>(dst + j) = w;
+	for (int j = 0; j < NV; j += 4) {
+		uint2 w;
+		w.x = wpk[j / 2]; w.y = wpk[j / 2 + 1];
+		*reinterpret_cast<uint2 *>(dst + j) = w;
+	}
+}
+
+// What a row leaves behind for the next one -- lane 31's tails at every level (CARRY), the droop FIR's last inputs
+// (VRING) and the last FIR output (FPRE) -- from the row's last 128 input samples `v` (4 per lane), written to the
+// parity-1 slots, which the first row of a stretch (parity 0) reads.  Every pass, the droop FIR and the discriminator
+// have finite memory: window output j of a pass needs its inputs 2j-5 .. 2j, so the window's y are exact from y[3] on,
+// its z from z[4], its o (P = 3) from o[5].  What is written needs no more than x[122..], y[58..], z[26..] and the last
+// ten o, so no word of it depends on anything before the window (tests/test_rows_reach.py pins this on the port).
+// Chunks start on row boundaries, so no chunk start (F7, F8) falls inside the window.
+template <int P, bool FIR>
+__device__ __forceinline__ void row_start_state(const FmDev &c, uint4 v, uint32_t *xs, int lane)
+{
+	typedef RowSmem<P> RS;
+	constexpr unsigned FULL = 0xffffffffu;
+	uint32_t *cw = xs + RS::CARRY;                        // [level][parity][8]; parity 1 is at + 8
+	// level 0: x[4l .. 4l+3], five inputs of history from lanes l-1 and l-2 -> y[2l], y[2l+1]
+	const uint32_t x0 = scale_rot_pack(v.x, 0, true), x1 = scale_rot_pack(v.y, 1, true);
+	const uint32_t x2 = scale_rot_pack(v.z, 2, true), x3 = scale_rot_pack(v.w, 3, true);
+	uint32_t h0 = __shfl_up_sync(FULL, x3, 2), h1 = __shfl_up_sync(FULL, x0, 1), h2 = __shfl_up_sync(FULL, x1, 1);
+	uint32_t h3 = __shfl_up_sync(FULL, x2, 1), h4 = __shfl_up_sync(FULL, x3, 1);
+	const uint32_t y0 = hb_tap(h0, h1, h2, h3, h4, x0), y1 = hb_tap(h2, h3, h4, x0, x1, x2);
+	if (lane == 31) {
+		*reinterpret_cast<uint4 *>(cw + 8) = make_uint4(h3, h4, x0, x1);
+		*reinterpret_cast<uint2 *>(cw + 8 + 4) = make_uint2(x2, x3);
+	}
+	uint32_t o0, o1 = 0u;                                 // the lane's decimated samples (P = 1: two, else one)
+	int m0, m1 = -1;                                      // their indices among the window's M decimated samples
+	constexpr int M = 128 >> P;
+	if constexpr (P == 1) {
+		o0 = y0; o1 = y1; m0 = 2 * lane; m1 = 2 * lane + 1;
+	} else {
+		// level 1: y[2l], y[2l+1], history from lanes l-1 .. l-3 -> z[l]
+		h0 = __shfl_up_sync(FULL, y1, 3); h1 = __shfl_up_sync(FULL, y0, 2); h2 = __shfl_up_sync(FULL, y1, 2);
+		h3 = __shfl_up_sync(FULL, y0, 1); h4 = __shfl_up_sync(FULL, y1, 1);
+		const uint32_t z = hb_tap(h0, h1, h2, h3, h4, y0);
+		if (lane == 31) {
+			*reinterpret_cast<uint4 *>(cw + 24) = make_uint4(h1, h2, h3, h4);
+			*reinterpret_cast<uint2 *>(cw + 24 + 4) = make_uint2(y0, y1);
 		}
+		if constexpr (P == 2) {
+			o0 = z; m0 = lane;
+		} else {
+			// level 2: z[l-5 .. l] -> o[l / 2] on the even lanes
+			h0 = __shfl_up_sync(FULL, z, 5); h1 = __shfl_up_sync(FULL, z, 4); h2 = __shfl_up_sync(FULL, z, 3);
+			h3 = __shfl_up_sync(FULL, z, 2); h4 = __shfl_up_sync(FULL, z, 1);
+			o0 = hb_tap(h0, h1, h2, h3, h4, z); m0 = (lane & 1) ? -1 : lane >> 1;
+			if (lane == 31) {
+				*reinterpret_cast<uint4 *>(cw + 40) = make_uint4(h0, h1, h2, h3);
+				*reinterpret_cast<uint2 *>(cw + 40 + 4) = make_uint2(h4, z);
+			}
+		}
+	}
+	constexpr int BO = 128 << P;
+	if constexpr (FIR) {
+		// the last ten o, biased, go where a row leaves its last twelve (VRING[m - M + 12]); the next row reads [3, 12),
+		// the last FIR output is the filter over [2, 11)
+		uint32_t *vr = xs + RS::VRING;
+		if (m0 >= M - 10) { vr[m0 - M + 12] = o0 + (FIR_B - (unsigned)BO) * 0x10001u; }
+		if (m1 >= M - 10) { vr[m1 - M + 12] = o1 + (FIR_B - (unsigned)BO) * 0x10001u; }
+		__syncwarp();
+		if (lane == 0) {
+			int di, dq;
+			droop9_words(c.fir, c.fir_bias, vr[2], vr[3], vr[4], vr[5], vr[6], vr[7], vr[8], vr[9], vr[10], di, dq);
+			xs[RS::FPRE + 1] = pack2(di, dq);
+		}
+	} else {
+		const uint32_t last = (P == 1) ? o1 : o0;
+		if (m0 == M - 1 || m1 == M - 1) { xs[RS::FPRE + 1] = pack2((int)(last & 0xffffu) - BO, (int)(last >> 16) - BO); }
 	}
 }
 
 // The rows [r0, r1) of one work item that this warp owns (rows are counted from the start of the channel's call).
+// The item's rows [own_lo, own_hi) split evenly over the front-end warps; the margin rows before own_lo come from
+// the previous items (rows_collect).
 template <int P, bool FIR>
 __device__ __forceinline__ void front_rows(const FmDev &c, const FmCall &k, const Item &it, int warp, int lane,
                                            int16_t *pcm_s, uint32_t *xs, RowRing &ring)
@@ -259,17 +333,23 @@ __device__ __forceinline__ void front_rows(const FmDev &c, const FmCall &k, cons
 	const int rows_total = (int)(k.n / ROW_LEN);
 	const int own_lo = it.b * k.n_own;
 	const int own_hi = own_lo + k.n_own < rows_total ? own_lo + k.n_own : rows_total;
-	const int buf_lo = own_lo - k.n_extra > 0 ? own_lo - k.n_extra : 0;
-	const int n_rows = own_hi - buf_lo;
-	const int per = (n_rows + k.fe_warps - 1) / k.fe_warps;
-	const int r0 = buf_lo + warp * per;
+	const int per = (own_hi - own_lo + k.fe_warps - 1) / k.fe_warps;
+	const int r0 = own_lo + warp * per;
 	const int r1 = r0 + per < own_hi ? r0 + per : own_hi;
 	if (r0 >= r1) { return; }
+	// line walks the rows' tensor-map coordinates; rows_left counts the loop; to_cs counts down to the next chunk start.
+	// Every row this warp copies it also consumes, so the ring is empty between items.
+	constexpr int S = ROWS_STAGES;
+	const int line0 = it.ch * (int)(k.n / 32) + 32 * r0;
+	int rows_left = r1 - r0;
+	if (lane == 0) {
+		for (int i = 0; i < S && i < rows_left; i++) { ring.issue((int)((ring.seq + i) % S), line0 + 32 * i); }
+	}
+	// what the row before the first one left behind: the call's carry at the start of the stream, else rebuilt from
+	// that row's last 128 samples (one coalesced 512-byte load; the input is not written during the launch)
 	const uint32_t *carry = k.carry_in + (size_t)it.ch * k.state_words;
-	const int rpc = k.chunk / ROW_LEN;              // rows per chunk
-	int par = 0;
-	// what the (non-existent) row before the first one left behind: the call's carry at the start of the stream,
-	// silence in front of a replayed row
+	uint4 tail = make_uint4(0u, 0u, 0u, 0u);
+	if (r0 > 0) { tail = __ldg(reinterpret_cast<const uint4 *>(k.in) + ((size_t)it.ch * (size_t)k.n + (size_t)r0 * ROW_LEN - 128) / 4 + lane); }
 	__syncwarp();
 	if (r0 == 0) {
 		if (lane < 6) {
@@ -279,37 +359,23 @@ __device__ __forceinline__ void front_rows(const FmDev &c, const FmCall &k, cons
 		if (FIR && lane < 9) { xs[RS::VRING + 3 + lane] = fir_bias_lanes(carry[ST_HDR + 6 * P + lane]); }
 		if (lane == 0) { xs[RS::FPRE + 1] = pack2((int)carry[ST_PRE_I], (int)carry[ST_PRE_Q]); }
 	} else {
-		if (lane < 6) {
-#pragma unroll
-			for (int l = 0; l < P; l++) { xs[RS::CARRY + (l * 2 + 1) * 8 + lane] = 0x00010001u * (128u << l); }
-		}
-		if (FIR && lane < 12) { xs[RS::VRING + lane] = fir_bias_lanes(0u); }
-		if (lane == 0) { xs[RS::FPRE + 1] = 0u; }
+		row_start_state<P, FIR>(c, tail, xs, lane);
 	}
 	__syncwarp();
-	int r = r0 == 0 ? 0 : r0 - 1;                   // one replayed row makes every filter exact (the chain remembers 16 << P samples)
-	// line walks the rows' tensor-map coordinates; rows_left counts the loop; to_cs counts down to the next chunk start.
-	// Every row this warp copies it also consumes, so the ring is empty between items.
-	constexpr int S = ROWS_STAGES;
-	const int line0 = it.ch * (int)(k.n / 32) + 32 * r;
-	int to_cs = r % rpc;                            // 0: this row starts a chunk
-	int rel = (int)((((long long)r * ROW_LEN) >> P) - it.m_lo) + NV * lane;
-	int skip = r0 - r;                              // rows whose PCM is not stored (the replayed one)
-	int rows_left = r1 - r;
-	if (lane == 0) {
-		for (int i = 0; i < S && i < rows_left; i++) { ring.issue((int)((ring.seq + i) % S), line0 + 32 * i); }
-	}
+	const int rpc = k.chunk / ROW_LEN;              // rows per chunk
+	int par = 0;
+	int to_cs = r0 % rpc;                           // 0: this row starts a chunk
+	int rel = (int)((((long long)r0 * ROW_LEN) >> P) - it.m_lo) + NV * lane;
 	for (int i = 0; rows_left > 0; rows_left--, i++) {
 		const int stage = (int)(ring.seq % S);
 		mbar_wait(&ring.bar[stage], (ring.seq / S) & 1u);
 		const int next_line = rows_left > S ? line0 + 32 * (i + S) : -1;
 		// a chunk's first row is its own instantiation (warp-uniform branch): the common rows carry no trace of it
-		if (to_cs == 0) { row_body<P, FIR, true>(c, xs, par, lane, skip <= 0, ring, stage, next_line, pcm_s, rel); }
-		else { row_body<P, FIR, false>(c, xs, par, lane, skip <= 0, ring, stage, next_line, pcm_s, rel); }
+		if (to_cs == 0) { row_body<P, FIR, true>(c, xs, par, lane, ring, stage, next_line, pcm_s, rel); }
+		else { row_body<P, FIR, false>(c, xs, par, lane, ring, stage, next_line, pcm_s, rel); }
 		ring.seq++;
 		par ^= 1;
 		rel += ROW_LEN >> P;
-		skip--;
 		if (++to_cs == rpc) { to_cs = 0; }
 	}
 	if (r1 == rows_total) {
@@ -328,4 +394,63 @@ __device__ __forceinline__ void front_rows(const FmDev &c, const FmCall &k, cons
 			co[ST_BOX_I] = 0u; co[ST_BOX_Q] = 0u; co[ST_BOX_N] = 0u;
 		}
 	}
+}
+
+// ---- margin hand-over between the items of a channel.  Item w's slot in k.margin holds n_extra rows of PCM: row r of
+// the item sits at (r - (own_hi - n_extra)) * row_pcm, and only its own rows are written.  pub[4 w + 2] = 1 says the
+// slot is complete.  (PCM_PAD_ROWS is 0: the shared buffer is linear.)
+#define BAR_PUB 3
+__device__ __forceinline__ int ld_acquire_gpu(const int *p)
+{
+	int v;
+	asm volatile("ld.acquire.gpu.global.b32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+	return v;
+}
+__device__ __forceinline__ void st_release_gpu(int *p, int v) { asm volatile("st.release.gpu.global.b32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
+
+// Front end, after its own rows: the last front-end warp waits for the others' rows (the others only arrive), copies
+// the item's last n_extra rows to its slot and raises the flag.  This never waits for a back end, so no item's margin
+// sits behind another item's serial stages.
+template <int P>
+__device__ __forceinline__ void rows_publish(const FmCall &k, const Item &it, int work, const int16_t *pcm_s, int warp, int lane)
+{
+	if (warp != k.fe_warps - 1) { asm volatile("bar.arrive %0, %1;" ::"r"(BAR_PUB), "r"(k.fe_threads) : "memory"); return; }
+	bar_sync(BAR_PUB, k.fe_threads);
+	if (it.b == k.n_cta - 1) { return; }                // the channel's last item: nobody reads its margin
+	constexpr int LG = 10 - P;                             // log2 of PCM samples per row
+	const int own_hi = (it.b + 1) * k.n_own;             // not the last item: never clipped at the end of the call
+	const int lo = it.b * k.n_own > own_hi - k.n_extra ? it.b * k.n_own : own_hi - k.n_extra;
+	const uint4 *src = reinterpret_cast<const uint4 *>(pcm_s + (((long long)lo << LG) - it.m_lo));
+	uint4 *dst = reinterpret_cast<uint4 *>(k.margin + ((size_t)work * k.n_extra + (lo - (own_hi - k.n_extra))) * (1 << LG));
+	const int n = ((own_hi - lo) << LG) / 8;
+	for (int i = lane; i < n; i += 32) { dst[i] = src[i]; }
+	__syncwarp();
+	if (lane == 0) { __threadfence(); st_release_gpu(k.pub + 4 * (size_t)work + 2, 1); }
+}
+
+// Back end, before pass 1: the margin rows [buf_lo, own_lo) of this item, from the slots of the older items of the
+// channel that own them (up to n_extra of them when items are shorter than the margin).  Progress: these are older
+// tickets, and a front end that holds a ticket waits for nothing but its own warps (it took the ticket after its
+// `empty` wait), so their flags always come.  Coherent loads: the slots are written during the launch.
+template <int P>
+__device__ __forceinline__ void rows_collect(const FmCall &k, const Item &it, int work, int16_t *pcm_s, int q, int lanes)
+{
+	const int own_lo = it.b * k.n_own;
+	const int buf_lo = own_lo - k.n_extra > 0 ? own_lo - k.n_extra : 0;
+	if (buf_lo == own_lo) { return; }
+	constexpr int LG = 10 - P;
+	const int first = buf_lo / k.n_own;                  // the oldest item holding a margin row
+	for (int j = first; j < it.b; j++) {
+		const int *f = k.pub + 4 * (size_t)(work - (it.b - j)) + 2;
+		while (ld_acquire_gpu(f) == 0) { __nanosleep(32); }
+	}
+	const int n = ((own_lo - buf_lo) << LG) / 8;
+	uint4 *dst = reinterpret_cast<uint4 *>(pcm_s + (((long long)buf_lo << LG) - it.m_lo));
+	for (int i = q; i < n; i += lanes) {
+		const int r = buf_lo + ((8 * i) >> LG);
+		const int j = r / k.n_own;
+		const size_t e = ((size_t)(work - (it.b - j)) * k.n_extra + (r - ((j + 1) * k.n_own - k.n_extra))) * (1 << LG) + ((8 * i) & ((1 << LG) - 1));
+		dst[i] = __ldcg(reinterpret_cast<const uint4 *>(k.margin + e));
+	}
+	bar_sync(BAR_BE, lanes);
 }
