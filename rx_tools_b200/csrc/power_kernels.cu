@@ -615,6 +615,122 @@ __global__ void __launch_bounds__(256) power_big_load(const int16_t *src, uint32
 	}
 }
 
+// big_decim: copy + the -F decimator (downsample_iq x P, then the droop FIR, :734-743) + the two remove_dc sums, in place
+// of big_load when boxcar == 0.  The host only routes shapes here whose every pass length buf_len >> j is a multiple of
+// 4 int16 and whose decimated span is whole N-blocks (buf_len = k * 2N * 2^P: every planner shape), so I and Q have
+// the same sample count n_l = buf_len >> (l+1) at every level l and the blocks read nothing past the decimated span.
+//
+// Each output of a pass is a pure function of ORIGINAL samples of its input (the in-place loop of fifth_order only ever
+// reads what it has not yet overwritten), so a CTA can produce a tile [m0, m1) of final samples from the level-0 span
+// that tile depends on: level l+1 sample k reads level-l samples 2k-5 .. 2k (k >= 5) or 0 .. 8 (the ease-in head,
+// k < 5), and the FIR adds final samples m0-9 .. m0-1.  The span is staged by one bulk copy from a 16-byte-aligned
+// start, every pass runs in place in shared memory, and only the tile's final samples go back to HBM.
+#define RXB_DECIM_RNG 16                    // byte offset of the per-level window table in shared memory
+#define RXB_DECIM_DATA 256                  // byte offset of the level-0 span
+#define RXB_DECIM_R 4                       // outputs per thread per in-place round
+__host__ __device__ __forceinline__ void decim_window(int m0, int m1, int P, int fir_on, int *lo, int *hi)
+{
+	// level-l window [lo[l], hi[l]] of a tile [m0, m1) of final samples, l = P down to 0
+	lo[P] = m0 - 9 * fir_on > 0 ? m0 - 9 * fir_on : 0;
+	hi[P] = m1 - 1;
+	for (int l = P; l > 0; l--) {
+		lo[l - 1] = 2 * lo[l] - 5 > 0 ? 2 * lo[l] - 5 : 0;
+		hi[l - 1] = hi[l] >= 5 ? 2 * hi[l] : 8;
+	}
+	lo[0] &= ~3;                            // whole 16-byte words of the hop buffer
+	hi[0] |= 3;
+}
+
+__device__ __forceinline__ int hb_taps(int a, int b, int c, int d, int e, int f) { return (a + (b + e) * 5 + (c + d) * 10 + f) >> 4; }
+
+// fifth_order output k of one component (sel 0 = I, 1 = Q) from the level window x, which starts at level index lo
+__device__ __forceinline__ int hb_out(const uint32_t *x, int lo, int k, int sel)
+{
+	const uint32_t *w = x - lo;             // w[i] = level sample i
+	if (k < 3) {
+		const int a = pw_get(w, 0, sel), b = pw_get(w, 1, sel), c = pw_get(w, 2, sel);
+		const int d = pw_get(w, 3, sel), e = pw_get(w, 4, sel), f = pw_get(w, 5, sel);
+		if (k == 0) { return ((a + b) * 10 + (c + d) * 5 + d + f) >> 4; }
+		if (k == 1) { return ((b + c) * 10 + (a + d) * 5 + e + f) >> 4; }
+		return hb_taps(a, b, c, d, e, f);
+	}
+	if (k == 3) { return hb_taps(pw_get(w, 2, sel), pw_get(w, 3, sel), pw_get(w, 4, sel), pw_get(w, 5, sel), pw_get(w, 5, sel), pw_get(w, 6, sel)); }
+	if (k == 4) { return hb_taps(pw_get(w, 4, sel), pw_get(w, 5, sel), pw_get(w, 5, sel), pw_get(w, 6, sel), pw_get(w, 7, sel), pw_get(w, 8, sel)); }
+	const int i = 2 * k - 5;
+	return hb_taps(pw_get(w, i, sel), pw_get(w, i + 1, sel), pw_get(w, i + 2, sel), pw_get(w, i + 3, sel), pw_get(w, i + 4, sel), pw_get(w, i + 5, sel));
+}
+
+// generic_fir output d >= 9 of one component: the 9-tap sum over ORIGINAL samples d-9 .. d-1, wrapping as pw_droop9
+__device__ __forceinline__ int fir_out(const uint32_t *x, int lo, int d, int sel, const int *c)
+{
+	const uint32_t *w = x - lo;
+	int acc = mul_w(pw_get(w, d - 9, sel) + pw_get(w, d - 1, sel), c[1]);
+	acc = add_w(acc, mul_w(pw_get(w, d - 8, sel) + pw_get(w, d - 2, sel), c[2]));
+	acc = add_w(acc, mul_w(pw_get(w, d - 7, sel) + pw_get(w, d - 3, sel), c[3]));
+	acc = add_w(acc, mul_w(pw_get(w, d - 6, sel) + pw_get(w, d - 4, sel), c[4]));
+	acc = add_w(acc, mul_w(pw_get(w, d - 5, sel), c[5]));
+	return acc >> 15;
+}
+
+struct DecimFir { int c[6]; };
+
+__global__ void __launch_bounds__(256) power_big_decim(const int16_t *src, uint32_t *work, int n_final, int tile, int P, int fir_on,
+                                                       const DecimFir fir, long long *sums)
+{
+	extern __shared__ __align__(128) unsigned char smem_raw[];
+	uint64_t *bar = reinterpret_cast<uint64_t *>(smem_raw);
+	int *win_lo = reinterpret_cast<int *>(smem_raw + RXB_DECIM_RNG);      // [11]
+	int *win_hi = win_lo + 11;                                             // [11]
+	uint32_t *x = reinterpret_cast<uint32_t *>(smem_raw + RXB_DECIM_DATA);
+	const int tid = threadIdx.x, T = blockDim.x;
+	const int m0 = blockIdx.x * tile;
+	const int m1 = m0 + tile < n_final ? m0 + tile : n_final;
+	if (tid == 0) {
+		decim_window(m0, m1, P, fir_on, win_lo, win_hi);
+		mbar_init(bar, 1);
+		const uint32_t bytes = (uint32_t)(win_hi[0] - win_lo[0] + 1) * 4u;
+		mbar_expect_tx(bar, bytes);
+		bulk_load(x, src + 2 * (size_t)win_lo[0], bytes, bar);
+	}
+	__syncthreads();
+	mbar_wait(bar, 0);
+	// downsample_iq, pass l: level l (window at win_lo[l]) -> level l+1, in place.  Output k lands at k - lo1 while the
+	// outputs of later rounds read at >= 2 (k' - lo1) > k - lo1 (lo = max(0, 2 lo1 - 5), rounded down), so a round only
+	// has to finish its reads before it writes.
+	for (int l = 0; l < P; l++) {
+		const int lo = win_lo[l], lo1 = win_lo[l + 1], n1 = win_hi[l + 1] - lo1 + 1;
+		for (int base = 0; base < n1; base += T * RXB_DECIM_R) {
+			uint32_t y[RXB_DECIM_R];
+#pragma unroll
+			for (int r = 0; r < RXB_DECIM_R; r++) {
+				const int j = base + r * T + tid;
+				if (j < n1) { y[r] = ppack(hb_out(x, lo, lo1 + j, 0), hb_out(x, lo, lo1 + j, 1)); }
+			}
+			__syncthreads();
+#pragma unroll
+			for (int r = 0; r < RXB_DECIM_R; r++) {
+				const int j = base + r * T + tid;
+				if (j < n1) { x[j] = y[r]; }
+			}
+			__syncthreads();
+		}
+	}
+	// droop FIR (samples 0..8 pass through), store the tile, sum it for remove_dc
+	const int loP = win_lo[P];
+	long long si = 0, sq = 0;
+	for (int m = m0 + tid; m < m1; m += T) {
+		uint32_t v = x[m - loP];
+		if (fir_on && m >= 9) { v = ppack(fir_out(x, loP, m, 0, fir.c), fir_out(x, loP, m, 1, fir.c)); }
+		work[m] = v;
+		si += plo(v); sq += phi(v);
+	}
+	for (int o = 16; o > 0; o >>= 1) { si += __shfl_down_sync(0xffffffffu, si, o); sq += __shfl_down_sync(0xffffffffu, sq, o); }
+	if ((tid & 31) == 0) {
+		atomicAdd(reinterpret_cast<unsigned long long *>(sums), (unsigned long long)si);
+		atomicAdd(reinterpret_cast<unsigned long long *>(sums + 1), (unsigned long long)sq);
+	}
+}
+
 __global__ void __launch_bounds__(256) power_big_window(const uint32_t *work, uint32_t *fft, const int16_t *win, const long long *sums,
                                                         int used_int16, int n_slots, int bin_e, int nblk)
 {
@@ -701,6 +817,7 @@ struct rxb200_power {
 	void *d_db = nullptr; size_t db_cap = 0;   // csv_dbm staging (rxb200_power_read_db)
 	int triv = 0;                              // see PowArgs::triv
 	uint32_t *d_work = nullptr, *d_fft = nullptr; long long *d_sums = nullptr;   // global-memory path (hop buffer beyond shared memory)
+	int decim_tile = 0; size_t decim_smem = 0;                                   // power_big_decim's tile (final samples) and shared memory
 	int force_v1 = 0;                          // RXB200_POWER_V1 (A/B knob, read once at create): generic kernel only
 	int fft8_threads = 0;                      // RXB200_POWER_THREADS = 512 | 1024 (A/B knob): CTA width of the fast path
 };
@@ -720,9 +837,14 @@ static int power_validate(const rxb200_power_params *p)
 			set_error("bin_e %d x downsample %d needs more than buf_len %d", p->bin_e, p->downsample, p->buf_len);
 			return RXB200_EINVAL;
 		}
-		if (need > 227 * 1024 && p->downsample > 1 && !p->boxcar) {
-			// the global-memory path (hop buffers beyond shared memory) carries the boxcar decimator only
-			set_error("bin_e %d with buf_len %d and -F decimation is not implemented (hop buffer beyond shared memory)", p->bin_e, p->buf_len);
+		if (need > 227 * 1024 && p->downsample > 1 && !p->boxcar &&
+		    (p->downsample_passes < 1 || p->downsample != (1 << p->downsample_passes) ||
+		     p->buf_len % ((2LL << p->bin_e) * p->downsample) != 0)) {
+			// power_big_decim assumes the planner's geometry (src/rtl_power.c:466-474, :504-507): downsample = 2^passes and
+			// the decimated span is whole N-blocks, so every pass keeps I and Q the same length and no block reads the
+			// leftovers of earlier passes.  This covers every plan the big path routes to it (boxcar 0, downsample > 1).
+			set_error("-F decimation of a hop buffer beyond shared memory needs downsample = 2^passes (%d, %d) and buf_len %d a multiple of 2 x %d x downsample",
+			          p->downsample, p->downsample_passes, p->buf_len, 1 << p->bin_e);
 			return RXB200_EUNSUPPORTED;
 		}
 		// the block loop runs while offset < buf_len/downsample (src/rtl_power.c:747): a partial last block is
@@ -837,6 +959,33 @@ static cudaError_t launch_fft8(int bin_e, int threads, const PowArgs &a, int blo
 #undef RXB_FFT8_CASE
 }
 
+// power_big_decim's tile: about four CTAs per SM (one CTA's serial passes leave the SM mostly idle), but no smaller than
+// four times the per-tile halo of 5 (+ 9 with the FIR) final samples, which keeps the level-0 read amplification near
+// 1.25 or below, and no larger than a level-0 span that fits shared memory.  `smem` covers the largest span over all
+// tiles (the 16-byte rounding varies from tile to tile).
+static int decim_span_max(int n_final, int tile, int P, int fir_on)
+{
+	int lo[11], hi[11], worst = 0;
+	for (int m0 = 0; m0 < n_final; m0 += tile) {
+		decim_window(m0, m0 + tile < n_final ? m0 + tile : n_final, P, fir_on, lo, hi);
+		if (hi[0] - lo[0] + 1 > worst) { worst = hi[0] - lo[0] + 1; }
+	}
+	return worst;
+}
+static void decim_plan(int n_final, int P, int fir_on, int n_sm, int *tile, size_t *smem)
+{
+	const int cap = (227 * 1024 - RXB_DECIM_DATA) / 4;                  // level-0 complex samples a CTA can stage
+	const int halo = 5 + 9 * fir_on;
+	int t = (n_final + 4 * n_sm - 1) / (4 * n_sm);
+	if (t < 4 * halo) { t = 4 * halo; }
+	const int t_cap = (cap - 7 - 5 * ((1 << P) - 1)) / (1 << P) + 1 - 9 * fir_on;
+	if (t > t_cap) { t = t_cap; }
+	if (t > n_final) { t = n_final; }
+	while (t > 1 && decim_span_max(n_final, t, P, fir_on) > cap) { t--; }
+	*tile = t;
+	*smem = RXB_DECIM_DATA + (size_t)decim_span_max(n_final, t, P, fir_on) * 4;
+}
+
 extern "C" int rxb200_power_accumulate_device(rxb200_power *h, const int16_t *d_hop_bufs, int n_pass,
                                               int hop_begin, int hop_end, int sync)
 {
@@ -871,18 +1020,34 @@ extern "C" int rxb200_power_accumulate_device(rxb200_power *h, const int16_t *d_
 			const int n_complex = h->p.buf_len / 2, ds = h->p.downsample;
 			const int used = h->p.buf_len / ds;                         // int16 span after decimation (:744-747)
 			const int nblk = (used + 2 * N - 1) / (2 * N);
+			const int n_slots = (n_complex + ds - 1) / ds;              // decimated complex samples (-F: exactly used / 2)
+			// -F passes only when the plan decimates: downsample == 1 keeps the plain copy, as the shared-memory kernel does
+			const bool decim = !h->p.boxcar && ds > 1 && h->p.downsample_passes > 0;
+			const int P = h->p.downsample_passes;
 			if (!h->d_work) {
-				RXB_CUDA(cudaMalloc(&h->d_work, (size_t)n_complex * sizeof(uint32_t)));
+				RXB_CUDA(cudaMalloc(&h->d_work, (size_t)n_slots * sizeof(uint32_t)));
 				RXB_CUDA(cudaMalloc(&h->d_fft, (size_t)nblk * N * sizeof(uint32_t)));
 				RXB_CUDA(cudaMalloc(&h->d_sums, 2 * sizeof(long long)));
+				if (decim) { decim_plan(n_slots, P, a.fir_on, h->n_sm, &h->decim_tile, &h->decim_smem); }
 			}
+			if (decim) {
+				// the attribute belongs to the kernel, not to this handle: allow the largest span any handle may plan
+				RXB_CUDA(cudaFuncSetAttribute(power_big_decim, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+			}
+			DecimFir fir;
+			for (int j = 0; j < 6; j++) { fir.c[j] = a.fir[j]; }
 			const int g = h->n_sm * 8;
 			for (int pass = 0; pass < n_pass; pass++) {
 				for (int hl = 0; hl < nh; hl++) {
 					const int16_t *src = d_hop_bufs + ((size_t)pass * nh + hl) * (size_t)h->p.buf_len;
 					RXB_CUDA(cudaMemsetAsync(h->d_sums, 0, 2 * sizeof(long long), h->stream));
-					power_big_load<<<g, 256, 0, h->stream>>>(src, h->d_work, n_complex, ds, h->d_sums);
-					power_big_window<<<g, 256, 0, h->stream>>>(h->d_work, h->d_fft, h->d_window, h->d_sums, used, (n_complex + ds - 1) / ds, h->p.bin_e, nblk);
+					if (decim) {
+						power_big_decim<<<(n_slots + h->decim_tile - 1) / h->decim_tile, 256, h->decim_smem, h->stream>>>(
+							src, h->d_work, n_slots, h->decim_tile, P, a.fir_on, fir, h->d_sums);
+					} else {
+						power_big_load<<<g, 256, 0, h->stream>>>(src, h->d_work, n_complex, ds, h->d_sums);
+					}
+					power_big_window<<<g, 256, 0, h->stream>>>(h->d_work, h->d_fft, h->d_window, h->d_sums, used, n_slots, h->p.bin_e, nblk);
 					for (int st = 0; st < h->p.bin_e; st++) { power_big_stage<<<g, 256, 0, h->stream>>>(h->d_fft, h->d_sine, h->p.bin_e, st, nblk); }
 					power_big_accum<<<g, 256, 0, h->stream>>>(h->d_fft, h->d_avg + (size_t)(hop_begin + hl) * N, h->p.bin_e, nblk, h->p.peak_hold);
 					RXB_CUDA(cudaGetLastError());
