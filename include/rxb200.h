@@ -162,7 +162,7 @@ typedef struct rxb200_fm_stats {
 	int warmup_len;
 	int kernel_kind;        /* 0: fm_fused_kernel (one segment per thread), 1: fm_split_kernel with warp rows (front and back
 	                           end on different items; the wbfm shape with 1..3 fifth_order passes, whole-row calls),
-	                           2: fm_split_kernel with per-thread segments (undecimated wbfm, behind a switch),
+	                           2: no longer produced (was fm_split_kernel with per-thread segments),
 	                           3: stream path, two launches -- fm_fused_kernel's front end alone (PCM to global memory), then
 	                              fm_back_kernel (the wbfm shape without decimating passes, long calls) */
 } rxb200_fm_stats;

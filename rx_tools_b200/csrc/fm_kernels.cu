@@ -194,43 +194,10 @@ __device__ __forceinline__ void front_store(const FrontState<P, SPEC> &s, uint32
 // B (lane = v + B, |v| <= B) the lane sum is < 64 B <= 32768, so no carry crosses lanes, and
 // (sum + 32 B) >> 4 == (sum >> 4) + 2 B exactly: the output lanes are biased by 2 B.  The int16
 // store of the reference never wraps here because |v| <= 128 << level after the 8-bit-range scale.
-// Pipe balance (HB_MAD): the integer adder/shifter pipe and the multiplier pipe each take a warp instruction every other
-// cycle; the row loop has ~550 instructions for the first against ~380 for the second, so the tap set's three adds are
-// the cheapest thing to move: as a chain of multiply-adds (inline PTX: the compiler would factor the sums out again)
-// the tap set costs four (HB_MAD 1) or five (HB_MAD 2: the last add through a multiplier the compiler cannot see
-// through, c_one == 1 in constant memory) multiplier-pipe instructions and one or none on the adder pipe.
-#ifndef HB_MAD
-#define HB_MAD 0
-#endif
-__constant__ int c_one = 1;
-__device__ __forceinline__ uint32_t mad_u32(uint32_t a, uint32_t b, uint32_t c)
-{
-	uint32_t d;
-	asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c));
-	return d;
-}
-template <int M>
-__device__ __forceinline__ uint32_t mad_imm(uint32_t a, uint32_t c)
-{
-	uint32_t d;
-	asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "n"(M), "r"(c));
-	return d;
-}
+// (Moving these adds onto the multiplier pipe did not pay: DESIGN.md §4.1, "Instruction rates".)
 __device__ __forceinline__ uint32_t hb_tap(uint32_t a, uint32_t b, uint32_t c, uint32_t d, uint32_t e, uint32_t f)
 {
-#if HB_MAD == 0
 	uint32_t s = a + f + (b + e) * 5u + (c + d) * 10u;
-#else
-	uint32_t s = mad_imm<5>(b, a);
-	s = mad_imm<5>(e, s);
-	s = mad_imm<10>(c, s);
-	s = mad_imm<10>(d, s);
-#if HB_MAD == 2
-	s = mad_u32(f, (uint32_t)c_one, s);
-#else
-	s += f;
-#endif
-#endif
 	return (s >> 4) & 0x0FFF0FFFu;
 }
 
@@ -390,9 +357,6 @@ __device__ __forceinline__ int fast_atan2_i(int y, int x)
 //   x >= 0: 4096 - sgn(n) T        x < 0: 12288 + sgn(n) T        negated for y < 0        0 for x == y == 0
 // which is the reference's truncating integer division on both branches (src/rtl_fm.c:485-506).  Returns the angle as
 // an integer-valued float.
-#ifndef DISC_F32
-#define DISC_F32 1
-#endif
 __device__ __forceinline__ float fast_atan2_f32(float y, float x)
 {
 	const float ax = fabsf(x), ay = fabsf(y);
@@ -418,13 +382,10 @@ __device__ __forceinline__ float fast_atan2_f32(float y, float x)
 // estimate's own: 4.1e-4 output units at most over 6 M operand pairs.  Whenever the fraction is within 1.5e-3 of an
 // integer (0.3 % of the samples) the truncation could go either way and the fp64 form decides.  Same results as
 // disc_std_lean; the algorithm restated in numpy and checked against fp64 atan2 (tests/test_host_logic.py::test_polar_disc_fp32_form).
-#ifndef DISC_STD_F32
-#define DISC_STD_F32 1
-#endif
 __device__ __forceinline__ int disc_std_f32(int cr, int cj)
 {
 	if (cj == 0 && cr >= 0) { return 0; }
-	if (!DISC_STD_F32 || (unsigned)cr + (1u << 24) >= (1u << 25) || (unsigned)cj + (1u << 24) >= (1u << 25)) { return disc_std_lean(cr, cj); }
+	if ((unsigned)cr + (1u << 24) >= (1u << 25) || (unsigned)cj + (1u << 24) >= (1u << 25)) { return disc_std_lean(cr, cj); }
 	const float ax = fabsf(__int2float_rn(cr)), ay = fabsf(__int2float_rn(cj));
 	const float a = fminf(ax, ay), b = fmaxf(ax, ay);                  // b >= 1
 	const float r = rcp_est(b);
@@ -617,13 +578,7 @@ __device__ __forceinline__ void post_decim(const FmDev &c, const FmCall &k, Fron
 __device__ __forceinline__ void scale_rot(uint32_t w, int pos, bool rotate, int &ri, int &rq, int dci = 0, int dcq = 0)
 {
 	// dc_block_raw_filter subtracts the chunk's running mean between the scale and the rotation (:850-857)
-	// SC_DP: the two halves of the CS16 word leave it through a two-way dot product (dp2a: I * 1 + Q * 0) instead of a
-	// byte permute / shift -- the same value from the other integer pipe (see HB_MAD)
-#ifndef SC_DP
-#define SC_DP 0
-#endif
-	const int wi16 = (SC_DP == 1 || SC_DP == 3) ? __dp2a_lo((int)w, 0x0001, 0) : lo16(w);
-	const int wq16 = (SC_DP == 1 || SC_DP == 2) ? __dp2a_lo((int)w, 0x0100, 0) : hi16(w);
+	const int wi16 = lo16(w), wq16 = hi16(w);
 	int xi = wrap16(scale_cs16(wi16) - dci), xq = wrap16(scale_cs16(wq16) - dcq);
 	if (!rotate) { pos = 0; }
 	switch (pos & 3) {
@@ -711,8 +666,7 @@ __device__ __forceinline__ void front_block(const FmDev &c, const FmCall &k, Fro
 		if (c.D == 1) {
 			// no decimation (-s at or above 1 Msps): every input sample is a PCM sample and a block is 8 consecutive entries of
 			// the global PCM array, 16-byte aligned (segments and halos are multiples of 8) -- one vector store per block
-			// instead of eight 2-byte stores to 32 different lines per warp.  Same arithmetic as post_decim's FM branch.
-#if DISC_F32
+			// instead of eight 2-byte stores to 32 different lines per warp.  Same results as post_decim's FM branch:
 			// the discriminator in FP32 (exact: see fast_atan2_f32); the angle leaves through the low 16 bits of
 			// angle + 1.5 * 2^23, two samples per byte permute
 			uint32_t ab[8];
@@ -738,26 +692,6 @@ __device__ __forceinline__ void front_block(const FmDev &c, const FmCall &k, Fro
 				w.z = __byte_perm(ab[4], ab[5], 0x5410); w.w = __byte_perm(ab[6], ab[7], 0x5410);
 				*reinterpret_cast<uint4 *>(e.out + e.m_lo + e.rel) = w;
 			}
-#else
-			int a[8];
-#pragma unroll
-			for (int j = 0; j < 8; j++) {
-				int di, dq;
-				scale_rot(v[j], j, rot, di, dq);
-				const int br = s.pre_i, bj = s.pre_q;
-				const int cr = add_w(mul_w(di, br), mul_w(dq, bj));
-				const int cj = sub_w(mul_w(dq, br), mul_w(di, bj));
-				// F8: the chunk's first sample (chunks start on block boundaries) goes through the libm discriminator
-				a[j] = (j == 0 && e.first_in_chunk) ? disc_std(cr, cj) : fast_atan2_i(cj, cr);
-				s.pre_i = di; s.pre_q = dq;
-			}
-			e.first_in_chunk = 0;
-			if (STORE) {
-				uint4 w;
-				w.x = pack2(a[0], a[1]); w.y = pack2(a[2], a[3]); w.z = pack2(a[4], a[5]); w.w = pack2(a[6], a[7]);
-				*reinterpret_cast<uint4 *>(e.out + e.m_lo + e.rel) = w;
-			}
-#endif
 			e.rel += 8;
 			return;
 		}
@@ -768,12 +702,7 @@ __device__ __forceinline__ void front_block(const FmDev &c, const FmCall &k, Fro
 		for (int j = 0; j < 8; j++) {
 			int xi, xq;
 			scale_rot(v[j], j, rot, xi, xq, e.rdc_i, e.rdc_q);
-			// BX_MAD: the running sums through the multiplier pipe (x * 1 + sum, see HB_MAD); 2: the I sum only
-#ifndef BX_MAD
-#define BX_MAD 0
-#endif
-			if (BX_MAD >= 1) { s.box_i = (int)mad_u32((uint32_t)xi, (uint32_t)c_one, (uint32_t)s.box_i); } else { s.box_i += xi; }
-			if (BX_MAD == 1) { s.box_q = (int)mad_u32((uint32_t)xq, (uint32_t)c_one, (uint32_t)s.box_q); } else { s.box_q += xq; }
+			s.box_i += xi; s.box_q += xq;
 			if (++s.box_n >= c.D) {
 				int di = wrap16(s.box_i), dq = wrap16(s.box_q);
 				s.box_i = 0; s.box_q = 0; s.box_n = 0;
@@ -831,9 +760,6 @@ __device__ __forceinline__ int pcm_load(const int16_t *pcm_s, int m) { return (i
 // (>= 1 / (2a)).  Two full-rate FP32 instructions on an 8-cycle dependency instead of subtract, 64-bit multiply-high
 // and add -- the multiply-high (IMAD.HI) is what the back kernel's warps were waiting for.  Bit-exact by construction
 // and by the parity suite; even a (ties round away from zero in the reference) keeps the integer form.
-#ifndef DEEMPH_F32
-#define DEEMPH_F32 1
-#endif
 #define DF_BIAS 0x4B008000
 template <bool EVEN, bool F32>
 struct DeemphOp {
@@ -892,8 +818,8 @@ struct DeemphOp<false, true> {
 	__device__ __forceinline__ State step(State s, Sample x) const { return __fmaf_rn(__fsub_rn(x, s), inv_a, s); }
 };
 template <bool EVEN>
-struct Deemph : DeemphOp<EVEN, (!EVEN && DEEMPH_F32 != 0)> {
-	__device__ __forceinline__ Deemph(const FmDev &c) : DeemphOp<EVEN, (!EVEN && DEEMPH_F32 != 0)>(c) {}
+struct Deemph : DeemphOp<EVEN, !EVEN> {
+	__device__ __forceinline__ Deemph(const FmDev &c) : DeemphOp<EVEN, !EVEN>(c) {}
 };
 
 // deemph_filter over PCM [m, m_end) of the shared buffer from BOTH bracket ends (replay before a
@@ -1750,17 +1676,16 @@ static fm_kernel_fn pick_back_kernel(int ws, int t)
 // move on to the next item; the hand-off is a pair of mbarriers per buffer (full: front end -> back end, empty:
 // back end -> front end), item tickets travel through shared memory.  An item still only ever waits for OLDER
 // items (look-back in back_item), every CTA of the grid is resident, so the oldest unfinished item always advances.
-//   FE 0: per-thread segments (front_item)   FE 1: warp rows with the droop FIR (fm_rows.cuh)   FE 2: rows, no FIR
+// The front end is the row front end (fm_rows.cuh: a warp per stretch, input through `in_map`); FIR: with the droop FIR.
 #define BAR_FE 2
 #define SPLIT_BE_MAX 128
-// The row front end reads its input through `in_map` (fm_rows.cuh); the segment front end ignores it.
-template <int P, int SPEC, int FE, int TMAX, int MINB>
+template <int P, int SPEC, bool FIR, int TMAX, int MINB>
 __global__ void __launch_bounds__(TMAX, MINB) fm_split_kernel(const FmDev c, const FmCall k, const __grid_constant__ CUtensorMap in_map)
 {
 	// [2][pcm_cap] PCM buffers, then the row exchange areas, then (from the next 1024-byte boundary) the row input rings
 	extern __shared__ __align__(16) int16_t pcm_s[];
 	__shared__ __align__(8) uint64_t s_full[2], s_empty[2];
-	__shared__ __align__(8) uint64_t s_ring_bar[FE == 0 ? 1 : (TMAX / 32) * ROWS_STAGES];
+	__shared__ __align__(8) uint64_t s_ring_bar[(TMAX / 32) * ROWS_STAGES];
 	__shared__ int s_ticket[2];
 	__shared__ int s_avg[SPLIT_BE_MAX], s_mrun[SPLIT_BE_MAX], s_start[SPLIT_BE_MAX];
 	__shared__ unsigned char s_ok[SPLIT_BE_MAX];
@@ -1771,22 +1696,18 @@ __global__ void __launch_bounds__(TMAX, MINB) fm_split_kernel(const FmDev c, con
 	if (tid == 0) {
 		mbar_init(&s_full[0], n_fe); mbar_init(&s_full[1], n_fe);
 		mbar_init(&s_empty[0], k.be_lanes); mbar_init(&s_empty[1], k.be_lanes);
-		if (FE != 0) {
-			for (int j = 0; j < k.fe_warps * ROWS_STAGES; j++) { mbar_init(&s_ring_bar[j], 1); }
-		}
+		for (int j = 0; j < k.fe_warps * ROWS_STAGES; j++) { mbar_init(&s_ring_bar[j], 1); }
 	}
 	__syncthreads();
 	const int total_work = k.n_ch * k.n_cta;
 	if (tid < n_fe) {
 		RowRing ring;
-		if (FE != 0) {
-			uint8_t *end = reinterpret_cast<uint8_t *>(pcm_s + 2 * (size_t)k.pcm_cap) + (size_t)k.fe_warps * k.xs_words * sizeof(uint32_t);
-			end += (0u - smem_u32(end)) & 1023u;
-			ring.map = &in_map;
-			ring.buf = end + (size_t)(tid >> 5) * ROWS_STAGES * ROW_BYTES;
-			ring.bar = s_ring_bar + (tid >> 5) * ROWS_STAGES;
-			ring.seq = 0;
-		}
+		uint8_t *end = reinterpret_cast<uint8_t *>(pcm_s + 2 * (size_t)k.pcm_cap) + (size_t)k.fe_warps * k.xs_words * sizeof(uint32_t);
+		end += (0u - smem_u32(end)) & 1023u;
+		ring.map = &in_map;
+		ring.buf = end + (size_t)(tid >> 5) * ROWS_STAGES * ROW_BYTES;
+		ring.bar = s_ring_bar + (tid >> 5) * ROWS_STAGES;
+		ring.seq = 0;
 		for (int i = 0;; i++) {
 			const int b = i & 1;
 			if (i >= 2) { mbar_wait(&s_empty[b], (uint32_t)(((i >> 1) - 1) & 1)); }   // the back end is done with item i-2
@@ -1799,12 +1720,9 @@ __global__ void __launch_bounds__(TMAX, MINB) fm_split_kernel(const FmDev c, con
 			if (work >= total_work) { mbar_arrive(&s_full[b]); break; }                // the back end sees the sentinel
 			const Item it = make_item(c, k, work);
 			int16_t *buf = pcm_s + (size_t)b * k.pcm_cap;
-			if constexpr (FE == 0) { front_item<P, SPEC>(c, k, it, tid, buf); }
-			else {
-				uint32_t *xs = reinterpret_cast<uint32_t *>(pcm_s + 2 * (size_t)k.pcm_cap) + (size_t)(tid >> 5) * k.xs_words;
-				front_rows<P, FE == 1>(c, k, it, tid >> 5, lane, buf, xs, ring);
-				rows_publish<P>(k, it, work, buf, tid >> 5, lane);
-			}
+			uint32_t *xs = reinterpret_cast<uint32_t *>(pcm_s + 2 * (size_t)k.pcm_cap) + (size_t)(tid >> 5) * k.xs_words;
+			front_rows<P, FIR>(c, k, it, tid >> 5, lane, buf, xs, ring);
+			rows_publish<P>(k, it, work, buf, tid >> 5, lane);
 			mbar_arrive(&s_full[b]);
 		}
 	} else {
@@ -1815,8 +1733,8 @@ __global__ void __launch_bounds__(TMAX, MINB) fm_split_kernel(const FmDev c, con
 			const int work = s_ticket[b];
 			if (work >= total_work) { break; }
 			const Item it = make_item(c, k, work);
-			if constexpr (FE != 0) { rows_collect<P>(k, it, work, pcm_s + (size_t)b * k.pcm_cap, q, k.be_lanes); }
-			back_item<SPEC, FE == 0 ? PCM_PAD_SEG : PCM_PAD_ROWS>(c, k, it, work, q, k.be_lanes, pcm_s + (size_t)b * k.pcm_cap, s_avg, s_mrun, s_ok, s_start);
+			rows_collect<P>(k, it, work, pcm_s + (size_t)b * k.pcm_cap, q, k.be_lanes);
+			back_item<SPEC, PCM_PAD_ROWS>(c, k, it, work, q, k.be_lanes, pcm_s + (size_t)b * k.pcm_cap, s_avg, s_mrun, s_ok, s_start);
 			mbar_arrive(&s_empty[b]);
 		}
 	}
@@ -1972,30 +1890,14 @@ typedef void (*fm_split_fn)(const FmDev, const FmCall, const CUtensorMap);
 static fm_split_fn pick_rows_kernel(int P, int fir_on)
 {
 #ifdef RXB_QUICK
-	return (P == 3 && fir_on) ? fm_split_kernel<3, 1, 1, ROWS_TMAX, ROWS_MINB> : nullptr;
+	return (P == 3 && fir_on) ? fm_split_kernel<3, 1, true, ROWS_TMAX, ROWS_MINB> : nullptr;
 #else
 	switch (P) {
-	case 1: return fir_on ? fm_split_kernel<1, 1, 1, ROWS_TMAX, ROWS_MINB> : fm_split_kernel<1, 1, 2, ROWS_TMAX, ROWS_MINB>;
-	case 2: return fir_on ? fm_split_kernel<2, 1, 1, ROWS_TMAX, ROWS_MINB> : fm_split_kernel<2, 1, 2, ROWS_TMAX, ROWS_MINB>;
-	case 3: return fir_on ? fm_split_kernel<3, 1, 1, ROWS_TMAX, ROWS_MINB> : fm_split_kernel<3, 1, 2, ROWS_TMAX, ROWS_MINB>;
+	case 1: return fir_on ? fm_split_kernel<1, 1, true, ROWS_TMAX, ROWS_MINB> : fm_split_kernel<1, 1, false, ROWS_TMAX, ROWS_MINB>;
+	case 2: return fir_on ? fm_split_kernel<2, 1, true, ROWS_TMAX, ROWS_MINB> : fm_split_kernel<2, 1, false, ROWS_TMAX, ROWS_MINB>;
+	case 3: return fir_on ? fm_split_kernel<3, 1, true, ROWS_TMAX, ROWS_MINB> : fm_split_kernel<3, 1, false, ROWS_TMAX, ROWS_MINB>;
 	default: return nullptr;
 	}
-#endif
-}
-// the split kernel with the SEGMENT front end: the undecimated wbfm shape (D <= 2 with de-emphasis), where the serial
-// stages are most of the work (62 % of the fused kernel's warp time is spent parked behind them)
-#ifndef SEGS_FE_THREADS
-#define SEGS_FE_THREADS 512
-#endif
-#ifndef SEGS_BE_LANES
-#define SEGS_BE_LANES 128
-#endif
-static fm_split_fn pick_segs_kernel(int P, int D, int deemph)
-{
-#ifdef RXB_QUICK
-	return nullptr;
-#else
-	return (P == 0 && D <= 2 && deemph) ? fm_split_kernel<0, 1, 0, SEGS_FE_THREADS + SEGS_BE_LANES, 1> : nullptr;
 #endif
 }
 
@@ -2054,15 +1956,10 @@ struct rxb200_fm {
 	rxb200_fm_stats stats;
 	fm_kernel_fn kern;
 	fm_split_fn kern_rows;         // split kernel with the row front end (null: shape not covered)
-	fm_split_fn kern_segs;         // split kernel with the segment front end (null: shape not covered)
 	fm_kernel_fn kern_front;       // stream path: front end alone (SPEC 4), PCM to global memory; fm_back_kernel follows
 	int16_t *d_pcm; size_t d_pcm_cap;   // its PCM scratch, int16 elements
-	size_t stream_min; int stream_piece, stream_win, stream_t, stream_warm_a;
+	size_t stream_min; int stream_piece, stream_win, stream_t;
 	int spec;
-	int last_rows;                 // 1: the last process call ran kern_rows
-	int rows_fe_warps, rows_be_lanes;
-	size_t segs_min;               // complex samples per call from which kern_segs is used
-	long long env_seg; int env_be_lanes;   // A/B knobs RXB200_FM_SEG / RXB200_FM_BE_LANES, read once at create
 	int threads;                   // CTA width of kern
 	int wide;                      // all-scalar fifth_order passes (raw DC block on)
 	int smem_optin, smem_per_sm, smem_reserved;
@@ -2173,17 +2070,17 @@ extern "C" int rxb200_fm_create(const rxb200_fm_params *params, int device, int 
 		int spec = h->wide ? 2 : ((params->mode == RXB200_MODE_FM && params->custom_atan == RXB200_ATAN_FAST &&
 		                           !params->offset_tuning && serial && plain) ? 1 : 0);
 		if (!h->wide && params->mode == RXB200_MODE_FM && params->custom_atan == RXB200_ATAN_LUT && !params->offset_tuning &&
-		    !serial && plain && params->downsample_passes == 0 && !getenv("RXB200_FM_NOSPEC3")) { spec = 3; }
+		    !serial && plain && params->downsample_passes == 0) { spec = 3; }
 		h->threads = fm_cta_threads(params->downsample_passes);
 		h->kern = pick_kernel(params->downsample_passes, spec, h->threads);
 		h->spec = spec;
 		const int fir_on = (params->downsample_passes > 0 && params->comp_fir_size == 9) ? 1 : 0;
-		h->kern_rows = (spec == 1 && !getenv("RXB200_FM_NOROWS")) ? pick_rows_kernel(params->downsample_passes, fir_on) : nullptr;
-		h->kern_segs = (spec == 1 && !getenv("RXB200_FM_NOSPLIT")) ? pick_segs_kernel(params->downsample_passes, params->downsample, params->deemph) : nullptr;
+		h->kern_rows = spec == 1 ? pick_rows_kernel(params->downsample_passes, fir_on) : nullptr;
 		// stream path (front kernel + back kernel): the wbfm shape without decimating passes, de-emphasis on
 #ifndef RXB_QUICK
-		h->kern_front = (spec == 1 && params->downsample_passes == 0 && params->deemph && !getenv("RXB200_FM_NOSTREAM")) ? pick_kernel(0, 4, h->threads) : nullptr;
+		h->kern_front = (spec == 1 && params->downsample_passes == 0 && params->deemph) ? pick_kernel(0, 4, h->threads) : nullptr;
 #endif
+		// stream path shape, read once (the tests reach shapes with them that a test-sized call would not pick)
 		h->stream_min = getenv("RXB200_FM_STREAM_MIN") ? (size_t)atoll(getenv("RXB200_FM_STREAM_MIN")) : (size_t)-1;   // -1: derived per call
 		h->stream_piece = getenv("RXB200_FM_STREAM_PIECE") ? atoi(getenv("RXB200_FM_STREAM_PIECE")) : 0;
 		{
@@ -2191,20 +2088,6 @@ extern "C" int rxb200_fm_create(const rxb200_fm_params *params, int device, int 
 			h->stream_win = (ws == 128 || ws == 256) ? ws : 128;
 			const int t = getenv("RXB200_FM_STREAM_T") ? atoi(getenv("RXB200_FM_STREAM_T")) : 0;
 			h->stream_t = (t == 32 || t == 64 || t == 128) ? t : 32;
-			const int wa = getenv("RXB200_FM_STREAM_WARM_A") ? atoi(getenv("RXB200_FM_STREAM_WARM_A")) : 0;
-			h->stream_warm_a = wa >= 16 ? wa : 20;
-		}
-		h->rows_fe_warps = ROWS_FE_WARPS; h->rows_be_lanes = ROWS_BE_LANES;
-		h->env_seg = getenv("RXB200_FM_SEG") ? atoll(getenv("RXB200_FM_SEG")) : 0;
-		h->env_be_lanes = getenv("RXB200_FM_BE_LANES") ? atoi(getenv("RXB200_FM_BE_LANES")) : 0;
-		// with de-emphasis at the capture rate (fm2a) the back end is a latency-bound chain of 16 a + 64 replay steps
-		// per piece and the split kernel's four back-end warps per SM finish an item later than the fused kernel's six
-		// -- the path stays behind a switch until the back end carries several pieces per lane
-		h->segs_min = getenv("RXB200_FM_SEGS_MIN") ? (size_t)atoll(getenv("RXB200_FM_SEGS_MIN")) : (size_t)-1;
-		{
-			// A/B knobs, read once at create: back-end lanes (32 | 64 ...) of the split kernel
-			const char *e = getenv("RXB200_FM_ROWS_BE");
-			if (e && atoi(e) >= 32 && atoi(e) <= SPLIT_BE_MAX && atoi(e) % 32 == 0 && ROWS_FE_WARPS * 32 + atoi(e) <= ROWS_TMAX) { h->rows_be_lanes = atoi(e); }
 		}
 	}
 	if (!h->kern) { set_error("no kernel for downsample_passes %d in this build", params->downsample_passes); delete h->h_lens; delete h; return RXB200_EUNSUPPORTED; }
@@ -2340,6 +2223,17 @@ static int fm_check_shape(const rxb200_fm *h, size_t n_int16, size_t chunk_int16
 
 static long long round_up_ll(long long v, long long g) { return ((v + g - 1) / g) * g; }
 
+// grows a device scratch buffer of the handle to at least `need` elements (the contents are not kept)
+template <typename T>
+static cudaError_t fm_reserve(T *&buf, size_t &cap, size_t need)
+{
+	if (need <= cap) { return cudaSuccess; }
+	cudaFree(buf); buf = nullptr; cap = 0;
+	const cudaError_t e = cudaMalloc(&buf, need * sizeof(T));
+	if (e == cudaSuccess) { cap = need; }
+	return e;
+}
+
 // ---- launch of the split kernel with the row front end (fm_rows.cuh).  Geometry in ROWS of ROW_LEN input samples:
 // an item owns `rows_own` rows; its PCM buffer also holds the `rows_margin` rows before them (the back end's replay
 // window), which the previous items of the channel hand over through global memory; the two PCM buffers and the
@@ -2394,7 +2288,7 @@ static int fm_launch_rows(rxb200_fm *h, const int16_t *d_in, size_t n_int16, siz
 	if (dv.deemph) { W_dec = h->tune_warm > 0 ? h->tune_warm : 16LL * p.deemph_a + 64; }
 	const long long margin_dec = W_dec + (dv.resample ? (p.rate_out / p.rate_out2 + 2) : 0) + 2;
 	const long long rows_margin = (margin_dec + row_pcm - 1) / row_pcm;
-	const int fe_warps = h->rows_fe_warps, be_lanes = h->rows_be_lanes;
+	const int fe_warps = ROWS_FE_WARPS, be_lanes = ROWS_BE_LANES;
 	const int threads = fe_warps * 32 + be_lanes;
 	CUtensorMap in_map;
 	{
@@ -2447,17 +2341,8 @@ static int fm_launch_rows(rxb200_fm *h, const int16_t *d_in, size_t n_int16, siz
 	if (per_sm < 1) { set_error("split kernel does not fit an SM (%zu bytes of shared memory, %d threads)", smem, threads); return RXB200_EUNSUPPORTED; }
 	const size_t total_work = (size_t)n_cta * h->n_channels;
 	const size_t need_sync = 4 + 4 * total_work;
-	if (need_sync > h->sync_cap) {
-		cudaFree(h->d_sync); h->d_sync = nullptr; h->sync_cap = 0;
-		RXB_CUDA(cudaMalloc(&h->d_sync, need_sync * sizeof(int)));
-		h->sync_cap = need_sync;
-	}
-	const size_t need_margin = total_work * (size_t)rows_margin * (size_t)row_pcm;
-	if (need_margin > h->margin_cap) {
-		cudaFree(h->d_margin); h->d_margin = nullptr; h->margin_cap = 0;
-		RXB_CUDA(cudaMalloc(&h->d_margin, need_margin * sizeof(int16_t)));
-		h->margin_cap = need_margin;
-	}
+	RXB_CUDA(fm_reserve(h->d_sync, h->sync_cap, need_sync));
+	RXB_CUDA(fm_reserve(h->d_margin, h->margin_cap, total_work * (size_t)rows_margin * (size_t)row_pcm));
 	FmCall k;
 	memset(&k, 0, sizeof k);
 	k.in = d_in; k.out = d_out; k.n = n; k.out_stride = (long long)out_stride; k.chunk = (int)(chunk_int16 / 2);
@@ -2477,73 +2362,8 @@ static int fm_launch_rows(rxb200_fm *h, const int16_t *d_in, size_t n_int16, siz
 	RXB_CUDA(cudaGetLastError());
 	RXB_CUDA(cudaEventRecord(h->ev1, h->stream));
 	h->cur ^= 1;
-	h->last_rows = 1;
 	h->stats.launches = 1; h->stats.segments = (int)(total_work * fe_warps); h->stats.segment_len = (int)(rows_own * ROW_LEN);
 	h->stats.warmup_len = (int)(W_dec << P); h->stats.fixup_segments = -1; h->stats.kernel_kind = 1;
-	return RXB200_OK;
-}
-
-// ---- launch of the split kernel with the segment front end: fm_launch's geometry for SEGS_FE_THREADS front-end
-// threads and two PCM buffers, one CTA per SM.
-static int fm_launch_segs(rxb200_fm *h, const int16_t *d_in, size_t n_int16, size_t chunk_int16, int16_t *d_out, size_t out_stride)
-{
-	const rxb200_fm_params &p = h->p;
-	const FmDev &dv = h->dev;
-	const long long n = (long long)(n_int16 / 2);
-	const int T = SEGS_FE_THREADS, be_lanes = SEGS_BE_LANES;
-	const long long D = dv.D, G = 8;
-	const long long halo = round_up_ll(3 * D, G);
-	const long long W_dec = h->tune_warm > 0 ? h->tune_warm : 16LL * p.deemph_a + 64;
-	const long long margin_dec = W_dec + (dv.resample ? (p.rate_out / p.rate_out2 + 2) : 0) + 2;
-	cudaFuncAttributes fa;
-	RXB_CUDA(cudaFuncGetAttributes(&fa, h->kern_segs));
-	const long long dyn_max = (long long)h->smem_optin - (long long)fa.sharedSizeBytes;
-	long long Sf = 0, n_extra = 0, pcm_cap = 0;
-	for (long long sf = h->tune_seg > 0 ? round_up_ll(h->tune_seg, G) : 4096; sf >= G; sf -= G) {
-		long long ne = (margin_dec * D + halo + sf - 1) / sf;
-		long long cap = (long long)T * (sf / D + 2) + 64;
-		cap += PCM_PAD_SEG * (cap >> 7) + 8;
-		cap = (cap + 7) & ~7LL;
-		if (2 * cap * (long long)sizeof(int16_t) <= dyn_max && ne <= T / 2) { Sf = sf; n_extra = ne; pcm_cap = cap; break; }
-	}
-	if (Sf == 0) { set_error("no segment length fits the split kernel's PCM buffers (replay %lld samples)", margin_dec * D); return RXB200_EUNSUPPORTED; }
-	const long long n_own = T - n_extra;
-	const long long n_cta = (n + n_own * Sf - 1) / (n_own * Sf);
-	const size_t smem = 2 * (size_t)pcm_cap * sizeof(int16_t);
-	RXB_CUDA(cudaFuncSetAttribute(h->kern_segs, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-	int per_sm = 1;
-	RXB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, h->kern_segs, T + be_lanes, smem));
-	if (per_sm < 1) { set_error("split kernel does not fit an SM (%zu bytes of shared memory)", smem); return RXB200_EUNSUPPORTED; }
-	const size_t total_work = (size_t)n_cta * h->n_channels;
-	const size_t need_sync = 4 + 4 * total_work;
-	if (need_sync > h->sync_cap) {
-		cudaFree(h->d_sync); h->d_sync = nullptr; h->sync_cap = 0;
-		RXB_CUDA(cudaMalloc(&h->d_sync, need_sync * sizeof(int)));
-		h->sync_cap = need_sync;
-	}
-	FmCall k;
-	memset(&k, 0, sizeof k);
-	k.in = d_in; k.out = d_out; k.n = n; k.out_stride = (long long)out_stride; k.chunk = (int)(chunk_int16 / 2);
-	k.n_ch = h->n_channels; k.Sf = (int)Sf; k.halo = (int)halo; k.n_extra = (int)n_extra; k.n_own = (int)n_own;
-	k.n_cta = (int)n_cta; k.W_dec = (int)W_dec; k.pcm_cap = (int)pcm_cap; k.direct_out = 0;
-	k.be_lanes = be_lanes; k.fe_threads = T; k.fe_warps = T / 32; k.xs_words = 0;
-	k.state_words = h->state_words; k.carry_in = h->d_carry[h->cur]; k.carry_out = h->d_carry[h->cur ^ 1];
-	k.ticket = h->d_sync; k.fix_count = h->d_sync + 1; k.pub = h->d_sync + 4;
-	k.n_chunks = (int)((n + k.chunk - 1) / k.chunk);
-	k.reduce_mode = 0; k.one = 1;
-	size_t blocks = (size_t)h->n_sm * per_sm;
-	if (blocks > total_work) { blocks = total_work; }
-	RXB_CUDA(cudaMemsetAsync(h->d_sync, 0, need_sync * sizeof(int), h->stream));
-	RXB_CUDA(cudaEventRecord(h->ev0, h->stream));
-	CUtensorMap no_map;                                  // the segment front end reads its input directly
-	memset(&no_map, 0, sizeof no_map);
-	h->kern_segs<<<(unsigned)blocks, T + be_lanes, smem, h->stream>>>(dv, k, no_map);
-	RXB_CUDA(cudaGetLastError());
-	RXB_CUDA(cudaEventRecord(h->ev1, h->stream));
-	h->cur ^= 1;
-	h->last_rows = 1;
-	h->stats.launches = 1; h->stats.segments = (int)(total_work * T); h->stats.segment_len = (int)Sf;
-	h->stats.warmup_len = (int)(W_dec * D); h->stats.fixup_segments = -1; h->stats.kernel_kind = 2;
 	return RXB200_OK;
 }
 
@@ -2551,9 +2371,6 @@ static int fm_launch(rxb200_fm *h, const int16_t *d_in, size_t n_int16, size_t c
                      size_t out_stride)
 {
 	if (fm_rows_shape_ok(h, n_int16, chunk_int16)) { return fm_launch_rows(h, d_in, n_int16, chunk_int16, d_out, out_stride); }
-	// the split kernel pays off once there are a few items per SM; short calls (streaming chunks) stay on the fused kernel
-	if (h->kern_segs && n_int16 / 2 >= h->segs_min) { return fm_launch_segs(h, d_in, n_int16, chunk_int16, d_out, out_stride); }
-	h->last_rows = 0;
 	const rxb200_fm_params &p = h->p;
 	const FmDev &dv = h->dev;
 	const long long n = (long long)(n_int16 / 2);
@@ -2581,7 +2398,7 @@ static int fm_launch(rxb200_fm *h, const int16_t *d_in, size_t n_int16, size_t c
 	// mod a that merges them -- a geometric wait with mean a.  16 a + 64 steps leave a fraction of a percent of the pieces
 	// open, each of which costs its item a probe and a second pass; with the stream path's long pieces
 	// four more a's of replay (e^-4: ~0.01 %) are cheaper than those stragglers.
-	if (stream && dv.deemph && h->tune_warm <= 0) { wd = (long long)h->stream_warm_a * p.deemph_a + 64; }
+	if (stream && dv.deemph && h->tune_warm <= 0) { wd = 20LL * p.deemph_a + 64; }
 	const fm_kernel_fn kern = stream ? h->kern_front : h->kern;
 	const int direct_out = stream ? 1 : ((dv.mode == RXB200_MODE_RAW || (!dv.deemph && !dv.resample && !dv.adc_on)) ? 1 : 0);
 	const long long W_dec = direct_out ? 0 : wd;
@@ -2589,7 +2406,6 @@ static int fm_launch(rxb200_fm *h, const int16_t *d_in, size_t n_int16, size_t c
 	const long long margin_dec = direct_out ? 0 : W_dec + (dv.resample ? (p.rate_out / p.rate_out2 + 2) : 0) + 2;
 	// segment per thread: ~128 decimated samples, at least 4 halos, capped so the PCM buffer stays small
 	long long Sf = h->tune_seg;
-	if (Sf <= 0) { Sf = h->env_seg; }
 	if (Sf <= 0) {
 		Sf = 128 * Dpcm;
 		if (Sf > 2048) { Sf = 2048; }
@@ -2607,9 +2423,9 @@ static int fm_launch(rxb200_fm *h, const int16_t *d_in, size_t n_int16, size_t c
 		const long long l = Dpcm / a * 8;
 		if (l <= 1024) { Gs = l; }
 	}
-	if (h->tune_seg <= 0 && h->env_seg <= 0 && Sf >= 2 * Gs) { Sf = (Sf / Gs) * Gs; }
+	if (h->tune_seg <= 0 && Sf >= 2 * Gs) { Sf = (Sf / Gs) * Gs; }
 	Sf = round_up_ll(Sf, G);
-	const bool sf_forced = (h->tune_seg > 0) || (h->env_seg > 0);
+	const bool sf_forced = h->tune_seg > 0;
 	long long n_extra = 0, n_own = 0, stretch = 0, n_cta = 0, ppt = 0, pcm_cap = 0;
 	size_t smem = 0;
 	auto geometry = [&](long long sf) -> bool {
@@ -2691,20 +2507,11 @@ static int fm_launch(rxb200_fm *h, const int16_t *d_in, size_t n_int16, size_t c
 		span = piece * back_t * Dpcm;
 		n_cta_b = (n + span - 1) / span;
 		pstride = (m_total + back_ws + 64 + 7) & ~7LL;      // a window may reach past the last sample
-		const size_t need = (size_t)pstride * h->n_channels;
-		if (need > h->d_pcm_cap) {
-			cudaFree(h->d_pcm); h->d_pcm = nullptr; h->d_pcm_cap = 0;
-			RXB_CUDA(cudaMalloc(&h->d_pcm, need * sizeof(int16_t)));
-			h->d_pcm_cap = need;
-		}
+		RXB_CUDA(fm_reserve(h->d_pcm, h->d_pcm_cap, (size_t)pstride * h->n_channels));
 	}
 	const size_t total_back = (size_t)n_cta_b * h->n_channels;
 	const size_t need_sync = 4 + 4 * (total_work > total_back ? total_work : total_back);
-	if (need_sync > h->sync_cap) {
-		cudaFree(h->d_sync); h->d_sync = nullptr; h->sync_cap = 0;
-		RXB_CUDA(cudaMalloc(&h->d_sync, need_sync * sizeof(int)));
-		h->sync_cap = need_sync;
-	}
+	RXB_CUDA(fm_reserve(h->d_sync, h->sync_cap, need_sync));
 	FmCall k;
 	memset(&k, 0, sizeof k);
 	k.in = d_in; k.out = d_out; k.n = n; k.out_stride = (long long)out_stride; k.chunk = (int)(chunk_int16 / 2);
@@ -2714,11 +2521,9 @@ static int fm_launch(rxb200_fm *h, const int16_t *d_in, size_t n_int16, size_t c
 	{
 		// back-end width: enough lanes that a piece is about half a replay long (more lanes shorten the
 		// phase in which the other warps idle, but every lane pays the full replay)
-		const char *e = h->env_be_lanes > 0 ? "x" : nullptr;
 		const long long item_pcm = n_own * Sf / Dpcm;
-		long long want = W_dec > 0 ? (2 * item_pcm / W_dec + 31) / 32 * 32 : 128;
-		int bl = e ? h->env_be_lanes : (int)want;
-		bl = (bl / 32) * 32;
+		const long long want = W_dec > 0 ? (2 * item_pcm / W_dec + 31) / 32 * 32 : 128;
+		int bl = (int)want;
 		if (bl < 32) { bl = 32; }
 		if (bl > T) { bl = T; }
 		k.be_lanes = bl;
@@ -2866,16 +2671,8 @@ extern "C" int rxb200_fm_process(rxb200_fm *h, const int16_t *cs16, size_t n_int
 	if (total > pcm_stride) { set_error("pcm_stride %zu < %zu outputs", pcm_stride, total); return RXB200_ECAPACITY; }
 	size_t in_elems = n_int16 * (size_t)h->n_channels;
 	size_t out_elems = (total + 8) * (size_t)h->n_channels;
-	if (in_elems > h->d_in_cap) {
-		cudaFree(h->d_in); h->d_in = nullptr; h->d_in_cap = 0;
-		RXB_CUDA(cudaMalloc(&h->d_in, in_elems * sizeof(int16_t)));
-		h->d_in_cap = in_elems;
-	}
-	if (out_elems > h->d_out_cap) {
-		cudaFree(h->d_out); h->d_out = nullptr; h->d_out_cap = 0;
-		RXB_CUDA(cudaMalloc(&h->d_out, out_elems * sizeof(int16_t)));
-		h->d_out_cap = out_elems;
-	}
+	RXB_CUDA(fm_reserve(h->d_in, h->d_in_cap, in_elems));
+	RXB_CUDA(fm_reserve(h->d_out, h->d_out_cap, out_elems));
 	RXB_CUDA(cudaMemcpyAsync(h->d_in, cs16, in_elems * sizeof(int16_t), cudaMemcpyHostToDevice, h->stream));
 	rc = fm_launch(h, h->d_in, n_int16, chunk_int16, h->d_out, total + 8);
 	if (rc != RXB200_OK) { return rc; }

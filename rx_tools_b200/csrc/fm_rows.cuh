@@ -213,12 +213,8 @@ __device__ __forceinline__ void row_body(const FmDev &c, uint32_t *xs, int par, 
 	// plus less than 32 for the floors -- and |cr| + |cj| <= 4 d^2 < 1.2e7 < 2^24
 	// (tests/test_host_logic.py::test_row_discriminator_operands_fit_fp32 recomputes the bound from the table).
 	// The FP32 form issues every cycle and leaves the adder pipe, which bounds this loop, ~16 instructions per output
-	// lighter.  ROWS_DISC_F32 0: the integer form.
-#ifndef ROWS_DISC_F32
-#define ROWS_DISC_F32 1
-#endif
+	// lighter than the integer form (DESIGN.md §4.1).
 	uint32_t wpk[NV / 2];                  // PCM, two samples per word
-#if ROWS_DISC_F32
 	{
 		uint32_t ab[NV];
 #pragma unroll
@@ -230,18 +226,6 @@ __device__ __forceinline__ void row_body(const FmDev &c, uint32_t *xs, int par, 
 #pragma unroll
 		for (int j = 0; j < NV; j += 2) { wpk[j / 2] = __byte_perm(ab[j], ab[j + 1], 0x5410); }
 	}
-#else
-	{
-		int pcm[NV];
-#pragma unroll
-		for (int j = 0; j < NV; j++) {
-			pcm[j] = fast_atan2_i(cj[j], cr[j]);
-			if (CS && j == 0 && lane == 0) { pcm[0] = disc_std(cr[0], cj[0]); }
-		}
-#pragma unroll
-		for (int j = 0; j < NV; j += 2) { wpk[j / 2] = ((uint32_t)pcm[j] & 0xffffu) | ((uint32_t)pcm[j + 1] << 16); }
-	}
-#endif
 	int16_t *dst = pcm_s + pcm_phys<PCM_PAD_ROWS>(rel);
 #pragma unroll
 	for (int j = 0; j < NV; j += 4) {

@@ -153,7 +153,7 @@ class FmDemod:
         s = _lib.FmStatsC()
         _lib.check(_lib.lib().rxb200_fm_last_stats(self._h, C.byref(s)))
         d = {f[0]: int(getattr(s, f[0])) for f in s._fields_}
-        d["kernel"] = {1: "fm_split_kernel", 2: "fm_split_kernel", 3: "fm_fused_kernel+fm_back_kernel"}.get(d["kernel_kind"], "fm_fused_kernel")
+        d["kernel"] = {1: "fm_split_kernel", 3: "fm_fused_kernel+fm_back_kernel"}.get(d["kernel_kind"], "fm_fused_kernel")
         return d
 
 

@@ -208,20 +208,21 @@ def test_levels(case, port):
 
 @pytest.mark.parametrize("seg", [0, 32, 64])
 @pytest.mark.parametrize("name", ["cfg2A", "zeros_deemph"])
-def test_split_kernel_with_segment_front_end(name, seg, port, monkeypatch):
-    """The undecimated wbfm shape on long calls runs the split kernel with per-thread segments (front-end threads and
-    back-end warps on different items, two PCM buffers).  RXB200_FM_SEGS_MIN=0 selects it for a test-sized call."""
-    monkeypatch.setenv("RXB200_FM_SEGS_MIN", "0")
+def test_fused_kernel_on_undecimated_wbfm(name, seg, port, monkeypatch):
+    """The undecimated wbfm shape on short-to-medium calls (streaming chunks) runs the fused kernel: per-thread segments,
+    then the CTA's first warps run the serial stages.  RXB200_FM_STREAM_MIN above the call length keeps a test-sized call
+    off the stream path."""
     case = next(c for c in fm_cases() if c.name == name)
     x = case.make_input()
+    monkeypatch.setenv("RXB200_FM_STREAM_MIN", str(x.size // 2 + 1))
     want = port.fm_run(case.params, x, case.chunk_int16)
     d = fm.FmDemod(case.params)
     if seg:
         d.tune(segment_len=seg)
     got = d.full_demod(x, case.chunk_int16)
     _compare(case, got, want)
-    assert d.stats()["kernel_kind"] == 2
-    # streaming: the carry written by the split kernel feeds the next call
+    assert d.stats()["kernel_kind"] == 0
+    # streaming: the carry written by the fused kernel feeds the next call
     d.reset()
     cut = (x.size // 3 // case.chunk_int16) * case.chunk_int16 or case.chunk_int16
     got2 = np.concatenate([d.full_demod(x[:cut], case.chunk_int16), d.full_demod(x[cut:], case.chunk_int16)])

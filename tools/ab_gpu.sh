@@ -50,6 +50,4 @@ for w in fm2a fm1 fm5a; do
 done
 # ---- CTA width against the shape (boxcar kernels exist in both widths), front end alone against the full chain
 timeout 300 python tools/width_sweep.py > $OUT/width_sweep.txt 2>&1; echo "width sweep rc=$? t=$((SECONDS-T0))"; cat $OUT/width_sweep.txt
-# ---- run-time knobs of the winner (replay length, back-end lanes)
-if [ -n "$AB_KNOBS" ]; then timeout 200 python tools/ab_sweep.py > $OUT/sweep.txt 2>&1; echo "sweep rc=$? t=$((SECONDS-T0))"; cat $OUT/sweep.txt; fi
 date
