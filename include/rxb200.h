@@ -170,8 +170,9 @@ int rxb200_fm_last_stats(rxb200_fm *h, rxb200_fm_stats *out);
 /* Tuning knobs (0 keeps the automatic choice): segment length in complex samples, de-emphasis
  * warm-up in decimated samples. */
 int rxb200_fm_tune(rxb200_fm *h, int segment_len, int deemph_warmup);
-/* Device time (CUDA events on the handle's stream) of the fused kernel alone in the last process
- * call, in milliseconds.  Synchronises the stream. */
+/* Device time (CUDA events on the handle's stream) of the last process call's main kernels, in
+ * milliseconds: the split kernel on the row path, the fused kernel's main pass (not its per-chunk
+ * reduction pre-passes), or the front and back kernels on the stream path.  Synchronises the stream. */
 int rxb200_fm_kernel_ms(rxb200_fm *h, float *ms);
 
 /* ======================================================================== rx_power

@@ -1935,38 +1935,38 @@ static const int k_droop9_host[11][10] = {
 };
 
 struct rxb200_fm {
-	rxb200_fm_params p;
-	int device;
-	int n_channels;
-	int n_sm;
-	FmDev dev;
-	int state_words;
-	cudaStream_t stream;
-	uint32_t *d_carry[2];
-	int cur;                       // which carry buffer holds the current state
-	int *d_sync; size_t sync_cap;  // [0] ticket, [1] fix_count, [4..] pub[n_ch*n_cta][4]
-	int16_t *d_margin; size_t margin_cap;   // row front end: margin hand-over slots (int16 entries)
-	int *d_atan_lut;
-	int16_t *d_in; size_t d_in_cap;                // int16 elements
-	int16_t *d_out; size_t d_out_cap;
+	rxb200_fm_params p{};
+	int device = 0;
+	int n_channels = 0;
+	int n_sm = 0;
+	FmDev dev{};
+	int state_words = 0;
+	cudaStream_t stream = nullptr;
+	uint32_t *d_carry[2] = {nullptr, nullptr};
+	int cur = 0;                   // which carry buffer holds the current state
+	int *d_sync = nullptr; size_t sync_cap = 0;  // [0] ticket, [1] fix_count, [4..] pub[n_ch*n_cta][4]
+	int16_t *d_margin = nullptr; size_t margin_cap = 0;   // row front end: margin hand-over slots (int16 entries)
+	int *d_atan_lut = nullptr;
+	int16_t *d_in = nullptr; size_t d_in_cap = 0;         // int16 elements
+	int16_t *d_out = nullptr; size_t d_out_cap = 0;
 	// host mirror of the closed-form counters
-	int h_box_n;                   // demod.prev_index
-	int h_lpr_phase;               // demod.prev_lpr_index
-	int tune_seg, tune_warm;
-	rxb200_fm_stats stats;
-	fm_kernel_fn kern;
-	fm_split_fn kern_rows;         // split kernel with the row front end (null: shape not covered)
-	fm_kernel_fn kern_front;       // stream path: front end alone (SPEC 4), PCM to global memory; fm_back_kernel follows
-	int16_t *d_pcm; size_t d_pcm_cap;   // its PCM scratch, int16 elements
-	size_t stream_min; int stream_piece, stream_win, stream_t;
-	int spec;
-	int threads;                   // CTA width of kern
-	int wide;                      // all-scalar fifth_order passes (raw DC block on)
-	int smem_optin, smem_per_sm, smem_reserved;
-	// per-chunk reduction stages
-	long long *d_sums; int *d_rdc, *d_sqz, *d_adc, *d_lens, *d_levels; size_t chunk_cap; int level_chunks;
-	std::vector<int> *h_lens;
-	cudaEvent_t ev0, ev1;
+	int h_box_n = 0;               // demod.prev_index
+	int h_lpr_phase = 0;           // demod.prev_lpr_index
+	int tune_seg = 0, tune_warm = 0;
+	rxb200_fm_stats stats{};
+	fm_kernel_fn kern = nullptr;
+	fm_split_fn kern_rows = nullptr;     // split kernel with the row front end (null: shape not covered)
+	fm_kernel_fn kern_front = nullptr;   // stream path: front end alone (SPEC 4), PCM to global memory; fm_back_kernel follows
+	int16_t *d_pcm = nullptr; size_t d_pcm_cap = 0;       // its PCM scratch, int16 elements
+	size_t stream_min = 0; int stream_piece = 0, stream_win = 0, stream_t = 0;
+	int threads = 0;               // CTA width of kern
+	int wide = 0;                  // all-scalar fifth_order passes (raw DC block on)
+	int smem_optin = 0, smem_per_sm = 0, smem_reserved = 0;
+	// per-chunk reduction stages, capacities in elements
+	long long *d_sums = nullptr; int *d_rdc = nullptr, *d_sqz = nullptr, *d_adc = nullptr, *d_lens = nullptr, *d_levels = nullptr;
+	size_t sums_cap = 0, rdc_cap = 0, sqz_cap = 0, adc_cap = 0, lens_cap = 0, levels_cap = 0; int level_chunks = 0;
+	std::vector<int> h_lens;       // host side of d_lens
+	cudaEvent_t ev0 = nullptr, ev1 = nullptr;
 };
 
 static int fm_validate(const rxb200_fm_params *p)
@@ -2056,13 +2056,11 @@ extern "C" int rxb200_fm_create(const rxb200_fm_params *params, int device, int 
 	RXB_CUDA(cudaSetDevice(device));
 	rxb200_fm *h = new (std::nothrow) rxb200_fm();
 	if (!h) { return RXB200_ENOMEM; }
-	memset(h, 0, sizeof *h);
 	h->p = *params; h->device = device; h->n_channels = n_channels;
 	// any per-chunk reduction stage selects the SPEC 2 kernel (all-scalar passes + stage bookkeeping)
 	h->wide = (params->dc_block_raw || params->squelch_level || params->dc_block_audio || params->post_downsample > 1 ||
 	           params->report_levels) ? 1 : 0;
 	h->state_words = fm_state_words(params->downsample_passes, h->wide);
-	h->h_lens = new std::vector<int>();
 	{
 		// wbfm shape: FM + fast_atan2 + rotation, with a serial stage (de-emphasis or resampler)
 		const bool serial = (params->deemph != 0) || (params->rate_out2 > 0);
@@ -2073,7 +2071,6 @@ extern "C" int rxb200_fm_create(const rxb200_fm_params *params, int device, int 
 		    !serial && plain && params->downsample_passes == 0) { spec = 3; }
 		h->threads = fm_cta_threads(params->downsample_passes);
 		h->kern = pick_kernel(params->downsample_passes, spec, h->threads);
-		h->spec = spec;
 		const int fir_on = (params->downsample_passes > 0 && params->comp_fir_size == 9) ? 1 : 0;
 		h->kern_rows = spec == 1 ? pick_rows_kernel(params->downsample_passes, fir_on) : nullptr;
 		// stream path (front kernel + back kernel): the wbfm shape without decimating passes, de-emphasis on
@@ -2090,7 +2087,7 @@ extern "C" int rxb200_fm_create(const rxb200_fm_params *params, int device, int 
 			h->stream_t = (t == 32 || t == 64 || t == 128) ? t : 32;
 		}
 	}
-	if (!h->kern) { set_error("no kernel for downsample_passes %d in this build", params->downsample_passes); delete h->h_lens; delete h; return RXB200_EUNSUPPORTED; }
+	if (!h->kern) { set_error("no kernel for downsample_passes %d in this build", params->downsample_passes); delete h; return RXB200_EUNSUPPORTED; }
 	cudaDeviceProp prop;
 	RXB_CUDA_OR(cudaGetDeviceProperties(&prop, device), rxb200_fm_destroy(h));
 	h->n_sm = prop.multiProcessorCount;
@@ -2148,7 +2145,6 @@ extern "C" void rxb200_fm_destroy(rxb200_fm *h)
 	cudaFree(h->d_carry[0]); cudaFree(h->d_carry[1]); cudaFree(h->d_sync); cudaFree(h->d_margin);
 	cudaFree(h->d_atan_lut); cudaFree(h->d_in); cudaFree(h->d_out); cudaFree(h->d_pcm);
 	cudaFree(h->d_sums); cudaFree(h->d_rdc); cudaFree(h->d_sqz); cudaFree(h->d_adc); cudaFree(h->d_lens); cudaFree(h->d_levels);
-	delete h->h_lens;
 	if (h->ev0) { cudaEventDestroy(h->ev0); }
 	if (h->ev1) { cudaEventDestroy(h->ev1); }
 	if (h->stream) { cudaStreamDestroy(h->stream); }
@@ -2164,10 +2160,11 @@ extern "C" int rxb200_fm_kernel_ms(rxb200_fm *h, float *ms)
 	return RXB200_OK;
 }
 
-// closed-form per-chunk result_len; advances the host mirrors when commit is set
-static size_t fm_count_outputs(rxb200_fm *h, size_t n_int16, size_t chunk_int16, int *chunk_result_len, bool commit)
+// closed-form per-chunk result_len, and the pre-passes' chunk table when `lens` is given; advances the host mirrors when commit is set
+static size_t fm_count_outputs(rxb200_fm *h, size_t n_int16, size_t chunk_int16, int *chunk_result_len, int *lens, bool commit)
 {
 	const rxb200_fm_params &p = h->p;
+	const size_t n_chunks = (n_int16 + chunk_int16 - 1) / chunk_int16;
 	long long box_n = h->h_box_n, phase = h->h_lpr_phase;
 	size_t total = 0, pos = 0, c = 0;
 	while (pos < n_int16) {
@@ -2175,11 +2172,10 @@ static size_t fm_count_outputs(rxb200_fm *h, size_t n_int16, size_t chunk_int16,
 		long long L = (long long)(len16 / 2), dec;
 		if (p.downsample_passes) { dec = L >> p.downsample_passes; }
 		else { dec = (box_n + L) / p.downsample; box_n = (box_n + L) % p.downsample; }
-		if (h->dev.post_ds > 1) {
-			// low_pass_simple needs a whole number of groups per chunk (otherwise the reference reads stale data)
-			if (dec % h->dev.post_ds != 0) { return (size_t)-1; }
-			dec /= h->dev.post_ds;
-		}
+		// low_pass_simple needs a whole number of groups per chunk (otherwise the reference reads stale data)
+		if (dec % h->dev.post_ds != 0) { return (size_t)-1; }
+		if (lens) { lens[c] = (int)L; lens[n_chunks + c] = (int)dec; lens[2 * n_chunks + c] = (int)(dec / h->dev.post_ds); }
+		dec /= h->dev.post_ds;
 		long long res;
 		if (p.mode == RXB200_MODE_RAW) { res = 2 * dec; }
 		else if (p.rate_out2 > 0) {
@@ -2234,16 +2230,34 @@ static cudaError_t fm_reserve(T *&buf, size_t &cap, size_t need)
 	return e;
 }
 
-// ---- launch of the split kernel with the row front end (fm_rows.cuh).  Geometry in ROWS of ROW_LEN input samples:
-// an item owns `rows_own` rows; its PCM buffer also holds the `rows_margin` rows before them (the back end's replay
-// window), which the previous items of the channel hand over through global memory; the two PCM buffers and the
-// warps' exchange areas share the CTA's dynamic shared memory.
-static bool fm_rows_shape_ok(const rxb200_fm *h, size_t n_int16, size_t chunk_int16)
+// Back-end replay in decimated samples: the de-emphasis bracket in front of a piece, 0 without de-emphasis.  The bracket
+// closes in two phases: the gap contracts by (1 - 1/a) per step (to 1 within ~11 a steps from the full int16 range), then
+// the two trajectories sit one apart until a sample lands on the one residue mod a that merges them -- a geometric wait
+// with mean a.  16 a + 64 steps leave a fraction of a percent of the pieces open, each of which costs its item a probe and
+// a second pass; with the stream path's long pieces four more a's of replay (e^-4: ~0.01 %) are cheaper than those
+// stragglers.
+static long long fm_replay(const rxb200_fm *h, bool stream)
 {
-	if (!h->kern_rows) { return false; }
-	const size_t n = n_int16 / 2, chunk = chunk_int16 / 2;
-	return chunk % ROW_LEN == 0 && n % ROW_LEN == 0 && n >= 16 * (size_t)ROW_LEN;
+	if (!h->dev.deemph) { return 0; }
+	if (h->tune_warm > 0) { return h->tune_warm; }
+	return (stream ? 20LL : 16LL) * h->p.deemph_a + 64;
 }
+
+// PCM a back end needs from before its stretch (decimated samples): the replay plus the resampler group in progress
+static long long fm_margin(const rxb200_fm *h, long long W_dec)
+{
+	return W_dec + (h->dev.resample ? (h->p.rate_out / h->p.rate_out2 + 2) : 0) + 2;
+}
+
+// sets a kernel's dynamic shared memory to `smem` and returns how many of its CTAs fit an SM
+template <typename K>
+static cudaError_t fm_occupancy(K kern, int threads, size_t smem, int *per_sm)
+{
+	const cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+	return e != cudaSuccess ? e : cudaOccupancyMaxActiveBlocksPerMultiprocessor(per_sm, kern, threads, smem);
+}
+
+struct FmGrid { int threads, per_sm; size_t smem; };   // CTA width, resident CTAs per SM, dynamic shared memory
 
 // The row front end's view of the input: [n_ch * n / 32] lines of 32 words (128 bytes), one box = one row
 // (32 lines), 128-byte swizzle (fm_rows.cuh).  cuTensorMapEncodeTiled comes from the driver at run time, so the
@@ -2276,25 +2290,20 @@ static int fm_rows_map(const int16_t *d_in, long long lines, CUtensorMap *map)
 	return RXB200_OK;
 }
 
-static int fm_launch_rows(rxb200_fm *h, const int16_t *d_in, size_t n_int16, size_t chunk_int16, int16_t *d_out, size_t out_stride)
+// ---- the split kernel with the row front end (fm_rows.cuh).  Geometry in ROWS of ROW_LEN input samples:
+// an item owns `rows_own` rows; its PCM buffer also holds the `rows_margin` rows before them (the back end's replay
+// window), which the previous items of the channel hand over through global memory; the two PCM buffers and the
+// warps' exchange areas share the CTA's dynamic shared memory.
+static int fm_plan_rows(const rxb200_fm *h, long long n, FmCall *k, FmGrid *g)
 {
-	const rxb200_fm_params &p = h->p;
-	const FmDev &dv = h->dev;
-	const long long n = (long long)(n_int16 / 2);
-	const int P = p.downsample_passes;
+	const int P = h->p.downsample_passes;
 	const long long rows_total = n / ROW_LEN;
 	const long long row_pcm = ROW_LEN >> P;                 // PCM samples per row
-	long long W_dec = 0;
-	if (dv.deemph) { W_dec = h->tune_warm > 0 ? h->tune_warm : 16LL * p.deemph_a + 64; }
-	const long long margin_dec = W_dec + (dv.resample ? (p.rate_out / p.rate_out2 + 2) : 0) + 2;
+	const long long W_dec = fm_replay(h, false);
+	const long long margin_dec = fm_margin(h, W_dec);
 	const long long rows_margin = (margin_dec + row_pcm - 1) / row_pcm;
 	const int fe_warps = ROWS_FE_WARPS, be_lanes = ROWS_BE_LANES;
 	const int threads = fe_warps * 32 + be_lanes;
-	CUtensorMap in_map;
-	{
-		const int rc = fm_rows_map(d_in, (long long)h->n_channels * (n / 32), &in_map);
-		if (rc != RXB200_OK) { return rc; }
-	}
 	const int xs_words = rows_xs_words(P);
 	// exchange areas, then the input rings from the next 1024-byte boundary (up to 1008 bytes of padding)
 	const size_t xs_bytes = (size_t)fe_warps * xs_words * sizeof(uint32_t) + 1008 + (size_t)fe_warps * ROWS_STAGES * ROW_BYTES;
@@ -2331,79 +2340,31 @@ static int fm_launch_rows(rxb200_fm *h, const int16_t *d_in, size_t n_int16, siz
 		}
 	}
 	if (rows_own > rows_total) { rows_own = rows_total; }
-	rows_item = rows_own + rows_margin;
-	const long long pcm_cap = cap_for(rows_item);
-	const size_t smem = 2 * (size_t)pcm_cap * sizeof(int16_t) + xs_bytes;
-	const long long n_cta = (rows_total + rows_own - 1) / rows_own;
-	RXB_CUDA(cudaFuncSetAttribute(h->kern_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-	int per_sm = 1;
-	RXB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, h->kern_rows, threads, smem));
-	if (per_sm < 1) { set_error("split kernel does not fit an SM (%zu bytes of shared memory, %d threads)", smem, threads); return RXB200_EUNSUPPORTED; }
-	const size_t total_work = (size_t)n_cta * h->n_channels;
-	const size_t need_sync = 4 + 4 * total_work;
-	RXB_CUDA(fm_reserve(h->d_sync, h->sync_cap, need_sync));
-	RXB_CUDA(fm_reserve(h->d_margin, h->margin_cap, total_work * (size_t)rows_margin * (size_t)row_pcm));
-	FmCall k;
-	memset(&k, 0, sizeof k);
-	k.in = d_in; k.out = d_out; k.n = n; k.out_stride = (long long)out_stride; k.chunk = (int)(chunk_int16 / 2);
-	k.margin = h->d_margin;
-	k.n_ch = h->n_channels; k.Sf = ROW_LEN; k.halo = 0; k.n_extra = (int)rows_margin; k.n_own = (int)rows_own;
-	k.n_cta = (int)n_cta; k.W_dec = (int)W_dec; k.pcm_cap = (int)pcm_cap; k.direct_out = 0;
-	k.be_lanes = be_lanes; k.fe_warps = fe_warps; k.fe_threads = fe_warps * 32; k.xs_words = xs_words;
-	k.state_words = h->state_words; k.carry_in = h->d_carry[h->cur]; k.carry_out = h->d_carry[h->cur ^ 1];
-	k.ticket = h->d_sync; k.fix_count = h->d_sync + 1; k.pub = h->d_sync + 4;
-	k.n_chunks = (int)((n + k.chunk - 1) / k.chunk);
-	k.reduce_mode = 0; k.one = 1;
-	size_t blocks = (size_t)h->n_sm * per_sm;
-	if (blocks > total_work) { blocks = total_work; }
-	RXB_CUDA(cudaMemsetAsync(h->d_sync, 0, need_sync * sizeof(int), h->stream));
-	RXB_CUDA(cudaEventRecord(h->ev0, h->stream));
-	h->kern_rows<<<(unsigned)blocks, threads, smem, h->stream>>>(dv, k, in_map);
-	RXB_CUDA(cudaGetLastError());
-	RXB_CUDA(cudaEventRecord(h->ev1, h->stream));
-	h->cur ^= 1;
-	h->stats.launches = 1; h->stats.segments = (int)(total_work * fe_warps); h->stats.segment_len = (int)(rows_own * ROW_LEN);
-	h->stats.warmup_len = (int)(W_dec << P); h->stats.fixup_segments = -1; h->stats.kernel_kind = 1;
+	const long long pcm_cap = cap_for(rows_own + rows_margin);
+	*g = {threads, 1, 2 * (size_t)pcm_cap * sizeof(int16_t) + xs_bytes};
+	RXB_CUDA(fm_occupancy(h->kern_rows, threads, g->smem, &g->per_sm));
+	if (g->per_sm < 1) { set_error("split kernel does not fit an SM (%zu bytes of shared memory, %d threads)", g->smem, threads); return RXB200_EUNSUPPORTED; }
+	k->Sf = ROW_LEN; k->n_extra = (int)rows_margin; k->n_own = (int)rows_own; k->n_cta = (int)((rows_total + rows_own - 1) / rows_own);
+	k->W_dec = (int)W_dec; k->pcm_cap = (int)pcm_cap; k->be_lanes = be_lanes; k->fe_warps = fe_warps; k->fe_threads = fe_warps * 32;
+	k->xs_words = xs_words;
 	return RXB200_OK;
 }
 
-static int fm_launch(rxb200_fm *h, const int16_t *d_in, size_t n_int16, size_t chunk_int16, int16_t *d_out,
-                     size_t out_stride)
+static int fm_plan_segments(const rxb200_fm *h, fm_kernel_fn kern, long long n, bool stream, FmCall *k, FmGrid *g)
 {
-	if (fm_rows_shape_ok(h, n_int16, chunk_int16)) { return fm_launch_rows(h, d_in, n_int16, chunk_int16, d_out, out_stride); }
-	const rxb200_fm_params &p = h->p;
 	const FmDev &dv = h->dev;
-	const long long n = (long long)(n_int16 / 2);
 	const int T = h->threads;
-	const int P = p.downsample_passes;
+	const int P = h->p.downsample_passes;
 	const long long Dtot = dv.D;
 	const long long G = (1LL << P) > 8 ? (1LL << P) : 8;
 	// front-end replay: decimated samples until cascade (6) + droop FIR (9) + discriminator (1) are exact
 	const long long dec_exact = (P ? (dv.fir_on ? 16 : 8) : 3) + (dv.post_ds > 1 ? dv.post_ds : 0);
 	const long long halo = round_up_ll(dec_exact * Dtot, G);
 	const long long Dpcm = Dtot * dv.post_ds;   // input samples per PCM sample
-	// back-end replay (decimated samples): de-emphasis bracket + one resampler group
-	long long wd = 0;
-	if (dv.deemph) { wd = h->tune_warm > 0 ? h->tune_warm : 16LL * p.deemph_a + 64; }
-	// Stream path: the front end of the whole call stores its PCM to global memory (SPEC 4 through the direct-output
-	// path), fm_back_kernel then runs the serial stages with pieces as long as the call allows.  In the fused kernel a
-	// piece is a lane's share of one shared-memory buffer -- at the capture rate (fm2a) 870 samples behind a 2960-step
-	// replay, and the item's front end recomputes the replay region too; here the replay is paid once per piece of
-	// a few thousand samples and the front end computes nothing twice.  Worth it from a few dozen replays of PCM per call.
-	const long long m_total = (n + Dtot - 1) / Dtot + 1;
-	const size_t stream_min = h->stream_min != (size_t)-1 ? h->stream_min : (size_t)(32 * wd * Dpcm / h->n_channels);
-	const bool stream = h->kern_front != nullptr && dv.deemph && (size_t)n >= stream_min;
-	// The bracket in front of a piece closes in two phases: the gap contracts by (1 - 1/a) per step (to 1 within ~11 a
-	// steps from the full int16 range), then the two trajectories sit one apart until a sample lands on the one residue
-	// mod a that merges them -- a geometric wait with mean a.  16 a + 64 steps leave a fraction of a percent of the pieces
-	// open, each of which costs its item a probe and a second pass; with the stream path's long pieces
-	// four more a's of replay (e^-4: ~0.01 %) are cheaper than those stragglers.
-	if (stream && dv.deemph && h->tune_warm <= 0) { wd = 20LL * p.deemph_a + 64; }
-	const fm_kernel_fn kern = stream ? h->kern_front : h->kern;
-	const int direct_out = stream ? 1 : ((dv.mode == RXB200_MODE_RAW || (!dv.deemph && !dv.resample && !dv.adc_on)) ? 1 : 0);
-	const long long W_dec = direct_out ? 0 : wd;
-	// PCM the CTA needs from before its stretch: the replay plus the resampler group in progress
-	const long long margin_dec = direct_out ? 0 : W_dec + (dv.resample ? (p.rate_out / p.rate_out2 + 2) : 0) + 2;
+	// the stream path's front kernel and the shapes without a serial stage store the output from the front end
+	const int direct_out = (stream || dv.mode == RXB200_MODE_RAW || (!dv.deemph && !dv.resample && !dv.adc_on)) ? 1 : 0;
+	const long long W_dec = direct_out ? 0 : fm_replay(h, false);
+	const long long margin_dec = direct_out ? 0 : fm_margin(h, W_dec);
 	// segment per thread: ~128 decimated samples, at least 4 halos, capped so the PCM buffer stays small
 	long long Sf = h->tune_seg;
 	if (Sf <= 0) {
@@ -2425,7 +2386,6 @@ static int fm_launch(rxb200_fm *h, const int16_t *d_in, size_t n_int16, size_t c
 	}
 	if (h->tune_seg <= 0 && Sf >= 2 * Gs) { Sf = (Sf / Gs) * Gs; }
 	Sf = round_up_ll(Sf, G);
-	const bool sf_forced = h->tune_seg > 0;
 	long long n_extra = 0, n_own = 0, stretch = 0, n_cta = 0, ppt = 0, pcm_cap = 0;
 	size_t smem = 0;
 	auto geometry = [&](long long sf) -> bool {
@@ -2452,11 +2412,10 @@ static int fm_launch(rxb200_fm *h, const int16_t *d_in, size_t n_int16, size_t c
 			return RXB200_EUNSUPPORTED;
 		}
 	}
-	RXB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
 	int per_sm = 1;
-	RXB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, T, smem));
+	RXB_CUDA(fm_occupancy(kern, T, smem, &per_sm));
 	if (per_sm < 1) { per_sm = 1; }
-	if (!sf_forced) {
+	if (h->tune_seg <= 0) {
 		// tail balancing: work items are handed out to n_sm*per_sm resident CTAs; prefer a slightly shorter
 		// segment when it turns a ragged last wave into full waves (cost = replay overhead x wave round-up)
 		const double slots = (double)h->n_sm * per_sm;
@@ -2486,170 +2445,215 @@ static int fm_launch(rxb200_fm *h, const int16_t *d_in, size_t n_int16, size_t c
 			Sf = pick;
 			geometry(Sf);
 		}
-		RXB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
 	}
-	const size_t total_work = (size_t)n_cta * h->n_channels;
-	// stream path: geometry of the back kernel -- BACK_T pieces per item, `piece` PCM samples each
-	long long piece = 0, span = 0, n_cta_b = 0, pstride = 0;
+	// the grid is sized by the occupancy at the final segment length
+	*g = {T, 1, smem};
+	RXB_CUDA(fm_occupancy(kern, T, smem, &g->per_sm));
+	if (g->per_sm < 1) { g->per_sm = 1; }
+	// back-end width: enough lanes that a piece is about half a replay long (more lanes shorten the
+	// phase in which the other warps idle, but every lane pays the full replay)
+	const long long item_pcm = n_own * Sf / Dpcm;
+	const long long want = W_dec > 0 ? (2 * item_pcm / W_dec + 31) / 32 * 32 : 128;
+	int bl = (int)want;
+	if (bl < 32) { bl = 32; }
+	if (bl > T) { bl = T; }
+	k->Sf = (int)Sf; k->halo = (int)halo; k->n_extra = (int)n_extra; k->n_own = (int)n_own; k->n_cta = (int)n_cta;
+	k->W_dec = (int)W_dec; k->pcm_cap = (int)pcm_cap; k->direct_out = direct_out; k->be_lanes = bl;
+	return RXB200_OK;
+}
+
+// stream path, back kernel: a CTA covers `span` input samples of a channel, a lane one piece of the PCM scratch
+struct FmBackPlan { fm_kernel_fn kern; long long W_dec, span, n_cta, pstride; FmGrid g; };
+
+static int fm_plan_back(const rxb200_fm *h, long long n, FmBackPlan *b)
+{
+	const long long Dtot = h->dev.D, Dpcm = Dtot * h->dev.post_ds;
+	const long long m_total = (n + Dtot - 1) / Dtot + 1;
 	const int back_t = h->stream_t, back_ws = h->stream_win;
-	const fm_kernel_fn kern_back = pick_back_kernel(back_ws, back_t);
-	const size_t smem_b = (size_t)(back_t / 32) * 2 * 32 * (back_ws / 2 + 2) * sizeof(uint32_t) + 64;      // + slack for win_outputs' read-ahead
-	int per_b = 1;
-	if (stream) {
-		RXB_CUDA(cudaFuncSetAttribute(kern_back, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_b));
-		RXB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_b, kern_back, back_t, smem_b));
-		if (per_b < 1) { per_b = 1; }
-		const long long lanes_target = (long long)h->n_sm * per_b * back_t;      // one piece per resident lane
-		piece = h->stream_piece > 0 ? h->stream_piece : (m_total * h->n_channels + lanes_target - 1) / lanes_target;
-		if (h->stream_piece <= 0 && piece < wd / 2) { piece = wd / 2; }
-		if (piece < 64) { piece = 64; }
-		if (piece * back_t * Dpcm > 0x40000000LL) { piece = 0x40000000LL / (back_t * Dpcm); }
-		span = piece * back_t * Dpcm;
-		n_cta_b = (n + span - 1) / span;
-		pstride = (m_total + back_ws + 64 + 7) & ~7LL;      // a window may reach past the last sample
-		RXB_CUDA(fm_reserve(h->d_pcm, h->d_pcm_cap, (size_t)pstride * h->n_channels));
+	b->kern = pick_back_kernel(back_ws, back_t);
+	b->W_dec = fm_replay(h, true);
+	b->g = {back_t, 1, (size_t)(back_t / 32) * 2 * 32 * (back_ws / 2 + 2) * sizeof(uint32_t) + 64};   // + slack for win_outputs' read-ahead
+	RXB_CUDA(fm_occupancy(b->kern, back_t, b->g.smem, &b->g.per_sm));
+	if (b->g.per_sm < 1) { b->g.per_sm = 1; }
+	const long long lanes_target = (long long)h->n_sm * b->g.per_sm * back_t;      // one piece per resident lane
+	long long piece = h->stream_piece > 0 ? h->stream_piece : (m_total * h->n_channels + lanes_target - 1) / lanes_target;
+	if (h->stream_piece <= 0 && piece < b->W_dec / 2) { piece = b->W_dec / 2; }
+	if (piece < 64) { piece = 64; }
+	if (piece * back_t * Dpcm > 0x40000000LL) { piece = 0x40000000LL / (back_t * Dpcm); }
+	b->span = piece * back_t * Dpcm;
+	b->n_cta = (n + b->span - 1) / b->span;
+	b->pstride = (m_total + back_ws + 64 + 7) & ~7LL;      // a window may reach past the last sample
+	return RXB200_OK;
+}
+
+// per-chunk scalars: sizes (closed form), accumulators, then one recurrence per stage in the reference's order: raw DC
+// block -> squelch (sees the DC-blocked data, its sums from pass(1)) -> audio DC block (sums from pass(2))
+template <typename Pass>
+static int fm_prepasses(rxb200_fm *h, FmCall &k, size_t n_int16, size_t chunk_int16, Pass pass, int *launches)
+{
+	const FmDev &dv = h->dev;
+	const int n_chunks = k.n_chunks;
+	const size_t cells = (size_t)n_chunks * h->n_channels;
+	RXB_CUDA(fm_reserve(h->d_sums, h->sums_cap, cells * 2));
+	RXB_CUDA(fm_reserve(h->d_rdc, h->rdc_cap, cells * 2));
+	RXB_CUDA(fm_reserve(h->d_sqz, h->sqz_cap, cells));
+	RXB_CUDA(fm_reserve(h->d_adc, h->adc_cap, cells));
+	RXB_CUDA(fm_reserve(h->d_levels, h->levels_cap, cells));
+	RXB_CUDA(fm_reserve(h->d_lens, h->lens_cap, (size_t)n_chunks * 3));
+	RXB_CUDA(cudaStreamSynchronize(h->stream));   // the previous call may still be reading the host vector
+	h->h_lens.assign((size_t)n_chunks * 3, 0);     // [0]: complex per chunk, [1]: decimated per chunk, [2]: PCM per chunk
+	fm_count_outputs(h, n_int16, chunk_int16, nullptr, h->h_lens.data(), false);   // -o was checked before the launch
+	for (int ci = 0; ci < n_chunks; ci++) {
+		if (h->h_lens[(size_t)n_chunks + ci] < 1) { set_error("a chunk produces no decimated sample"); return RXB200_EUNSUPPORTED; }
 	}
-	const size_t total_back = (size_t)n_cta_b * h->n_channels;
+	RXB_CUDA(cudaMemcpyAsync(h->d_lens, h->h_lens.data(), h->h_lens.size() * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+	const unsigned cb = (unsigned)((h->n_channels + 63) / 64);
+	if (dv.rdc_on) {
+		RXB_CUDA(cudaMemsetAsync(h->d_sums, 0, cells * 2 * sizeof(long long), h->stream));
+		dim3 grid(8, (unsigned)n_chunks, (unsigned)h->n_channels);
+		fm_rdc_sum_kernel<<<grid, 256, 0, h->stream>>>(k.in, k.n, k.chunk, n_chunks, h->d_sums);
+		RXB_CUDA(cudaGetLastError());
+		fm_rdc_recur_kernel<<<cb, 64, 0, h->stream>>>(h->d_sums, h->d_lens, n_chunks, h->n_channels, dv.rdc_k, k.carry_in, k.carry_out,
+		                                               h->state_words, h->d_rdc);
+		RXB_CUDA(cudaGetLastError());
+		*launches += 2;
+		k.rdc = h->d_rdc;
+	}
+	if (dv.squelch || dv.levels) {
+		RXB_CUDA(cudaMemsetAsync(h->d_sums, 0, cells * 2 * sizeof(long long), h->stream));
+		k.sums = h->d_sums;
+		const int rc = pass(1);
+		if (rc != RXB200_OK) { return rc; }
+		fm_squelch_kernel<<<cb, 64, 0, h->stream>>>(h->d_sums, h->d_lens + n_chunks, n_chunks, h->n_channels, dv.squelch, k.carry_in,
+		                                             k.carry_out, h->state_words, h->d_sqz, dv.levels ? h->d_levels : nullptr);
+		RXB_CUDA(cudaGetLastError());
+		(*launches)++;
+		k.sqz = dv.squelch ? h->d_sqz : nullptr;
+		h->level_chunks = n_chunks;
+	}
+	if (dv.adc_on) {
+		RXB_CUDA(cudaMemsetAsync(h->d_sums, 0, cells * 2 * sizeof(long long), h->stream));
+		k.sums = h->d_sums;
+		const int rc = pass(2);
+		if (rc != RXB200_OK) { return rc; }
+		fm_adc_recur_kernel<<<cb, 64, 0, h->stream>>>(h->d_sums, h->d_lens + 2 * (size_t)n_chunks, n_chunks, h->n_channels, dv.adc_k,
+		                                               k.carry_in, k.carry_out, h->state_words, h->d_adc);
+		RXB_CUDA(cudaGetLastError());
+		(*launches)++;
+		k.adc = h->d_adc;
+	}
+	k.sums = nullptr;
+	return RXB200_OK;
+}
+
+// Plans and launches one call -- the split kernel where the shape allows it, else the fused kernel, or on the stream
+// path the front and back kernels -- then advances the host mirrors of the closed-form counters.
+static int fm_launch(rxb200_fm *h, const int16_t *d_in, size_t n_int16, size_t chunk_int16, int16_t *d_out, size_t out_stride)
+{
+	const FmDev &dv = h->dev;
+	const long long n = (long long)(n_int16 / 2);
+	const bool rows = h->kern_rows && (chunk_int16 / 2) % ROW_LEN == 0 && n % ROW_LEN == 0 && n >= 16LL * ROW_LEN;
+	// Stream path: the front end of the whole call stores its PCM to global memory (SPEC 4 through the direct-output
+	// path), fm_back_kernel then runs the serial stages with pieces as long as the call allows.  In the fused kernel a
+	// piece is a lane's share of one shared-memory buffer -- at the capture rate (fm2a) 870 samples behind a 2960-step
+	// replay, and the item's front end recomputes the replay region too; here the replay is paid once per piece of
+	// a few thousand samples and the front end computes nothing twice.  Worth it from a few dozen replays of PCM per call.
+	const long long Dpcm = (long long)dv.D * dv.post_ds;
+	const size_t stream_min = h->stream_min != (size_t)-1 ? h->stream_min : (size_t)(32 * fm_replay(h, false) * Dpcm / h->n_channels);
+	const bool stream = h->kern_front != nullptr && dv.deemph && (size_t)n >= stream_min;
+	const fm_kernel_fn kern = stream ? h->kern_front : h->kern;
+	FmCall k = {};
+	FmGrid g;
+	CUtensorMap in_map;
+	int rc = rows ? fm_rows_map(d_in, (long long)h->n_channels * (n / 32), &in_map) : RXB200_OK;
+	if (rc == RXB200_OK) { rc = rows ? fm_plan_rows(h, n, &k, &g) : fm_plan_segments(h, kern, n, stream, &k, &g); }
+	if (rc != RXB200_OK) { return rc; }
+	const size_t total_work = (size_t)k.n_cta * h->n_channels;
+	FmBackPlan b = {};
+	if (stream) {
+		rc = fm_plan_back(h, n, &b);
+		if (rc != RXB200_OK) { return rc; }
+		RXB_CUDA(fm_reserve(h->d_pcm, h->d_pcm_cap, (size_t)b.pstride * h->n_channels));
+	}
+	const size_t total_back = (size_t)b.n_cta * h->n_channels;
 	const size_t need_sync = 4 + 4 * (total_work > total_back ? total_work : total_back);
 	RXB_CUDA(fm_reserve(h->d_sync, h->sync_cap, need_sync));
-	FmCall k;
-	memset(&k, 0, sizeof k);
-	k.in = d_in; k.out = d_out; k.n = n; k.out_stride = (long long)out_stride; k.chunk = (int)(chunk_int16 / 2);
-	if (stream) { k.out = h->d_pcm; k.out_stride = pstride; }
-	k.n_ch = h->n_channels; k.Sf = (int)Sf; k.halo = (int)halo; k.n_extra = (int)n_extra; k.n_own = (int)n_own;
-	k.n_cta = (int)n_cta; k.W_dec = (int)W_dec; k.pcm_cap = (int)pcm_cap; k.direct_out = direct_out;
-	{
-		// back-end width: enough lanes that a piece is about half a replay long (more lanes shorten the
-		// phase in which the other warps idle, but every lane pays the full replay)
-		const long long item_pcm = n_own * Sf / Dpcm;
-		const long long want = W_dec > 0 ? (2 * item_pcm / W_dec + 31) / 32 * 32 : 128;
-		int bl = (int)want;
-		if (bl < 32) { bl = 32; }
-		if (bl > T) { bl = T; }
-		k.be_lanes = bl;
+	if (rows) {
+		RXB_CUDA(fm_reserve(h->d_margin, h->margin_cap, total_work * (size_t)k.n_extra * (size_t)(ROW_LEN >> dv.P)));
+		k.margin = h->d_margin;
 	}
+	// the fields every kernel of the call shares; the stream path's front kernel writes the PCM scratch
+	k.in = d_in; k.out = stream ? h->d_pcm : d_out; k.out_stride = stream ? b.pstride : (long long)out_stride;
+	k.n = n; k.chunk = (int)(chunk_int16 / 2); k.n_chunks = (int)((n + k.chunk - 1) / k.chunk); k.n_ch = h->n_channels;
 	k.state_words = h->state_words; k.carry_in = h->d_carry[h->cur]; k.carry_out = h->d_carry[h->cur ^ 1];
-	k.ticket = h->d_sync; k.fix_count = h->d_sync + 1; k.pub = h->d_sync + 4;
-	const int n_chunks = (int)((n + k.chunk - 1) / k.chunk);
-	k.n_chunks = n_chunks;
-	RXB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, T, smem));
-	if (per_sm < 1) { per_sm = 1; }
-	size_t blocks = (size_t)h->n_sm * per_sm;
+	k.ticket = h->d_sync; k.fix_count = h->d_sync + 1; k.pub = h->d_sync + 4; k.one = 1;
+	size_t blocks = (size_t)h->n_sm * g.per_sm;
 	if (blocks > total_work) { blocks = total_work; }
 	int launches = 0;
-	auto run_fused = [&](int reduce_mode) -> int {
-		k.reduce_mode = reduce_mode; k.one = 1;
+	// one pass over the call; ev0/ev1 bracket the main pass (reduce_mode 0, the time rxb200_fm_kernel_ms reports)
+	auto pass = [&](int reduce_mode) -> int {
+		k.reduce_mode = reduce_mode;
 		RXB_CUDA(cudaMemsetAsync(h->d_sync, 0, need_sync * sizeof(int), h->stream));
 		if (reduce_mode == 0) { RXB_CUDA(cudaEventRecord(h->ev0, h->stream)); }
-		kern<<<(unsigned)blocks, T, smem, h->stream>>>(dv, k);
+		if (rows) { h->kern_rows<<<(unsigned)blocks, g.threads, g.smem, h->stream>>>(dv, k, in_map); }
+		else { kern<<<(unsigned)blocks, g.threads, g.smem, h->stream>>>(dv, k); }
 		RXB_CUDA(cudaGetLastError());
 		if (reduce_mode == 0) { RXB_CUDA(cudaEventRecord(h->ev1, h->stream)); }
 		launches++;
 		return RXB200_OK;
 	};
 	if (dv.rdc_on || dv.squelch || dv.adc_on || dv.levels) {
-		// per-chunk scalars: sizes (closed form), accumulators, then one recurrence per stage in the
-		// reference's order: raw DC block -> squelch (sees the DC-blocked data) -> audio DC block
-		const size_t cells = (size_t)n_chunks * h->n_channels;
-		if (cells > h->chunk_cap) {
-			cudaFree(h->d_sums); cudaFree(h->d_rdc); cudaFree(h->d_sqz); cudaFree(h->d_adc); cudaFree(h->d_lens); cudaFree(h->d_levels);
-			h->d_sums = nullptr; h->d_rdc = h->d_sqz = h->d_adc = h->d_lens = h->d_levels = nullptr; h->chunk_cap = 0;
-			RXB_CUDA(cudaMalloc(&h->d_sums, cells * 2 * sizeof(long long)));
-			RXB_CUDA(cudaMalloc(&h->d_rdc, cells * 2 * sizeof(int)));
-			RXB_CUDA(cudaMalloc(&h->d_sqz, cells * sizeof(int)));
-			RXB_CUDA(cudaMalloc(&h->d_adc, cells * sizeof(int)));
-			RXB_CUDA(cudaMalloc(&h->d_levels, cells * sizeof(int)));
-			RXB_CUDA(cudaMalloc(&h->d_lens, (size_t)n_chunks * 3 * sizeof(int)));
-			h->chunk_cap = cells;
-		}
-		std::vector<int> &lens = *h->h_lens;       // [0]: complex per chunk, [1]: decimated per chunk, [2]: PCM per chunk
-		RXB_CUDA(cudaStreamSynchronize(h->stream));   // the previous call may still be reading the host vector
-		lens.assign((size_t)n_chunks * 3, 0);
-		long long box_n = h->h_box_n;
-		for (int ci = 0; ci < n_chunks; ci++) {
-			long long L = (long long)k.chunk < n - (long long)ci * k.chunk ? k.chunk : n - (long long)ci * k.chunk;
-			long long dec = P ? (L >> P) : (box_n + L) / p.downsample;
-			if (!P) { box_n = (box_n + L) % p.downsample; }
-			lens[ci] = (int)L; lens[(size_t)n_chunks + ci] = (int)dec;
-			lens[(size_t)2 * n_chunks + ci] = (int)(dec / dv.post_ds);
-			if (dec < 1) { set_error("a chunk produces no decimated sample"); return RXB200_EUNSUPPORTED; }
-		}
-		RXB_CUDA(cudaMemcpyAsync(h->d_lens, lens.data(), lens.size() * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-		const unsigned cb = (unsigned)((h->n_channels + 63) / 64);
-		if (dv.rdc_on) {
-			RXB_CUDA(cudaMemsetAsync(h->d_sums, 0, cells * 2 * sizeof(long long), h->stream));
-			dim3 grid(8, (unsigned)n_chunks, (unsigned)h->n_channels);
-			fm_rdc_sum_kernel<<<grid, 256, 0, h->stream>>>(d_in, n, k.chunk, n_chunks, h->d_sums);
-			RXB_CUDA(cudaGetLastError());
-			fm_rdc_recur_kernel<<<cb, 64, 0, h->stream>>>(h->d_sums, h->d_lens, n_chunks, h->n_channels, dv.rdc_k, k.carry_in, k.carry_out,
-			                                               h->state_words, h->d_rdc);
-			RXB_CUDA(cudaGetLastError());
-			launches += 2;
-			k.rdc = h->d_rdc;
-		}
-		if (dv.squelch || dv.levels) {
-			RXB_CUDA(cudaMemsetAsync(h->d_sums, 0, cells * 2 * sizeof(long long), h->stream));
-			k.sums = h->d_sums;
-			int rc2 = run_fused(1);
-			if (rc2 != RXB200_OK) { return rc2; }
-			fm_squelch_kernel<<<cb, 64, 0, h->stream>>>(h->d_sums, h->d_lens + n_chunks, n_chunks, h->n_channels, dv.squelch, k.carry_in,
-			                                             k.carry_out, h->state_words, h->d_sqz, dv.levels ? h->d_levels : nullptr);
-			RXB_CUDA(cudaGetLastError());
-			launches++;
-			k.sqz = dv.squelch ? h->d_sqz : nullptr;
-			h->level_chunks = n_chunks;
-		}
-		if (dv.adc_on) {
-			RXB_CUDA(cudaMemsetAsync(h->d_sums, 0, cells * 2 * sizeof(long long), h->stream));
-			k.sums = h->d_sums;
-			int rc2 = run_fused(2);
-			if (rc2 != RXB200_OK) { return rc2; }
-			fm_adc_recur_kernel<<<cb, 64, 0, h->stream>>>(h->d_sums, h->d_lens + 2 * (size_t)n_chunks, n_chunks, h->n_channels, dv.adc_k,
-			                                               k.carry_in, k.carry_out, h->state_words, h->d_adc);
-			RXB_CUDA(cudaGetLastError());
-			launches++;
-			k.adc = h->d_adc;
-		}
-		k.sums = nullptr;
+		rc = fm_prepasses(h, k, n_int16, chunk_int16, pass, &launches);
+		if (rc != RXB200_OK) { return rc; }
 	}
-	{
-		int rc2 = run_fused(0);
-		if (rc2 != RXB200_OK) { return rc2; }
-	}
+	rc = pass(0);
+	if (rc != RXB200_OK) { return rc; }
 	if (stream) {
 		FmCall kb = k;
 		kb.out = d_out; kb.out_stride = (long long)out_stride; kb.direct_out = 0;
-		kb.pcm_g = h->d_pcm; kb.pcm_g_stride = pstride;
-		kb.n_extra = 0; kb.n_own = 1; kb.Sf = (int)span; kb.n_cta = (int)n_cta_b; kb.W_dec = (int)wd; kb.be_lanes = back_t;
+		kb.pcm_g = h->d_pcm; kb.pcm_g_stride = b.pstride;
+		kb.n_extra = 0; kb.n_own = 1; kb.Sf = (int)b.span; kb.n_cta = (int)b.n_cta; kb.W_dec = (int)b.W_dec; kb.be_lanes = b.g.threads;
 		kb.ticket = h->d_sync + 2;
-		size_t blocks_b = (size_t)h->n_sm * per_b;
+		size_t blocks_b = (size_t)h->n_sm * b.g.per_sm;
 		if (blocks_b > total_back) { blocks_b = total_back; }
-		kern_back<<<(unsigned)blocks_b, back_t, smem_b, h->stream>>>(dv, kb);
+		b.kern<<<(unsigned)blocks_b, b.g.threads, b.g.smem, h->stream>>>(dv, kb);
 		RXB_CUDA(cudaGetLastError());
 		RXB_CUDA(cudaEventRecord(h->ev1, h->stream));
 		launches++;
 	}
 	h->cur ^= 1;
-	h->stats.launches = launches; h->stats.segments = (int)(total_work * T); h->stats.segment_len = (int)Sf;
-	h->stats.warmup_len = (int)((stream ? wd : W_dec) * Dtot); h->stats.fixup_segments = -1; h->stats.kernel_kind = stream ? 3 : 0;
+	h->stats.launches = launches; h->stats.segments = (int)(total_work * (rows ? k.fe_warps : g.threads));
+	h->stats.segment_len = rows ? k.n_own * ROW_LEN : k.Sf; h->stats.warmup_len = (int)((stream ? b.W_dec : k.W_dec) * (long long)dv.D);
+	h->stats.fixup_segments = -1; h->stats.kernel_kind = rows ? 1 : (stream ? 3 : 0);
+	fm_count_outputs(h, n_int16, chunk_int16, nullptr, nullptr, true);
+	return RXB200_OK;
+}
+
+// what both process calls check before they launch, and the call's output count (*total PCM samples per channel)
+static int fm_prologue(rxb200_fm *h, const void *in, const void *out, size_t n_int16, size_t chunk_int16, size_t pcm_stride,
+                       int *chunk_result_len, size_t *total, size_t *n_pcm)
+{
+	if (!h || !in || !out) { set_error("null argument"); return RXB200_EINVAL; }
+	const int rc = fm_check_shape(h, n_int16, chunk_int16);
+	if (rc != RXB200_OK) { return rc; }
+	RXB_CUDA(cudaSetDevice(h->device));
+	if (n_int16 == 0) { h->level_chunks = 0; if (n_pcm) { *n_pcm = 0; } }
+	*total = fm_count_outputs(h, n_int16, chunk_int16, chunk_result_len, nullptr, false);
+	if (*total == (size_t)-1) { set_error("-o %d needs every chunk to decimate to a multiple of it", h->dev.post_ds); return RXB200_EUNSUPPORTED; }
+	if (*total > pcm_stride) { set_error("pcm_stride %zu < %zu outputs", pcm_stride, *total); return RXB200_ECAPACITY; }
 	return RXB200_OK;
 }
 
 extern "C" int rxb200_fm_process_device(rxb200_fm *h, const int16_t *d_cs16, size_t n_int16, size_t chunk_int16,
                                         int16_t *d_pcm, size_t pcm_stride, size_t *n_pcm, int sync)
 {
-	if (!h || !d_cs16 || !d_pcm) { set_error("null argument"); return RXB200_EINVAL; }
-	if (((uintptr_t)d_cs16 & 31u) != 0) { set_error("d_cs16 must be 32-byte aligned"); return RXB200_EINVAL; }
-	int rc = fm_check_shape(h, n_int16, chunk_int16);
-	if (rc != RXB200_OK) { return rc; }
-	RXB_CUDA(cudaSetDevice(h->device));
-	if (n_int16 == 0) { h->level_chunks = 0; if (n_pcm) { *n_pcm = 0; } return RXB200_OK; }
-	size_t total = fm_count_outputs(h, n_int16, chunk_int16, nullptr, false);
-	if (total == (size_t)-1) { set_error("-o %d needs every chunk to decimate to a multiple of it", h->dev.post_ds); return RXB200_EUNSUPPORTED; }
-	if (total > pcm_stride) { set_error("pcm_stride %zu < %zu outputs", pcm_stride, total); return RXB200_ECAPACITY; }
+	// null arguments are reported first, by fm_prologue
+	if (h && d_cs16 && d_pcm && ((uintptr_t)d_cs16 & 31u) != 0) { set_error("d_cs16 must be 32-byte aligned"); return RXB200_EINVAL; }
+	size_t total = 0;
+	int rc = fm_prologue(h, d_cs16, d_pcm, n_int16, chunk_int16, pcm_stride, nullptr, &total, n_pcm);
+	if (rc != RXB200_OK || n_int16 == 0) { return rc; }
 	rc = fm_launch(h, d_cs16, n_int16, chunk_int16, d_pcm, pcm_stride);
 	if (rc != RXB200_OK) { return rc; }
-	fm_count_outputs(h, n_int16, chunk_int16, nullptr, true);
 	if (n_pcm) { *n_pcm = total; }
 	if (sync) {
 		RXB_CUDA(cudaStreamSynchronize(h->stream));
@@ -2661,22 +2665,16 @@ extern "C" int rxb200_fm_process_device(rxb200_fm *h, const int16_t *d_cs16, siz
 extern "C" int rxb200_fm_process(rxb200_fm *h, const int16_t *cs16, size_t n_int16, size_t chunk_int16,
                                  int16_t *pcm, size_t pcm_stride, size_t *n_pcm, int *chunk_result_len)
 {
-	if (!h || !cs16 || !pcm) { set_error("null argument"); return RXB200_EINVAL; }
-	int rc = fm_check_shape(h, n_int16, chunk_int16);
-	if (rc != RXB200_OK) { return rc; }
-	RXB_CUDA(cudaSetDevice(h->device));
-	if (n_int16 == 0) { h->level_chunks = 0; if (n_pcm) { *n_pcm = 0; } return RXB200_OK; }
-	size_t total = fm_count_outputs(h, n_int16, chunk_int16, chunk_result_len, false);
-	if (total == (size_t)-1) { set_error("-o %d needs every chunk to decimate to a multiple of it", h->dev.post_ds); return RXB200_EUNSUPPORTED; }
-	if (total > pcm_stride) { set_error("pcm_stride %zu < %zu outputs", pcm_stride, total); return RXB200_ECAPACITY; }
-	size_t in_elems = n_int16 * (size_t)h->n_channels;
-	size_t out_elems = (total + 8) * (size_t)h->n_channels;
+	size_t total = 0;
+	int rc = fm_prologue(h, cs16, pcm, n_int16, chunk_int16, pcm_stride, chunk_result_len, &total, n_pcm);
+	if (rc != RXB200_OK || n_int16 == 0) { return rc; }
+	const size_t in_elems = n_int16 * (size_t)h->n_channels;
+	const size_t out_elems = (total + 8) * (size_t)h->n_channels;
 	RXB_CUDA(fm_reserve(h->d_in, h->d_in_cap, in_elems));
 	RXB_CUDA(fm_reserve(h->d_out, h->d_out_cap, out_elems));
 	RXB_CUDA(cudaMemcpyAsync(h->d_in, cs16, in_elems * sizeof(int16_t), cudaMemcpyHostToDevice, h->stream));
 	rc = fm_launch(h, h->d_in, n_int16, chunk_int16, h->d_out, total + 8);
 	if (rc != RXB200_OK) { return rc; }
-	fm_count_outputs(h, n_int16, chunk_int16, nullptr, true);
 	if (pcm_stride == total + 8 || h->n_channels == 1) {
 		RXB_CUDA(cudaMemcpyAsync(pcm, h->d_out, (h->n_channels == 1 ? total : out_elems) * sizeof(int16_t),
 		                         cudaMemcpyDeviceToHost, h->stream));
