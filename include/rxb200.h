@@ -168,7 +168,10 @@ typedef struct rxb200_fm_stats {
 } rxb200_fm_stats;
 int rxb200_fm_last_stats(rxb200_fm *h, rxb200_fm_stats *out);
 /* Tuning knobs (0 keeps the automatic choice): segment length in complex samples, de-emphasis
- * warm-up in decimated samples. */
+ * warm-up in decimated samples.  The warm-up (default 16*deemph_a + 64) plus the resampler group
+ * must fit one CTA's PCM buffer: a call whose warm-up the split kernel cannot hold runs on the fused
+ * kernel (kernel_kind 0); beyond 32750 decimated samples with fifth_order passes (fewer for long
+ * boxcars, DESIGN.md section 6) the call returns RXB200_EUNSUPPORTED. */
 int rxb200_fm_tune(rxb200_fm *h, int segment_len, int deemph_warmup);
 /* Device time (CUDA events on the handle's stream) of the last process call's main kernels, in
  * milliseconds: the split kernel on the row path, the fused kernel's main pass (not its per-chunk

@@ -2293,7 +2293,9 @@ static int fm_rows_map(const int16_t *d_in, long long lines, CUtensorMap *map)
 // ---- the split kernel with the row front end (fm_rows.cuh).  Geometry in ROWS of ROW_LEN input samples:
 // an item owns `rows_own` rows; its PCM buffer also holds the `rows_margin` rows before them (the back end's replay
 // window), which the previous items of the channel hand over through global memory; the two PCM buffers and the
-// warps' exchange areas share the CTA's dynamic shared memory.
+// warps' exchange areas share the CTA's dynamic shared memory.  Returns FM_ROWS_NO_ROOM when the margin leaves no room
+// for an item's own rows (a de-emphasis replay longer than the PCM buffers hold): fm_launch takes the fused kernel then.
+#define FM_ROWS_NO_ROOM 1
 static int fm_plan_rows(const rxb200_fm *h, long long n, FmCall *k, FmGrid *g)
 {
 	const int P = h->p.downsample_passes;
@@ -2320,7 +2322,7 @@ static int fm_plan_rows(const rxb200_fm *h, long long n, FmCall *k, FmGrid *g)
 	long long rows_item = ((dyn_max - (long long)xs_bytes) / 2 / (long long)sizeof(int16_t)) / (row_pcm + (row_pcm * PCM_PAD_ROWS) / 128 + 1);
 	while (rows_item > rows_margin + 1 && 2 * cap_for(rows_item) * (long long)sizeof(int16_t) + (long long)xs_bytes > dyn_max) { rows_item--; }
 	long long rows_own = rows_item - rows_margin;
-	if (rows_own < 1) { set_error("the back-end replay (%lld PCM samples) does not fit the split kernel's PCM buffers", margin_dec); return RXB200_EUNSUPPORTED; }
+	if (rows_own < 1) { return FM_ROWS_NO_ROOM; }
 	if (h->tune_seg > 0) {
 		long long t = h->tune_seg / ROW_LEN;
 		if (t < 1) { t = 1; }
@@ -2388,13 +2390,17 @@ static int fm_plan_segments(const rxb200_fm *h, fm_kernel_fn kern, long long n, 
 	Sf = round_up_ll(Sf, G);
 	long long n_extra = 0, n_own = 0, stretch = 0, n_cta = 0, ppt = 0, pcm_cap = 0;
 	size_t smem = 0;
+	// the PCM buffer shares the opt-in limit with the kernel's static shared memory
+	cudaFuncAttributes fa;
+	RXB_CUDA(cudaFuncGetAttributes(&fa, kern));
+	const long long smem_max = (long long)h->smem_optin - (long long)fa.sharedSizeBytes;
 	auto geometry = [&](long long sf) -> bool {
 		n_extra = direct_out ? 0 : (margin_dec * Dpcm + halo + sf - 1) / sf;
 		ppt = sf / Dpcm + 2;
 		pcm_cap = direct_out ? 8 : (long long)T * ppt + 64;
 		pcm_cap += PCM_PAD_SEG * (pcm_cap >> 7) + 8;
 		smem = (size_t)pcm_cap * sizeof(int16_t);
-		if ((long long)smem > h->smem_optin || n_extra > T / 2) { return false; }
+		if ((long long)smem > smem_max || n_extra > T / 2) { return false; }
 		n_own = T - n_extra;
 		stretch = n_own * sf;
 		n_cta = (n + stretch - 1) / stretch;
@@ -2552,7 +2558,7 @@ static int fm_launch(rxb200_fm *h, const int16_t *d_in, size_t n_int16, size_t c
 {
 	const FmDev &dv = h->dev;
 	const long long n = (long long)(n_int16 / 2);
-	const bool rows = h->kern_rows && (chunk_int16 / 2) % ROW_LEN == 0 && n % ROW_LEN == 0 && n >= 16LL * ROW_LEN;
+	bool rows = h->kern_rows && (chunk_int16 / 2) % ROW_LEN == 0 && n % ROW_LEN == 0 && n >= 16LL * ROW_LEN;
 	// Stream path: the front end of the whole call stores its PCM to global memory (SPEC 4 through the direct-output
 	// path), fm_back_kernel then runs the serial stages with pieces as long as the call allows.  In the fused kernel a
 	// piece is a lane's share of one shared-memory buffer -- at the capture rate (fm2a) 870 samples behind a 2960-step
@@ -2565,8 +2571,9 @@ static int fm_launch(rxb200_fm *h, const int16_t *d_in, size_t n_int16, size_t c
 	FmCall k = {};
 	FmGrid g;
 	CUtensorMap in_map;
-	int rc = rows ? fm_rows_map(d_in, (long long)h->n_channels * (n / 32), &in_map) : RXB200_OK;
-	if (rc == RXB200_OK) { rc = rows ? fm_plan_rows(h, n, &k, &g) : fm_plan_segments(h, kern, n, stream, &k, &g); }
+	int rc = rows ? fm_plan_rows(h, n, &k, &g) : RXB200_OK;
+	if (rc == FM_ROWS_NO_ROOM) { rows = false; k = {}; rc = RXB200_OK; }   // the same call on the fused kernel
+	if (rc == RXB200_OK) { rc = rows ? fm_rows_map(d_in, (long long)h->n_channels * (n / 32), &in_map) : fm_plan_segments(h, kern, n, stream, &k, &g); }
 	if (rc != RXB200_OK) { return rc; }
 	const size_t total_work = (size_t)k.n_cta * h->n_channels;
 	FmBackPlan b = {};

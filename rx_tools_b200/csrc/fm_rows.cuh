@@ -124,6 +124,27 @@ __device__ __forceinline__ void droop9_words(const int (&c)[6], int fir_bias, ui
 	dq = wrap16(aq >> 15);
 }
 
+// ||x| - |y|| of fast_atan2 for the conjugate product (cr, cj); its 4096 (|x| - |y|) leaves int32 from 2^19 on, where
+// FP32 does not wrap with it
+__device__ __forceinline__ float row_angle_n(int cr, int cj)
+{
+	return fabsf(__fsub_rn(fabsf(__int2float_rn(cr)), fabsf(__int2float_rn(cj))));
+}
+
+// A lane's NV discriminator outputs as the low 16 bits of angle + 1.5 * 2^23.  WRAPS: operands whose product leaves
+// int32 take the integer form.
+template <int NV, bool CS, bool WRAPS>
+__device__ __forceinline__ void row_angles(const int *cr, const int *cj, int lane, uint32_t *ab)
+{
+#pragma unroll
+	for (int j = 0; j < NV; j++) {
+		float ang = fast_atan2_f32(__int2float_rn(cj[j]), __int2float_rn(cr[j]));
+		if (WRAPS && row_angle_n(cr[j], cj[j]) >= 524288.0f) { ang = __int2float_rn(fast_atan2_i(cj[j], cr[j])); }
+		if (CS && j == 0 && lane == 0) { ang = __int2float_rn(disc_std(cr[0], cj[0])); }   // F8: the first sample of a chunk goes through atan2
+		ab[j] = (uint32_t)__float_as_int(__fadd_rn(ang, 12582912.0f));      // low 16 bits of angle + 1.5 * 2^23: the int16 value
+	}
+}
+
 // One row of one lane, read from stage `stage` of the ring.  Once level 0 is through (its exchange has every lane's
 // inputs consumed) lane 0 refills the stage with the row ROWS_STAGES ahead, at `next_line` (< 0: none left).
 // par = parity of the row (which carry slot lane 31 writes); CS = the row starts a chunk;
@@ -213,16 +234,18 @@ __device__ __forceinline__ void row_body(const FmDev &c, uint32_t *xs, int par, 
 	// plus less than 32 for the floors -- and |cr| + |cj| <= 4 d^2 < 1.2e7 < 2^24
 	// (tests/test_host_logic.py::test_row_discriminator_operands_fit_fp32 recomputes the bound from the table).
 	// The FP32 form issues every cycle and leaves the adder pipe, which bounds this loop, ~16 instructions per output
-	// lighter than the integer form (DESIGN.md §4.1).
+	// lighter than the integer form (DESIGN.md §4.1).  One case it does not reproduce: the reference's 4096 (|x| - |y|)
+	// wraps in int32 once ||x| - |y|| >= 2^19 (decimated samples beyond ~724, e.g. from full-scale noise).  A row in which
+	// some lane has such an operand, rare, takes row_angles<..., true>, where those operands go through the integer form,
+	// which wraps the same way; every other row keeps the straight FP32 loop.
 	uint32_t wpk[NV / 2];                  // PCM, two samples per word
 	{
 		uint32_t ab[NV];
+		bool wraps = false;
 #pragma unroll
-		for (int j = 0; j < NV; j++) {
-			float ang = fast_atan2_f32(__int2float_rn(cj[j]), __int2float_rn(cr[j]));
-			if (CS && j == 0 && lane == 0) { ang = __int2float_rn(disc_std(cr[0], cj[0])); }   // F8: the first sample of a chunk goes through atan2
-			ab[j] = (uint32_t)__float_as_int(__fadd_rn(ang, 12582912.0f));      // low 16 bits of angle + 1.5 * 2^23: the int16 value
-		}
+		for (int j = 0; j < NV; j++) { wraps |= row_angle_n(cr[j], cj[j]) >= 524288.0f; }
+		if (__any_sync(0xffffffffu, wraps)) { row_angles<NV, CS, true>(cr, cj, lane, ab); }
+		else { row_angles<NV, CS, false>(cr, cj, lane, ab); }
 #pragma unroll
 		for (int j = 0; j < NV; j += 2) { wpk[j / 2] = __byte_perm(ab[j], ab[j + 1], 0x5410); }
 	}
