@@ -80,7 +80,8 @@ static struct {
 	int direct_sampling, rtlagc;
 	int print_levels, level_no, level_max, level_max_max; double level_sum;   /* -L (src/rtl_fm.c:96-100) */
 	volatile int mute;                 /* int16 to zero at the start of the next read */
-	size_t multiple;                   /* chunk granularity librxb200 accepts */
+	size_t multiple;                   /* chunk granularity librxb200 accepts, int16 */
+	size_t min_chunk;                  /* shortest chunk handed on, int16 */
 	int failed;                        /* a library call failed: exit status 1 */
 	rxb200_fm *fm;
 	FILE *out;
@@ -140,8 +141,9 @@ static void *reader_thread(void *arg)
 {
 	(void)arg;
 	/* what a read left over past the library's chunk granularity is carried into the next slot, never dropped: the
-	 * stream stays continuous whatever lengths the device returns (the reference hands any length on, :894-899) */
-	static int16_t rem[4096];
+	 * stream stays continuous whatever lengths the device returns (the reference hands any length on, :894-899).
+	 * Where every length is accepted (see main) nothing is carried but a read too short to decimate to a sample */
+	static int16_t rem[8192];
 	size_t rem_n = 0;
 	SoapySDRDevice_activateStream(G.dev, G.stream, 0, 0, 0);
 	for (;;) {
@@ -157,7 +159,8 @@ static void *reader_thread(void *arg)
 			break;
 		}
 		size_t n16 = rem_n + (size_t)r * 2;
-		const size_t over = n16 % G.multiple;           /* librxb200 chunk granularity: the excess opens the next slot */
+		/* librxb200 chunk granularity: the excess opens the next slot; so does all of a read shorter than the minimum */
+		const size_t over = n16 < G.min_chunk ? n16 : n16 % G.multiple;
 		n16 -= over;
 		memcpy(rem, s->data + n16, over * sizeof(int16_t));
 		rem_n = over;
@@ -326,9 +329,15 @@ int main(int argc, char **argv)
 	if (G.freq_len > 1) { G.terminate_on_squelch = 0; }
 	G.filename = (argc <= optind) ? "-" : argv[optind];
 	if (rxb200_fm_derive(&G.cli, &G.der) != RXB200_OK) { fprintf(stderr, "rxb200: %s\n", rxb200_last_error()); return 1; }
-	{   /* chunk granularity accepted by the library: 16 int16 and 2*2^P int16 */
+	if (G.der.params.downsample_passes == 0 && G.der.params.post_downsample <= 1) {
+		/* no fifth_order passes and no -o: the library takes any whole number of complex samples, so every read is one
+		 * chunk as it was read, like the reference's; only a read too short to complete a boxcar waits for the next */
+		G.multiple = 2;
+		G.min_chunk = 2 * (size_t)G.der.params.downsample;
+	} else {   /* chunk granularity accepted by the library: 16 int16 and 2*2^P int16 */
 		size_t m = (size_t)2 << G.der.params.downsample_passes;
 		G.multiple = m > 16 ? m : 16;
+		G.min_chunk = 0;
 	}
 	G.der.params.report_levels = G.print_levels ? 1 : 0;
 	G.level_no = 1;

@@ -7,7 +7,8 @@
  *      compiled against host/soapy_replay and linked with this file so every symbol
  *      resolves; the harness feeds samples from memory (soapy_fake_set_memory).
  *   2. the drop-in host shells (host/rx_fm_b200, host/rx_power_b200) run hardware-free
- *      with `-d driver=file,path=capture.cs16[,loop=1]`.
+ *      with `-d driver=file,path=capture.cs16[,loop=1][,reads=a:b:c]`; reads= caps successive reads at a, b, c, a, ...
+ *      complex elements, the way a device that reads in packets returns them.
  *
  * Behaviour that matters: readStream (copies the next numElems CS16 complex elements,
  * returns the count, SOAPY_SDR_TIMEOUT... never; returns -2 STREAM_ERROR at end of data so
@@ -34,6 +35,9 @@ struct SoapySDRDevice {
 	double rate;
 	double bw;
 	long long reads;        /* number of readStream calls served */
+	size_t read_len[64];    /* reads=a:b:c: a read returns at most these many complex elements, in turn (a device reading in packets) */
+	int n_read_len;         /* 0: a read returns whatever was asked for, as far as the capture goes */
+	int read_idx;
 };
 struct SoapySDRStream { int active; };
 
@@ -141,6 +145,18 @@ SoapySDRDevice *SoapySDRDevice_makeStrArgs(const char *args)
 		if (load_file(v) != 0) { return NULL; }
 	}
 	g_dev.loop = (args && kw_find(args, "loop", v, sizeof v)) ? atoi(v) : g_dev.loop;
+	g_dev.n_read_len = 0; g_dev.read_idx = 0;
+	if (args && kw_find(args, "reads", v, sizeof v)) {
+		char *p = v;
+		while (*p && g_dev.n_read_len < 64) {
+			char *e;
+			long n = strtol(p, &e, 10);
+			if (e == p || n < 1) { g_err = "fake: reads=a:b:c takes positive element counts"; return NULL; }
+			g_dev.read_len[g_dev.n_read_len++] = (size_t)n;
+			p = (*e == ':') ? e + 1 : e;
+			if (*e != ':' && *e) { g_err = "fake: reads=a:b:c takes positive element counts"; return NULL; }
+		}
+	}
 	return &g_dev;
 }
 int SoapySDRDevice_unmake(SoapySDRDevice *d) { (void)d; return 0; }
@@ -184,6 +200,11 @@ int SoapySDRDevice_readStream(SoapySDRDevice *d, SoapySDRStream *s, void * const
 	}
 	avail = d->n_complex - d->pos;
 	n = numElems < avail ? numElems : avail;
+	if (d->n_read_len) {
+		const size_t cap = d->read_len[d->read_idx];
+		d->read_idx = (d->read_idx + 1) % d->n_read_len;
+		if (n > cap) { n = cap; }
+	}
 	memcpy(buffs[0], (const unsigned char *)d->mem + d->elem_size * d->pos, n * d->elem_size);
 	d->pos += n;
 	return (int)n;

@@ -130,8 +130,13 @@ size_t rxb200_fm_max_output(const rxb200_fm *h, size_t n_int16, size_t chunk_int
  *   pcm       : HOST pointer, channel c's concatenated demod.result at pcm + c*pcm_stride.
  *   n_pcm     : receives the int16 count produced per channel (identical for all channels).
  *   chunk_result_len : optional, receives demod.result_len of every chunk (n_chunks ints).
- * Constraints (RXB200_EUNSUPPORTED otherwise): chunk_int16 % 16 == 0, chunk_int16 <= 262144,
- * every chunk (the last one included) a multiple of 2*2^P int16. */
+ * Constraints (RXB200_EUNSUPPORTED otherwise): 2 <= chunk_int16 <= 262144.  Without fifth_order
+ * passes (downsample_passes == 0) chunk_int16 and n_int16 may be any even count, the last chunk
+ * any even length (whole complex samples, as readStream returns them).  With passes every chunk
+ * (the last one included) is a multiple of 16 int16 and of 2*2^P int16.  Every chunk must produce
+ * a decimated sample when a per-chunk reduction stage is on, and decimate to a multiple of
+ * post_downsample.  rxb200_fm_process_device wants d_cs16 32-byte aligned, or 4-byte aligned for
+ * a call without passes whose chunk or length is not a multiple of 16 int16. */
 int rxb200_fm_process(rxb200_fm *h, const int16_t *cs16, size_t n_int16, size_t chunk_int16,
                       int16_t *pcm, size_t pcm_stride, size_t *n_pcm, int *chunk_result_len);
 

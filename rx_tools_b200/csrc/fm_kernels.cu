@@ -1310,6 +1310,43 @@ __device__ __forceinline__ void front_run(const FmDev &c, const FmCall &k, Front
 	}
 }
 
+// front_run for calls whose chunk or length is not a multiple of 8 complex samples (boxcar shapes only, P = 0).  A
+// channel's base, and with it every block, is then only 4-byte aligned, the segment that ends the channel may end inside
+// a block, and a chunk may start between any two samples: each sample is one 32-bit load (the loads of a block issue
+// together, none past t_end), and the chunk bookkeeping -- rotation phase, F8's first_in_chunk, the per-chunk
+// scalars and sums -- runs before every sample, so the samples on each side of a boundary see their own chunk's values.
+template <int SPEC, bool STORE>
+__device__ __forceinline__ void front_run_any(const FmDev &c, const FmCall &k, FrontState<0, SPEC> &s, EmitCtx &e,
+                                              const uint32_t *__restrict__ in, int t, int t_end, unsigned &u, int ch)
+{
+	const bool rot = Spec<SPEC>::rotate(c);
+	for (; t < t_end; t += 8) {
+		const int nb = t_end - t;
+		uint32_t v[8];
+#pragma unroll
+		for (int j = 0; j < 8; j++) { v[j] = j < nb ? __ldg(in + t + j) : 0u; }
+#pragma unroll
+		for (int j = 0; j < 8; j++) {
+			if (j < nb) {
+				if (u >= (unsigned)k.chunk) { u = 0u; }
+				if (u == 0u) {
+#pragma unroll 1
+					for (int z = 0; z < k.one; z++) { front_chunk_start<0, SPEC, STORE>(c, k, s, e, ch); }
+				}
+				int xi, xq;
+				scale_rot(v[j], (int)(u & 3u), rot, xi, xq, e.rdc_i, e.rdc_q);   // rotate16_90 restarts with every chunk
+				u++;
+				s.box_i += xi; s.box_q += xq;
+				if (++s.box_n >= c.D) {
+					int di = wrap16(s.box_i), dq = wrap16(s.box_q);
+					s.box_i = 0; s.box_q = 0; s.box_n = 0;
+					post_decim<0, SPEC, STORE>(c, k, s, e, di, dq);
+				}
+			}
+		}
+	}
+}
+
 // geometry of one work item (one CTA stretch of one channel)
 struct Item {
 	int ch, b;
@@ -1336,8 +1373,8 @@ __device__ __forceinline__ Item make_item(const FmDev &c, const FmCall &k, int w
 	return it;
 }
 
-// ---- front end of one work item: one segment per thread (tid 0..T-1)
-template <int P, int SPEC>
+// ---- front end of one work item: one segment per thread (tid 0..T-1).  ANY: the any-length front end (front_run_any)
+template <int P, int SPEC, bool ANY>
 __device__ __forceinline__ void front_item(const FmDev &c, const FmCall &k, const Item &it, int tid, int16_t *pcm_s)
 {
 	const uint32_t *carry = k.carry_in + (size_t)it.ch * k.state_words;
@@ -1371,9 +1408,16 @@ __device__ __forceinline__ void front_item(const FmDev &c, const FmCall &k, cons
 	}
 	// offsets relative to t0 fit 32 bits (a segment plus its halo)
 	const int16_t *__restrict__ in = k.in + 2 * ((size_t)it.ch * (size_t)k.n + (size_t)t0);
-	const int t_last = (int)(end - t0) - 8;
-	front_run<P, SPEC, false>(c, k, s, e, in, 0, (int)(start - t0), t_last, u, it.ch);
-	front_run<P, SPEC, true>(c, k, s, e, in, (int)(start - t0), (int)(end - t0), t_last, u, it.ch);
+	if constexpr (ANY) {
+		static_assert(P == 0 && (SPEC == 0 || SPEC == 2), "the any-length front end is the generic boxcar one");
+		const uint32_t *in_w = reinterpret_cast<const uint32_t *>(in);
+		front_run_any<SPEC, false>(c, k, s, e, in_w, 0, (int)(start - t0), u, it.ch);
+		front_run_any<SPEC, true>(c, k, s, e, in_w, (int)(start - t0), (int)(end - t0), u, it.ch);
+	} else {
+		const int t_last = (int)(end - t0) - 8;
+		front_run<P, SPEC, false>(c, k, s, e, in, 0, (int)(start - t0), t_last, u, it.ch);
+		front_run<P, SPEC, true>(c, k, s, e, in, (int)(start - t0), (int)(end - t0), t_last, u, it.ch);
+	}
 	if (SPEC == 2 && k.reduce_mode == 1) { chunk_enter<true>(c, k, e, it.ch, e.chunk_idx); }   // flush the last chunk's sums
 	if (end == k.n && (SPEC != 2 || k.reduce_mode == 0)) {
 		// this thread saw the end of the stream: its registers are the next call's carry
@@ -1601,7 +1645,8 @@ __device__ __forceinline__ void back_item(const FmDev &c, const FmCall &k, const
 // `be_lanes/32` warps run the back end out of the shared PCM buffer.  Work items are handed out by an
 // atomic ticket, oldest first (the cross-item look-back only ever waits for an older ticket).
 // The occupancy target is stated for 256 threads and scales with the width (same threads per SM).
-template <int P, int SPEC, int T>
+// ANY: the any-length front end (front_run_any), for the calls fm_any_length picks.
+template <int P, int SPEC, int T, bool ANY = false>
 __global__ void __launch_bounds__(T, (FM_MAX_THREADS / T) * (SPEC == 2 ? (P <= 3 ? 2 : 1) : (P <= 3 ? RXB_OCC : (P <= 6 ? 2 : 1)))) fm_fused_kernel(const FmDev c, const FmCall k)
 {
 	extern __shared__ __align__(16) int16_t pcm_s[];
@@ -1619,7 +1664,7 @@ __global__ void __launch_bounds__(T, (FM_MAX_THREADS / T) * (SPEC == 2 ? (P <= 3
 		const int work = s_work;
 		if (work >= total_work) { break; }
 		const Item it = make_item(c, k, work);
-		front_item<P, SPEC>(c, k, it, tid, pcm_s);
+		front_item<P, SPEC, ANY>(c, k, it, tid, pcm_s);
 		if (direct || (SPEC == 2 && k.reduce_mode == 1)) {
 			if (tid == 0 && it.b == k.n_cta - 1 && (SPEC != 2 || k.reduce_mode == 0)) {
 				const uint32_t *carry = k.carry_in + (size_t)it.ch * k.state_words;
@@ -1914,6 +1959,20 @@ static fm_kernel_fn pick_kernel(int P, int spec, int threads)
 	return pick_kernel_p<0>(P, threads);
 }
 
+// The any-length variant: the generic boxcar kernel (SPEC 0, or SPEC 2 with the per-chunk reduction stages) in one CTA
+// width; every other specialisation's shape is also a SPEC 0 shape
+#define FM_ANY_THREADS 256
+static fm_kernel_fn pick_any_kernel(int P, int spec)
+{
+#ifdef RXB_QUICK
+	(void)P; (void)spec;
+	return nullptr;
+#else
+	if (P != 0) { return nullptr; }
+	return spec == 2 ? fm_fused_kernel<0, 2, FM_ANY_THREADS, true> : fm_fused_kernel<0, 0, FM_ANY_THREADS, true>;
+#endif
+}
+
 }  // namespace rxb
 
 // ================================================================================ host side
@@ -1958,6 +2017,7 @@ struct rxb200_fm {
 	fm_split_fn kern_rows = nullptr;     // split kernel with the row front end (null: shape not covered)
 	fm_kernel_fn kern_front = nullptr;   // stream path: front end alone (SPEC 4), PCM to global memory; fm_back_kernel follows
 	int16_t *d_pcm = nullptr; size_t d_pcm_cap = 0;       // its PCM scratch, int16 elements
+	fm_kernel_fn kern_any = nullptr;     // any-length calls (P = 0, chunk or call not a multiple of 8 complex), FM_ANY_THREADS wide
 	size_t stream_min = 0; int stream_piece = 0, stream_win = 0, stream_t = 0;
 	int threads = 0;               // CTA width of kern
 	int wide = 0;                  // all-scalar fifth_order passes (raw DC block on)
@@ -2073,6 +2133,7 @@ extern "C" int rxb200_fm_create(const rxb200_fm_params *params, int device, int 
 		h->kern = pick_kernel(params->downsample_passes, spec, h->threads);
 		const int fir_on = (params->downsample_passes > 0 && params->comp_fir_size == 9) ? 1 : 0;
 		h->kern_rows = spec == 1 ? pick_rows_kernel(params->downsample_passes, fir_on) : nullptr;
+		h->kern_any = pick_any_kernel(params->downsample_passes, spec);
 		// stream path (front kernel + back kernel): the wbfm shape without decimating passes, de-emphasis on
 #ifndef RXB_QUICK
 		h->kern_front = (spec == 1 && params->downsample_passes == 0 && params->deemph) ? pick_kernel(0, 4, h->threads) : nullptr;
@@ -2201,9 +2262,18 @@ extern "C" size_t rxb200_fm_max_output(const rxb200_fm *h, size_t n_int16, size_
 	return dec;
 }
 
+// A call the any-length kernel runs: no fifth_order passes, and a chunk or the call not a multiple of 8 complex samples
+// (the vector kernels' block).  Every other call keeps the kernels and plans of the 8-sample granule.
+static bool fm_any_length(const rxb200_fm *h, size_t n_int16, size_t chunk_int16)
+{
+	return h->kern_any != nullptr && (chunk_int16 % 16 != 0 || n_int16 % 16 != 0);
+}
+
 static int fm_check_shape(const rxb200_fm *h, size_t n_int16, size_t chunk_int16)
 {
-	size_t g16 = 16;                                  // 8 complex per vector step
+	// Without passes any whole number of complex samples (the any-length kernel takes what the vector kernels cannot);
+	// with passes 8 complex per vector step and 2^P complex per chunk (DESIGN.md section 6)
+	size_t g16 = h->kern_any ? 2 : 16;
 	size_t p16 = (size_t)2 << h->p.downsample_passes; // 2^P complex
 	if (p16 > g16) { g16 = p16; }
 	if (chunk_int16 == 0 || chunk_int16 > 262144 || chunk_int16 % g16 != 0) {
@@ -2352,10 +2422,9 @@ static int fm_plan_rows(const rxb200_fm *h, long long n, FmCall *k, FmGrid *g)
 	return RXB200_OK;
 }
 
-static int fm_plan_segments(const rxb200_fm *h, fm_kernel_fn kern, long long n, bool stream, FmCall *k, FmGrid *g)
+static int fm_plan_segments(const rxb200_fm *h, fm_kernel_fn kern, int T, long long n, bool stream, FmCall *k, FmGrid *g)
 {
 	const FmDev &dv = h->dev;
-	const int T = h->threads;
 	const int P = h->p.downsample_passes;
 	const long long Dtot = dv.D;
 	const long long G = (1LL << P) > 8 ? (1LL << P) : 8;
@@ -2566,14 +2635,16 @@ static int fm_launch(rxb200_fm *h, const int16_t *d_in, size_t n_int16, size_t c
 	// a few thousand samples and the front end computes nothing twice.  Worth it from a few dozen replays of PCM per call.
 	const long long Dpcm = (long long)dv.D * dv.post_ds;
 	const size_t stream_min = h->stream_min != (size_t)-1 ? h->stream_min : (size_t)(32 * fm_replay(h, false) * Dpcm / h->n_channels);
-	const bool stream = h->kern_front != nullptr && dv.deemph && (size_t)n >= stream_min;
-	const fm_kernel_fn kern = stream ? h->kern_front : h->kern;
+	// an any-length call runs on its own kernel, front and back end fused, whatever the shape would take otherwise
+	const bool any = fm_any_length(h, n_int16, chunk_int16);
+	const bool stream = !any && h->kern_front != nullptr && dv.deemph && (size_t)n >= stream_min;
+	const fm_kernel_fn kern = any ? h->kern_any : (stream ? h->kern_front : h->kern);
 	FmCall k = {};
 	FmGrid g;
 	CUtensorMap in_map;
 	int rc = rows ? fm_plan_rows(h, n, &k, &g) : RXB200_OK;
 	if (rc == FM_ROWS_NO_ROOM) { rows = false; k = {}; rc = RXB200_OK; }   // the same call on the fused kernel
-	if (rc == RXB200_OK) { rc = rows ? fm_rows_map(d_in, (long long)h->n_channels * (n / 32), &in_map) : fm_plan_segments(h, kern, n, stream, &k, &g); }
+	if (rc == RXB200_OK) { rc = rows ? fm_rows_map(d_in, (long long)h->n_channels * (n / 32), &in_map) : fm_plan_segments(h, kern, any ? FM_ANY_THREADS : h->threads, n, stream, &k, &g); }
 	if (rc != RXB200_OK) { return rc; }
 	const size_t total_work = (size_t)k.n_cta * h->n_channels;
 	FmBackPlan b = {};
@@ -2654,8 +2725,12 @@ static int fm_prologue(rxb200_fm *h, const void *in, const void *out, size_t n_i
 extern "C" int rxb200_fm_process_device(rxb200_fm *h, const int16_t *d_cs16, size_t n_int16, size_t chunk_int16,
                                         int16_t *d_pcm, size_t pcm_stride, size_t *n_pcm, int sync)
 {
-	// null arguments are reported first, by fm_prologue
-	if (h && d_cs16 && d_pcm && ((uintptr_t)d_cs16 & 31u) != 0) { set_error("d_cs16 must be 32-byte aligned"); return RXB200_EINVAL; }
+	// null arguments are reported first, by fm_prologue; the any-length kernel reads one complex sample at a time
+	const uintptr_t align = (h && fm_any_length(h, n_int16, chunk_int16)) ? 4u : 32u;
+	if (h && d_cs16 && d_pcm && ((uintptr_t)d_cs16 & (align - 1u)) != 0) {
+		set_error("d_cs16 must be %d-byte aligned", (int)align);
+		return RXB200_EINVAL;
+	}
 	size_t total = 0;
 	int rc = fm_prologue(h, d_cs16, d_pcm, n_int16, chunk_int16, pcm_stride, nullptr, &total, n_pcm);
 	if (rc != RXB200_OK || n_int16 == 0) { return rc; }
