@@ -229,8 +229,8 @@ int rxb200_sine_table(int log2_n, int16_t *sine);
 
 typedef struct rxb200_power rxb200_power;
 
-/* window_coefs: N ints (the global window_coefs table); sinewave: 3N/4 int16 (the global Sinewave)
- * or NULL to build it with rxb200_sine_table. */
+/* window_coefs: N ints (the global window_coefs table; only w mod 2^16 changes the result); sinewave:
+ * 3N/4 int16 (the global Sinewave, any values, -32768 included) or NULL to build it with rxb200_sine_table. */
 int rxb200_power_create(const rxb200_power_params *params, const int *window_coefs,
                         const int16_t *sinewave, int device, rxb200_power **out);
 void rxb200_power_destroy(rxb200_power *h);
@@ -251,6 +251,23 @@ void *rxb200_power_stream(rxb200_power *h);
 int rxb200_power_last_launches(rxb200_power *h);
 /* Device time of the batched kernel alone in the last accumulate call (ms); synchronises. */
 int rxb200_power_kernel_ms(rxb200_power *h, float *ms);
+/* What the last accumulate call with n_pass > 0 ran (kernel RXB200_POWER_PATH_NONE before the first). */
+#define RXB200_POWER_PATH_NONE 0
+#define RXB200_POWER_PATH_RMS 1          /* power_rms_kernel (bin_e == 0)                                     */
+#define RXB200_POWER_PATH_FFT8 2         /* power_fft8_kernel<bin_e, threads>                                 */
+#define RXB200_POWER_PATH_GENERIC 3      /* power_fft_kernel<nb>                                              */
+#define RXB200_POWER_PATH_BIG_LOAD 4     /* hop buffer beyond shared memory: copy / boxcar, then the FFT steps  */
+#define RXB200_POWER_PATH_BIG_DECIM 5    /* hop buffer beyond shared memory: -F passes, then the FFT steps      */
+typedef struct rxb200_power_path {
+	int kernel;             /* RXB200_POWER_PATH_*                                                          */
+	int bin_e;
+	int threads;            /* CTA width of the main kernel                                                 */
+	int nb;                 /* GENERIC: bins each thread accumulates in registers, 0 = straight to global; else -1 */
+	int tables_in_smem;     /* GENERIC: sine and window tables staged in shared memory; FFT8: 1; else 0      */
+	int slices;             /* CTAs per hop, each taking every slices-th pass; 0 on the big paths           */
+	int launches;           /* kernel launches of the call (rxb200_power_last_launches)                     */
+} rxb200_power_path;
+int rxb200_power_last_path(rxb200_power *h, rxb200_power_path *out);
 
 /* csv_dbm()'s numeric half ON THE DEVICE (src/rtl_power.c:783-811): DC-bin patch, half swap, crop and
  * power -> dB in the reference's fp64 operation order, so that only the final dB values leave the GPU.

@@ -248,12 +248,17 @@ class Port:
 
     def power_scan(self, params: PowerParams, window: np.ndarray, hop_bufs: np.ndarray,
                    n_pass: int, n_hops: int, avg: Optional[np.ndarray] = None,
-                   samples: Optional[np.ndarray] = None):
+                   samples: Optional[np.ndarray] = None, sine: Optional[np.ndarray] = None):
+        """sine: a caller's Sinewave table (3N/4 int16), else the one sine_table() builds."""
         n = 1 << params.bin_e
         hb = _i16(hop_bufs).reshape(-1)
         assert hb.size == n_pass * n_hops * params.buf_len
         win = np.ascontiguousarray(window, dtype=np.int32)
-        sine = self.sine_table(max(params.bin_e, 1))
+        if sine is None:
+            sine = self.sine_table(max(params.bin_e, 1))
+        else:
+            sine = _i16(sine)
+            assert sine.size >= n * 3 // 4
         avg = np.zeros((n_hops, n), dtype=np.int64) if avg is None else avg
         samples = np.zeros(n_hops, dtype=np.int32) if samples is None else samples
         pc = params.to_c()

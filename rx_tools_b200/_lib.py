@@ -47,6 +47,13 @@ class PowerParamsC(C.Structure):
         "n_hops", "bin_e", "buf_len", "downsample", "downsample_passes", "comp_fir_size", "boxcar", "peak_hold")]
 
 
+class PowerPathC(C.Structure):
+    _fields_ = [(n, C.c_int) for n in ("kernel", "bin_e", "threads", "nb", "tables_in_smem", "slices", "launches")]
+
+
+POWER_PATHS = {0: "none", 1: "rms", 2: "fft8", 3: "generic", 4: "big_load", 5: "big_decim"}
+
+
 class PowerPlanC(C.Structure):
     _fields_ = [("params", PowerParamsC), ("rate", C.c_int), ("crop", C.c_double),
                 ("first_freq", C.c_int64), ("freq_step", C.c_int64), ("bin_size_hz", C.c_double)]
@@ -62,7 +69,7 @@ SYMBOLS = [
     "rxb200_power_destroy", "rxb200_power_accumulate", "rxb200_power_accumulate_device", "rxb200_power_read",
     "rxb200_power_device_avg", "rxb200_power_reset", "rxb200_power_stream", "rxb200_power_last_launches",
     "rxb200_power_format_row", "rxb200_power_kernel_ms", "rxb200_power_row_len", "rxb200_power_read_db",
-    "rxb200_power_format_db_row",
+    "rxb200_power_format_db_row", "rxb200_power_last_path",
     "rxb200_comm_unique_id", "rxb200_comm_create", "rxb200_comm_create_all", "rxb200_comm_destroy", "rxb200_comm_size",
     "rxb200_comm_rank", "rxb200_power_shard", "rxb200_power_gather",
     "rxb200_power_group_create", "rxb200_power_group_destroy", "rxb200_power_group_size", "rxb200_power_group_member",
@@ -116,6 +123,7 @@ def lib() -> C.CDLL:
     L.rxb200_power_stream.restype = C.c_void_p
     L.rxb200_power_stream.argtypes = [C.c_void_p]
     L.rxb200_power_last_launches.argtypes = [C.c_void_p]
+    L.rxb200_power_last_path.argtypes = [C.c_void_p, C.POINTER(PowerPathC)]
     L.rxb200_power_format_row.argtypes = [pi64, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_double, C.c_int,
                                           C.c_char_p, sz]
     L.rxb200_power_row_len.argtypes = [C.c_int, C.c_double]

@@ -47,6 +47,10 @@ __device__ __forceinline__ int q15(int a, int b)
 	return (a * b + 16384) >> 15;     // (a mulhi-by-2^17 form on the multiplier pipe instead of the shifter measured slower)
 }
 
+// wi = -Sinewave[j] >> 1 (src/rtl_power.c:298-301): the negation is stored in an int16 before the shift, so -(-32768)
+// stays -32768.  Only a caller's table can hold -32768 (sine_table's entries are round(32767 sin)).
+__device__ __forceinline__ int neg_half(int s) { return (int)(int16_t)(-s) >> 1; }
+
 __device__ __forceinline__ long long block_sum(long long v, long long *red, int tid, int nthreads)
 {
 	for (int o = 16; o > 0; o >>= 1) { v += __shfl_down_sync(0xffffffffu, v, o); }
@@ -243,7 +247,7 @@ __global__ void __launch_bounds__(256) power_fft_kernel(const PowArgs a)
 					int j = i + l;
 					int jt = m << k;
 					int wr = (int)sine[jt + N / 4] >> 1;
-					int wi = (-(int)sine[jt]) >> 1;
+					int wi = neg_half(sine[jt]);
 					uint32_t u = x[i], v = x[j];
 					int vr = plo(v), vi = phi(v);
 					int tr = q15(wr, vr) - q15(wi, vi);
@@ -425,10 +429,10 @@ __global__ void __launch_bounds__(T, 1024 / T) power_fft8_kernel(const PowArgs a
 	const int hop = a.hop_begin + hop_local;
 	const int uu = tid & (UPB - 1);            // the same in every half (UPB divides T)
 
-	// tables: packed twiddles (wr = Sinewave[j + N/4] >> 1, wi = (-Sinewave[j]) >> 1, src/rtl_power.c:298-301)
+	// tables: packed twiddles (wr = Sinewave[j + N/4] >> 1, wi = (int16)(-Sinewave[j]) >> 1, src/rtl_power.c:298-301)
 	for (int i = tid; i < N / 2; i += T) {
 		int wr = (int)a.sine[i + N / 4] >> 1;
-		int wi = (-(int)a.sine[i]) >> 1;
+		int wi = neg_half(a.sine[i]);
 		tw[i] = ppack(wr, wi);
 	}
 	for (int i = tid; i < N; i += T) { win[i] = a.window[i]; }
@@ -596,9 +600,12 @@ __global__ void __launch_bounds__(256) power_rms_kernel(const PowArgs a)
 //   big_window: (x - ave) * w with int16 wrap (:749-758), stored bit-reversed (fix_fft's swap pass, :275-290)
 //   big_stage:  one radix-2 stage over every N-block (:291-318)
 //   big_accum:  real_conj accumulate / peak hold (:760-768)
-__global__ void __launch_bounds__(256) power_big_load(const int16_t *src, uint32_t *work, int n_complex, int ds, long long *sums)
+__global__ void __launch_bounds__(256) power_big_load(const int16_t *src, uint32_t *work, int n_complex, int ds, int used_int16,
+                                                      long long *sums)
 {
 	const int n_out = (n_complex + ds - 1) / ds;
+	// remove_dc sums the first used_int16 int16 (:744-745): a partial last slot of the boxcar may lie past that span
+	const int n_i = (used_int16 + 1) / 2, n_q = used_int16 / 2;
 	long long si = 0, sq = 0;
 	for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < n_out; k += gridDim.x * blockDim.x) {
 		int a = 0, b = 0;
@@ -606,7 +613,8 @@ __global__ void __launch_bounds__(256) power_big_load(const int16_t *src, uint32
 		for (int i = k * ds; i < e; i++) { a += src[2 * i]; b += src[2 * i + 1]; }
 		a = (int)(int16_t)a; b = (int)(int16_t)b;                 // the in-place int16 "+=" of the reference wraps
 		work[k] = ppack(a, b);
-		si += a; sq += b;
+		if (k < n_i) { si += a; }
+		if (k < n_q) { sq += b; }
 	}
 	for (int o = 16; o > 0; o >>= 1) { si += __shfl_down_sync(0xffffffffu, si, o); sq += __shfl_down_sync(0xffffffffu, sq, o); }
 	if ((threadIdx.x & 31) == 0) {
@@ -762,7 +770,7 @@ __global__ void __launch_bounds__(256) power_big_stage(uint32_t *fft, const int1
 		const int i = ((t >> s) << (s + 1)) + m, j = i + l;
 		const int jt = m << k;
 		const int wr = (int)sine[jt + N / 4] >> 1;
-		const int wi = (-(int)sine[jt]) >> 1;
+		const int wi = neg_half(sine[jt]);
 		const uint32_t u = x[i], v = x[j];
 		const int vr = plo(v), vi = phi(v);
 		const int tr = q15(wr, vr) - q15(wi, vi);
@@ -820,6 +828,7 @@ struct rxb200_power {
 	int decim_tile = 0; size_t decim_smem = 0;                                   // power_big_decim's tile (final samples) and shared memory
 	int force_v1 = 0;                          // RXB200_POWER_V1 (A/B knob, read once at create): generic kernel only
 	int fft8_threads = 0;                      // RXB200_POWER_THREADS = 512 | 1024 (A/B knob): CTA width of the fast path
+	rxb200_power_path path = {};               // what the last accumulate ran (rxb200_power_last_path)
 };
 
 static int power_validate(const rxb200_power_params *p)
@@ -1008,6 +1017,7 @@ extern "C" int rxb200_power_accumulate_device(rxb200_power *h, const int16_t *d_
 	if (slices < 1) { slices = 1; }
 	a.slices = slices;
 	const int blocks = nh * slices;
+	rxb200_power_path path = {RXB200_POWER_PATH_RMS, h->p.bin_e, 256, -1, 0, slices, 1};
 	RXB_CUDA(cudaEventRecord(h->ev0, h->stream));
 	if (h->p.bin_e == 0) {
 		power_rms_kernel<<<blocks, 256, 0, h->stream>>>(a);
@@ -1045,7 +1055,7 @@ extern "C" int rxb200_power_accumulate_device(rxb200_power *h, const int16_t *d_
 						power_big_decim<<<(n_slots + h->decim_tile - 1) / h->decim_tile, 256, h->decim_smem, h->stream>>>(
 							src, h->d_work, n_slots, h->decim_tile, P, a.fir_on, fir, h->d_sums);
 					} else {
-						power_big_load<<<g, 256, 0, h->stream>>>(src, h->d_work, n_complex, ds, h->d_sums);
+						power_big_load<<<g, 256, 0, h->stream>>>(src, h->d_work, n_complex, ds, used, h->d_sums);
 					}
 					power_big_window<<<g, 256, 0, h->stream>>>(h->d_work, h->d_fft, h->d_window, h->d_sums, used, n_slots, h->p.bin_e, nblk);
 					for (int st = 0; st < h->p.bin_e; st++) { power_big_stage<<<g, 256, 0, h->stream>>>(h->d_fft, h->d_sine, h->p.bin_e, st, nblk); }
@@ -1056,6 +1066,7 @@ extern "C" int rxb200_power_accumulate_device(rxb200_power *h, const int16_t *d_
 			for (int i = hop_begin; i < hop_end; i++) { h->samples[i] += n_pass * nblk * ds; }           // :769
 			RXB_CUDA(cudaEventRecord(h->ev1, h->stream));
 			h->launches = n_pass * nh * (3 + h->p.bin_e);
+			h->path = {decim ? RXB200_POWER_PATH_BIG_DECIM : RXB200_POWER_PATH_BIG_LOAD, h->p.bin_e, 256, -1, 0, 0, h->launches};
 			if (sync) { RXB_CUDA(cudaStreamSynchronize(h->stream)); }
 			return RXB200_OK;
 		}
@@ -1083,8 +1094,10 @@ extern "C" int rxb200_power_accumulate_device(rxb200_power *h, const int16_t *d_
 			const size_t sm8 = 16 + 512 + 2 * (8192 + 1024) * 4 + (size_t)(N / 2 > 4 ? N / 2 : 4) * 4 + (size_t)N * 2;
 			e = launch_fft8(h->p.bin_e, threads, a, nh * sl, sm8, h->stream);
 			if (e != cudaSuccess) { set_error("power_fft8_kernel launch: %s", cudaGetErrorString(e)); return RXB200_ECUDA; }
+			path = {RXB200_POWER_PATH_FFT8, h->p.bin_e, threads, -1, 1, sl, 1};
 		} else {
 		const int nb = N / 256;
+		path = {RXB200_POWER_PATH_GENERIC, h->p.bin_e, 256, nb <= 1 ? 1 : (nb <= 16 ? nb : 0), a.tables_in_smem, slices, 1};
 		if (nb <= 1) { e = launch_fft<1>(a, blocks, smem, h->stream); }
 		else if (nb == 2) { e = launch_fft<2>(a, blocks, smem, h->stream); }
 		else if (nb == 4) { e = launch_fft<4>(a, blocks, smem, h->stream); }
@@ -1099,6 +1112,7 @@ extern "C" int rxb200_power_accumulate_device(rxb200_power *h, const int16_t *d_
 	}
 	RXB_CUDA(cudaEventRecord(h->ev1, h->stream));
 	h->launches = 1;
+	h->path = path;
 	if (sync) { RXB_CUDA(cudaStreamSynchronize(h->stream)); }
 	return RXB200_OK;
 }
@@ -1204,6 +1218,12 @@ extern "C" int rxb200_power_reset(rxb200_power *h)
 
 extern "C" void *rxb200_power_stream(rxb200_power *h) { return h ? (void *)h->stream : nullptr; }
 extern "C" int rxb200_power_last_launches(rxb200_power *h) { return h ? h->launches : 0; }
+extern "C" int rxb200_power_last_path(rxb200_power *h, rxb200_power_path *out)
+{
+	if (!h || !out) { set_error("null argument"); return RXB200_EINVAL; }
+	*out = h->path;
+	return RXB200_OK;
+}
 
 // ================================================================================ multi-GPU (SURVEY.md §8e)
 // Tuner hops are independent; rank r of n owns the contiguous hops [r*per, (r+1)*per), per = ceil(n_hops/n).

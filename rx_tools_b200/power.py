@@ -142,6 +142,15 @@ class PowerScanner:
     def reset(self) -> None:
         _lib.check(_lib.lib().rxb200_power_reset(self._h))
 
+    def last_path(self) -> dict:
+        """What the last scanner call ran (rxb200_power_last_path): kernel is one of "none", "rms", "fft8", "generic",
+        "big_load", "big_decim"."""
+        out = _lib.PowerPathC()
+        _lib.check(_lib.lib().rxb200_power_last_path(self._h, C.byref(out)))
+        d = {n: int(getattr(out, n)) for n, _ in out._fields_}
+        d["kernel"] = _lib.POWER_PATHS[d["kernel"]]
+        return d
+
     def kernel_ms(self) -> float:
         ms = C.c_float(0)
         _lib.check(_lib.lib().rxb200_power_kernel_ms(self._h, C.byref(ms)))
