@@ -114,6 +114,17 @@ __device__ __forceinline__ void mbar_arrive(uint64_t *bar)
 {
 	asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
+
+// flags that other CTAs poll during a launch.  A release store makes the writer's earlier writes -- and, being
+// cumulative, those of threads it synchronised with (a __syncwarp or barrier before it) -- visible to a reader that
+// acquires the flag.  That is all a hand-over needs; a __threadfence() (fence.sc) before the flag is not.
+__device__ __forceinline__ int ld_acquire_gpu(const int *p)
+{
+	int v;
+	asm volatile("ld.acquire.gpu.global.b32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+	return v;
+}
+__device__ __forceinline__ void st_release_gpu(int *p, int v) { asm volatile("st.release.gpu.global.b32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
 #endif
 
 }  // namespace rxb

@@ -41,7 +41,6 @@ namespace rxb {
 #define RXB_L2_AHEAD 64
 #define RXB_OCC 3                // resident CTAs per SM of the P <= 3 kernels, stated for 256 threads
 #define FM_MAX_PACKED 3          // fifth_order passes run as packed I/Q SWAR (bias keeps lanes unsigned)
-
 // ------------------------------------------------------------------------------ device config
 struct FmDev {
 	int mode, D, P, PL, fir_on, atan_mode, out_scale, post_ds;
@@ -92,6 +91,29 @@ struct FmCall {
 	const int16_t *pcm_g;     // fm_back_kernel: [n_ch][pcm_g_stride] PCM of the whole call in global memory (null elsewhere)
 	long long pcm_g_stride;
 };
+
+// Scratch builds (-DRXB_PROF): per-warp clock64() sums of the split kernel's phases in a device array that
+// tools/fm_prof.py reads back (rxb200_fm_prof_read).  Compiles to nothing by default.
+#ifdef RXB_PROF
+#define PROF_CTAS 1024
+#define PROF_SLOTS 16
+enum { PF_WARPID = 0, PF_SMID, PF_TOTAL, PF_ITEMS, PF_ROWS, PF_FRONT, PF_BAR_FE, PF_EMPTY, PF_RING, PF_PUBLISH,
+       PF_FULL, PF_COLLECT, PF_PASS1, PF_CHAIN, PF_PASS2 };
+__device__ unsigned long long rxb_prof[PROF_CTAS * 32 * PROF_SLOTS];
+__device__ __forceinline__ unsigned long long *prof_slot(int s)
+{
+	return rxb_prof + ((size_t)blockIdx.x * 32 + (threadIdx.x >> 5)) * PROF_SLOTS + s;
+}
+#define PROF_CLK(var_) const long long var_ = clock64()
+#define PROF_ADD(slot_, t_) do { if (blockIdx.x < PROF_CTAS && (threadIdx.x & 31) == 0) { *prof_slot(slot_) += (unsigned long long)(clock64() - (t_)); } } while (0)
+#define PROF_SET(slot_, val_) do { if (blockIdx.x < PROF_CTAS && (threadIdx.x & 31) == 0) { *prof_slot(slot_) = (unsigned long long)(val_); } } while (0)
+#define PROF_INC(slot_, val_) do { if (blockIdx.x < PROF_CTAS && (threadIdx.x & 31) == 0) { *prof_slot(slot_) += (unsigned long long)(val_); } } while (0)
+#else
+#define PROF_CLK(var_) do { } while (0)
+#define PROF_ADD(slot_, t_) do { } while (0)
+#define PROF_SET(slot_, val_) do { } while (0)
+#define PROF_INC(slot_, val_) do { } while (0)
+#endif
 
 enum { ST_BOX_I = 0, ST_BOX_Q, ST_BOX_N, ST_PRE_I, ST_PRE_Q, ST_AVG, ST_LPR_ACC, ST_LPR_PHASE,
        ST_SQ_HITS, ST_ADC, ST_RDC_I, ST_RDC_Q, ST_HDR = 16 };
@@ -1472,6 +1494,14 @@ __device__ __forceinline__ void run_piece_win(const FmDev &c, const LaneWin<WS> 
 #define FM_BE_MAX_LANES 256
 #define BAR_BE 1                 // named barrier of the back-end warps (id 0 is __syncthreads)
 __device__ __forceinline__ void bar_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
+// bar_sync that also returns whether `v` holds in every participating thread
+__device__ __forceinline__ bool bar_sync_and(int id, int count, bool v)
+{
+	int r;
+	asm volatile("{\n\t.reg .pred p, q;\n\tsetp.ne.s32 p, %1, 0;\n\tbar.red.and.pred q, %2, %3, p;\n\tselp.s32 %0, 1, 0, q;\n\t}"
+	             : "=r"(r) : "r"((int)v), "r"(id), "r"(count) : "memory");
+	return r != 0;
+}
 
 // WS > 0: the PCM is the call's global array and replay / outputs go through per-lane windows of WS samples in `win_rows`
 // (fm_back_kernel; whole warps call, every lane takes part in the window fills)
@@ -1493,6 +1523,7 @@ __device__ __forceinline__ void back_item(const FmDev &c, const FmCall &k, const
 	if (per < 1) { per = 1; }
 	const int last_q = n_out > 0 ? (n_out - 1) / per : 0;
 	const bool store = (SPEC != 2) || (k.reduce_mode == 0);
+	PROF_CLK(tb0);
 	AdcCtx axs;
 	axs.adc = k.adc ? k.adc + (size_t)it.ch * k.n_chunks : nullptr;
 	axs.sums = (k.reduce_mode == 2) ? k.sums + 2 * (size_t)it.ch * k.n_chunks : nullptr;
@@ -1548,7 +1579,9 @@ __device__ __forceinline__ void back_item(const FmDev &c, const FmCall &k, const
 		else { if (active && kind == PK_EXACT) { run_piece<PAD>(c, pcm_s, out, p, m_run, avg, ax, store); } }
 		s_avg[q] = avg; s_mrun[q] = m_run; s_ok[q] = (unsigned char)kind;
 	}
-	bar_sync(BAR_BE, lanes);
+	const bool all_exact = bar_sync_and(BAR_BE, lanes, kind == PK_EXACT);
+	PROF_ADD(PF_PASS1, tb0);
+	PROF_CLK(tb1);
 	// ---- chain (thread 0).  Across items the published word is a decoupled look-back: 1 = exact end state,
 	// 2 = "this item passes its start state through" (the reader keeps walking back).  An item whose end state
 	// is anchored by one of its own pieces publishes before it looks at anybody else.
@@ -1565,48 +1598,58 @@ __device__ __forceinline__ void back_item(const FmDev &c, const FmCall &k, const
 		};
 		auto publish = [&](int flag, int value) {
 			volatile int *mp = pub + 4 * (size_t)work;
-			if (flag == 1) { mp[1] = value; __threadfence(); }
-			mp[0] = flag;
+			// flag 1: the value goes out before the flag (a release store; the reader fences after seeing the flag)
+			if (flag == 1) { mp[1] = value; st_release_gpu(const_cast<int *>(mp), 1); }
+			else { mp[0] = flag; }
 		};
-		int anchor = -1, n_open = 0, published = 0, fixes = 0;
-		for (int j = last_q; j >= 0; j--) {
-			const int kj = s_ok[j];
-			if (kj == PK_EXACT || kj == PK_MERGED) { anchor = j; break; }
-			if (kj == PK_OPEN) { n_open++; }
+		// Every piece started exact (the common case with signal): the last piece is the anchor, nothing needs a start
+		// state, and what the loops below would do is publish its end state.  A single thread walking the pieces
+		// through dependent shared-memory loads is on the back end's critical path, so skip it.
+		if (all_exact) {
+			if (!last_cta) { publish(1, s_avg[last_q]); }
+		} else {
+			int anchor = -1, n_open = 0, published = 0, fixes = 0;
+			for (int j = last_q; j >= 0; j--) {
+				const int kj = s_ok[j];
+				if (kj == PK_EXACT || kj == PK_MERGED) { anchor = j; break; }
+				if (kj == PK_OPEN) { n_open++; }
+			}
+			if (!last_cta) {
+				if (anchor >= 0) {
+					int cur = s_avg[anchor];
+					for (int j = anchor + 1; j <= last_q; j++) { if (s_ok[j] == PK_OPEN) { cur = serial_end(j, cur); } }
+					publish(1, cur); published = 1;
+				} else if (n_open == 0) { publish(2, 0); published = 2; }
+			}
+			// start states, left to right (piece 0: the closest older item of this channel that knows its end state)
+			int cur = 0;
+			for (int j = 0; j <= last_q; j++) {
+				const int kj = s_ok[j];
+				if (kj == PK_EXACT) { cur = s_avg[j]; continue; }
+				int start;
+				if (j == 0) {
+					int w = work - 1;
+					for (;;) {
+						const int f = pub[4 * (size_t)w];
+						if (f == 0) { __nanosleep(32); continue; }
+						if (f == 1) { __threadfence(); start = pub[4 * (size_t)w + 1]; break; }
+						w--;                                              // f == 2: that item passes its start through
+					}
+				} else { start = cur; }
+				s_start[j] = start;
+				if (kj == PK_MERGED) { cur = s_avg[j]; }
+				else if (kj == PK_IDENT) { cur = start; }
+				else { cur = serial_end(j, start); }
+				s_avg[j] = cur;
+				fixes++;
+			}
+			if (!last_cta && published != 1) { publish(1, s_avg[last_q]); }
+			if (fixes) { atomicAdd(k.fix_count, fixes); }
 		}
-		if (!last_cta) {
-			if (anchor >= 0) {
-				int cur = s_avg[anchor];
-				for (int j = anchor + 1; j <= last_q; j++) { if (s_ok[j] == PK_OPEN) { cur = serial_end(j, cur); } }
-				publish(1, cur); published = 1;
-			} else if (n_open == 0) { publish(2, 0); published = 2; }
-		}
-		// start states, left to right (piece 0: the closest older item of this channel that knows its end state)
-		int cur = 0;
-		for (int j = 0; j <= last_q; j++) {
-			const int kj = s_ok[j];
-			if (kj == PK_EXACT) { cur = s_avg[j]; continue; }
-			int start;
-			if (j == 0) {
-				int w = work - 1;
-				for (;;) {
-					const int f = pub[4 * (size_t)w];
-					if (f == 0) { __nanosleep(32); continue; }
-					if (f == 1) { __threadfence(); start = pub[4 * (size_t)w + 1]; break; }
-					w--;                                              // f == 2: that item passes its start through
-				}
-			} else { start = cur; }
-			s_start[j] = start;
-			if (kj == PK_MERGED) { cur = s_avg[j]; }
-			else if (kj == PK_IDENT) { cur = start; }
-			else { cur = serial_end(j, start); }
-			s_avg[j] = cur;
-			fixes++;
-		}
-		if (!last_cta && published != 1) { publish(1, s_avg[last_q]); }
-		if (fixes) { atomicAdd(k.fix_count, fixes); }
 	}
 	bar_sync(BAR_BE, lanes);
+	PROF_ADD(PF_CHAIN, tb1);
+	PROF_CLK(tb2);
 	// ---- pass 2: the pieces that had no exact start in pass 1 now run from the state the chain gave them
 	if constexpr (WIN) {
 		const bool run = active && kind != PK_EXACT;
@@ -1639,6 +1682,7 @@ __device__ __forceinline__ void back_item(const FmDev &c, const FmCall &k, const
 			co[ST_LPR_PHASE] = c.resample ? (uint32_t)(((long long)it.phase0 + (it.m_lo + it.m_hi) * (long long)c.slow) % (long long)c.fast) : 0u;
 		}
 	}
+	PROF_ADD(PF_PASS2, tb2);
 }
 
 // Persistent CTA of T threads: all warps run the front end of a work item, then the first
@@ -1745,6 +1789,15 @@ __global__ void __launch_bounds__(TMAX, MINB) fm_split_kernel(const FmDev c, con
 	}
 	__syncthreads();
 	const int total_work = k.n_ch * k.n_cta;
+#ifdef RXB_PROF
+	{
+		unsigned wid, smid;
+		asm volatile("mov.u32 %0, %%warpid;" : "=r"(wid));
+		asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
+		PROF_SET(PF_WARPID, wid); PROF_SET(PF_SMID, smid);
+	}
+#endif
+	PROF_CLK(t_start);
 	if (tid < n_fe) {
 		RowRing ring;
 		uint8_t *end = reinterpret_cast<uint8_t *>(pcm_s + 2 * (size_t)k.pcm_cap) + (size_t)k.fe_warps * k.xs_words * sizeof(uint32_t);
@@ -1755,34 +1808,49 @@ __global__ void __launch_bounds__(TMAX, MINB) fm_split_kernel(const FmDev c, con
 		ring.seq = 0;
 		for (int i = 0;; i++) {
 			const int b = i & 1;
+			PROF_CLK(t0);
 			if (i >= 2) { mbar_wait(&s_empty[b], (uint32_t)(((i >> 1) - 1) & 1)); }   // the back end is done with item i-2
+			PROF_ADD(PF_EMPTY, t0);
 			// one barrier per item lines the front-end warps up behind the ticket (measured: letting them run ahead on a
 			// sequence number instead costs 9 % -- the early warps only reach the `empty` wait sooner and take issue
 			// slots from the warp the back end is waiting for)
 			if (tid == 0) { s_ticket[b] = atomicAdd(k.ticket, 1); }
+			PROF_CLK(t1);
 			bar_sync(BAR_FE, n_fe);
+			PROF_ADD(PF_BAR_FE, t1);
 			const int work = s_ticket[b];
 			if (work >= total_work) { mbar_arrive(&s_full[b]); break; }                // the back end sees the sentinel
 			const Item it = make_item(c, k, work);
 			int16_t *buf = pcm_s + (size_t)b * k.pcm_cap;
 			uint32_t *xs = reinterpret_cast<uint32_t *>(pcm_s + 2 * (size_t)k.pcm_cap) + (size_t)(tid >> 5) * k.xs_words;
+			PROF_CLK(t2);
 			front_rows<P, FIR>(c, k, it, tid >> 5, lane, buf, xs, ring);
+			PROF_ADD(PF_FRONT, t2);
+			PROF_CLK(t3);
 			rows_publish<P>(k, it, work, buf, tid >> 5, lane);
+			PROF_ADD(PF_PUBLISH, t3);
+			PROF_INC(PF_ITEMS, 1);
 			mbar_arrive(&s_full[b]);
 		}
 	} else {
 		const int q = tid - n_fe;
 		for (int i = 0;; i++) {
 			const int b = i & 1;
+			PROF_CLK(t0);
 			mbar_wait(&s_full[b], (uint32_t)((i >> 1) & 1));
+			PROF_ADD(PF_FULL, t0);
 			const int work = s_ticket[b];
 			if (work >= total_work) { break; }
 			const Item it = make_item(c, k, work);
+			PROF_CLK(t1);
 			rows_collect<P>(k, it, work, pcm_s + (size_t)b * k.pcm_cap, q, k.be_lanes);
+			PROF_ADD(PF_COLLECT, t1);
 			back_item<SPEC, PCM_PAD_ROWS>(c, k, it, work, q, k.be_lanes, pcm_s + (size_t)b * k.pcm_cap, s_avg, s_mrun, s_ok, s_start);
+			PROF_INC(PF_ITEMS, 1);
 			mbar_arrive(&s_empty[b]);
 		}
 	}
+	PROF_ADD(PF_TOTAL, t_start);
 }
 
 // ---- per-chunk reduction pre-passes: the scalar recurrences across chunks (one thread per channel)
@@ -1921,6 +1989,8 @@ typedef void (*fm_split_fn)(const FmDev, const FmCall, const CUtensorMap);
 // the sweep of the P = 3 kernel alone (same bench line, fm2b only, two rounds; H100 80GB HBM3 SXM, 400 W power limit,
 // SM clock 1530-1680 MHz inside the kernel by clock64 against %globaltimer):
 //   7 + 1 x 2 531 / 530    6 + 1 x 2 507 / 508    4 + 1 x 3 500 / 500    5 + 1 x 3 457 / 459
+// and later (H100 80GB HBM3, 400 W, three rounds of 20 steps, even row split; DESIGN.md §4.1): 7 + 1 x 2 522-524,
+// 6 + 2 x 2 501-504, 15 + 1 x 1 487-488.
 // The P = 1 and P = 2 shapes share the choice and were not timed.
 #ifndef ROWS_FE_WARPS
 #define ROWS_FE_WARPS 7
@@ -2366,6 +2436,7 @@ static int fm_rows_map(const int16_t *d_in, long long lines, CUtensorMap *map)
 // warps' exchange areas share the CTA's dynamic shared memory.  Returns FM_ROWS_NO_ROOM when the margin leaves no room
 // for an item's own rows (a de-emphasis replay longer than the PCM buffers hold): fm_launch takes the fused kernel then.
 #define FM_ROWS_NO_ROOM 1
+
 static int fm_plan_rows(const rxb200_fm *h, long long n, FmCall *k, FmGrid *g)
 {
 	const int P = h->p.downsample_passes;
@@ -2815,3 +2886,18 @@ extern "C" int rxb200_fm_tune(rxb200_fm *h, int segment_len, int deemph_warmup)
 	h->tune_seg = segment_len; h->tune_warm = deemph_warmup;
 	return RXB200_OK;
 }
+
+#ifdef RXB_PROF
+// scratch builds: copy the per-warp phase sums out (clear = 1: and zero them), [PROF_CTAS][32][PROF_SLOTS] words
+extern "C" int rxb200_fm_prof_read(unsigned long long *dst, size_t n, int clear)
+{
+	const size_t all = (size_t)PROF_CTAS * 32 * PROF_SLOTS;
+	if (dst && n) { RXB_CUDA(cudaMemcpyFromSymbol(dst, rxb_prof, (n < all ? n : all) * sizeof(unsigned long long))); }
+	if (clear) {
+		void *p = nullptr;
+		RXB_CUDA(cudaGetSymbolAddress(&p, rxb_prof));
+		RXB_CUDA(cudaMemset(p, 0, all * sizeof(unsigned long long)));
+	}
+	return RXB200_OK;
+}
+#endif

@@ -344,6 +344,7 @@ __device__ __forceinline__ void front_rows(const FmDev &c, const FmCall &k, cons
 	const int r0 = own_lo + warp * per;
 	const int r1 = r0 + per < own_hi ? r0 + per : own_hi;
 	if (r0 >= r1) { return; }
+	PROF_INC(PF_ROWS, r1 - r0);
 	// line walks the rows' tensor-map coordinates; rows_left counts the loop; to_cs counts down to the next chunk start.
 	// Every row this warp copies it also consumes, so the ring is empty between items.
 	constexpr int S = ROWS_STAGES;
@@ -375,7 +376,9 @@ __device__ __forceinline__ void front_rows(const FmDev &c, const FmCall &k, cons
 	int rel = (int)((((long long)r0 * ROW_LEN) >> P) - it.m_lo) + NV * lane;
 	for (int i = 0; rows_left > 0; rows_left--, i++) {
 		const int stage = (int)(ring.seq % S);
+		PROF_CLK(tw);
 		mbar_wait(&ring.bar[stage], (ring.seq / S) & 1u);
+		PROF_ADD(PF_RING, tw);
 		const int next_line = rows_left > S ? line0 + 32 * (i + S) : -1;
 		// a chunk's first row is its own instantiation (warp-uniform branch): the common rows carry no trace of it
 		if (to_cs == 0) { row_body<P, FIR, true>(c, xs, par, lane, ring, stage, next_line, pcm_s, rel); }
@@ -407,13 +410,6 @@ __device__ __forceinline__ void front_rows(const FmDev &c, const FmCall &k, cons
 // the item sits at (r - (own_hi - n_extra)) * row_pcm, and only its own rows are written.  pub[4 w + 2] = 1 says the
 // slot is complete.  (PCM_PAD_ROWS is 0: the shared buffer is linear.)
 #define BAR_PUB 3
-__device__ __forceinline__ int ld_acquire_gpu(const int *p)
-{
-	int v;
-	asm volatile("ld.acquire.gpu.global.b32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-	return v;
-}
-__device__ __forceinline__ void st_release_gpu(int *p, int v) { asm volatile("st.release.gpu.global.b32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
 
 // Front end, after its own rows: the last front-end warp waits for the others' rows (the others only arrive), copies
 // the item's last n_extra rows to its slot and raises the flag.  This never waits for a back end, so no item's margin
@@ -431,8 +427,8 @@ __device__ __forceinline__ void rows_publish(const FmCall &k, const Item &it, in
 	uint4 *dst = reinterpret_cast<uint4 *>(k.margin + ((size_t)work * k.n_extra + (lo - (own_hi - k.n_extra))) * (1 << LG));
 	const int n = ((own_hi - lo) << LG) / 8;
 	for (int i = lane; i < n; i += 32) { dst[i] = src[i]; }
-	__syncwarp();
-	if (lane == 0) { __threadfence(); st_release_gpu(k.pub + 4 * (size_t)work + 2, 1); }
+	__syncwarp();                                          // the lanes' copies are ordered before lane 0's release
+	if (lane == 0) { st_release_gpu(k.pub + 4 * (size_t)work + 2, 1); }
 }
 
 // Back end, before pass 1: the margin rows [buf_lo, own_lo) of this item, from the slots of the older items of the
