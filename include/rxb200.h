@@ -145,6 +145,27 @@ int rxb200_fm_process(rxb200_fm *h, const int16_t *cs16, size_t n_int16, size_t 
 int rxb200_fm_process_device(rxb200_fm *h, const int16_t *d_cs16, size_t n_int16, size_t chunk_int16,
                              int16_t *d_pcm, size_t pcm_stride, size_t *n_pcm, int sync);
 
+/* "One rtlsdr_callback()+full_demod() per channel on a read of n_int16" -- the reference's call
+ * site for each readStream read (src/rtl_fm.c:828-863, :923), so a stream demodulated read by read
+ * gives the reference's bytes whatever lengths the device returns.  Channel c's read is at
+ * cs16 + c*n_int16; pcm, pcm_stride and n_pcm as in rxb200_fm_process.
+ * Constraints (RXB200_EUNSUPPORTED otherwise): n_int16 even, 2 <= n_int16 <= 262144, and with
+ * fifth_order passes n_int16 >= 2*2^P (below that the reference reads before its buffer).  The
+ * read must produce a decimated sample when a per-chunk reduction stage is on, and decimate to a
+ * multiple of post_downsample.  A read rxb200_fm_process(h, cs16, n_int16, n_int16, ...) takes
+ * runs exactly as that call; a read with passes off their granule runs on the read kernel
+ * (kernel_kind 0), where every pass ends where the reference's does: raw mode then returns
+ * n_int16 >> P values, an odd count when L_P = n_int16 >> P is odd.  A refused call leaves the
+ * handle's state untouched.  levels, squelch_hits, last_stats and kernel_ms report the read as
+ * one chunk.  Calls of every process entry point may follow one another on one handle. */
+int rxb200_fm_process_read(rxb200_fm *h, const int16_t *cs16, size_t n_int16, int16_t *pcm,
+                           size_t pcm_stride, size_t *n_pcm);
+
+/* Same with DEVICE pointers, like rxb200_fm_process_device; d_cs16 needs only 4-byte alignment
+ * (a read below 32-byte alignment runs on the any-length kernel of its pass count). */
+int rxb200_fm_process_read_device(rxb200_fm *h, const int16_t *d_cs16, size_t n_int16, int16_t *d_pcm,
+                                  size_t pcm_stride, size_t *n_pcm, int sync);
+
 /* squelch_hits after the last processed chunk, per channel (demod.squelch_hits,
  * src/rtl_fm.c:781-790) so the host thread can keep the hop logic of :928-933. */
 int rxb200_fm_squelch_hits(rxb200_fm *h, int *hits /* n_channels */);

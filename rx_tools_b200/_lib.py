@@ -63,7 +63,8 @@ class PowerPlanC(C.Structure):
 SYMBOLS = [
     "rxb200_last_error", "rxb200_abi_version", "rxb200_device_count",
     "rxb200_fm_derive", "rxb200_fm_create", "rxb200_fm_destroy", "rxb200_fm_reset", "rxb200_fm_max_output",
-    "rxb200_fm_process", "rxb200_fm_process_device", "rxb200_fm_squelch_hits", "rxb200_fm_levels", "rxb200_fm_stream",
+    "rxb200_fm_process", "rxb200_fm_process_device", "rxb200_fm_process_read", "rxb200_fm_process_read_device",
+    "rxb200_fm_squelch_hits", "rxb200_fm_levels", "rxb200_fm_stream",
     "rxb200_fm_last_stats", "rxb200_fm_tune", "rxb200_fm_kernel_ms",
     "rxb200_power_plan_range", "rxb200_window_table", "rxb200_sine_table", "rxb200_power_create",
     "rxb200_power_destroy", "rxb200_power_accumulate", "rxb200_power_accumulate_device", "rxb200_power_read",
@@ -99,6 +100,8 @@ def lib() -> C.CDLL:
     L.rxb200_fm_max_output.argtypes = [C.c_void_p, sz, sz]
     L.rxb200_fm_process.argtypes = [C.c_void_p, C.c_void_p, sz, sz, C.c_void_p, sz, C.POINTER(sz), pint]
     L.rxb200_fm_process_device.argtypes = [C.c_void_p, C.c_void_p, sz, sz, C.c_void_p, sz, C.POINTER(sz), C.c_int]
+    L.rxb200_fm_process_read.argtypes = [C.c_void_p, C.c_void_p, sz, C.c_void_p, sz, C.POINTER(sz)]
+    L.rxb200_fm_process_read_device.argtypes = [C.c_void_p, C.c_void_p, sz, C.c_void_p, sz, C.POINTER(sz), C.c_int]
     L.rxb200_fm_squelch_hits.argtypes = [C.c_void_p, pint]
     L.rxb200_fm_levels.argtypes = [C.c_void_p, pint, C.c_size_t, C.POINTER(C.c_size_t)]
     L.rxb200_fm_stream.restype = C.c_void_p

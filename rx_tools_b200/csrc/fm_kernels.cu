@@ -1369,6 +1369,164 @@ __device__ __forceinline__ void front_run_any(const FmDev &c, const FmCall &k, F
 	}
 }
 
+// ---- one device read per call with fifth_order passes (rxb200_fm_process_read), any even length: the call is one chunk
+// of n complex samples.  Pass l runs over L_l = 2n >> l int16 (src/rtl_fm.c:759-776): ceil(L_l / 2) I and floor(L_l / 2)
+// Q samples, so in-chunk index i is a pair while i < n >> l, and index n >> l is an I sample alone when L_l is odd.  A
+// pass takes only the first samples of the previous pass's outputs; the windows of the passes still advanced over the rest.
+// Only the last 2^P samples of a read can meet such an end (tail_push); the rest run through scalar_push.
+
+// generic_fir on the I lane alone (the Q component's count ends one sample earlier)
+__device__ __forceinline__ int droop9_i(uint32_t (&h)[9], const int (&c)[6], int di)
+{
+	int ai = mul_w(lo16(h[0]) + lo16(h[8]), c[1]);
+	ai = add_w(ai, mul_w(lo16(h[1]) + lo16(h[7]), c[2]));
+	ai = add_w(ai, mul_w(lo16(h[2]) + lo16(h[6]), c[3]));
+	ai = add_w(ai, mul_w(lo16(h[3]) + lo16(h[5]), c[4]));
+	ai = add_w(ai, mul_w(lo16(h[4]), c[5]));
+#pragma unroll
+	for (int j = 0; j < 8; j++) { h[j] = (h[j] & 0xffff0000u) | (h[j + 1] & 0xffffu); }
+	h[8] = (h[8] & 0xffff0000u) | ((uint32_t)di & 0xffffu);
+	return wrap16(ai >> 15);
+}
+
+// The lone I sample left after the passes when L_P is odd (src/rtl_fm.c:770-790, :612-613): the droop FIR and rms() count
+// it, the squelch zeroes it, raw mode emits it, and fm_demod's carry becomes (last pair's Q, lone I).
+template <int P, bool STORE>
+__device__ __forceinline__ void lone_post(const FmDev &c, const FmCall &k, FrontState<P, 2> &s, EmitCtx &e, int di)
+{
+	if (c.fir_on) { di = droop9_i(s.fh, c.fir, di); }
+	if (k.reduce_mode == 1) {
+		if (STORE) { e.red_t += di; e.red_p += (long long)di * di; }
+		return;
+	}
+	if (e.sq_zero) { di = 0; }
+	if (c.mode == RXB200_MODE_FM) { s.pre_i = s.pre_q; s.pre_q = di; }
+	else if (c.mode == RXB200_MODE_RAW && STORE && k.reduce_mode == 0) { e.out[2 * (e.m_lo + e.rel)] = (int16_t)di; }
+}
+
+// scalar_push near the end of a read: the sample enters pass L (or, L == P, the stages after the passes) as a pair, as an
+// I sample alone (q false), or not at all
+template <int L, int P, bool STORE>
+__device__ __forceinline__ void tail_push(const FmDev &c, const FmCall &k, FrontState<P, 2> &s, EmitCtx &e, int xi, int xq,
+                                          unsigned idx, bool q, unsigned n)
+{
+	if constexpr (L > 0) {
+		if (idx >= (n >> L)) {
+			if (idx > (n >> L) || ((n >> (L - 1)) & 1u) == 0u) { return; }
+			q = false;
+		}
+	}
+	if constexpr (L == P) {
+		if (q) { post_decim<P, 2, STORE>(c, k, s, e, xi, xq); } else { lone_post<P, STORE>(c, k, s, e, xi); }
+	} else {
+		if (idx & 1u) { s.pi[L] = xi; if (q) { s.pq[L] = xq; } return; }
+		if (idx == 0u) {
+#pragma unroll
+			for (int j = 0; j < 5; j++) { s.wi[L][j] = s.wi[L][j + 1]; if (q) { s.wq[L][j] = s.wq[L][j + 1]; } }
+		} else {
+#pragma unroll
+			for (int j = 0; j < 4; j++) { s.wi[L][j] = s.wi[L][j + 2]; if (q) { s.wq[L][j] = s.wq[L][j + 2]; } }
+			s.wi[L][4] = s.pi[L]; if (q) { s.wq[L][4] = s.pq[L]; }
+		}
+		s.wi[L][5] = xi; if (q) { s.wq[L][5] = xq; }
+		int yi = wrap16((s.wi[L][0] + (s.wi[L][1] + s.wi[L][4]) * 5 + (s.wi[L][2] + s.wi[L][3]) * 10 + s.wi[L][5]) >> 4);
+		int yq = wrap16((s.wq[L][0] + (s.wq[L][1] + s.wq[L][4]) * 5 + (s.wq[L][2] + s.wq[L][3]) * 10 + s.wq[L][5]) >> 4);
+		tail_push<L + 1, P, STORE>(c, k, s, e, yi, yq, idx >> 1, q, n);
+	}
+}
+
+// front_run for a read with passes: one 32-bit load per complex sample (4-byte alignment, nothing read past t_end); u is
+// the in-chunk index of sample t
+template <int P, bool STORE>
+__device__ __forceinline__ void front_run_read(const FmDev &c, const FmCall &k, FrontState<P, 2> &s, EmitCtx &e,
+                                               const uint32_t *__restrict__ in, int t, int t_end, unsigned &u, int ch)
+{
+	const bool rot = Spec<2>::rotate(c);
+	const unsigned n = (unsigned)k.n;
+	const unsigned tail = (n >> P) << P;              // from here on a sample may meet the end of a pass's count
+	const int t_main = t + (int)(u >= tail ? 0u : min(tail - u, (unsigned)(t_end - t)));
+	for (; t < t_main; t += 8) {
+		const int nb = t_main - t;
+		uint32_t v[8];
+#pragma unroll
+		for (int j = 0; j < 8; j++) { v[j] = j < nb ? __ldg(in + t + j) : 0u; }
+#pragma unroll
+		for (int j = 0; j < 8; j++) {
+			if (j < nb) {
+				if (u == 0u) {
+#pragma unroll 1
+					for (int z = 0; z < k.one; z++) { front_chunk_start<P, 2, STORE>(c, k, s, e, ch); }
+				}
+				int xi, xq, oi, oq;
+				scale_rot(v[j], (int)(u & 3u), rot, xi, xq, e.rdc_i, e.rdc_q);
+				if (scalar_push<0, P, 2>(s, xi, xq, u, oi, oq)) { post_decim<P, 2, STORE>(c, k, s, e, oi, oq); }
+				u++;
+			}
+		}
+	}
+	t = t_main > t_end ? t_end : t_main;
+#pragma unroll 1
+	for (; t < t_end; t++, u++) {                     // u >= tail > 0: no chunk starts here
+		int xi, xq;
+		scale_rot(__ldg(in + t), (int)(u & 3u), rot, xi, xq, e.rdc_i, e.rdc_q);
+		tail_push<0, P, STORE>(c, k, s, e, xi, xq, u, true, n);
+	}
+}
+
+// The read kernel keeps every pass scalar (FrontState<P, 2>); the carry keeps the handle's layout (fm_state_words), so
+// that calls of every entry point can follow one another: c.PL packed levels, lanes biased by 128 << l, holding the
+// pass's last six inputs -- the window a..e of the next chunk's first output, then the sample an even count left
+// pending -- and the scalar levels after them.
+template <int P>
+__device__ __forceinline__ void read_load(const FmDev &c, FrontState<P, 2> &s, const uint32_t *g)
+{
+	s.box_i = (int)g[ST_BOX_I]; s.box_q = (int)g[ST_BOX_Q]; s.box_n = (int)g[ST_BOX_N];
+	s.pre_i = (int)g[ST_PRE_I]; s.pre_q = (int)g[ST_PRE_Q];
+	const int PL = c.PL;
+#pragma unroll
+	for (int l = 0; l < P; l++) {
+		if (l < PL) {
+			const int b = 128 << l;
+			s.wi[l][0] = 0; s.wq[l][0] = 0;       // a: shifted out before the next output
+#pragma unroll
+			for (int j = 0; j < 5; j++) { const uint32_t w = g[ST_HDR + 6 * l + j]; s.wi[l][j + 1] = (int)(w & 0xffffu) - b; s.wq[l][j + 1] = (int)(w >> 16) - b; }
+			const uint32_t w = g[ST_HDR + 6 * l + 5];
+			s.pi[l] = (int)(w & 0xffffu) - b; s.pq[l] = (int)(w >> 16) - b;
+		} else {
+			const uint32_t *gl = g + ST_HDR + 6 * PL + 7 * (l - PL);
+#pragma unroll
+			for (int j = 0; j < 6; j++) { s.wi[l][j] = lo16(gl[j]); s.wq[l][j] = hi16(gl[j]); }
+			s.pi[l] = lo16(gl[6]); s.pq[l] = hi16(gl[6]);
+		}
+	}
+#pragma unroll
+	for (int j = 0; j < 9; j++) { s.fh[j] = g[ST_HDR + 6 * PL + 7 * (P - PL) + j]; }
+}
+
+template <int P>
+__device__ __forceinline__ void read_store(const FmDev &c, const FrontState<P, 2> &s, uint32_t *g)
+{
+	g[ST_BOX_I] = (uint32_t)s.box_i; g[ST_BOX_Q] = (uint32_t)s.box_q; g[ST_BOX_N] = (uint32_t)s.box_n;
+	g[ST_PRE_I] = (uint32_t)s.pre_i; g[ST_PRE_Q] = (uint32_t)s.pre_q;
+	const int PL = c.PL;
+#pragma unroll
+	for (int l = 0; l < P; l++) {
+		if (l < PL) {
+			const int b = 128 << l;
+#pragma unroll
+			for (int j = 0; j < 5; j++) { g[ST_HDR + 6 * l + j] = pack2(s.wi[l][j + 1] + b, s.wq[l][j + 1] + b); }
+			g[ST_HDR + 6 * l + 5] = pack2(s.pi[l] + b, s.pq[l] + b);
+		} else {
+			uint32_t *gl = g + ST_HDR + 6 * PL + 7 * (l - PL);
+#pragma unroll
+			for (int j = 0; j < 6; j++) { gl[j] = pack2(s.wi[l][j], s.wq[l][j]); }
+			gl[6] = pack2(s.pi[l], s.pq[l]);
+		}
+	}
+#pragma unroll
+	for (int j = 0; j < 9; j++) { g[ST_HDR + 6 * PL + 7 * (P - PL) + j] = s.fh[j]; }
+}
+
 // geometry of one work item (one CTA stretch of one channel)
 struct Item {
 	int ch, b;
@@ -1395,7 +1553,8 @@ __device__ __forceinline__ Item make_item(const FmDev &c, const FmCall &k, int w
 	return it;
 }
 
-// ---- front end of one work item: one segment per thread (tid 0..T-1).  ANY: the any-length front end (front_run_any)
+// ---- front end of one work item: one segment per thread (tid 0..T-1).  ANY: the any-length front end (front_run_any;
+// front_run_read with passes)
 template <int P, int SPEC, bool ANY>
 __device__ __forceinline__ void front_item(const FmDev &c, const FmCall &k, const Item &it, int tid, int16_t *pcm_s)
 {
@@ -1408,7 +1567,10 @@ __device__ __forceinline__ void front_item(const FmDev &c, const FmCall &k, cons
 	const long long end = start + k.Sf < k.n ? start + k.Sf : k.n;
 	long long t0 = start - k.halo;
 	FrontState<P, SPEC> s;
-	if (t0 <= 0) { t0 = 0; front_load<P, SPEC>(s, carry); }
+	if (t0 <= 0) {
+		t0 = 0;
+		if constexpr (ANY && P > 0) { read_load<P>(c, s, carry); } else { front_load<P, SPEC>(s, carry); }
+	}
 	else {
 		front_zero<P, SPEC>(s);
 		if (P == 0) { s.box_n = (int)((t0 + it.box_n0) % c.D); }
@@ -1430,8 +1592,13 @@ __device__ __forceinline__ void front_item(const FmDev &c, const FmCall &k, cons
 	}
 	// offsets relative to t0 fit 32 bits (a segment plus its halo)
 	const int16_t *__restrict__ in = k.in + 2 * ((size_t)it.ch * (size_t)k.n + (size_t)t0);
-	if constexpr (ANY) {
-		static_assert(P == 0 && (SPEC == 0 || SPEC == 2), "the any-length front end is the generic boxcar one");
+	if constexpr (ANY && P > 0) {
+		static_assert(SPEC == 2, "the read front end keeps every pass scalar");
+		const uint32_t *in_w = reinterpret_cast<const uint32_t *>(in);
+		front_run_read<P, false>(c, k, s, e, in_w, 0, (int)(start - t0), u, it.ch);
+		front_run_read<P, true>(c, k, s, e, in_w, (int)(start - t0), (int)(end - t0), u, it.ch);
+	} else if constexpr (ANY) {
+		static_assert(SPEC == 0 || SPEC == 2, "the any-length front end is the generic boxcar one");
 		const uint32_t *in_w = reinterpret_cast<const uint32_t *>(in);
 		front_run_any<SPEC, false>(c, k, s, e, in_w, 0, (int)(start - t0), u, it.ch);
 		front_run_any<SPEC, true>(c, k, s, e, in_w, (int)(start - t0), (int)(end - t0), u, it.ch);
@@ -1443,7 +1610,8 @@ __device__ __forceinline__ void front_item(const FmDev &c, const FmCall &k, cons
 	if (SPEC == 2 && k.reduce_mode == 1) { chunk_enter<true>(c, k, e, it.ch, e.chunk_idx); }   // flush the last chunk's sums
 	if (end == k.n && (SPEC != 2 || k.reduce_mode == 0)) {
 		// this thread saw the end of the stream: its registers are the next call's carry
-		front_store<P, SPEC>(s, k.carry_out + (size_t)it.ch * k.state_words);
+		if constexpr (ANY && P > 0) { read_store<P>(c, s, k.carry_out + (size_t)it.ch * k.state_words); }
+		else { front_store<P, SPEC>(s, k.carry_out + (size_t)it.ch * k.state_words); }
 	}
 }
 
@@ -1689,7 +1857,8 @@ __device__ __forceinline__ void back_item(const FmDev &c, const FmCall &k, const
 // `be_lanes/32` warps run the back end out of the shared PCM buffer.  Work items are handed out by an
 // atomic ticket, oldest first (the cross-item look-back only ever waits for an older ticket).
 // The occupancy target is stated for 256 threads and scales with the width (same threads per SM).
-// ANY: the any-length front end (front_run_any), for the calls fm_any_length picks.
+// ANY: the any-length front end (front_run_any), for the calls fm_any_length picks; with passes (SPEC 2) the read
+// kernel (front_run_read), for the reads fm_read_any picks.
 template <int P, int SPEC, int T, bool ANY = false>
 __global__ void __launch_bounds__(T, (FM_MAX_THREADS / T) * (SPEC == 2 ? (P <= 3 ? 2 : 1) : (P <= 3 ? RXB_OCC : (P <= 6 ? 2 : 1)))) fm_fused_kernel(const FmDev c, const FmCall k)
 {
@@ -1895,9 +2064,10 @@ __global__ void fm_rdc_recur_kernel(const long long *sums, const int *chunk_len,
 	carry_out[(size_t)ch * state_words + ST_RDC_Q] = (uint32_t)aq;
 }
 
-// rms() + squelch decision (src/rtl_fm.c:739-757, :781-790); dec_len = decimated complex samples of the chunk
-__global__ void fm_squelch_kernel(const long long *sums, const int *dec_len, int n_chunks, int n_ch, int level,
-                                  const uint32_t *carry_in, uint32_t *carry_out, int state_words, int *sqz, int *levels)
+// rms() + squelch decision (src/rtl_fm.c:739-757, :781-790); lp_len = LEN_MUL * len[ci] int16
+template <int LEN_MUL>
+__device__ __forceinline__ void squelch_recur(const long long *sums, const int *len_tab, int n_chunks, int n_ch, int level,
+                                              const uint32_t *carry_in, uint32_t *carry_out, int state_words, int *sqz, int *levels)
 {
 	const int ch = blockIdx.x * blockDim.x + threadIdx.x;
 	if (ch >= n_ch) { return; }
@@ -1905,7 +2075,7 @@ __global__ void fm_squelch_kernel(const long long *sums, const int *dec_len, int
 	for (int ci = 0; ci < n_chunks; ci++) {
 		const long long *sm = sums + 2 * ((size_t)ch * n_chunks + ci);
 		const long long t = sm[0], p = sm[1];
-		const int len = 2 * dec_len[ci];                         // lp_len counts int16
+		const int len = LEN_MUL * len_tab[ci];                   // lp_len counts int16
 		// dc = (double)(t*step)/len; err = t*2*dc - dc*dc*len; (int)sqrt((p-err)/len) -- same order, no FMA
 		const double dc = __ddiv_rn((double)t, (double)len);
 		const double err = __dsub_rn(__dmul_rn((double)(t * 2), dc), __dmul_rn(__dmul_rn(dc, dc), (double)len));
@@ -1918,6 +2088,20 @@ __global__ void fm_squelch_kernel(const long long *sums, const int *dec_len, int
 		}
 	}
 	carry_out[(size_t)ch * state_words + ST_SQ_HITS] = (uint32_t)hits;
+}
+
+// dec_len = decimated complex samples of the chunk: lp_len is even
+__global__ void fm_squelch_kernel(const long long *sums, const int *dec_len, int n_chunks, int n_ch, int level,
+                                  const uint32_t *carry_in, uint32_t *carry_out, int state_words, int *sqz, int *levels)
+{
+	squelch_recur<2>(sums, dec_len, n_chunks, n_ch, level, carry_in, carry_out, state_words, sqz, levels);
+}
+
+// lp_len int16 of the chunk: a read with passes leaves an odd count when L_P is odd (rxb200_fm_process_read)
+__global__ void fm_squelch_lp_kernel(const long long *sums, const int *lp_len, int n_chunks, int n_ch, int level,
+                                     const uint32_t *carry_in, uint32_t *carry_out, int state_words, int *sqz, int *levels)
+{
+	squelch_recur<1>(sums, lp_len, n_chunks, n_ch, level, carry_in, carry_out, state_words, sqz, levels);
 }
 
 // dc_block_audio_filter recurrence (src/rtl_fm.c:691-696); pcm_len = result_len of the chunk before low_pass_real
@@ -2043,6 +2227,30 @@ static fm_kernel_fn pick_any_kernel(int P, int spec)
 #endif
 }
 
+// The read kernel (rxb200_fm_process_read with passes, a read off their granule): SPEC 2's all-scalar passes and stage
+// bookkeeping serve every shape -- with no reduction stage on, that bookkeeping stays idle
+static fm_kernel_fn pick_read_kernel(int P)
+{
+#ifdef RXB_QUICK
+	(void)P;
+	return nullptr;
+#else
+	switch (P) {
+	case 1: return fm_fused_kernel<1, 2, FM_ANY_THREADS, true>;
+	case 2: return fm_fused_kernel<2, 2, FM_ANY_THREADS, true>;
+	case 3: return fm_fused_kernel<3, 2, FM_ANY_THREADS, true>;
+	case 4: return fm_fused_kernel<4, 2, FM_ANY_THREADS, true>;
+	case 5: return fm_fused_kernel<5, 2, FM_ANY_THREADS, true>;
+	case 6: return fm_fused_kernel<6, 2, FM_ANY_THREADS, true>;
+	case 7: return fm_fused_kernel<7, 2, FM_ANY_THREADS, true>;
+	case 8: return fm_fused_kernel<8, 2, FM_ANY_THREADS, true>;
+	case 9: return fm_fused_kernel<9, 2, FM_ANY_THREADS, true>;
+	case 10: return fm_fused_kernel<10, 2, FM_ANY_THREADS, true>;
+	default: return nullptr;
+	}
+#endif
+}
+
 }  // namespace rxb
 
 // ================================================================================ host side
@@ -2088,6 +2296,7 @@ struct rxb200_fm {
 	fm_kernel_fn kern_front = nullptr;   // stream path: front end alone (SPEC 4), PCM to global memory; fm_back_kernel follows
 	int16_t *d_pcm = nullptr; size_t d_pcm_cap = 0;       // its PCM scratch, int16 elements
 	fm_kernel_fn kern_any = nullptr;     // any-length calls (P = 0, chunk or call not a multiple of 8 complex), FM_ANY_THREADS wide
+	fm_kernel_fn kern_read = nullptr;    // rxb200_fm_process_read with passes (P >= 1) off their granule, FM_ANY_THREADS wide
 	size_t stream_min = 0; int stream_piece = 0, stream_win = 0, stream_t = 0;
 	int threads = 0;               // CTA width of kern
 	int wide = 0;                  // all-scalar fifth_order passes (raw DC block on)
@@ -2204,6 +2413,7 @@ extern "C" int rxb200_fm_create(const rxb200_fm_params *params, int device, int 
 		const int fir_on = (params->downsample_passes > 0 && params->comp_fir_size == 9) ? 1 : 0;
 		h->kern_rows = spec == 1 ? pick_rows_kernel(params->downsample_passes, fir_on) : nullptr;
 		h->kern_any = pick_any_kernel(params->downsample_passes, spec);
+		h->kern_read = pick_read_kernel(params->downsample_passes);
 		// stream path (front kernel + back kernel): the wbfm shape without decimating passes, de-emphasis on
 #ifndef RXB_QUICK
 		h->kern_front = (spec == 1 && params->downsample_passes == 0 && params->deemph) ? pick_kernel(0, 4, h->threads) : nullptr;
@@ -2305,10 +2515,15 @@ static size_t fm_count_outputs(rxb200_fm *h, size_t n_int16, size_t chunk_int16,
 		else { dec = (box_n + L) / p.downsample; box_n = (box_n + L) % p.downsample; }
 		// low_pass_simple needs a whole number of groups per chunk (otherwise the reference reads stale data)
 		if (dec % h->dev.post_ds != 0) { return (size_t)-1; }
-		if (lens) { lens[c] = (int)L; lens[n_chunks + c] = (int)dec; lens[2 * n_chunks + c] = (int)(dec / h->dev.post_ds); }
+		// lowpassed int16 after the passes: odd when a read's L_P is (rxb200_fm_process_read), else 2 * dec
+		const long long lp = p.downsample_passes ? (long long)(len16 >> p.downsample_passes) : 2 * dec;
+		if (lens) {
+			lens[c] = (int)L; lens[n_chunks + c] = (int)dec; lens[2 * n_chunks + c] = (int)(dec / h->dev.post_ds);
+			lens[3 * n_chunks + c] = (int)lp;
+		}
 		dec /= h->dev.post_ds;
 		long long res;
-		if (p.mode == RXB200_MODE_RAW) { res = 2 * dec; }
+		if (p.mode == RXB200_MODE_RAW) { res = lp; }
 		else if (p.rate_out2 > 0) {
 			long long tot = phase + dec * (long long)p.rate_out2;
 			res = tot / p.rate_out; phase = tot % p.rate_out;
@@ -2635,7 +2850,8 @@ static int fm_plan_back(const rxb200_fm *h, long long n, FmBackPlan *b)
 // per-chunk scalars: sizes (closed form), accumulators, then one recurrence per stage in the reference's order: raw DC
 // block -> squelch (sees the DC-blocked data, its sums from pass(1)) -> audio DC block (sums from pass(2))
 template <typename Pass>
-static int fm_prepasses(rxb200_fm *h, FmCall &k, size_t n_int16, size_t chunk_int16, Pass pass, int *launches)
+// read: the call runs on the read kernel, whose rms() divides by an lp_len that may be odd
+static int fm_prepasses(rxb200_fm *h, FmCall &k, size_t n_int16, size_t chunk_int16, bool read, Pass pass, int *launches)
 {
 	const FmDev &dv = h->dev;
 	const int n_chunks = k.n_chunks;
@@ -2645,9 +2861,9 @@ static int fm_prepasses(rxb200_fm *h, FmCall &k, size_t n_int16, size_t chunk_in
 	RXB_CUDA(fm_reserve(h->d_sqz, h->sqz_cap, cells));
 	RXB_CUDA(fm_reserve(h->d_adc, h->adc_cap, cells));
 	RXB_CUDA(fm_reserve(h->d_levels, h->levels_cap, cells));
-	RXB_CUDA(fm_reserve(h->d_lens, h->lens_cap, (size_t)n_chunks * 3));
+	RXB_CUDA(fm_reserve(h->d_lens, h->lens_cap, (size_t)n_chunks * 4));
 	RXB_CUDA(cudaStreamSynchronize(h->stream));   // the previous call may still be reading the host vector
-	h->h_lens.assign((size_t)n_chunks * 3, 0);     // [0]: complex per chunk, [1]: decimated per chunk, [2]: PCM per chunk
+	h->h_lens.assign((size_t)n_chunks * 4, 0);     // [0]: complex per chunk, [1]: decimated per chunk, [2]: PCM per chunk, [3]: lp_len
 	fm_count_outputs(h, n_int16, chunk_int16, nullptr, h->h_lens.data(), false);   // -o was checked before the launch
 	for (int ci = 0; ci < n_chunks; ci++) {
 		if (h->h_lens[(size_t)n_chunks + ci] < 1) { set_error("a chunk produces no decimated sample"); return RXB200_EUNSUPPORTED; }
@@ -2670,8 +2886,13 @@ static int fm_prepasses(rxb200_fm *h, FmCall &k, size_t n_int16, size_t chunk_in
 		k.sums = h->d_sums;
 		const int rc = pass(1);
 		if (rc != RXB200_OK) { return rc; }
-		fm_squelch_kernel<<<cb, 64, 0, h->stream>>>(h->d_sums, h->d_lens + n_chunks, n_chunks, h->n_channels, dv.squelch, k.carry_in,
-		                                             k.carry_out, h->state_words, h->d_sqz, dv.levels ? h->d_levels : nullptr);
+		if (read) {
+			fm_squelch_lp_kernel<<<cb, 64, 0, h->stream>>>(h->d_sums, h->d_lens + 3 * (size_t)n_chunks, n_chunks, h->n_channels, dv.squelch,
+			                                                k.carry_in, k.carry_out, h->state_words, h->d_sqz, dv.levels ? h->d_levels : nullptr);
+		} else {
+			fm_squelch_kernel<<<cb, 64, 0, h->stream>>>(h->d_sums, h->d_lens + n_chunks, n_chunks, h->n_channels, dv.squelch, k.carry_in,
+			                                             k.carry_out, h->state_words, h->d_sqz, dv.levels ? h->d_levels : nullptr);
+		}
 		RXB_CUDA(cudaGetLastError());
 		(*launches)++;
 		k.sqz = dv.squelch ? h->d_sqz : nullptr;
@@ -2693,12 +2914,14 @@ static int fm_prepasses(rxb200_fm *h, FmCall &k, size_t n_int16, size_t chunk_in
 }
 
 // Plans and launches one call -- the split kernel where the shape allows it, else the fused kernel, or on the stream
-// path the front and back kernels -- then advances the host mirrors of the closed-form counters.
-static int fm_launch(rxb200_fm *h, const int16_t *d_in, size_t n_int16, size_t chunk_int16, int16_t *d_out, size_t out_stride)
+// path the front and back kernels -- then advances the host mirrors of the closed-form counters.  any: the call runs on
+// the any-length kernel of its pass count instead (kern_any without passes, kern_read with them).
+static int fm_launch(rxb200_fm *h, const int16_t *d_in, size_t n_int16, size_t chunk_int16, int16_t *d_out, size_t out_stride,
+                     bool any)
 {
 	const FmDev &dv = h->dev;
 	const long long n = (long long)(n_int16 / 2);
-	bool rows = h->kern_rows && (chunk_int16 / 2) % ROW_LEN == 0 && n % ROW_LEN == 0 && n >= 16LL * ROW_LEN;
+	bool rows = !any && h->kern_rows && (chunk_int16 / 2) % ROW_LEN == 0 && n % ROW_LEN == 0 && n >= 16LL * ROW_LEN;
 	// Stream path: the front end of the whole call stores its PCM to global memory (SPEC 4 through the direct-output
 	// path), fm_back_kernel then runs the serial stages with pieces as long as the call allows.  In the fused kernel a
 	// piece is a lane's share of one shared-memory buffer -- at the capture rate (fm2a) 870 samples behind a 2960-step
@@ -2707,9 +2930,8 @@ static int fm_launch(rxb200_fm *h, const int16_t *d_in, size_t n_int16, size_t c
 	const long long Dpcm = (long long)dv.D * dv.post_ds;
 	const size_t stream_min = h->stream_min != (size_t)-1 ? h->stream_min : (size_t)(32 * fm_replay(h, false) * Dpcm / h->n_channels);
 	// an any-length call runs on its own kernel, front and back end fused, whatever the shape would take otherwise
-	const bool any = fm_any_length(h, n_int16, chunk_int16);
 	const bool stream = !any && h->kern_front != nullptr && dv.deemph && (size_t)n >= stream_min;
-	const fm_kernel_fn kern = any ? h->kern_any : (stream ? h->kern_front : h->kern);
+	const fm_kernel_fn kern = any ? (dv.P ? h->kern_read : h->kern_any) : (stream ? h->kern_front : h->kern);
 	FmCall k = {};
 	FmGrid g;
 	CUtensorMap in_map;
@@ -2752,7 +2974,7 @@ static int fm_launch(rxb200_fm *h, const int16_t *d_in, size_t n_int16, size_t c
 		return RXB200_OK;
 	};
 	if (dv.rdc_on || dv.squelch || dv.adc_on || dv.levels) {
-		rc = fm_prepasses(h, k, n_int16, chunk_int16, pass, &launches);
+		rc = fm_prepasses(h, k, n_int16, chunk_int16, any && dv.P > 0, pass, &launches);
 		if (rc != RXB200_OK) { return rc; }
 	}
 	rc = pass(0);
@@ -2779,11 +3001,35 @@ static int fm_launch(rxb200_fm *h, const int16_t *d_in, size_t n_int16, size_t c
 }
 
 // what both process calls check before they launch, and the call's output count (*total PCM samples per channel)
+// rxb200_fm_process_read's shapes: one read of any even length, at least 2^P complex samples with passes (fm_demod
+// reads lowpassed[-1] below that)
+static int fm_check_read(const rxb200_fm *h, size_t n_int16)
+{
+	const size_t lo = h->p.downsample_passes ? ((size_t)2 << h->p.downsample_passes) : 2;
+	if (n_int16 < lo || n_int16 > 262144 || n_int16 % 2 != 0) {
+		set_error("a read of n_int16=%zu must be even, at least %zu and at most 262144", n_int16, lo);
+		return RXB200_EUNSUPPORTED;
+	}
+	return RXB200_OK;
+}
+
+// Where a read runs: on whatever rxb200_fm_process(h, x, n, n, ...) runs when that call takes it and the input is 32-byte
+// aligned, else on the any-length kernel of its pass count (a read with passes off their granule, or a device read at
+// 4-byte alignment)
+static bool fm_read_any(const rxb200_fm *h, size_t n_int16, bool aligned32)
+{
+	const size_t p16 = (size_t)2 << h->p.downsample_passes;
+	const size_t g16 = p16 > 16 ? p16 : 16;
+	return !aligned32 || fm_any_length(h, n_int16, n_int16) || (h->p.downsample_passes > 0 && n_int16 % g16 != 0);
+}
+
+// what every process call checks before it launches, and the call's output count (*total PCM samples per channel);
+// read: a call of rxb200_fm_process_read (one chunk, its own shape rule)
 static int fm_prologue(rxb200_fm *h, const void *in, const void *out, size_t n_int16, size_t chunk_int16, size_t pcm_stride,
-                       int *chunk_result_len, size_t *total, size_t *n_pcm)
+                       int *chunk_result_len, size_t *total, size_t *n_pcm, bool read = false)
 {
 	if (!h || !in || !out) { set_error("null argument"); return RXB200_EINVAL; }
-	const int rc = fm_check_shape(h, n_int16, chunk_int16);
+	const int rc = read ? fm_check_read(h, n_int16) : fm_check_shape(h, n_int16, chunk_int16);
 	if (rc != RXB200_OK) { return rc; }
 	RXB_CUDA(cudaSetDevice(h->device));
 	if (n_int16 == 0) { h->level_chunks = 0; if (n_pcm) { *n_pcm = 0; } }
@@ -2793,19 +3039,22 @@ static int fm_prologue(rxb200_fm *h, const void *in, const void *out, size_t n_i
 	return RXB200_OK;
 }
 
-extern "C" int rxb200_fm_process_device(rxb200_fm *h, const int16_t *d_cs16, size_t n_int16, size_t chunk_int16,
-                                        int16_t *d_pcm, size_t pcm_stride, size_t *n_pcm, int sync)
+static int fm_process_device(rxb200_fm *h, const int16_t *d_cs16, size_t n_int16, size_t chunk_int16, int16_t *d_pcm,
+                             size_t pcm_stride, size_t *n_pcm, int sync, bool read)
 {
-	// null arguments are reported first, by fm_prologue; the any-length kernel reads one complex sample at a time
-	const uintptr_t align = (h && fm_any_length(h, n_int16, chunk_int16)) ? 4u : 32u;
+	// null arguments are reported first, by fm_prologue; the any-length kernels read one complex sample at a time
+	const bool aligned32 = ((uintptr_t)d_cs16 & 31u) == 0;
+	const bool any = h && (read ? fm_read_any(h, n_int16, aligned32) : fm_any_length(h, n_int16, chunk_int16));
+	const uintptr_t align = any ? 4u : 32u;
 	if (h && d_cs16 && d_pcm && ((uintptr_t)d_cs16 & (align - 1u)) != 0) {
 		set_error("d_cs16 must be %d-byte aligned", (int)align);
 		return RXB200_EINVAL;
 	}
 	size_t total = 0;
-	int rc = fm_prologue(h, d_cs16, d_pcm, n_int16, chunk_int16, pcm_stride, nullptr, &total, n_pcm);
+	int rc = fm_prologue(h, d_cs16, d_pcm, n_int16, chunk_int16, pcm_stride, nullptr, &total, n_pcm, read);
 	if (rc != RXB200_OK || n_int16 == 0) { return rc; }
-	rc = fm_launch(h, d_cs16, n_int16, chunk_int16, d_pcm, pcm_stride);
+	if (any && !(h->dev.P ? h->kern_read : h->kern_any)) { set_error("no any-length kernel for downsample_passes %d in this build", h->dev.P); return RXB200_EUNSUPPORTED; }
+	rc = fm_launch(h, d_cs16, n_int16, chunk_int16, d_pcm, pcm_stride, any);
 	if (rc != RXB200_OK) { return rc; }
 	if (n_pcm) { *n_pcm = total; }
 	if (sync) {
@@ -2815,18 +3064,20 @@ extern "C" int rxb200_fm_process_device(rxb200_fm *h, const int16_t *d_cs16, siz
 	return RXB200_OK;
 }
 
-extern "C" int rxb200_fm_process(rxb200_fm *h, const int16_t *cs16, size_t n_int16, size_t chunk_int16,
-                                 int16_t *pcm, size_t pcm_stride, size_t *n_pcm, int *chunk_result_len)
+static int fm_process_host(rxb200_fm *h, const int16_t *cs16, size_t n_int16, size_t chunk_int16, int16_t *pcm,
+                           size_t pcm_stride, size_t *n_pcm, int *chunk_result_len, bool read)
 {
 	size_t total = 0;
-	int rc = fm_prologue(h, cs16, pcm, n_int16, chunk_int16, pcm_stride, chunk_result_len, &total, n_pcm);
+	int rc = fm_prologue(h, cs16, pcm, n_int16, chunk_int16, pcm_stride, chunk_result_len, &total, n_pcm, read);
 	if (rc != RXB200_OK || n_int16 == 0) { return rc; }
+	const bool any = read ? fm_read_any(h, n_int16, true) : fm_any_length(h, n_int16, chunk_int16);
+	if (any && !(h->dev.P ? h->kern_read : h->kern_any)) { set_error("no any-length kernel for downsample_passes %d in this build", h->dev.P); return RXB200_EUNSUPPORTED; }
 	const size_t in_elems = n_int16 * (size_t)h->n_channels;
 	const size_t out_elems = (total + 8) * (size_t)h->n_channels;
 	RXB_CUDA(fm_reserve(h->d_in, h->d_in_cap, in_elems));
 	RXB_CUDA(fm_reserve(h->d_out, h->d_out_cap, out_elems));
 	RXB_CUDA(cudaMemcpyAsync(h->d_in, cs16, in_elems * sizeof(int16_t), cudaMemcpyHostToDevice, h->stream));
-	rc = fm_launch(h, h->d_in, n_int16, chunk_int16, h->d_out, total + 8);
+	rc = fm_launch(h, h->d_in, n_int16, chunk_int16, h->d_out, total + 8, any);
 	if (rc != RXB200_OK) { return rc; }
 	if (pcm_stride == total + 8 || h->n_channels == 1) {
 		RXB_CUDA(cudaMemcpyAsync(pcm, h->d_out, (h->n_channels == 1 ? total : out_elems) * sizeof(int16_t),
@@ -2839,6 +3090,30 @@ extern "C" int rxb200_fm_process(rxb200_fm *h, const int16_t *cs16, size_t n_int
 	RXB_CUDA(cudaStreamSynchronize(h->stream));
 	if (n_pcm) { *n_pcm = total; }
 	return RXB200_OK;
+}
+
+extern "C" int rxb200_fm_process_device(rxb200_fm *h, const int16_t *d_cs16, size_t n_int16, size_t chunk_int16,
+                                        int16_t *d_pcm, size_t pcm_stride, size_t *n_pcm, int sync)
+{
+	return fm_process_device(h, d_cs16, n_int16, chunk_int16, d_pcm, pcm_stride, n_pcm, sync, false);
+}
+
+extern "C" int rxb200_fm_process(rxb200_fm *h, const int16_t *cs16, size_t n_int16, size_t chunk_int16,
+                                 int16_t *pcm, size_t pcm_stride, size_t *n_pcm, int *chunk_result_len)
+{
+	return fm_process_host(h, cs16, n_int16, chunk_int16, pcm, pcm_stride, n_pcm, chunk_result_len, false);
+}
+
+extern "C" int rxb200_fm_process_read(rxb200_fm *h, const int16_t *cs16, size_t n_int16, int16_t *pcm, size_t pcm_stride,
+                                      size_t *n_pcm)
+{
+	return fm_process_host(h, cs16, n_int16, n_int16, pcm, pcm_stride, n_pcm, nullptr, true);
+}
+
+extern "C" int rxb200_fm_process_read_device(rxb200_fm *h, const int16_t *d_cs16, size_t n_int16, int16_t *d_pcm,
+                                             size_t pcm_stride, size_t *n_pcm, int sync)
+{
+	return fm_process_device(h, d_cs16, n_int16, n_int16, d_pcm, pcm_stride, n_pcm, sync, true);
 }
 
 extern "C" int rxb200_fm_squelch_hits(rxb200_fm *h, int *hits)

@@ -126,6 +126,30 @@ class FmDemod:
                                                        C.byref(n_pcm), 1 if sync else 0))
         return int(n_pcm.value)
 
+    def process_read(self, cs16: np.ndarray) -> np.ndarray:
+        """One device read per channel: ``rtlsdr_callback`` + ``full_demod`` once on the whole of it, whatever its
+        length (``rxb200_fm_process_read``).  cs16: int16[n_int16] or int16[n_channels][n_int16]."""
+        x = np.ascontiguousarray(cs16, dtype=np.int16)
+        single = x.ndim == 1
+        x2 = x.reshape(1, -1) if single else x
+        assert x2.shape[0] == self.n_channels, (x2.shape, self.n_channels)
+        n_int16 = x2.shape[1]
+        cap = self.max_output(n_int16, max(n_int16, 1)) + 8
+        out = np.empty((self.n_channels, cap), dtype=np.int16)
+        n_pcm = C.c_size_t(0)
+        _lib.check(_lib.lib().rxb200_fm_process_read(self._h, x2.ctypes.data, n_int16, out.ctypes.data, cap,
+                                                     C.byref(n_pcm)))
+        res = out[:, :n_pcm.value].copy()
+        return res[0] if single else res
+
+    def process_read_device(self, d_in_ptr: int, n_int16: int, d_out_ptr: int, out_stride: int,
+                            sync: bool = False) -> int:
+        """``process_read`` on device pointers (4-byte alignment is enough); returns PCM count per channel."""
+        n_pcm = C.c_size_t(0)
+        _lib.check(_lib.lib().rxb200_fm_process_read_device(self._h, d_in_ptr, n_int16, d_out_ptr, out_stride,
+                                                            C.byref(n_pcm), 1 if sync else 0))
+        return int(n_pcm.value)
+
     def levels(self) -> np.ndarray:
         """rms() of every chunk of the last call, int32[n_channels][n_chunks] (needs report_levels;
         the ``sr`` of src/rtl_fm.c:792-806)."""
