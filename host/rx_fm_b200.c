@@ -6,7 +6,7 @@
  * hand-off (src/rtl_fm.c:858-862, SURVEY F12) — no chunk is ever overwritten before it was consumed
  * and a file replay is deterministic.  Every DSP stage of rtlsdr_callback()+full_demod() is one call:
  * rxb200_fm_process_read(), one stream read (<= 131072 complex) per call, like the reference's chunks
- * (rxb200_fm_process on re-blocked chunks with -o N).
+ * (a read re-blocked to the library's chunk granularity with -o N).
  */
 #include <errno.h>
 #include <math.h>
@@ -83,7 +83,6 @@ static struct {
 	volatile int mute;                 /* int16 to zero at the start of the next read */
 	size_t multiple;                   /* chunk granularity librxb200 accepts, int16 */
 	size_t min_chunk;                  /* shortest chunk handed on, int16 */
-	int per_read;                      /* every chunk is one read: rxb200_fm_process_read, the reference's call site */
 	int failed;                        /* a library call failed: exit status 1 */
 	rxb200_fm *fm;
 	FILE *out;
@@ -201,8 +200,8 @@ static void *demod_thread(void *arg)
 		if (in->eof) { q_end_get(&G.q_raw); break; }
 		Slot *out = q_begin_put(&G.q_pcm);
 		size_t n_pcm = 0;
-		int rc = G.per_read ? rxb200_fm_process_read(G.fm, in->data, in->n, out->data, 2 * CHUNK_COMPLEX, &n_pcm)
-		                    : rxb200_fm_process(G.fm, in->data, in->n, in->n, out->data, 2 * CHUNK_COMPLEX, &n_pcm, NULL);
+		/* a slot re-blocked for -o N is a read rxb200_fm_process(h, x, n, n) takes, and runs exactly as that call */
+		int rc = rxb200_fm_process_read(G.fm, in->data, in->n, out->data, 2 * CHUNK_COMPLEX, &n_pcm);
 		q_end_get(&G.q_raw);
 		if (rc != RXB200_OK) { fprintf(stderr, "rxb200: %s\n", rxb200_last_error()); g_stop = 1; G.failed = 1; n_pcm = 0; }
 		if (G.print_levels && rc == RXB200_OK) {                                  /* :792-806, one chunk per call */
@@ -332,19 +331,13 @@ int main(int argc, char **argv)
 	if (G.freq_len > 1) { G.terminate_on_squelch = 0; }
 	G.filename = (argc <= optind) ? "-" : argv[optind];
 	if (rxb200_fm_derive(&G.cli, &G.der) != RXB200_OK) { fprintf(stderr, "rxb200: %s\n", rxb200_last_error()); return 1; }
-	if (G.der.params.downsample_passes == 0 && G.der.params.post_downsample <= 1) {
-		/* no fifth_order passes and no -o: the library takes any whole number of complex samples, so every read is one
-		 * chunk as it was read, like the reference's; only a read too short to complete a boxcar waits for the next */
+	if (G.der.params.post_downsample <= 1) {
+		/* no -o: every read is handed on as it was read, one rxb200_fm_process_read per read, like the reference's
+		 * full_demod per read; only a read too short to complete a boxcar, or with fifth_order passes shorter than 2^P
+		 * complex samples (for which the reference reads before its buffer), waits for the next */
+		const int P = G.der.params.downsample_passes;
 		G.multiple = 2;
-		G.min_chunk = 2 * (size_t)G.der.params.downsample;
-		G.per_read = 1;
-	} else if (G.der.params.post_downsample <= 1) {
-		/* fifth_order passes, no -o: every read is handed on as it was read, one rxb200_fm_process_read per read, like
-		 * the reference's full_demod per read; only a read shorter than 2^P complex samples (for which the reference
-		 * reads before its buffer) waits for the next */
-		G.multiple = 2;
-		G.min_chunk = (size_t)2 << G.der.params.downsample_passes;
-		G.per_read = 1;
+		G.min_chunk = P ? (size_t)2 << P : 2 * (size_t)G.der.params.downsample;
 	} else {   /* -o N: chunk granularity accepted by the library: 16 int16 and 2*2^P int16 */
 		size_t m = (size_t)2 << G.der.params.downsample_passes;
 		G.multiple = m > 16 ? m : 16;

@@ -153,7 +153,7 @@ int rxb200_fm_process_device(rxb200_fm *h, const int16_t *d_cs16, size_t n_int16
  * fifth_order passes n_int16 >= 2*2^P (below that the reference reads before its buffer).  The
  * read must produce a decimated sample when a per-chunk reduction stage is on, and decimate to a
  * multiple of post_downsample.  A read rxb200_fm_process(h, cs16, n_int16, n_int16, ...) takes
- * runs exactly as that call; a read with passes off their granule runs on the read kernel
+ * runs exactly as that call; a read with passes off their granule runs on the any-length kernel
  * (kernel_kind 0), where every pass ends where the reference's does: raw mode then returns
  * n_int16 >> P values, an odd count when L_P = n_int16 >> P is odd.  A refused call leaves the
  * handle's state untouched.  levels, squelch_hits, last_stats and kernel_ms report the read as

@@ -1332,48 +1332,13 @@ __device__ __forceinline__ void front_run(const FmDev &c, const FmCall &k, Front
 	}
 }
 
-// front_run for calls whose chunk or length is not a multiple of 8 complex samples (boxcar shapes only, P = 0).  A
-// channel's base, and with it every block, is then only 4-byte aligned, the segment that ends the channel may end inside
-// a block, and a chunk may start between any two samples: each sample is one 32-bit load (the loads of a block issue
-// together, none past t_end), and the chunk bookkeeping -- rotation phase, F8's first_in_chunk, the per-chunk
-// scalars and sums -- runs before every sample, so the samples on each side of a boundary see their own chunk's values.
-template <int SPEC, bool STORE>
-__device__ __forceinline__ void front_run_any(const FmDev &c, const FmCall &k, FrontState<0, SPEC> &s, EmitCtx &e,
-                                              const uint32_t *__restrict__ in, int t, int t_end, unsigned &u, int ch)
-{
-	const bool rot = Spec<SPEC>::rotate(c);
-	for (; t < t_end; t += 8) {
-		const int nb = t_end - t;
-		uint32_t v[8];
-#pragma unroll
-		for (int j = 0; j < 8; j++) { v[j] = j < nb ? __ldg(in + t + j) : 0u; }
-#pragma unroll
-		for (int j = 0; j < 8; j++) {
-			if (j < nb) {
-				if (u >= (unsigned)k.chunk) { u = 0u; }
-				if (u == 0u) {
-#pragma unroll 1
-					for (int z = 0; z < k.one; z++) { front_chunk_start<0, SPEC, STORE>(c, k, s, e, ch); }
-				}
-				int xi, xq;
-				scale_rot(v[j], (int)(u & 3u), rot, xi, xq, e.rdc_i, e.rdc_q);   // rotate16_90 restarts with every chunk
-				u++;
-				s.box_i += xi; s.box_q += xq;
-				if (++s.box_n >= c.D) {
-					int di = wrap16(s.box_i), dq = wrap16(s.box_q);
-					s.box_i = 0; s.box_q = 0; s.box_n = 0;
-					post_decim<0, SPEC, STORE>(c, k, s, e, di, dq);
-				}
-			}
-		}
-	}
-}
-
-// ---- one device read per call with fifth_order passes (rxb200_fm_process_read), any even length: the call is one chunk
-// of n complex samples.  Pass l runs over L_l = 2n >> l int16 (src/rtl_fm.c:759-776): ceil(L_l / 2) I and floor(L_l / 2)
-// Q samples, so in-chunk index i is a pair while i < n >> l, and index n >> l is an I sample alone when L_l is odd.  A
-// pass takes only the first samples of the previous pass's outputs; the windows of the passes still advanced over the rest.
-// Only the last 2^P samples of a read can meet such an end (tail_push); the rest run through scalar_push.
+// ---- the any-length front end: calls whose chunk or length is not a multiple of 8 complex samples without passes, and
+// one read of any even length per call with fifth_order passes (rxb200_fm_process_read).
+// With passes the call is one chunk of n complex samples.  Pass l runs over L_l = 2n >> l int16 (src/rtl_fm.c:759-776):
+// ceil(L_l / 2) I and floor(L_l / 2) Q samples, so in-chunk index i is a pair while i < n >> l, and index n >> l is an I
+// sample alone when L_l is odd.  A pass takes only the first samples of the previous pass's outputs; the windows of the
+// passes still advanced over the rest.  Only the last 2^P samples of a read can meet such an end (tail_push); the rest
+// run through scalar_push.
 
 // generic_fir on the I lane alone (the Q component's count ends one sample earlier)
 __device__ __forceinline__ int droop9_i(uint32_t (&h)[9], const int (&c)[6], int di)
@@ -1435,16 +1400,20 @@ __device__ __forceinline__ void tail_push(const FmDev &c, const FmCall &k, Front
 	}
 }
 
-// front_run for a read with passes: one 32-bit load per complex sample (4-byte alignment, nothing read past t_end); u is
-// the in-chunk index of sample t
-template <int P, bool STORE>
-__device__ __forceinline__ void front_run_read(const FmDev &c, const FmCall &k, FrontState<P, 2> &s, EmitCtx &e,
-                                               const uint32_t *__restrict__ in, int t, int t_end, unsigned &u, int ch)
+// front_run of the any-length front end: one 32-bit load per complex sample, since a channel's base, and with it every
+// block, is only 4-byte aligned (the loads of a block issue together, none past t_end: the segment that ends the channel
+// may end inside a block).  u is the in-chunk index of sample t.  Without passes a chunk may start between any two
+// samples, so the chunk bookkeeping -- rotation phase, F8's first_in_chunk, the per-chunk scalars and sums -- runs before
+// every sample and the samples on each side of a boundary see their own chunk's values; with passes the call is one
+// chunk (k.chunk == k.n), and its samples from (n >> P) << P on go through tail_push.
+template <int P, int SPEC, bool STORE>
+__device__ __forceinline__ void front_run_any(const FmDev &c, const FmCall &k, FrontState<P, SPEC> &s, EmitCtx &e,
+                                              const uint32_t *__restrict__ in, int t, int t_end, unsigned &u, int ch)
 {
-	const bool rot = Spec<2>::rotate(c);
+	const bool rot = Spec<SPEC>::rotate(c);
 	const unsigned n = (unsigned)k.n;
 	const unsigned tail = (n >> P) << P;              // from here on a sample may meet the end of a pass's count
-	const int t_main = t + (int)(u >= tail ? 0u : min(tail - u, (unsigned)(t_end - t)));
+	const int t_main = P == 0 ? t_end : t + (int)(u >= tail ? 0u : min(tail - u, (unsigned)(t_end - t)));
 	for (; t < t_main; t += 8) {
 		const int nb = t_main - t;
 		uint32_t v[8];
@@ -1453,36 +1422,50 @@ __device__ __forceinline__ void front_run_read(const FmDev &c, const FmCall &k, 
 #pragma unroll
 		for (int j = 0; j < 8; j++) {
 			if (j < nb) {
+				if constexpr (P == 0) { if (u >= (unsigned)k.chunk) { u = 0u; } }
 				if (u == 0u) {
 #pragma unroll 1
-					for (int z = 0; z < k.one; z++) { front_chunk_start<P, 2, STORE>(c, k, s, e, ch); }
+					for (int z = 0; z < k.one; z++) { front_chunk_start<P, SPEC, STORE>(c, k, s, e, ch); }
 				}
-				int xi, xq, oi, oq;
-				scale_rot(v[j], (int)(u & 3u), rot, xi, xq, e.rdc_i, e.rdc_q);
-				if (scalar_push<0, P, 2>(s, xi, xq, u, oi, oq)) { post_decim<P, 2, STORE>(c, k, s, e, oi, oq); }
-				u++;
+				int xi, xq;
+				scale_rot(v[j], (int)(u & 3u), rot, xi, xq, e.rdc_i, e.rdc_q);   // rotate16_90 restarts with every chunk
+				if constexpr (P == 0) {
+					u++;
+					s.box_i += xi; s.box_q += xq;
+					if (++s.box_n >= c.D) {
+						int di = wrap16(s.box_i), dq = wrap16(s.box_q);
+						s.box_i = 0; s.box_q = 0; s.box_n = 0;
+						post_decim<0, SPEC, STORE>(c, k, s, e, di, dq);
+					}
+				} else {
+					int oi, oq;
+					if (scalar_push<0, P, SPEC>(s, xi, xq, u, oi, oq)) { post_decim<P, SPEC, STORE>(c, k, s, e, oi, oq); }
+					u++;
+				}
 			}
 		}
 	}
-	t = t_main > t_end ? t_end : t_main;
+	if constexpr (P > 0) {
+		t = t_main > t_end ? t_end : t_main;
 #pragma unroll 1
-	for (; t < t_end; t++, u++) {                     // u >= tail > 0: no chunk starts here
-		int xi, xq;
-		scale_rot(__ldg(in + t), (int)(u & 3u), rot, xi, xq, e.rdc_i, e.rdc_q);
-		tail_push<0, P, STORE>(c, k, s, e, xi, xq, u, true, n);
+		for (; t < t_end; t++, u++) {                 // u >= tail > 0: no chunk starts here
+			int xi, xq;
+			scale_rot(__ldg(in + t), (int)(u & 3u), rot, xi, xq, e.rdc_i, e.rdc_q);
+			tail_push<0, P, STORE>(c, k, s, e, xi, xq, u, true, n);
+		}
 	}
 }
 
-// The read kernel keeps every pass scalar (FrontState<P, 2>); the carry keeps the handle's layout (fm_state_words), so
-// that calls of every entry point can follow one another: c.PL packed levels, lanes biased by 128 << l, holding the
-// pass's last six inputs -- the window a..e of the next chunk's first output, then the sample an even count left
-// pending -- and the scalar levels after them.
-template <int P>
-__device__ __forceinline__ void read_load(const FmDev &c, FrontState<P, 2> &s, const uint32_t *g)
+// The any-length front end keeps every pass scalar (FrontState<P, 2>); the carry keeps the handle's layout
+// (fm_state_words), so that calls of every entry point can follow one another: c.PL packed levels, lanes biased by
+// 128 << l, holding the pass's last six inputs -- the window a..e of the next chunk's first output, then the sample an
+// even count left pending -- and the scalar levels after them.  Without passes these are front_load / front_store's words.
+template <int P, int SPEC>
+__device__ __forceinline__ void any_load(const FmDev &c, FrontState<P, SPEC> &s, const uint32_t *g)
 {
 	s.box_i = (int)g[ST_BOX_I]; s.box_q = (int)g[ST_BOX_Q]; s.box_n = (int)g[ST_BOX_N];
 	s.pre_i = (int)g[ST_PRE_I]; s.pre_q = (int)g[ST_PRE_Q];
-	const int PL = c.PL;
+	const int PL = P == 0 ? 0 : c.PL;
 #pragma unroll
 	for (int l = 0; l < P; l++) {
 		if (l < PL) {
@@ -1503,12 +1486,12 @@ __device__ __forceinline__ void read_load(const FmDev &c, FrontState<P, 2> &s, c
 	for (int j = 0; j < 9; j++) { s.fh[j] = g[ST_HDR + 6 * PL + 7 * (P - PL) + j]; }
 }
 
-template <int P>
-__device__ __forceinline__ void read_store(const FmDev &c, const FrontState<P, 2> &s, uint32_t *g)
+template <int P, int SPEC>
+__device__ __forceinline__ void any_store(const FmDev &c, const FrontState<P, SPEC> &s, uint32_t *g)
 {
 	g[ST_BOX_I] = (uint32_t)s.box_i; g[ST_BOX_Q] = (uint32_t)s.box_q; g[ST_BOX_N] = (uint32_t)s.box_n;
 	g[ST_PRE_I] = (uint32_t)s.pre_i; g[ST_PRE_Q] = (uint32_t)s.pre_q;
-	const int PL = c.PL;
+	const int PL = P == 0 ? 0 : c.PL;
 #pragma unroll
 	for (int l = 0; l < P; l++) {
 		if (l < PL) {
@@ -1553,8 +1536,7 @@ __device__ __forceinline__ Item make_item(const FmDev &c, const FmCall &k, int w
 	return it;
 }
 
-// ---- front end of one work item: one segment per thread (tid 0..T-1).  ANY: the any-length front end (front_run_any;
-// front_run_read with passes)
+// ---- front end of one work item: one segment per thread (tid 0..T-1).  ANY: the any-length front end (front_run_any)
 template <int P, int SPEC, bool ANY>
 __device__ __forceinline__ void front_item(const FmDev &c, const FmCall &k, const Item &it, int tid, int16_t *pcm_s)
 {
@@ -1569,7 +1551,7 @@ __device__ __forceinline__ void front_item(const FmDev &c, const FmCall &k, cons
 	FrontState<P, SPEC> s;
 	if (t0 <= 0) {
 		t0 = 0;
-		if constexpr (ANY && P > 0) { read_load<P>(c, s, carry); } else { front_load<P, SPEC>(s, carry); }
+		if constexpr (ANY) { any_load<P, SPEC>(c, s, carry); } else { front_load<P, SPEC>(s, carry); }
 	}
 	else {
 		front_zero<P, SPEC>(s);
@@ -1592,16 +1574,12 @@ __device__ __forceinline__ void front_item(const FmDev &c, const FmCall &k, cons
 	}
 	// offsets relative to t0 fit 32 bits (a segment plus its halo)
 	const int16_t *__restrict__ in = k.in + 2 * ((size_t)it.ch * (size_t)k.n + (size_t)t0);
-	if constexpr (ANY && P > 0) {
-		static_assert(SPEC == 2, "the read front end keeps every pass scalar");
+	if constexpr (ANY) {
+		static_assert(P == 0 || SPEC == 2, "with passes the any-length front end keeps every pass scalar");
+		static_assert(P > 0 || SPEC == 0 || SPEC == 2, "without passes the any-length front end is the generic boxcar one");
 		const uint32_t *in_w = reinterpret_cast<const uint32_t *>(in);
-		front_run_read<P, false>(c, k, s, e, in_w, 0, (int)(start - t0), u, it.ch);
-		front_run_read<P, true>(c, k, s, e, in_w, (int)(start - t0), (int)(end - t0), u, it.ch);
-	} else if constexpr (ANY) {
-		static_assert(SPEC == 0 || SPEC == 2, "the any-length front end is the generic boxcar one");
-		const uint32_t *in_w = reinterpret_cast<const uint32_t *>(in);
-		front_run_any<SPEC, false>(c, k, s, e, in_w, 0, (int)(start - t0), u, it.ch);
-		front_run_any<SPEC, true>(c, k, s, e, in_w, (int)(start - t0), (int)(end - t0), u, it.ch);
+		front_run_any<P, SPEC, false>(c, k, s, e, in_w, 0, (int)(start - t0), u, it.ch);
+		front_run_any<P, SPEC, true>(c, k, s, e, in_w, (int)(start - t0), (int)(end - t0), u, it.ch);
 	} else {
 		const int t_last = (int)(end - t0) - 8;
 		front_run<P, SPEC, false>(c, k, s, e, in, 0, (int)(start - t0), t_last, u, it.ch);
@@ -1610,7 +1588,7 @@ __device__ __forceinline__ void front_item(const FmDev &c, const FmCall &k, cons
 	if (SPEC == 2 && k.reduce_mode == 1) { chunk_enter<true>(c, k, e, it.ch, e.chunk_idx); }   // flush the last chunk's sums
 	if (end == k.n && (SPEC != 2 || k.reduce_mode == 0)) {
 		// this thread saw the end of the stream: its registers are the next call's carry
-		if constexpr (ANY && P > 0) { read_store<P>(c, s, k.carry_out + (size_t)it.ch * k.state_words); }
+		if constexpr (ANY) { any_store<P, SPEC>(c, s, k.carry_out + (size_t)it.ch * k.state_words); }
 		else { front_store<P, SPEC>(s, k.carry_out + (size_t)it.ch * k.state_words); }
 	}
 }
@@ -1857,8 +1835,7 @@ __device__ __forceinline__ void back_item(const FmDev &c, const FmCall &k, const
 // `be_lanes/32` warps run the back end out of the shared PCM buffer.  Work items are handed out by an
 // atomic ticket, oldest first (the cross-item look-back only ever waits for an older ticket).
 // The occupancy target is stated for 256 threads and scales with the width (same threads per SM).
-// ANY: the any-length front end (front_run_any), for the calls fm_any_length picks; with passes (SPEC 2) the read
-// kernel (front_run_read), for the reads fm_read_any picks.
+// ANY: the any-length front end (front_run_any), for the calls fm_route sends there.
 template <int P, int SPEC, int T, bool ANY = false>
 __global__ void __launch_bounds__(T, (FM_MAX_THREADS / T) * (SPEC == 2 ? (P <= 3 ? 2 : 1) : (P <= 3 ? RXB_OCC : (P <= 6 ? 2 : 1)))) fm_fused_kernel(const FmDev c, const FmCall k)
 {
@@ -2064,10 +2041,9 @@ __global__ void fm_rdc_recur_kernel(const long long *sums, const int *chunk_len,
 	carry_out[(size_t)ch * state_words + ST_RDC_Q] = (uint32_t)aq;
 }
 
-// rms() + squelch decision (src/rtl_fm.c:739-757, :781-790); lp_len = LEN_MUL * len[ci] int16
-template <int LEN_MUL>
-__device__ __forceinline__ void squelch_recur(const long long *sums, const int *len_tab, int n_chunks, int n_ch, int level,
-                                              const uint32_t *carry_in, uint32_t *carry_out, int state_words, int *sqz, int *levels)
+// rms() + squelch decision (src/rtl_fm.c:739-757, :781-790); lp_len = the chunk's lowpassed int16 (fm_count_outputs)
+__global__ void fm_squelch_kernel(const long long *sums, const int *lp_len, int n_chunks, int n_ch, int level,
+                                  const uint32_t *carry_in, uint32_t *carry_out, int state_words, int *sqz, int *levels)
 {
 	const int ch = blockIdx.x * blockDim.x + threadIdx.x;
 	if (ch >= n_ch) { return; }
@@ -2075,7 +2051,7 @@ __device__ __forceinline__ void squelch_recur(const long long *sums, const int *
 	for (int ci = 0; ci < n_chunks; ci++) {
 		const long long *sm = sums + 2 * ((size_t)ch * n_chunks + ci);
 		const long long t = sm[0], p = sm[1];
-		const int len = LEN_MUL * len_tab[ci];                   // lp_len counts int16
+		const int len = lp_len[ci];
 		// dc = (double)(t*step)/len; err = t*2*dc - dc*dc*len; (int)sqrt((p-err)/len) -- same order, no FMA
 		const double dc = __ddiv_rn((double)t, (double)len);
 		const double err = __dsub_rn(__dmul_rn((double)(t * 2), dc), __dmul_rn(__dmul_rn(dc, dc), (double)len));
@@ -2088,20 +2064,6 @@ __device__ __forceinline__ void squelch_recur(const long long *sums, const int *
 		}
 	}
 	carry_out[(size_t)ch * state_words + ST_SQ_HITS] = (uint32_t)hits;
-}
-
-// dec_len = decimated complex samples of the chunk: lp_len is even
-__global__ void fm_squelch_kernel(const long long *sums, const int *dec_len, int n_chunks, int n_ch, int level,
-                                  const uint32_t *carry_in, uint32_t *carry_out, int state_words, int *sqz, int *levels)
-{
-	squelch_recur<2>(sums, dec_len, n_chunks, n_ch, level, carry_in, carry_out, state_words, sqz, levels);
-}
-
-// lp_len int16 of the chunk: a read with passes leaves an odd count when L_P is odd (rxb200_fm_process_read)
-__global__ void fm_squelch_lp_kernel(const long long *sums, const int *lp_len, int n_chunks, int n_ch, int level,
-                                     const uint32_t *carry_in, uint32_t *carry_out, int state_words, int *sqz, int *levels)
-{
-	squelch_recur<1>(sums, lp_len, n_chunks, n_ch, level, carry_in, carry_out, state_words, sqz, levels);
 }
 
 // dc_block_audio_filter recurrence (src/rtl_fm.c:691-696); pcm_len = result_len of the chunk before low_pass_real
@@ -2213,8 +2175,9 @@ static fm_kernel_fn pick_kernel(int P, int spec, int threads)
 	return pick_kernel_p<0>(P, threads);
 }
 
-// The any-length variant: the generic boxcar kernel (SPEC 0, or SPEC 2 with the per-chunk reduction stages) in one CTA
-// width; every other specialisation's shape is also a SPEC 0 shape
+// The any-length kernel, in one CTA width.  Without passes the generic boxcar kernel (SPEC 0, or SPEC 2 with the per-chunk
+// reduction stages): every other specialisation's shape is also a SPEC 0 shape.  With passes SPEC 2's all-scalar passes
+// and stage bookkeeping serve every shape -- with no reduction stage on, that bookkeeping stays idle.
 #define FM_ANY_THREADS 256
 static fm_kernel_fn pick_any_kernel(int P, int spec)
 {
@@ -2222,20 +2185,8 @@ static fm_kernel_fn pick_any_kernel(int P, int spec)
 	(void)P; (void)spec;
 	return nullptr;
 #else
-	if (P != 0) { return nullptr; }
-	return spec == 2 ? fm_fused_kernel<0, 2, FM_ANY_THREADS, true> : fm_fused_kernel<0, 0, FM_ANY_THREADS, true>;
-#endif
-}
-
-// The read kernel (rxb200_fm_process_read with passes, a read off their granule): SPEC 2's all-scalar passes and stage
-// bookkeeping serve every shape -- with no reduction stage on, that bookkeeping stays idle
-static fm_kernel_fn pick_read_kernel(int P)
-{
-#ifdef RXB_QUICK
-	(void)P;
-	return nullptr;
-#else
 	switch (P) {
+	case 0: return spec == 2 ? fm_fused_kernel<0, 2, FM_ANY_THREADS, true> : fm_fused_kernel<0, 0, FM_ANY_THREADS, true>;
 	case 1: return fm_fused_kernel<1, 2, FM_ANY_THREADS, true>;
 	case 2: return fm_fused_kernel<2, 2, FM_ANY_THREADS, true>;
 	case 3: return fm_fused_kernel<3, 2, FM_ANY_THREADS, true>;
@@ -2295,8 +2246,7 @@ struct rxb200_fm {
 	fm_split_fn kern_rows = nullptr;     // split kernel with the row front end (null: shape not covered)
 	fm_kernel_fn kern_front = nullptr;   // stream path: front end alone (SPEC 4), PCM to global memory; fm_back_kernel follows
 	int16_t *d_pcm = nullptr; size_t d_pcm_cap = 0;       // its PCM scratch, int16 elements
-	fm_kernel_fn kern_any = nullptr;     // any-length calls (P = 0, chunk or call not a multiple of 8 complex), FM_ANY_THREADS wide
-	fm_kernel_fn kern_read = nullptr;    // rxb200_fm_process_read with passes (P >= 1) off their granule, FM_ANY_THREADS wide
+	fm_kernel_fn kern_any = nullptr;     // the any-length kernel (the calls fm_route sends there), FM_ANY_THREADS wide
 	size_t stream_min = 0; int stream_piece = 0, stream_win = 0, stream_t = 0;
 	int threads = 0;               // CTA width of kern
 	int wide = 0;                  // all-scalar fifth_order passes (raw DC block on)
@@ -2413,7 +2363,6 @@ extern "C" int rxb200_fm_create(const rxb200_fm_params *params, int device, int 
 		const int fir_on = (params->downsample_passes > 0 && params->comp_fir_size == 9) ? 1 : 0;
 		h->kern_rows = spec == 1 ? pick_rows_kernel(params->downsample_passes, fir_on) : nullptr;
 		h->kern_any = pick_any_kernel(params->downsample_passes, spec);
-		h->kern_read = pick_read_kernel(params->downsample_passes);
 		// stream path (front kernel + back kernel): the wbfm shape without decimating passes, de-emphasis on
 #ifndef RXB_QUICK
 		h->kern_front = (spec == 1 && params->downsample_passes == 0 && params->deemph) ? pick_kernel(0, 4, h->threads) : nullptr;
@@ -2515,7 +2464,9 @@ static size_t fm_count_outputs(rxb200_fm *h, size_t n_int16, size_t chunk_int16,
 		else { dec = (box_n + L) / p.downsample; box_n = (box_n + L) % p.downsample; }
 		// low_pass_simple needs a whole number of groups per chunk (otherwise the reference reads stale data)
 		if (dec % h->dev.post_ds != 0) { return (size_t)-1; }
-		// lowpassed int16 after the passes: odd when a read's L_P is (rxb200_fm_process_read), else 2 * dec
+		// lowpassed int16 after the passes, what rms() divides by: odd when a read's L_P is (rxb200_fm_process_read).
+		// For every chunk rxb200_fm_process takes lp == 2 * dec: without passes by construction, and with them every
+		// chunk is a multiple of 2 << P int16, so len16 >> P == 2 * ((len16 / 2) >> P)
 		const long long lp = p.downsample_passes ? (long long)(len16 >> p.downsample_passes) : 2 * dec;
 		if (lens) {
 			lens[c] = (int)L; lens[n_chunks + c] = (int)dec; lens[2 * n_chunks + c] = (int)(dec / h->dev.post_ds);
@@ -2547,26 +2498,37 @@ extern "C" size_t rxb200_fm_max_output(const rxb200_fm *h, size_t n_int16, size_
 	return dec;
 }
 
-// A call the any-length kernel runs: no fifth_order passes, and a chunk or the call not a multiple of 8 complex samples
-// (the vector kernels' block).  Every other call keeps the kernels and plans of the 8-sample granule.
-static bool fm_any_length(const rxb200_fm *h, size_t n_int16, size_t chunk_int16)
+// Whether a call's shape is taken (else EUNSUPPORTED), and *any: whether it runs on the any-length kernel; every other
+// call keeps the kernels and plans of the vector kernels' granule, 8 complex samples per block and 2^P per chunk
+// (DESIGN.md section 6).  *any is set for a refused shape too: a device input's alignment follows from it and is
+// reported first.  aligned32: the input is 32-byte aligned.
+// - rxb200_fm_process without passes: any even chunk of at most 262144 int16 and any even call, on the any-length
+//   kernel when the chunk or the call is not a multiple of 16 int16;
+// - rxb200_fm_process with passes: chunk and call multiples of the granule;
+// - rxb200_fm_process_read: one read of any even length from 2 << P int16 (fm_demod reads lowpassed[-1] below that; 2
+//   without passes) to 262144, on whatever rxb200_fm_process(h, x, n, n) runs when that call takes it and the input is
+//   32-byte aligned, else on the any-length kernel.
+static int fm_route(const rxb200_fm *h, size_t n_int16, size_t chunk_int16, bool read, bool aligned32, bool *any)
 {
-	return h->kern_any != nullptr && (chunk_int16 % 16 != 0 || n_int16 % 16 != 0);
-}
-
-static int fm_check_shape(const rxb200_fm *h, size_t n_int16, size_t chunk_int16)
-{
-	// Without passes any whole number of complex samples (the any-length kernel takes what the vector kernels cannot);
-	// with passes 8 complex per vector step and 2^P complex per chunk (DESIGN.md section 6)
-	size_t g16 = h->kern_any ? 2 : 16;
-	size_t p16 = (size_t)2 << h->p.downsample_passes; // 2^P complex
-	if (p16 > g16) { g16 = p16; }
-	if (chunk_int16 == 0 || chunk_int16 > 262144 || chunk_int16 % g16 != 0) {
-		set_error("chunk_int16=%zu must be a multiple of %zu and <= 262144", chunk_int16, g16);
+	const int P = h->p.downsample_passes;
+	const size_t p16 = (size_t)2 << P, g16 = p16 > 16 ? p16 : 16;   // 2^P complex; the granule
+	if (read) {
+		*any = !aligned32 || n_int16 % g16 != 0;
+		const size_t lo = P ? p16 : 2;
+		if (n_int16 < lo || n_int16 > 262144 || n_int16 % 2 != 0) {
+			set_error("a read of n_int16=%zu must be even, at least %zu and at most 262144", n_int16, lo);
+			return RXB200_EUNSUPPORTED;
+		}
+		return RXB200_OK;
+	}
+	*any = P == 0 && (chunk_int16 % 16 != 0 || n_int16 % 16 != 0);
+	const size_t m16 = P ? g16 : 2;
+	if (chunk_int16 == 0 || chunk_int16 > 262144 || chunk_int16 % m16 != 0) {
+		set_error("chunk_int16=%zu must be a multiple of %zu and <= 262144", chunk_int16, m16);
 		return RXB200_EUNSUPPORTED;
 	}
-	if (n_int16 % g16 != 0) {
-		set_error("n_int16=%zu must be a multiple of %zu (last chunk included)", n_int16, g16);
+	if (n_int16 % m16 != 0) {
+		set_error("n_int16=%zu must be a multiple of %zu (last chunk included)", n_int16, m16);
 		return RXB200_EUNSUPPORTED;
 	}
 	return RXB200_OK;
@@ -2850,8 +2812,7 @@ static int fm_plan_back(const rxb200_fm *h, long long n, FmBackPlan *b)
 // per-chunk scalars: sizes (closed form), accumulators, then one recurrence per stage in the reference's order: raw DC
 // block -> squelch (sees the DC-blocked data, its sums from pass(1)) -> audio DC block (sums from pass(2))
 template <typename Pass>
-// read: the call runs on the read kernel, whose rms() divides by an lp_len that may be odd
-static int fm_prepasses(rxb200_fm *h, FmCall &k, size_t n_int16, size_t chunk_int16, bool read, Pass pass, int *launches)
+static int fm_prepasses(rxb200_fm *h, FmCall &k, size_t n_int16, size_t chunk_int16, Pass pass, int *launches)
 {
 	const FmDev &dv = h->dev;
 	const int n_chunks = k.n_chunks;
@@ -2886,13 +2847,8 @@ static int fm_prepasses(rxb200_fm *h, FmCall &k, size_t n_int16, size_t chunk_in
 		k.sums = h->d_sums;
 		const int rc = pass(1);
 		if (rc != RXB200_OK) { return rc; }
-		if (read) {
-			fm_squelch_lp_kernel<<<cb, 64, 0, h->stream>>>(h->d_sums, h->d_lens + 3 * (size_t)n_chunks, n_chunks, h->n_channels, dv.squelch,
-			                                                k.carry_in, k.carry_out, h->state_words, h->d_sqz, dv.levels ? h->d_levels : nullptr);
-		} else {
-			fm_squelch_kernel<<<cb, 64, 0, h->stream>>>(h->d_sums, h->d_lens + n_chunks, n_chunks, h->n_channels, dv.squelch, k.carry_in,
-			                                             k.carry_out, h->state_words, h->d_sqz, dv.levels ? h->d_levels : nullptr);
-		}
+		fm_squelch_kernel<<<cb, 64, 0, h->stream>>>(h->d_sums, h->d_lens + 3 * (size_t)n_chunks, n_chunks, h->n_channels, dv.squelch,
+		                                             k.carry_in, k.carry_out, h->state_words, h->d_sqz, dv.levels ? h->d_levels : nullptr);
 		RXB_CUDA(cudaGetLastError());
 		(*launches)++;
 		k.sqz = dv.squelch ? h->d_sqz : nullptr;
@@ -2915,7 +2871,7 @@ static int fm_prepasses(rxb200_fm *h, FmCall &k, size_t n_int16, size_t chunk_in
 
 // Plans and launches one call -- the split kernel where the shape allows it, else the fused kernel, or on the stream
 // path the front and back kernels -- then advances the host mirrors of the closed-form counters.  any: the call runs on
-// the any-length kernel of its pass count instead (kern_any without passes, kern_read with them).
+// the any-length kernel (kern_any) instead.
 static int fm_launch(rxb200_fm *h, const int16_t *d_in, size_t n_int16, size_t chunk_int16, int16_t *d_out, size_t out_stride,
                      bool any)
 {
@@ -2931,7 +2887,7 @@ static int fm_launch(rxb200_fm *h, const int16_t *d_in, size_t n_int16, size_t c
 	const size_t stream_min = h->stream_min != (size_t)-1 ? h->stream_min : (size_t)(32 * fm_replay(h, false) * Dpcm / h->n_channels);
 	// an any-length call runs on its own kernel, front and back end fused, whatever the shape would take otherwise
 	const bool stream = !any && h->kern_front != nullptr && dv.deemph && (size_t)n >= stream_min;
-	const fm_kernel_fn kern = any ? (dv.P ? h->kern_read : h->kern_any) : (stream ? h->kern_front : h->kern);
+	const fm_kernel_fn kern = any ? h->kern_any : (stream ? h->kern_front : h->kern);
 	FmCall k = {};
 	FmGrid g;
 	CUtensorMap in_map;
@@ -2974,7 +2930,7 @@ static int fm_launch(rxb200_fm *h, const int16_t *d_in, size_t n_int16, size_t c
 		return RXB200_OK;
 	};
 	if (dv.rdc_on || dv.squelch || dv.adc_on || dv.levels) {
-		rc = fm_prepasses(h, k, n_int16, chunk_int16, any && dv.P > 0, pass, &launches);
+		rc = fm_prepasses(h, k, n_int16, chunk_int16, pass, &launches);
 		if (rc != RXB200_OK) { return rc; }
 	}
 	rc = pass(0);
@@ -3000,60 +2956,35 @@ static int fm_launch(rxb200_fm *h, const int16_t *d_in, size_t n_int16, size_t c
 	return RXB200_OK;
 }
 
-// what both process calls check before they launch, and the call's output count (*total PCM samples per channel)
-// rxb200_fm_process_read's shapes: one read of any even length, at least 2^P complex samples with passes (fm_demod
-// reads lowpassed[-1] below that)
-static int fm_check_read(const rxb200_fm *h, size_t n_int16)
-{
-	const size_t lo = h->p.downsample_passes ? ((size_t)2 << h->p.downsample_passes) : 2;
-	if (n_int16 < lo || n_int16 > 262144 || n_int16 % 2 != 0) {
-		set_error("a read of n_int16=%zu must be even, at least %zu and at most 262144", n_int16, lo);
-		return RXB200_EUNSUPPORTED;
-	}
-	return RXB200_OK;
-}
-
-// Where a read runs: on whatever rxb200_fm_process(h, x, n, n, ...) runs when that call takes it and the input is 32-byte
-// aligned, else on the any-length kernel of its pass count (a read with passes off their granule, or a device read at
-// 4-byte alignment)
-static bool fm_read_any(const rxb200_fm *h, size_t n_int16, bool aligned32)
-{
-	const size_t p16 = (size_t)2 << h->p.downsample_passes;
-	const size_t g16 = p16 > 16 ? p16 : 16;
-	return !aligned32 || fm_any_length(h, n_int16, n_int16) || (h->p.downsample_passes > 0 && n_int16 % g16 != 0);
-}
-
-// what every process call checks before it launches, and the call's output count (*total PCM samples per channel);
-// read: a call of rxb200_fm_process_read (one chunk, its own shape rule)
+// what every process call checks before it launches, in the order its refusals are reported, and the call's output
+// count (*total PCM samples per channel) and route (*any, fm_route).  device: `in` is a device pointer, read at the
+// alignment of the kernel the call runs on (the any-length kernel reads one complex sample at a time); a host input is
+// staged into the handle's buffer, which is aligned.  read: a call of rxb200_fm_process_read (one chunk, its own shape rule)
 static int fm_prologue(rxb200_fm *h, const void *in, const void *out, size_t n_int16, size_t chunk_int16, size_t pcm_stride,
-                       int *chunk_result_len, size_t *total, size_t *n_pcm, bool read = false)
+                       int *chunk_result_len, size_t *total, size_t *n_pcm, bool read, bool device, bool *any)
 {
 	if (!h || !in || !out) { set_error("null argument"); return RXB200_EINVAL; }
-	const int rc = read ? fm_check_read(h, n_int16) : fm_check_shape(h, n_int16, chunk_int16);
+	const uintptr_t addr = device ? (uintptr_t)in : 0u;
+	const int rc = fm_route(h, n_int16, chunk_int16, read, (addr & 31u) == 0, any);
+	const uintptr_t align = *any ? 4u : 32u;
+	if ((addr & (align - 1u)) != 0) { set_error("d_cs16 must be %d-byte aligned", (int)align); return RXB200_EINVAL; }
 	if (rc != RXB200_OK) { return rc; }
 	RXB_CUDA(cudaSetDevice(h->device));
 	if (n_int16 == 0) { h->level_chunks = 0; if (n_pcm) { *n_pcm = 0; } }
 	*total = fm_count_outputs(h, n_int16, chunk_int16, chunk_result_len, nullptr, false);
 	if (*total == (size_t)-1) { set_error("-o %d needs every chunk to decimate to a multiple of it", h->dev.post_ds); return RXB200_EUNSUPPORTED; }
 	if (*total > pcm_stride) { set_error("pcm_stride %zu < %zu outputs", pcm_stride, *total); return RXB200_ECAPACITY; }
+	if (*any && !h->kern_any) { set_error("no any-length kernel for downsample_passes %d in this build", h->dev.P); return RXB200_EUNSUPPORTED; }
 	return RXB200_OK;
 }
 
 static int fm_process_device(rxb200_fm *h, const int16_t *d_cs16, size_t n_int16, size_t chunk_int16, int16_t *d_pcm,
                              size_t pcm_stride, size_t *n_pcm, int sync, bool read)
 {
-	// null arguments are reported first, by fm_prologue; the any-length kernels read one complex sample at a time
-	const bool aligned32 = ((uintptr_t)d_cs16 & 31u) == 0;
-	const bool any = h && (read ? fm_read_any(h, n_int16, aligned32) : fm_any_length(h, n_int16, chunk_int16));
-	const uintptr_t align = any ? 4u : 32u;
-	if (h && d_cs16 && d_pcm && ((uintptr_t)d_cs16 & (align - 1u)) != 0) {
-		set_error("d_cs16 must be %d-byte aligned", (int)align);
-		return RXB200_EINVAL;
-	}
 	size_t total = 0;
-	int rc = fm_prologue(h, d_cs16, d_pcm, n_int16, chunk_int16, pcm_stride, nullptr, &total, n_pcm, read);
+	bool any = false;
+	int rc = fm_prologue(h, d_cs16, d_pcm, n_int16, chunk_int16, pcm_stride, nullptr, &total, n_pcm, read, true, &any);
 	if (rc != RXB200_OK || n_int16 == 0) { return rc; }
-	if (any && !(h->dev.P ? h->kern_read : h->kern_any)) { set_error("no any-length kernel for downsample_passes %d in this build", h->dev.P); return RXB200_EUNSUPPORTED; }
 	rc = fm_launch(h, d_cs16, n_int16, chunk_int16, d_pcm, pcm_stride, any);
 	if (rc != RXB200_OK) { return rc; }
 	if (n_pcm) { *n_pcm = total; }
@@ -3068,10 +2999,9 @@ static int fm_process_host(rxb200_fm *h, const int16_t *cs16, size_t n_int16, si
                            size_t pcm_stride, size_t *n_pcm, int *chunk_result_len, bool read)
 {
 	size_t total = 0;
-	int rc = fm_prologue(h, cs16, pcm, n_int16, chunk_int16, pcm_stride, chunk_result_len, &total, n_pcm, read);
+	bool any = false;
+	int rc = fm_prologue(h, cs16, pcm, n_int16, chunk_int16, pcm_stride, chunk_result_len, &total, n_pcm, read, false, &any);
 	if (rc != RXB200_OK || n_int16 == 0) { return rc; }
-	const bool any = read ? fm_read_any(h, n_int16, true) : fm_any_length(h, n_int16, chunk_int16);
-	if (any && !(h->dev.P ? h->kern_read : h->kern_any)) { set_error("no any-length kernel for downsample_passes %d in this build", h->dev.P); return RXB200_EUNSUPPORTED; }
 	const size_t in_elems = n_int16 * (size_t)h->n_channels;
 	const size_t out_elems = (total + 8) * (size_t)h->n_channels;
 	RXB_CUDA(fm_reserve(h->d_in, h->d_in_cap, in_elems));

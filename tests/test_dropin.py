@@ -40,6 +40,8 @@ def _oracle_params(p):
     (["-M", "fm", "-s", "24k", "-A", "lut"], dict(rate_s=24000, custom_atan=2)),
     (["-M", "am", "-s", "12k", "-r", "6k"], dict(mode=fm.MODE_AM, rate_s=12000, rate_r=6000)),
     (["-M", "raw", "-s", "250k"], dict(mode=fm.MODE_RAW, rate_s=250000)),
+    (["-M", "wbfm", "-s", "300k", "-F", "9", "-r", "48k", "-o", "2"],
+     dict(wbfm=1, rate_s=300000, rate_r=48000, use_F=1, comp_fir_size=9, post_downsample=2)),
 ])
 def test_rx_fm_output_bytes(tmp_path, port, args, kw):
     x = synth.cfg2_iq(4 * 131072, seed=31)
