@@ -344,6 +344,35 @@ int rxb200_power_group_accumulate(rxb200_power_group *g, const int16_t *hop_bufs
 int rxb200_power_group_gather(rxb200_power_group *g);
 int rxb200_power_group_reset(rxb200_power_group *g);
 
+/* ======================================================================== rx_fm on several GPUs (SURVEY.md §8e)
+ * Channels are independent demod_state streams, so they split over GPUs with no exchange at all: one process, n_dev
+ * rxb200_fm handles, member i owning the contiguous channels [b, e) that rxb200_power_shard(n_channels, n_dev, i, &b, &e)
+ * gives (5 channels over 4 members: 2 + 2 + 1 + 0).  A member whose range is empty has no handle.  devices == NULL
+ * means 0..n_dev-1; an ordinal may repeat (several members on one GPU).
+ * The group behaves byte for byte like ONE rxb200_fm handle with n_channels channels: the same pcm, n_pcm,
+ * chunk_result_len, squelch hits, levels ([n_channels][n_chunks]) and refusal codes, over any sequence of process,
+ * process_read and reset calls.  cs16 and pcm are HOST pointers laid out as for rxb200_fm_process (channel c at
+ * cs16 + c*n_int16 and pcm + c*pcm_stride).  A call refused for its shape or capacity is refused before any member
+ * starts and leaves every member's state untouched.  Each member copies its block of channels to its GPU, runs
+ * rxb200_fm_process_device / _read_device and copies its PCM rows back, all on its own stream; the call returns when
+ * every member is done, also after a CUDA failure, and leaves the caller's current device as it found it.  The copies
+ * of different GPUs overlap only with pinned (page-locked) host buffers: with pageable ones they run one after the
+ * other and only the kernels overlap them (the bytes are the same either way). */
+typedef struct rxb200_fm_group rxb200_fm_group;
+int rxb200_fm_group_create(const rxb200_fm_params *params, int n_channels, int n_dev, const int *devices,
+                           rxb200_fm_group **out);
+void rxb200_fm_group_destroy(rxb200_fm_group *g);
+int rxb200_fm_group_size(const rxb200_fm_group *g);
+/* member i's handle (its channels are channel 0.. of that handle), NULL for a member that owns no channel */
+rxb200_fm *rxb200_fm_group_member(rxb200_fm_group *g, int i);
+int rxb200_fm_group_process(rxb200_fm_group *g, const int16_t *cs16, size_t n_int16, size_t chunk_int16,
+                            int16_t *pcm, size_t pcm_stride, size_t *n_pcm, int *chunk_result_len);
+int rxb200_fm_group_process_read(rxb200_fm_group *g, const int16_t *cs16, size_t n_int16,
+                                 int16_t *pcm, size_t pcm_stride, size_t *n_pcm);
+int rxb200_fm_group_squelch_hits(rxb200_fm_group *g, int *hits /* n_channels */);
+int rxb200_fm_group_levels(rxb200_fm_group *g, int *levels, size_t cap, size_t *n_chunks);
+int rxb200_fm_group_reset(rxb200_fm_group *g);
+
 /* ======================================================================== rx_sdr (SURVEY.md §8f row 4)
  * The pointwise sample-format conversions of rx_sdr's recorder loop (src/rtl_sdr.c:348-391):
  *   RXB200_CVT_CS16_CS8  : (uint8_t)(int)(x/32767.0*128.0+0.4)       per int16 (:367-370)

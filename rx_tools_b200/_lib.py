@@ -75,6 +75,9 @@ SYMBOLS = [
     "rxb200_comm_rank", "rxb200_power_shard", "rxb200_power_gather",
     "rxb200_power_group_create", "rxb200_power_group_destroy", "rxb200_power_group_size", "rxb200_power_group_member",
     "rxb200_power_group_accumulate", "rxb200_power_group_gather", "rxb200_power_group_reset",
+    "rxb200_fm_group_create", "rxb200_fm_group_destroy", "rxb200_fm_group_size", "rxb200_fm_group_member",
+    "rxb200_fm_group_process", "rxb200_fm_group_process_read", "rxb200_fm_group_squelch_hits", "rxb200_fm_group_levels",
+    "rxb200_fm_group_reset",
     "rxb200_sdr_convert", "rxb200_sdr_convert_device",
 ]
 
@@ -151,6 +154,17 @@ def lib() -> C.CDLL:
     L.rxb200_power_group_accumulate.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
     L.rxb200_power_group_gather.argtypes = [C.c_void_p]
     L.rxb200_power_group_reset.argtypes = [C.c_void_p]
+    L.rxb200_fm_group_create.argtypes = [C.POINTER(FmParamsC), C.c_int, C.c_int, pint, C.POINTER(C.c_void_p)]
+    L.rxb200_fm_group_destroy.argtypes = [C.c_void_p]
+    L.rxb200_fm_group_destroy.restype = None
+    L.rxb200_fm_group_size.argtypes = [C.c_void_p]
+    L.rxb200_fm_group_member.argtypes = [C.c_void_p, C.c_int]
+    L.rxb200_fm_group_member.restype = C.c_void_p
+    L.rxb200_fm_group_process.argtypes = [C.c_void_p, C.c_void_p, sz, sz, C.c_void_p, sz, C.POINTER(sz), pint]
+    L.rxb200_fm_group_process_read.argtypes = [C.c_void_p, C.c_void_p, sz, C.c_void_p, sz, C.POINTER(sz)]
+    L.rxb200_fm_group_squelch_hits.argtypes = [C.c_void_p, pint]
+    L.rxb200_fm_group_levels.argtypes = [C.c_void_p, pint, sz, C.POINTER(sz)]
+    L.rxb200_fm_group_reset.argtypes = [C.c_void_p]
     L.rxb200_sdr_convert.argtypes = [C.c_int, C.c_void_p, sz, C.c_void_p, C.c_int]
     L.rxb200_sdr_convert_device.argtypes = [C.c_int, C.c_void_p, sz, C.c_void_p, C.c_void_p]
     _lib = L

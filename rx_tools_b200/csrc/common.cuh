@@ -11,6 +11,12 @@ namespace rxb {
 
 void set_error(const char *fmt, ...);
 
+// fm_kernels.cu: every refusal of a host-pointer rx_fm call (rxb200_fm_process, or rxb200_fm_process_read when read is
+// set), in the order the call reports them, without enqueuing anything; *total receives the call's PCM count per
+// channel.  fm_group.cpp checks every member with it before any member starts.
+int fm_check_host_call(rxb200_fm *h, const int16_t *cs16, size_t n_int16, size_t chunk_int16, int16_t *pcm,
+                       size_t pcm_stride, int *chunk_result_len, size_t *n_pcm, bool read, size_t *total);
+
 #define RXB_CUDA(call)                                                                   \
 	do {                                                                                 \
 		cudaError_t e__ = (call);                                                        \

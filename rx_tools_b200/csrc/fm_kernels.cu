@@ -2809,6 +2809,22 @@ static int fm_plan_back(const rxb200_fm *h, long long n, FmBackPlan *b)
 	return RXB200_OK;
 }
 
+// whether a call runs the per-chunk reduction stages (fm_prepasses) before its main pass
+static bool fm_chunk_stages(const FmDev &dv) { return dv.rdc_on || dv.squelch || dv.adc_on || dv.levels; }
+
+// the pre-passes' chunk table -- [0]: complex per chunk, [1]: decimated per chunk, [2]: PCM per chunk, [3]: lp_len --
+// and the refusal of a call in which a chunk produces no decimated sample
+static int fm_chunk_table(rxb200_fm *h, size_t n_int16, size_t chunk_int16, std::vector<int> &lens)
+{
+	const size_t n_chunks = (n_int16 + chunk_int16 - 1) / chunk_int16;
+	lens.assign(n_chunks * 4, 0);
+	fm_count_outputs(h, n_int16, chunk_int16, nullptr, lens.data(), false);   // -o was checked before the launch
+	for (size_t ci = 0; ci < n_chunks; ci++) {
+		if (lens[n_chunks + ci] < 1) { set_error("a chunk produces no decimated sample"); return RXB200_EUNSUPPORTED; }
+	}
+	return RXB200_OK;
+}
+
 // per-chunk scalars: sizes (closed form), accumulators, then one recurrence per stage in the reference's order: raw DC
 // block -> squelch (sees the DC-blocked data, its sums from pass(1)) -> audio DC block (sums from pass(2))
 template <typename Pass>
@@ -2824,11 +2840,7 @@ static int fm_prepasses(rxb200_fm *h, FmCall &k, size_t n_int16, size_t chunk_in
 	RXB_CUDA(fm_reserve(h->d_levels, h->levels_cap, cells));
 	RXB_CUDA(fm_reserve(h->d_lens, h->lens_cap, (size_t)n_chunks * 4));
 	RXB_CUDA(cudaStreamSynchronize(h->stream));   // the previous call may still be reading the host vector
-	h->h_lens.assign((size_t)n_chunks * 4, 0);     // [0]: complex per chunk, [1]: decimated per chunk, [2]: PCM per chunk, [3]: lp_len
-	fm_count_outputs(h, n_int16, chunk_int16, nullptr, h->h_lens.data(), false);   // -o was checked before the launch
-	for (int ci = 0; ci < n_chunks; ci++) {
-		if (h->h_lens[(size_t)n_chunks + ci] < 1) { set_error("a chunk produces no decimated sample"); return RXB200_EUNSUPPORTED; }
-	}
+	if (const int rc = fm_chunk_table(h, n_int16, chunk_int16, h->h_lens); rc != RXB200_OK) { return rc; }
 	RXB_CUDA(cudaMemcpyAsync(h->d_lens, h->h_lens.data(), h->h_lens.size() * sizeof(int), cudaMemcpyHostToDevice, h->stream));
 	const unsigned cb = (unsigned)((h->n_channels + 63) / 64);
 	if (dv.rdc_on) {
@@ -2929,7 +2941,7 @@ static int fm_launch(rxb200_fm *h, const int16_t *d_in, size_t n_int16, size_t c
 		launches++;
 		return RXB200_OK;
 	};
-	if (dv.rdc_on || dv.squelch || dv.adc_on || dv.levels) {
+	if (fm_chunk_stages(dv)) {
 		rc = fm_prepasses(h, k, n_int16, chunk_int16, pass, &launches);
 		if (rc != RXB200_OK) { return rc; }
 	}
@@ -2976,6 +2988,16 @@ static int fm_prologue(rxb200_fm *h, const void *in, const void *out, size_t n_i
 	if (*total > pcm_stride) { set_error("pcm_stride %zu < %zu outputs", pcm_stride, *total); return RXB200_ECAPACITY; }
 	if (*any && !h->kern_any) { set_error("no any-length kernel for downsample_passes %d in this build", h->dev.P); return RXB200_EUNSUPPORTED; }
 	return RXB200_OK;
+}
+
+int rxb::fm_check_host_call(rxb200_fm *h, const int16_t *cs16, size_t n_int16, size_t chunk_int16, int16_t *pcm,
+                            size_t pcm_stride, int *chunk_result_len, size_t *n_pcm, bool read, size_t *total)
+{
+	bool any = false;
+	const int rc = fm_prologue(h, cs16, pcm, n_int16, chunk_int16, pcm_stride, chunk_result_len, total, n_pcm, read, false, &any);
+	if (rc != RXB200_OK || n_int16 == 0 || !fm_chunk_stages(h->dev)) { return rc; }
+	std::vector<int> lens;
+	return fm_chunk_table(h, n_int16, chunk_int16, lens);
 }
 
 static int fm_process_device(rxb200_fm *h, const int16_t *d_cs16, size_t n_int16, size_t chunk_int16, int16_t *d_pcm,

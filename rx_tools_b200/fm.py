@@ -181,6 +181,89 @@ class FmDemod:
         return d
 
 
+class FmGroup:
+    """``n_channels`` streams split over several GPUs (``rxb200_fm_group_*``): member i owns a contiguous block of the
+    channels and its own ``rxb200_fm`` handle; the group's results are byte for byte those of one ``FmDemod`` with all
+    the channels.  devices: one CUDA ordinal per member (may repeat), or None for ``range(n_dev)``."""
+
+    def __init__(self, params, n_channels: int, devices=None, n_dev: Optional[int] = None):
+        self.params = FmParams.from_any(params)
+        self.n_channels = n_channels
+        devs = None if devices is None else np.ascontiguousarray(devices, dtype=np.int32)
+        self.n_dev = len(devs) if devs is not None else int(n_dev or 1)
+        self._g = C.c_void_p()
+        pc = self.params.to_c()
+        dp = None if devs is None else devs.ctypes.data_as(C.POINTER(C.c_int))
+        _lib.check(_lib.lib().rxb200_fm_group_create(C.byref(pc), n_channels, self.n_dev, dp, C.byref(self._g)))
+
+    def close(self) -> None:
+        if _lib is not None and getattr(self, "_g", None) is not None and self._g:
+            _lib.lib().rxb200_fm_group_destroy(self._g)
+            self._g = None
+
+    __del__ = close
+
+    def member(self, i: int) -> int:
+        """Member i's rxb200_fm handle as an integer, 0 for a member that owns no channel."""
+        return int(_lib.lib().rxb200_fm_group_member(self._g, i) or 0)
+
+    def reset(self) -> None:
+        _lib.check(_lib.lib().rxb200_fm_group_reset(self._g))
+
+    def _cap(self, n_int16: int, chunk_int16: int) -> int:
+        return int(_lib.lib().rxb200_fm_max_output(C.c_void_p(self.member(0)), n_int16, chunk_int16)) + 8
+
+    def _input(self, cs16):
+        x = np.ascontiguousarray(cs16, dtype=np.int16)
+        x2 = x.reshape(1, -1) if x.ndim == 1 else x
+        assert x2.shape[0] == self.n_channels, (x2.shape, self.n_channels)
+        return x2, x.ndim == 1
+
+    def full_demod(self, cs16: np.ndarray, chunk_int16: int = MAXIMUM_BUF_LENGTH, return_chunks: bool = False):
+        """As ``FmDemod.full_demod`` (``rxb200_fm_group_process``)."""
+        x2, single = self._input(cs16)
+        n_int16 = x2.shape[1]
+        cap = self._cap(n_int16, chunk_int16)
+        out = np.empty((self.n_channels, cap), dtype=np.int16)
+        lens = np.zeros(max(1, -(-n_int16 // chunk_int16)), dtype=np.int32)
+        n_pcm = C.c_size_t(0)
+        _lib.check(_lib.lib().rxb200_fm_group_process(self._g, x2.ctypes.data, n_int16, chunk_int16, out.ctypes.data, cap,
+                                                      C.byref(n_pcm), lens.ctypes.data_as(C.POINTER(C.c_int))))
+        res = out[:, :n_pcm.value].copy()
+        res = res[0] if single else res
+        return (res, lens) if return_chunks else res
+
+    def process_read(self, cs16: np.ndarray) -> np.ndarray:
+        """As ``FmDemod.process_read`` (``rxb200_fm_group_process_read``)."""
+        x2, single = self._input(cs16)
+        n_int16 = x2.shape[1]
+        cap = self._cap(n_int16, max(n_int16, 1))
+        out = np.empty((self.n_channels, cap), dtype=np.int16)
+        n_pcm = C.c_size_t(0)
+        _lib.check(_lib.lib().rxb200_fm_group_process_read(self._g, x2.ctypes.data, n_int16, out.ctypes.data, cap,
+                                                           C.byref(n_pcm)))
+        res = out[:, :n_pcm.value].copy()
+        return res[0] if single else res
+
+    def squelch_hits(self) -> np.ndarray:
+        """demod.squelch_hits of every channel after the last call, int32[n_channels]."""
+        h = np.zeros(self.n_channels, dtype=np.int32)
+        _lib.check(_lib.lib().rxb200_fm_group_squelch_hits(self._g, h.ctypes.data_as(C.POINTER(C.c_int))))
+        return h
+
+    def levels(self) -> np.ndarray:
+        """As ``FmDemod.levels``: int32[n_channels][n_chunks] of the last call (needs report_levels)."""
+        n = C.c_size_t(0)
+        rc = _lib.lib().rxb200_fm_group_levels(self._g, np.zeros(1, np.int32).ctypes.data_as(C.POINTER(C.c_int)), 0,
+                                               C.byref(n))
+        if rc != _lib.ECAPACITY:
+            _lib.check(rc)
+        buf = np.zeros((self.n_channels, int(n.value)), dtype=np.int32)
+        _lib.check(_lib.lib().rxb200_fm_group_levels(self._g, buf.ctypes.data_as(C.POINTER(C.c_int)), buf.size,
+                                                     C.byref(n)))
+        return buf
+
+
 # ---- rx_sdr sample-format conversions (src/rtl_sdr.c:348-391) -------------------------------------------
 CVT_CS16_CS8, CVT_CS16_CU8, CVT_CS16_CF32, CVT_CS12_CS16 = range(4)
 
