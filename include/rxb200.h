@@ -373,6 +373,60 @@ int rxb200_fm_group_squelch_hits(rxb200_fm_group *g, int *hits /* n_channels */)
 int rxb200_fm_group_levels(rxb200_fm_group *g, int *levels, size_t cap, size_t *n_chunks);
 int rxb200_fm_group_reset(rxb200_fm_group *g);
 
+/* ======================================================================== rx_fm channels of one capture
+ * Several channels of ONE wideband CS16 capture: channel k is the reference's rtlsdr_callback() + full_demod() run on
+ * mix_k(x), what a tuner set f_k (Hz) away from the capture's centre would have delivered (DESIGN.md section 4.4).  The
+ * integer mixer, for a capture rate R (Hz, > 0) and an offset f with |f| < R/2:
+ *   period L = R / gcd(R, |f|) complex samples (1 for f = 0), at most 2^20 (RXB200_EUNSUPPORTED beyond);
+ *   table entry m = (c, s) = ((int)round(32768 cos t), (int)round(32768 sin t)), t = -2 pi r / R in fp64, where
+ *     r = (m f) mod R taken in 64-bit integers as the representative in (-R/2, R/2] (the same angle modulo 2 pi; it
+ *     makes the tables of f and -f exact conjugates);
+ *   complex sample n of the stream (counted from create or reset, across calls) uses entry p = (phase + n) mod L:
+ *     I' = (int16)((I c - Q s + 2^14) >> 15),  Q' = (int16)((I s + Q c + 2^14) >> 15)   (arithmetic shift, int16 wrap).
+ * Unity 2^15 makes f = 0 the identity and f = +-R/4 an exact rotation.  Then the chain runs as configured: pick
+ * offset_tuning = 1 (the mixer already put the channel at DC, so rotate16_90 should not run) and downsample =
+ * R / rate_in, so the boxcar is the channel filter. */
+
+/* The mixer table of (R, f): table receives 2*L int32 (c, s pairs), *period receives L.  RXB200_EINVAL for R <= 0 or
+ * |f| >= R/2, RXB200_EUNSUPPORTED for L > 2^20, RXB200_ECAPACITY (with *period set) when cap < 2*L int32. */
+int rxb200_fm_mix_table(int capture_rate, int offset_hz, int32_t *table, size_t cap, size_t *period);
+/* The mixer alone on DEVICE pointers, on `stream` (a cudaStream_t, may be NULL): n_complex samples of d_src, starting
+ * at table entry phase mod L (phase >= 0), to d_dst.  Both pointers 4-byte aligned; 16-byte aligned ones take vector
+ * loads and stores.  Asynchronous. */
+int rxb200_mix_device(int capture_rate, int offset_hz, long long phase, const int16_t *d_src, size_t n_complex,
+                      int16_t *d_dst, void *stream);
+
+/* A handle of n_channels channels of one capture: one rxb200_fm handle with n_channels channels (the member) plus the
+ * mixer of each channel, whose phases start at 0.  Every call takes ONE input stream: the capture's n_int16 int16.
+ * fm_mix_kernel reads it once and writes the n_channels mixed streams to a scratch buffer of the handle ([n_channels]
+ * [n_int16], rows n_int16 apart from a 256-byte aligned base); the member's rxb200_fm_process_device / _read_device
+ * then runs on that buffer, so every kernel route, carry, statistic and result of the member is that of a plain handle
+ * fed the mixed streams.  pcm, pcm_stride, n_pcm and chunk_result_len are those of rxb200_fm_process*, channel k's PCM
+ * at pcm + k*pcm_stride.  Refusals are those of the matching rxb200_fm_process* call, checked before anything is
+ * launched, except that a device capture needs only 4-byte alignment; a refused call changes neither the phases nor
+ * the member's state.  A successful call advances every phase by its n_int16 / 2 complex samples. */
+typedef struct rxb200_fm_mix rxb200_fm_mix;
+int rxb200_fm_mix_create(const rxb200_fm_params *params, int capture_rate, const int *offsets_hz, int n_channels,
+                         int device, rxb200_fm_mix **out);
+void rxb200_fm_mix_destroy(rxb200_fm_mix *m);
+/* phases back to 0 and the member back to the state right after create */
+int rxb200_fm_mix_reset(rxb200_fm_mix *m);
+/* the inner handle, for rxb200_fm_last_stats / _kernel_ms / _tune / _stream (and the mixer runs on its stream) */
+rxb200_fm *rxb200_fm_mix_member(rxb200_fm_mix *m);
+int rxb200_fm_mix_process(rxb200_fm_mix *m, const int16_t *cs16, size_t n_int16, size_t chunk_int16, int16_t *pcm,
+                          size_t pcm_stride, size_t *n_pcm, int *chunk_result_len);
+int rxb200_fm_mix_process_device(rxb200_fm_mix *m, const int16_t *d_cs16, size_t n_int16, size_t chunk_int16,
+                                 int16_t *d_pcm, size_t pcm_stride, size_t *n_pcm, int sync);
+int rxb200_fm_mix_process_read(rxb200_fm_mix *m, const int16_t *cs16, size_t n_int16, int16_t *pcm, size_t pcm_stride,
+                               size_t *n_pcm);
+int rxb200_fm_mix_process_read_device(rxb200_fm_mix *m, const int16_t *d_cs16, size_t n_int16, int16_t *d_pcm,
+                                      size_t pcm_stride, size_t *n_pcm, int sync);
+int rxb200_fm_mix_squelch_hits(rxb200_fm_mix *m, int *hits /* n_channels */);
+int rxb200_fm_mix_levels(rxb200_fm_mix *m, int *levels, size_t cap, size_t *n_chunks);
+/* Device time (CUDA events on the member's stream) of the last successful call's fm_mix_kernel, in milliseconds;
+ * synchronises the stream. */
+int rxb200_fm_mix_kernel_ms(rxb200_fm_mix *m, float *ms);
+
 /* ======================================================================== rx_sdr (SURVEY.md §8f row 4)
  * The pointwise sample-format conversions of rx_sdr's recorder loop (src/rtl_sdr.c:348-391):
  *   RXB200_CVT_CS16_CS8  : (uint8_t)(int)(x/32767.0*128.0+0.4)       per int16 (:367-370)

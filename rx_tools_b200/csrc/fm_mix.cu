@@ -1,0 +1,354 @@
+// fm_mix.cu — several rx_fm channels of one wideband capture (include/rxb200.h, "rx_fm channels of one capture").
+// fm_mix_kernel mixes the capture to baseband once per channel with that channel's integer table, reading the capture
+// once and writing one CS16 stream per channel; a plain rxb200_fm handle with one channel per stream then runs the
+// chain on them through its device entry points.  The chain itself is not touched here.
+#include <algorithm>
+#include <new>
+#include <vector>
+#include "common.cuh"
+
+namespace rxb {
+
+#define MIX_THREADS 256
+#define MIX_UNIT 8                   // complex samples per thread and trip: 32 bytes of capture
+#define MIX_GROUP 256                // channels per grid row (blockIdx.y): the capture is read once per group
+#define MIX_SMEM_MAX (96 * 1024)     // the largest table range a CTA stages in shared memory; beyond, reads go through L1
+
+struct MixChan {
+	int off;         // first entry of the channel's table in the concatenated tables
+	int L;           // period
+	unsigned m;      // floor((2^32 - 1) / L): t mod L for t < 2^21 with one multiply-high and one correction
+	int pad;
+};
+
+// one complex sample through the mixer: (I + jQ)(c + js) in Q15, rounded, arithmetic shift, int16 wrap
+__device__ __forceinline__ uint32_t mix_one(uint32_t w, int2 cs)
+{
+	const int I = (int)(int16_t)(w & 0xffffu), Q = (int)(int16_t)(w >> 16);
+	const int i2 = (I * cs.x - Q * cs.y + 16384) >> 15;      // |x| |(c, s)| sqrt(2) < 2^31: no overflow
+	const int q2 = (I * cs.y + Q * cs.x + 16384) >> 15;
+	return ((uint32_t)i2 & 0xffffu) | ((uint32_t)q2 << 16);
+}
+
+// Grid-stride over units of MIX_UNIT complex samples: each thread loads its unit once, then writes it mixed with every
+// channel of its group.  Stream row c of dst is dst + c*dst_stride; sample n of the call uses entry (pos + n) mod L of
+// its channel.  VEC: src, dst and the row stride are 16-byte aligned, a whole unit moves as two 16-byte vectors (the
+// call's last, partial unit and every unit otherwise move 4 bytes at a time).  SMEM: the group's tables are staged in
+// shared memory.
+template <bool VEC, bool SMEM>
+__global__ void __launch_bounds__(MIX_THREADS) fm_mix_kernel(const int16_t *__restrict__ src, long long n,
+                                                            int16_t *__restrict__ dst, long long dst_stride,
+                                                            const int2 *__restrict__ tab, const MixChan *__restrict__ chan,
+                                                            int n_ch, unsigned long long pos)
+{
+	__shared__ MixChan s_ch[MIX_GROUP];
+	__shared__ int s_q[MIX_GROUP];          // each channel's table entry at the trip's first sample
+	extern __shared__ int2 s_tab[];
+	const int c0 = (int)blockIdx.y * MIX_GROUP;
+	const int nc = min(MIX_GROUP, n_ch - c0);
+	for (int c = threadIdx.x; c < nc; c += blockDim.x) { s_ch[c] = chan[c0 + c]; }
+	__syncthreads();
+	const int lo = s_ch[0].off;             // the group's tables are one range of the concatenated tables
+	if (SMEM) {
+		const int hi = s_ch[nc - 1].off + s_ch[nc - 1].L;
+		for (int e = threadIdx.x; e < hi - lo; e += blockDim.x) { s_tab[e] = tab[lo + e]; }
+	}
+	const long long units = (n + MIX_UNIT - 1) / MIX_UNIT;
+	for (long long u0 = (long long)blockIdx.x * blockDim.x; u0 < units; u0 += (long long)gridDim.x * blockDim.x) {
+		__syncthreads();                    // the previous trip is done with s_q (and the first trip sees the tables)
+		const unsigned long long first = pos + (unsigned long long)u0 * MIX_UNIT;
+		for (int c = threadIdx.x; c < nc; c += blockDim.x) { s_q[c] = (int)(first % (unsigned long long)s_ch[c].L); }
+		__syncthreads();
+		const long long u = u0 + threadIdx.x;
+		if (u >= units) { continue; }
+		const long long s = u * MIX_UNIT;
+		const int cnt = n - s < MIX_UNIT ? (int)(n - s) : MIX_UNIT;
+		const bool vec = VEC && cnt == MIX_UNIT;
+		const uint32_t *in = reinterpret_cast<const uint32_t *>(src) + s;
+		uint32_t w[MIX_UNIT];
+		if (vec) {
+			const uint4 a = __ldg(reinterpret_cast<const uint4 *>(in)), b = __ldg(reinterpret_cast<const uint4 *>(in) + 1);
+			w[0] = a.x; w[1] = a.y; w[2] = a.z; w[3] = a.w; w[4] = b.x; w[5] = b.y; w[6] = b.z; w[7] = b.w;
+		} else {
+#pragma unroll
+			for (int j = 0; j < MIX_UNIT; j++) { w[j] = j < cnt ? __ldg(in + j) : 0u; }
+		}
+		for (int c = 0; c < nc; c++) {
+			const MixChan ch = s_ch[c];
+			const unsigned L = (unsigned)ch.L;
+			const unsigned t = (unsigned)s_q[c] + (unsigned)threadIdx.x * MIX_UNIT;   // < 2^20 + 2^11
+			unsigned p = t - __umulhi(t, ch.m) * L;                                    // the quotient is low by at most 1
+			if (p >= L) { p -= L; }
+			const int base = SMEM ? ch.off - lo : ch.off;
+			uint32_t o[MIX_UNIT];
+#pragma unroll
+			for (int j = 0; j < MIX_UNIT; j++) {
+				const int2 cs = SMEM ? s_tab[base + (int)p] : __ldg(tab + base + (int)p);
+				o[j] = mix_one(w[j], cs);
+				if (++p == L) { p = 0; }
+			}
+			uint32_t *row = reinterpret_cast<uint32_t *>(dst + (long long)(c0 + c) * dst_stride) + s;
+			if (vec) {
+				reinterpret_cast<uint4 *>(row)[0] = make_uint4(o[0], o[1], o[2], o[3]);
+				reinterpret_cast<uint4 *>(row)[1] = make_uint4(o[4], o[5], o[6], o[7]);
+			} else {
+#pragma unroll
+				for (int j = 0; j < MIX_UNIT; j++) { if (j < cnt) { row[j] = o[j]; } }
+			}
+		}
+	}
+}
+
+typedef void (*mix_kernel_fn)(const int16_t *, long long, int16_t *, long long, const int2 *, const MixChan *, int,
+                              unsigned long long);
+
+// Launches fm_mix_kernel on the current device: n complex samples of src to n_ch rows of dst, dst_stride int16 apart.
+// chan is the host copy of d_chan (for the table range each group stages).
+static int mix_launch(const int16_t *src, long long n, int16_t *dst, long long dst_stride, const int2 *d_tab,
+                      const MixChan *d_chan, const std::vector<MixChan> &chan, unsigned long long pos, cudaStream_t st)
+{
+	const int n_ch = (int)chan.size();
+	const int groups = (n_ch + MIX_GROUP - 1) / MIX_GROUP;
+	size_t smem = 0;
+	for (int g = 0; g < groups; g++) {
+		const MixChan &a = chan[(size_t)g * MIX_GROUP], &b = chan[(size_t)std::min(n_ch, (g + 1) * MIX_GROUP) - 1];
+		const size_t bytes = (size_t)(b.off + b.L - a.off) * sizeof(int2);
+		if (bytes > smem) { smem = bytes; }
+	}
+	const bool use_smem = smem <= MIX_SMEM_MAX;
+	if (!use_smem) { smem = 0; }
+	const bool vec = ((uintptr_t)src & 15u) == 0 && ((uintptr_t)dst & 15u) == 0 && ((size_t)dst_stride * 2) % 16 == 0;
+	const mix_kernel_fn kern = vec ? (use_smem ? fm_mix_kernel<true, true> : fm_mix_kernel<true, false>)
+	                               : (use_smem ? fm_mix_kernel<false, true> : fm_mix_kernel<false, false>);
+	if (use_smem) { RXB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, MIX_SMEM_MAX)); }
+	int dev = 0, n_sm = 0, per_sm = 0;
+	RXB_CUDA(cudaGetDevice(&dev));
+	RXB_CUDA(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
+	RXB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, MIX_THREADS, smem));
+	const long long units = (n + MIX_UNIT - 1) / MIX_UNIT;
+	long long bx = (units + MIX_THREADS - 1) / MIX_THREADS;
+	const long long fill = (long long)n_sm * (per_sm > 0 ? per_sm : 1) / groups;
+	if (bx > fill) { bx = fill > 0 ? fill : 1; }
+	kern<<<dim3((unsigned)bx, (unsigned)groups), MIX_THREADS, smem, st>>>(src, n, dst, dst_stride, d_tab, d_chan, n_ch, pos);
+	RXB_CUDA(cudaGetLastError());
+	return RXB200_OK;
+}
+
+static MixChan mix_chan(int off, size_t L)
+{
+	return MixChan{off, (int)L, (unsigned)(0xffffffffu / (unsigned)L), 0};
+}
+
+// the table of (R, f) into a vector; *period receives its length
+static int mix_table(int capture_rate, int offset_hz, std::vector<int32_t> &t, size_t *period)
+{
+	int rc = rxb200_fm_mix_table(capture_rate, offset_hz, nullptr, 0, period);
+	if (rc != RXB200_ECAPACITY) { return rc; }
+	t.resize(2 * *period);
+	return rxb200_fm_mix_table(capture_rate, offset_hz, t.data(), t.size(), period);
+}
+
+}  // namespace rxb
+using namespace rxb;
+
+struct rxb200_fm_mix {
+	rxb200_fm *h = nullptr;                      // the member: one channel per mixed stream
+	int device = 0;
+	int n_channels = 0;
+	std::vector<MixChan> chan;                   // host copy of d_chan
+	int2 *d_tab = nullptr;                       // every channel's table, concatenated
+	MixChan *d_chan = nullptr;
+	unsigned long long pos = 0;                  // complex samples since create or reset: channel k's phase is pos mod L_k
+	int16_t *d_cap = nullptr; size_t cap_cap = 0;   // host calls: the capture (int16 elements)
+	int16_t *d_mix = nullptr; size_t mix_cap = 0;   // the mixed streams, [n_channels][n_int16]
+	int16_t *d_out = nullptr; size_t out_cap = 0;   // host calls: the PCM rows, total + 8 apart
+	cudaEvent_t ev0 = nullptr, ev1 = nullptr;    // around the last fm_mix_kernel
+};
+
+namespace {
+
+template <typename T>
+cudaError_t reserve(T *&buf, size_t &cap, size_t need)
+{
+	if (need <= cap) { return cudaSuccess; }
+	cudaFree(buf); buf = nullptr; cap = 0;
+	const cudaError_t e = cudaMalloc(&buf, need * sizeof(T));
+	if (e == cudaSuccess) { cap = need; }
+	return e;
+}
+
+// One call of any process entry point.  device: cs16 and pcm are device pointers (the member's device entry point
+// writes pcm), else host pointers staged through the handle's buffers.  read: one read (chunk_int16 == n_int16).
+int mix_call(rxb200_fm_mix *m, const int16_t *cs16, size_t n_int16, size_t chunk_int16, int16_t *pcm, size_t pcm_stride,
+             size_t *n_pcm, int *chunk_result_len, bool read, bool device, int sync)
+{
+	if (!m) { set_error("null argument"); return RXB200_EINVAL; }
+	if (device && ((uintptr_t)cs16 & 3u) != 0) { set_error("d_cs16 must be 4-byte aligned"); return RXB200_EINVAL; }
+	// the member's own refusals, on the shape its call will see (the mixed streams sit in an aligned buffer)
+	size_t total = 0;
+	int rc = rxb::fm_check_host_call(m->h, cs16, n_int16, chunk_int16, pcm, pcm_stride, chunk_result_len, n_pcm, read,
+	                                 &total);
+	if (rc != RXB200_OK || n_int16 == 0) { return rc; }
+	RXB_CUDA(cudaSetDevice(m->device));
+	const cudaStream_t st = (cudaStream_t)rxb200_fm_stream(m->h);
+	const size_t K = (size_t)m->n_channels;
+	RXB_CUDA(reserve(m->d_mix, m->mix_cap, n_int16 * K));
+	const int16_t *src = cs16;
+	if (!device) {
+		RXB_CUDA(reserve(m->d_cap, m->cap_cap, n_int16));
+		RXB_CUDA(reserve(m->d_out, m->out_cap, (total + 8) * K));
+		RXB_CUDA(cudaMemcpyAsync(m->d_cap, cs16, n_int16 * sizeof(int16_t), cudaMemcpyHostToDevice, st));
+		src = m->d_cap;
+	}
+	RXB_CUDA(cudaEventRecord(m->ev0, st));
+	rc = mix_launch(src, (long long)(n_int16 / 2), m->d_mix, (long long)n_int16, m->d_tab, m->d_chan, m->chan, m->pos, st);
+	if (rc != RXB200_OK) { return rc; }
+	RXB_CUDA(cudaEventRecord(m->ev1, st));
+	int16_t *out = device ? pcm : m->d_out;
+	const size_t stride = device ? pcm_stride : total + 8;
+	size_t n = 0;
+	rc = read ? rxb200_fm_process_read_device(m->h, m->d_mix, n_int16, out, stride, &n, device ? sync : 0)
+	          : rxb200_fm_process_device(m->h, m->d_mix, n_int16, chunk_int16, out, stride, &n, device ? sync : 0);
+	if (rc != RXB200_OK) { return rc; }
+	if (!device) {
+		if (total) {
+			RXB_CUDA(cudaMemcpy2DAsync(pcm, pcm_stride * sizeof(int16_t), m->d_out, (total + 8) * sizeof(int16_t),
+			                           total * sizeof(int16_t), K, cudaMemcpyDeviceToHost, st));
+		}
+		RXB_CUDA(cudaStreamSynchronize(st));
+	}
+	m->pos += n_int16 / 2;
+	if (n_pcm) { *n_pcm = total; }
+	return RXB200_OK;
+}
+
+}  // namespace
+
+extern "C" int rxb200_mix_device(int capture_rate, int offset_hz, long long phase, const int16_t *d_src, size_t n_complex,
+                                 int16_t *d_dst, void *stream)
+{
+	if (!d_src || !d_dst || phase < 0) { set_error("bad mix request (null pointer or negative phase)"); return RXB200_EINVAL; }
+	if (((uintptr_t)d_src & 3u) || ((uintptr_t)d_dst & 3u)) { set_error("pointers must be 4-byte aligned"); return RXB200_EINVAL; }
+	std::vector<int32_t> t;
+	size_t L = 0;
+	int rc = mix_table(capture_rate, offset_hz, t, &L);
+	if (rc != RXB200_OK || n_complex == 0) { return rc; }
+	const cudaStream_t st = (cudaStream_t)stream;
+	const std::vector<MixChan> chan(1, mix_chan(0, L));
+	int2 *d_tab = nullptr;
+	MixChan *d_chan = nullptr;
+	RXB_CUDA(cudaMallocAsync(&d_tab, L * sizeof(int2), st));
+	if (cudaMallocAsync(&d_chan, sizeof(MixChan), st) != cudaSuccess) {
+		cudaFreeAsync(d_tab, st); set_error("cudaMallocAsync failed"); return RXB200_ECUDA;
+	}
+	// from pageable memory: each copy has read its source when it returns
+	if (cudaMemcpyAsync(d_tab, t.data(), L * sizeof(int2), cudaMemcpyHostToDevice, st) != cudaSuccess ||
+	    cudaMemcpyAsync(d_chan, chan.data(), sizeof(MixChan), cudaMemcpyHostToDevice, st) != cudaSuccess) {
+		set_error("table upload failed: %s", cudaGetErrorString(cudaGetLastError()));
+		rc = RXB200_ECUDA;
+	}
+	if (rc == RXB200_OK) {
+		rc = mix_launch(d_src, (long long)n_complex, d_dst, 0, d_tab, d_chan, chan, (unsigned long long)phase % L, st);
+	}
+	cudaFreeAsync(d_tab, st);
+	cudaFreeAsync(d_chan, st);
+	return rc;
+}
+
+extern "C" void rxb200_fm_mix_destroy(rxb200_fm_mix *m)
+{
+	if (!m) { return; }
+	rxb200_fm_destroy(m->h);   // synchronises the stream the mixer runs on
+	cudaSetDevice(m->device);
+	cudaFree(m->d_tab); cudaFree(m->d_chan); cudaFree(m->d_cap); cudaFree(m->d_mix); cudaFree(m->d_out);
+	if (m->ev0) { cudaEventDestroy(m->ev0); }
+	if (m->ev1) { cudaEventDestroy(m->ev1); }
+	delete m;
+}
+
+extern "C" int rxb200_fm_mix_create(const rxb200_fm_params *params, int capture_rate, const int *offsets_hz,
+                                    int n_channels, int device, rxb200_fm_mix **out)
+{
+	if (!params || !offsets_hz || !out || n_channels < 1) { set_error("bad mix arguments (n_channels >= 1)"); return RXB200_EINVAL; }
+	*out = nullptr;
+	// every table first: a refused offset fails before any device work
+	std::vector<int32_t> all, t;
+	std::vector<MixChan> chan;
+	for (int k = 0; k < n_channels; k++) {
+		size_t L = 0;
+		const int rc = mix_table(capture_rate, offsets_hz[k], t, &L);
+		if (rc != RXB200_OK) { return rc; }
+		if (all.size() / 2 + L > (size_t)INT32_MAX) { set_error("mixer tables beyond 2^31 entries"); return RXB200_EUNSUPPORTED; }
+		chan.push_back(mix_chan((int)(all.size() / 2), L));
+		all.insert(all.end(), t.begin(), t.end());
+	}
+	rxb200_fm_mix *m = new (std::nothrow) rxb200_fm_mix();
+	if (!m) { return RXB200_ENOMEM; }
+	m->device = device;
+	m->n_channels = n_channels;
+	m->chan = chan;
+	const int rc = rxb200_fm_create(params, device, n_channels, &m->h);
+	if (rc != RXB200_OK) { delete m; return rc; }
+	RXB_CUDA_OR(cudaSetDevice(device), rxb200_fm_mix_destroy(m));
+	RXB_CUDA_OR(cudaMalloc(&m->d_tab, all.size() * sizeof(int32_t)), rxb200_fm_mix_destroy(m));
+	RXB_CUDA_OR(cudaMalloc(&m->d_chan, chan.size() * sizeof(MixChan)), rxb200_fm_mix_destroy(m));
+	RXB_CUDA_OR(cudaMemcpy(m->d_tab, all.data(), all.size() * sizeof(int32_t), cudaMemcpyHostToDevice), rxb200_fm_mix_destroy(m));
+	RXB_CUDA_OR(cudaMemcpy(m->d_chan, chan.data(), chan.size() * sizeof(MixChan), cudaMemcpyHostToDevice), rxb200_fm_mix_destroy(m));
+	RXB_CUDA_OR(cudaEventCreate(&m->ev0), rxb200_fm_mix_destroy(m));
+	RXB_CUDA_OR(cudaEventCreate(&m->ev1), rxb200_fm_mix_destroy(m));
+	*out = m;
+	return RXB200_OK;
+}
+
+extern "C" int rxb200_fm_mix_reset(rxb200_fm_mix *m)
+{
+	if (!m) { return RXB200_EINVAL; }
+	const int rc = rxb200_fm_reset(m->h);
+	if (rc == RXB200_OK) { m->pos = 0; }
+	return rc;
+}
+
+extern "C" rxb200_fm *rxb200_fm_mix_member(rxb200_fm_mix *m) { return m ? m->h : nullptr; }
+
+extern "C" int rxb200_fm_mix_process(rxb200_fm_mix *m, const int16_t *cs16, size_t n_int16, size_t chunk_int16,
+                                     int16_t *pcm, size_t pcm_stride, size_t *n_pcm, int *chunk_result_len)
+{
+	return mix_call(m, cs16, n_int16, chunk_int16, pcm, pcm_stride, n_pcm, chunk_result_len, false, false, 1);
+}
+
+extern "C" int rxb200_fm_mix_process_device(rxb200_fm_mix *m, const int16_t *d_cs16, size_t n_int16, size_t chunk_int16,
+                                            int16_t *d_pcm, size_t pcm_stride, size_t *n_pcm, int sync)
+{
+	return mix_call(m, d_cs16, n_int16, chunk_int16, d_pcm, pcm_stride, n_pcm, nullptr, false, true, sync);
+}
+
+extern "C" int rxb200_fm_mix_process_read(rxb200_fm_mix *m, const int16_t *cs16, size_t n_int16, int16_t *pcm,
+                                          size_t pcm_stride, size_t *n_pcm)
+{
+	return mix_call(m, cs16, n_int16, n_int16, pcm, pcm_stride, n_pcm, nullptr, true, false, 1);
+}
+
+extern "C" int rxb200_fm_mix_process_read_device(rxb200_fm_mix *m, const int16_t *d_cs16, size_t n_int16, int16_t *d_pcm,
+                                                 size_t pcm_stride, size_t *n_pcm, int sync)
+{
+	return mix_call(m, d_cs16, n_int16, n_int16, d_pcm, pcm_stride, n_pcm, nullptr, true, true, sync);
+}
+
+extern "C" int rxb200_fm_mix_squelch_hits(rxb200_fm_mix *m, int *hits)
+{
+	return m ? rxb200_fm_squelch_hits(m->h, hits) : RXB200_EINVAL;
+}
+
+extern "C" int rxb200_fm_mix_levels(rxb200_fm_mix *m, int *levels, size_t cap, size_t *n_chunks)
+{
+	return m ? rxb200_fm_levels(m->h, levels, cap, n_chunks) : RXB200_EINVAL;
+}
+
+extern "C" int rxb200_fm_mix_kernel_ms(rxb200_fm_mix *m, float *ms)
+{
+	if (!m || !ms) { return RXB200_EINVAL; }
+	RXB_CUDA(cudaSetDevice(m->device));
+	RXB_CUDA(cudaEventSynchronize(m->ev1));
+	RXB_CUDA(cudaEventElapsedTime(ms, m->ev0, m->ev1));
+	return RXB200_OK;
+}

@@ -88,6 +88,31 @@ extern "C" int rxb200_fm_derive(const rxb200_fm_cli *cli, rxb200_fm_derived *out
 	return RXB200_OK;
 }
 
+// The mixer table of a channel f Hz away from the centre of a capture at R Hz (include/rxb200.h, "rx_fm channels of one
+// capture"): Q15 with unity 2^15, one entry per complex sample of the period R / gcd(R, |f|).  The angle's residue is
+// exact (64-bit integers); only cos / sin of it are fp64, and its symmetric representative makes f and -f conjugates.
+#define RXB_MIX_MAX_PERIOD (1 << 20)
+extern "C" int rxb200_fm_mix_table(int capture_rate, int offset_hz, int32_t *table, size_t cap, size_t *period)
+{
+	if (!period) { set_error("null argument"); return RXB200_EINVAL; }
+	const long long R = capture_rate, f = offset_hz;
+	if (R <= 0 || 2 * (f < 0 ? -f : f) >= R) { set_error("mixer needs capture_rate > 0 and |offset| < capture_rate/2 (%d, %d)", capture_rate, offset_hz); return RXB200_EINVAL; }
+	long long a = R, b = f < 0 ? -f : f;
+	while (b) { const long long t = a % b; a = b; b = t; }
+	const long long L = R / a;
+	if (L > RXB_MIX_MAX_PERIOD) { set_error("mixer period %lld > 2^20 samples (capture_rate %d, offset %d)", L, capture_rate, offset_hz); return RXB200_EUNSUPPORTED; }
+	*period = (size_t)L;
+	if (!table || cap < 2 * (size_t)L) { set_error("mixer table capacity %zu < %lld", cap, 2 * L); return RXB200_ECAPACITY; }
+	for (long long m = 0; m < L; m++) {
+		long long r = ((m * f) % R + R) % R;          // |m f| < 2^20 * 2^31: no overflow
+		if (2 * r > R) { r -= R; }                      // (-R/2, R/2]
+		const double t = -2.0 * M_PI * (double)r / (double)R;
+		table[2 * m] = (int32_t)round(32768.0 * cos(t));
+		table[2 * m + 1] = (int32_t)round(32768.0 * sin(t));
+	}
+	return RXB200_OK;
+}
+
 // ---------------------------------------------------------------------------------- rx_power
 #define RXB_MAXIMUM_RATE 2800000      /* src/rtl_power.c:74 */
 #define RXB_MINIMUM_RATE 1000000      /* :75 */

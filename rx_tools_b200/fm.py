@@ -264,6 +264,141 @@ class FmGroup:
         return buf
 
 
+# ---- several channels of one capture (rxb200_fm_mix_*) ------------------------------------------------------
+def mix_table(capture_rate: int, offset_hz: int) -> np.ndarray:
+    """The integer mixer of a channel offset_hz away from the centre of a capture at capture_rate:
+    int32[period][2] of (c, s) in Q15 with unity 2^15 (``rxb200_fm_mix_table``)."""
+    period = C.c_size_t(0)
+    rc = _lib.lib().rxb200_fm_mix_table(capture_rate, offset_hz, None, 0, C.byref(period))
+    if rc != _lib.ECAPACITY:
+        _lib.check(rc)
+    t = np.zeros((int(period.value), 2), dtype=np.int32)
+    _lib.check(_lib.lib().rxb200_fm_mix_table(capture_rate, offset_hz, t.ctypes.data_as(C.POINTER(C.c_int32)), t.size,
+                                              C.byref(period)))
+    return t
+
+
+def mix_device(capture_rate: int, offset_hz: int, phase: int, d_src_ptr: int, n_complex: int, d_dst_ptr: int,
+               stream: int = 0) -> None:
+    """The mixer alone on device pointers (``rxb200_mix_device``), asynchronous on ``stream``."""
+    _lib.check(_lib.lib().rxb200_mix_device(capture_rate, offset_hz, phase, d_src_ptr, n_complex, d_dst_ptr,
+                                            stream or None))
+
+
+class FmMix:
+    """``len(offsets_hz)`` channels of ONE CS16 capture at ``capture_rate`` (``rxb200_fm_mix_*``): channel k is
+    ``FmDemod`` run on the capture mixed down by ``offsets_hz[k]`` with ``mix_table``; the mixers' phases carry across
+    calls.  Every call takes the one capture, int16[n_int16], and returns int16[n_channels][n_pcm]."""
+
+    def __init__(self, params, capture_rate: int, offsets_hz, device: int = 0):
+        self.params = FmParams.from_any(params)
+        self.capture_rate = capture_rate
+        offs = np.ascontiguousarray(offsets_hz, dtype=np.int32)
+        self.offsets_hz = offs.tolist()
+        self.n_channels = len(offs)
+        self._m = C.c_void_p()
+        pc = self.params.to_c()
+        _lib.check(_lib.lib().rxb200_fm_mix_create(C.byref(pc), capture_rate, offs.ctypes.data_as(C.POINTER(C.c_int)),
+                                                   self.n_channels, device, C.byref(self._m)))
+
+    def close(self) -> None:
+        if _lib is not None and getattr(self, "_m", None) is not None and self._m:
+            _lib.lib().rxb200_fm_mix_destroy(self._m)
+            self._m = None
+
+    __del__ = close
+
+    def member(self) -> int:
+        """The inner rxb200_fm handle (one channel per mixed stream) as an integer."""
+        return int(_lib.lib().rxb200_fm_mix_member(self._m) or 0)
+
+    def reset(self) -> None:
+        _lib.check(_lib.lib().rxb200_fm_mix_reset(self._m))
+
+    def _cap(self, n_int16: int, chunk_int16: int) -> int:
+        return int(_lib.lib().rxb200_fm_max_output(C.c_void_p(self.member()), n_int16, chunk_int16)) + 8
+
+    def full_demod(self, cs16: np.ndarray, chunk_int16: int = MAXIMUM_BUF_LENGTH, return_chunks: bool = False):
+        """As ``FmDemod.full_demod`` on every channel (``rxb200_fm_mix_process``); cs16: the capture, int16[n_int16]."""
+        x = np.ascontiguousarray(cs16, dtype=np.int16).reshape(-1)
+        n_int16 = x.size
+        cap = self._cap(n_int16, chunk_int16)
+        out = np.empty((self.n_channels, cap), dtype=np.int16)
+        lens = np.zeros(max(1, -(-n_int16 // chunk_int16)), dtype=np.int32)
+        n_pcm = C.c_size_t(0)
+        _lib.check(_lib.lib().rxb200_fm_mix_process(self._m, x.ctypes.data, n_int16, chunk_int16, out.ctypes.data, cap,
+                                                    C.byref(n_pcm), lens.ctypes.data_as(C.POINTER(C.c_int))))
+        res = out[:, :n_pcm.value].copy()
+        return (res, lens) if return_chunks else res
+
+    def process_read(self, cs16: np.ndarray) -> np.ndarray:
+        """As ``FmDemod.process_read`` on every channel (``rxb200_fm_mix_process_read``)."""
+        x = np.ascontiguousarray(cs16, dtype=np.int16).reshape(-1)
+        n_int16 = x.size
+        cap = self._cap(n_int16, max(n_int16, 1))
+        out = np.empty((self.n_channels, cap), dtype=np.int16)
+        n_pcm = C.c_size_t(0)
+        _lib.check(_lib.lib().rxb200_fm_mix_process_read(self._m, x.ctypes.data, n_int16, out.ctypes.data, cap,
+                                                         C.byref(n_pcm)))
+        return out[:, :n_pcm.value].copy()
+
+    def process_device(self, d_in_ptr: int, n_int16: int, chunk_int16: int, d_out_ptr: int, out_stride: int,
+                       sync: bool = False) -> int:
+        """Device pointers: the capture (4-byte alignment is enough) and [n_channels][out_stride] PCM; returns the PCM
+        count per channel."""
+        n_pcm = C.c_size_t(0)
+        _lib.check(_lib.lib().rxb200_fm_mix_process_device(self._m, d_in_ptr, n_int16, chunk_int16, d_out_ptr,
+                                                           out_stride, C.byref(n_pcm), 1 if sync else 0))
+        return int(n_pcm.value)
+
+    def process_read_device(self, d_in_ptr: int, n_int16: int, d_out_ptr: int, out_stride: int,
+                            sync: bool = False) -> int:
+        """``process_read`` on device pointers; returns the PCM count per channel."""
+        n_pcm = C.c_size_t(0)
+        _lib.check(_lib.lib().rxb200_fm_mix_process_read_device(self._m, d_in_ptr, n_int16, d_out_ptr, out_stride,
+                                                                C.byref(n_pcm), 1 if sync else 0))
+        return int(n_pcm.value)
+
+    def squelch_hits(self) -> np.ndarray:
+        """demod.squelch_hits of every channel after the last call, int32[n_channels]."""
+        h = np.zeros(self.n_channels, dtype=np.int32)
+        _lib.check(_lib.lib().rxb200_fm_mix_squelch_hits(self._m, h.ctypes.data_as(C.POINTER(C.c_int))))
+        return h
+
+    def levels(self) -> np.ndarray:
+        """As ``FmDemod.levels``: int32[n_channels][n_chunks] of the last call (needs report_levels)."""
+        n = C.c_size_t(0)
+        rc = _lib.lib().rxb200_fm_mix_levels(self._m, np.zeros(1, np.int32).ctypes.data_as(C.POINTER(C.c_int)), 0,
+                                             C.byref(n))
+        if rc != _lib.ECAPACITY:
+            _lib.check(rc)
+        buf = np.zeros((self.n_channels, int(n.value)), dtype=np.int32)
+        _lib.check(_lib.lib().rxb200_fm_mix_levels(self._m, buf.ctypes.data_as(C.POINTER(C.c_int)), buf.size,
+                                                   C.byref(n)))
+        return buf
+
+    def stats(self) -> dict:
+        s = _lib.FmStatsC()
+        _lib.check(_lib.lib().rxb200_fm_last_stats(C.c_void_p(self.member()), C.byref(s)))
+        return {f[0]: int(getattr(s, f[0])) for f in s._fields_}
+
+    @property
+    def stream(self) -> int:
+        return int(_lib.lib().rxb200_fm_stream(C.c_void_p(self.member())) or 0)
+
+    def mix_ms(self) -> float:
+        """Device time of the last call's fm_mix_kernel."""
+        ms = C.c_float(0)
+        _lib.check(_lib.lib().rxb200_fm_mix_kernel_ms(self._m, C.byref(ms)))
+        return float(ms.value)
+
+    def kernel_ms(self) -> float:
+        """Device time of the last call's chain kernels (``rxb200_fm_kernel_ms`` of the member)."""
+        ms = C.c_float(0)
+        _lib.check(_lib.lib().rxb200_fm_kernel_ms(C.c_void_p(self.member()), C.byref(ms)))
+        return float(ms.value)
+
+
 # ---- rx_sdr sample-format conversions (src/rtl_sdr.c:348-391) -------------------------------------------
 CVT_CS16_CS8, CVT_CS16_CU8, CVT_CS16_CF32, CVT_CS12_CS16 = range(4)
 
