@@ -427,6 +427,41 @@ int rxb200_fm_mix_levels(rxb200_fm_mix *m, int *levels, size_t cap, size_t *n_ch
  * synchronises the stream. */
 int rxb200_fm_mix_kernel_ms(rxb200_fm_mix *m, float *ms);
 
+/* ======================================================================== rx_fm channels of one capture on several GPUs
+ * The channels of ONE capture split over GPUs: one process, n_dev rxb200_fm_mix handles, member i owning the contiguous
+ * channels [b, e) that rxb200_power_shard(n_channels, n_dev, i, &b, &e) gives, with offsets offsets_hz[b..e).  A member
+ * whose range is empty has no handle.  devices == NULL means 0..n_dev-1; an ordinal may repeat (several members on one
+ * GPU).  Every member gets its own copy of the capture (4 bytes per complex sample) and mixes and demodulates only its
+ * channels, so a call's mixer writes and chain work, which grow with the channel count, split over the GPUs.
+ * The group behaves byte for byte like ONE rxb200_fm_mix handle with n_channels channels: the same pcm, n_pcm,
+ * chunk_result_len, squelch hits, levels ([n_channels][n_chunks]) and refusal codes, over any sequence of process,
+ * process_read and reset calls.  cs16 and pcm are HOST pointers laid out as for rxb200_fm_mix_process (the one capture
+ * at cs16, channel k's PCM at pcm + k*pcm_stride).  Create checks every channel's table (rxb200_fm_mix_table) before it
+ * creates any member: a bad offset on any channel gets the code rxb200_fm_mix_create returns, before any device is
+ * touched.  A call refused for its shape or capacity is refused before any member starts and moves no member's phases
+ * and carries.  Each member copies the whole capture to its GPU, runs rxb200_fm_mix_process_device / _read_device and
+ * copies its PCM rows back, all on its own stream; the call returns when every member that started is done, also after
+ * a failure, and leaves the caller's current device as it found it.  A call that fails after members started
+ * (RXB200_ECUDA, RXB200_ENOMEM) may leave the members at different phases and carries; rxb200_fm_mix_group_reset brings
+ * every member back to the state right after create.  The capture copies of different GPUs overlap only with a pinned
+ * (page-locked) capture: from pageable memory the N copies run one after the other and only the kernels overlap them
+ * (the bytes are the same either way). */
+typedef struct rxb200_fm_mix_group rxb200_fm_mix_group;
+int rxb200_fm_mix_group_create(const rxb200_fm_params *params, int capture_rate, const int *offsets_hz, int n_channels,
+                               int n_dev, const int *devices, rxb200_fm_mix_group **out);
+void rxb200_fm_mix_group_destroy(rxb200_fm_mix_group *g);
+int rxb200_fm_mix_group_size(const rxb200_fm_mix_group *g);
+/* member i's mixing handle (its channels are channel 0.. of that handle), NULL for a member that owns no channel */
+rxb200_fm_mix *rxb200_fm_mix_group_member(rxb200_fm_mix_group *g, int i);
+int rxb200_fm_mix_group_process(rxb200_fm_mix_group *g, const int16_t *cs16, size_t n_int16, size_t chunk_int16,
+                                int16_t *pcm, size_t pcm_stride, size_t *n_pcm, int *chunk_result_len);
+int rxb200_fm_mix_group_process_read(rxb200_fm_mix_group *g, const int16_t *cs16, size_t n_int16, int16_t *pcm,
+                                     size_t pcm_stride, size_t *n_pcm);
+int rxb200_fm_mix_group_squelch_hits(rxb200_fm_mix_group *g, int *hits /* n_channels */);
+int rxb200_fm_mix_group_levels(rxb200_fm_mix_group *g, int *levels, size_t cap, size_t *n_chunks);
+/* every member's phases back to 0 and its chain back to the state right after create */
+int rxb200_fm_mix_group_reset(rxb200_fm_mix_group *g);
+
 /* ======================================================================== rx_sdr (SURVEY.md §8f row 4)
  * The pointwise sample-format conversions of rx_sdr's recorder loop (src/rtl_sdr.c:348-391):
  *   RXB200_CVT_CS16_CS8  : (uint8_t)(int)(x/32767.0*128.0+0.4)       per int16 (:367-370)

@@ -81,6 +81,9 @@ SYMBOLS = [
     "rxb200_fm_mix_table", "rxb200_mix_device", "rxb200_fm_mix_create", "rxb200_fm_mix_destroy", "rxb200_fm_mix_reset",
     "rxb200_fm_mix_member", "rxb200_fm_mix_process", "rxb200_fm_mix_process_device", "rxb200_fm_mix_process_read",
     "rxb200_fm_mix_process_read_device", "rxb200_fm_mix_squelch_hits", "rxb200_fm_mix_levels", "rxb200_fm_mix_kernel_ms",
+    "rxb200_fm_mix_group_create", "rxb200_fm_mix_group_destroy", "rxb200_fm_mix_group_size",
+    "rxb200_fm_mix_group_member", "rxb200_fm_mix_group_process", "rxb200_fm_mix_group_process_read",
+    "rxb200_fm_mix_group_squelch_hits", "rxb200_fm_mix_group_levels", "rxb200_fm_mix_group_reset",
     "rxb200_sdr_convert", "rxb200_sdr_convert_device",
 ]
 
@@ -183,6 +186,18 @@ def lib() -> C.CDLL:
     L.rxb200_fm_mix_squelch_hits.argtypes = [C.c_void_p, pint]
     L.rxb200_fm_mix_levels.argtypes = [C.c_void_p, pint, sz, C.POINTER(sz)]
     L.rxb200_fm_mix_kernel_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float)]
+    L.rxb200_fm_mix_group_create.argtypes = [C.POINTER(FmParamsC), C.c_int, pint, C.c_int, C.c_int, pint,
+                                             C.POINTER(C.c_void_p)]
+    L.rxb200_fm_mix_group_destroy.argtypes = [C.c_void_p]
+    L.rxb200_fm_mix_group_destroy.restype = None
+    L.rxb200_fm_mix_group_size.argtypes = [C.c_void_p]
+    L.rxb200_fm_mix_group_member.argtypes = [C.c_void_p, C.c_int]
+    L.rxb200_fm_mix_group_member.restype = C.c_void_p
+    L.rxb200_fm_mix_group_process.argtypes = [C.c_void_p, C.c_void_p, sz, sz, C.c_void_p, sz, C.POINTER(sz), pint]
+    L.rxb200_fm_mix_group_process_read.argtypes = [C.c_void_p, C.c_void_p, sz, C.c_void_p, sz, C.POINTER(sz)]
+    L.rxb200_fm_mix_group_squelch_hits.argtypes = [C.c_void_p, pint]
+    L.rxb200_fm_mix_group_levels.argtypes = [C.c_void_p, pint, sz, C.POINTER(sz)]
+    L.rxb200_fm_mix_group_reset.argtypes = [C.c_void_p]
     L.rxb200_sdr_convert.argtypes = [C.c_int, C.c_void_p, sz, C.c_void_p, C.c_int]
     L.rxb200_sdr_convert_device.argtypes = [C.c_int, C.c_void_p, sz, C.c_void_p, C.c_void_p]
     _lib = L

@@ -399,6 +399,92 @@ class FmMix:
         return float(ms.value)
 
 
+class FmMixGroup:
+    """The channels of ONE capture split over several GPUs (``rxb200_fm_mix_group_*``): member i is a ``FmMix`` on its
+    own GPU with a contiguous block of the offsets, and every member gets a copy of the capture; the group's results
+    are byte for byte those of one ``FmMix`` with all the offsets.  devices: one CUDA ordinal per member (may repeat),
+    or None for ``range(n_dev)``."""
+
+    def __init__(self, params, capture_rate: int, offsets_hz, devices=None, n_dev: Optional[int] = None):
+        self.params = FmParams.from_any(params)
+        self.capture_rate = capture_rate
+        offs = np.ascontiguousarray(offsets_hz, dtype=np.int32)
+        self.offsets_hz = offs.tolist()
+        self.n_channels = len(offs)
+        devs = None if devices is None else np.ascontiguousarray(devices, dtype=np.int32)
+        self.n_dev = len(devs) if devs is not None else int(n_dev or 1)
+        self._g = C.c_void_p()
+        pc = self.params.to_c()
+        dp = None if devs is None else devs.ctypes.data_as(C.POINTER(C.c_int))
+        _lib.check(_lib.lib().rxb200_fm_mix_group_create(C.byref(pc), capture_rate,
+                                                         offs.ctypes.data_as(C.POINTER(C.c_int)), self.n_channels,
+                                                         self.n_dev, dp, C.byref(self._g)))
+
+    def close(self) -> None:
+        if _lib is not None and getattr(self, "_g", None) is not None and self._g:
+            _lib.lib().rxb200_fm_mix_group_destroy(self._g)
+            self._g = None
+
+    __del__ = close
+
+    def member(self, i: int) -> int:
+        """Member i's rxb200_fm_mix handle as an integer, 0 for a member that owns no channel."""
+        return int(_lib.lib().rxb200_fm_mix_group_member(self._g, i) or 0)
+
+    def inner(self, i: int) -> int:
+        """The inner rxb200_fm handle of member i (``rxb200_fm_mix_member``), 0 for a member that owns no channel."""
+        m = self.member(i)
+        return int(_lib.lib().rxb200_fm_mix_member(C.c_void_p(m)) or 0) if m else 0
+
+    def reset(self) -> None:
+        _lib.check(_lib.lib().rxb200_fm_mix_group_reset(self._g))
+
+    def _cap(self, n_int16: int, chunk_int16: int) -> int:
+        return int(_lib.lib().rxb200_fm_max_output(C.c_void_p(self.inner(0)), n_int16, chunk_int16)) + 8
+
+    def full_demod(self, cs16: np.ndarray, chunk_int16: int = MAXIMUM_BUF_LENGTH, return_chunks: bool = False):
+        """As ``FmMix.full_demod`` (``rxb200_fm_mix_group_process``); cs16: the capture, int16[n_int16]."""
+        x = np.ascontiguousarray(cs16, dtype=np.int16).reshape(-1)
+        n_int16 = x.size
+        cap = self._cap(n_int16, chunk_int16)
+        out = np.empty((self.n_channels, cap), dtype=np.int16)
+        lens = np.zeros(max(1, -(-n_int16 // chunk_int16)), dtype=np.int32)
+        n_pcm = C.c_size_t(0)
+        _lib.check(_lib.lib().rxb200_fm_mix_group_process(self._g, x.ctypes.data, n_int16, chunk_int16, out.ctypes.data,
+                                                          cap, C.byref(n_pcm), lens.ctypes.data_as(C.POINTER(C.c_int))))
+        res = out[:, :n_pcm.value].copy()
+        return (res, lens) if return_chunks else res
+
+    def process_read(self, cs16: np.ndarray) -> np.ndarray:
+        """As ``FmMix.process_read`` (``rxb200_fm_mix_group_process_read``)."""
+        x = np.ascontiguousarray(cs16, dtype=np.int16).reshape(-1)
+        n_int16 = x.size
+        cap = self._cap(n_int16, max(n_int16, 1))
+        out = np.empty((self.n_channels, cap), dtype=np.int16)
+        n_pcm = C.c_size_t(0)
+        _lib.check(_lib.lib().rxb200_fm_mix_group_process_read(self._g, x.ctypes.data, n_int16, out.ctypes.data, cap,
+                                                               C.byref(n_pcm)))
+        return out[:, :n_pcm.value].copy()
+
+    def squelch_hits(self) -> np.ndarray:
+        """demod.squelch_hits of every channel after the last call, int32[n_channels]."""
+        h = np.zeros(self.n_channels, dtype=np.int32)
+        _lib.check(_lib.lib().rxb200_fm_mix_group_squelch_hits(self._g, h.ctypes.data_as(C.POINTER(C.c_int))))
+        return h
+
+    def levels(self) -> np.ndarray:
+        """As ``FmDemod.levels``: int32[n_channels][n_chunks] of the last call (needs report_levels)."""
+        n = C.c_size_t(0)
+        rc = _lib.lib().rxb200_fm_mix_group_levels(self._g, np.zeros(1, np.int32).ctypes.data_as(C.POINTER(C.c_int)), 0,
+                                                   C.byref(n))
+        if rc != _lib.ECAPACITY:
+            _lib.check(rc)
+        buf = np.zeros((self.n_channels, int(n.value)), dtype=np.int32)
+        _lib.check(_lib.lib().rxb200_fm_mix_group_levels(self._g, buf.ctypes.data_as(C.POINTER(C.c_int)), buf.size,
+                                                         C.byref(n)))
+        return buf
+
+
 # ---- rx_sdr sample-format conversions (src/rtl_sdr.c:348-391) -------------------------------------------
 CVT_CS16_CS8, CVT_CS16_CU8, CVT_CS16_CF32, CVT_CS12_CS16 = range(4)
 
