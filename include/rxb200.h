@@ -423,9 +423,51 @@ int rxb200_fm_mix_process_read_device(rxb200_fm_mix *m, const int16_t *d_cs16, s
                                       size_t pcm_stride, size_t *n_pcm, int sync);
 int rxb200_fm_mix_squelch_hits(rxb200_fm_mix *m, int *hits /* n_channels */);
 int rxb200_fm_mix_levels(rxb200_fm_mix *m, int *levels, size_t cap, size_t *n_chunks);
-/* Device time (CUDA events on the member's stream) of the last successful call's fm_mix_kernel, in milliseconds;
- * synchronises the stream. */
+/* Device time (CUDA events on the member's stream) of the last successful call's fm_mix_kernel (fm_ddc_kernel for a
+ * decimating handle), in milliseconds; synchronises the stream. */
 int rxb200_fm_mix_kernel_ms(rxb200_fm_mix *m, float *ms);
+
+/* ---- decimating mixing handles: mixer, channel filter and decimation before the chain (a digital down-converter)
+ * A decimating handle has a capture rate R and K offsets as above, plus one rxb200_ddc shared by every channel: a
+ * decimation factor M (1..4096), T int32 taps h[0..T) (1 <= T <= 8192, copied at create) and a rounding shift S
+ * (0..62).  For channel k let z[n] = mix_k(x)[n], n counting capture samples from create or reset across calls, and
+ * z[n] = 0 for n < 0.  Output m >= 0 is emitted at capture sample e_m = m*M + M - 1; for I and Q separately
+ *     A = sum_{j<T} h[j] * z[e_m - j]   (exact, 64-bit);   y = S ? (A + 2^(S-1)) >> S : A   (arithmetic);
+ *     out = y saturated to [-32768, 32767].
+ * Channel k is the reference's rtlsdr_callback() + full_demod() on that decimated CS16 stream, through the member's
+ * chain with any parameters; typically offset_tuning = 1 and downsample = R / (M * rate_in).
+ * A call covering capture samples [n0, n0 + c) hands the chain the floor((n0+c)/M) - floor(n0/M) outputs whose e_m
+ * falls in it (rxb200_fm_mix_decimated_len).  Read calls (_process_read*): those outputs are one read of the member; a
+ * read with no output runs no chain call, returns n_pcm = 0 and zero level chunks, and still advances the phases and
+ * the filter history; a decimated read the member refuses (for example fewer than 2^P complex samples with passes)
+ * refuses the whole call.  Chunk calls (_process*): chunk_int16 must be a multiple of 2M (else RXB200_EUNSUPPORTED);
+ * capture chunk c is then decimated chunk c of chunk_int16 / M int16 at any phase, the last partial capture chunk the
+ * decimated remainder, and chunk_result_len entries of capture chunks with no decimated sample are 0.  Every other
+ * refusal is the member's on the decimated shape; a refused call changes nothing.  fm_ddc_kernel mixes and filters in
+ * one pass (int32 accumulation when sum |h| * 32768 + 2^(S-1) < 2^31, else int64), so only the decimated streams,
+ * [K][n_dec_int16], reach the scratch buffer.  Reset also zeroes the filter history.  M = 1, h = {1}, S = 0 gives
+ * the bytes of the plain mixing handle. */
+typedef struct rxb200_ddc {
+	int decim;             /* M */
+	int n_taps;            /* T */
+	const int32_t *taps;   /* h[0..T) */
+	int shift;             /* S */
+} rxb200_ddc;
+/* RXB200_EINVAL for a NULL ddc or taps, M, T or S out of range, or sum |h| * 32768 + 2^(S-1) >= 2^63; every refusal
+ * of rxb200_fm_mix_create otherwise.  The handle takes every rxb200_fm_mix_* entry point. */
+int rxb200_fm_mix_create_ddc(const rxb200_fm_params *params, int capture_rate, const int *offsets_hz, int n_channels,
+                             const rxb200_ddc *ddc, int device, rxb200_fm_mix **out);
+/* *n_dec_int16: the int16 per channel the next call of n_int16 capture int16 hands the chain, at the current phase
+ * (n_int16 for a plain mixing handle), so that a caller with passes can check a read before making it. */
+int rxb200_fm_mix_decimated_len(const rxb200_fm_mix *m, size_t n_int16, size_t *n_dec_int16);
+/* A bound on the PCM per channel of a call of n_int16 capture int16 in chunks of chunk_int16, at any phase (any
+ * mixing handle). */
+size_t rxb200_fm_mix_max_output(const rxb200_fm_mix *m, size_t n_int16, size_t chunk_int16);
+/* The DDC alone on DEVICE pointers, stateless, on `stream`: the samples before d_src are zero, the mixer starts at
+ * table entry phase mod L (phase >= 0), and floor(n_complex / M) outputs go to d_dst, e_m counted from d_src.  Both
+ * pointers 4-byte aligned.  Asynchronous. */
+int rxb200_ddc_device(int capture_rate, int offset_hz, long long phase, const rxb200_ddc *ddc, const int16_t *d_src,
+                      size_t n_complex, int16_t *d_dst, void *stream);
 
 /* ======================================================================== rx_fm channels of one capture on several GPUs
  * The channels of ONE capture split over GPUs: one process, n_dev rxb200_fm_mix handles, member i owning the contiguous
@@ -449,6 +491,12 @@ int rxb200_fm_mix_kernel_ms(rxb200_fm_mix *m, float *ms);
 typedef struct rxb200_fm_mix_group rxb200_fm_mix_group;
 int rxb200_fm_mix_group_create(const rxb200_fm_params *params, int capture_rate, const int *offsets_hz, int n_channels,
                                int n_dev, const int *devices, rxb200_fm_mix_group **out);
+/* The same with decimating members (rxb200_fm_mix_create_ddc), all sharing one rxb200_ddc: the group behaves like ONE
+ * decimating handle with every channel, and every member checks a call's refusals on the decimated shape it will see.
+ * The ddc is checked before the offsets. */
+int rxb200_fm_mix_group_create_ddc(const rxb200_fm_params *params, int capture_rate, const int *offsets_hz,
+                                   int n_channels, const rxb200_ddc *ddc, int n_dev, const int *devices,
+                                   rxb200_fm_mix_group **out);
 void rxb200_fm_mix_group_destroy(rxb200_fm_mix_group *g);
 int rxb200_fm_mix_group_size(const rxb200_fm_mix_group *g);
 /* member i's mixing handle (its channels are channel 0.. of that handle), NULL for a member that owns no channel */

@@ -54,6 +54,10 @@ class PowerPathC(C.Structure):
 POWER_PATHS = {0: "none", 1: "rms", 2: "fft8", 3: "generic", 4: "big_load", 5: "big_decim"}
 
 
+class DdcC(C.Structure):
+    _fields_ = [("decim", C.c_int), ("n_taps", C.c_int), ("taps", C.POINTER(C.c_int32)), ("shift", C.c_int)]
+
+
 class PowerPlanC(C.Structure):
     _fields_ = [("params", PowerParamsC), ("rate", C.c_int), ("crop", C.c_double),
                 ("first_freq", C.c_int64), ("freq_step", C.c_int64), ("bin_size_hz", C.c_double)]
@@ -84,6 +88,8 @@ SYMBOLS = [
     "rxb200_fm_mix_group_create", "rxb200_fm_mix_group_destroy", "rxb200_fm_mix_group_size",
     "rxb200_fm_mix_group_member", "rxb200_fm_mix_group_process", "rxb200_fm_mix_group_process_read",
     "rxb200_fm_mix_group_squelch_hits", "rxb200_fm_mix_group_levels", "rxb200_fm_mix_group_reset",
+    "rxb200_fm_mix_create_ddc", "rxb200_fm_mix_decimated_len", "rxb200_fm_mix_max_output", "rxb200_ddc_device",
+    "rxb200_fm_mix_group_create_ddc",
     "rxb200_sdr_convert", "rxb200_sdr_convert_device",
 ]
 
@@ -198,6 +204,15 @@ def lib() -> C.CDLL:
     L.rxb200_fm_mix_group_squelch_hits.argtypes = [C.c_void_p, pint]
     L.rxb200_fm_mix_group_levels.argtypes = [C.c_void_p, pint, sz, C.POINTER(sz)]
     L.rxb200_fm_mix_group_reset.argtypes = [C.c_void_p]
+    L.rxb200_fm_mix_create_ddc.argtypes = [C.POINTER(FmParamsC), C.c_int, pint, C.c_int, C.POINTER(DdcC), C.c_int,
+                                           C.POINTER(C.c_void_p)]
+    L.rxb200_fm_mix_decimated_len.argtypes = [C.c_void_p, sz, C.POINTER(sz)]
+    L.rxb200_fm_mix_max_output.argtypes = [C.c_void_p, sz, sz]
+    L.rxb200_fm_mix_max_output.restype = sz
+    L.rxb200_ddc_device.argtypes = [C.c_int, C.c_int, C.c_longlong, C.POINTER(DdcC), C.c_void_p, sz, C.c_void_p,
+                                    C.c_void_p]
+    L.rxb200_fm_mix_group_create_ddc.argtypes = [C.POINTER(FmParamsC), C.c_int, pint, C.c_int, C.POINTER(DdcC),
+                                                 C.c_int, pint, C.POINTER(C.c_void_p)]
     L.rxb200_sdr_convert.argtypes = [C.c_int, C.c_void_p, sz, C.c_void_p, C.c_int]
     L.rxb200_sdr_convert_device.argtypes = [C.c_int, C.c_void_p, sz, C.c_void_p, C.c_void_p]
     _lib = L

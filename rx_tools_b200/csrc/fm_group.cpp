@@ -133,8 +133,10 @@ int group_process(Group *g, const int16_t *cs16, size_t n_int16, size_t chunk_in
 	size_t total = 0;
 	for (Member &mb : g->mb) {
 		if (!mb.h) { continue; }
-		const int rc = rxb::fm_check_host_call(mb.h, cs16, n_int16, chunk_int16, pcm, pcm_stride, chunk_result_len, n_pcm,
-		                                       read, &total);
+		const int rc = mb.m ? rxb::fm_mix_check_host_call(mb.m, cs16, n_int16, chunk_int16, pcm, pcm_stride,
+		                                                  chunk_result_len, n_pcm, read, &total)
+		                    : rxb::fm_check_host_call(mb.h, cs16, n_int16, chunk_int16, pcm, pcm_stride, chunk_result_len,
+		                                              n_pcm, read, &total);
 		if (rc != RXB200_OK) { return rc; }
 	}
 	if (n_int16 == 0) { return RXB200_OK; }
@@ -256,14 +258,21 @@ extern "C" int rxb200_fm_group_reset(rxb200_fm_group *g) { return group_reset(g)
 // ---- channels of one capture: rxb200_fm_mix_group_*
 extern "C" void rxb200_fm_mix_group_destroy(rxb200_fm_mix_group *g) { group_destroy(g); }
 
-extern "C" int rxb200_fm_mix_group_create(const rxb200_fm_params *params, int capture_rate, const int *offsets_hz,
-                                          int n_channels, int n_dev, const int *devices, rxb200_fm_mix_group **out)
+namespace {
+
+// rxb200_fm_mix_group_create and rxb200_fm_mix_group_create_ddc (ddc != NULL: decimating members)
+int mix_group_create(const rxb200_fm_params *params, int capture_rate, const int *offsets_hz, int n_channels,
+                     const rxb200_ddc *ddc, int n_dev, const int *devices, rxb200_fm_mix_group **out)
 {
 	if (!params || !offsets_hz || !out || n_channels < 1 || n_dev < 1) {
 		set_error("bad mix group arguments (n_channels >= 1, n_dev >= 1)");
 		return RXB200_EINVAL;
 	}
 	*out = nullptr;
+	if (ddc) {
+		const int rc = rxb::ddc_check(ddc, nullptr);
+		if (rc != RXB200_OK) { return rc; }
+	}
 	// every channel's table first, so that a bad offset on any member is refused before any device work
 	for (int k = 0; k < n_channels; k++) {
 		size_t period = 0;
@@ -271,10 +280,28 @@ extern "C" int rxb200_fm_mix_group_create(const rxb200_fm_params *params, int ca
 		if (rc != RXB200_ECAPACITY) { return rc; }
 	}
 	return group_create(n_channels, n_dev, devices, [&](Member &mb, int nch) {
-		const int rc = rxb200_fm_mix_create(params, capture_rate, offsets_hz + mb.ch_begin, nch, mb.device, &mb.m);
+		const int *offs = offsets_hz + mb.ch_begin;
+		const int rc = ddc ? rxb200_fm_mix_create_ddc(params, capture_rate, offs, nch, ddc, mb.device, &mb.m)
+		                   : rxb200_fm_mix_create(params, capture_rate, offs, nch, mb.device, &mb.m);
 		mb.h = rxb200_fm_mix_member(mb.m);
 		return rc;
 	}, out);
+}
+
+}  // namespace
+
+extern "C" int rxb200_fm_mix_group_create(const rxb200_fm_params *params, int capture_rate, const int *offsets_hz,
+                                          int n_channels, int n_dev, const int *devices, rxb200_fm_mix_group **out)
+{
+	return mix_group_create(params, capture_rate, offsets_hz, n_channels, nullptr, n_dev, devices, out);
+}
+
+extern "C" int rxb200_fm_mix_group_create_ddc(const rxb200_fm_params *params, int capture_rate, const int *offsets_hz,
+                                              int n_channels, const rxb200_ddc *ddc, int n_dev, const int *devices,
+                                              rxb200_fm_mix_group **out)
+{
+	if (!ddc) { set_error("null ddc"); return RXB200_EINVAL; }
+	return mix_group_create(params, capture_rate, offsets_hz, n_channels, ddc, n_dev, devices, out);
 }
 
 extern "C" int rxb200_fm_mix_group_size(const rxb200_fm_mix_group *g) { return g ? (int)g->mb.size() : 0; }

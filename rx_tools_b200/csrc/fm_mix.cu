@@ -3,6 +3,7 @@
 // once and writing one CS16 stream per channel; a plain rxb200_fm handle with one channel per stream then runs the
 // chain on them through its device entry points.  The chain itself is not touched here.
 #include <algorithm>
+#include <cstring>
 #include <new>
 #include <vector>
 #include "common.cuh"
@@ -148,7 +149,166 @@ static int mix_table(int capture_rate, int offset_hz, std::vector<int32_t> &t, s
 	return rxb200_fm_mix_table(capture_rate, offset_hz, t.data(), t.size(), period);
 }
 
+// ---- the decimating down-converter (rxb200_fm_mix_create_ddc, rxb200_ddc_device)
+#define DDC_THREADS 256
+#define DDC_SPAN 8192                // capture samples a CTA stages at most (T <= 8192: one output always fits)
+#define DDC_REACH (1 << 20)          // capture samples a CTA's span covers at most: table offsets stay below 2^21
+
+struct DdcArgs {
+	const uint32_t *src;             // the call's capture, one word per complex sample
+	const uint32_t *hist;            // the T - 1 raw capture samples before src
+	long long n_out;                 // outputs per channel
+	long long r0;                    // src index of the first emission point
+	unsigned long long pos;          // the mixer: src[i] uses table entry (pos + i) mod L
+	uint32_t *dst;                   // channel row c at dst + c * dst_stride, one word per output
+	long long dst_stride;
+	const int32_t *taps;             // reversed: taps[t] = h[T - 1 - t]
+	const int2 *tab;
+	const MixChan *chan;
+	int n_ch, M, T, S;
+	int ws;                          // staged samples between two outputs' windows: M when T >= M, else T
+	unsigned ws_m;                   // floor((2^32 - 1) / ws)
+	int U;                           // outputs per CTA
+	int lpo;                         // lanes per output (a power of two <= 32)
+};
+
+// staged sample s -> its offset from the CTA's first staged sample: windows of T samples, M apart, stored ws apart
+__device__ __forceinline__ int ddc_off(int s, const DdcArgs &a)
+{
+	unsigned q = __umulhi((unsigned)s, a.ws_m);
+	int r = s - (int)q * a.ws;
+	if (r >= a.ws) { q++; r -= a.ws; }
+	return (int)q * a.M + r;
+}
+
+// one output: y = S == 0 ? A : (A + 2^(S-1)) >> S (arithmetic), saturated to int16
+template <typename Acc>
+__device__ __forceinline__ int ddc_out(Acc acc, int S)
+{
+	long long y = (long long)acc;
+	if (S) { y = (y + (1ll << (S - 1))) >> S; }
+	return (int)(y < -32768 ? -32768 : (y > 32767 ? 32767 : y));
+}
+
+// One CTA: U consecutive outputs of every channel of its grid row (up to 256 channels, blockIdx.y).  It stages the
+// capture samples its outputs' windows cover once (the handle's history before the call's first sample), then per
+// channel mixes them into shared memory with the channel's table and runs the T-tap dot product at the emission points
+// only, lpo lanes per output.  Acc: int when sum |h| * 32768 + 2^(S-1) < 2^31, else long long (no partial sum can
+// overflow either way).
+template <typename Acc>
+__global__ void __launch_bounds__(DDC_THREADS) fm_ddc_kernel(const DdcArgs a)
+{
+	extern __shared__ int4 ddc_smem[];
+	__shared__ MixChan s_ch[MIX_GROUP];
+	__shared__ unsigned s_base[MIX_GROUP];  // each channel's table entry at the CTA's first staged sample
+	const int T = a.T;
+	const int room = (a.U - 1) * a.ws + T;
+	int32_t *s_h = reinterpret_cast<int32_t *>(ddc_smem);
+	uint32_t *s_x = reinterpret_cast<uint32_t *>(s_h + T);
+	uint32_t *s_z = s_x + room;
+	const int c0 = (int)blockIdx.y * MIX_GROUP;
+	const int nc = min(MIX_GROUP, a.n_ch - c0);
+	const long long u0 = (long long)blockIdx.x * a.U;
+	const int U = (int)min((long long)a.U, a.n_out - u0);
+	const int n = (U - 1) * a.ws + T;
+	const long long b0 = u0 * a.M + a.r0 - (T - 1);       // src index of the first staged sample, >= -(T - 1)
+	const long long g0 = (long long)a.pos + b0;            // its mixer position (< 0 only for zero history samples)
+	for (int j = threadIdx.x; j < T; j += blockDim.x) { s_h[j] = a.taps[j]; }
+	for (int c = threadIdx.x; c < nc; c += blockDim.x) {
+		const MixChan ch = a.chan[c0 + c];
+		long long q = g0 % ch.L;
+		s_base[c] = (unsigned)(q < 0 ? q + ch.L : q);
+		s_ch[c] = ch;
+	}
+	for (int s = threadIdx.x; s < n; s += blockDim.x) {
+		const long long i = b0 + ddc_off(s, a);
+		s_x[s] = i >= 0 ? __ldg(a.src + i) : a.hist[(T - 1) + i];
+	}
+	__syncthreads();
+	const int lane = (int)threadIdx.x & (a.lpo - 1), sub = (int)threadIdx.x / a.lpo, n_sub = (int)blockDim.x / a.lpo;
+	for (int c = 0; c < nc; c++) {
+		const MixChan ch = s_ch[c];
+		const unsigned L = (unsigned)ch.L, base = s_base[c];
+		for (int s = threadIdx.x; s < n; s += blockDim.x) {
+			const unsigned t = base + (unsigned)ddc_off(s, a);      // < 2^20 + DDC_REACH
+			unsigned p = t - __umulhi(t, ch.m) * L;               // the quotient is low by at most 1
+			if (p >= L) { p -= L; }
+			s_z[s] = mix_one(s_x[s], __ldg(a.tab + ch.off + (int)p));
+		}
+		__syncthreads();
+		uint32_t *row = a.dst + (long long)(c0 + c) * a.dst_stride + u0;
+		for (int ub = 0; ub < U; ub += n_sub) {                  // the same trip count on every lane of a warp
+			const int u = ub + sub;
+			Acc ai = 0, aq = 0;
+			if (u < U) {
+				const uint32_t *z = s_z + u * a.ws;
+				for (int j = lane; j < T; j += a.lpo) {
+					const uint32_t w = z[j];
+					const Acc h = (Acc)s_h[j];
+					ai += h * (Acc)(int16_t)(w & 0xffffu);
+					aq += h * (Acc)(int16_t)(w >> 16);
+				}
+			}
+			for (int o = a.lpo >> 1; o > 0; o >>= 1) {
+				ai += __shfl_xor_sync(0xffffffffu, ai, o);
+				aq += __shfl_xor_sync(0xffffffffu, aq, o);
+			}
+			if (u < U && lane == 0) {
+				row[u] = ((uint32_t)ddc_out(ai, a.S) & 0xffffu) | ((uint32_t)ddc_out(aq, a.S) << 16);
+			}
+		}
+		__syncthreads();                    // every output of this channel is made before s_z is overwritten
+	}
+}
+
+// Launches fm_ddc_kernel on the current device for a.n_out > 0 outputs per channel; fills a's launch shape
+static int ddc_launch(DdcArgs a, bool wide, cudaStream_t st)
+{
+	const int T = a.T, M = a.M;
+	a.ws = T >= M ? M : T;
+	a.ws_m = 0xffffffffu / (unsigned)a.ws;
+	a.lpo = 1;
+	while (a.lpo < 32 && a.lpo < T) { a.lpo <<= 1; }
+	const int groups = (a.n_ch + MIX_GROUP - 1) / MIX_GROUP;
+	int dev = 0, n_sm = 0;
+	RXB_CUDA(cudaGetDevice(&dev));
+	RXB_CUDA(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
+	// as many outputs per CTA as the staging room and the reach allow, but at least two CTAs per SM when there is work
+	long long U = std::min((long long)(DDC_SPAN - T) / a.ws, (long long)(DDC_REACH - T) / M) + 1;
+	const long long ctas = std::max(1ll, (2ll * n_sm + groups - 1) / groups);
+	U = std::max(1ll, std::min(U, (a.n_out + ctas - 1) / ctas));
+	a.U = (int)U;
+	const size_t smem = ((size_t)T + 2 * ((size_t)(a.U - 1) * a.ws + T)) * sizeof(uint32_t);
+	void (*kern)(const DdcArgs) = wide ? fm_ddc_kernel<long long> : fm_ddc_kernel<int>;
+	RXB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+	const long long bx = (a.n_out + U - 1) / U;
+	kern<<<dim3((unsigned)bx, (unsigned)groups), DDC_THREADS, smem, st>>>(a);
+	RXB_CUDA(cudaGetLastError());
+	return RXB200_OK;
+}
+
 }  // namespace rxb
+
+// the DDC's arguments: M, T and S in range, taps given, and sum |h| * 32768 + 2^(S-1) < 2^63 (which these ranges
+// already bound by 2^59 + 2^61); *wide: the sum reaches 2^31, so the kernel accumulates in 64 bits
+int rxb::ddc_check(const rxb200_ddc *d, bool *wide)
+{
+	if (!d || !d->taps) { set_error("null ddc or taps"); return RXB200_EINVAL; }
+	if (d->decim < 1 || d->decim > 4096 || d->n_taps < 1 || d->n_taps > 8192 || d->shift < 0 || d->shift > 62) {
+		set_error("ddc decim %d, n_taps %d, shift %d: need 1 <= decim <= 4096, 1 <= n_taps <= 8192, 0 <= shift <= 62",
+		          d->decim, d->n_taps, d->shift);
+		return RXB200_EINVAL;
+	}
+	unsigned long long sum = 0;
+	for (int j = 0; j < d->n_taps; j++) {
+		const long long h = d->taps[j];
+		sum += (unsigned long long)(h < 0 ? -h : h);
+	}
+	const unsigned long long g = sum * 32768ull + (d->shift ? 1ull << (d->shift - 1) : 0ull);
+	if (g >= (1ull << 63)) { set_error("sum |taps| * 32768 + 2^(shift-1) >= 2^63"); return RXB200_EINVAL; }
+	if (wide) { *wide = g >= (1ull << 31); }
+	return RXB200_OK;
+}
 using namespace rxb;
 
 struct rxb200_fm_mix {
@@ -162,7 +322,14 @@ struct rxb200_fm_mix {
 	int16_t *d_cap = nullptr; size_t cap_cap = 0;   // host calls: the capture (int16 elements)
 	int16_t *d_mix = nullptr; size_t mix_cap = 0;   // the mixed streams, [n_channels][n_int16]
 	int16_t *d_out = nullptr; size_t out_cap = 0;   // host calls: the PCM rows, total + 8 apart
-	cudaEvent_t ev0 = nullptr, ev1 = nullptr;    // around the last fm_mix_kernel
+	cudaEvent_t ev0 = nullptr, ev1 = nullptr;    // around the last fm_mix_kernel (fm_ddc_kernel)
+	// a decimating handle (rxb200_fm_mix_create_ddc): fm_ddc_kernel writes the decimated streams to d_mix ([n_channels]
+	// [n_dec_int16]) and the member runs on those
+	bool ddc = false, wide = false;              // wide: the kernel accumulates in 64 bits
+	int decim = 1, n_taps = 1, shift = 0;
+	int32_t *d_taps = nullptr;                   // reversed
+	int16_t *d_hist[2] = {nullptr, nullptr};     // the raw capture's last T - 1 samples before pos (zero before 0)
+	int cur_hist = 0;                            // d_hist[cur_hist] is the live one, the other the next call's
 };
 
 namespace {
@@ -177,6 +344,119 @@ cudaError_t reserve(T *&buf, size_t &cap, size_t need)
 	return e;
 }
 
+// int16 a decimating handle hands the chain from a call of n_int16 capture int16 after pos capture samples: the
+// outputs whose emission point m*M + M - 1 falls in the call
+size_t ddc_len(unsigned long long pos, size_t n_int16, int decim)
+{
+	const unsigned long long M = (unsigned long long)decim;
+	return 2 * (size_t)((pos + n_int16 / 2) / M - pos / M);
+}
+
+// The refusals of a decimating handle's call and what its member's call will be: *n16 and *chunk16, the decimated
+// call (n16 == 0: no member call).  The member's own refusals run on that shape.  A read with no output reports what
+// an empty call of the member reports (no PCM, no level chunks); chunk_result_len entries of capture chunks past the
+// member's chunks are 0.
+int ddc_check_call(rxb200_fm_mix *m, const int16_t *cs16, size_t n_int16, size_t chunk_int16, int16_t *pcm,
+                   size_t pcm_stride, int *chunk_result_len, size_t *n_pcm, bool read, size_t *total, size_t *n16,
+                   size_t *chunk16)
+{
+	if (!cs16 || !pcm) { set_error("null argument"); return RXB200_EINVAL; }
+	const size_t M = (size_t)m->decim;
+	if (n_int16 % 2 != 0) { set_error("n_int16=%zu must be even", n_int16); return RXB200_EUNSUPPORTED; }
+	if (!read && (chunk_int16 == 0 || chunk_int16 % (2 * M) != 0)) {
+		set_error("chunk_int16=%zu must be a multiple of 2 * decim = %zu", chunk_int16, 2 * M);
+		return RXB200_EUNSUPPORTED;
+	}
+	*n16 = ddc_len(m->pos, n_int16, m->decim);
+	*chunk16 = read ? *n16 : chunk_int16 / M;
+	if (read && *n16 == 0 && n_int16 > 0) {
+		return rxb::fm_check_host_call(m->h, cs16, 0, 262144, pcm, pcm_stride, nullptr, n_pcm, false, total);
+	}
+	const int rc = rxb::fm_check_host_call(m->h, cs16, *n16, *chunk16, pcm, pcm_stride, chunk_result_len, n_pcm, read,
+	                                       total);
+	if (rc == RXB200_OK && !read && chunk_result_len) {
+		const size_t caps = (n_int16 + chunk_int16 - 1) / chunk_int16, decs = (*n16 + *chunk16 - 1) / *chunk16;
+		for (size_t c = decs; c < caps; c++) { chunk_result_len[c] = 0; }
+	}
+	return rc;
+}
+
+// The next history: the last T - 1 samples of (history, the call's c capture samples at src), into the spare buffer
+int ddc_carry(rxb200_fm_mix *m, const int16_t *src, size_t c, cudaStream_t st)
+{
+	const size_t H = (size_t)m->n_taps - 1, w = 2 * sizeof(int16_t);
+	if (H == 0) { return RXB200_OK; }
+	const int16_t *old = m->d_hist[m->cur_hist];
+	int16_t *next = m->d_hist[m->cur_hist ^ 1];
+	if (c >= H) {
+		RXB_CUDA(cudaMemcpyAsync(next, src + 2 * (c - H), H * w, cudaMemcpyDeviceToDevice, st));
+	} else {
+		RXB_CUDA(cudaMemcpyAsync(next, old + 2 * c, (H - c) * w, cudaMemcpyDeviceToDevice, st));
+		RXB_CUDA(cudaMemcpyAsync(next + 2 * (H - c), src, c * w, cudaMemcpyDeviceToDevice, st));
+	}
+	return RXB200_OK;
+}
+
+// mix_call for a decimating handle: fm_ddc_kernel, then the member on the decimated streams
+int ddc_call(rxb200_fm_mix *m, const int16_t *cs16, size_t n_int16, size_t chunk_int16, int16_t *pcm, size_t pcm_stride,
+             size_t *n_pcm, int *chunk_result_len, bool read, bool device, int sync)
+{
+	size_t total = 0, n16 = 0, chunk16 = 0;
+	int rc = ddc_check_call(m, cs16, n_int16, chunk_int16, pcm, pcm_stride, chunk_result_len, n_pcm, read, &total, &n16,
+	                        &chunk16);
+	if (rc != RXB200_OK || n_int16 == 0) { return rc; }
+	RXB_CUDA(cudaSetDevice(m->device));
+	const cudaStream_t st = (cudaStream_t)rxb200_fm_stream(m->h);
+	const size_t K = (size_t)m->n_channels, c = n_int16 / 2;
+	if (n16) { RXB_CUDA(reserve(m->d_mix, m->mix_cap, n16 * K)); }
+	const int16_t *src = cs16;
+	if (!device) {
+		RXB_CUDA(reserve(m->d_cap, m->cap_cap, n_int16));
+		if (n16) { RXB_CUDA(reserve(m->d_out, m->out_cap, (total + 8) * K)); }
+		RXB_CUDA(cudaMemcpyAsync(m->d_cap, cs16, n_int16 * sizeof(int16_t), cudaMemcpyHostToDevice, st));
+		src = m->d_cap;
+	}
+	RXB_CUDA(cudaEventRecord(m->ev0, st));
+	if (n16) {
+		DdcArgs a{};
+		a.src = reinterpret_cast<const uint32_t *>(src);
+		a.hist = reinterpret_cast<const uint32_t *>(m->d_hist[m->cur_hist]);
+		a.n_out = (long long)(n16 / 2);
+		a.r0 = (long long)(m->decim - 1) - (long long)(m->pos % (unsigned long long)m->decim);
+		a.pos = m->pos;
+		a.dst = reinterpret_cast<uint32_t *>(m->d_mix);
+		a.dst_stride = (long long)(n16 / 2);
+		a.taps = m->d_taps; a.tab = m->d_tab; a.chan = m->d_chan;
+		a.n_ch = m->n_channels; a.M = m->decim; a.T = m->n_taps; a.S = m->shift;
+		rc = ddc_launch(a, m->wide, st);
+		if (rc != RXB200_OK) { return rc; }
+	}
+	RXB_CUDA(cudaEventRecord(m->ev1, st));
+	rc = ddc_carry(m, src, c, st);
+	if (rc != RXB200_OK) { return rc; }
+	if (n16) {
+		int16_t *out = device ? pcm : m->d_out;
+		const size_t stride = device ? pcm_stride : total + 8;
+		size_t n = 0;
+		rc = read ? rxb200_fm_process_read_device(m->h, m->d_mix, n16, out, stride, &n, device ? sync : 0)
+		          : rxb200_fm_process_device(m->h, m->d_mix, n16, chunk16, out, stride, &n, device ? sync : 0);
+		if (rc != RXB200_OK) { return rc; }
+	}
+	if (!device) {
+		if (total) {
+			RXB_CUDA(cudaMemcpy2DAsync(pcm, pcm_stride * sizeof(int16_t), m->d_out, (total + 8) * sizeof(int16_t),
+			                           total * sizeof(int16_t), K, cudaMemcpyDeviceToHost, st));
+		}
+		RXB_CUDA(cudaStreamSynchronize(st));
+	} else if (sync) {
+		RXB_CUDA(cudaStreamSynchronize(st));
+	}
+	if (m->n_taps > 1) { m->cur_hist ^= 1; }
+	m->pos += c;
+	if (n_pcm) { *n_pcm = total; }
+	return RXB200_OK;
+}
+
 // One call of any process entry point.  device: cs16 and pcm are device pointers (the member's device entry point
 // writes pcm), else host pointers staged through the handle's buffers.  read: one read (chunk_int16 == n_int16).
 int mix_call(rxb200_fm_mix *m, const int16_t *cs16, size_t n_int16, size_t chunk_int16, int16_t *pcm, size_t pcm_stride,
@@ -184,6 +464,7 @@ int mix_call(rxb200_fm_mix *m, const int16_t *cs16, size_t n_int16, size_t chunk
 {
 	if (!m) { set_error("null argument"); return RXB200_EINVAL; }
 	if (device && ((uintptr_t)cs16 & 3u) != 0) { set_error("d_cs16 must be 4-byte aligned"); return RXB200_EINVAL; }
+	if (m->ddc) { return ddc_call(m, cs16, n_int16, chunk_int16, pcm, pcm_stride, n_pcm, chunk_result_len, read, device, sync); }
 	// the member's own refusals, on the shape its call will see (the mixed streams sit in an aligned buffer)
 	size_t total = 0;
 	int rc = rxb::fm_check_host_call(m->h, cs16, n_int16, chunk_int16, pcm, pcm_stride, chunk_result_len, n_pcm, read,
@@ -261,15 +542,18 @@ extern "C" void rxb200_fm_mix_destroy(rxb200_fm_mix *m)
 	rxb200_fm_destroy(m->h);   // synchronises the stream the mixer runs on
 	cudaSetDevice(m->device);
 	cudaFree(m->d_tab); cudaFree(m->d_chan); cudaFree(m->d_cap); cudaFree(m->d_mix); cudaFree(m->d_out);
+	cudaFree(m->d_taps); cudaFree(m->d_hist[0]); cudaFree(m->d_hist[1]);
 	if (m->ev0) { cudaEventDestroy(m->ev0); }
 	if (m->ev1) { cudaEventDestroy(m->ev1); }
 	delete m;
 }
 
-extern "C" int rxb200_fm_mix_create(const rxb200_fm_params *params, int capture_rate, const int *offsets_hz,
-                                    int n_channels, int device, rxb200_fm_mix **out)
+namespace {
+
+// rxb200_fm_mix_create and rxb200_fm_mix_create_ddc (ddc != NULL, already checked)
+int mix_create(const rxb200_fm_params *params, int capture_rate, const int *offsets_hz, int n_channels,
+               const rxb200_ddc *ddc, bool wide, int device, rxb200_fm_mix **out)
 {
-	if (!params || !offsets_hz || !out || n_channels < 1) { set_error("bad mix arguments (n_channels >= 1)"); return RXB200_EINVAL; }
 	*out = nullptr;
 	// every table first: a refused offset fails before any device work
 	std::vector<int32_t> all, t;
@@ -296,16 +580,136 @@ extern "C" int rxb200_fm_mix_create(const rxb200_fm_params *params, int capture_
 	RXB_CUDA_OR(cudaMemcpy(m->d_chan, chan.data(), chan.size() * sizeof(MixChan), cudaMemcpyHostToDevice), rxb200_fm_mix_destroy(m));
 	RXB_CUDA_OR(cudaEventCreate(&m->ev0), rxb200_fm_mix_destroy(m));
 	RXB_CUDA_OR(cudaEventCreate(&m->ev1), rxb200_fm_mix_destroy(m));
+	if (ddc) {
+		m->ddc = true; m->wide = wide;
+		m->decim = ddc->decim; m->n_taps = ddc->n_taps; m->shift = ddc->shift;
+		const size_t T = (size_t)ddc->n_taps, hist_bytes = std::max<size_t>(1, T - 1) * 2 * sizeof(int16_t);
+		std::vector<int32_t> rev(ddc->taps, ddc->taps + T);
+		std::reverse(rev.begin(), rev.end());
+		RXB_CUDA_OR(cudaMalloc(&m->d_taps, T * sizeof(int32_t)), rxb200_fm_mix_destroy(m));
+		RXB_CUDA_OR(cudaMemcpy(m->d_taps, rev.data(), T * sizeof(int32_t), cudaMemcpyHostToDevice), rxb200_fm_mix_destroy(m));
+		for (int i = 0; i < 2; i++) {
+			RXB_CUDA_OR(cudaMalloc(&m->d_hist[i], hist_bytes), rxb200_fm_mix_destroy(m));
+			RXB_CUDA_OR(cudaMemset(m->d_hist[i], 0, hist_bytes), rxb200_fm_mix_destroy(m));
+		}
+	}
 	*out = m;
 	return RXB200_OK;
+}
+
+}  // namespace
+
+extern "C" int rxb200_fm_mix_create(const rxb200_fm_params *params, int capture_rate, const int *offsets_hz,
+                                    int n_channels, int device, rxb200_fm_mix **out)
+{
+	if (!params || !offsets_hz || !out || n_channels < 1) { set_error("bad mix arguments (n_channels >= 1)"); return RXB200_EINVAL; }
+	return mix_create(params, capture_rate, offsets_hz, n_channels, nullptr, false, device, out);
+}
+
+extern "C" int rxb200_fm_mix_create_ddc(const rxb200_fm_params *params, int capture_rate, const int *offsets_hz,
+                                        int n_channels, const rxb200_ddc *ddc, int device, rxb200_fm_mix **out)
+{
+	if (!params || !offsets_hz || !out || n_channels < 1) { set_error("bad mix arguments (n_channels >= 1)"); return RXB200_EINVAL; }
+	*out = nullptr;
+	bool wide = false;
+	const int rc = rxb::ddc_check(ddc, &wide);
+	if (rc != RXB200_OK) { return rc; }
+	return mix_create(params, capture_rate, offsets_hz, n_channels, ddc, wide, device, out);
+}
+
+int rxb::fm_mix_check_host_call(rxb200_fm_mix *m, const int16_t *cs16, size_t n_int16, size_t chunk_int16, int16_t *pcm,
+                                size_t pcm_stride, int *chunk_result_len, size_t *n_pcm, bool read, size_t *total)
+{
+	if (!m) { set_error("null argument"); return RXB200_EINVAL; }
+	if (!m->ddc) {
+		return rxb::fm_check_host_call(m->h, cs16, n_int16, chunk_int16, pcm, pcm_stride, chunk_result_len, n_pcm, read,
+		                               total);
+	}
+	size_t n16 = 0, chunk16 = 0;
+	return ddc_check_call(m, cs16, n_int16, chunk_int16, pcm, pcm_stride, chunk_result_len, n_pcm, read, total, &n16,
+	                      &chunk16);
+}
+
+extern "C" int rxb200_fm_mix_decimated_len(const rxb200_fm_mix *m, size_t n_int16, size_t *n_dec_int16)
+{
+	if (!m || !n_dec_int16) { set_error("null argument"); return RXB200_EINVAL; }
+	*n_dec_int16 = m->ddc ? ddc_len(m->pos, n_int16, m->decim) : n_int16;
+	return RXB200_OK;
+}
+
+extern "C" size_t rxb200_fm_mix_max_output(const rxb200_fm_mix *m, size_t n_int16, size_t chunk_int16)
+{
+	if (!m || chunk_int16 == 0) { return 0; }
+	if (!m->ddc) { return rxb200_fm_max_output(m->h, n_int16, chunk_int16); }
+	// floor((p + c) / M) - floor(p / M) <= ceil(c / M) at any phase p
+	const size_t M = (size_t)m->decim, n16 = 2 * ((n_int16 / 2 + M - 1) / M);
+	return rxb200_fm_max_output(m->h, n16, chunk_int16 / M ? chunk_int16 / M : 2);
+}
+
+extern "C" int rxb200_ddc_device(int capture_rate, int offset_hz, long long phase, const rxb200_ddc *ddc,
+                                 const int16_t *d_src, size_t n_complex, int16_t *d_dst, void *stream)
+{
+	if (!d_src || !d_dst || phase < 0) { set_error("bad ddc request (null pointer or negative phase)"); return RXB200_EINVAL; }
+	if (((uintptr_t)d_src & 3u) || ((uintptr_t)d_dst & 3u)) { set_error("pointers must be 4-byte aligned"); return RXB200_EINVAL; }
+	bool wide = false;
+	int rc = rxb::ddc_check(ddc, &wide);
+	if (rc != RXB200_OK) { return rc; }
+	std::vector<int32_t> t;
+	size_t L = 0;
+	rc = mix_table(capture_rate, offset_hz, t, &L);
+	const size_t T = (size_t)ddc->n_taps, n_out = n_complex / (size_t)ddc->decim;
+	if (rc != RXB200_OK || n_out == 0) { return rc; }
+	// one device block: the table, the channel, the reversed taps and a zero history
+	const size_t o_chan = L * sizeof(int2), o_taps = o_chan + sizeof(MixChan), o_hist = o_taps + T * sizeof(int32_t);
+	const size_t bytes = o_hist + std::max<size_t>(1, T - 1) * sizeof(uint32_t);
+	std::vector<unsigned char> h(bytes, 0);
+	const MixChan ch = mix_chan(0, L);
+	memcpy(h.data(), t.data(), o_chan);
+	memcpy(h.data() + o_chan, &ch, sizeof(MixChan));
+	for (size_t j = 0; j < T; j++) { memcpy(h.data() + o_taps + j * sizeof(int32_t), ddc->taps + (T - 1 - j), sizeof(int32_t)); }
+	const cudaStream_t st = (cudaStream_t)stream;
+	unsigned char *d = nullptr;
+	RXB_CUDA(cudaMallocAsync((void **)&d, bytes, st));
+	// from pageable memory: the copy has read its source when it returns
+	if (cudaMemcpyAsync(d, h.data(), bytes, cudaMemcpyHostToDevice, st) != cudaSuccess) {
+		set_error("ddc upload failed: %s", cudaGetErrorString(cudaGetLastError()));
+		rc = RXB200_ECUDA;
+	}
+	if (rc == RXB200_OK) {
+		DdcArgs a{};
+		a.src = reinterpret_cast<const uint32_t *>(d_src);
+		a.hist = reinterpret_cast<const uint32_t *>(d + o_hist);
+		a.n_out = (long long)n_out;
+		a.r0 = ddc->decim - 1;
+		a.pos = (unsigned long long)phase % L;
+		a.dst = reinterpret_cast<uint32_t *>(d_dst);
+		a.dst_stride = 0;
+		a.taps = reinterpret_cast<const int32_t *>(d + o_taps);
+		a.tab = reinterpret_cast<const int2 *>(d);
+		a.chan = reinterpret_cast<const MixChan *>(d + o_chan);
+		a.n_ch = 1; a.M = ddc->decim; a.T = ddc->n_taps; a.S = ddc->shift;
+		rc = ddc_launch(a, wide, st);
+	}
+	cudaFreeAsync(d, st);
+	return rc;
 }
 
 extern "C" int rxb200_fm_mix_reset(rxb200_fm_mix *m)
 {
 	if (!m) { return RXB200_EINVAL; }
 	const int rc = rxb200_fm_reset(m->h);
-	if (rc == RXB200_OK) { m->pos = 0; }
-	return rc;
+	if (rc != RXB200_OK) { return rc; }
+	if (m->ddc) {
+		// behind any call still running on the member's stream
+		const cudaStream_t st = (cudaStream_t)rxb200_fm_stream(m->h);
+		const size_t hist_bytes = std::max<size_t>(1, (size_t)m->n_taps - 1) * 2 * sizeof(int16_t);
+		RXB_CUDA(cudaSetDevice(m->device));
+		RXB_CUDA(cudaMemsetAsync(m->d_hist[0], 0, hist_bytes, st));
+		RXB_CUDA(cudaMemsetAsync(m->d_hist[1], 0, hist_bytes, st));
+		m->cur_hist = 0;
+	}
+	m->pos = 0;
+	return RXB200_OK;
 }
 
 extern "C" rxb200_fm *rxb200_fm_mix_member(rxb200_fm_mix *m) { return m ? m->h : nullptr; }

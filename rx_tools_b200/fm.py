@@ -285,21 +285,46 @@ def mix_device(capture_rate: int, offset_hz: int, phase: int, d_src_ptr: int, n_
                                             stream or None))
 
 
+def _ddc_c(ddc):
+    """(decim, taps, shift) -> (rxb200_ddc, the int32 taps it points at, to be kept alive for the call)."""
+    decim, taps, shift = ddc
+    t = np.ascontiguousarray(taps, dtype=np.int32).reshape(-1)
+    return _lib.DdcC(int(decim), int(t.size), t.ctypes.data_as(C.POINTER(C.c_int32)), int(shift)), t
+
+
+def ddc_device(capture_rate: int, offset_hz: int, phase: int, ddc, d_src_ptr: int, n_complex: int, d_dst_ptr: int,
+               stream: int = 0) -> None:
+    """The down-converter alone on device pointers (``rxb200_ddc_device``), asynchronous on ``stream``: zero samples
+    before d_src, the mixer from entry phase mod L, floor(n_complex / decim) outputs.  ddc: (decim, taps, shift)."""
+    d, _t = _ddc_c(ddc)
+    _lib.check(_lib.lib().rxb200_ddc_device(capture_rate, offset_hz, phase, C.byref(d), d_src_ptr, n_complex, d_dst_ptr,
+                                            stream or None))
+
+
 class FmMix:
     """``len(offsets_hz)`` channels of ONE CS16 capture at ``capture_rate`` (``rxb200_fm_mix_*``): channel k is
     ``FmDemod`` run on the capture mixed down by ``offsets_hz[k]`` with ``mix_table``; the mixers' phases carry across
-    calls.  Every call takes the one capture, int16[n_int16], and returns int16[n_channels][n_pcm]."""
+    calls.  Every call takes the one capture, int16[n_int16], and returns int16[n_channels][n_pcm].
+    ddc = (decim, taps, shift): a decimating handle (``rxb200_fm_mix_create_ddc``), each channel filtered by the int32
+    taps, rounded by the shift and decimated by decim before the chain."""
 
-    def __init__(self, params, capture_rate: int, offsets_hz, device: int = 0):
+    def __init__(self, params, capture_rate: int, offsets_hz, device: int = 0, ddc=None):
         self.params = FmParams.from_any(params)
         self.capture_rate = capture_rate
         offs = np.ascontiguousarray(offsets_hz, dtype=np.int32)
         self.offsets_hz = offs.tolist()
         self.n_channels = len(offs)
+        self.ddc = ddc
         self._m = C.c_void_p()
         pc = self.params.to_c()
-        _lib.check(_lib.lib().rxb200_fm_mix_create(C.byref(pc), capture_rate, offs.ctypes.data_as(C.POINTER(C.c_int)),
-                                                   self.n_channels, device, C.byref(self._m)))
+        po = offs.ctypes.data_as(C.POINTER(C.c_int))
+        if ddc is None:
+            _lib.check(_lib.lib().rxb200_fm_mix_create(C.byref(pc), capture_rate, po, self.n_channels, device,
+                                                       C.byref(self._m)))
+        else:
+            d, _t = _ddc_c(ddc)
+            _lib.check(_lib.lib().rxb200_fm_mix_create_ddc(C.byref(pc), capture_rate, po, self.n_channels, C.byref(d),
+                                                           device, C.byref(self._m)))
 
     def close(self) -> None:
         if _lib is not None and getattr(self, "_m", None) is not None and self._m:
@@ -315,8 +340,19 @@ class FmMix:
     def reset(self) -> None:
         _lib.check(_lib.lib().rxb200_fm_mix_reset(self._m))
 
+    def max_output(self, n_int16: int, chunk_int16: int = MAXIMUM_BUF_LENGTH) -> int:
+        """A bound on the PCM per channel of a call of n_int16 capture int16, at any phase
+        (``rxb200_fm_mix_max_output``)."""
+        return int(_lib.lib().rxb200_fm_mix_max_output(self._m, n_int16, chunk_int16))
+
+    def decimated_len(self, n_int16: int) -> int:
+        """int16 per channel the next call of n_int16 capture int16 hands the chain (``rxb200_fm_mix_decimated_len``)."""
+        n = C.c_size_t(0)
+        _lib.check(_lib.lib().rxb200_fm_mix_decimated_len(self._m, n_int16, C.byref(n)))
+        return int(n.value)
+
     def _cap(self, n_int16: int, chunk_int16: int) -> int:
-        return int(_lib.lib().rxb200_fm_max_output(C.c_void_p(self.member()), n_int16, chunk_int16)) + 8
+        return self.max_output(n_int16, chunk_int16) + 8
 
     def full_demod(self, cs16: np.ndarray, chunk_int16: int = MAXIMUM_BUF_LENGTH, return_chunks: bool = False):
         """As ``FmDemod.full_demod`` on every channel (``rxb200_fm_mix_process``); cs16: the capture, int16[n_int16]."""
@@ -387,7 +423,7 @@ class FmMix:
         return int(_lib.lib().rxb200_fm_stream(C.c_void_p(self.member())) or 0)
 
     def mix_ms(self) -> float:
-        """Device time of the last call's fm_mix_kernel."""
+        """Device time of the last call's fm_mix_kernel (fm_ddc_kernel for a decimating handle)."""
         ms = C.c_float(0)
         _lib.check(_lib.lib().rxb200_fm_mix_kernel_ms(self._m, C.byref(ms)))
         return float(ms.value)
@@ -403,22 +439,29 @@ class FmMixGroup:
     """The channels of ONE capture split over several GPUs (``rxb200_fm_mix_group_*``): member i is a ``FmMix`` on its
     own GPU with a contiguous block of the offsets, and every member gets a copy of the capture; the group's results
     are byte for byte those of one ``FmMix`` with all the offsets.  devices: one CUDA ordinal per member (may repeat),
-    or None for ``range(n_dev)``."""
+    or None for ``range(n_dev)``.  ddc = (decim, taps, shift): decimating members (``rxb200_fm_mix_group_create_ddc``),
+    byte for byte one ``FmMix`` with that ddc."""
 
-    def __init__(self, params, capture_rate: int, offsets_hz, devices=None, n_dev: Optional[int] = None):
+    def __init__(self, params, capture_rate: int, offsets_hz, devices=None, n_dev: Optional[int] = None, ddc=None):
         self.params = FmParams.from_any(params)
         self.capture_rate = capture_rate
         offs = np.ascontiguousarray(offsets_hz, dtype=np.int32)
         self.offsets_hz = offs.tolist()
         self.n_channels = len(offs)
+        self.ddc = ddc
         devs = None if devices is None else np.ascontiguousarray(devices, dtype=np.int32)
         self.n_dev = len(devs) if devs is not None else int(n_dev or 1)
         self._g = C.c_void_p()
         pc = self.params.to_c()
         dp = None if devs is None else devs.ctypes.data_as(C.POINTER(C.c_int))
-        _lib.check(_lib.lib().rxb200_fm_mix_group_create(C.byref(pc), capture_rate,
-                                                         offs.ctypes.data_as(C.POINTER(C.c_int)), self.n_channels,
-                                                         self.n_dev, dp, C.byref(self._g)))
+        po = offs.ctypes.data_as(C.POINTER(C.c_int))
+        if ddc is None:
+            _lib.check(_lib.lib().rxb200_fm_mix_group_create(C.byref(pc), capture_rate, po, self.n_channels, self.n_dev,
+                                                             dp, C.byref(self._g)))
+        else:
+            d, _t = _ddc_c(ddc)
+            _lib.check(_lib.lib().rxb200_fm_mix_group_create_ddc(C.byref(pc), capture_rate, po, self.n_channels,
+                                                                 C.byref(d), self.n_dev, dp, C.byref(self._g)))
 
     def close(self) -> None:
         if _lib is not None and getattr(self, "_g", None) is not None and self._g:
@@ -440,7 +483,7 @@ class FmMixGroup:
         _lib.check(_lib.lib().rxb200_fm_mix_group_reset(self._g))
 
     def _cap(self, n_int16: int, chunk_int16: int) -> int:
-        return int(_lib.lib().rxb200_fm_max_output(C.c_void_p(self.inner(0)), n_int16, chunk_int16)) + 8
+        return int(_lib.lib().rxb200_fm_mix_max_output(C.c_void_p(self.member(0)), n_int16, chunk_int16)) + 8
 
     def full_demod(self, cs16: np.ndarray, chunk_int16: int = MAXIMUM_BUF_LENGTH, return_chunks: bool = False):
         """As ``FmMix.full_demod`` (``rxb200_fm_mix_group_process``); cs16: the capture, int16[n_int16]."""
