@@ -143,7 +143,7 @@ static void *reader_thread(void *arg)
 	(void)arg;
 	/* what a read left over past the library's chunk granularity is carried into the next slot, never dropped: the
 	 * stream stays continuous whatever lengths the device returns (the reference hands any length on, :894-899).
-	 * Where every length is accepted (see main) nothing is carried but a read too short to decimate to a sample */
+	 * Where every length is accepted (see main) nothing is carried but a read below min_chunk */
 	static int16_t rem[8192];
 	size_t rem_n = 0;
 	SoapySDRDevice_activateStream(G.dev, G.stream, 0, 0, 0);
@@ -333,11 +333,14 @@ int main(int argc, char **argv)
 	if (rxb200_fm_derive(&G.cli, &G.der) != RXB200_OK) { fprintf(stderr, "rxb200: %s\n", rxb200_last_error()); return 1; }
 	if (G.der.params.post_downsample <= 1) {
 		/* no -o: every read is handed on as it was read, one rxb200_fm_process_read per read, like the reference's
-		 * full_demod per read; only a read too short to complete a boxcar, or with fifth_order passes shorter than 2^P
-		 * complex samples (for which the reference reads before its buffer), waits for the next */
-		const int P = G.der.params.downsample_passes;
+		 * full_demod per read, reads too short to complete a boxcar included.  Only a read with fifth_order passes
+		 * shorter than 2^P complex samples (for which the reference reads before its buffer), or one too short to
+		 * complete a boxcar when a per-chunk stage is on (the reference divides by its empty length), waits for the next */
+		const rxb200_fm_params *q = &G.der.params;
+		const int P = q->downsample_passes;
+		const int per_chunk = q->squelch_level || q->dc_block_audio || q->dc_block_raw || G.print_levels;
 		G.multiple = 2;
-		G.min_chunk = P ? (size_t)2 << P : 2 * (size_t)G.der.params.downsample;
+		G.min_chunk = P ? (size_t)2 << P : (per_chunk ? 2 * (size_t)q->downsample : 2);
 	} else {   /* -o N: chunk granularity accepted by the library: 16 int16 and 2*2^P int16 */
 		size_t m = (size_t)2 << G.der.params.downsample_passes;
 		G.multiple = m > 16 ? m : 16;

@@ -135,7 +135,9 @@ size_t rxb200_fm_max_output(const rxb200_fm *h, size_t n_int16, size_t chunk_int
  * any even length (whole complex samples, as readStream returns them).  With passes every chunk
  * (the last one included) is a multiple of 16 int16 and of 2*2^P int16.  Every chunk must produce
  * a decimated sample when a per-chunk reduction stage is on, and decimate to a multiple of
- * post_downsample.  rxb200_fm_process_device wants d_cs16 32-byte aligned, or 4-byte aligned for
+ * post_downsample.  Otherwise a chunk shorter than the boxcar may complete none: fm_demod's carried
+ * sample then becomes (0, 0), as the reference pinned in tests reads it (DESIGN.md section 4.1), so
+ * the next FM output is 0.  rxb200_fm_process_device wants d_cs16 32-byte aligned, or 4-byte aligned for
  * a call without passes whose chunk or length is not a multiple of 16 int16. */
 int rxb200_fm_process(rxb200_fm *h, const int16_t *cs16, size_t n_int16, size_t chunk_int16,
                       int16_t *pcm, size_t pcm_stride, size_t *n_pcm, int *chunk_result_len);
@@ -152,7 +154,8 @@ int rxb200_fm_process_device(rxb200_fm *h, const int16_t *d_cs16, size_t n_int16
  * Constraints (RXB200_EUNSUPPORTED otherwise): n_int16 even, 2 <= n_int16 <= 262144, and with
  * fifth_order passes n_int16 >= 2*2^P (below that the reference reads before its buffer).  The
  * read must produce a decimated sample when a per-chunk reduction stage is on, and decimate to a
- * multiple of post_downsample.  A read rxb200_fm_process(h, cs16, n_int16, n_int16, ...) takes
+ * multiple of post_downsample; otherwise a read shorter than the boxcar is accepted and carries
+ * (0, 0) on as in rxb200_fm_process.  A read rxb200_fm_process(h, cs16, n_int16, n_int16, ...) takes
  * runs exactly as that call; a read with passes off their granule runs on the any-length kernel
  * (kernel_kind 0), where every pass ends where the reference's does: raw mode then returns
  * n_int16 >> P values, an odd count when L_P = n_int16 >> P is odd.  A refused call leaves the

@@ -292,8 +292,14 @@ static void fm_discriminate(orx_fm *o)
 		}
 		o->pcm[k / 2] = (int16_t)v;
 	}
-	o->last_i = lp[o->iq_len - 2];
-	o->last_q = lp[o->iq_len - 1];
+	if (o->iq_len == 0) {
+		/* A chunk that completes no boxcar: :612-613 read lowpassed[-2], lowpassed[-1], the high half of
+		 * struct demod_state's `thread` (:126-127).  The reference harness never starts that thread, so both are 0. */
+		o->last_i = o->last_q = 0;
+	} else {
+		o->last_i = lp[o->iq_len - 2];
+		o->last_q = lp[o->iq_len - 1];
+	}
 	o->pcm_len = o->iq_len / 2;
 }
 

@@ -1263,10 +1263,14 @@ __device__ __forceinline__ void chunk_enter(const FmDev &c, const FmCall &k, Emi
 	if (c.post_ds > 1) { e.pds_acc = 0; e.pds_cnt = 0; }       // groups never span chunks
 }
 
-// chunk start inside front_run: every pass forgets the odd sample it was holding (SURVEY F7)
+// chunk start inside front_run: every pass forgets the odd sample it was holding (SURVEY F7).  Without passes a chunk
+// shorter than the boxcar may complete none: fm_demod then carries lowpassed[-2], lowpassed[-1] (src/rtl_fm.c:612-613),
+// which the pinned reference reads as 0 (DESIGN.md §4.1).  first_in_chunk still set here means the chunk just left
+// emitted nothing; only the FM discriminator reads pre.  The call's own first chunk start is not counted (front_item)
 template <int P, int SPEC, bool STORE>
 __device__ __forceinline__ void front_chunk_start(const FmDev &c, const FmCall &k, FrontState<P, SPEC> &s, EmitCtx &e, int ch)
 {
+	if constexpr (P == 0) { if (e.first_in_chunk) { s.pre_i = 0; s.pre_q = 0; } }
 	e.first_in_chunk = 1;
 	if (SPEC == 2) { chunk_enter<STORE>(c, k, e, ch, e.chunk_idx + 1); }
 #pragma unroll
@@ -1562,8 +1566,10 @@ __device__ __forceinline__ void front_item(const FmDev &c, const FmCall &k, cons
 	EmitCtx e;
 	e.pcm = pcm_s; e.out = k.out + (size_t)it.ch * (size_t)k.out_stride; e.m_lo = it.m_lo;
 	e.rel = (int)(m0 - it.m_lo);
+	// whether the chunk in progress at t0 has emitted nothing yet.  At the call's start the previous call's carry already
+	// holds the empty-chunk rule, so 0: the first chunk start must not apply it again
 	e.first_in_chunk = 0;
-	if (P == 0) { e.first_in_chunk = (dec_raw(c, t0 - u, it.box_n0) == dec_raw(c, t0, it.box_n0)) ? 1 : 0; }
+	if (P == 0 && t0 > 0) { e.first_in_chunk = (dec_raw(c, t0 - u, it.box_n0) == dec_raw(c, t0, it.box_n0)) ? 1 : 0; }
 	e.rdc_i = e.rdc_q = 0; e.sq_zero = 0; e.red_t = 0; e.red_p = 0;
 	e.pds_acc = 0; e.pds_cnt = 0; e.chunk_idx = 0;
 	if (SPEC == 2) {
@@ -1587,7 +1593,9 @@ __device__ __forceinline__ void front_item(const FmDev &c, const FmCall &k, cons
 	}
 	if (SPEC == 2 && k.reduce_mode == 1) { chunk_enter<true>(c, k, e, it.ch, e.chunk_idx); }   // flush the last chunk's sums
 	if (end == k.n && (SPEC != 2 || k.reduce_mode == 0)) {
-		// this thread saw the end of the stream: its registers are the next call's carry
+		// this thread saw the end of the stream: its registers are the next call's carry, with pre = (0, 0) when the
+		// call's last chunk emitted nothing (front_chunk_start)
+		if constexpr (P == 0) { if (e.first_in_chunk) { s.pre_i = 0; s.pre_q = 0; } }
 		if constexpr (ANY) { any_store<P, SPEC>(c, s, k.carry_out + (size_t)it.ch * k.state_words); }
 		else { front_store<P, SPEC>(s, k.carry_out + (size_t)it.ch * k.state_words); }
 	}

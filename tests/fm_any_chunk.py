@@ -27,6 +27,8 @@ USB = P(mode=M_USB, downsample=42, output_scale=6, rate_out=24000)              
 LSB = P(mode=M_LSB, downsample=42, output_scale=6, rate_out=24000)                            # -M lsb
 RAW = P(mode=M_RAW, downsample=42, output_scale=6, rate_out=24000)                            # -M raw
 FM5A = P(mode=M_FM, downsample=100, custom_atan=2, rate_out=24000)                            # bench fm5a channel
+NBFM12 = P(mode=M_FM, downsample=12, custom_atan=2, rate_out=25000)                           # 300 kHz -> 25 kHz, lut
+SHORT_STD = P(mode=M_FM, downsample=10, custom_atan=0, rate_out=100000)
 CLI = {"fm1": (FM1, dict(rate_s=1024000, rate_r=24000)),
        "fm2a": (FM2A, dict(wbfm=1, rate_s=2400000, rate_r=48000)),
        "wbfm": (WBFM, dict(wbfm=1)),
@@ -65,6 +67,32 @@ def shapes():
 
 
 INTEGER = lambda p: not (p.mode == M_FM and p.custom_atan == 0)    # noqa: E731  every result through integer arithmetic
+
+
+def per_chunk(p):
+    """A per-chunk stage is on: the library refuses a chunk that completes no boxcar (the reference divides by its empty
+    length, or takes the rms of nothing)."""
+    return bool(p.squelch_level or p.dc_block_raw or p.dc_block_audio)
+
+
+def shortest(p):
+    """Shortest chunk in complex samples a ragged draw of shape p may take: one sample, or two boxcars with a per-chunk
+    stage."""
+    return 2 * p.downsample if per_chunk(p) else 1
+
+
+# -o 2 at D = 12 without a per-chunk stage: chunk lengths (complex) that decimate to 2, 0, 2, 0, ... from a boxcar phase
+# of 0 and bring it back to 0, so that every chunk of the cycle, repeated, decimates to 0 or 2
+O2_CYCLE = [24, 6, 18, 4, 20, 11, 13]
+
+
+def after_empty(result_len):
+    """PCM indices of the first output of each chunk that follows a chunk with no output (the stream's first chunk
+    excluded): without a serial stage after the discriminator, the sample the reference makes from (0, 0)."""
+    rl = np.asarray(result_len, dtype=np.int64)
+    start = np.concatenate([[0], np.cumsum(rl)[:-1]])
+    hit = np.flatnonzero((rl[1:] > 0) & (rl[:-1] == 0)) + 1
+    return start[hit]
 
 
 def signal(n_complex, seed, quiet=False):
@@ -191,14 +219,13 @@ def ref_levels_seq(ref, params, cs16, lens16):
 
 
 def seq_len(lens16):
-    """A stream for a ragged sequence: the whole sequence, then its first chunk one sample short (every chunk, the
-    last one included, at least two boxcars long when ragged_lens drew it so)."""
+    """A stream for a ragged sequence: the whole sequence, then its first chunk one sample short."""
     return sum(lens16) // 2 + lens16[0] // 2 - 1
 
 
 def golden_cases():
-    """name -> (params, input, lens16): the benchmark shapes at chunks of 131071 / 131069 complex and one
-    ragged sequence per mode.  lens16 repeats until the stream ends (seq_bounds)."""
+    """name -> (params, input, lens16): the benchmark shapes at chunks of 131071 / 131069 complex, one ragged sequence
+    per mode, and sequences of chunks shorter than the boxcar.  lens16 repeats until the stream ends (seq_bounds)."""
     out = {}
     x1 = synth.cfg1_iq(1 << 20)
     for atan, an in ((0, "std"), (1, "fast"), (2, "lut")):
@@ -212,4 +239,12 @@ def golden_cases():
                     ("seq_am", AM), ("seq_usb", USB), ("seq_lsb", LSB), ("seq_raw", RAW)):
         lens = ragged_lens(rng, 12, 2 * p.downsample, 9000)
         out[name] = (p, signal(seq_len(lens), 400 + len(out)), lens)
+    # chunks shorter than the boxcar, runs of them completing none (the carried sample becomes (0, 0)); own rng, so
+    # the cases above keep their bytes
+    rng = np.random.default_rng(78)
+    for name, p, lo, hi in (("short_fm_lut_d12", NBFM12, 1, 24), ("short_fm_lut_d100", FM5A, 1, 130),
+                            ("short_fm_std_d10", SHORT_STD, 1, 20), ("short_fm_fast_d6_deemph", WBFM, 1, 12),
+                            ("short_am_d42", AM, 1, 84)):
+        lens = ragged_lens(rng, 40, lo, hi) + [2] * 12 + ragged_lens(rng, 8, lo, hi)
+        out[name] = (p, signal(seq_len(lens), 500 + len(out)), lens)
     return out

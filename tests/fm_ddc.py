@@ -76,7 +76,7 @@ def decimated_len(pos, n_int16, decim):
 
 READS = [2 * 20011, 2 * 37, 2 * 6007, 2 * 33331]     # complex 20011, 37, 6007, 33331: none a multiple of any M below
 READS_LONG = [2 * 20011, 2 * 6007, 2 * 33331]         # every read decimates past 2^P samples (fm2b's passes) and
-                                                      # hands the chain at least one boxcar (D = 12, 42)
+                                                      # hands the chain at least one boxcar (the squelch at D = 42)
 
 NBFM12 = with_(P(mode=M_FM, downsample=12, custom_atan=2, rate_out=25000), offset_tuning=1)   # 300 kHz -> 25 kHz, lut
 
@@ -85,6 +85,9 @@ SHAPES = {
     # 19.2 Msps, M = 64, 257 taps, 300 kHz into a D = 12 lut NBFM chain, channels on a 25 kHz raster out to +-9 MHz
     "nbfm_m64_t257": (NBFM12, 19_200_000, [-9_000_000, -25000, 0, 25000, 9_000_000],
                       (64, lowpass(257, 12500 / 19.2e6), 15), {}, READS_LONG),
+    # the same on READS: the 37-sample read decimates to 0 or 1 sample, a chain read that completes no boxcar
+    "nbfm_m64_t257_short": (NBFM12, 19_200_000, [-9_000_000, -25000, 0, 25000, 9_000_000],
+                            (64, lowpass(257, 12500 / 19.2e6), 15), {}, READS),
     # 19.2 Msps, M = 8 into fm2b's -F 9 chain (2.4 Msps, 3 passes), three broadcast channels
     "fm2b_f9_m8": (with_(frd.FM2B, offset_tuning=1), 19_200_000, [-4_800_000, 0, 3_000_000],
                    (8, lowpass(33, 120e3 / 19.2e6), 15), dict(deviation=75000.0), READS_LONG),

@@ -333,10 +333,6 @@ def fused_draw(seed: int) -> Draw:
     G = max(16, 2 << p.downsample_passes)            # int16 granularity of a chunk
     n16 = G * int(rng.integers(40_000 // G, 40_000 // G + 200_000 // (n_ch * G)))
     chunk16 = G * int(rng.integers((16 * D) // G + 1, min(262144, n16) // G + 1))
-    # the reference reads past a chunk that decimates to nothing: keep the last chunk at least a few boxcar periods
-    tail = (n16 % chunk16) // 2
-    if tail and p.downsample_passes == 0 and tail < 4 * D:
-        n16 += G * -(-(8 * D - 2 * tail) // G)
     cuts = _cuts(rng, -(-n16 // chunk16), chunk16, n16)
     x, kinds = _inputs(rng, n_ch, n16 // 2)
     exp = [expected_kind(p, n_ch, b - a_, chunk16, env, 0) for a_, b in zip(cuts[:-1], cuts[1:])]

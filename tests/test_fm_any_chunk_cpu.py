@@ -49,11 +49,46 @@ def test_ragged_sequences_port_equals_reference(name, port, ref_fm):
     p = SHAPES[name]
     rng = np.random.default_rng(zlib.crc32(name.encode()))
     for k in range(3):
-        lens = fac.ragged_lens(rng, 12, 2 * p.downsample, 6000 if k else 300)
+        lens = fac.ragged_lens(rng, 12, fac.shortest(p), 6000 if k else 300)
         x = _input(name, fac.seq_len(lens), 50 + k)
         a = fac.port_run_seq(port, p, x, lens, return_chunks=True)
         b = fac.ref_run_seq(ref_fm, p, x, lens, return_chunks=True)
         _assert_same(a, b, (name, k, lens))
+
+
+# chunks that complete no boxcar, in runs: (parameters, chunk lengths in complex samples, stream length)
+EMPTY_RUNS = {
+    "fm5a_chunks_of_1": (fac.FM5A, [1], 2500),
+    "lut_d12_chunks_of_8": (fac.NBFM12, [8], 1603),
+    "lut_d12_mixed": (fac.NBFM12, [8, 1, 3, 40, 2, 2, 5, 11, 24], 3001),
+    **{f"{an}_d10_mixed": (fac.with_(fac.SHORT_STD, custom_atan=a), [3, 4, 9, 1, 16, 2, 7], 2001)
+       for a, an in ((0, "std"), (1, "fast"), (2, "lut"), (3, "ale"))},
+    "fast_d6_deemph_resample": (fac.WBFM, [2, 3, 1, 5, 13], 3000),
+    "lut_d3_deemph_even": (fac.shapes()["fm_lut_d3_deemph_even"], [1, 1, 2, 1, 4], 1000),
+    "am_d42": (fac.AM, [8, 30, 1, 50], 3000),
+    "raw_d42": (fac.RAW, [8, 30, 1, 50], 3000),
+    # -o 2 at D = 12: the boxcar phase returns to 0 every cycle, every chunk decimates to 0 or 2
+    "lut_d12_o2": (fac.with_(fac.NBFM12, post_downsample=2), fac.O2_CYCLE, 20 * sum(fac.O2_CYCLE)),
+    "std_d12_o2_deemph": (fac.with_(fac.NBFM12, custom_atan=0, post_downsample=2, deemph=1, deemph_a=7),
+                          fac.O2_CYCLE, 20 * sum(fac.O2_CYCLE)),
+}
+
+
+@pytest.mark.ref
+@pytest.mark.parametrize("name", sorted(EMPTY_RUNS))
+def test_empty_chunk_runs_port_equals_reference(name, port, ref_fm):
+    """Runs of chunks too short to complete a boxcar: after each, fm_demod carries (0, 0) in the reference, and the next
+    emitting chunk's first output is exactly 0."""
+    p, chunks, n = EMPTY_RUNS[name]
+    lens = [2 * c for c in chunks]
+    x = fac.signal(n, zlib.crc32(name.encode()) % 1000)
+    a = fac.port_run_seq(port, p, x, lens, return_chunks=True)
+    b = fac.ref_run_seq(ref_fm, p, x, lens, return_chunks=True)
+    _assert_same(a, b, name)
+    assert np.any(a[1] == 0) and np.any(a[1] > 0), name
+    if p.mode == fac.M_FM and not (p.deemph or p.rate_out2 > 0 or p.post_downsample > 1):
+        zero = fac.after_empty(a[1])
+        assert zero.size and np.all(a[0][zero] == 0), name
 
 
 @pytest.mark.ref

@@ -180,10 +180,12 @@ def _random_case(rng):
         p["rdc_block_const"] = int(rng.choice([1, 9, 30]))
     elif opt < 0.45:
         p["dc_block_audio"] = 1
-    # any chunk length that decimates to a sample or more; a stream with a short last chunk of at least one boxcar
-    chunk_c = int(rng.integers(max(D, 2), min(131072, D * int(rng.integers(2, 400))) + 1))
+    # any chunk length, down to one sample when no per-chunk stage is on (such a stage refuses a chunk that decimates
+    # to nothing); a stream with a shorter last chunk
+    lo = D if "squelch_level" in p or "dc_block_raw" in p or "dc_block_audio" in p else 1
+    chunk_c = int(rng.integers(lo, min(131072, D * int(rng.integers(2, 400))) + 1))
     n_chunks = int(rng.integers(2, 9))
-    tail = int(rng.integers(D, chunk_c + 1))
+    tail = int(rng.integers(lo, chunk_c + 1))
     return oracle.FmParams(**p), chunk_c, (n_chunks - 1) * chunk_c + tail
 
 
@@ -288,16 +290,29 @@ def _run(cmd):
     return r
 
 
-def _capture(tmp_path, x):
+SHORT_READS = [1021, 5, 333, 17, 41, 4093]      # reads of 5, 17 and 41 samples complete no boxcar at D = 42
+
+
+def _capture(tmp_path, x, reads=READS):
     cap = tmp_path / "cap.cs16"
     x.tofile(cap)
-    return f"driver=file,path={cap},reads={':'.join(map(str, READS))}"
+    return f"driver=file,path={cap},reads={':'.join(map(str, reads))}"
 
 
-def _stream(n_complex, seed):
+def _stream(n_complex, seed, reads=READS):
     # whole cycles of reads plus a last read that still holds two boxcars
-    n = (n_complex // sum(READS)) * sum(READS) + 611
+    n = (n_complex // sum(reads)) * sum(reads) + 611
     return fac.signal(n, seed)
+
+
+def _dropin_equals_port(tmp_path, port, args, p, reads):
+    x = _stream(120_000, 5, reads)
+    out = tmp_path / "out.raw"
+    _run([RX_FM, "-f", "100M", "-d", _capture(tmp_path, x, reads)] + args + [str(out)])
+    want = fac.port_run_seq(port, p, x, [2 * r for r in reads])
+    got = np.fromfile(out, dtype=np.int16)
+    assert got.size == want.size
+    assert np.array_equal(got, want)
 
 
 @pytest.mark.parametrize("args,p", [
@@ -307,13 +322,17 @@ def _stream(n_complex, seed):
     (["-M", "raw"], fac.RAW),
 ])
 def test_dropin_reads_of_odd_lengths(tmp_path, port, built, args, p):
-    x = _stream(120_000, 5)
-    out = tmp_path / "out.raw"
-    _run([RX_FM, "-f", "100M", "-d", _capture(tmp_path, x)] + args + [str(out)])
-    want = fac.port_run_seq(port, p, x, [2 * r for r in READS])
-    got = np.fromfile(out, dtype=np.int16)
-    assert got.size == want.size
-    assert np.array_equal(got, want)
+    _dropin_equals_port(tmp_path, port, args, p, READS)
+
+
+@pytest.mark.parametrize("args,p", [
+    (["-M", "fm", "-s", "24k", "-A", "lut"], fac.FM24K_LUT),
+    (["-M", "wbfm"], fac.WBFM),
+])
+def test_dropin_reads_shorter_than_the_boxcar(tmp_path, port, built, args, p):
+    """Without -o, passes or a per-chunk stage every read is handed on as it came, reads too short to complete a
+    boxcar included."""
+    _dropin_equals_port(tmp_path, port, args, p, SHORT_READS)
 
 
 def test_dropin_level_printing_per_read(tmp_path, port, built):

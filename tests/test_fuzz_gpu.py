@@ -56,10 +56,12 @@ def _random_case(rng):
     n_chunks = int(rng.integers(2, 9))
     n_c = chunk_c * n_chunks
     if rng.random() < 0.4 and not p.get("post_downsample", 1) > 1:
-        # ragged last chunk: shorter but still long enough to produce output (the reference's fm_demod reads
-        # out of bounds on a chunk that decimates to nothing)
-        tail = int(rng.integers(max(1, 4 * D * 2 // gran + 1), max(2, chunk_c * 2 // gran))) * (gran // 2)
-        n_c = n_c - chunk_c + max(min(tail, chunk_c), gran // 2 * ((4 * D) // (gran // 2) + 1))
+        # ragged last chunk: without passes or a per-chunk stage as short as one block, which may complete no boxcar;
+        # otherwise still long enough to produce output (a per-chunk stage refuses a chunk that decimates to nothing)
+        short = P == 0 and not (p.get("squelch_level") or p.get("dc_block_raw") or p.get("dc_block_audio"))
+        tail = int(rng.integers(1 if short else max(1, 4 * D * 2 // gran + 1), max(2, chunk_c * 2 // gran))) * (gran // 2)
+        n_c = n_c - chunk_c + (min(tail, chunk_c) if short else
+                               max(min(tail, chunk_c), gran // 2 * ((4 * D) // (gran // 2) + 1)))
         n_c = min(n_c, chunk_c * n_chunks)
     return p, chunk_c, n_c
 
