@@ -130,11 +130,11 @@ int group_process(Group *g, const int16_t *cs16, size_t n_int16, size_t chunk_in
 	if (!g || !cs16 || !pcm) { set_error("null argument"); return RXB200_EINVAL; }
 	DeviceGuard guard;
 	// every refusal first, on every member, so that a refused call starts none of them
-	size_t total = 0;
+	size_t total = 0, n16 = 0, chunk16 = 0;
 	for (Member &mb : g->mb) {
 		if (!mb.h) { continue; }
 		const int rc = mb.m ? rxb::fm_mix_check_host_call(mb.m, cs16, n_int16, chunk_int16, pcm, pcm_stride,
-		                                                  chunk_result_len, n_pcm, read, &total)
+		                                                  chunk_result_len, n_pcm, read, &total, &n16, &chunk16)
 		                    : rxb::fm_check_host_call(mb.h, cs16, n_int16, chunk_int16, pcm, pcm_stride, chunk_result_len,
 		                                              n_pcm, read, &total);
 		if (rc != RXB200_OK) { return rc; }

@@ -1,7 +1,10 @@
 // fm_mix.cu — several rx_fm channels of one wideband capture (include/rxb200.h, "rx_fm channels of one capture").
 // fm_mix_kernel mixes the capture to baseband once per channel with that channel's integer table, reading the capture
 // once and writing one CS16 stream per channel; a plain rxb200_fm handle with one channel per stream then runs the
-// chain on them through its device entry points.  The chain itself is not touched here.
+// chain on them through its device entry points.  A decimating handle (rxb200_fm_mix_create_ddc) runs fm_ddc_kernel
+// instead, which mixes, filters and decimates, and carries the capture's last T - 1 samples between calls.  Every
+// process entry point of both kinds goes through mix_call, whose refusals and member shape come from
+// fm_mix_check_host_call (which the group uses too).  The chain itself is not touched here.
 #include <algorithm>
 #include <cstring>
 #include <new>
@@ -352,14 +355,24 @@ size_t ddc_len(unsigned long long pos, size_t n_int16, int decim)
 	return 2 * (size_t)((pos + n_int16 / 2) / M - pos / M);
 }
 
-// The refusals of a decimating handle's call and what its member's call will be: *n16 and *chunk16, the decimated
-// call (n16 == 0: no member call).  The member's own refusals run on that shape.  A read with no output reports what
-// an empty call of the member reports (no PCM, no level chunks); chunk_result_len entries of capture chunks past the
-// member's chunks are 0.
-int ddc_check_call(rxb200_fm_mix *m, const int16_t *cs16, size_t n_int16, size_t chunk_int16, int16_t *pcm,
-                   size_t pcm_stride, int *chunk_result_len, size_t *n_pcm, bool read, size_t *total, size_t *n16,
-                   size_t *chunk16)
+}  // namespace
+
+// Every refusal of a mixing handle's call, in the order the call reports them, without enqueuing anything; *total
+// receives the PCM count per channel, *n16 and *chunk16 the member's call (n16 == 0: no member call).  A plain handle's
+// member sees the call's own shape.  A decimating handle's member sees the decimated one: a read with no output reports
+// what an empty call of the member reports (no PCM, no level chunks), and chunk_result_len entries of capture chunks
+// past the member's chunks are 0.
+int rxb::fm_mix_check_host_call(rxb200_fm_mix *m, const int16_t *cs16, size_t n_int16, size_t chunk_int16, int16_t *pcm,
+                                size_t pcm_stride, int *chunk_result_len, size_t *n_pcm, bool read, size_t *total,
+                                size_t *n16, size_t *chunk16)
 {
+	if (!m) { set_error("null argument"); return RXB200_EINVAL; }
+	if (!m->ddc) {
+		*n16 = n_int16;
+		*chunk16 = chunk_int16;
+		return rxb::fm_check_host_call(m->h, cs16, n_int16, chunk_int16, pcm, pcm_stride, chunk_result_len, n_pcm, read,
+		                               total);
+	}
 	if (!cs16 || !pcm) { set_error("null argument"); return RXB200_EINVAL; }
 	const size_t M = (size_t)m->decim;
 	if (n_int16 % 2 != 0) { set_error("n_int16=%zu must be even", n_int16); return RXB200_EUNSUPPORTED; }
@@ -381,7 +394,10 @@ int ddc_check_call(rxb200_fm_mix *m, const int16_t *cs16, size_t n_int16, size_t
 	return rc;
 }
 
-// The next history: the last T - 1 samples of (history, the call's c capture samples at src), into the spare buffer
+namespace {
+
+// The next history: the last T - 1 samples of (history, the call's c capture samples at src), into the spare buffer.
+// A plain handle has T = 1: no history.
 int ddc_carry(rxb200_fm_mix *m, const int16_t *src, size_t c, cudaStream_t st)
 {
 	const size_t H = (size_t)m->n_taps - 1, w = 2 * sizeof(int16_t);
@@ -397,13 +413,34 @@ int ddc_carry(rxb200_fm_mix *m, const int16_t *src, size_t c, cudaStream_t st)
 	return RXB200_OK;
 }
 
-// mix_call for a decimating handle: fm_ddc_kernel, then the member on the decimated streams
-int ddc_call(rxb200_fm_mix *m, const int16_t *cs16, size_t n_int16, size_t chunk_int16, int16_t *pcm, size_t pcm_stride,
+// a decimating handle's front stage: fm_ddc_kernel from the call's capture at src to n16 int16 per channel in d_mix
+int ddc_front(rxb200_fm_mix *m, const int16_t *src, size_t n16, cudaStream_t st)
+{
+	DdcArgs a{};
+	a.src = reinterpret_cast<const uint32_t *>(src);
+	a.hist = reinterpret_cast<const uint32_t *>(m->d_hist[m->cur_hist]);
+	a.n_out = (long long)(n16 / 2);
+	a.r0 = (long long)(m->decim - 1) - (long long)(m->pos % (unsigned long long)m->decim);
+	a.pos = m->pos;
+	a.dst = reinterpret_cast<uint32_t *>(m->d_mix);
+	a.dst_stride = (long long)(n16 / 2);
+	a.taps = m->d_taps; a.tab = m->d_tab; a.chan = m->d_chan;
+	a.n_ch = m->n_channels; a.M = m->decim; a.T = m->n_taps; a.S = m->shift;
+	return ddc_launch(a, m->wide, st);
+}
+
+// One call of any process entry point.  device: cs16 and pcm are device pointers (the member's device entry point
+// writes pcm), else host pointers staged through the handle's buffers.  read: one read (chunk_int16 == n_int16).  The
+// front stage (fm_mix_kernel, or fm_ddc_kernel for a decimating handle) writes the member's input to d_mix; when it has
+// no output (n16 == 0) neither it nor the member runs, but the phases and the history still advance.
+int mix_call(rxb200_fm_mix *m, const int16_t *cs16, size_t n_int16, size_t chunk_int16, int16_t *pcm, size_t pcm_stride,
              size_t *n_pcm, int *chunk_result_len, bool read, bool device, int sync)
 {
+	if (!m) { set_error("null argument"); return RXB200_EINVAL; }
+	if (device && ((uintptr_t)cs16 & 3u) != 0) { set_error("d_cs16 must be 4-byte aligned"); return RXB200_EINVAL; }
 	size_t total = 0, n16 = 0, chunk16 = 0;
-	int rc = ddc_check_call(m, cs16, n_int16, chunk_int16, pcm, pcm_stride, chunk_result_len, n_pcm, read, &total, &n16,
-	                        &chunk16);
+	int rc = rxb::fm_mix_check_host_call(m, cs16, n_int16, chunk_int16, pcm, pcm_stride, chunk_result_len, n_pcm, read,
+	                                     &total, &n16, &chunk16);
 	if (rc != RXB200_OK || n_int16 == 0) { return rc; }
 	RXB_CUDA(cudaSetDevice(m->device));
 	const cudaStream_t st = (cudaStream_t)rxb200_fm_stream(m->h);
@@ -418,17 +455,8 @@ int ddc_call(rxb200_fm_mix *m, const int16_t *cs16, size_t n_int16, size_t chunk
 	}
 	RXB_CUDA(cudaEventRecord(m->ev0, st));
 	if (n16) {
-		DdcArgs a{};
-		a.src = reinterpret_cast<const uint32_t *>(src);
-		a.hist = reinterpret_cast<const uint32_t *>(m->d_hist[m->cur_hist]);
-		a.n_out = (long long)(n16 / 2);
-		a.r0 = (long long)(m->decim - 1) - (long long)(m->pos % (unsigned long long)m->decim);
-		a.pos = m->pos;
-		a.dst = reinterpret_cast<uint32_t *>(m->d_mix);
-		a.dst_stride = (long long)(n16 / 2);
-		a.taps = m->d_taps; a.tab = m->d_tab; a.chan = m->d_chan;
-		a.n_ch = m->n_channels; a.M = m->decim; a.T = m->n_taps; a.S = m->shift;
-		rc = ddc_launch(a, m->wide, st);
+		rc = m->ddc ? ddc_front(m, src, n16, st)
+		            : mix_launch(src, (long long)c, m->d_mix, (long long)n16, m->d_tab, m->d_chan, m->chan, m->pos, st);
 		if (rc != RXB200_OK) { return rc; }
 	}
 	RXB_CUDA(cudaEventRecord(m->ev1, st));
@@ -448,8 +476,8 @@ int ddc_call(rxb200_fm_mix *m, const int16_t *cs16, size_t n_int16, size_t chunk
 			                           total * sizeof(int16_t), K, cudaMemcpyDeviceToHost, st));
 		}
 		RXB_CUDA(cudaStreamSynchronize(st));
-	} else if (sync) {
-		RXB_CUDA(cudaStreamSynchronize(st));
+	} else if (sync && n16 == 0) {
+		RXB_CUDA(cudaStreamSynchronize(st));    // with output, the member's call has synchronised
 	}
 	if (m->n_taps > 1) { m->cur_hist ^= 1; }
 	m->pos += c;
@@ -457,49 +485,39 @@ int ddc_call(rxb200_fm_mix *m, const int16_t *cs16, size_t n_int16, size_t chunk
 	return RXB200_OK;
 }
 
-// One call of any process entry point.  device: cs16 and pcm are device pointers (the member's device entry point
-// writes pcm), else host pointers staged through the handle's buffers.  read: one read (chunk_int16 == n_int16).
-int mix_call(rxb200_fm_mix *m, const int16_t *cs16, size_t n_int16, size_t chunk_int16, int16_t *pcm, size_t pcm_stride,
-             size_t *n_pcm, int *chunk_result_len, bool read, bool device, int sync)
+// The device block of a one-channel call of the mixer or the DDC alone: the table, the channel record and, for a DDC,
+// the reversed taps and a zero history, uploaded with one allocation and one copy on st.  The caller frees o->d with
+// cudaFreeAsync on st behind its launch.
+struct OneChannel {
+	unsigned char *d = nullptr;
+	const int2 *tab = nullptr;
+	const MixChan *chan = nullptr;
+	const int32_t *taps = nullptr;
+	const uint32_t *hist = nullptr;
+};
+
+int upload_one(const std::vector<int32_t> &t, size_t L, const rxb200_ddc *ddc, cudaStream_t st, OneChannel *o)
 {
-	if (!m) { set_error("null argument"); return RXB200_EINVAL; }
-	if (device && ((uintptr_t)cs16 & 3u) != 0) { set_error("d_cs16 must be 4-byte aligned"); return RXB200_EINVAL; }
-	if (m->ddc) { return ddc_call(m, cs16, n_int16, chunk_int16, pcm, pcm_stride, n_pcm, chunk_result_len, read, device, sync); }
-	// the member's own refusals, on the shape its call will see (the mixed streams sit in an aligned buffer)
-	size_t total = 0;
-	int rc = rxb::fm_check_host_call(m->h, cs16, n_int16, chunk_int16, pcm, pcm_stride, chunk_result_len, n_pcm, read,
-	                                 &total);
-	if (rc != RXB200_OK || n_int16 == 0) { return rc; }
-	RXB_CUDA(cudaSetDevice(m->device));
-	const cudaStream_t st = (cudaStream_t)rxb200_fm_stream(m->h);
-	const size_t K = (size_t)m->n_channels;
-	RXB_CUDA(reserve(m->d_mix, m->mix_cap, n_int16 * K));
-	const int16_t *src = cs16;
-	if (!device) {
-		RXB_CUDA(reserve(m->d_cap, m->cap_cap, n_int16));
-		RXB_CUDA(reserve(m->d_out, m->out_cap, (total + 8) * K));
-		RXB_CUDA(cudaMemcpyAsync(m->d_cap, cs16, n_int16 * sizeof(int16_t), cudaMemcpyHostToDevice, st));
-		src = m->d_cap;
+	const size_t T = ddc ? (size_t)ddc->n_taps : 0;
+	const size_t o_chan = L * sizeof(int2), o_taps = o_chan + sizeof(MixChan), o_hist = o_taps + T * sizeof(int32_t);
+	const size_t bytes = o_hist + (ddc ? std::max<size_t>(1, T - 1) * sizeof(uint32_t) : 0);
+	std::vector<unsigned char> h(bytes, 0);
+	const MixChan ch = mix_chan(0, L);
+	memcpy(h.data(), t.data(), o_chan);
+	memcpy(h.data() + o_chan, &ch, sizeof(MixChan));
+	for (size_t j = 0; j < T; j++) { memcpy(h.data() + o_taps + j * sizeof(int32_t), ddc->taps + (T - 1 - j), sizeof(int32_t)); }
+	RXB_CUDA(cudaMallocAsync((void **)&o->d, bytes, st));
+	// from pageable memory: the copy has read its source when it returns
+	if (cudaMemcpyAsync(o->d, h.data(), bytes, cudaMemcpyHostToDevice, st) != cudaSuccess) {
+		set_error("%s upload failed: %s", ddc ? "ddc" : "table", cudaGetErrorString(cudaGetLastError()));
+		cudaFreeAsync(o->d, st);
+		o->d = nullptr;
+		return RXB200_ECUDA;
 	}
-	RXB_CUDA(cudaEventRecord(m->ev0, st));
-	rc = mix_launch(src, (long long)(n_int16 / 2), m->d_mix, (long long)n_int16, m->d_tab, m->d_chan, m->chan, m->pos, st);
-	if (rc != RXB200_OK) { return rc; }
-	RXB_CUDA(cudaEventRecord(m->ev1, st));
-	int16_t *out = device ? pcm : m->d_out;
-	const size_t stride = device ? pcm_stride : total + 8;
-	size_t n = 0;
-	rc = read ? rxb200_fm_process_read_device(m->h, m->d_mix, n_int16, out, stride, &n, device ? sync : 0)
-	          : rxb200_fm_process_device(m->h, m->d_mix, n_int16, chunk_int16, out, stride, &n, device ? sync : 0);
-	if (rc != RXB200_OK) { return rc; }
-	if (!device) {
-		if (total) {
-			RXB_CUDA(cudaMemcpy2DAsync(pcm, pcm_stride * sizeof(int16_t), m->d_out, (total + 8) * sizeof(int16_t),
-			                           total * sizeof(int16_t), K, cudaMemcpyDeviceToHost, st));
-		}
-		RXB_CUDA(cudaStreamSynchronize(st));
-	}
-	m->pos += n_int16 / 2;
-	if (n_pcm) { *n_pcm = total; }
+	o->tab = reinterpret_cast<const int2 *>(o->d);
+	o->chan = reinterpret_cast<const MixChan *>(o->d + o_chan);
+	o->taps = reinterpret_cast<const int32_t *>(o->d + o_taps);
+	o->hist = reinterpret_cast<const uint32_t *>(o->d + o_hist);
 	return RXB200_OK;
 }
 
@@ -515,24 +533,12 @@ extern "C" int rxb200_mix_device(int capture_rate, int offset_hz, long long phas
 	int rc = mix_table(capture_rate, offset_hz, t, &L);
 	if (rc != RXB200_OK || n_complex == 0) { return rc; }
 	const cudaStream_t st = (cudaStream_t)stream;
-	const std::vector<MixChan> chan(1, mix_chan(0, L));
-	int2 *d_tab = nullptr;
-	MixChan *d_chan = nullptr;
-	RXB_CUDA(cudaMallocAsync(&d_tab, L * sizeof(int2), st));
-	if (cudaMallocAsync(&d_chan, sizeof(MixChan), st) != cudaSuccess) {
-		cudaFreeAsync(d_tab, st); set_error("cudaMallocAsync failed"); return RXB200_ECUDA;
-	}
-	// from pageable memory: each copy has read its source when it returns
-	if (cudaMemcpyAsync(d_tab, t.data(), L * sizeof(int2), cudaMemcpyHostToDevice, st) != cudaSuccess ||
-	    cudaMemcpyAsync(d_chan, chan.data(), sizeof(MixChan), cudaMemcpyHostToDevice, st) != cudaSuccess) {
-		set_error("table upload failed: %s", cudaGetErrorString(cudaGetLastError()));
-		rc = RXB200_ECUDA;
-	}
-	if (rc == RXB200_OK) {
-		rc = mix_launch(d_src, (long long)n_complex, d_dst, 0, d_tab, d_chan, chan, (unsigned long long)phase % L, st);
-	}
-	cudaFreeAsync(d_tab, st);
-	cudaFreeAsync(d_chan, st);
+	OneChannel o;
+	rc = upload_one(t, L, nullptr, st, &o);
+	if (rc != RXB200_OK) { return rc; }
+	rc = mix_launch(d_src, (long long)n_complex, d_dst, 0, o.tab, o.chan, std::vector<MixChan>(1, mix_chan(0, L)),
+	                (unsigned long long)phase % L, st);
+	cudaFreeAsync(o.d, st);
 	return rc;
 }
 
@@ -617,19 +623,6 @@ extern "C" int rxb200_fm_mix_create_ddc(const rxb200_fm_params *params, int capt
 	return mix_create(params, capture_rate, offsets_hz, n_channels, ddc, wide, device, out);
 }
 
-int rxb::fm_mix_check_host_call(rxb200_fm_mix *m, const int16_t *cs16, size_t n_int16, size_t chunk_int16, int16_t *pcm,
-                                size_t pcm_stride, int *chunk_result_len, size_t *n_pcm, bool read, size_t *total)
-{
-	if (!m) { set_error("null argument"); return RXB200_EINVAL; }
-	if (!m->ddc) {
-		return rxb::fm_check_host_call(m->h, cs16, n_int16, chunk_int16, pcm, pcm_stride, chunk_result_len, n_pcm, read,
-		                               total);
-	}
-	size_t n16 = 0, chunk16 = 0;
-	return ddc_check_call(m, cs16, n_int16, chunk_int16, pcm, pcm_stride, chunk_result_len, n_pcm, read, total, &n16,
-	                      &chunk16);
-}
-
 extern "C" int rxb200_fm_mix_decimated_len(const rxb200_fm_mix *m, size_t n_int16, size_t *n_dec_int16)
 {
 	if (!m || !n_dec_int16) { set_error("null argument"); return RXB200_EINVAL; }
@@ -657,40 +650,24 @@ extern "C" int rxb200_ddc_device(int capture_rate, int offset_hz, long long phas
 	std::vector<int32_t> t;
 	size_t L = 0;
 	rc = mix_table(capture_rate, offset_hz, t, &L);
-	const size_t T = (size_t)ddc->n_taps, n_out = n_complex / (size_t)ddc->decim;
+	const size_t n_out = n_complex / (size_t)ddc->decim;
 	if (rc != RXB200_OK || n_out == 0) { return rc; }
-	// one device block: the table, the channel, the reversed taps and a zero history
-	const size_t o_chan = L * sizeof(int2), o_taps = o_chan + sizeof(MixChan), o_hist = o_taps + T * sizeof(int32_t);
-	const size_t bytes = o_hist + std::max<size_t>(1, T - 1) * sizeof(uint32_t);
-	std::vector<unsigned char> h(bytes, 0);
-	const MixChan ch = mix_chan(0, L);
-	memcpy(h.data(), t.data(), o_chan);
-	memcpy(h.data() + o_chan, &ch, sizeof(MixChan));
-	for (size_t j = 0; j < T; j++) { memcpy(h.data() + o_taps + j * sizeof(int32_t), ddc->taps + (T - 1 - j), sizeof(int32_t)); }
 	const cudaStream_t st = (cudaStream_t)stream;
-	unsigned char *d = nullptr;
-	RXB_CUDA(cudaMallocAsync((void **)&d, bytes, st));
-	// from pageable memory: the copy has read its source when it returns
-	if (cudaMemcpyAsync(d, h.data(), bytes, cudaMemcpyHostToDevice, st) != cudaSuccess) {
-		set_error("ddc upload failed: %s", cudaGetErrorString(cudaGetLastError()));
-		rc = RXB200_ECUDA;
-	}
-	if (rc == RXB200_OK) {
-		DdcArgs a{};
-		a.src = reinterpret_cast<const uint32_t *>(d_src);
-		a.hist = reinterpret_cast<const uint32_t *>(d + o_hist);
-		a.n_out = (long long)n_out;
-		a.r0 = ddc->decim - 1;
-		a.pos = (unsigned long long)phase % L;
-		a.dst = reinterpret_cast<uint32_t *>(d_dst);
-		a.dst_stride = 0;
-		a.taps = reinterpret_cast<const int32_t *>(d + o_taps);
-		a.tab = reinterpret_cast<const int2 *>(d);
-		a.chan = reinterpret_cast<const MixChan *>(d + o_chan);
-		a.n_ch = 1; a.M = ddc->decim; a.T = ddc->n_taps; a.S = ddc->shift;
-		rc = ddc_launch(a, wide, st);
-	}
-	cudaFreeAsync(d, st);
+	OneChannel o;
+	rc = upload_one(t, L, ddc, st, &o);
+	if (rc != RXB200_OK) { return rc; }
+	DdcArgs a{};
+	a.src = reinterpret_cast<const uint32_t *>(d_src);
+	a.hist = o.hist;
+	a.n_out = (long long)n_out;
+	a.r0 = ddc->decim - 1;
+	a.pos = (unsigned long long)phase % L;
+	a.dst = reinterpret_cast<uint32_t *>(d_dst);
+	a.dst_stride = 0;
+	a.taps = o.taps; a.tab = o.tab; a.chan = o.chan;
+	a.n_ch = 1; a.M = ddc->decim; a.T = ddc->n_taps; a.S = ddc->shift;
+	rc = ddc_launch(a, wide, st);
+	cudaFreeAsync(o.d, st);
 	return rc;
 }
 

@@ -73,8 +73,117 @@ def derive_params(mode: int = MODE_FM, rate_s: int = 0, rate_r: int = 0, use_F: 
     return Derived(FmParams.from_any(out.params), out.capture_rate, out.capture_freq_offset, out.output_rate)
 
 
-class FmDemod:
+class _Handle:
+    """What the four rx_fm handle kinds share: ``_prefix`` names their C entry points (``<prefix>_process`` ...), ``_h``
+    holds the handle.  A subclass states how it is created, whether its input is per-channel streams
+    (``_streams``: int16[n_int16] or int16[n_channels][n_int16]) or one capture (int16[n_int16]), and ``_bound``, the
+    PCM per channel a call can make."""
+
+    _prefix = ""
+    _streams = True
+
+    def _fn(self, name: str):
+        return getattr(_lib.lib(), f"{self._prefix}_{name}")
+
+    def close(self) -> None:
+        if _lib is not None and getattr(self, "_h", None) is not None and self._h:
+            self._fn("destroy")(self._h)
+            self._h = None
+
+    __del__ = close
+
+    def reset(self) -> None:
+        _lib.check(self._fn("reset")(self._h))
+
+    def _input(self, cs16):
+        """(the input as one C array, n_int16, whether a 1-D input of a one-channel stream handle returns 1-D)"""
+        x = np.ascontiguousarray(cs16, dtype=np.int16)
+        if not self._streams:
+            x = x.reshape(-1)
+            return x, x.size, False
+        x2 = x.reshape(1, -1) if x.ndim == 1 else x
+        assert x2.shape[0] == self.n_channels, (x2.shape, self.n_channels)
+        return x2, x2.shape[1], x.ndim == 1
+
+    def full_demod(self, cs16: np.ndarray, chunk_int16: int = MAXIMUM_BUF_LENGTH, return_chunks: bool = False):
+        """Host arrays in, host arrays out (``<prefix>_process``): ``rtlsdr_callback`` + ``full_demod`` once per chunk.
+        Returns the concatenated ``demod.result`` per channel, int16[n_channels][n_pcm] (int16[n_pcm] for a 1-D input
+        of one channel stream), and with return_chunks the PCM count of each chunk."""
+        x, n_int16, single = self._input(cs16)
+        cap = self._bound(n_int16, chunk_int16) + 8
+        out = np.empty((self.n_channels, cap), dtype=np.int16)
+        lens = np.zeros(max(1, -(-n_int16 // chunk_int16)), dtype=np.int32)
+        n_pcm = C.c_size_t(0)
+        _lib.check(self._fn("process")(self._h, x.ctypes.data, n_int16, chunk_int16, out.ctypes.data, cap,
+                                       C.byref(n_pcm), lens.ctypes.data_as(C.POINTER(C.c_int))))
+        res = out[:, :n_pcm.value].copy()
+        res = res[0] if single else res
+        return (res, lens) if return_chunks else res
+
+    def process_read(self, cs16: np.ndarray) -> np.ndarray:
+        """One device read: ``rtlsdr_callback`` + ``full_demod`` once on the whole of it, whatever its length
+        (``<prefix>_process_read``).  Shapes as ``full_demod``."""
+        x, n_int16, single = self._input(cs16)
+        cap = self._bound(n_int16, max(n_int16, 1)) + 8
+        out = np.empty((self.n_channels, cap), dtype=np.int16)
+        n_pcm = C.c_size_t(0)
+        _lib.check(self._fn("process_read")(self._h, x.ctypes.data, n_int16, out.ctypes.data, cap, C.byref(n_pcm)))
+        res = out[:, :n_pcm.value].copy()
+        return res[0] if single else res
+
+    def squelch_hits(self) -> np.ndarray:
+        """demod.squelch_hits of every channel after the last call, int32[n_channels]."""
+        h = np.zeros(self.n_channels, dtype=np.int32)
+        _lib.check(self._fn("squelch_hits")(self._h, h.ctypes.data_as(C.POINTER(C.c_int))))
+        return h
+
+    def levels(self) -> np.ndarray:
+        """rms() of every chunk of the last call, int32[n_channels][n_chunks] (needs report_levels; the ``sr`` of
+        src/rtl_fm.c:792-806)."""
+        fn, n = self._fn("levels"), C.c_size_t(0)
+        rc = fn(self._h, np.zeros(1, np.int32).ctypes.data_as(C.POINTER(C.c_int)), 0, C.byref(n))
+        if rc != _lib.ECAPACITY:
+            _lib.check(rc)
+        buf = np.zeros((self.n_channels, int(n.value)), dtype=np.int32)
+        _lib.check(fn(self._h, buf.ctypes.data_as(C.POINTER(C.c_int)), buf.size, C.byref(n)))
+        return buf
+
+
+class _OneGpu(_Handle):
+    """The device entry points of the single-GPU kinds (``FmDemod``, ``FmMix``)."""
+
+    def process_device(self, d_in_ptr: int, n_int16: int, chunk_int16: int, d_out_ptr: int, out_stride: int,
+                       sync: bool = False) -> int:
+        """Device pointers (e.g. torch tensors' data_ptr()): the input and [n_channels][out_stride] PCM; returns the PCM
+        count per channel."""
+        n_pcm = C.c_size_t(0)
+        _lib.check(self._fn("process_device")(self._h, d_in_ptr, n_int16, chunk_int16, d_out_ptr, out_stride,
+                                              C.byref(n_pcm), 1 if sync else 0))
+        return int(n_pcm.value)
+
+    def process_read_device(self, d_in_ptr: int, n_int16: int, d_out_ptr: int, out_stride: int,
+                            sync: bool = False) -> int:
+        """``process_read`` on device pointers (4-byte alignment is enough); returns the PCM count per channel."""
+        n_pcm = C.c_size_t(0)
+        _lib.check(self._fn("process_read_device")(self._h, d_in_ptr, n_int16, d_out_ptr, out_stride, C.byref(n_pcm),
+                                                   1 if sync else 0))
+        return int(n_pcm.value)
+
+
+def _devices(devices, n_dev):
+    """A group's member ordinals as a C array (None: range(n_dev)) and its member count."""
+    devs = None if devices is None else np.ascontiguousarray(devices, dtype=np.int32)
+    return devs, len(devs) if devs is not None else int(n_dev or 1)
+
+
+def _ptr(a):
+    return None if a is None else a.ctypes.data_as(C.POINTER(C.c_int))
+
+
+class FmDemod(_OneGpu):
     """One handle = ``n_channels`` independent demod_state streams with identical parameters."""
+
+    _prefix = "rxb200_fm"
 
     def __init__(self, params, device: int = 0, n_channels: int = 1):
         self.params = FmParams.from_any(params)
@@ -83,86 +192,13 @@ class FmDemod:
         pc = self.params.to_c()
         _lib.check(_lib.lib().rxb200_fm_create(C.byref(pc), device, n_channels, C.byref(self._h)))
 
-    def close(self) -> None:
-        if _lib is not None and getattr(self, "_h", None) is not None and self._h:
-            _lib.lib().rxb200_fm_destroy(self._h)
-            self._h = None
-
-    __del__ = close
-
-    def reset(self) -> None:
-        _lib.check(_lib.lib().rxb200_fm_reset(self._h))
-
     def tune(self, segment_len: int = 0, deemph_warmup: int = 0) -> None:
         _lib.check(_lib.lib().rxb200_fm_tune(self._h, segment_len, deemph_warmup))
 
     def max_output(self, n_int16: int, chunk_int16: int = MAXIMUM_BUF_LENGTH) -> int:
         return int(_lib.lib().rxb200_fm_max_output(self._h, n_int16, chunk_int16))
 
-    def full_demod(self, cs16: np.ndarray, chunk_int16: int = MAXIMUM_BUF_LENGTH, return_chunks: bool = False):
-        """Host arrays in, host arrays out.  cs16: int16[n_int16] (one channel) or
-        int16[n_channels][n_int16].  Returns the concatenated ``demod.result`` per channel."""
-        x = np.ascontiguousarray(cs16, dtype=np.int16)
-        single = x.ndim == 1
-        x2 = x.reshape(1, -1) if single else x
-        assert x2.shape[0] == self.n_channels, (x2.shape, self.n_channels)
-        n_int16 = x2.shape[1]
-        cap = self.max_output(n_int16, chunk_int16) + 8
-        out = np.empty((self.n_channels, cap), dtype=np.int16)
-        n_chunks = max(1, -(-n_int16 // chunk_int16))
-        lens = np.zeros(n_chunks, dtype=np.int32)
-        n_pcm = C.c_size_t(0)
-        _lib.check(_lib.lib().rxb200_fm_process(self._h, x2.ctypes.data, n_int16, chunk_int16, out.ctypes.data, cap,
-                                                C.byref(n_pcm), lens.ctypes.data_as(C.POINTER(C.c_int))))
-        res = out[:, :n_pcm.value].copy()
-        res = res[0] if single else res
-        return (res, lens) if return_chunks else res
-
-    def process_device(self, d_in_ptr: int, n_int16: int, chunk_int16: int, d_out_ptr: int, out_stride: int,
-                       sync: bool = False) -> int:
-        """Device pointers (e.g. torch tensors' data_ptr()); returns PCM count per channel."""
-        n_pcm = C.c_size_t(0)
-        _lib.check(_lib.lib().rxb200_fm_process_device(self._h, d_in_ptr, n_int16, chunk_int16, d_out_ptr, out_stride,
-                                                       C.byref(n_pcm), 1 if sync else 0))
-        return int(n_pcm.value)
-
-    def process_read(self, cs16: np.ndarray) -> np.ndarray:
-        """One device read per channel: ``rtlsdr_callback`` + ``full_demod`` once on the whole of it, whatever its
-        length (``rxb200_fm_process_read``).  cs16: int16[n_int16] or int16[n_channels][n_int16]."""
-        x = np.ascontiguousarray(cs16, dtype=np.int16)
-        single = x.ndim == 1
-        x2 = x.reshape(1, -1) if single else x
-        assert x2.shape[0] == self.n_channels, (x2.shape, self.n_channels)
-        n_int16 = x2.shape[1]
-        cap = self.max_output(n_int16, max(n_int16, 1)) + 8
-        out = np.empty((self.n_channels, cap), dtype=np.int16)
-        n_pcm = C.c_size_t(0)
-        _lib.check(_lib.lib().rxb200_fm_process_read(self._h, x2.ctypes.data, n_int16, out.ctypes.data, cap,
-                                                     C.byref(n_pcm)))
-        res = out[:, :n_pcm.value].copy()
-        return res[0] if single else res
-
-    def process_read_device(self, d_in_ptr: int, n_int16: int, d_out_ptr: int, out_stride: int,
-                            sync: bool = False) -> int:
-        """``process_read`` on device pointers (4-byte alignment is enough); returns PCM count per channel."""
-        n_pcm = C.c_size_t(0)
-        _lib.check(_lib.lib().rxb200_fm_process_read_device(self._h, d_in_ptr, n_int16, d_out_ptr, out_stride,
-                                                            C.byref(n_pcm), 1 if sync else 0))
-        return int(n_pcm.value)
-
-    def levels(self) -> np.ndarray:
-        """rms() of every chunk of the last call, int32[n_channels][n_chunks] (needs report_levels;
-        the ``sr`` of src/rtl_fm.c:792-806)."""
-        cap = 1024
-        while True:
-            buf = np.zeros(cap, dtype=np.int32)
-            n = C.c_size_t(0)
-            rc = _lib.lib().rxb200_fm_levels(self._h, buf.ctypes.data_as(C.POINTER(C.c_int)), cap, C.byref(n))
-            if rc == _lib.ECAPACITY:
-                cap = int(n.value) * self.n_channels
-                continue
-            _lib.check(rc)
-            return buf[:int(n.value) * self.n_channels].reshape(self.n_channels, int(n.value)).copy()
+    _bound = max_output
 
     @property
     def stream(self) -> int:
@@ -181,87 +217,28 @@ class FmDemod:
         return d
 
 
-class FmGroup:
+class FmGroup(_Handle):
     """``n_channels`` streams split over several GPUs (``rxb200_fm_group_*``): member i owns a contiguous block of the
     channels and its own ``rxb200_fm`` handle; the group's results are byte for byte those of one ``FmDemod`` with all
     the channels.  devices: one CUDA ordinal per member (may repeat), or None for ``range(n_dev)``."""
 
+    _prefix = "rxb200_fm_group"
+    _g = property(lambda self: self._h)     # the handle under the name callers of earlier releases read
+
     def __init__(self, params, n_channels: int, devices=None, n_dev: Optional[int] = None):
         self.params = FmParams.from_any(params)
         self.n_channels = n_channels
-        devs = None if devices is None else np.ascontiguousarray(devices, dtype=np.int32)
-        self.n_dev = len(devs) if devs is not None else int(n_dev or 1)
-        self._g = C.c_void_p()
+        devs, self.n_dev = _devices(devices, n_dev)
+        self._h = C.c_void_p()
         pc = self.params.to_c()
-        dp = None if devs is None else devs.ctypes.data_as(C.POINTER(C.c_int))
-        _lib.check(_lib.lib().rxb200_fm_group_create(C.byref(pc), n_channels, self.n_dev, dp, C.byref(self._g)))
-
-    def close(self) -> None:
-        if _lib is not None and getattr(self, "_g", None) is not None and self._g:
-            _lib.lib().rxb200_fm_group_destroy(self._g)
-            self._g = None
-
-    __del__ = close
+        _lib.check(_lib.lib().rxb200_fm_group_create(C.byref(pc), n_channels, self.n_dev, _ptr(devs), C.byref(self._h)))
 
     def member(self, i: int) -> int:
         """Member i's rxb200_fm handle as an integer, 0 for a member that owns no channel."""
-        return int(_lib.lib().rxb200_fm_group_member(self._g, i) or 0)
+        return int(_lib.lib().rxb200_fm_group_member(self._h, i) or 0)
 
-    def reset(self) -> None:
-        _lib.check(_lib.lib().rxb200_fm_group_reset(self._g))
-
-    def _cap(self, n_int16: int, chunk_int16: int) -> int:
-        return int(_lib.lib().rxb200_fm_max_output(C.c_void_p(self.member(0)), n_int16, chunk_int16)) + 8
-
-    def _input(self, cs16):
-        x = np.ascontiguousarray(cs16, dtype=np.int16)
-        x2 = x.reshape(1, -1) if x.ndim == 1 else x
-        assert x2.shape[0] == self.n_channels, (x2.shape, self.n_channels)
-        return x2, x.ndim == 1
-
-    def full_demod(self, cs16: np.ndarray, chunk_int16: int = MAXIMUM_BUF_LENGTH, return_chunks: bool = False):
-        """As ``FmDemod.full_demod`` (``rxb200_fm_group_process``)."""
-        x2, single = self._input(cs16)
-        n_int16 = x2.shape[1]
-        cap = self._cap(n_int16, chunk_int16)
-        out = np.empty((self.n_channels, cap), dtype=np.int16)
-        lens = np.zeros(max(1, -(-n_int16 // chunk_int16)), dtype=np.int32)
-        n_pcm = C.c_size_t(0)
-        _lib.check(_lib.lib().rxb200_fm_group_process(self._g, x2.ctypes.data, n_int16, chunk_int16, out.ctypes.data, cap,
-                                                      C.byref(n_pcm), lens.ctypes.data_as(C.POINTER(C.c_int))))
-        res = out[:, :n_pcm.value].copy()
-        res = res[0] if single else res
-        return (res, lens) if return_chunks else res
-
-    def process_read(self, cs16: np.ndarray) -> np.ndarray:
-        """As ``FmDemod.process_read`` (``rxb200_fm_group_process_read``)."""
-        x2, single = self._input(cs16)
-        n_int16 = x2.shape[1]
-        cap = self._cap(n_int16, max(n_int16, 1))
-        out = np.empty((self.n_channels, cap), dtype=np.int16)
-        n_pcm = C.c_size_t(0)
-        _lib.check(_lib.lib().rxb200_fm_group_process_read(self._g, x2.ctypes.data, n_int16, out.ctypes.data, cap,
-                                                           C.byref(n_pcm)))
-        res = out[:, :n_pcm.value].copy()
-        return res[0] if single else res
-
-    def squelch_hits(self) -> np.ndarray:
-        """demod.squelch_hits of every channel after the last call, int32[n_channels]."""
-        h = np.zeros(self.n_channels, dtype=np.int32)
-        _lib.check(_lib.lib().rxb200_fm_group_squelch_hits(self._g, h.ctypes.data_as(C.POINTER(C.c_int))))
-        return h
-
-    def levels(self) -> np.ndarray:
-        """As ``FmDemod.levels``: int32[n_channels][n_chunks] of the last call (needs report_levels)."""
-        n = C.c_size_t(0)
-        rc = _lib.lib().rxb200_fm_group_levels(self._g, np.zeros(1, np.int32).ctypes.data_as(C.POINTER(C.c_int)), 0,
-                                               C.byref(n))
-        if rc != _lib.ECAPACITY:
-            _lib.check(rc)
-        buf = np.zeros((self.n_channels, int(n.value)), dtype=np.int32)
-        _lib.check(_lib.lib().rxb200_fm_group_levels(self._g, buf.ctypes.data_as(C.POINTER(C.c_int)), buf.size,
-                                                     C.byref(n)))
-        return buf
+    def _bound(self, n_int16: int, chunk_int16: int) -> int:
+        return int(_lib.lib().rxb200_fm_max_output(C.c_void_p(self.member(0)), n_int16, chunk_int16))
 
 
 # ---- several channels of one capture (rxb200_fm_mix_*) ------------------------------------------------------
@@ -301,12 +278,16 @@ def ddc_device(capture_rate: int, offset_hz: int, phase: int, ddc, d_src_ptr: in
                                             stream or None))
 
 
-class FmMix:
+class FmMix(_OneGpu):
     """``len(offsets_hz)`` channels of ONE CS16 capture at ``capture_rate`` (``rxb200_fm_mix_*``): channel k is
     ``FmDemod`` run on the capture mixed down by ``offsets_hz[k]`` with ``mix_table``; the mixers' phases carry across
     calls.  Every call takes the one capture, int16[n_int16], and returns int16[n_channels][n_pcm].
     ddc = (decim, taps, shift): a decimating handle (``rxb200_fm_mix_create_ddc``), each channel filtered by the int32
     taps, rounded by the shift and decimated by decim before the chain."""
+
+    _prefix = "rxb200_fm_mix"
+    _streams = False
+    _m = property(lambda self: self._h)     # the handle under the name callers of earlier releases read
 
     def __init__(self, params, capture_rate: int, offsets_hz, device: int = 0, ddc=None):
         self.params = FmParams.from_any(params)
@@ -315,103 +296,32 @@ class FmMix:
         self.offsets_hz = offs.tolist()
         self.n_channels = len(offs)
         self.ddc = ddc
-        self._m = C.c_void_p()
+        self._h = C.c_void_p()
         pc = self.params.to_c()
-        po = offs.ctypes.data_as(C.POINTER(C.c_int))
         if ddc is None:
-            _lib.check(_lib.lib().rxb200_fm_mix_create(C.byref(pc), capture_rate, po, self.n_channels, device,
-                                                       C.byref(self._m)))
+            _lib.check(_lib.lib().rxb200_fm_mix_create(C.byref(pc), capture_rate, _ptr(offs), self.n_channels, device,
+                                                       C.byref(self._h)))
         else:
             d, _t = _ddc_c(ddc)
-            _lib.check(_lib.lib().rxb200_fm_mix_create_ddc(C.byref(pc), capture_rate, po, self.n_channels, C.byref(d),
-                                                           device, C.byref(self._m)))
-
-    def close(self) -> None:
-        if _lib is not None and getattr(self, "_m", None) is not None and self._m:
-            _lib.lib().rxb200_fm_mix_destroy(self._m)
-            self._m = None
-
-    __del__ = close
+            _lib.check(_lib.lib().rxb200_fm_mix_create_ddc(C.byref(pc), capture_rate, _ptr(offs), self.n_channels,
+                                                           C.byref(d), device, C.byref(self._h)))
 
     def member(self) -> int:
         """The inner rxb200_fm handle (one channel per mixed stream) as an integer."""
-        return int(_lib.lib().rxb200_fm_mix_member(self._m) or 0)
-
-    def reset(self) -> None:
-        _lib.check(_lib.lib().rxb200_fm_mix_reset(self._m))
+        return int(_lib.lib().rxb200_fm_mix_member(self._h) or 0)
 
     def max_output(self, n_int16: int, chunk_int16: int = MAXIMUM_BUF_LENGTH) -> int:
         """A bound on the PCM per channel of a call of n_int16 capture int16, at any phase
         (``rxb200_fm_mix_max_output``)."""
-        return int(_lib.lib().rxb200_fm_mix_max_output(self._m, n_int16, chunk_int16))
+        return int(_lib.lib().rxb200_fm_mix_max_output(self._h, n_int16, chunk_int16))
+
+    _bound = max_output
 
     def decimated_len(self, n_int16: int) -> int:
         """int16 per channel the next call of n_int16 capture int16 hands the chain (``rxb200_fm_mix_decimated_len``)."""
         n = C.c_size_t(0)
-        _lib.check(_lib.lib().rxb200_fm_mix_decimated_len(self._m, n_int16, C.byref(n)))
+        _lib.check(_lib.lib().rxb200_fm_mix_decimated_len(self._h, n_int16, C.byref(n)))
         return int(n.value)
-
-    def _cap(self, n_int16: int, chunk_int16: int) -> int:
-        return self.max_output(n_int16, chunk_int16) + 8
-
-    def full_demod(self, cs16: np.ndarray, chunk_int16: int = MAXIMUM_BUF_LENGTH, return_chunks: bool = False):
-        """As ``FmDemod.full_demod`` on every channel (``rxb200_fm_mix_process``); cs16: the capture, int16[n_int16]."""
-        x = np.ascontiguousarray(cs16, dtype=np.int16).reshape(-1)
-        n_int16 = x.size
-        cap = self._cap(n_int16, chunk_int16)
-        out = np.empty((self.n_channels, cap), dtype=np.int16)
-        lens = np.zeros(max(1, -(-n_int16 // chunk_int16)), dtype=np.int32)
-        n_pcm = C.c_size_t(0)
-        _lib.check(_lib.lib().rxb200_fm_mix_process(self._m, x.ctypes.data, n_int16, chunk_int16, out.ctypes.data, cap,
-                                                    C.byref(n_pcm), lens.ctypes.data_as(C.POINTER(C.c_int))))
-        res = out[:, :n_pcm.value].copy()
-        return (res, lens) if return_chunks else res
-
-    def process_read(self, cs16: np.ndarray) -> np.ndarray:
-        """As ``FmDemod.process_read`` on every channel (``rxb200_fm_mix_process_read``)."""
-        x = np.ascontiguousarray(cs16, dtype=np.int16).reshape(-1)
-        n_int16 = x.size
-        cap = self._cap(n_int16, max(n_int16, 1))
-        out = np.empty((self.n_channels, cap), dtype=np.int16)
-        n_pcm = C.c_size_t(0)
-        _lib.check(_lib.lib().rxb200_fm_mix_process_read(self._m, x.ctypes.data, n_int16, out.ctypes.data, cap,
-                                                         C.byref(n_pcm)))
-        return out[:, :n_pcm.value].copy()
-
-    def process_device(self, d_in_ptr: int, n_int16: int, chunk_int16: int, d_out_ptr: int, out_stride: int,
-                       sync: bool = False) -> int:
-        """Device pointers: the capture (4-byte alignment is enough) and [n_channels][out_stride] PCM; returns the PCM
-        count per channel."""
-        n_pcm = C.c_size_t(0)
-        _lib.check(_lib.lib().rxb200_fm_mix_process_device(self._m, d_in_ptr, n_int16, chunk_int16, d_out_ptr,
-                                                           out_stride, C.byref(n_pcm), 1 if sync else 0))
-        return int(n_pcm.value)
-
-    def process_read_device(self, d_in_ptr: int, n_int16: int, d_out_ptr: int, out_stride: int,
-                            sync: bool = False) -> int:
-        """``process_read`` on device pointers; returns the PCM count per channel."""
-        n_pcm = C.c_size_t(0)
-        _lib.check(_lib.lib().rxb200_fm_mix_process_read_device(self._m, d_in_ptr, n_int16, d_out_ptr, out_stride,
-                                                                C.byref(n_pcm), 1 if sync else 0))
-        return int(n_pcm.value)
-
-    def squelch_hits(self) -> np.ndarray:
-        """demod.squelch_hits of every channel after the last call, int32[n_channels]."""
-        h = np.zeros(self.n_channels, dtype=np.int32)
-        _lib.check(_lib.lib().rxb200_fm_mix_squelch_hits(self._m, h.ctypes.data_as(C.POINTER(C.c_int))))
-        return h
-
-    def levels(self) -> np.ndarray:
-        """As ``FmDemod.levels``: int32[n_channels][n_chunks] of the last call (needs report_levels)."""
-        n = C.c_size_t(0)
-        rc = _lib.lib().rxb200_fm_mix_levels(self._m, np.zeros(1, np.int32).ctypes.data_as(C.POINTER(C.c_int)), 0,
-                                             C.byref(n))
-        if rc != _lib.ECAPACITY:
-            _lib.check(rc)
-        buf = np.zeros((self.n_channels, int(n.value)), dtype=np.int32)
-        _lib.check(_lib.lib().rxb200_fm_mix_levels(self._m, buf.ctypes.data_as(C.POINTER(C.c_int)), buf.size,
-                                                   C.byref(n)))
-        return buf
 
     def stats(self) -> dict:
         s = _lib.FmStatsC()
@@ -425,7 +335,7 @@ class FmMix:
     def mix_ms(self) -> float:
         """Device time of the last call's fm_mix_kernel (fm_ddc_kernel for a decimating handle)."""
         ms = C.c_float(0)
-        _lib.check(_lib.lib().rxb200_fm_mix_kernel_ms(self._m, C.byref(ms)))
+        _lib.check(_lib.lib().rxb200_fm_mix_kernel_ms(self._h, C.byref(ms)))
         return float(ms.value)
 
     def kernel_ms(self) -> float:
@@ -435,12 +345,16 @@ class FmMix:
         return float(ms.value)
 
 
-class FmMixGroup:
+class FmMixGroup(_Handle):
     """The channels of ONE capture split over several GPUs (``rxb200_fm_mix_group_*``): member i is a ``FmMix`` on its
     own GPU with a contiguous block of the offsets, and every member gets a copy of the capture; the group's results
     are byte for byte those of one ``FmMix`` with all the offsets.  devices: one CUDA ordinal per member (may repeat),
     or None for ``range(n_dev)``.  ddc = (decim, taps, shift): decimating members (``rxb200_fm_mix_group_create_ddc``),
     byte for byte one ``FmMix`` with that ddc."""
+
+    _prefix = "rxb200_fm_mix_group"
+    _streams = False
+    _g = property(lambda self: self._h)     # the handle under the name callers of earlier releases read
 
     def __init__(self, params, capture_rate: int, offsets_hz, devices=None, n_dev: Optional[int] = None, ddc=None):
         self.params = FmParams.from_any(params)
@@ -449,83 +363,28 @@ class FmMixGroup:
         self.offsets_hz = offs.tolist()
         self.n_channels = len(offs)
         self.ddc = ddc
-        devs = None if devices is None else np.ascontiguousarray(devices, dtype=np.int32)
-        self.n_dev = len(devs) if devs is not None else int(n_dev or 1)
-        self._g = C.c_void_p()
+        devs, self.n_dev = _devices(devices, n_dev)
+        self._h = C.c_void_p()
         pc = self.params.to_c()
-        dp = None if devs is None else devs.ctypes.data_as(C.POINTER(C.c_int))
-        po = offs.ctypes.data_as(C.POINTER(C.c_int))
         if ddc is None:
-            _lib.check(_lib.lib().rxb200_fm_mix_group_create(C.byref(pc), capture_rate, po, self.n_channels, self.n_dev,
-                                                             dp, C.byref(self._g)))
+            _lib.check(_lib.lib().rxb200_fm_mix_group_create(C.byref(pc), capture_rate, _ptr(offs), self.n_channels,
+                                                             self.n_dev, _ptr(devs), C.byref(self._h)))
         else:
             d, _t = _ddc_c(ddc)
-            _lib.check(_lib.lib().rxb200_fm_mix_group_create_ddc(C.byref(pc), capture_rate, po, self.n_channels,
-                                                                 C.byref(d), self.n_dev, dp, C.byref(self._g)))
-
-    def close(self) -> None:
-        if _lib is not None and getattr(self, "_g", None) is not None and self._g:
-            _lib.lib().rxb200_fm_mix_group_destroy(self._g)
-            self._g = None
-
-    __del__ = close
+            _lib.check(_lib.lib().rxb200_fm_mix_group_create_ddc(C.byref(pc), capture_rate, _ptr(offs), self.n_channels,
+                                                                 C.byref(d), self.n_dev, _ptr(devs), C.byref(self._h)))
 
     def member(self, i: int) -> int:
         """Member i's rxb200_fm_mix handle as an integer, 0 for a member that owns no channel."""
-        return int(_lib.lib().rxb200_fm_mix_group_member(self._g, i) or 0)
+        return int(_lib.lib().rxb200_fm_mix_group_member(self._h, i) or 0)
 
     def inner(self, i: int) -> int:
         """The inner rxb200_fm handle of member i (``rxb200_fm_mix_member``), 0 for a member that owns no channel."""
         m = self.member(i)
         return int(_lib.lib().rxb200_fm_mix_member(C.c_void_p(m)) or 0) if m else 0
 
-    def reset(self) -> None:
-        _lib.check(_lib.lib().rxb200_fm_mix_group_reset(self._g))
-
-    def _cap(self, n_int16: int, chunk_int16: int) -> int:
-        return int(_lib.lib().rxb200_fm_mix_max_output(C.c_void_p(self.member(0)), n_int16, chunk_int16)) + 8
-
-    def full_demod(self, cs16: np.ndarray, chunk_int16: int = MAXIMUM_BUF_LENGTH, return_chunks: bool = False):
-        """As ``FmMix.full_demod`` (``rxb200_fm_mix_group_process``); cs16: the capture, int16[n_int16]."""
-        x = np.ascontiguousarray(cs16, dtype=np.int16).reshape(-1)
-        n_int16 = x.size
-        cap = self._cap(n_int16, chunk_int16)
-        out = np.empty((self.n_channels, cap), dtype=np.int16)
-        lens = np.zeros(max(1, -(-n_int16 // chunk_int16)), dtype=np.int32)
-        n_pcm = C.c_size_t(0)
-        _lib.check(_lib.lib().rxb200_fm_mix_group_process(self._g, x.ctypes.data, n_int16, chunk_int16, out.ctypes.data,
-                                                          cap, C.byref(n_pcm), lens.ctypes.data_as(C.POINTER(C.c_int))))
-        res = out[:, :n_pcm.value].copy()
-        return (res, lens) if return_chunks else res
-
-    def process_read(self, cs16: np.ndarray) -> np.ndarray:
-        """As ``FmMix.process_read`` (``rxb200_fm_mix_group_process_read``)."""
-        x = np.ascontiguousarray(cs16, dtype=np.int16).reshape(-1)
-        n_int16 = x.size
-        cap = self._cap(n_int16, max(n_int16, 1))
-        out = np.empty((self.n_channels, cap), dtype=np.int16)
-        n_pcm = C.c_size_t(0)
-        _lib.check(_lib.lib().rxb200_fm_mix_group_process_read(self._g, x.ctypes.data, n_int16, out.ctypes.data, cap,
-                                                               C.byref(n_pcm)))
-        return out[:, :n_pcm.value].copy()
-
-    def squelch_hits(self) -> np.ndarray:
-        """demod.squelch_hits of every channel after the last call, int32[n_channels]."""
-        h = np.zeros(self.n_channels, dtype=np.int32)
-        _lib.check(_lib.lib().rxb200_fm_mix_group_squelch_hits(self._g, h.ctypes.data_as(C.POINTER(C.c_int))))
-        return h
-
-    def levels(self) -> np.ndarray:
-        """As ``FmDemod.levels``: int32[n_channels][n_chunks] of the last call (needs report_levels)."""
-        n = C.c_size_t(0)
-        rc = _lib.lib().rxb200_fm_mix_group_levels(self._g, np.zeros(1, np.int32).ctypes.data_as(C.POINTER(C.c_int)), 0,
-                                                   C.byref(n))
-        if rc != _lib.ECAPACITY:
-            _lib.check(rc)
-        buf = np.zeros((self.n_channels, int(n.value)), dtype=np.int32)
-        _lib.check(_lib.lib().rxb200_fm_mix_group_levels(self._g, buf.ctypes.data_as(C.POINTER(C.c_int)), buf.size,
-                                                         C.byref(n)))
-        return buf
+    def _bound(self, n_int16: int, chunk_int16: int) -> int:
+        return int(_lib.lib().rxb200_fm_mix_max_output(C.c_void_p(self.member(0)), n_int16, chunk_int16))
 
 
 # ---- rx_sdr sample-format conversions (src/rtl_sdr.c:348-391) -------------------------------------------

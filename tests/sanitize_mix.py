@@ -1,6 +1,8 @@
 """Small run of several rx_fm channels of one capture for compute-sanitizer (memcheck): an odd-length capture from a
 tensor of exactly its size at a 4-byte offset, through the host and the device entry points of a mixing handle, and the
-mixer alone -- the partial last unit of the capture is where a read past it would show.
+mixer alone -- the partial last unit of the capture is where a read past it would show.  Then a decimating handle on
+the same kind of capture: fm_ddc_kernel's staged windows and its reads of the history, and the history carry, with a
+read shorter than M (no output) and one shorter than T - 1 (the carry keeps part of the old history).
 
     compute-sanitizer --tool memcheck python tests/sanitize_mix.py
 """
@@ -14,6 +16,7 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 import torch  # noqa: E402
 
+import fm_ddc as fdd  # noqa: E402
 import fm_mix as fmx  # noqa: E402
 from rx_tools_b200 import fm  # noqa: E402
 
@@ -35,3 +38,28 @@ for name in ("fm5a_lut_d100", "fm2b_f9", "fm_lut_d42_squelch"):
     ok = ok and np.array_equal(dst.cpu().numpy(), fmx.mix_model(x, fm.mix_table(rate, offs[-1]), 5))
     print(name, "exact" if ok else "DIFFERS")
     mx.close()
+
+p, rate, offs, ddc, cap, _ = fdd.case_input("am_m100")
+M, T = ddc[0], ddc[1].size
+lens = [2 * 2003, 2 * 37, 2 * 251]                    # odd complex counts; 37 < M, and 37, 251 < T - 1
+assert 37 < M and 251 < T - 1
+x = cap[:sum(lens)]
+host, dev = fm.FmMix(p, rate, offs, ddc=ddc), fm.FmMix(p, rate, offs, ddc=ddc)
+buf = torch.from_numpy(np.concatenate([np.zeros(2, np.int16), x])).cuda()   # exactly the capture after 4 bytes
+stride = 2 * sum(lens) // (2 * M) + 8
+out = torch.zeros(len(offs) * stride, dtype=torch.int16, device="cuda")
+ok, pos = True, 0
+for n16 in lens:
+    want = host.process_read(x[pos:pos + n16])
+    k = dev.process_read_device(buf.data_ptr() + 4 + 2 * pos, n16, out.data_ptr(), stride, sync=True)
+    ok = ok and np.array_equal(out.view(len(offs), stride)[:, :k].cpu().numpy(), want)
+    pos += n16
+host.reset()
+dev.reset()
+chunk = 2 * M * 4                                     # the last chunk of the first read is 3 samples
+want = host.full_demod(x[:lens[0]], chunk)
+k = dev.process_device(buf.data_ptr() + 4, lens[0], chunk, out.data_ptr(), stride, sync=True)
+ok = ok and np.array_equal(out.view(len(offs), stride)[:, :k].cpu().numpy(), want)
+print("am_m100 ddc", "exact" if ok else "DIFFERS")
+host.close()
+dev.close()

@@ -43,13 +43,6 @@ def _compare(p, got, want, what):
             assert diff.max(initial=0) <= 1, what
 
 
-def _hits(d):
-    import ctypes as C
-    h = np.zeros(d.n_channels, dtype=np.int32)
-    _lib.check(_lib.lib().rxb200_fm_squelch_hits(d._h, h.ctypes.data_as(C.POINTER(C.c_int))))
-    return h
-
-
 def _levels_handle(p):
     q = fm.FmParams.from_any(p)
     q.report_levels = 1
@@ -70,7 +63,7 @@ def test_uniform_odd_chunks(name, port):
         assert np.array_equal(gl, wl), (name, c)
         _compare(p, got, want, (name, c))
         if p.squelch_level:
-            assert _hits(d)[0] == wh[-1]
+            assert d.squelch_hits()[0] == wh[-1]
     d.close()
 
 
@@ -106,7 +99,7 @@ def test_ragged_call_sequences(name, port):
         assert parts[-1].size == wl[c] and parts_l[-1].size == wl[c], (name, c)
         assert dl.levels()[0].tolist() == [want_lv[c]], (name, c)
         if p.squelch_level:
-            assert _hits(d)[0] == wh[c] and _hits(dl)[0] == wh[c], (name, c)
+            assert d.squelch_hits()[0] == wh[c] and dl.squelch_hits()[0] == wh[c], (name, c)
     _compare(p, np.concatenate(parts), want, name)
     _compare(p, np.concatenate(parts_l), want, (name, "levels"))
     d.close()
@@ -216,7 +209,7 @@ def test_random_configuration_any_chunk(seed, port):
         raise
     _compare(p, got, want, (vars(p), chunk_c, n_c))
     if p.squelch_level:
-        assert _hits(d)[0] == wh[-1]
+        assert d.squelch_hits()[0] == wh[-1]
     d.close()
 
 

@@ -12,8 +12,8 @@ import pytest
 
 import fm_any_chunk as fac
 import fm_ddc as fdd
+import fm_handles as fh
 import fm_mix as fmx
-import fm_read as frd
 from rx_tools_b200 import _lib, fm
 
 pytestmark = pytest.mark.gpu
@@ -21,19 +21,6 @@ pytestmark = pytest.mark.gpu
 HERE = os.path.dirname(os.path.abspath(__file__))
 GOLDEN = os.path.join(HERE, "golden", "fm_ddc_golden.json")
 IDENTITY = (1, np.ones(1, np.int32), 0)
-
-
-def _torch():
-    import torch
-    return torch
-
-
-def _every_int16(seed):
-    rng = np.random.default_rng(seed)
-    x = np.empty(2 * 65536, dtype=np.int16)
-    x[0::2] = rng.permutation(np.arange(-32768, 32768)).astype(np.int16)
-    x[1::2] = rng.permutation(np.arange(-32768, 32768)).astype(np.int16)
-    return x
 
 
 def _tap_sets(decim, n_taps, seed):
@@ -52,11 +39,11 @@ CASES = sorted({(m, t) for m in (1, 2, 7, 64, 4096) for t in (1, m, 4 * m + 1, 8
 
 @pytest.mark.parametrize("decim,n_taps", CASES)
 def test_ddc_device_equals_model(decim, n_taps):
-    torch = _torch()
+    torch = fh.torch()
     rate, f = 2_400_000, 37500
     t = fm.mix_table(rate, f)
     L = t.shape[0]
-    x = _every_int16(decim * 7 + n_taps)
+    x = fh.every_int16(decim * 7 + n_taps)
     n_max = min(65536, max(decim + 3, (1 << 22) * decim // n_taps))     # keeps the model's work bounded
     # the capture 0, 4 and 16 bytes past a 256-byte aligned allocation
     srcs = {off16: torch.from_numpy(np.concatenate([np.zeros(off16, np.int16), x])).cuda() for off16 in (0, 2, 8)}
@@ -81,10 +68,10 @@ def test_ddc_device_equals_model(decim, n_taps):
 
 def test_ddc_device_source_offsets():
     """The source at 4- and 16-byte offsets into a buffer reads the right samples."""
-    torch = _torch()
+    torch = fh.torch()
     rate, f, ddc = 1_008_000, 24000, (3, fdd.lowpass(17, 0.1), 15)
     t = fm.mix_table(rate, f)
-    x = _every_int16(3)[:2 * 10001]
+    x = fh.every_int16(3)[:2 * 10001]
     for pad in (2, 8):                                    # int16 of padding: 4 and 16 bytes
         buf = torch.from_numpy(np.concatenate([np.full(pad, 77, np.int16), x])).cuda()
         dst = torch.zeros(2 * (10001 // 3) + 8, dtype=torch.int16, device="cuda")
@@ -96,7 +83,7 @@ def test_ddc_device_source_offsets():
 
 
 def test_ddc_device_refusals():
-    torch = _torch()
+    torch = fh.torch()
     buf = torch.zeros(64, dtype=torch.int16, device="cuda")
     p = buf.data_ptr()
     good = (2, [1, 1], 1)
@@ -113,29 +100,10 @@ def test_ddc_device_refusals():
         assert e.value.code == code, args
 
 
-def _reads(obj, x, lens16):
-    parts, counts = [], []
-    for pos, n in fac.seq_bounds(x.size, lens16):
-        r = obj.process_read(x[pos:pos + n])
-        parts.append(r)
-        counts.append(r.shape[-1])
-    return np.concatenate(parts, axis=-1), counts
-
-
-# the routes of a plain handle (tests/test_fm_mix_gpu.py): parameters, process or read, chunk, call lengths, kernel_kind
-ROUTES = {
-    "rows": (frd.FM2B, "process", 8 * 2048, [2 * 32768, 2 * 32768], 1),
-    "stream": (fac.FM2A, "process", 32768, [2 * 98304, 2 * 98304], 3),
-    "spec3": (fac.FM5A, "process", 2 * 25000, [2 * 50000, 2 * 25000], 0),
-    "any": (fac.FM5A, "process", 2 * 2003, [2 * 3 * 2003, 2 * (2 * 2003 + 457)], 0),
-    "read_passes": (frd.FM2B, "read", 0, [2 * 1021, 2 * 333, 2 * 4093], 0),
-}
-
-
-@pytest.mark.parametrize("name", sorted(ROUTES))
+@pytest.mark.parametrize("name", sorted(fh.KERNEL_ROUTES))
 def test_identity_is_a_plain_mixing_handle(name):
     """M = 1, h = {1}, S = 0 gives the bytes of a plain mixing handle, on the route the plain handle takes."""
-    p, mode, chunk, lens, kind = ROUTES[name]
+    p, mode, chunk, lens, kind = fh.KERNEL_ROUTES[name]
     x = fac.signal(sum(lens) // 2, 41)
     offs = [0, 300_000]
     dd = fm.FmMix(p, 2_400_000, offs, ddc=IDENTITY)
@@ -156,25 +124,6 @@ def test_identity_is_a_plain_mixing_handle(name):
     mx.close()
 
 
-def _port_channels(port, p, rate, offs, ddc, x, lens16):
-    """The port on each channel's decimated stream, one chain read per capture read with output."""
-    out = []
-    for f in offs:
-        y, lens = fdd.nonempty(fdd.decimated_reads(x, fm.mix_table(rate, f), ddc, lens16))
-        out.append(fac.port_run_seq(port, p, y, lens, return_chunks=True))
-    return out
-
-
-def _compare(p, got, want, what):
-    assert got.size == want.size, (what, got.size, want.size)
-    if fac.INTEGER(p):
-        bad = np.flatnonzero(got != want)
-        assert bad.size == 0, (what, bad[:5])
-    else:
-        diff = np.abs(got.astype(np.int32) - want.astype(np.int32))
-        assert np.count_nonzero(diff) <= max(2, int(1e-4 * diff.size)) and diff.max(initial=0) <= 1, what
-
-
 @pytest.mark.parametrize("k", [1, 3, 8, 33, 257])
 def test_k_channels_equal_the_port(k, port):
     p, rate, _, ddc, _, reads = fdd.SHAPES["nbfm_m64_t257"]
@@ -182,9 +131,9 @@ def test_k_channels_equal_the_port(k, port):
     lens = [2 * 9001, 2 * 5003, 2 * 7919]
     x = fmx.capture(fdd.n_complex_for(lens), rate, offs[::7], 810 + k)
     mx = fm.FmMix(p, rate, offs, ddc=ddc)
-    got, _ = _reads(mx, x, lens)
-    for j, (want, _, wh) in enumerate(_port_channels(port, p, rate, offs, ddc, x, lens)):
-        _compare(p, got[j], want, (k, offs[j]))
+    got, _ = fh.reads(mx, x, lens)
+    for j, (want, _, wh) in enumerate(fh.port_channels(port, p, rate, offs, x, lens, ddc)):
+        fh.compare(p, got[j], want, (k, offs[j]))
         assert mx.squelch_hits()[j] == wh[-1]
     mx.close()
 
@@ -195,10 +144,10 @@ def test_shapes_equal_the_port(name, port):
     p = fm.FmParams.from_any(p)
     p.report_levels = 1 if p.squelch_level else 0
     mx = fm.FmMix(p, rate, offs, ddc=ddc)
-    got, counts = _reads(mx, x, reads)
+    got, counts = fh.reads(mx, x, reads)
     q = fac.P(**p.reference_fields())
-    for j, (want, rl, wh) in enumerate(_port_channels(port, q, rate, offs, ddc, x, reads)):
-        _compare(p, got[j], want, (name, offs[j]))
+    for j, (want, rl, wh) in enumerate(fh.port_channels(port, q, rate, offs, x, reads, ddc)):
+        fh.compare(p, got[j], want, (name, offs[j]))
         dec = fdd.decimated_reads(x, fm.mix_table(rate, offs[j]), ddc, reads)
         assert [c for c, d in zip(counts, dec) if d.size] == rl.tolist(), (name, j)
         assert all(c == 0 for c, d in zip(counts, dec) if not d.size), (name, j)
@@ -270,7 +219,7 @@ def test_carries_across_reads_chunks_mixed_and_reset(name, port):
         y, _ = fdd.ddc_model(x, fm.mix_table(rate, f), ddc[1], M, ddc[2])
         assert y.size == sum(lens)
         want = fac.port_run_seq(port, p, y, lens)
-        _compare(p, first[j], want, (name, j))
+        fh.compare(p, first[j], want, (name, j))
     mx.reset()
     again = _run_ops(mx, x, ops)
     assert again.tobytes() == first.tobytes()
@@ -290,10 +239,10 @@ def test_chunk_result_len_of_chunks_without_output():
 
 @pytest.mark.parametrize("name", ["nbfm_m64_t257", "fm2b_f9_m8"])
 def test_device_entries_with_an_unaligned_capture(name):
-    torch = _torch()
+    torch = fh.torch()
     p, rate, offs, ddc, x, reads = fdd.case_input(name, seed=8)
     host = fm.FmMix(p, rate, offs, ddc=ddc)
-    want_reads, _ = _reads(host, x, reads)
+    want_reads, _ = fh.reads(host, x, reads)
     host.reset()
     M = ddc[0]
     chunk = 2 * M * (4096 if p.downsample_passes else 1021)
@@ -375,7 +324,7 @@ def test_golden():
         g = gold[name]
         assert g["capture_sha256"] == hashlib.sha256(x.tobytes()).hexdigest(), name
         mx = fm.FmMix(p, rate, offs, ddc=ddc)
-        got, counts = _reads(mx, x, g["lens_int16"])
+        got, counts = fh.reads(mx, x, g["lens_int16"])
         for j, c in enumerate(g["channels"]):
             assert c["offset_hz"] == offs[j]
             assert [n for n, d in zip(counts, c["dec_len"]) if d] == c["result_len"], (name, j)

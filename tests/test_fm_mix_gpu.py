@@ -2,7 +2,6 @@
 every int16 value, a zero offset against a plain handle on every kernel route, K channels against the port on the
 model's mixed streams, the phase across calls, reads and reset, the device entry points with an unaligned capture,
 refusals that leave the phases and the member alone, and the golden hashes of the reference."""
-import ctypes as C
 import hashlib
 import json
 import os
@@ -11,8 +10,8 @@ import numpy as np
 import pytest
 
 import fm_any_chunk as fac
+import fm_handles as fh
 import fm_mix as fmx
-import fm_read as frd
 from rx_tools_b200 import _lib, fm
 
 pytestmark = pytest.mark.gpu
@@ -21,25 +20,11 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 GOLDEN = os.path.join(HERE, "golden", "fm_mix_golden.json")
 
 
-def _torch():
-    import torch
-    return torch
-
-
-def _every_int16(seed):
-    """65 536 complex samples whose I and Q each take every int16 value once."""
-    rng = np.random.default_rng(seed)
-    x = np.empty(2 * 65536, dtype=np.int16)
-    x[0::2] = rng.permutation(np.arange(-32768, 32768)).astype(np.int16)
-    x[1::2] = rng.permutation(np.arange(-32768, 32768)).astype(np.int16)
-    return x
-
-
 @pytest.mark.parametrize("rate,f", [(2_400_000, 12500), (2_400_000, -37500), (1_008_000, 24000), (48_000, 7),
                                     (2_400_000, 600_000), (2_400_000, 0), (1 << 20, 1)])
 def test_mix_device_equals_model(rate, f):
-    torch = _torch()
-    x = _every_int16(rate % 1000 + f % 1000)
+    torch = fh.torch()
+    x = fh.every_int16(rate % 1000 + f % 1000)
     t = fm.mix_table(rate, f)
     L = t.shape[0]
     src = torch.from_numpy(np.concatenate([np.zeros(8, np.int16), x])).cuda()
@@ -61,7 +46,7 @@ def test_mix_device_equals_model(rate, f):
 
 
 def test_mix_device_refusals():
-    torch = _torch()
+    torch = fh.torch()
     buf = torch.zeros(64, dtype=torch.int16, device="cuda")
     p = buf.data_ptr()
     for args, code in (((2_400_000, 1_200_000, 0, p, 8, p), _lib.EINVAL), ((2_400_001, 1, 0, p, 8, p), _lib.EUNSUPPORTED),
@@ -72,53 +57,11 @@ def test_mix_device_refusals():
         assert e.value.code == code, args
 
 
-def _port_channels(port, p, rate, offs, x, lens16, chans=None):
-    """The port on the model's mixed stream of each channel, read by read over lens16: [(pcm, result_len, hits)]."""
-    out = []
-    for k in (range(len(offs)) if chans is None else chans):
-        y = fmx.mix_model(x, fm.mix_table(rate, offs[k]))
-        out.append(fac.port_run_seq(port, p, y, lens16, return_chunks=True))
-    return out
-
-
-def _compare(p, got, want, what):
-    assert got.size == want.size, (what, got.size, want.size)
-    diff = np.abs(got.astype(np.int32) - want.astype(np.int32))
-    if fac.INTEGER(p):
-        bad = np.flatnonzero(diff)
-        assert bad.size == 0, (what, bad[:5], got[bad[:5]], want[bad[:5]])
-    else:
-        # fp64 atan2 on every sample (CUDA libm against glibc): a last-ulp difference may move a sample by 1 LSB
-        assert np.count_nonzero(diff) <= max(2, int(1e-4 * diff.size)), (what, np.flatnonzero(diff)[:5])
-        assert diff.max(initial=0) <= 1, what
-
-
-def _reads(obj, x, lens16):
-    """process_read over the read sequence: (pcm per channel, PCM count per read)."""
-    parts, counts = [], []
-    for pos, n in fac.seq_bounds(x.size, lens16):
-        r = obj.process_read(x[pos:pos + n])
-        parts.append(r)
-        counts.append(r.shape[-1])
-    return np.concatenate(parts, axis=-1), counts
-
-
-# name -> (parameters, process or read, chunk int16, call lengths in int16, kernel_kind, input of one stream);
-# the shapes of tests/test_fm_group_gpu.py that reach each route of a plain handle
-ROUTES = {
-    "rows": (frd.FM2B, "process", 8 * 2048, [2 * 32768, 2 * 32768], 1),
-    "stream": (fac.FM2A, "process", 32768, [2 * 98304, 2 * 98304], 3),
-    "spec3": (fac.FM5A, "process", 2 * 25000, [2 * 50000, 2 * 25000], 0),
-    "any": (fac.FM5A, "process", 2 * 2003, [2 * 3 * 2003, 2 * (2 * 2003 + 457)], 0),
-    "read_passes": (frd.FM2B, "read", 0, [2 * 1021, 2 * 333, 2 * 4093], 0),
-}
-
-
-@pytest.mark.parametrize("name", sorted(ROUTES))
+@pytest.mark.parametrize("name", sorted(fh.KERNEL_ROUTES))
 def test_zero_offset_is_a_plain_handle(name):
     """Channel f = 0 of a two-channel handle is byte for byte a plain one-channel handle on the capture, on the route
     the plain handle takes."""
-    p, mode, chunk, lens, kind = ROUTES[name]
+    p, mode, chunk, lens, kind = fh.KERNEL_ROUTES[name]
     x = fac.signal(sum(lens) // 2, 40)
     mx = fm.FmMix(p, 2_400_000, [0, 300_000])
     d = fm.FmDemod(p)
@@ -143,9 +86,9 @@ def test_k_channels_equal_the_port(k, port):
     offs = [12500 * (j - k // 2) for j in range(k)]                       # a 12.5 kHz raster, up to +-200 kHz
     x = fmx.capture(fmx.n_complex_for(fmx.READS), rate, offs[::5], 800 + k)
     mx = fm.FmMix(p, rate, offs)
-    got, _ = _reads(mx, x, fmx.READS)
-    for j, (want, _, wh) in enumerate(_port_channels(port, p, rate, offs, x, fmx.READS)):
-        _compare(p, got[j], want, (k, offs[j]))
+    got, _ = fh.reads(mx, x, fmx.READS)
+    for j, (want, _, wh) in enumerate(fh.port_channels(port, p, rate, offs, x, fmx.READS)):
+        fh.compare(p, got[j], want, (k, offs[j]))
         assert mx.squelch_hits()[j] == wh[-1]
     mx.close()
 
@@ -157,10 +100,10 @@ def test_shapes_equal_the_port(name, port):
     p = fm.FmParams.from_any(p)
     p.report_levels = 1 if p.squelch_level else 0
     mx = fm.FmMix(p, rate, offs)
-    got, _ = _reads(mx, x, fmx.READS)
-    ref = _port_channels(port, fac.P(**fm.FmParams.from_any(p).reference_fields()), rate, offs, x, fmx.READS)
+    got, _ = fh.reads(mx, x, fmx.READS)
+    ref = fh.port_channels(port, fac.P(**fm.FmParams.from_any(p).reference_fields()), rate, offs, x, fmx.READS)
     for j, (want, _, wh) in enumerate(ref):
-        _compare(p, got[j], want, (name, offs[j]))
+        fh.compare(p, got[j], want, (name, offs[j]))
         assert mx.squelch_hits()[j] == wh[-1], (name, j)
     if p.report_levels:
         # -L of the last read against the port's level of that read
@@ -183,25 +126,25 @@ def test_phase_across_calls_reads_and_reset(port):
     several = np.concatenate([mx.full_demod(x[a:b], c16) for a, b in zip(cuts, cuts[1:])], axis=1)
     assert several.tobytes() == one.tobytes()
     mx.reset()
-    reads, _ = _reads(mx, x, [c16])
+    reads, _ = fh.reads(mx, x, [c16])
     assert reads.tobytes() == one.tobytes()
     # ragged reads (1021:333:4093), twice with a reset between: the phases restart at 0
     mx.reset()
-    first, counts = _reads(mx, x, fmx.READS)
+    first, counts = fh.reads(mx, x, fmx.READS)
     mx.reset()
-    again, _ = _reads(mx, x, fmx.READS)
+    again, _ = fh.reads(mx, x, fmx.READS)
     assert again.tobytes() == first.tobytes()
-    for j, (want, rl, _) in enumerate(_port_channels(port, p, rate, offs, x, fmx.READS)):
+    for j, (want, rl, _) in enumerate(fh.port_channels(port, p, rate, offs, x, fmx.READS)):
         assert first[j].tobytes() == want.tobytes() and counts == rl.tolist(), j
     mx.close()
 
 
 @pytest.mark.parametrize("name", ["fm5a_lut_d100", "fm2b_f9"])
 def test_device_entries_with_an_unaligned_capture(name):
-    torch = _torch()
+    torch = fh.torch()
     p, rate, offs, x = fmx.case_input(name, seed=7)
     host = fm.FmMix(p, rate, offs)
-    want_reads, counts = _reads(host, x, fmx.READS)
+    want_reads, counts = fh.reads(host, x, fmx.READS)
     host.reset()
     chunk = 2 * 4096 if p.downsample_passes else 2 * 1021
     n = (x.size // chunk) * chunk
@@ -225,15 +168,8 @@ def test_device_entries_with_an_unaligned_capture(name):
     mx.close()
 
 
-def _raw(mx, x, chunk, stride, pcm=True):
-    out = np.zeros((mx.n_channels, max(stride, 1)), dtype=np.int16)
-    n_pcm = C.c_size_t(0)
-    return _lib.lib().rxb200_fm_mix_process(mx._m, x.ctypes.data, x.size, chunk, out.ctypes.data if pcm else None,
-                                            stride, C.byref(n_pcm), None)
-
-
 def test_refusals_leave_state_alone(port):
-    torch = _torch()
+    torch = fh.torch()
     p, rate, offs, kw = fmx.SHAPES["fm2b_f9"]
     chunk = 8 * 2048
     x = fmx.capture(3 * chunk // 2, rate, offs, 8, **kw)
@@ -245,9 +181,9 @@ def test_refusals_leave_state_alone(port):
         with pytest.raises(_lib.Rxb200Error) as e:
             call()
         assert e.value.code == code
-    assert _raw(mx, rest, chunk, 1) == _lib.ECAPACITY
-    assert _raw(mx, rest, chunk, 1 << 16, pcm=False) == _lib.EINVAL
-    assert _lib.lib().rxb200_fm_mix_process(mx._m, None, rest.size, chunk, rest.ctypes.data, 1 << 16, None,
+    assert fh.raw_process(mx, rest, chunk, 1) == _lib.ECAPACITY
+    assert fh.raw_process(mx, rest, chunk, 1 << 16, pcm=False) == _lib.EINVAL
+    assert _lib.lib().rxb200_fm_mix_process(mx._h, None, rest.size, chunk, rest.ctypes.data, 1 << 16, None,
                                             None) == _lib.EINVAL
     d_in = torch.from_numpy(np.concatenate([np.zeros(1, np.int16), rest])).cuda()
     d_out = torch.zeros(1 << 16, dtype=torch.int16, device="cuda")
@@ -255,7 +191,7 @@ def test_refusals_leave_state_alone(port):
         mx.process_device(d_in.data_ptr() + 2, rest.size, chunk, d_out.data_ptr(), 1 << 14)
     assert e.value.code == _lib.EINVAL
     b = mx.full_demod(rest, chunk)
-    want = _port_channels(port, p, rate, offs, x[:3 * chunk], [chunk])
+    want = fh.port_channels(port, p, rate, offs, x[:3 * chunk], [chunk])
     for j in range(len(offs)):
         assert np.concatenate([a[j], b[j]]).tobytes() == want[j][0].tobytes(), j
     mx.close()
@@ -288,7 +224,7 @@ def test_golden():
         g = gold[name]
         assert g["capture_sha256"] == hashlib.sha256(x.tobytes()).hexdigest(), name
         mx = fm.FmMix(p, rate, offs)
-        got, counts = _reads(mx, x, g["lens_int16"])
+        got, counts = fh.reads(mx, x, g["lens_int16"])
         for j, c in enumerate(g["channels"]):
             assert c["offset_hz"] == offs[j]
             if fac.INTEGER(p):

@@ -5,7 +5,6 @@ members that own no channel.  The golden hashes of the reference hold through a 
 ragged reads and restart at reset, refused calls leave every member's phases and carries alone, and the caller's current
 device stays.  Members repeat ordinal 0, so one H100 runs the whole group; the same cases run on distinct ordinals where
 the box has that many GPUs."""
-import ctypes as C
 import hashlib
 import json
 import os
@@ -14,8 +13,8 @@ import numpy as np
 import pytest
 
 import fm_any_chunk as fac
+import fm_handles as fh
 import fm_mix as fmx
-import fm_read as frd
 from rx_tools_b200 import _lib, fm, sharding
 
 pytestmark = pytest.mark.gpu
@@ -25,80 +24,14 @@ GOLDEN = os.path.join(HERE, "golden", "fm_mix_golden.json")
 RATE = 2_400_000
 
 
-def _n_gpus():
-    return int(_lib.lib().rxb200_device_count())
-
-
-LAYOUTS = [("same", [0, 0]), ("same", [0, 0, 0]), ("same", [0, 0, 0, 0]),
-           ("distinct", [0, 1]), ("distinct", [0, 1, 2]), ("distinct", [0, 1, 2, 3])]
-LAYOUT_IDS = [f"{k}-{len(d)}" for k, d in LAYOUTS]
-
-
-def _devices(layout):
-    kind, devs = layout
-    if _n_gpus() < max(devs) + 1:
-        pytest.skip(f"needs {max(devs) + 1} GPUs")
-    return devs
-
-
-def _with_levels(p):
-    q = fm.FmParams.from_any(p)
-    q.report_levels = 1
-    return q
-
-
 def _offsets(k):
     """k channels on a 12.5 kHz raster around the capture's centre (up to +-200 kHz at k = 33)."""
     return [12500 * (j - k // 2) for j in range(k)]
 
 
-# name -> (parameters, process or read, chunk int16, call lengths in int16, kernel_kind every handle reports, input):
-# the route shapes of tests/test_fm_mix_gpu.py (ROUTES), and the per-chunk reduction stages (squelch with -L)
-ROUTES = {
-    "rows": (frd.FM2B, "process", 8 * 2048, [2 * 32768, 2 * 32768], 1, fac.signal),
-    "stream": (fac.FM2A, "process", 32768, [2 * 98304, 2 * 98304], 3, fac.signal),
-    "spec3": (fac.FM5A, "process", 2 * 25000, [2 * 50000, 2 * 25000], 0, fac.signal),
-    "any": (fac.FM5A, "process", 2 * 2003, [2 * 3 * 2003, 2 * (2 * 2003 + 457)], 0, fac.signal),
-    "read_passes": (frd.FM2B, "read", 0, [2 * 1021, 2 * 333, 2 * 4093], 0, fac.signal),
-    "squelch_levels": (_with_levels(fac.with_(fac.FM24K_LUT, squelch_level=60)), "process", 2 * 2003,
-                       [2 * 4 * 2003, 2 * (2003 + 457)], 0, fac.loud_quiet),
-}
-
-
-def _inner_kinds(g):
-    kinds = []
-    for i in range(g.n_dev):
-        h = g.inner(i)
-        if h:
-            s = _lib.FmStatsC()
-            _lib.check(_lib.lib().rxb200_fm_last_stats(C.c_void_p(h), C.byref(s)))
-            kinds.append(s.kernel_kind)
-    return kinds
-
-
-def _call(obj, mode, x, chunk):
-    """One call on a FmMix or a FmMixGroup: (pcm, chunk result lengths or None)."""
-    if mode == "read":
-        return obj.process_read(x), None
-    return obj.full_demod(x, chunk, return_chunks=True)
-
-
-def _same_as_single(g, mx, mode, x, chunk, what):
-    """One call on both; everything the group reports equals the single mixing handle's."""
-    got, gl = _call(g, mode, x, chunk)
-    want, wl = _call(mx, mode, x, chunk)
-    assert got.shape == want.shape and got.tobytes() == want.tobytes(), what
-    if wl is not None:
-        assert gl.tolist() == wl.tolist(), what
-    assert g.squelch_hits().tolist() == mx.squelch_hits().tolist(), what
-    if g.params.report_levels:
-        assert g.levels().tolist() == mx.levels().tolist(), what
-    return got
-
-
 def _members_match_shards(g):
     """Member i has a handle exactly when its shard of the channels is not empty; returns how many have one."""
-    assert _lib.lib().rxb200_fm_mix_group_size(g._g) == g.n_dev
+    assert _lib.lib().rxb200_fm_mix_group_size(g._h) == g.n_dev
     owners = 0
     for i in range(g.n_dev):
         b, e = sharding.unit_range(i, g.n_dev, g.n_channels)
@@ -108,14 +41,14 @@ def _members_match_shards(g):
     return owners
 
 
-@pytest.mark.parametrize("layout", LAYOUTS, ids=LAYOUT_IDS)
+@pytest.mark.parametrize("layout", fh.LAYOUTS, ids=fh.LAYOUT_IDS)
 @pytest.mark.parametrize("k", [1, 3, 5, 8, 33])
-@pytest.mark.parametrize("name", sorted(ROUTES))
+@pytest.mark.parametrize("name", sorted(fh.ROUTES))
 def test_routes_match_one_mixing_handle(name, k, layout):
     """Every call of the route's sequence, a reset, and its first call again; every member's inner handle runs the
     kernel the single handle runs."""
-    devices = _devices(layout)
-    p, mode, chunk, lens, kind, make = ROUTES[name]
+    devices = fh.devices(layout)
+    p, mode, chunk, lens, kind, make = fh.ROUTES[name]
     offs = _offsets(k)
     x = make(sum(lens) // 2, 50 + k)
     g = fm.FmMixGroup(p, RATE, offs, devices)
@@ -128,20 +61,20 @@ def test_routes_match_one_mixing_handle(name, k, layout):
             mx.reset()
             continue
         pos, n = step
-        _same_as_single(g, mx, mode, x[pos:pos + n], chunk, (name, k, c))
+        fh.same_as_single(g, mx, mode, x[pos:pos + n], chunk, (name, k, c))
         assert mx.stats()["kernel_kind"] == kind, (name, k, c, mx.stats())
-        kinds = _inner_kinds(g)
+        kinds = fh.kernel_kinds(map(g.inner, range(g.n_dev)))
         assert len(kinds) == owners and kinds == [kind] * len(kinds), (name, k, c, kinds)
     g.close()
     mx.close()
 
 
-@pytest.mark.parametrize("layout", LAYOUTS, ids=LAYOUT_IDS)
+@pytest.mark.parametrize("layout", fh.LAYOUTS, ids=fh.LAYOUT_IDS)
 def test_mixed_call_sequence_then_reset(layout):
     """process and process_read calls of several lengths on one group, reset, and the sequence again: chunk result
     lengths, squelch hits and levels after every call."""
-    devices = _devices(layout)
-    p = ROUTES["squelch_levels"][0]
+    devices = fh.devices(layout)
+    p = fh.ROUTES["squelch_levels"][0]
     offs = _offsets(7)
     calls = [("process", 2 * 2003, 2 * 3 * 2003), ("read", 0, 2 * 1777), ("process", 2 * 4096, 2 * 8 * 4096),
              ("read", 0, 2 * 5003), ("process", 2 * 999, 2 * (5 * 999 + 431)), ("read", 0, 2 * 257)]
@@ -151,23 +84,13 @@ def test_mixed_call_sequence_then_reset(layout):
     for rnd in range(2):
         pos = 0
         for c, (mode, chunk, n) in enumerate(calls):
-            _same_as_single(g, mx, mode, x[pos:pos + n], chunk, (rnd, c, mode))
+            fh.same_as_single(g, mx, mode, x[pos:pos + n], chunk, (rnd, c, mode))
             pos += n
         g.reset()
         mx.reset()
         assert g.squelch_hits().tolist() == mx.squelch_hits().tolist()
     g.close()
     mx.close()
-
-
-def _reads(obj, x, lens16):
-    """process_read over the read sequence: (pcm per channel, PCM count per read)."""
-    parts, counts = [], []
-    for pos, n in fac.seq_bounds(x.size, lens16):
-        r = obj.process_read(x[pos:pos + n])
-        parts.append(r)
-        counts.append(r.shape[-1])
-    return np.concatenate(parts, axis=-1), counts
 
 
 def test_golden_through_a_group_of_three():
@@ -180,9 +103,9 @@ def test_golden_through_a_group_of_three():
         gd = gold[name]
         assert gd["capture_sha256"] == hashlib.sha256(x.tobytes()).hexdigest(), name
         g = fm.FmMixGroup(p, rate, offs, [0, 0, 0])
-        got, counts = _reads(g, x, gd["lens_int16"])
+        got, counts = fh.reads(g, x, gd["lens_int16"])
         mx = fm.FmMix(p, rate, offs)
-        want, _ = _reads(mx, x, gd["lens_int16"])
+        want, _ = fh.reads(mx, x, gd["lens_int16"])
         assert got.tobytes() == want.tobytes(), name
         for j, c in enumerate(gd["channels"]):
             assert c["offset_hz"] == offs[j]
@@ -193,48 +116,34 @@ def test_golden_through_a_group_of_three():
         mx.close()
 
 
-@pytest.mark.parametrize("layout", LAYOUTS, ids=LAYOUT_IDS)
+@pytest.mark.parametrize("layout", fh.LAYOUTS, ids=fh.LAYOUT_IDS)
 def test_phases_across_ragged_reads_and_reset(layout):
     """Ragged reads (1021:333:4093) over part of the capture, a reset, the whole read sequence, then chunk calls that
     end off a chunk: the phases run on across every call and restart at the reset, as in the single handle."""
-    devices = _devices(layout)
+    devices = fh.devices(layout)
     p, rate, offs, x = fmx.case_input("fm5a_lut_d100", seed=6)
     offs = offs + [-50000, 62500, 100000]                 # 7 channels: every member of 4 owns some
     g = fm.FmMixGroup(p, rate, offs, devices)
     mx = fm.FmMix(p, rate, offs)
     bounds = list(fac.seq_bounds(x.size, fmx.READS))
     for c, (pos, n) in enumerate(bounds[:len(bounds) // 2]):
-        _same_as_single(g, mx, "read", x[pos:pos + n], 0, ("first half", c))
+        fh.same_as_single(g, mx, "read", x[pos:pos + n], 0, ("first half", c))
     g.reset()
     mx.reset()
     parts = []
     for c, (pos, n) in enumerate(bounds):
-        parts.append(_same_as_single(g, mx, "read", x[pos:pos + n], 0, ("after reset", c)))
+        parts.append(fh.same_as_single(g, mx, "read", x[pos:pos + n], 0, ("after reset", c)))
     c16 = 2 * 1021
     cuts = [0, 3 * c16, 4 * c16 + 2 * 17, 11 * c16, x.size]
     for a, b in zip(cuts, cuts[1:]):
-        _same_as_single(g, mx, "process", x[a:b], c16, ("chunks", a))
+        fh.same_as_single(g, mx, "process", x[a:b], c16, ("chunks", a))
     g.close()
     mx.close()
     # the reads after the reset are those of a fresh single handle
     fresh = fm.FmMix(p, rate, offs)
-    want, _ = _reads(fresh, x, fmx.READS)
+    want, _ = fh.reads(fresh, x, fmx.READS)
     assert np.concatenate(parts, axis=1).tobytes() == want.tobytes()
     fresh.close()
-
-
-def _raw_process(g, x, chunk, stride, pcm=True):
-    out = np.zeros((g.n_channels, max(stride, 1)), dtype=np.int16)
-    n_pcm = C.c_size_t(0)
-    return _lib.lib().rxb200_fm_mix_group_process(g._g, x.ctypes.data, x.size, chunk, out.ctypes.data if pcm else None,
-                                                  stride, C.byref(n_pcm), None)
-
-
-def _raw_single(mx, x, chunk, stride, pcm=True):
-    out = np.zeros((mx.n_channels, max(stride, 1)), dtype=np.int16)
-    n_pcm = C.c_size_t(0)
-    return _lib.lib().rxb200_fm_mix_process(mx._m, x.ctypes.data, x.size, chunk, out.ctypes.data if pcm else None,
-                                            stride, C.byref(n_pcm), None)
 
 
 def _refused(g, mx, call, code):
@@ -244,9 +153,9 @@ def _refused(g, mx, call, code):
         assert e.value.code == code, (obj, e.value)
 
 
-@pytest.mark.parametrize("layout", LAYOUTS, ids=LAYOUT_IDS)
+@pytest.mark.parametrize("layout", fh.LAYOUTS, ids=fh.LAYOUT_IDS)
 def test_refusals_leave_every_member_alone(layout):
-    devices = _devices(layout)
+    devices = fh.devices(layout)
     # fifth_order passes (fm2b shape), 5 channels: chunk 8 rows
     p, rate, _, kw = fmx.SHAPES["fm2b_f9"]
     offs = [-600000, -300000, 0, 450000, 900000]
@@ -255,7 +164,7 @@ def test_refusals_leave_every_member_alone(layout):
     g = fm.FmMixGroup(p, rate, offs, devices)
     mx = fm.FmMix(p, rate, offs)
     pos = chunk
-    _same_as_single(g, mx, "process", x[:pos], chunk, "first")
+    fh.same_as_single(g, mx, "process", x[:pos], chunk, "first")
     rest = np.ascontiguousarray(x[pos:pos + chunk])
     refusals = [
         (lambda o: o.full_demod(rest[:2 * 1001], 2 * 1001), _lib.EUNSUPPORTED),      # a chunk off the passes' granule
@@ -263,16 +172,16 @@ def test_refusals_leave_every_member_alone(layout):
     ]
     for c, (call, code) in enumerate(refusals):
         _refused(g, mx, call, code)
-        _same_as_single(g, mx, "process", x[pos:pos + chunk], chunk, ("after refusal", c))
+        fh.same_as_single(g, mx, "process", x[pos:pos + chunk], chunk, ("after refusal", c))
         pos += chunk
     for c, (stride, pcm, code) in enumerate(((1, True, _lib.ECAPACITY), (1 << 16, False, _lib.EINVAL))):
-        assert _raw_process(g, rest, chunk, stride, pcm) == code
-        assert _raw_single(mx, rest, chunk, stride, pcm) == code
-        _same_as_single(g, mx, "process", x[pos:pos + chunk], chunk, ("after raw refusal", c))
+        assert fh.raw_process(g, rest, chunk, stride, pcm) == code
+        assert fh.raw_process(mx, rest, chunk, stride, pcm) == code
+        fh.same_as_single(g, mx, "process", x[pos:pos + chunk], chunk, ("after raw refusal", c))
         pos += chunk
-    assert _lib.lib().rxb200_fm_mix_group_process(g._g, None, rest.size, chunk, rest.ctypes.data, 1 << 16, None,
+    assert _lib.lib().rxb200_fm_mix_group_process(g._h, None, rest.size, chunk, rest.ctypes.data, 1 << 16, None,
                                                   None) == _lib.EINVAL
-    _same_as_single(g, mx, "process", x[pos:pos + chunk], chunk, "after a null capture")
+    fh.same_as_single(g, mx, "process", x[pos:pos + chunk], chunk, "after a null capture")
     g.close()
     mx.close()
     # per-chunk reduction stages: a last chunk of 4 complex samples makes no decimated sample, so the call is refused
@@ -283,11 +192,11 @@ def test_refusals_leave_every_member_alone(layout):
     x = fmx.capture(6000, rate, offs, 9, quiet_half=True)
     g = fm.FmMixGroup(q, rate, offs, devices)
     mx = fm.FmMix(q, rate, offs)
-    _same_as_single(g, mx, "process", x[:2 * 3000], 2 * 1000, "first")
+    fh.same_as_single(g, mx, "process", x[:2 * 3000], 2 * 1000, "first")
     lv = g.levels()
     _refused(g, mx, lambda o: o.full_demod(x[2 * 3000:2 * 3000 + 2 * 1004], 2 * 1000), _lib.EUNSUPPORTED)
     assert g.levels().tolist() == lv.tolist()
-    _same_as_single(g, mx, "process", x[2 * 3000:], 2 * 1000, "after the refusal")
+    fh.same_as_single(g, mx, "process", x[2 * 3000:], 2 * 1000, "after the refusal")
     g.close()
     mx.close()
 
@@ -295,10 +204,10 @@ def test_refusals_leave_every_member_alone(layout):
 def test_caller_device_is_kept():
     """A group whose members sit on another GPU leaves the caller's current device as it was, after every entry
     point."""
-    if _n_gpus() < 2:
+    if fh.n_gpus() < 2:
         pytest.skip("needs 2 GPUs")
     import torch
-    p = ROUTES["squelch_levels"][0]
+    p = fh.ROUTES["squelch_levels"][0]
     offs = _offsets(3)
     x = fac.loud_quiet(4000, 600)
     for caller, members in ((0, [1, 1]), (1, [0, 0, 0])):

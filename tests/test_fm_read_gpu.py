@@ -3,7 +3,6 @@ length with the squelch hits and -L level after each read, a seeded sweep, sever
 4-byte alignment ending where its allocation ends, reads on the read kernel followed on one handle by calls of the row
 and fused kernels and the reverse, the golden hashes of the reference, refusals that leave the state alone, and
 rx_fm_b200 -M wbfm -s 300k -F 9 -r 48k over a device that returns reads of other lengths than the passes' granule."""
-import ctypes as C
 import hashlib
 import json
 import os
@@ -34,12 +33,6 @@ def _compare(p, got, want, what):
         assert bad.size == 0, (what, bad[:5], got[bad[:5]], want[bad[:5]])
     else:       # fp64 atan2 (CUDA libm vs glibc): a last-ulp difference may move an isolated sample by 1 LSB
         assert np.count_nonzero(diff) <= max(2, int(1e-4 * diff.size)), (what, np.flatnonzero(diff)[:5])
-
-
-def _hits(d):
-    h = np.zeros(d.n_channels, dtype=np.int32)
-    _lib.check(_lib.lib().rxb200_fm_squelch_hits(d._h, h.ctypes.data_as(C.POINTER(C.c_int))))
-    return h
 
 
 def _off_granule(n16, p_):
@@ -73,7 +66,7 @@ def test_read_sequences(name, port):
     def check(c, part):
         assert part.size == wl[c], (name, c)
         if p.squelch_level:
-            assert _hits(d)[0] == wh[c], (name, c)
+            assert d.squelch_hits()[0] == wh[c], (name, c)
 
     got = _run_reads(d, x, lens, check)
     got_l = []
@@ -81,7 +74,7 @@ def test_read_sequences(name, port):
         got_l.append(dl.process_read(x[pos:pos + n]))
         assert dl.levels()[0].tolist() == [want_lv[c]], (name, c)
         if p.squelch_level:
-            assert _hits(dl)[0] == wh[c], (name, c)
+            assert dl.squelch_hits()[0] == wh[c], (name, c)
     _compare(p, got, want, name)
     _compare(p, np.concatenate(got_l), want, (name, "levels"))
     d.close()
@@ -228,7 +221,7 @@ def test_refusals_leave_the_state_alone(port):
     assert e.value.code == _lib.EUNSUPPORTED
     h.close()
     b = d.process_read(x[lens[0]:])
-    assert _hits(d)[0] == wh[-1]
+    assert d.squelch_hits()[0] == wh[-1]
     _compare(p, np.concatenate([a, b]), want, "after refusals")
     d.close()
     # rxb200_fm_process keeps its granule with passes

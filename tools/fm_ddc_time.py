@@ -72,7 +72,7 @@ def run(kind, k, x_pin, d_x, reps):
 
     def host_call():
         mx.reset()
-        _lib.check(_lib.lib().rxb200_fm_mix_process(mx._m, x_pin.data_ptr(), n, CHUNK, h_out.data_ptr(), cap,
+        _lib.check(_lib.lib().rxb200_fm_mix_process(mx._h, x_pin.data_ptr(), n, CHUNK, h_out.data_ptr(), cap,
                                                     C.byref(n_pcm), None))
 
     dev_ms = timed(device_call, reps)

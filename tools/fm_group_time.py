@@ -92,7 +92,7 @@ def main():
         h_out.zero_()
 
         def group_call():
-            _lib.check(L.rxb200_fm_group_process(g._g, h_in.data_ptr(), n_int16, CHUNK, h_out.data_ptr(), cap,
+            _lib.check(L.rxb200_fm_group_process(g._h, h_in.data_ptr(), n_int16, CHUNK, h_out.data_ptr(), cap,
                                                  C.byref(n_pcm), None))
         group_call()
         equal = n_pcm.value == want.shape[1] and h_out.numpy()[:, :n_pcm.value].tobytes() == want.tobytes()

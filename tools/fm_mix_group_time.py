@@ -66,7 +66,7 @@ def main():
     for K, raster in RASTERS.items():
         offs = [raster * (k - K // 2) for k in range(K)]
         mx = fm.FmMix(p, RATE, offs)
-        cap = mx._cap(n_int16, CHUNK)
+        cap = mx.max_output(n_int16, CHUNK) + 8
         h_out = torch.zeros((K, cap), dtype=torch.int16, pin_memory=True)
         n_pcm = C.c_size_t(0)
 
@@ -77,7 +77,7 @@ def main():
             rows.append(row)
 
         def single_call():
-            _lib.check(L.rxb200_fm_mix_process(mx._m, h_cap.data_ptr(), n_int16, CHUNK, h_out.data_ptr(), cap,
+            _lib.check(L.rxb200_fm_mix_process(mx._h, h_cap.data_ptr(), n_int16, CHUNK, h_out.data_ptr(), cap,
                                                C.byref(n_pcm), None))
         single_call()
         want = h_out.numpy()[:, :n_pcm.value].copy()
@@ -92,7 +92,7 @@ def main():
             h_out.zero_()
 
             def group_call():
-                _lib.check(L.rxb200_fm_mix_group_process(g._g, h_cap.data_ptr(), n_int16, CHUNK, h_out.data_ptr(), cap,
+                _lib.check(L.rxb200_fm_mix_group_process(g._h, h_cap.data_ptr(), n_int16, CHUNK, h_out.data_ptr(), cap,
                                                          C.byref(n_pcm), None))
             group_call()
             equal = n_pcm.value == want.shape[1] and h_out.numpy()[:, :n_pcm.value].tobytes() == want.tobytes()

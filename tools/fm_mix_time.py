@@ -56,7 +56,7 @@ def main():
     for K in KS:
         offs = [12500 * (k - K // 2) for k in range(K)]
         mx = fm.FmMix(p, RATE, offs)
-        cap = mx._cap(n_int16, CHUNK)
+        cap = mx.max_output(n_int16, CHUNK) + 8
         d_out = torch.zeros((K, cap), dtype=torch.int16, device="cuda")
         # device-resident
         stream = torch.cuda.ExternalStream(mx.stream)
@@ -76,7 +76,7 @@ def main():
         n_pcm = C.c_size_t(0)
 
         def mix_call():
-            _lib.check(L.rxb200_fm_mix_process(mx._m, h_cap.data_ptr(), n_int16, CHUNK, h_out.data_ptr(), cap,
+            _lib.check(L.rxb200_fm_mix_process(mx._h, h_cap.data_ptr(), n_int16, CHUNK, h_out.data_ptr(), cap,
                                                C.byref(n_pcm), None))
         mx.reset()
         mix_call()
