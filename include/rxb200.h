@@ -56,6 +56,10 @@ int rxb200_device_count(void);
 #define RXB200_ATAN_FAST 1  /* polar_disc_fast    :508 (integer)     */
 #define RXB200_ATAN_LUT  2  /* polar_disc_lut     :528 (integer LUT) */
 #define RXB200_ATAN_ALE  3  /* esbensen           :566 (integer)     */
+/* One deviation from the reference in -A lut: where (cj << 8) wraps to INT_MIN with |cr| = 1 (cj = 2^23 mod 2^24,
+ * reachable once decimated samples pass 2048), polar_disc_lut indexes its table at INT_MIN (cr = 1) or divides INT_MIN
+ * by -1 (cr = -1) and the reference process crashes; the library returns cj > 0 ? 8192 : -8192 there, the value its
+ * linear-range branch gives every other |x| it cannot look up (DESIGN.md section 6). */
 
 /* The configuration fields of struct demod_state / dongle_state the DSP reads, with the reference's
  * names (src/rtl_fm.c:124-159).  Fill them as main()/optimal_settings() would, or let
@@ -206,6 +210,33 @@ int rxb200_fm_tune(rxb200_fm *h, int segment_len, int deemph_warmup);
  * milliseconds: the split kernel on the row path, the fused kernel's main pass (not its per-chunk
  * reduction pre-passes), or the front and back kernels on the stream path.  Synchronises the stream. */
 int rxb200_fm_kernel_ms(rxb200_fm *h, float *ms);
+
+/* The discriminators alone, for tests: one thread per element of n quads (ar, aj, br, bj) of int32 -- the sample
+ * x[n] = (ar, aj) and the one before it -- in DEVICE memory (16-byte aligned), on `stream` (a cudaStream_t, may be NULL).
+ * The kernel forms the conjugate product cr = ar br + aj bj, cj = aj br - ar bj with int32 wrap, as the chains do (so the
+ * quad (cr, cj, 1, 0) hands any operand pair through), and writes d_out[i] (int32) of the device function `form` names:
+ *   RXB200_DISC_STD      disc_std_f32: every -A std sample
+ *   RXB200_DISC_FAST     fast_atan2_i: -A fast on the fused and any-length kernels
+ *   RXB200_DISC_LUT      disc_lut on the host-built table: -A lut
+ *   RXB200_DISC_ALE      disc_ale: -A ale
+ *   RXB200_DISC_ATAN2    disc_std (libm atan2): the first FM sample of every chunk in every mode
+ *   RXB200_DISC_STD_FP64 disc_std_lean: the fp64 form alone, also on operands disc_std_f32 decides in FP32
+ *   RXB200_DISC_ROWS     the int16 the row front end stores for one sample (FP32 fast_atan2, the integer form past
+ *                        ||cr| - |cj|| >= 2^19); exact for |cr| + |cj| < 2^24, which its operands always meet
+ *   RXB200_DISC_STREAM   the int16 the undecimated stream front end stores (FP32 product and fast_atan2); exact for
+ *                        8-bit-range samples
+ *   RXB200_DISC_AM       (int16)(int)sqrt(ar^2 + aj^2) with int32 wrap: the AM envelope
+ * Asynchronous (the LUT form's table is freed behind the launch).  RXB200_EINVAL for an unknown form or bad pointer. */
+#define RXB200_DISC_STD      RXB200_ATAN_STD
+#define RXB200_DISC_FAST     RXB200_ATAN_FAST
+#define RXB200_DISC_LUT      RXB200_ATAN_LUT
+#define RXB200_DISC_ALE      RXB200_ATAN_ALE
+#define RXB200_DISC_ATAN2    4
+#define RXB200_DISC_STD_FP64 5
+#define RXB200_DISC_ROWS     6
+#define RXB200_DISC_STREAM   7
+#define RXB200_DISC_AM       8
+int rxb200_fm_disc_device(int form, const int32_t *d_quads, size_t n, int32_t *d_out, void *stream);
 
 /* ======================================================================== rx_power
  * Replaces scanner()'s per-hop body (src/rtl_power.c:709-771): copy, boxcar | downsample_iq x P +

@@ -116,6 +116,41 @@ def _p16(a: np.ndarray):
     return a.ctypes.data_as(C.POINTER(C.c_int16))
 
 
+def _entry(L: C.CDLL, name: str, restype, argtypes):
+    """An entry point of a checker library, typed on first use.  The libraries travel prebuilt (oracle/_ref cannot be
+    rebuilt where the reference sources are absent), so one built before an entry point existed must still serve every
+    caller that does not need it: only a call of the missing entry point fails, and it says how to fix that."""
+    fn = getattr(L, name, None)
+    if fn is None:
+        raise RuntimeError(f"{L._name} has no {name}: it was built before this entry point existed; "
+                           "rebuild it with oracle.build(force=True) where the reference sources are present")
+    fn.restype = restype
+    fn.argtypes = argtypes
+    return fn
+
+
+def conj_product(quads: np.ndarray):
+    """(cr, cj) = x[n] * conj(x[n-1]) of int32 quads [n][4] (ar, aj, br, bj) with int32 wrap (src/rtl_fm.c:470-480)."""
+    q = np.asarray(quads, dtype=np.int64).reshape(-1, 4)
+    cr = (q[:, 0] * q[:, 2] + q[:, 1] * q[:, 3]).astype(np.uint64).astype(np.uint32).view(np.int32)
+    cj = (q[:, 1] * q[:, 2] - q[:, 0] * q[:, 3]).astype(np.uint64).astype(np.uint32).view(np.int32)
+    return cr, cj
+
+
+def _check_defined(form: int, q: np.ndarray) -> None:
+    """The port's C division traps (and ends the process) on two operand sets no int16 chain produces: fast_atan2 at
+    cr == cj == INT_MIN (a division by zero), esbensen at divisors 0 and -1.  Refuse them before the call."""
+    if form in (ATAN_FAST, 6, 7):
+        cr, cj = conj_product(q)
+        if np.any((cr == np.iinfo(np.int32).min) & (cj == np.iinfo(np.int32).min)):
+            raise ValueError("fast_atan2 is undefined at cr == cj == INT_MIN")
+    if form == ATAN_ALE:
+        a = q[:, :2].astype(np.int64)
+        den = ((a * a).sum(axis=1) + 1).astype(np.uint64).astype(np.uint32).view(np.int32)
+        if np.any((den == 0) | (den == -1)):
+            raise ValueError("esbensen's divisor is 0 or -1")
+
+
 WINDOWS = {"rectangle": 0, "hamming": 1, "blackman": 2, "blackman-harris": 3, "hann-poisson": 4,
            "youssef": 5, "kaiser": 6, "bartlett": 7, "hann": 8}
 
@@ -160,6 +195,7 @@ class Port:
         L.orx_fast_atan2.restype = C.c_int
         L.orx_fast_atan2.argtypes = [C.c_int, C.c_int]
         self.L = L
+        self._atan = None
 
     # ---- rx_fm
     def fm_run(self, params: FmParams, cs16: np.ndarray, chunk_int16: int = 262144,
@@ -215,6 +251,27 @@ class Port:
         t = np.empty(131072, dtype=np.int32)
         self.L.orx_build_atan_table(t.ctypes.data_as(C.POINTER(C.c_int)))
         return t
+
+    def disc_many(self, form: int, quads: np.ndarray, want_near: bool = True):
+        """orx_disc_many: the port's discriminator ``form`` (rxb200_fm_disc_device's numbering) over int32 quads
+        [n][4] of (ar, aj, br, bj) -> (int32 results [n], bool flags [n]: the std value lies within 2^-30 of an
+        integer; None unless want_near)."""
+        q = np.ascontiguousarray(quads, dtype=np.int32).reshape(-1, 4)
+        _check_defined(form, q)
+        if form == ATAN_LUT and self._atan is None:
+            self._atan = self.atan_table()
+        out = np.empty(q.shape[0], dtype=np.int32)
+        near = np.empty(q.shape[0], dtype=np.uint8) if want_near else None
+        tab = self._atan.ctypes.data if form == ATAN_LUT else None
+        fn = _entry(self.L, "orx_disc_many", C.c_int, [C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p])
+        if fn(form, q.ctypes.data, q.shape[0], tab, out.ctypes.data, near.ctypes.data if want_near else None) != 0:
+            raise ValueError(form)
+        return out, (near.astype(bool) if want_near else None)
+
+    def std_near_count(self) -> int:
+        """polar_discriminant evaluations of the port's chain runs (every -A std sample and every chunk's first
+        sample) whose value lay within 2^-30 of an integer, since the last call (read and reset)."""
+        return int(_entry(self.L, "orx_std_near_count", C.c_long, [])())
 
     def droop9(self, row: int) -> np.ndarray:
         t = np.zeros(10, dtype=np.int32)
@@ -302,6 +359,18 @@ class RefFm:
         L.ref_fm_atan_lut.argtypes = [C.POINTER(C.c_int), C.c_int]
         L.ref_fm_cic9.argtypes = [C.c_int, C.POINTER(C.c_int)]
         self.L = L
+
+    def disc_many(self, form: int, quads: np.ndarray):
+        """ref_fm_disc_many: the reference's own polar_discriminant / polar_disc_fast / polar_disc_lut / esbensen
+        (form 0-3) over int32 quads [n][4] -> (int32 results [n], bool skipped [n]); a skipped quad is one the
+        reference would crash on, never handed to it (its result reads 0)."""
+        q = np.ascontiguousarray(quads, dtype=np.int32).reshape(-1, 4)
+        out = np.empty(q.shape[0], dtype=np.int32)
+        skipped = np.empty(q.shape[0], dtype=np.uint8)
+        fn = _entry(self.L, "ref_fm_disc_many", C.c_long, [C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p])
+        if fn(form, q.ctypes.data, q.shape[0], out.ctypes.data, skipped.ctypes.data) < 0:
+            raise ValueError(form)
+        return out, skipped.astype(bool)
 
     def run(self, params: FmParams, cs16: np.ndarray, chunk_int16: int = 262144, return_chunks: bool = False):
         x = _i16(cs16)

@@ -242,6 +242,36 @@ double ref_fm_time(const int16_t *in, size_t n_int16, size_t chunk_int16, int re
 	return (double)(t1.tv_sec - t0.tv_sec) + 1e-9 * (double)(t1.tv_nsec - t0.tv_nsec);
 }
 
+/* The reference's own discriminators over n quads (ar, aj, br, bj) of int32: form 0 polar_discriminant, 1
+ * polar_disc_fast, 2 polar_disc_lut, 3 esbensen.  Quads the reference cannot evaluate -- it would crash the process --
+ * are not handed to it: skipped[i] = 1 and out[i] = 0.  Those are polar_disc_lut's (cj << 8) == INT_MIN with |cr| = 1
+ * (a table read at INT_MIN, or INT_MIN / -1), fast_atan2's cr == cj == INT_MIN (a division by zero) and esbensen's
+ * divisors 0 and -1.  Returns the number skipped, or -1 for an unknown form. */
+long ref_fm_disc_many(int form, const int32_t *quads, size_t n, int32_t *out, uint8_t *skipped)
+{
+	size_t i;
+	long n_skip = 0;
+	if (form < 0 || form > 3) { return -1; }
+	if (form == 2 && !atan_lut) { atan_lut_init(); }
+	for (i = 0; i < n; i++) {
+		const int ar = quads[4 * i], aj = quads[4 * i + 1], br = quads[4 * i + 2], bj = quads[4 * i + 3];
+		int cr, cj, bad = 0, den;
+		multiply(ar, aj, br, -bj, &cr, &cj);
+		if (form == 1) { bad = cr == INT32_MIN && cj == INT32_MIN; }
+		if (form == 2) { bad = cr != 0 && cj != 0 && (int)((unsigned)cj << atan_lut_coef) == INT32_MIN && (cr == 1 || cr == -1); }
+		if (form == 3) { den = ar * ar + aj * aj + 1; bad = den == 0 || den == -1; }
+		skipped[i] = (uint8_t)bad;
+		if (bad) { out[i] = 0; n_skip++; continue; }
+		switch (form) {
+		case 0: out[i] = polar_discriminant(ar, aj, br, bj); break;
+		case 1: out[i] = polar_disc_fast(ar, aj, br, bj); break;
+		case 2: out[i] = polar_disc_lut(ar, aj, br, bj); break;
+		default: out[i] = esbensen(ar, aj, br, bj); break;
+		}
+	}
+	return n_skip;
+}
+
 /* Table exports so the host-side builders can be pinned against the reference's. */
 int ref_fm_atan_lut(int *dst, int n)
 {

@@ -234,6 +234,36 @@ int orx_disc_std(int ar, int aj, int br, int bj)
 	return (int)(atan2((double)cj, (double)cr) / 3.14159 * (double)(1 << 14));
 }
 
+/* polar_discriminant, and *near = 1 when its value v = atan2(cj, cr) / 3.14159 * 2^14 (glibc) lies within 2^-30 of an
+ * integer: the
+ * only operands where an atan2 that differs from glibc's in the last few ulps (CUDA's: |v| < 2^14, so a few ulps of
+ * atan2 move v by < 2^-35) can truncate to a different integer.  atan2(0, x >= 0) is exactly +0 in every libm and does not count. */
+static int disc_std_near(int ar, int aj, int br, int bj, int *near)
+{
+	int cr, cj;
+	double v;
+	conj_product(ar, aj, br, bj, &cr, &cj);
+	v = atan2((double)cj, (double)cr) / 3.14159 * (double)(1 << 14);
+	*near = !(cj == 0 && cr >= 0) && fabs(v - rint(v)) < 0x1p-30;
+	return (int)v;
+}
+
+/* polar_discriminant evaluations of chain runs (fm_discriminate: -A std samples and every chunk's first sample) that
+ * were near an integer, since the last orx_std_near_count() */
+static long g_std_near = 0;
+static int disc_std_counted(int ar, int aj, int br, int bj)
+{
+	int near, v = disc_std_near(ar, aj, br, bj, &near);
+	g_std_near += near;
+	return v;
+}
+long orx_std_near_count(void)
+{
+	long c = g_std_near;
+	g_std_near = 0;
+	return c;
+}
+
 /* fast_atan2 + polar_disc_fast, src/rtl_fm.c:485-513.  pi == 1<<14. */
 int orx_fast_atan2(int y, int x)
 {
@@ -251,17 +281,21 @@ int orx_disc_fast(int ar, int aj, int br, int bj)
 	return orx_fast_atan2(cj, cr);
 }
 
-/* polar_disc_lut, src/rtl_fm.c:528-564 */
+/* polar_disc_lut, src/rtl_fm.c:528-564.  One deviation: where (cj << 8) is INT_MIN and |cr| = 1 the reference reads
+ * atan_lut[INT_MIN] (cr = 1) or divides INT_MIN by -1 (cr = -1) and crashes; here, as in the library, the quotient
+ * INT_MIN takes the linear-range branch (include/rxb200.h, RXB200_ATAN_LUT). */
 int orx_disc_lut(const int *tab, int ar, int aj, int br, int bj)
 {
-	int cr, cj, q, qa;
+	int cr, cj, q, qa, num;
 	conj_product(ar, aj, br, bj, &cr, &cj);
 	if (cr == 0 || cj == 0) {
 		if (cr == 0 && cj == 0) { return 0; }
 		if (cr == 0) { return cj > 0 ? (1 << 13) : -(1 << 13); }
 		return cr > 0 ? 0 : (1 << 14);
 	}
-	q = (int)((unsigned)cj << ORX_ATAN_COEF) / cr;
+	num = (int)((unsigned)cj << ORX_ATAN_COEF);
+	if (num == INT32_MIN && (cr == 1 || cr == -1)) { return cj > 0 ? (1 << 13) : -(1 << 13); }
+	q = num / cr;
 	qa = q < 0 ? -q : q;
 	if (qa >= ORX_ATAN_SIZE) { return cj > 0 ? (1 << 13) : -(1 << 13); }
 	if (q > 0) { return cj > 0 ? tab[q] : tab[q] - (1 << 14); }
@@ -276,16 +310,45 @@ int orx_disc_ale(int ar, int aj, int br, int bj)
 	return 2608 * cj / (ar * ar + aj * aj + 1);
 }
 
+/* n quads (ar, aj, br, bj) of int32 through one discriminator, numbered as rxb200_fm_disc_device's forms: 0 std, 1 fast,
+ * 2 lut (tab: the atan table), 3 ale, 4 atan2 and 5 the fp64 form (both polar_discriminant here), 6 and 7 the int16 that
+ * the row and stream front ends store (fast_atan2's, stored), 8 the AM envelope (int16)sqrt(ar^2 + aj^2).  near (may
+ * be NULL) receives disc_std_near()'s flag for every quad.  Returns 0, or -1 for an unknown form. */
+int orx_disc_many(int form, const int32_t *quads, size_t n, const int *tab, int32_t *out, uint8_t *near)
+{
+	size_t i;
+	if (form < 0 || form > 8 || (form == 2 && !tab)) { return -1; }
+	for (i = 0; i < n; i++) {
+		const int ar = quads[4 * i], aj = quads[4 * i + 1], br = quads[4 * i + 2], bj = quads[4 * i + 3];
+		int v;
+		switch (form) {
+		case 1: v = orx_disc_fast(ar, aj, br, bj); break;
+		case 2: v = orx_disc_lut(tab, ar, aj, br, bj); break;
+		case 3: v = orx_disc_ale(ar, aj, br, bj); break;
+		case 6: case 7: v = (int16_t)orx_disc_fast(ar, aj, br, bj); break;
+		case 8: v = (int16_t)sqrt(ar * ar + aj * aj); break;      /* am_demod, src/rtl_fm.c:617-632 */
+		default: v = orx_disc_std(ar, aj, br, bj); break;
+		}
+		out[i] = v;
+		if (near) {
+			int f;
+			disc_std_near(ar, aj, br, bj, &f);
+			near[i] = (uint8_t)f;
+		}
+	}
+	return 0;
+}
+
 /* fm_demod, src/rtl_fm.c:584-615: first output of every chunk uses the atan2 path whatever
  * the selected mode (SURVEY F8). */
 static void fm_discriminate(orx_fm *o)
 {
 	const int16_t *lp = o->iq;
 	int k, v = 0;
-	o->pcm[0] = (int16_t)orx_disc_std(lp[0], lp[1], o->last_i, o->last_q);
+	o->pcm[0] = (int16_t)disc_std_counted(lp[0], lp[1], o->last_i, o->last_q);
 	for (k = 2; k < o->iq_len - 1; k += 2) {
 		switch (o->p.custom_atan) {
-		case 0: v = orx_disc_std(lp[k], lp[k + 1], lp[k - 2], lp[k - 1]); break;
+		case 0: v = disc_std_counted(lp[k], lp[k + 1], lp[k - 2], lp[k - 1]); break;
 		case 1: v = orx_disc_fast(lp[k], lp[k + 1], lp[k - 2], lp[k - 1]); break;
 		case 2: v = orx_disc_lut(o->atan_tab, lp[k], lp[k + 1], lp[k - 2], lp[k - 1]); break;
 		case 3: v = orx_disc_ale(lp[k], lp[k + 1], lp[k - 2], lp[k - 1]); break;

@@ -69,7 +69,7 @@ SYMBOLS = [
     "rxb200_fm_derive", "rxb200_fm_create", "rxb200_fm_destroy", "rxb200_fm_reset", "rxb200_fm_max_output",
     "rxb200_fm_process", "rxb200_fm_process_device", "rxb200_fm_process_read", "rxb200_fm_process_read_device",
     "rxb200_fm_squelch_hits", "rxb200_fm_levels", "rxb200_fm_stream",
-    "rxb200_fm_last_stats", "rxb200_fm_tune", "rxb200_fm_kernel_ms",
+    "rxb200_fm_last_stats", "rxb200_fm_tune", "rxb200_fm_kernel_ms", "rxb200_fm_disc_device",
     "rxb200_power_plan_range", "rxb200_window_table", "rxb200_sine_table", "rxb200_power_create",
     "rxb200_power_destroy", "rxb200_power_accumulate", "rxb200_power_accumulate_device", "rxb200_power_read",
     "rxb200_power_device_avg", "rxb200_power_reset", "rxb200_power_stream", "rxb200_power_last_launches",
@@ -124,6 +124,7 @@ def lib() -> C.CDLL:
     L.rxb200_fm_last_stats.argtypes = [C.c_void_p, C.POINTER(FmStatsC)]
     L.rxb200_fm_tune.argtypes = [C.c_void_p, C.c_int, C.c_int]
     L.rxb200_fm_kernel_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float)]
+    L.rxb200_fm_disc_device.argtypes = [C.c_int, C.c_void_p, sz, C.c_void_p, C.c_void_p]
     L.rxb200_power_kernel_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float)]
     L.rxb200_power_plan_range.argtypes = [C.c_int64, C.c_int64, C.c_int64, C.c_double, C.c_int, C.c_int, C.c_int,
                                           C.POINTER(PowerPlanC)]

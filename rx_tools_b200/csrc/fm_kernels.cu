@@ -448,7 +448,10 @@ __device__ __forceinline__ int disc_lut(const int *__restrict__ lut, int cr, int
 	}
 	int x = div_c((int)((unsigned)cj << 8), cr);
 	int xa = x < 0 ? neg_w(x) : x;
-	if (xa >= 131072 || xa < 0) { return cj > 0 ? (1 << 13) : -(1 << 13); }
+	// |x| >= 131072, and x = INT_MIN, whose xa wraps negative (cj = 2^23 mod 2^24 over |cr| = 1: the reference reads
+	// atan_lut[INT_MIN] or divides INT_MIN by -1 there; see RXB200_ATAN_LUT).  One unsigned compare: nvcc treats
+	// x < 0 ? -x : x as never negative and drops a separate signed xa < 0 test, and the table would be read at INT_MIN.
+	if ((unsigned)xa >= 131072u) { return cj > 0 ? (1 << 13) : -(1 << 13); }
 	if (x > 0) { return cj > 0 ? __ldg(lut + x) : __ldg(lut + x) - (1 << 14); }
 	return cj > 0 ? (1 << 14) - __ldg(lut + xa) : -__ldg(lut + xa);
 }
@@ -2210,6 +2213,45 @@ static fm_kernel_fn pick_any_kernel(int P, int spec)
 #endif
 }
 
+// ---- the discriminators alone (rxb200_fm_disc_device): element i is the quad (ar, aj, br, bj) = x[n], x[n-1], whose
+// conjugate product the chains form with the same wrapping expression; every form calls the very device function the
+// kernels above inline, so a test can hold each one to the reference at operands a chain only rarely reaches
+__global__ void fm_disc_kernel(int form, const int4 *__restrict__ quads, long long n, const int *__restrict__ lut,
+                               int32_t *__restrict__ out)
+{
+	for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+		const int4 q = quads[i];
+		const int ar = q.x, aj = q.y, br = q.z, bj = q.w;
+		const int cr = add_w(mul_w(ar, br), mul_w(aj, bj));
+		const int cj = sub_w(mul_w(aj, br), mul_w(ar, bj));
+		int r = 0;
+		switch (form) {
+		case RXB200_DISC_STD: r = disc_std_f32(cr, cj); break;
+		case RXB200_DISC_FAST: r = fast_atan2_i(cj, cr); break;
+		case RXB200_DISC_LUT: r = disc_lut(lut, cr, cj); break;
+		case RXB200_DISC_ALE: r = disc_ale(ar, aj, br, bj); break;
+		case RXB200_DISC_ATAN2: r = disc_std(cr, cj); break;
+		case RXB200_DISC_STD_FP64: r = disc_std_lean(cr, cj); break;
+		case RXB200_DISC_ROWS: {
+			uint32_t ab;
+			row_angles<1, false, true>(&cr, &cj, 0, &ab);
+			r = wrap16((int)ab);
+			break;
+		}
+		case RXB200_DISC_STREAM: {      // front_block's undecimated loop, one sample
+			const float fi = __int2float_rn(ar), fq = __int2float_rn(aj), fbr = __int2float_rn(br), fbj = __int2float_rn(bj);
+			const float fcr = __fmaf_rn(fi, fbr, __fmul_rn(fq, fbj));
+			const float fcj = __fmaf_rn(fq, fbr, -__fmul_rn(fi, fbj));
+			r = wrap16(__float_as_int(__fadd_rn(fast_atan2_f32(fcj, fcr), 12582912.0f)));
+			break;
+		}
+		case RXB200_DISC_AM: r = wrap16((int)sqrt((double)add_w(mul_w(ar, ar), mul_w(aj, aj)))); break;
+		default: break;
+		}
+		out[i] = r;
+	}
+}
+
 }  // namespace rxb
 
 // ================================================================================ host side
@@ -2229,6 +2271,14 @@ static const int k_droop9_host[11][10] = {
 	{9, -119, -577, 5917, -26067, 77473, -26067, 5917, -577, -119},
 	{9, -199, -362, 5303, -25505, 77489, -25505, 5303, -362, -199},
 };
+
+// atan_lut_init (src/rtl_fm.c:515-526): host libm; rxb200_fm_create uploads it once per -A lut handle
+static std::vector<int> atan_lut_host()
+{
+	std::vector<int> lut(131072);
+	for (int i = 0; i < 131072; i++) { lut[i] = (int)(atan((double)i / (double)(1 << 8)) / 3.14159 * (double)(1 << 14)); }
+	return lut;
+}
 
 struct rxb200_fm {
 	rxb200_fm_params p{};
@@ -2399,9 +2449,7 @@ extern "C" int rxb200_fm_create(const rxb200_fm_params *params, int device, int 
 	RXB_CUDA_OR(cudaMalloc(&h->d_carry[0], cbytes), rxb200_fm_destroy(h));
 	RXB_CUDA_OR(cudaMalloc(&h->d_carry[1], cbytes), rxb200_fm_destroy(h));
 	if (params->custom_atan == RXB200_ATAN_LUT && params->mode == RXB200_MODE_FM) {
-		// atan_lut_init (src/rtl_fm.c:515-526): host libm, uploaded once
-		std::vector<int> lut(131072);
-		for (int i = 0; i < 131072; i++) { lut[i] = (int)(atan((double)i / (double)(1 << 8)) / 3.14159 * (double)(1 << 14)); }
+		const std::vector<int> lut = atan_lut_host();
 		RXB_CUDA_OR(cudaMalloc(&h->d_atan_lut, lut.size() * sizeof(int)), rxb200_fm_destroy(h));
 		RXB_CUDA_OR(cudaMemcpy(h->d_atan_lut, lut.data(), lut.size() * sizeof(int), cudaMemcpyHostToDevice), rxb200_fm_destroy(h));
 	}
@@ -3119,6 +3167,32 @@ extern "C" int rxb200_fm_tune(rxb200_fm *h, int segment_len, int deemph_warmup)
 {
 	if (!h || segment_len < 0 || deemph_warmup < 0) { return RXB200_EINVAL; }
 	h->tune_seg = segment_len; h->tune_warm = deemph_warmup;
+	return RXB200_OK;
+}
+
+extern "C" int rxb200_fm_disc_device(int form, const int32_t *d_quads, size_t n, int32_t *d_out, void *stream)
+{
+	if (form < RXB200_DISC_STD || form > RXB200_DISC_AM) { set_error("unknown discriminator form %d", form); return RXB200_EINVAL; }
+	if (!d_quads || !d_out) { set_error("bad disc request (null pointer)"); return RXB200_EINVAL; }
+	if ((uintptr_t)d_quads & 15u) { set_error("quads must be 16-byte aligned"); return RXB200_EINVAL; }
+	if (n == 0) { return RXB200_OK; }
+	const cudaStream_t st = (cudaStream_t)stream;
+	int *d_lut = nullptr;
+	if (form == RXB200_DISC_LUT) {
+		const std::vector<int> lut = atan_lut_host();
+		RXB_CUDA(cudaMallocAsync((void **)&d_lut, lut.size() * sizeof(int), st));
+		// from pageable memory: the copy has read its source when it returns
+		if (cudaMemcpyAsync(d_lut, lut.data(), lut.size() * sizeof(int), cudaMemcpyHostToDevice, st) != cudaSuccess) {
+			set_error("lut upload failed: %s", cudaGetErrorString(cudaGetLastError()));
+			cudaFreeAsync(d_lut, st);
+			return RXB200_ECUDA;
+		}
+	}
+	const long long want = ((long long)n + 255) / 256, blocks = want < 8192 ? want : 8192;
+	fm_disc_kernel<<<(unsigned)blocks, 256, 0, st>>>(form, reinterpret_cast<const int4 *>(d_quads), (long long)n, d_lut, d_out);
+	const cudaError_t e = cudaGetLastError();
+	if (d_lut) { cudaFreeAsync(d_lut, st); }
+	if (e != cudaSuccess) { set_error("fm_disc_kernel launch failed: %s", cudaGetErrorString(e)); return RXB200_ECUDA; }
 	return RXB200_OK;
 }
 

@@ -17,6 +17,8 @@ from . import _lib
 
 MODE_FM, MODE_AM, MODE_USB, MODE_LSB, MODE_RAW = range(5)
 ATAN_STD, ATAN_FAST, ATAN_LUT, ATAN_ALE = range(4)
+# forms of disc_device (RXB200_DISC_*): the four discriminators, then the other device code a chain's samples run through
+DISC_STD, DISC_FAST, DISC_LUT, DISC_ALE, DISC_ATAN2, DISC_STD_FP64, DISC_ROWS, DISC_STREAM, DISC_AM = range(9)
 MAXIMUM_BUF_LENGTH = 262144          # src/rtl_fm.c:80-82
 
 
@@ -276,6 +278,16 @@ def ddc_device(capture_rate: int, offset_hz: int, phase: int, ddc, d_src_ptr: in
     d, _t = _ddc_c(ddc)
     _lib.check(_lib.lib().rxb200_ddc_device(capture_rate, offset_hz, phase, C.byref(d), d_src_ptr, n_complex, d_dst_ptr,
                                             stream or None))
+
+
+def disc_device(form: int, quads, stream: int = 0):
+    """One discriminator alone on the device (``rxb200_fm_disc_device``): quads is a contiguous int32 CUDA tensor
+    [n][4] of (ar, aj, br, bj); returns the int32 [n] results, a new tensor on the same device, written asynchronously
+    on ``stream``.  form: DISC_*."""
+    assert quads.dim() == 2 and quads.shape[1] == 4 and quads.is_contiguous() and quads.element_size() == 4
+    out = quads.new_empty((quads.shape[0],))
+    _lib.check(_lib.lib().rxb200_fm_disc_device(form, quads.data_ptr(), quads.shape[0], out.data_ptr(), stream or None))
+    return out
 
 
 class FmMix(_OneGpu):

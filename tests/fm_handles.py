@@ -10,6 +10,7 @@ import pytest
 
 import fm_any_chunk as fac
 import fm_ddc as fdd
+import fm_disc as fd
 import fm_mix as fmx
 import fm_read as frd
 from rx_tools_b200 import _lib, fm
@@ -54,14 +55,16 @@ def port_channels(port, p, rate, offs, x, lens16, ddc=None):
 
 
 def compare(p, got, want, what):
-    """PCM against the port: exact for the integer discriminators, else at most a few samples 1 LSB apart."""
+    """PCM against the port: exact, except that -A std may have a few samples 1 LSB apart when the port met a
+    polar_discriminant value within 2^-30 of an integer in the running test (fm_disc.port_met_near_integer)."""
     assert got.size == want.size, (what, got.size, want.size)
     diff = np.abs(got.astype(np.int32) - want.astype(np.int32))
-    if fac.INTEGER(p):
+    near = fd.port_met_near_integer()
+    if fac.INTEGER(p) or not near:
         bad = np.flatnonzero(diff)
         assert bad.size == 0, (what, bad[:5], got[bad[:5]], want[bad[:5]])
     else:
-        # fp64 atan2 on every sample (CUDA libm against glibc): a last-ulp difference may move a sample by 1 LSB
+        # the port met an fp64 atan2 value within 2^-30 of an integer: CUDA's libm may truncate it 1 LSB the other way
         assert np.count_nonzero(diff) <= max(2, int(1e-4 * diff.size)), (what, np.flatnonzero(diff)[:5])
         assert diff.max(initial=0) <= 1, what
 

@@ -38,6 +38,17 @@ def test_no_cpu_fallback_without_device():
     assert e.value.code == _lib.ENODEV
 
 
+def test_disc_device_refuses_before_any_device_work():
+    """rxb200_fm_disc_device checks its form and pointers before it touches a device (also where there is none)."""
+    L = _lib.lib()
+    for form in (-1, 9):
+        assert L.rxb200_fm_disc_device(form, None, 1, None, None) == _lib.EINVAL
+    assert L.rxb200_fm_disc_device(0, None, 1, None, None) == _lib.EINVAL
+    assert L.rxb200_fm_disc_device(0, 16, 1, None, None) == _lib.EINVAL
+    assert L.rxb200_fm_disc_device(0, 4, 1, 16, None) == _lib.EINVAL         # quads not 16-byte aligned
+    assert _lib.lib().rxb200_last_error()
+
+
 def test_product_never_imports_oracle():
     pkg = os.path.join(ROOT, "rx_tools_b200")
     for dirpath, _, files in os.walk(pkg):

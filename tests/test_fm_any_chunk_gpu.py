@@ -14,6 +14,7 @@ import numpy as np
 import pytest
 
 import fm_any_chunk as fac
+import fm_disc as fd
 import oracle
 from rx_tools_b200 import _lib, fm, synth
 
@@ -32,12 +33,13 @@ def _input(p, n_complex, seed):
 def _compare(p, got, want, what):
     assert got.size == want.size, (what, got.size, want.size)
     diff = np.abs(got.astype(np.int32) - want.astype(np.int32))
-    if fac.INTEGER(p):
+    near = fd.port_met_near_integer()
+    if fac.INTEGER(p) or not near:
         bad = np.flatnonzero(diff)
         assert bad.size == 0, (what, bad[:5], got[bad[:5]], want[bad[:5]])
     else:
-        # every sample through fp64 atan2 (CUDA libm vs glibc): a last-ulp difference may move an isolated sample by
-        # 1 LSB, and the serial stages after it may smear such a flip over a few outputs
+        # the port met a polar_discriminant value within 2^-30 of an integer, where CUDA's atan2 and glibc's may
+        # truncate differently: that sample may be 1 LSB off, and the serial stages after it may smear the flip
         assert np.count_nonzero(diff) <= max(2, int(1e-4 * diff.size)), (what, np.flatnonzero(diff)[:5])
         if not p.deemph and p.rate_out2 <= 0 and not p.dc_block_audio:
             assert diff.max(initial=0) <= 1, what

@@ -1,12 +1,15 @@
 """rx_fm parity: the CUDA path (through the C-ABI, host buffers) against the port oracle and the
 committed golden vectors.  Integer discriminators must be bit-exact; the atan2 path is compared
-with the tolerance north_star states (1e-5 relative -> at most 1 LSB on isolated samples)."""
+byte for byte too, unless the port met a value within 2^-30 of an integer (fm_disc.port_met_near_integer): only then
+may CUDA's atan2 truncate differently from glibc's, and the tolerance north_star states applies (1e-5 relative -> at
+most 1 LSB on isolated samples)."""
 import json
 import os
 
 import numpy as np
 import pytest
 
+import fm_disc as fd
 import oracle
 from cases import fm_cases, fm_optional_cases
 from rx_tools_b200 import _lib, fm
@@ -19,12 +22,13 @@ FM_GOLD = json.load(open(os.path.join(G, "fm_golden.json")))
 
 def _compare(case, got, want):
     assert got.size == want.size
-    if case.exact:
+    near = fd.port_met_near_integer()
+    if case.exact or not near:
         bad = np.flatnonzero(got != want)
         assert bad.size == 0, f"{bad.size} mismatches, first at {bad[:5]}: got {got[bad[:5]]} want {want[bad[:5]]}"
     else:
-        # fp64 atan2 on the GPU vs glibc: results are truncated to int, so a last-ulp difference can move
-        # an isolated sample by 1 LSB (north_star tolerance 1e-5 relative on the float path)
+        # the port met an fp64 atan2 value within 2^-30 of an integer: CUDA's libm and glibc's may truncate it
+        # differently, so an isolated sample may be 1 LSB off (north_star tolerance 1e-5 relative on the float path)
         d = np.abs(got.astype(np.int32) - want.astype(np.int32))
         assert d.max() <= 1, d.max()
         assert np.count_nonzero(d) <= max(1, int(1e-5 * d.size)), np.count_nonzero(d)

@@ -13,6 +13,7 @@ import numpy as np
 import pytest
 
 import fm_any_chunk as fac
+import fm_disc as fd
 import fm_read as frd
 import oracle
 from rx_tools_b200 import _lib, fm, synth
@@ -28,10 +29,11 @@ SHAPES = frd.shapes()
 def _compare(p, got, want, what):
     assert got.size == want.size, (what, got.size, want.size)
     diff = np.abs(got.astype(np.int32) - want.astype(np.int32))
-    if fac.INTEGER(p):
+    near = fd.port_met_near_integer()
+    if fac.INTEGER(p) or not near:
         bad = np.flatnonzero(diff)
         assert bad.size == 0, (what, bad[:5], got[bad[:5]], want[bad[:5]])
-    else:       # fp64 atan2 (CUDA libm vs glibc): a last-ulp difference may move an isolated sample by 1 LSB
+    else:       # the port met an atan2 value within 2^-30 of an integer: CUDA's libm may truncate it the other way
         assert np.count_nonzero(diff) <= max(2, int(1e-4 * diff.size)), (what, np.flatnonzero(diff)[:5])
 
 

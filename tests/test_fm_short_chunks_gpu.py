@@ -11,6 +11,7 @@ import pytest
 
 import fm_any_chunk as fac
 import fm_ddc as fdd
+import fm_disc as fd
 import fm_mix as fmx
 from rx_tools_b200 import fm
 
@@ -71,10 +72,11 @@ def _check(p, got, want, rl, what):
         keep[z] = False
         got, want = got[keep], want[keep]
     diff = np.abs(got.astype(np.int32) - want.astype(np.int32))
-    if fac.INTEGER(p):
+    near = fd.port_met_near_integer()
+    if fac.INTEGER(p) or not near:
         bad = np.flatnonzero(diff)
         assert bad.size == 0, (what, bad[:5], got[bad[:5]], want[bad[:5]])
-    else:
+    else:       # the port met an atan2 value within 2^-30 of an integer: CUDA's libm may truncate it the other way
         assert np.count_nonzero(diff) <= max(2, int(1e-4 * diff.size)), (what, np.flatnonzero(diff)[:5])
         if _zero_after_empty(p):
             assert diff.max(initial=0) <= 1, what

@@ -3,13 +3,16 @@ oracle/_ref produced for the exact inputs of tests/full_inputs.py (minted in the
 tests/golden/make_full_golden.py; the reference needs ~50 s for all of it).  The CUDA path runs the same inputs
 through the C-ABI and must reproduce the hashes: 1 GiB rx_fm streams (2 048 chunks, every per-chunk result_len),
 cfg1 at 2^20 samples (24 576 PCM), 256 channels x 2.4 M (cfg5A), 871 hops x 36 sweeps (every row + the CSV), 610
-hop buffers (cfg3).  The fp64 atan2 outputs are compared with the reference's vectors (<= 1 LSB on <= 1e-5)."""
+hop buffers (cfg3).  The fp64 atan2 outputs are compared with the reference's vectors byte for byte, unless the port, run
+over the same input, meets an atan2 value within 2^-30 of an integer (where CUDA's libm and glibc's may truncate
+differently): then <= 1 LSB on <= 1e-5 of the samples."""
 import json
 import os
 
 import numpy as np
 import pytest
 
+import fm_disc as fd
 import full_inputs as FI
 import oracle
 from cases import fm_cases
@@ -22,8 +25,13 @@ GOLD = json.load(open(os.path.join(G, "full_golden.json")))
 VEC = np.load(os.path.join(G, "full_std_vectors.npz"))
 
 
-def _close_to_reference(got, want):
+def _close_to_reference(got, want, params, x, chunk16):
     assert got.size == want.size
+    oracle.port().fm_run(params, x, chunk16)
+    if not fd.port_met_near_integer():
+        bad = np.flatnonzero(got != want)
+        assert bad.size == 0, (bad.size, bad[:5], got[bad[:5]], want[bad[:5]])
+        return
     d = np.abs(got.astype(np.int32) - want.astype(np.int32))
     assert d.max() <= 1, d.max()
     assert np.count_nonzero(d) <= max(1, int(1e-5 * d.size)), np.count_nonzero(d)
@@ -69,7 +77,7 @@ def test_cfg1_at_two_to_the_twenty(nm, atan):
     got = dem.full_demod(x, FI.CHUNK16)
     assert got.size == g["n_out"] == 24576                   # BASELINE.md §2: 2^20 samples -> exactly 24 576 PCM
     if atan == 0:
-        _close_to_reference(got, VEC["cfg1_std_full"])
+        _close_to_reference(got, VEC["cfg1_std_full"], oracle.FmParams(**p.reference_fields()), x, FI.CHUNK16)
     else:
         assert digest(got) == g["output_sha256"]
     dem.close()
@@ -79,8 +87,9 @@ def test_cfg1_at_two_to_the_twenty(nm, atan):
 def test_atan2_cases_against_reference_vectors(case):
     """The float path against what the reference itself produced (not only the port)."""
     dem = fm.FmDemod(case.params)
-    got = dem.full_demod(case.make_input(), case.chunk_int16)
-    _close_to_reference(got, VEC["case_" + case.name])
+    x = case.make_input()
+    got = dem.full_demod(x, case.chunk_int16)
+    _close_to_reference(got, VEC["case_" + case.name], case.params, x, case.chunk_int16)
     dem.close()
 
 

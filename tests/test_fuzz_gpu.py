@@ -1,9 +1,11 @@
 """Randomised parity: random demod_state configurations, chunk lengths, stream lengths (ragged last chunk), call
 splits and input statistics (loud, quiet, silent stretches) — CUDA path vs the port oracle, bit-exact (integer
-discriminators) or within 1 LSB on isolated samples (atan2)."""
+discriminators, and atan2 unless the port met a value within 2^-30 of an integer) or within 1 LSB on isolated samples
+(atan2 when it did)."""
 import numpy as np
 import pytest
 
+import fm_disc as fd
 import oracle
 from rx_tools_b200 import _lib, fm
 
@@ -116,15 +118,14 @@ def test_random_configuration(seed, port):
         raise
     assert got.size == want.size, (pd, chunk_c, n_c)
     diff = np.abs(got.astype(np.int32) - want.astype(np.int32))
-    if params.mode == 0 and params.custom_atan == 0:
-        # every sample through fp64 atan2 (CUDA libm vs glibc): results are truncated to int, a last-ulp difference
-        # may move an isolated sample by 1 LSB (north_star: 1e-5 relative on the float path); downstream IIR /
-        # resampler stages can smear such a flip over a few outputs
+    if params.mode == 0 and params.custom_atan == 0 and fd.port_met_near_integer():
+        # the port met an fp64 atan2 value within 2^-30 of an integer, where CUDA's libm and glibc's may truncate
+        # differently: that sample may be 1 LSB off, and downstream IIR / resampler stages can smear the flip
         assert np.count_nonzero(diff) <= max(2, int(1e-4 * diff.size)), (pd, np.flatnonzero(diff)[:5])
         if not params.deemph and params.rate_out2 <= 0 and not params.dc_block_audio:
             assert diff.max(initial=0) <= 1
     else:
-        # integer paths (only the first FM sample of a chunk uses atan2): bit-exact
+        # integer paths, and -A std wherever no atan2 value came near an integer: bit-exact
         bad = np.flatnonzero(diff)
         assert bad.size == 0, (pd, chunk_c, n_c, bad[:5], got[bad[:5]], want[bad[:5]])
     if params.squelch_level:
