@@ -46,6 +46,21 @@ int ddc_check(const rxb200_ddc *ddc, bool *wide);
 		}                                                                                \
 	} while (0)
 
+// grows a device buffer to at least `need` elements (the contents are not kept)
+template <typename T>
+cudaError_t reserve(T *&buf, size_t &cap, size_t need)
+{
+	if (need <= cap) { return cudaSuccess; }
+	cudaFree(buf); buf = nullptr; cap = 0;
+	const cudaError_t e = cudaMalloc(&buf, need * sizeof(T));
+	if (e == cudaSuccess) { cap = need; }
+	return e;
+}
+
+// fm_kernels.cu: the droop-compensation FIR rows for 0..10 downsampling passes (cic_9_tables, src/rtl_fm.c:287-300;
+// rtl_power.c has the same table), {taps, c1..c9} x 2^15.  The rows are symmetric, so the kernels take the first six.
+extern const int k_droop9_host[11][10];
+
 // ---- two's-complement helpers: the reference relies on x86 wrap-around for int overflow and
 // on truncating stores to int16_t (SURVEY.md §7 hard part 5); unsigned arithmetic makes the
 // wrap well-defined here.

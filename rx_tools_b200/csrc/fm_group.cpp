@@ -8,6 +8,7 @@
 #include <vector>
 #include "common.cuh"
 
+using rxb::reserve;
 using rxb::set_error;
 
 namespace {
@@ -39,16 +40,6 @@ struct DeviceGuard {
 	DeviceGuard() { if (cudaGetDevice(&dev) != cudaSuccess) { cudaGetLastError(); dev = -1; } }
 	~DeviceGuard() { if (dev >= 0) { cudaSetDevice(dev); } }
 };
-
-// grows a member's staging buffer to at least `need` int16 (the contents are not kept)
-cudaError_t reserve(int16_t *&buf, size_t &cap, size_t need)
-{
-	if (need <= cap) { return cudaSuccess; }
-	cudaFree(buf); buf = nullptr; cap = 0;
-	const cudaError_t e = cudaMalloc(&buf, need * sizeof(int16_t));
-	if (e == cudaSuccess) { cap = need; }
-	return e;
-}
 
 template <typename G>
 void group_destroy(G *g)

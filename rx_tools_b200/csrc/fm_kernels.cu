@@ -2257,7 +2257,7 @@ __global__ void fm_disc_kernel(int form, const int4 *__restrict__ quads, long lo
 // ================================================================================ host side
 using namespace rxb;
 
-static const int k_droop9_host[11][10] = {
+const int rxb::k_droop9_host[11][10] = {
 	// droop-compensation FIR rows (cic_9_tables, src/rtl_fm.c:287-300): {taps, c1..c9} x 2^15
 	{0, 0, 0, 0, 0, 0, 0, 0, 0, 0},
 	{9, -156,  -97, 2798, -15489, 61019, -15489, 2798,  -97, -156},
@@ -2592,17 +2592,6 @@ static int fm_route(const rxb200_fm *h, size_t n_int16, size_t chunk_int16, bool
 
 static long long round_up_ll(long long v, long long g) { return ((v + g - 1) / g) * g; }
 
-// grows a device scratch buffer of the handle to at least `need` elements (the contents are not kept)
-template <typename T>
-static cudaError_t fm_reserve(T *&buf, size_t &cap, size_t need)
-{
-	if (need <= cap) { return cudaSuccess; }
-	cudaFree(buf); buf = nullptr; cap = 0;
-	const cudaError_t e = cudaMalloc(&buf, need * sizeof(T));
-	if (e == cudaSuccess) { cap = need; }
-	return e;
-}
-
 // Back-end replay in decimated samples: the de-emphasis bracket in front of a piece, 0 without de-emphasis.  The bracket
 // closes in two phases: the gap contracts by (1 - 1/a) per step (to 1 within ~11 a steps from the full int16 range), then
 // the two trajectories sit one apart until a sample lands on the one residue mod a that merges them -- a geometric wait
@@ -2889,12 +2878,12 @@ static int fm_prepasses(rxb200_fm *h, FmCall &k, size_t n_int16, size_t chunk_in
 	const FmDev &dv = h->dev;
 	const int n_chunks = k.n_chunks;
 	const size_t cells = (size_t)n_chunks * h->n_channels;
-	RXB_CUDA(fm_reserve(h->d_sums, h->sums_cap, cells * 2));
-	RXB_CUDA(fm_reserve(h->d_rdc, h->rdc_cap, cells * 2));
-	RXB_CUDA(fm_reserve(h->d_sqz, h->sqz_cap, cells));
-	RXB_CUDA(fm_reserve(h->d_adc, h->adc_cap, cells));
-	RXB_CUDA(fm_reserve(h->d_levels, h->levels_cap, cells));
-	RXB_CUDA(fm_reserve(h->d_lens, h->lens_cap, (size_t)n_chunks * 4));
+	RXB_CUDA(reserve(h->d_sums, h->sums_cap, cells * 2));
+	RXB_CUDA(reserve(h->d_rdc, h->rdc_cap, cells * 2));
+	RXB_CUDA(reserve(h->d_sqz, h->sqz_cap, cells));
+	RXB_CUDA(reserve(h->d_adc, h->adc_cap, cells));
+	RXB_CUDA(reserve(h->d_levels, h->levels_cap, cells));
+	RXB_CUDA(reserve(h->d_lens, h->lens_cap, (size_t)n_chunks * 4));
 	RXB_CUDA(cudaStreamSynchronize(h->stream));   // the previous call may still be reading the host vector
 	if (const int rc = fm_chunk_table(h, n_int16, chunk_int16, h->h_lens); rc != RXB200_OK) { return rc; }
 	RXB_CUDA(cudaMemcpyAsync(h->d_lens, h->h_lens.data(), h->h_lens.size() * sizeof(int), cudaMemcpyHostToDevice, h->stream));
@@ -2968,13 +2957,13 @@ static int fm_launch(rxb200_fm *h, const int16_t *d_in, size_t n_int16, size_t c
 	if (stream) {
 		rc = fm_plan_back(h, n, &b);
 		if (rc != RXB200_OK) { return rc; }
-		RXB_CUDA(fm_reserve(h->d_pcm, h->d_pcm_cap, (size_t)b.pstride * h->n_channels));
+		RXB_CUDA(reserve(h->d_pcm, h->d_pcm_cap, (size_t)b.pstride * h->n_channels));
 	}
 	const size_t total_back = (size_t)b.n_cta * h->n_channels;
 	const size_t need_sync = 4 + 4 * (total_work > total_back ? total_work : total_back);
-	RXB_CUDA(fm_reserve(h->d_sync, h->sync_cap, need_sync));
+	RXB_CUDA(reserve(h->d_sync, h->sync_cap, need_sync));
 	if (rows) {
-		RXB_CUDA(fm_reserve(h->d_margin, h->margin_cap, total_work * (size_t)k.n_extra * (size_t)(ROW_LEN >> dv.P)));
+		RXB_CUDA(reserve(h->d_margin, h->margin_cap, total_work * (size_t)k.n_extra * (size_t)(ROW_LEN >> dv.P)));
 		k.margin = h->d_margin;
 	}
 	// the fields every kernel of the call shares; the stream path's front kernel writes the PCM scratch
@@ -3082,8 +3071,8 @@ static int fm_process_host(rxb200_fm *h, const int16_t *cs16, size_t n_int16, si
 	if (rc != RXB200_OK || n_int16 == 0) { return rc; }
 	const size_t in_elems = n_int16 * (size_t)h->n_channels;
 	const size_t out_elems = (total + 8) * (size_t)h->n_channels;
-	RXB_CUDA(fm_reserve(h->d_in, h->d_in_cap, in_elems));
-	RXB_CUDA(fm_reserve(h->d_out, h->d_out_cap, out_elems));
+	RXB_CUDA(reserve(h->d_in, h->d_in_cap, in_elems));
+	RXB_CUDA(reserve(h->d_out, h->d_out_cap, out_elems));
 	RXB_CUDA(cudaMemcpyAsync(h->d_in, cs16, in_elems * sizeof(int16_t), cudaMemcpyHostToDevice, h->stream));
 	rc = fm_launch(h, h->d_in, n_int16, chunk_int16, h->d_out, total + 8, any);
 	if (rc != RXB200_OK) { return rc; }

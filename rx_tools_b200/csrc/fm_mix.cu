@@ -337,16 +337,6 @@ struct rxb200_fm_mix {
 
 namespace {
 
-template <typename T>
-cudaError_t reserve(T *&buf, size_t &cap, size_t need)
-{
-	if (need <= cap) { return cudaSuccess; }
-	cudaFree(buf); buf = nullptr; cap = 0;
-	const cudaError_t e = cudaMalloc(&buf, need * sizeof(T));
-	if (e == cudaSuccess) { cap = need; }
-	return e;
-}
-
 // int16 a decimating handle hands the chain from a call of n_int16 capture int16 after pos capture samples: the
 // outputs whose emission point m*M + M - 1 falls in the call
 size_t ddc_len(unsigned long long pos, size_t n_int16, int decim)

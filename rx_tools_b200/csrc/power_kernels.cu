@@ -62,29 +62,8 @@ __device__ __forceinline__ long long block_sum(long long v, long long *red, int 
 	return t;
 }
 
-// ---- small-span decimators, in place on the shared hop buffer (rare path: only when the planner
-// chose downsample > 1).  Every output depends only on ORIGINAL samples at higher (or equal) positions
-// than where it is stored, so each is done in rounds of "all threads read, barrier, all threads write".
-
-// boxcar (src/rtl_power.c:723-733): slot k = int16-wrapped sum of samples [k*ds, (k+1)*ds); the
-// sources are zeroed, so everything past the last slot is zero.
-__device__ void pw_boxcar(uint32_t *buf, int ncomplex, int ds, int tid, int T)
-{
-	const int nslots = (ncomplex + ds - 1) / ds;
-	for (int base = 0; base < nslots; base += T) {
-		const int k = base + tid;
-		int si = 0, sq = 0;
-		if (k < nslots) {
-			int e = (k + 1) * ds < ncomplex ? (k + 1) * ds : ncomplex;
-			for (int i = k * ds; i < e; i++) { uint32_t w = buf[i]; si += plo(w); sq += phi(w); }
-		}
-		__syncthreads();
-		if (k < nslots) { buf[k] = ppack(si, sq); }
-		__syncthreads();
-	}
-	for (int i = nslots + tid; i < ncomplex; i += T) { buf[i] = 0u; }
-	__syncthreads();
-}
+// ---- the reference's steps, one sample, bin or butterfly at a time.  The shared-memory kernel below and the
+// global-memory kernels of large hop buffers both call these; a buffer is packed I/Q words in either memory.
 
 // one component (sel 0 = I, 1 = Q) of sample i
 __device__ __forceinline__ int pw_get(const uint32_t *buf, int i, int sel) { return sel ? phi(buf[i]) : plo(buf[i]); }
@@ -94,41 +73,128 @@ __device__ __forceinline__ void pw_put(uint32_t *buf, int i, int sel, int v)
 	h[sel] = (uint16_t)v;
 }
 
-// stateless fifth_order with its "ease-in" head (src/rtl_power.c:582-607) on one component.
-// `length` is the reference's argument (an int16 span); outputs k = 0 .. while 4k < length.
+// boxcar slot k (src/rtl_power.c:723-733): the int16-wrapped sums of samples [k*ds, (k+1)*ds) of the first n
+__device__ __forceinline__ uint32_t boxcar_slot(const uint32_t *x, int k, int ds, int n)
+{
+	const int e = (k + 1) * ds < n ? (k + 1) * ds : n;
+	int si = 0, sq = 0;
+	for (int i = k * ds; i < e; i++) { const uint32_t w = x[i]; si += plo(w); sq += phi(w); }
+	return ppack(si, sq);
+}
+
+__device__ __forceinline__ int hb_taps(int a, int b, int c, int d, int e, int f) { return (a + (b + e) * 5 + (c + d) * 10 + f) >> 4; }
+
+// fifth_order output k with its "ease-in" head (src/rtl_power.c:582-607) of one component from the level window x,
+// which starts at level index lo
+__device__ __forceinline__ int hb_out(const uint32_t *x, int lo, int k, int sel)
+{
+	const uint32_t *w = x - lo;             // w[i] = level sample i
+	if (k < 3) {
+		const int a = pw_get(w, 0, sel), b = pw_get(w, 1, sel), c = pw_get(w, 2, sel);
+		const int d = pw_get(w, 3, sel), e = pw_get(w, 4, sel), f = pw_get(w, 5, sel);
+		if (k == 0) { return ((a + b) * 10 + (c + d) * 5 + d + f) >> 4; }
+		if (k == 1) { return ((b + c) * 10 + (a + d) * 5 + e + f) >> 4; }
+		return hb_taps(a, b, c, d, e, f);
+	}
+	if (k == 3) { return hb_taps(pw_get(w, 2, sel), pw_get(w, 3, sel), pw_get(w, 4, sel), pw_get(w, 5, sel), pw_get(w, 5, sel), pw_get(w, 6, sel)); }
+	if (k == 4) { return hb_taps(pw_get(w, 4, sel), pw_get(w, 5, sel), pw_get(w, 5, sel), pw_get(w, 6, sel), pw_get(w, 7, sel), pw_get(w, 8, sel)); }
+	const int i = 2 * k - 5;
+	return hb_taps(pw_get(w, i, sel), pw_get(w, i + 1, sel), pw_get(w, i + 2, sel), pw_get(w, i + 3, sel), pw_get(w, i + 4, sel), pw_get(w, i + 5, sel));
+}
+
+// generic_fir (src/rtl_power.c:626-654) output d >= 9 of one component: the 9-tap sum over ORIGINAL samples
+// d-9 .. d-1 of the window x, which starts at index lo
+__device__ __forceinline__ int fir_out(const uint32_t *x, int lo, int d, int sel, const int *c)
+{
+	const uint32_t *w = x - lo;
+	int acc = mul_w(pw_get(w, d - 9, sel) + pw_get(w, d - 1, sel), c[1]);
+	acc = add_w(acc, mul_w(pw_get(w, d - 8, sel) + pw_get(w, d - 2, sel), c[2]));
+	acc = add_w(acc, mul_w(pw_get(w, d - 7, sel) + pw_get(w, d - 3, sel), c[3]));
+	acc = add_w(acc, mul_w(pw_get(w, d - 6, sel) + pw_get(w, d - 4, sel), c[4]));
+	acc = add_w(acc, mul_w(pw_get(w, d - 5, sel), c[5]));
+	return acc >> 15;
+}
+
+// remove_dc (src/rtl_power.c:609-624, :744-745) over the first `used` int16: I is summed over samples < n_i and
+// divided by used, Q over samples < n_q and divided by used - 1
+struct Dc { int n_i, n_q, ave_i, ave_q; };
+__device__ __forceinline__ Dc dc_average(long long si, long long sq, int used)
+{
+	return {(used + 1) / 2, used / 2, (int)(int16_t)(si / (long long)used), (int)(int16_t)(sq / (long long)(used - 1))};
+}
+
+// window multiply of sample g (word u) with int16 wrap (:749-758)
+__device__ __forceinline__ uint32_t dc_window(uint32_t u, int g, const Dc &dc, int w)
+{
+	return ppack((plo(u) - (g < dc.n_i ? dc.ave_i : 0)) * w, (phi(u) - (g < dc.n_q ? dc.ave_q : 0)) * w);
+}
+
+// butterfly t of radix-2 DIT stage s on the N-block x, every stage halves (:291-318)
+__device__ __forceinline__ void dit_bfly(uint32_t *x, int t, int s, int bin_e, const int16_t *sine)
+{
+	const int N = 1 << bin_e;
+	const int l = 1 << s, k = bin_e - 1 - s;
+	const int m = t & (l - 1);
+	const int i = ((t >> s) << (s + 1)) + m, j = i + l;
+	const int jt = m << k;
+	const int wr = (int)sine[jt + N / 4] >> 1;
+	const int wi = neg_half(sine[jt]);
+	const uint32_t u = x[i], v = x[j];
+	const int vr = plo(v), vi = phi(v);
+	const int tr = q15(wr, vr) - q15(wi, vi);
+	const int ti = q15(wr, vi) + q15(wi, vr);
+	const int qr = plo(u) >> 1, qi = phi(u) >> 1;
+	x[j] = ppack(qr - tr, qi - ti);
+	x[i] = ppack(qr + tr, qi + ti);
+}
+
+// real_conj (:664-668) of one bin, its sum or peak hold (:760-768), and the flush of a partial result to avg
+__device__ __forceinline__ long long bin_power(uint32_t w)
+{
+	const int re = plo(w), im = phi(w);
+	return (long long)(re * re) + (long long)(im * im);
+}
+__device__ __forceinline__ void fold(long long &acc, long long v, int peak_hold) { if (peak_hold) { acc = v > acc ? v : acc; } else { acc += v; } }
+__device__ __forceinline__ void flush(long long *dst, long long v, int peak_hold)
+{
+	if (peak_hold) { atomicMax(dst, v); } else { atomicAdd(reinterpret_cast<unsigned long long *>(dst), (unsigned long long)v); }
+}
+
+// ---- small-span decimators, in place on the shared hop buffer (rare path: only when the planner
+// chose downsample > 1).  Every output depends only on ORIGINAL samples at higher (or equal) positions
+// than where it is stored, so each is done in rounds of "all threads read, barrier, all threads write".
+
+// boxcar: slot k replaces sample k; the sources are zeroed, so everything past the last slot is zero.
+__device__ void pw_boxcar(uint32_t *buf, int ncomplex, int ds, int tid, int T)
+{
+	const int nslots = (ncomplex + ds - 1) / ds;
+	for (int base = 0; base < nslots; base += T) {
+		const int k = base + tid;
+		const uint32_t y = k < nslots ? boxcar_slot(buf, k, ds, ncomplex) : 0u;
+		__syncthreads();
+		if (k < nslots) { buf[k] = y; }
+		__syncthreads();
+	}
+	for (int i = nslots + tid; i < ncomplex; i += T) { buf[i] = 0u; }
+	__syncthreads();
+}
+
+// stateless fifth_order on one component.  `length` is the reference's argument (an int16 span); outputs
+// k = 0 .. while 4k < length.
 __device__ void pw_halfband(uint32_t *buf, int length, int sel, int tid, int T)
 {
 	const int nout = (length + 3) / 4 > 3 ? (length + 3) / 4 : 3;
 	for (int base = 0; base < nout; base += T) {
 		const int k = base + tid;
-		int y = 0;
-		if (k < nout) {
-			if (k < 3) {
-				int a = pw_get(buf, 0, sel), b = pw_get(buf, 1, sel), c = pw_get(buf, 2, sel);
-				int d = pw_get(buf, 3, sel), e = pw_get(buf, 4, sel), f = pw_get(buf, 5, sel);
-				if (k == 0) { y = ((a + b) * 10 + (c + d) * 5 + d + f) >> 4; }
-				else if (k == 1) { y = ((b + c) * 10 + (a + d) * 5 + e + f) >> 4; }
-				else { y = (a + (b + e) * 5 + (c + d) * 10 + f) >> 4; }
-			} else {
-				// k = 3: (x2,x3,x4,x5,x5,x6); k = 4: (x4,x5,x5,x6,x7,x8); k >= 5: x[2k-5 .. 2k]
-				int i0, i1, i2, i3, i4, i5;
-				if (k == 3) { i0 = 2; i1 = 3; i2 = 4; i3 = 5; i4 = 5; i5 = 6; }
-				else if (k == 4) { i0 = 4; i1 = 5; i2 = 5; i3 = 6; i4 = 7; i5 = 8; }
-				else { i0 = 2 * k - 5; i1 = i0 + 1; i2 = i0 + 2; i3 = i0 + 3; i4 = i0 + 4; i5 = i0 + 5; }
-				int a = pw_get(buf, i0, sel), b = pw_get(buf, i1, sel), c = pw_get(buf, i2, sel);
-				int d = pw_get(buf, i3, sel), e = pw_get(buf, i4, sel), f = pw_get(buf, i5, sel);
-				y = (a + (b + e) * 5 + (c + d) * 10 + f) >> 4;
-			}
-		}
+		const int y = k < nout ? hb_out(buf, 0, k, sel) : 0;
 		__syncthreads();
 		if (k < nout) { pw_put(buf, k, sel, y); }
 		__syncthreads();
 	}
 }
 
-// stateless generic_fir (src/rtl_power.c:626-654) on one component: samples 0..8 pass through, sample
-// d >= 9 becomes the 9-tap sum over ORIGINAL samples d-9 .. d-1.  Done from the top down so that a
-// round's stores never touch what a later round still has to read.
+// stateless generic_fir on one component: samples 0..8 pass through.  Done from the top down so that a round's
+// stores never touch what a later round still has to read.
 __device__ void pw_droop9(uint32_t *buf, int length, int sel, const int *c, int tid, int T)
 {
 	const int ncomp = (length + 1) / 2;           // samples d with 2d < length
@@ -136,19 +202,7 @@ __device__ void pw_droop9(uint32_t *buf, int length, int sel, const int *c, int 
 	const int nfil = ncomp - 9;
 	for (int top = nfil; top > 0; top -= T) {
 		const int j = top - 1 - tid;              // filtered index within [0, nfil)
-		int y = 0;
-		if (j >= 0) {
-			const int d = j + 9;
-			int h0 = pw_get(buf, d - 9, sel), h1 = pw_get(buf, d - 8, sel), h2 = pw_get(buf, d - 7, sel);
-			int h3 = pw_get(buf, d - 6, sel), h4 = pw_get(buf, d - 5, sel), h5 = pw_get(buf, d - 4, sel);
-			int h6 = pw_get(buf, d - 3, sel), h7 = pw_get(buf, d - 2, sel), h8 = pw_get(buf, d - 1, sel);
-			int acc = mul_w(h0 + h8, c[1]);
-			acc = add_w(acc, mul_w(h1 + h7, c[2]));
-			acc = add_w(acc, mul_w(h2 + h6, c[3]));
-			acc = add_w(acc, mul_w(h3 + h5, c[4]));
-			acc = add_w(acc, mul_w(h4, c[5]));
-			y = acc >> 15;
-		}
+		const int y = j >= 0 ? fir_out(buf, 0, j + 9, sel, c) : 0;
 		__syncthreads();
 		if (j >= 0) { pw_put(buf, j + 9, sel, y); }
 		__syncthreads();
@@ -211,74 +265,34 @@ __global__ void __launch_bounds__(256) power_fft_kernel(const PowArgs a)
 				}
 			}
 		}
-		// remove_dc: sum of one component divided by the int16 span (src/rtl_power.c:609-624)
 		long long si = 0, sq = 0;
 		for (int i = tid; i < n_i; i += T) { uint32_t w = buf[i]; si += plo(w); if (i < n_q) { sq += phi(w); } }
-		si = block_sum(si, red, tid, T);
-		sq = block_sum(sq, red, tid, T);
-		const int ave_i = (int)(int16_t)(si / (long long)used);
-		const int ave_q = (int)(int16_t)(sq / (long long)(used - 1));
+		const Dc dc = dc_average(block_sum(si, red, tid, T), block_sum(sq, red, tid, T), used);
 		for (int blk = 0; blk < nblk; blk++) {
 			uint32_t *x = buf + (size_t)blk * N;
-			// window (x - ave) * w with int16 wrap (:749-758) fused with the bit-reversal swap (:275-290)
+			// window multiply fused with the bit-reversal swap (:275-290)
 			for (int i = tid; i < N; i += T) {
-				int r = (int)(__brev((unsigned)i) >> (32 - a.bin_e));
-				// remove_dc only touched the first n_i / n_q samples of the buffer
-				const int gi = blk * N + i, gr = blk * N + r;
-				if (i < r) {
-					uint32_t u = x[i], v = x[r];
-					int wi_ = win[i], wr_ = win[r];
-					x[r] = ppack((plo(u) - (gi < n_i ? ave_i : 0)) * wi_, (phi(u) - (gi < n_q ? ave_q : 0)) * wi_);
-					x[i] = ppack((plo(v) - (gr < n_i ? ave_i : 0)) * wr_, (phi(v) - (gr < n_q ? ave_q : 0)) * wr_);
-				} else if (i == r) {
-					uint32_t u = x[i];
-					int wi_ = win[i];
-					x[i] = ppack((plo(u) - (gi < n_i ? ave_i : 0)) * wi_, (phi(u) - (gi < n_q ? ave_q : 0)) * wi_);
+				const int r = (int)(__brev((unsigned)i) >> (32 - a.bin_e));
+				if (i <= r) {
+					const uint32_t u = dc_window(x[i], blk * N + i, dc, win[i]), v = dc_window(x[r], blk * N + r, dc, win[r]);
+					x[r] = u;
+					x[i] = v;
 				}
 			}
 			__syncthreads();
-			// radix-2 DIT stages, every stage halves (:291-318)
 			for (int s = 0; s < a.bin_e; s++) {
-				const int l = 1 << s;
-				const int k = a.bin_e - 1 - s;
-				for (int t = tid; t < N / 2; t += T) {
-					int m = t & (l - 1);
-					int i = ((t >> s) << (s + 1)) + m;
-					int j = i + l;
-					int jt = m << k;
-					int wr = (int)sine[jt + N / 4] >> 1;
-					int wi = neg_half(sine[jt]);
-					uint32_t u = x[i], v = x[j];
-					int vr = plo(v), vi = phi(v);
-					int tr = q15(wr, vr) - q15(wi, vi);
-					int ti = q15(wr, vi) + q15(wi, vr);
-					int qr = plo(u) >> 1, qi = phi(u) >> 1;
-					x[j] = ppack(qr - tr, qi - ti);
-					x[i] = ppack(qr + tr, qi + ti);
-				}
+				for (int t = tid; t < N / 2; t += T) { dit_bfly(x, t, s, a.bin_e, sine); }
 				__syncthreads();
 			}
-			// real_conj accumulate (:664-668, :760-768)
 			if (NB > 0) {
 #pragma unroll
 				for (int b = 0; b < (NB > 0 ? NB : 1); b++) {
-					int j = tid + b * T;
-					if (j < N) {
-						uint32_t w = x[j];
-						int re = plo(w), im = phi(w);
-						long long pw = (long long)(re * re) + (long long)(im * im);
-						if (a.peak_hold) { acc[b] = pw > acc[b] ? pw : acc[b]; } else { acc[b] += pw; }
-					}
+					const int j = tid + b * T;
+					if (j < N) { fold(acc[b], bin_power(x[j]), a.peak_hold); }
 				}
 			} else {
 				long long *row = a.avg + (size_t)hop * N;
-				for (int j = tid; j < N; j += T) {
-					uint32_t w = x[j];
-					int re = plo(w), im = phi(w);
-					long long pw = (long long)(re * re) + (long long)(im * im);
-					if (a.peak_hold) { atomicMax(row + j, pw); }
-					else { atomicAdd(reinterpret_cast<unsigned long long *>(row + j), (unsigned long long)pw); }
-				}
+				for (int j = tid; j < N; j += T) { flush(row + j, bin_power(x[j]), a.peak_hold); }
 			}
 		}
 		__syncthreads();       // everyone done with buf before the next TMA overwrites it
@@ -287,11 +301,8 @@ __global__ void __launch_bounds__(256) power_fft_kernel(const PowArgs a)
 		long long *row = a.avg + (size_t)hop * N;
 #pragma unroll
 		for (int b = 0; b < (NB > 0 ? NB : 1); b++) {
-			int j = tid + b * T;
-			if (j < N) {
-				if (a.peak_hold) { atomicMax(row + j, acc[b]); }
-				else { atomicAdd(reinterpret_cast<unsigned long long *>(row + j), (unsigned long long)acc[b]); }
-			}
+			const int j = tid + b * T;
+			if (j < N) { flush(row + j, acc[b], a.peak_hold); }
 		}
 	}
 }
@@ -582,13 +593,10 @@ __global__ void __launch_bounds__(256) power_rms_kernel(const PowArgs a)
 			double e2 = __dmul_rn(__dmul_rn(dc, dc), (double)a.buf_len);
 			double err = __dsub_rn(e1, e2);
 			p -= (long long)round(err);
-			if (a.peak_hold) { acc = p > acc ? p : acc; } else { acc += p; }
+			fold(acc, p, a.peak_hold);
 		}
 	}
-	if (tid == 0) {
-		if (a.peak_hold) { atomicMax(a.avg + hop, acc); }
-		else { atomicAdd(reinterpret_cast<unsigned long long *>(a.avg + hop), (unsigned long long)acc); }
-	}
+	if (tid == 0) { flush(a.avg + hop, acc, a.peak_hold); }
 }
 
 
@@ -600,7 +608,7 @@ __global__ void __launch_bounds__(256) power_rms_kernel(const PowArgs a)
 //   big_window: (x - ave) * w with int16 wrap (:749-758), stored bit-reversed (fix_fft's swap pass, :275-290)
 //   big_stage:  one radix-2 stage over every N-block (:291-318)
 //   big_accum:  real_conj accumulate / peak hold (:760-768)
-__global__ void __launch_bounds__(256) power_big_load(const int16_t *src, uint32_t *work, int n_complex, int ds, int used_int16,
+__global__ void __launch_bounds__(256) power_big_load(const uint32_t *src, uint32_t *work, int n_complex, int ds, int used_int16,
                                                       long long *sums)
 {
 	const int n_out = (n_complex + ds - 1) / ds;
@@ -608,13 +616,10 @@ __global__ void __launch_bounds__(256) power_big_load(const int16_t *src, uint32
 	const int n_i = (used_int16 + 1) / 2, n_q = used_int16 / 2;
 	long long si = 0, sq = 0;
 	for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < n_out; k += gridDim.x * blockDim.x) {
-		int a = 0, b = 0;
-		const int e = (k + 1) * ds < n_complex ? (k + 1) * ds : n_complex;
-		for (int i = k * ds; i < e; i++) { a += src[2 * i]; b += src[2 * i + 1]; }
-		a = (int)(int16_t)a; b = (int)(int16_t)b;                 // the in-place int16 "+=" of the reference wraps
-		work[k] = ppack(a, b);
-		if (k < n_i) { si += a; }
-		if (k < n_q) { sq += b; }
+		const uint32_t v = boxcar_slot(src, k, ds, n_complex);
+		work[k] = v;
+		if (k < n_i) { si += plo(v); }
+		if (k < n_q) { sq += phi(v); }
 	}
 	for (int o = 16; o > 0; o >>= 1) { si += __shfl_down_sync(0xffffffffu, si, o); sq += __shfl_down_sync(0xffffffffu, sq, o); }
 	if ((threadIdx.x & 31) == 0) {
@@ -647,37 +652,6 @@ __host__ __device__ __forceinline__ void decim_window(int m0, int m1, int P, int
 	}
 	lo[0] &= ~3;                            // whole 16-byte words of the hop buffer
 	hi[0] |= 3;
-}
-
-__device__ __forceinline__ int hb_taps(int a, int b, int c, int d, int e, int f) { return (a + (b + e) * 5 + (c + d) * 10 + f) >> 4; }
-
-// fifth_order output k of one component (sel 0 = I, 1 = Q) from the level window x, which starts at level index lo
-__device__ __forceinline__ int hb_out(const uint32_t *x, int lo, int k, int sel)
-{
-	const uint32_t *w = x - lo;             // w[i] = level sample i
-	if (k < 3) {
-		const int a = pw_get(w, 0, sel), b = pw_get(w, 1, sel), c = pw_get(w, 2, sel);
-		const int d = pw_get(w, 3, sel), e = pw_get(w, 4, sel), f = pw_get(w, 5, sel);
-		if (k == 0) { return ((a + b) * 10 + (c + d) * 5 + d + f) >> 4; }
-		if (k == 1) { return ((b + c) * 10 + (a + d) * 5 + e + f) >> 4; }
-		return hb_taps(a, b, c, d, e, f);
-	}
-	if (k == 3) { return hb_taps(pw_get(w, 2, sel), pw_get(w, 3, sel), pw_get(w, 4, sel), pw_get(w, 5, sel), pw_get(w, 5, sel), pw_get(w, 6, sel)); }
-	if (k == 4) { return hb_taps(pw_get(w, 4, sel), pw_get(w, 5, sel), pw_get(w, 5, sel), pw_get(w, 6, sel), pw_get(w, 7, sel), pw_get(w, 8, sel)); }
-	const int i = 2 * k - 5;
-	return hb_taps(pw_get(w, i, sel), pw_get(w, i + 1, sel), pw_get(w, i + 2, sel), pw_get(w, i + 3, sel), pw_get(w, i + 4, sel), pw_get(w, i + 5, sel));
-}
-
-// generic_fir output d >= 9 of one component: the 9-tap sum over ORIGINAL samples d-9 .. d-1, wrapping as pw_droop9
-__device__ __forceinline__ int fir_out(const uint32_t *x, int lo, int d, int sel, const int *c)
-{
-	const uint32_t *w = x - lo;
-	int acc = mul_w(pw_get(w, d - 9, sel) + pw_get(w, d - 1, sel), c[1]);
-	acc = add_w(acc, mul_w(pw_get(w, d - 8, sel) + pw_get(w, d - 2, sel), c[2]));
-	acc = add_w(acc, mul_w(pw_get(w, d - 7, sel) + pw_get(w, d - 3, sel), c[3]));
-	acc = add_w(acc, mul_w(pw_get(w, d - 6, sel) + pw_get(w, d - 4, sel), c[4]));
-	acc = add_w(acc, mul_w(pw_get(w, d - 5, sel), c[5]));
-	return acc >> 15;
 }
 
 struct DecimFir { int c[6]; };
@@ -743,41 +717,24 @@ __global__ void __launch_bounds__(256) power_big_window(const uint32_t *work, ui
                                                         int used_int16, int n_slots, int bin_e, int nblk)
 {
 	const int N = 1 << bin_e;
-	const int n_i = (used_int16 + 1) / 2, n_q = used_int16 / 2;
-	const int ave_i = (int)(int16_t)(sums[0] / (long long)used_int16);
-	const int ave_q = (int)(int16_t)(sums[1] / (long long)(used_int16 - 1));
+	const Dc dc = dc_average(sums[0], sums[1], used_int16);
 	const long long total = (long long)nblk * N;
 	for (long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x; g < total; g += (long long)gridDim.x * blockDim.x) {
 		const int i = (int)(g & (N - 1));
 		const long long base = g - i;
 		const int r = (int)(__brev((unsigned)i) >> (32 - bin_e));
 		// past the decimated span the reference transforms what the boxcar left there: a partial last slot, then zeros
-		const uint32_t u = g < n_slots ? work[g] : 0u;
-		const int w = win[i];
-		fft[base + r] = ppack((plo(u) - (g < n_i ? ave_i : 0)) * w, (phi(u) - (g < n_q ? ave_q : 0)) * w);
+		fft[base + r] = dc_window(g < n_slots ? work[g] : 0u, (int)g, dc, win[i]);
 	}
 }
 
 __global__ void __launch_bounds__(256) power_big_stage(uint32_t *fft, const int16_t *sine, int bin_e, int s, int nblk)
 {
 	const int N = 1 << bin_e;
-	const int l = 1 << s, k = bin_e - 1 - s;
 	const long long total = (long long)nblk * (N / 2);
 	for (long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x; g < total; g += (long long)gridDim.x * blockDim.x) {
 		const int t = (int)(g & (N / 2 - 1));
-		uint32_t *x = fft + (g - t) * 2;
-		const int m = t & (l - 1);
-		const int i = ((t >> s) << (s + 1)) + m, j = i + l;
-		const int jt = m << k;
-		const int wr = (int)sine[jt + N / 4] >> 1;
-		const int wi = neg_half(sine[jt]);
-		const uint32_t u = x[i], v = x[j];
-		const int vr = plo(v), vi = phi(v);
-		const int tr = q15(wr, vr) - q15(wi, vi);
-		const int ti = q15(wr, vi) + q15(wi, vr);
-		const int qr = plo(u) >> 1, qi = phi(u) >> 1;
-		x[j] = ppack(qr - tr, qi - ti);
-		x[i] = ppack(qr + tr, qi + ti);
+		dit_bfly(fft + (g - t) * 2, t, s, bin_e, sine);
 	}
 }
 
@@ -786,12 +743,7 @@ __global__ void __launch_bounds__(256) power_big_accum(const uint32_t *fft, long
 	const int N = 1 << bin_e;
 	for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < N; j += gridDim.x * blockDim.x) {
 		long long acc = row[j];
-		for (int b = 0; b < nblk; b++) {
-			const uint32_t w = fft[(size_t)b * N + j];
-			const int re = plo(w), im = phi(w);
-			const long long pw = (long long)(re * re) + (long long)(im * im);
-			if (peak_hold) { acc = pw > acc ? pw : acc; } else { acc += pw; }
-		}
+		for (int b = 0; b < nblk; b++) { fold(acc, bin_power(fft[(size_t)b * N + j]), peak_hold); }
 		row[j] = acc;
 	}
 }
@@ -799,14 +751,6 @@ __global__ void __launch_bounds__(256) power_big_accum(const uint32_t *fft, long
 }  // namespace rxb
 
 using namespace rxb;
-
-// cic_9_tables (src/rtl_power.c: same table as rtl_fm.c:287-300), first six entries of each row
-static const int k_cic9_power[11][6] = {
-	{0, 0, 0, 0, 0, 0}, {9, -156, -97, 2798, -15489, 61019}, {9, -128, -568, 5593, -24125, 74126},
-	{9, -129, -639, 6187, -26281, 77511}, {9, -122, -612, 6082, -26353, 77818}, {9, -120, -602, 6015, -26269, 77757},
-	{9, -120, -582, 5951, -26128, 77542}, {9, -119, -580, 5931, -26094, 77505}, {9, -119, -578, 5921, -26077, 77484},
-	{9, -119, -577, 5917, -26067, 77473}, {9, -199, -362, 5303, -25505, 77489},
-};
 
 #define RXB_ROW_PAD 16        // >= the largest communicator size - 1
 struct rxb200_power {
@@ -819,17 +763,21 @@ struct rxb200_power {
 	int16_t *d_sine, *d_window;
 	int16_t *d_in; size_t d_in_cap;
 	std::vector<int> samples;  // tunes[i].samples mirror (deterministic, kept on the host)
-	int launches;
 	int n_sm;
 	cudaEvent_t ev0, ev1;
-	void *d_db = nullptr; size_t db_cap = 0;   // csv_dbm staging (rxb200_power_read_db)
+	unsigned char *d_db = nullptr; size_t db_cap = 0;   // csv_dbm staging (rxb200_power_read_db)
 	int triv = 0;                              // see PowArgs::triv
 	uint32_t *d_work = nullptr, *d_fft = nullptr; long long *d_sums = nullptr;   // global-memory path (hop buffer beyond shared memory)
-	int decim_tile = 0; size_t decim_smem = 0;                                   // power_big_decim's tile (final samples) and shared memory
 	int force_v1 = 0;                          // RXB200_POWER_V1 (A/B knob, read once at create): generic kernel only
 	int fft8_threads = 0;                      // RXB200_POWER_THREADS = 512 | 1024 (A/B knob): CTA width of the fast path
 	rxb200_power_path path = {};               // what the last accumulate ran (rxb200_power_last_path)
 };
+
+#define RXB_SMEM_MAX (227 * 1024)          // dynamic shared memory a CTA may opt in to on sm_90
+
+// power_fft_kernel's shared memory without its tables: the mbarrier, the reduction scratch and the hop buffer.  A hop
+// buffer for which this exceeds RXB_SMEM_MAX runs on the global-memory kernels.
+static size_t hop_smem(int buf_len) { return 16 + 256 + (size_t)buf_len * 2; }
 
 static int power_validate(const rxb200_power_params *p)
 {
@@ -841,12 +789,11 @@ static int power_validate(const rxb200_power_params *p)
 			set_error("bad downsample %d / passes %d", p->downsample, p->downsample_passes);
 			return RXB200_EINVAL;
 		}
-		long long need = 16 + 256 + (long long)p->buf_len * 2;     // tables move to global memory when they do not fit
 		if ((long long)(2 << p->bin_e) * p->downsample > p->buf_len) {
 			set_error("bin_e %d x downsample %d needs more than buf_len %d", p->bin_e, p->downsample, p->buf_len);
 			return RXB200_EINVAL;
 		}
-		if (need > 227 * 1024 && p->downsample > 1 && !p->boxcar &&
+		if (hop_smem(p->buf_len) > RXB_SMEM_MAX && p->downsample > 1 && !p->boxcar &&
 		    (p->downsample_passes < 1 || p->downsample != (1 << p->downsample_passes) ||
 		     p->buf_len % ((2LL << p->bin_e) * p->downsample) != 0)) {
 			// power_big_decim assumes the planner's geometry (src/rtl_power.c:466-474, :504-507): downsample = 2^passes and
@@ -884,7 +831,7 @@ extern "C" int rxb200_power_create(const rxb200_power_params *params, const int 
 	rxb200_power *h = new (std::nothrow) rxb200_power();
 	if (!h) { return RXB200_ENOMEM; }
 	h->p = *params; h->device = device; h->d_avg = nullptr; h->d_samples = nullptr; h->d_sine = nullptr; h->d_window = nullptr;
-	h->d_in = nullptr; h->d_in_cap = 0; h->launches = 0;
+	h->d_in = nullptr; h->d_in_cap = 0;
 	h->samples.assign(params->n_hops, 0);
 	h->force_v1 = getenv("RXB200_POWER_V1") ? 1 : 0;
 	h->fft8_threads = getenv("RXB200_POWER_THREADS") ? atoi(getenv("RXB200_POWER_THREADS")) : 0;
@@ -938,12 +885,23 @@ extern "C" int rxb200_power_kernel_ms(rxb200_power *h, float *ms)
 }
 
 template <int NB>
-static cudaError_t launch_fft(const PowArgs &a, int blocks, size_t smem, cudaStream_t st)
+static cudaError_t launch_fft_nb(const PowArgs &a, int blocks, size_t smem, cudaStream_t st)
 {
 	cudaError_t e = cudaFuncSetAttribute(power_fft_kernel<NB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
 	if (e != cudaSuccess) { return e; }
 	power_fft_kernel<NB><<<blocks, 256, smem, st>>>(a);
 	return cudaGetLastError();
+}
+static cudaError_t launch_fft(int nb, const PowArgs &a, int blocks, size_t smem, cudaStream_t st)
+{
+	switch (nb) {
+	case 1: return launch_fft_nb<1>(a, blocks, smem, st);
+	case 2: return launch_fft_nb<2>(a, blocks, smem, st);
+	case 4: return launch_fft_nb<4>(a, blocks, smem, st);
+	case 8: return launch_fft_nb<8>(a, blocks, smem, st);
+	case 16: return launch_fft_nb<16>(a, blocks, smem, st);
+	default: return launch_fft_nb<0>(a, blocks, smem, st);
+	}
 }
 
 template <int E, int T>
@@ -983,7 +941,7 @@ static int decim_span_max(int n_final, int tile, int P, int fir_on)
 }
 static void decim_plan(int n_final, int P, int fir_on, int n_sm, int *tile, size_t *smem)
 {
-	const int cap = (227 * 1024 - RXB_DECIM_DATA) / 4;                  // level-0 complex samples a CTA can stage
+	const int cap = (RXB_SMEM_MAX - RXB_DECIM_DATA) / 4;                 // level-0 complex samples a CTA can stage
 	const int halo = 5 + 9 * fir_on;
 	int t = (n_final + 4 * n_sm - 1) / (4 * n_sm);
 	if (t < 4 * halo) { t = 4 * halo; }
@@ -995,6 +953,76 @@ static void decim_plan(int n_final, int P, int fir_on, int n_sm, int *tile, size
 	*smem = RXB_DECIM_DATA + (size_t)decim_span_max(n_final, t, P, fir_on) * 4;
 }
 
+// droop compensation after the -F passes (src/rtl_power.c:739-742)
+static int fir_on(const rxb200_power_params &p) { return (p.comp_fir_size == 9 && p.downsample_passes >= 1 && p.downsample_passes <= 10) ? 1 : 0; }
+
+// One accumulate call's launch
+struct PowerPlan {
+	rxb200_power_path path;   // what rxb200_power_last_path reports; PowArgs takes its slices and tables_in_smem
+	int blocks;               // CTAs of the kernel that reads the hop buffers (the global-memory path: big_load or big_decim)
+	size_t smem;              // its dynamic shared memory
+	int tile;                 // power_big_decim: final samples per CTA
+	int nblk, n_slots;        // bin_e > 0: N-blocks per hop buffer (:747), complex samples after decimation
+	int samples;              // added to every hop's `samples` per pass (:428, :769)
+};
+
+static void power_plan(const rxb200_power *h, int n_pass, int nh, PowerPlan *pl)
+{
+	const rxb200_power_params &p = h->p;
+	*pl = {};
+	// enough CTAs for ~4 per SM, never more slices than passes
+	int slices = (h->n_sm * 4 + nh - 1) / nh;
+	if (slices > n_pass) { slices = n_pass; }
+	if (slices < 1) { slices = 1; }
+	pl->blocks = nh * slices;
+	if (p.bin_e == 0) {
+		pl->path = {RXB200_POWER_PATH_RMS, 0, 256, -1, 0, slices, 1};
+		pl->samples = 1;
+		return;
+	}
+	const int N = 1 << p.bin_e;
+	pl->nblk = (p.buf_len / p.downsample + 2 * N - 1) / (2 * N);      // over the int16 span after decimation (:744-747)
+	pl->n_slots = (p.buf_len / 2 + p.downsample - 1) / p.downsample;  // -F: exactly half that span
+	pl->samples = pl->nblk * p.downsample;
+	if (hop_smem(p.buf_len) > RXB_SMEM_MAX) {
+		// -F passes only when the plan decimates: downsample == 1 keeps the plain copy, as the shared-memory kernel does
+		const bool decim = !p.boxcar && p.downsample > 1 && p.downsample_passes > 0;
+		pl->path = {decim ? RXB200_POWER_PATH_BIG_DECIM : RXB200_POWER_PATH_BIG_LOAD, p.bin_e, 256, -1, 0, 0, n_pass * nh * (3 + p.bin_e)};
+		pl->blocks = h->n_sm * 8;
+		if (decim) {
+			decim_plan(pl->n_slots, p.downsample_passes, fir_on(p), h->n_sm, &pl->tile, &pl->smem);
+			pl->blocks = (pl->n_slots + pl->tile - 1) / pl->tile;
+		}
+		return;
+	}
+	if (p.downsample == 1 && p.buf_len == 16384 && p.bin_e >= 3 && p.bin_e <= 13 && !h->force_v1) {
+		// one CTA per (hop, pass-slice); 1024 threads: ~1 CTA per SM resident, 512 threads: 2
+		const int threads = fft8_threads(p.bin_e, h->fft8_threads);
+		// slices of the passes per hop: the launch takes ceil(nh*sl / resident CTAs) rounds of ceil(n_pass / sl) hop
+		// buffers each -- pick the split with the fewest buffer-times (a sharded rank owns few hops: 109 of 871 at
+		// eight GPUs, where "about one CTA per slot" left 31 CTAs for a second round of 12 buffers each)
+		const long long slots = (long long)h->n_sm * (1024 / threads);
+		int sl = 1;
+		long long best = -1;
+		for (int c = 1; c <= n_pass && (long long)c <= 2 * slots; c++) {
+			// + 1: a CTA's fixed cost (tables, accumulator flush) is about one hop buffer's worth of work
+			const long long rounds = ((long long)nh * c + slots - 1) / slots;
+			const long long t = rounds * ((n_pass + c - 1) / c + 1) * 4096 + c;   // ties: fewer slices (fewer atomic flushes)
+			if (best < 0 || t < best) { best = t; sl = c; }
+		}
+		pl->path = {RXB200_POWER_PATH_FFT8, p.bin_e, threads, -1, 1, sl, 1};
+		pl->blocks = nh * sl;
+		pl->smem = 16 + 512 + 2 * (8192 + 1024) * 4 + (size_t)(N / 2 > 4 ? N / 2 : 4) * 4 + (size_t)N * 2;
+		return;
+	}
+	// the sine and window tables go to shared memory when they fit beside the hop buffer
+	const size_t with_tables = hop_smem(p.buf_len) + (size_t)((N * 3 / 4 + 7) & ~7) * 2 + (size_t)N * 2;
+	const int in_smem = with_tables <= RXB_SMEM_MAX ? 1 : 0;
+	const int nb = N / 256;
+	pl->path = {RXB200_POWER_PATH_GENERIC, p.bin_e, 256, nb <= 1 ? 1 : (nb <= 16 ? nb : 0), in_smem, slices, 1};
+	pl->smem = in_smem ? with_tables : hop_smem(p.buf_len);
+}
+
 extern "C" int rxb200_power_accumulate_device(rxb200_power *h, const int16_t *d_hop_bufs, int n_pass,
                                               int hop_begin, int hop_end, int sync)
 {
@@ -1003,116 +1031,67 @@ extern "C" int rxb200_power_accumulate_device(rxb200_power *h, const int16_t *d_
 	if (((uintptr_t)d_hop_bufs & 15u) != 0) { set_error("hop buffers must be 16-byte aligned"); return RXB200_EINVAL; }
 	if (n_pass == 0) { return RXB200_OK; }
 	RXB_CUDA(cudaSetDevice(h->device));
+	const rxb200_power_params &p = h->p;
 	const int nh = hop_end - hop_begin;
+	PowerPlan pl;
+	power_plan(h, n_pass, nh, &pl);
+	const bool big = pl.path.kernel == RXB200_POWER_PATH_BIG_LOAD || pl.path.kernel == RXB200_POWER_PATH_BIG_DECIM;
+	if (big && !h->d_work) {
+		RXB_CUDA(cudaMalloc(&h->d_work, (size_t)pl.n_slots * sizeof(uint32_t)));
+		RXB_CUDA(cudaMalloc(&h->d_fft, (size_t)pl.nblk * ((size_t)1 << p.bin_e) * sizeof(uint32_t)));
+		RXB_CUDA(cudaMalloc(&h->d_sums, 2 * sizeof(long long)));
+	}
 	PowArgs a;
 	a.bufs = d_hop_bufs; a.avg = h->d_avg; a.sine = h->d_sine; a.window = h->d_window;
-	a.n_pass = n_pass; a.n_hops_call = nh; a.hop_begin = hop_begin; a.buf_len = h->p.buf_len;
-	a.bin_e = h->p.bin_e; a.peak_hold = h->p.peak_hold; a.triv = h->triv;
-	a.ds = h->p.downsample; a.ds_passes = h->p.downsample_passes; a.boxcar = h->p.boxcar;
-	a.fir_on = (h->p.comp_fir_size == 9 && h->p.downsample_passes >= 1 && h->p.downsample_passes <= 10) ? 1 : 0;
-	for (int j = 0; j < 6; j++) { a.fir[j] = k_cic9_power[h->p.downsample_passes <= 10 ? h->p.downsample_passes : 0][j]; }
-	// enough CTAs for ~4 per SM, never more slices than passes
-	int slices = (h->n_sm * 4 + nh - 1) / nh;
-	if (slices > n_pass) { slices = n_pass; }
-	if (slices < 1) { slices = 1; }
-	a.slices = slices;
-	const int blocks = nh * slices;
-	rxb200_power_path path = {RXB200_POWER_PATH_RMS, h->p.bin_e, 256, -1, 0, slices, 1};
+	a.n_pass = n_pass; a.n_hops_call = nh; a.hop_begin = hop_begin; a.buf_len = p.buf_len;
+	a.bin_e = p.bin_e; a.peak_hold = p.peak_hold; a.triv = h->triv;
+	a.ds = p.downsample; a.ds_passes = p.downsample_passes; a.boxcar = p.boxcar;
+	a.fir_on = fir_on(p);
+	for (int j = 0; j < 6; j++) { a.fir[j] = k_droop9_host[p.downsample_passes <= 10 ? p.downsample_passes : 0][j]; }
+	a.slices = pl.path.slices; a.tables_in_smem = pl.path.tables_in_smem;
+
 	RXB_CUDA(cudaEventRecord(h->ev0, h->stream));
-	if (h->p.bin_e == 0) {
-		power_rms_kernel<<<blocks, 256, 0, h->stream>>>(a);
-		RXB_CUDA(cudaGetLastError());
-		for (int i = hop_begin; i < hop_end; i++) { h->samples[i] += n_pass; }                      // :428
-	} else {
-		const int N = 1 << h->p.bin_e;
-		if (16 + 256 + (size_t)h->p.buf_len * 2 > 227 * 1024) {
-			// ---- hop buffer beyond shared memory: the reference's loop step by step on a global work buffer
-			const int n_complex = h->p.buf_len / 2, ds = h->p.downsample;
-			const int used = h->p.buf_len / ds;                         // int16 span after decimation (:744-747)
-			const int nblk = (used + 2 * N - 1) / (2 * N);
-			const int n_slots = (n_complex + ds - 1) / ds;              // decimated complex samples (-F: exactly used / 2)
-			// -F passes only when the plan decimates: downsample == 1 keeps the plain copy, as the shared-memory kernel does
-			const bool decim = !h->p.boxcar && ds > 1 && h->p.downsample_passes > 0;
-			const int P = h->p.downsample_passes;
-			if (!h->d_work) {
-				RXB_CUDA(cudaMalloc(&h->d_work, (size_t)n_slots * sizeof(uint32_t)));
-				RXB_CUDA(cudaMalloc(&h->d_fft, (size_t)nblk * N * sizeof(uint32_t)));
-				RXB_CUDA(cudaMalloc(&h->d_sums, 2 * sizeof(long long)));
-				if (decim) { decim_plan(n_slots, P, a.fir_on, h->n_sm, &h->decim_tile, &h->decim_smem); }
-			}
-			if (decim) {
-				// the attribute belongs to the kernel, not to this handle: allow the largest span any handle may plan
-				RXB_CUDA(cudaFuncSetAttribute(power_big_decim, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-			}
-			DecimFir fir;
-			for (int j = 0; j < 6; j++) { fir.c[j] = a.fir[j]; }
-			const int g = h->n_sm * 8;
-			for (int pass = 0; pass < n_pass; pass++) {
-				for (int hl = 0; hl < nh; hl++) {
-					const int16_t *src = d_hop_bufs + ((size_t)pass * nh + hl) * (size_t)h->p.buf_len;
-					RXB_CUDA(cudaMemsetAsync(h->d_sums, 0, 2 * sizeof(long long), h->stream));
-					if (decim) {
-						power_big_decim<<<(n_slots + h->decim_tile - 1) / h->decim_tile, 256, h->decim_smem, h->stream>>>(
-							src, h->d_work, n_slots, h->decim_tile, P, a.fir_on, fir, h->d_sums);
-					} else {
-						power_big_load<<<g, 256, 0, h->stream>>>(src, h->d_work, n_complex, ds, used, h->d_sums);
-					}
-					power_big_window<<<g, 256, 0, h->stream>>>(h->d_work, h->d_fft, h->d_window, h->d_sums, used, n_slots, h->p.bin_e, nblk);
-					for (int st = 0; st < h->p.bin_e; st++) { power_big_stage<<<g, 256, 0, h->stream>>>(h->d_fft, h->d_sine, h->p.bin_e, st, nblk); }
-					power_big_accum<<<g, 256, 0, h->stream>>>(h->d_fft, h->d_avg + (size_t)(hop_begin + hl) * N, h->p.bin_e, nblk, h->p.peak_hold);
-					RXB_CUDA(cudaGetLastError());
+	cudaError_t e = cudaSuccess;
+	switch (pl.path.kernel) {
+	case RXB200_POWER_PATH_RMS:
+		power_rms_kernel<<<pl.blocks, 256, 0, h->stream>>>(a);
+		e = cudaGetLastError();
+		break;
+	case RXB200_POWER_PATH_FFT8: e = launch_fft8(p.bin_e, pl.path.threads, a, pl.blocks, pl.smem, h->stream); break;
+	case RXB200_POWER_PATH_GENERIC: e = launch_fft(pl.path.nb, a, pl.blocks, pl.smem, h->stream); break;
+	default: {
+		// the reference's loop step by step on the global work buffers, one hop buffer at a time
+		const bool decim = pl.path.kernel == RXB200_POWER_PATH_BIG_DECIM;
+		if (decim) {
+			// the attribute belongs to the kernel, not to this handle: allow the largest span any handle may plan
+			RXB_CUDA(cudaFuncSetAttribute(power_big_decim, cudaFuncAttributeMaxDynamicSharedMemorySize, RXB_SMEM_MAX));
+		}
+		DecimFir fir;
+		for (int j = 0; j < 6; j++) { fir.c[j] = a.fir[j]; }
+		const int g = h->n_sm * 8, used = p.buf_len / p.downsample, N = 1 << p.bin_e;
+		for (int pass = 0; pass < n_pass; pass++) {
+			for (int hl = 0; hl < nh; hl++) {
+				const int16_t *src = d_hop_bufs + ((size_t)pass * nh + hl) * (size_t)p.buf_len;
+				RXB_CUDA(cudaMemsetAsync(h->d_sums, 0, 2 * sizeof(long long), h->stream));
+				if (decim) {
+					power_big_decim<<<pl.blocks, 256, pl.smem, h->stream>>>(src, h->d_work, pl.n_slots, pl.tile, p.downsample_passes,
+					                                                         a.fir_on, fir, h->d_sums);
+				} else {
+					power_big_load<<<pl.blocks, 256, 0, h->stream>>>(reinterpret_cast<const uint32_t *>(src), h->d_work, p.buf_len / 2,
+					                                                 p.downsample, used, h->d_sums);
 				}
+				power_big_window<<<g, 256, 0, h->stream>>>(h->d_work, h->d_fft, h->d_window, h->d_sums, used, pl.n_slots, p.bin_e, pl.nblk);
+				for (int st = 0; st < p.bin_e; st++) { power_big_stage<<<g, 256, 0, h->stream>>>(h->d_fft, h->d_sine, p.bin_e, st, pl.nblk); }
+				power_big_accum<<<g, 256, 0, h->stream>>>(h->d_fft, h->d_avg + (size_t)(hop_begin + hl) * N, p.bin_e, pl.nblk, p.peak_hold);
+				RXB_CUDA(cudaGetLastError());
 			}
-			for (int i = hop_begin; i < hop_end; i++) { h->samples[i] += n_pass * nblk * ds; }           // :769
-			RXB_CUDA(cudaEventRecord(h->ev1, h->stream));
-			h->launches = n_pass * nh * (3 + h->p.bin_e);
-			h->path = {decim ? RXB200_POWER_PATH_BIG_DECIM : RXB200_POWER_PATH_BIG_LOAD, h->p.bin_e, 256, -1, 0, 0, h->launches};
-			if (sync) { RXB_CUDA(cudaStreamSynchronize(h->stream)); }
-			return RXB200_OK;
 		}
-		size_t smem = 16 + 256 + (size_t)h->p.buf_len * 2 + (size_t)((N * 3 / 4 + 7) & ~7) * 2 + (size_t)N * 2;
-		a.tables_in_smem = 1;
-		if (smem > 227 * 1024) { smem = 16 + 256 + (size_t)h->p.buf_len * 2; a.tables_in_smem = 0; }
-		cudaError_t e;
-		const bool fast = (h->p.downsample == 1 && h->p.buf_len == 16384 && h->p.bin_e >= 3 && h->p.bin_e <= 13 && !h->force_v1);
-		if (fast) {
-			// one CTA per (hop, pass-slice); 1024 threads: ~1 CTA per SM resident, 512 threads: 2
-			const int threads = fft8_threads(h->p.bin_e, h->fft8_threads);
-			// slices of the passes per hop: the launch takes ceil(nh*sl / resident CTAs) rounds of ceil(n_pass / sl) hop
-			// buffers each -- pick the split with the fewest buffer-times (a sharded rank owns few hops: 109 of 871 at
-			// eight GPUs, where "about one CTA per slot" left 31 CTAs for a second round of 12 buffers each)
-			const long long slots = (long long)h->n_sm * (1024 / threads);
-			int sl = 1;
-			long long best = -1;
-			for (int c = 1; c <= n_pass && (long long)c <= 2 * slots; c++) {
-				// + 1: a CTA's fixed cost (tables, accumulator flush) is about one hop buffer's worth of work
-				const long long rounds = ((long long)nh * c + slots - 1) / slots;
-				const long long t = rounds * ((n_pass + c - 1) / c + 1) * 4096 + c;   // ties: fewer slices (fewer atomic flushes)
-				if (best < 0 || t < best) { best = t; sl = c; }
-			}
-			a.slices = sl;
-			const size_t sm8 = 16 + 512 + 2 * (8192 + 1024) * 4 + (size_t)(N / 2 > 4 ? N / 2 : 4) * 4 + (size_t)N * 2;
-			e = launch_fft8(h->p.bin_e, threads, a, nh * sl, sm8, h->stream);
-			if (e != cudaSuccess) { set_error("power_fft8_kernel launch: %s", cudaGetErrorString(e)); return RXB200_ECUDA; }
-			path = {RXB200_POWER_PATH_FFT8, h->p.bin_e, threads, -1, 1, sl, 1};
-		} else {
-		const int nb = N / 256;
-		path = {RXB200_POWER_PATH_GENERIC, h->p.bin_e, 256, nb <= 1 ? 1 : (nb <= 16 ? nb : 0), a.tables_in_smem, slices, 1};
-		if (nb <= 1) { e = launch_fft<1>(a, blocks, smem, h->stream); }
-		else if (nb == 2) { e = launch_fft<2>(a, blocks, smem, h->stream); }
-		else if (nb == 4) { e = launch_fft<4>(a, blocks, smem, h->stream); }
-		else if (nb == 8) { e = launch_fft<8>(a, blocks, smem, h->stream); }
-		else if (nb == 16) { e = launch_fft<16>(a, blocks, smem, h->stream); }
-		else { e = launch_fft<0>(a, blocks, smem, h->stream); }
-		if (e != cudaSuccess) { set_error("power_fft_kernel launch: %s", cudaGetErrorString(e)); return RXB200_ECUDA; }
-		}
-		const int used_len = h->p.buf_len / h->p.downsample;
-		const int per_buf = (used_len + 2 * N - 1) / (2 * N);
-		for (int i = hop_begin; i < hop_end; i++) { h->samples[i] += n_pass * per_buf * h->p.downsample; }   // :769
 	}
+	}
+	if (e != cudaSuccess) { set_error("rx_power launch (path %d): %s", pl.path.kernel, cudaGetErrorString(e)); return RXB200_ECUDA; }
+	for (int i = hop_begin; i < hop_end; i++) { h->samples[i] += n_pass * pl.samples; }
 	RXB_CUDA(cudaEventRecord(h->ev1, h->stream));
-	h->launches = 1;
-	h->path = path;
+	h->path = pl.path;
 	if (sync) { RXB_CUDA(cudaStreamSynchronize(h->stream)); }
 	return RXB200_OK;
 }
@@ -1124,11 +1103,7 @@ extern "C" int rxb200_power_accumulate(rxb200_power *h, const int16_t *hop_bufs,
 	RXB_CUDA(cudaSetDevice(h->device));
 	size_t elems = (size_t)n_pass * (size_t)(hop_end - hop_begin) * (size_t)h->p.buf_len;
 	if (elems == 0) { return RXB200_OK; }
-	if (elems > h->d_in_cap) {
-		cudaFree(h->d_in); h->d_in = nullptr; h->d_in_cap = 0;
-		RXB_CUDA(cudaMalloc(&h->d_in, elems * sizeof(int16_t)));
-		h->d_in_cap = elems;
-	}
+	RXB_CUDA(reserve(h->d_in, h->d_in_cap, elems));
 	RXB_CUDA(cudaMemcpyAsync(h->d_in, hop_bufs, elems * sizeof(int16_t), cudaMemcpyHostToDevice, h->stream));
 	return rxb200_power_accumulate_device(h, h->d_in, n_pass, hop_begin, hop_end, 1);
 }
@@ -1184,11 +1159,7 @@ extern "C" int rxb200_power_read_db(rxb200_power *h, int rate, double crop, doub
 	RXB_CUDA(cudaSetDevice(h->device));
 	const int n_hops = h->p.n_hops;
 	const size_t need = (size_t)n_hops * row_len * sizeof(double) + (size_t)n_hops * sizeof(int);
-	if (need > h->db_cap) {
-		cudaFree(h->d_db); h->d_db = nullptr; h->db_cap = 0;
-		RXB_CUDA(cudaMalloc(&h->d_db, need));
-		h->db_cap = need;
-	}
+	RXB_CUDA(reserve(h->d_db, h->db_cap, need));
 	double *d_db = reinterpret_cast<double *>(h->d_db);
 	int *d_smp = reinterpret_cast<int *>(d_db + (size_t)n_hops * row_len);
 	RXB_CUDA(cudaMemcpyAsync(d_smp, h->samples.data(), (size_t)n_hops * sizeof(int), cudaMemcpyHostToDevice, h->stream));
@@ -1217,7 +1188,7 @@ extern "C" int rxb200_power_reset(rxb200_power *h)
 }
 
 extern "C" void *rxb200_power_stream(rxb200_power *h) { return h ? (void *)h->stream : nullptr; }
-extern "C" int rxb200_power_last_launches(rxb200_power *h) { return h ? h->launches : 0; }
+extern "C" int rxb200_power_last_launches(rxb200_power *h) { return h ? h->path.launches : 0; }
 extern "C" int rxb200_power_last_path(rxb200_power *h, rxb200_power_path *out)
 {
 	if (!h || !out) { set_error("null argument"); return RXB200_EINVAL; }
@@ -1424,11 +1395,7 @@ extern "C" int rxb200_power_group_accumulate(rxb200_power_group *g, const int16_
 		rxb200_power *h = g->h[(size_t)i];
 		RXB_CUDA(cudaSetDevice(h->device));
 		const size_t elems = (size_t)n_pass * (size_t)(e - b) * (size_t)p.buf_len;
-		if (elems > h->d_in_cap) {
-			cudaFree(h->d_in); h->d_in = nullptr; h->d_in_cap = 0;
-			RXB_CUDA(cudaMalloc(&h->d_in, elems * sizeof(int16_t)));
-			h->d_in_cap = elems;
-		}
+		RXB_CUDA(reserve(h->d_in, h->d_in_cap, elems));
 		// the member's hops of every pass, packed [n_pass][e-b][buf_len] on its device
 		RXB_CUDA(cudaMemcpy2DAsync(h->d_in, (size_t)(e - b) * p.buf_len * sizeof(int16_t),
 		                           hop_bufs + (size_t)(b - hop_begin) * p.buf_len, (size_t)nh * p.buf_len * sizeof(int16_t),
