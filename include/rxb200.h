@@ -556,7 +556,10 @@ int rxb200_fm_mix_group_reset(rxb200_fm_mix_group *g);
 #define RXB200_CVT_CS16_CF32 2
 #define RXB200_CVT_CS12_CS16 3
 int rxb200_sdr_convert(int kind, const void *src, size_t n_elems, void *dst, int device);
-/* Same with device pointers on `stream` (a cudaStream_t, may be NULL). */
+/* Same with device pointers on `stream` (a cudaStream_t, may be NULL).  Asynchronous.  Alignment, else RXB200_EINVAL
+ * before any CUDA call:
+ *   RXB200_CVT_CS16_CS8, _CS16_CU8, _CS16_CF32 : d_src and d_dst 16-byte aligned
+ *   RXB200_CVT_CS12_CS16                       : d_dst 4-byte aligned (one 32-bit store per element); d_src any */
 int rxb200_sdr_convert_device(int kind, const void *d_src, size_t n_elems, void *d_dst, void *stream);
 
 #ifdef __cplusplus

@@ -76,6 +76,8 @@ static size_t out_bytes(int kind, size_t n) { return kind == RXB200_CVT_CS16_CF3
 extern "C" int rxb200_sdr_convert_device(int kind, const void *d_src, size_t n_elems, void *d_dst, void *stream)
 {
 	if (kind < 0 || kind > 3 || !d_src || !d_dst) { set_error("bad convert request"); return RXB200_EINVAL; }
+	// the CS12 unpack reads bytes and stores one 32-bit word per element; the CS16 kinds move 16-byte vectors
+	if (kind == RXB200_CVT_CS12_CS16 && ((uintptr_t)d_dst & 3u)) { set_error("CS12 d_dst must be 4-byte aligned"); return RXB200_EINVAL; }
 	if (kind != RXB200_CVT_CS12_CS16 && (((uintptr_t)d_src & 15u) || ((uintptr_t)d_dst & 15u))) { set_error("pointers must be 16-byte aligned"); return RXB200_EINVAL; }
 	if (n_elems == 0) { return RXB200_OK; }
 	int dev = 0, sm = 132;
