@@ -147,7 +147,11 @@ int rxb200_fm_process(rxb200_fm *h, const int16_t *cs16, size_t n_int16, size_t 
                       int16_t *pcm, size_t pcm_stride, size_t *n_pcm, int *chunk_result_len);
 
 /* Same with DEVICE pointers (inputs already resident in HBM); asynchronous on the handle's stream
- * unless sync != 0.  n_pcm is computed on the host (closed form) and valid at return. */
+ * unless sync != 0.  n_pcm is computed on the host (closed form) and valid at return.  A call on
+ * the split kernel (kernel_kind 1) that directly follows the handle's previous split call on its
+ * stream may start reading d_cs16 while that call is still running: a kernel the caller puts on
+ * the handle's stream between two calls must not write the second call's input (copies,
+ * and anything ordered before the first call, may). */
 int rxb200_fm_process_device(rxb200_fm *h, const int16_t *d_cs16, size_t n_int16, size_t chunk_int16,
                              int16_t *d_pcm, size_t pcm_stride, size_t *n_pcm, int sync);
 
@@ -206,9 +210,11 @@ int rxb200_fm_last_stats(rxb200_fm *h, rxb200_fm_stats *out);
  * kernel (kernel_kind 0); beyond 32750 decimated samples with fifth_order passes (fewer for long
  * boxcars, DESIGN.md section 6) the call returns RXB200_EUNSUPPORTED. */
 int rxb200_fm_tune(rxb200_fm *h, int segment_len, int deemph_warmup);
-/* Device time (CUDA events on the handle's stream) of the last process call's main kernels, in
- * milliseconds: the split kernel on the row path, the fused kernel's main pass (not its per-chunk
- * reduction pre-passes), or the front and back kernels on the stream path.  Synchronises the stream. */
+/* Device time of the last process call's main kernels, in milliseconds: on the row path the split
+ * kernel from its first CTA's start to its last CTA's end by the GPU's global timer (no event sits
+ * between two calls there, since one would keep the next call from starting early), else CUDA
+ * events on the handle's stream around the fused kernel's main pass (not its per-chunk reduction
+ * pre-passes) or the front and back kernels on the stream path.  Synchronises the stream. */
 int rxb200_fm_kernel_ms(rxb200_fm *h, float *ms);
 
 /* The discriminators alone, for tests: one thread per element of n quads (ar, aj, br, bj) of int32 -- the sample

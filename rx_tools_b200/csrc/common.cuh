@@ -23,6 +23,9 @@ int fm_mix_check_host_call(rxb200_fm_mix *m, const int16_t *cs16, size_t n_int16
                            size_t pcm_stride, int *chunk_result_len, size_t *n_pcm, bool read, size_t *total,
                            size_t *n16, size_t *chunk16);
 int ddc_check(const rxb200_ddc *ddc, bool *wide);
+// fm_kernels.cu: something other than the handle's own split kernel (a kernel that writes the next call's input, a copy)
+// now precedes its next call on its stream, so that call must not start early (fm_split_kernel, I1)
+void fm_unchain(rxb200_fm *h);
 
 #define RXB_CUDA(call)                                                                   \
 	do {                                                                                 \

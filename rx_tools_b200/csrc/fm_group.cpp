@@ -94,6 +94,7 @@ int enqueue_in(Member &mb, const int16_t *cs16, size_t n_int16, size_t chunk_int
 	*started = true;
 	RXB_CUDA(cudaMemcpyAsync(mb.d_in, src, in_elems * sizeof(int16_t), cudaMemcpyHostToDevice,
 	                         (cudaStream_t)rxb200_fm_stream(mb.h)));
+	rxb::fm_unchain(mb.h);
 	size_t n = 0;
 	if (mb.m) {
 		return read ? rxb200_fm_mix_process_read_device(mb.m, mb.d_in, n_int16, mb.d_out, total + 8, &n, 0)

@@ -78,6 +78,10 @@ struct FmCall {
 	uint32_t *carry_out;      // [n_ch][state_words]
 	int *ticket;              // work counter
 	int *pub;                 // [n_ch*n_cta][4]  flag, avg, margin flag (row front end), -
+	int tag;                  // call tag of the flags in pub (0 but on the split kernel, fm_split_kernel)
+	unsigned long long *ticket64, ticket_base;   // split kernel: monotonic work counter, its value at this call's start
+	int *fix_next;            // split kernel: fix_count of the other call parity, cleared for the next call
+	unsigned long long *stamps;   // split kernel: [CTA][2] %globaltimer at the CTA's start and end (rxb200_fm_kernel_ms)
 	int16_t *margin;          // row front end: [n_ch*n_cta][n_extra * row PCM] the margin hand-over (fm_rows.cuh)
 	int *fix_count;           // lanes that had to be re-run from a neighbour's state
 	// per-chunk scalars of the optional reduction stages, [n_ch][n_chunks]; null when the stage is off
@@ -90,6 +94,9 @@ struct FmCall {
 	int one;                  // always 1 (see front_run)
 	const int16_t *pcm_g;     // fm_back_kernel: [n_ch][pcm_g_stride] PCM of the whole call in global memory (null elsewhere)
 	long long pcm_g_stride;
+#ifdef RXB_PROF
+	int prof_call;            // timeline slot of this call (rxb_prof_ts)
+#endif
 };
 
 // Scratch builds (-DRXB_PROF): per-warp clock64() sums of the split kernel's phases in a device array that
@@ -108,7 +115,15 @@ __device__ __forceinline__ unsigned long long *prof_slot(int s)
 #define PROF_ADD(slot_, t_) do { if (blockIdx.x < PROF_CTAS && (threadIdx.x & 31) == 0) { *prof_slot(slot_) += (unsigned long long)(clock64() - (t_)); } } while (0)
 #define PROF_SET(slot_, val_) do { if (blockIdx.x < PROF_CTAS && (threadIdx.x & 31) == 0) { *prof_slot(slot_) = (unsigned long long)(val_); } } while (0)
 #define PROF_INC(slot_, val_) do { if (blockIdx.x < PROF_CTAS && (threadIdx.x & 31) == 0) { *prof_slot(slot_) += (unsigned long long)(val_); } } while (0)
+// and a %globaltimer timeline of the split kernel per CTA, for PROF_CALLS consecutive calls (slot = FmCall::prof_call):
+// entry, the back end's first `full`, the front end's sentinel ticket, the end of the back end's last item, exit
+#define PROF_CALLS 4
+enum { TS_ENTRY = 0, TS_FIRST_FULL, TS_SENTINEL, TS_LAST_END, TS_EXIT, TS_N = 8 };
+__device__ unsigned long long rxb_prof_ts[PROF_CALLS * PROF_CTAS * TS_N];
+#define PROF_TS(call_, ev_) do { if (blockIdx.x < PROF_CTAS) { unsigned long long t_; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_)); \
+	rxb_prof_ts[((size_t)(call_) * PROF_CTAS + blockIdx.x) * TS_N + (ev_)] = t_; } } while (0)
 #else
+#define PROF_TS(call_, ev_) do { } while (0)
 #define PROF_CLK(var_) do { } while (0)
 #define PROF_ADD(slot_, t_) do { } while (0)
 #define PROF_SET(slot_, val_) do { } while (0)
@@ -1756,8 +1771,8 @@ __device__ __forceinline__ void back_item(const FmDev &c, const FmCall &k, const
 		auto publish = [&](int flag, int value) {
 			volatile int *mp = pub + 4 * (size_t)work;
 			// flag 1: the value goes out before the flag (a release store; the reader fences after seeing the flag)
-			if (flag == 1) { mp[1] = value; st_release_gpu(const_cast<int *>(mp), 1); }
-			else { mp[0] = flag; }
+			if (flag == 1) { mp[1] = value; st_release_gpu(const_cast<int *>(mp), k.tag | 1); }
+			else { mp[0] = k.tag | flag; }
 		};
 		// Every piece started exact (the common case with signal): the last piece is the anchor, nothing needs a start
 		// state, and what the loops below would do is publish its end state.  A single thread walking the pieces
@@ -1788,9 +1803,9 @@ __device__ __forceinline__ void back_item(const FmDev &c, const FmCall &k, const
 					int w = work - 1;
 					for (;;) {
 						const int f = pub[4 * (size_t)w];
-						if (f == 0) { __nanosleep(32); continue; }
-						if (f == 1) { __threadfence(); start = pub[4 * (size_t)w + 1]; break; }
-						w--;                                              // f == 2: that item passes its start through
+						if (f == (k.tag | 1)) { __threadfence(); start = pub[4 * (size_t)w + 1]; break; }
+						if (f == (k.tag | 2)) { w--; continue; }        // that item passes its start through
+						__nanosleep(32);                                  // not published yet (another tag: an older call's word)
 					}
 				} else { start = cur; }
 				s_start[j] = start;
@@ -1923,6 +1938,33 @@ static fm_kernel_fn pick_back_kernel(int ws, int t)
 // back end -> front end), item tickets travel through shared memory.  An item still only ever waits for OLDER
 // items (look-back in back_item), every CTA of the grid is resident, so the oldest unfinished item always advances.
 // The front end is the row front end (fm_rows.cuh: a warp per stretch, input through `in_map`); FIR: with the droop FIR.
+//
+// Back-to-back calls on one handle overlap (programmatic dependent launch, fm_launch): this call's CTAs take the SM
+// slots the previous call's CTAs leave and run the front end of their first items while that call drains.  What makes
+// that safe:
+//  I1  Before griddepcontrol.wait a CTA reads nothing the previous grid writes and writes nothing the previous grid reads
+//      or writes, apart from this call's own sync and margin slots (k.ticket64, k.pub, k.margin, double-buffered by call
+//      parity on the host).  So these wait: the front end of a channel's first item (its start state is carry_in) and
+//      of its last one (it writes carry_out), and the back end before its first item (it writes out, carry_out and
+//      fix_count and reads carry_in).  The front end of every other item reads only the input, and row_start_state
+//      rebuilds its state from input samples.
+//  I2  A CTA runs griddepcontrol.launch_dependents only once it has drawn its sentinel ticket and its own wait has
+//      returned.  The call after this one therefore starts only when the call before this one has completed, and that
+//      call's parity slots are free again.
+//  I3  Every grid fits fully resident (fm_launch caps the grid at n_sm x per_sm), so all of a call's CTAs are resident
+//      before any of the next call's can be, and the call always finishes; the look-back above still only waits for
+//      older items of the same call.
+// The slots are never cleared between calls: tickets count on from the host's mirror of the counter (k.ticket_base),
+// and the flags in k.pub carry the call's tag, so a word left by an older call reads as "not published yet".
+__device__ __forceinline__ void grid_dep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+__device__ __forceinline__ unsigned long long global_timer()
+{
+	unsigned long long t;
+	asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+	return t;
+}
+__device__ __forceinline__ void grid_dep_launch() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+
 #define BAR_FE 2
 #define SPLIT_BE_MAX 128
 template <int P, int SPEC, bool FIR, int TMAX, int MINB>
@@ -1940,6 +1982,8 @@ __global__ void __launch_bounds__(TMAX, MINB) fm_split_kernel(const FmDev c, con
 	int lane;
 	asm volatile("mov.u32 %0, %%laneid;" : "=r"(lane));     // volatile: read once (the compiler would re-read the special register at every use)
 	if (tid == 0) {
+		PROF_TS(k.prof_call, TS_ENTRY);
+		k.stamps[2 * blockIdx.x] = global_timer();
 		mbar_init(&s_full[0], n_fe); mbar_init(&s_full[1], n_fe);
 		mbar_init(&s_empty[0], k.be_lanes); mbar_init(&s_empty[1], k.be_lanes);
 		for (int j = 0; j < k.fe_warps * ROWS_STAGES; j++) { mbar_init(&s_ring_bar[j], 1); }
@@ -1971,13 +2015,22 @@ __global__ void __launch_bounds__(TMAX, MINB) fm_split_kernel(const FmDev c, con
 			// one barrier per item lines the front-end warps up behind the ticket (measured: letting them run ahead on a
 			// sequence number instead costs 9 % -- the early warps only reach the `empty` wait sooner and take issue
 			// slots from the warp the back end is waiting for)
-			if (tid == 0) { s_ticket[b] = atomicAdd(k.ticket, 1); }
+			if (tid == 0) { s_ticket[b] = (int)(atomicAdd(k.ticket64, 1ull) - k.ticket_base); }
 			PROF_CLK(t1);
 			bar_sync(BAR_FE, n_fe);
 			PROF_ADD(PF_BAR_FE, t1);
 			const int work = s_ticket[b];
-			if (work >= total_work) { mbar_arrive(&s_full[b]); break; }                // the back end sees the sentinel
+			if (work >= total_work) {                                                  // the back end sees the sentinel
+				if (tid == 0) {
+					PROF_TS(k.prof_call, TS_SENTINEL);
+					grid_dep_wait();                                                     // I2
+					grid_dep_launch();
+				}
+				mbar_arrive(&s_full[b]);
+				break;
+			}
 			const Item it = make_item(c, k, work);
+			if (it.b == 0 || it.b == k.n_cta - 1) { grid_dep_wait(); }                // I1: carry_in / carry_out
 			int16_t *buf = pcm_s + (size_t)b * k.pcm_cap;
 			uint32_t *xs = reinterpret_cast<uint32_t *>(pcm_s + 2 * (size_t)k.pcm_cap) + (size_t)(tid >> 5) * k.xs_words;
 			PROF_CLK(t2);
@@ -1991,11 +2044,14 @@ __global__ void __launch_bounds__(TMAX, MINB) fm_split_kernel(const FmDev c, con
 		}
 	} else {
 		const int q = tid - n_fe;
+		grid_dep_wait();                                                             // I1
+		if (blockIdx.x == 0 && q == 0) { *k.fix_next = 0; }    // the call before this one has completed; only this call's count is reported
 		for (int i = 0;; i++) {
 			const int b = i & 1;
 			PROF_CLK(t0);
 			mbar_wait(&s_full[b], (uint32_t)((i >> 1) & 1));
 			PROF_ADD(PF_FULL, t0);
+			if (i == 0 && q == 0) { PROF_TS(k.prof_call, TS_FIRST_FULL); }
 			const int work = s_ticket[b];
 			if (work >= total_work) { break; }
 			const Item it = make_item(c, k, work);
@@ -2005,9 +2061,15 @@ __global__ void __launch_bounds__(TMAX, MINB) fm_split_kernel(const FmDev c, con
 			back_item<SPEC, PCM_PAD_ROWS>(c, k, it, work, q, k.be_lanes, pcm_s + (size_t)b * k.pcm_cap, s_avg, s_mrun, s_ok, s_start);
 			PROF_INC(PF_ITEMS, 1);
 			mbar_arrive(&s_empty[b]);
+			if (q == 0) { PROF_TS(k.prof_call, TS_LAST_END); }
 		}
 	}
 	PROF_ADD(PF_TOTAL, t_start);
+	__syncthreads();                                     // both ends are done: the CTA's end
+	if (tid == 0) {
+		PROF_TS(k.prof_call, TS_EXIT);
+		k.stamps[2 * blockIdx.x + 1] = global_timer();
+	}
 }
 
 // ---- per-chunk reduction pre-passes: the scalar recurrences across chunks (one thread per channel)
@@ -2291,7 +2353,15 @@ struct rxb200_fm {
 	uint32_t *d_carry[2] = {nullptr, nullptr};
 	int cur = 0;                   // which carry buffer holds the current state
 	int *d_sync = nullptr; size_t sync_cap = 0;  // [0] ticket, [1] fix_count, [4..] pub[n_ch*n_cta][4]
-	int16_t *d_margin = nullptr; size_t margin_cap = 0;   // row front end: margin hand-over slots (int16 entries)
+	// the split kernel's own sync words and margin hand-over slots (int16 entries), one set per call parity, never cleared
+	// between calls (fm_split_kernel, I1-I3): [0..1] the 64-bit ticket, [2] fix_count, [4..] pub[n_ch*n_cta][4]
+	int *d_chain[2] = {nullptr, nullptr}; size_t chain_cap = 0;
+	int16_t *d_margin[2] = {nullptr, nullptr}; size_t margin_cap = 0;
+	unsigned long long chain_base[2] = {0, 0};   // host mirror of each parity's ticket counter
+	unsigned chain_calls = 0;      // split-kernel calls since the slots were last cleared: parity and tag of the next one
+	bool chained = false;          // the last work this library put on the stream is this handle's split kernel
+	int *fix_src = nullptr;        // where the last call's fix_count is
+	unsigned long long *stamp_src = nullptr; int stamp_n = 0;   // the last call's CTA stamps when it ran the split kernel
 	int *d_atan_lut = nullptr;
 	int16_t *d_in = nullptr; size_t d_in_cap = 0;         // int16 elements
 	int16_t *d_out = nullptr; size_t d_out_cap = 0;
@@ -2479,16 +2549,19 @@ extern "C" int rxb200_fm_reset(rxb200_fm *h)
 	RXB_CUDA(cudaMemcpyAsync(h->d_carry[0], init.data(), cbytes, cudaMemcpyHostToDevice, h->stream));
 	RXB_CUDA(cudaMemcpyAsync(h->d_carry[1], init.data(), cbytes, cudaMemcpyHostToDevice, h->stream));
 	RXB_CUDA(cudaStreamSynchronize(h->stream));
-	h->cur = 0; h->h_box_n = 0; h->h_lpr_phase = 0;
+	h->cur = 0; h->h_box_n = 0; h->h_lpr_phase = 0; h->chained = false;
 	return RXB200_OK;
 }
+
+void rxb::fm_unchain(rxb200_fm *h) { h->chained = false; }
 
 extern "C" void rxb200_fm_destroy(rxb200_fm *h)
 {
 	if (!h) { return; }
 	cudaSetDevice(h->device);
 	if (h->stream) { cudaStreamSynchronize(h->stream); }
-	cudaFree(h->d_carry[0]); cudaFree(h->d_carry[1]); cudaFree(h->d_sync); cudaFree(h->d_margin);
+	cudaFree(h->d_carry[0]); cudaFree(h->d_carry[1]); cudaFree(h->d_sync);
+	cudaFree(h->d_chain[0]); cudaFree(h->d_chain[1]); cudaFree(h->d_margin[0]); cudaFree(h->d_margin[1]);
 	cudaFree(h->d_atan_lut); cudaFree(h->d_in); cudaFree(h->d_out); cudaFree(h->d_pcm);
 	cudaFree(h->d_sums); cudaFree(h->d_rdc); cudaFree(h->d_sqz); cudaFree(h->d_adc); cudaFree(h->d_lens); cudaFree(h->d_levels);
 	if (h->ev0) { cudaEventDestroy(h->ev0); }
@@ -2501,6 +2574,17 @@ extern "C" int rxb200_fm_kernel_ms(rxb200_fm *h, float *ms)
 {
 	if (!h || !ms) { return RXB200_EINVAL; }
 	RXB_CUDA(cudaSetDevice(h->device));
+	if (h->stamp_src) {
+		// the split kernel: no event may sit between two calls (it would stop the next call from starting early), so the
+		// kernel stamps each CTA's start and end with the global timer
+		std::vector<unsigned long long> t(2 * (size_t)h->stamp_n);
+		RXB_CUDA(cudaMemcpyAsync(t.data(), h->stamp_src, t.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
+		RXB_CUDA(cudaStreamSynchronize(h->stream));
+		unsigned long long t0 = t[0], t1 = t[1];
+		for (int b = 1; b < h->stamp_n; b++) { t0 = t[2 * b] < t0 ? t[2 * b] : t0; t1 = t[2 * b + 1] > t1 ? t[2 * b + 1] : t1; }
+		*ms = (float)((double)(t1 - t0) * 1e-6);
+		return RXB200_OK;
+	}
 	RXB_CUDA(cudaEventSynchronize(h->ev1));
 	RXB_CUDA(cudaEventElapsedTime(ms, h->ev0, h->ev1));
 	return RXB200_OK;
@@ -2926,6 +3010,38 @@ static int fm_prepasses(rxb200_fm *h, FmCall &k, size_t n_int16, size_t chunk_in
 	return RXB200_OK;
 }
 
+// The split kernel's slots for `work` items of `margin` int16 each and `blocks` CTAs, in both parities.  They are cleared when they are
+// (re)allocated and when the call tag would wrap, after the calls still using them have finished; the tickets then
+// count from 0 again.
+#define FM_CHAIN_CALLS (1u << 28)      // tags ((calls + 1) << 2 | flag) stay positive ints
+static int fm_chain_reserve(rxb200_fm *h, size_t work, size_t blocks, size_t margin)
+{
+	const size_t need = 4 + 4 * work + 4 * blocks;
+	const bool grow = need > h->chain_cap || margin > h->margin_cap;
+	if (!grow && h->chain_calls + 1u < FM_CHAIN_CALLS) { return RXB200_OK; }
+	RXB_CUDA(cudaStreamSynchronize(h->stream));
+	if (grow) {
+		for (int p = 0; p < 2; p++) {
+			cudaFree(h->d_chain[p]); cudaFree(h->d_margin[p]); h->d_chain[p] = nullptr; h->d_margin[p] = nullptr;
+		}
+		h->chain_cap = h->margin_cap = 0;
+		for (int p = 0; p < 2; p++) {
+			RXB_CUDA(cudaMalloc(&h->d_chain[p], need * sizeof(int)));
+			RXB_CUDA(cudaMalloc(&h->d_margin[p], (margin ? margin : 1) * sizeof(int16_t)));
+		}
+		h->chain_cap = need; h->margin_cap = margin;
+	}
+	for (int p = 0; p < 2; p++) { RXB_CUDA(cudaMemsetAsync(h->d_chain[p], 0, h->chain_cap * sizeof(int), h->stream)); }
+	h->chain_base[0] = h->chain_base[1] = 0;
+	h->chain_calls = 0;
+	h->chained = false;
+	return RXB200_OK;
+}
+
+#ifdef RXB_PROF
+static unsigned h_prof_calls = 0;      // split-kernel calls since the last rxb200_fm_prof_timeline clear
+#endif
+
 // Plans and launches one call -- the split kernel where the shape allows it, else the fused kernel, or on the stream
 // path the front and back kernels -- then advances the host mirrors of the closed-form counters.  any: the call runs on
 // the any-length kernel (kern_any) instead.
@@ -2961,28 +3077,51 @@ static int fm_launch(rxb200_fm *h, const int16_t *d_in, size_t n_int16, size_t c
 	}
 	const size_t total_back = (size_t)b.n_cta * h->n_channels;
 	const size_t need_sync = 4 + 4 * (total_work > total_back ? total_work : total_back);
-	RXB_CUDA(reserve(h->d_sync, h->sync_cap, need_sync));
-	if (rows) {
-		RXB_CUDA(reserve(h->d_margin, h->margin_cap, total_work * (size_t)k.n_extra * (size_t)(ROW_LEN >> dv.P)));
-		k.margin = h->d_margin;
-	}
+	size_t blocks = (size_t)h->n_sm * g.per_sm;
+	if (blocks > total_work) { blocks = total_work; }
+	if (rows) { rc = fm_chain_reserve(h, total_work, blocks, total_work * (size_t)k.n_extra * (size_t)(ROW_LEN >> dv.P)); }
+	else { RXB_CUDA(reserve(h->d_sync, h->sync_cap, need_sync)); }
+	if (rc != RXB200_OK) { return rc; }
+	const int par = (int)(h->chain_calls & 1u);
 	// the fields every kernel of the call shares; the stream path's front kernel writes the PCM scratch
 	k.in = d_in; k.out = stream ? h->d_pcm : d_out; k.out_stride = stream ? b.pstride : (long long)out_stride;
 	k.n = n; k.chunk = (int)(chunk_int16 / 2); k.n_chunks = (int)((n + k.chunk - 1) / k.chunk); k.n_ch = h->n_channels;
 	k.state_words = h->state_words; k.carry_in = h->d_carry[h->cur]; k.carry_out = h->d_carry[h->cur ^ 1];
-	k.ticket = h->d_sync; k.fix_count = h->d_sync + 1; k.pub = h->d_sync + 4; k.one = 1;
-	size_t blocks = (size_t)h->n_sm * g.per_sm;
-	if (blocks > total_work) { blocks = total_work; }
+	k.one = 1;
+	if (rows) {
+		k.ticket64 = reinterpret_cast<unsigned long long *>(h->d_chain[par]); k.ticket_base = h->chain_base[par];
+		k.fix_count = h->d_chain[par] + 2; k.fix_next = h->d_chain[par ^ 1] + 2; k.pub = h->d_chain[par] + 4;
+		k.margin = h->d_margin[par];
+		k.tag = (int)((h->chain_calls + 1u) << 2);
+		k.stamps = reinterpret_cast<unsigned long long *>(h->d_chain[par] + 4 + 4 * total_work);
+	} else {
+		k.ticket = h->d_sync; k.fix_count = h->d_sync + 1; k.pub = h->d_sync + 4;
+	}
 	int launches = 0;
-	// one pass over the call; ev0/ev1 bracket the main pass (reduce_mode 0, the time rxb200_fm_kernel_ms reports)
+#ifdef RXB_PROF
+	if (rows) { k.prof_call = h_prof_calls++ % PROF_CALLS; }
+#endif
+	// one pass over the call; ev0/ev1 bracket the main pass (reduce_mode 0, the time rxb200_fm_kernel_ms reports) but for
+	// the split kernel, which stamps its own time
 	auto pass = [&](int reduce_mode) -> int {
 		k.reduce_mode = reduce_mode;
-		RXB_CUDA(cudaMemsetAsync(h->d_sync, 0, need_sync * sizeof(int), h->stream));
-		if (reduce_mode == 0) { RXB_CUDA(cudaEventRecord(h->ev0, h->stream)); }
-		if (rows) { h->kern_rows<<<(unsigned)blocks, g.threads, g.smem, h->stream>>>(dv, k, in_map); }
+		if (!rows) { RXB_CUDA(cudaMemsetAsync(h->d_sync, 0, need_sync * sizeof(int), h->stream)); }
+		if (reduce_mode == 0 && !rows) { RXB_CUDA(cudaEventRecord(h->ev0, h->stream)); }
+		if (rows) {
+			// right behind this handle's previous split call, this one may start while that one drains (I1-I3)
+			cudaLaunchAttribute attr;
+			attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+			attr.val.programmaticStreamSerializationAllowed = h->chained ? 1 : 0;
+			cudaLaunchConfig_t cfg = {};
+			cfg.gridDim = dim3((unsigned)blocks); cfg.blockDim = dim3((unsigned)g.threads);
+			cfg.dynamicSmemBytes = g.smem; cfg.stream = h->stream; cfg.attrs = &attr; cfg.numAttrs = 1;
+			RXB_CUDA(cudaLaunchKernelEx(&cfg, h->kern_rows, dv, k, in_map));
+			h->chain_base[par] += total_work + blocks;     // every CTA draws one sentinel ticket
+			h->chain_calls++;
+		}
 		else { kern<<<(unsigned)blocks, g.threads, g.smem, h->stream>>>(dv, k); }
 		RXB_CUDA(cudaGetLastError());
-		if (reduce_mode == 0) { RXB_CUDA(cudaEventRecord(h->ev1, h->stream)); }
+		if (reduce_mode == 0 && !rows) { RXB_CUDA(cudaEventRecord(h->ev1, h->stream)); }
 		launches++;
 		return RXB200_OK;
 	};
@@ -3006,6 +3145,9 @@ static int fm_launch(rxb200_fm *h, const int16_t *d_in, size_t n_int16, size_t c
 		launches++;
 	}
 	h->cur ^= 1;
+	h->chained = rows;
+	h->fix_src = k.fix_count;
+	h->stamp_src = rows ? k.stamps : nullptr; h->stamp_n = (int)blocks;
 	h->stats.launches = launches; h->stats.segments = (int)(total_work * (rows ? k.fe_warps : g.threads));
 	h->stats.segment_len = rows ? k.n_own * ROW_LEN : k.Sf; h->stats.warmup_len = (int)((stream ? b.W_dec : k.W_dec) * (long long)dv.D);
 	h->stats.fixup_segments = -1; h->stats.kernel_kind = rows ? 1 : (stream ? 3 : 0);
@@ -3057,7 +3199,7 @@ static int fm_process_device(rxb200_fm *h, const int16_t *d_cs16, size_t n_int16
 	if (n_pcm) { *n_pcm = total; }
 	if (sync) {
 		RXB_CUDA(cudaStreamSynchronize(h->stream));
-		RXB_CUDA(cudaMemcpy(&h->stats.fixup_segments, h->d_sync + 1, sizeof(int), cudaMemcpyDeviceToHost));
+		RXB_CUDA(cudaMemcpy(&h->stats.fixup_segments, h->fix_src, sizeof(int), cudaMemcpyDeviceToHost));
 	}
 	return RXB200_OK;
 }
@@ -3074,6 +3216,7 @@ static int fm_process_host(rxb200_fm *h, const int16_t *cs16, size_t n_int16, si
 	RXB_CUDA(reserve(h->d_in, h->d_in_cap, in_elems));
 	RXB_CUDA(reserve(h->d_out, h->d_out_cap, out_elems));
 	RXB_CUDA(cudaMemcpyAsync(h->d_in, cs16, in_elems * sizeof(int16_t), cudaMemcpyHostToDevice, h->stream));
+	h->chained = false;
 	rc = fm_launch(h, h->d_in, n_int16, chunk_int16, h->d_out, total + 8, any);
 	if (rc != RXB200_OK) { return rc; }
 	if (pcm_stride == total + 8 || h->n_channels == 1) {
@@ -3083,7 +3226,7 @@ static int fm_process_host(rxb200_fm *h, const int16_t *cs16, size_t n_int16, si
 		RXB_CUDA(cudaMemcpy2DAsync(pcm, pcm_stride * sizeof(int16_t), h->d_out, (total + 8) * sizeof(int16_t),
 		                           total * sizeof(int16_t), (size_t)h->n_channels, cudaMemcpyDeviceToHost, h->stream));
 	}
-	RXB_CUDA(cudaMemcpyAsync(&h->stats.fixup_segments, h->d_sync + 1, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+	RXB_CUDA(cudaMemcpyAsync(&h->stats.fixup_segments, h->fix_src, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
 	RXB_CUDA(cudaStreamSynchronize(h->stream));
 	if (n_pcm) { *n_pcm = total; }
 	return RXB200_OK;
@@ -3143,10 +3286,10 @@ extern "C" void *rxb200_fm_stream(rxb200_fm *h) { return h ? (void *)h->stream :
 extern "C" int rxb200_fm_last_stats(rxb200_fm *h, rxb200_fm_stats *out)
 {
 	if (!h || !out) { return RXB200_EINVAL; }
-	if (h->stats.fixup_segments < 0 && h->d_sync) {
+	if (h->stats.fixup_segments < 0 && h->fix_src) {
 		RXB_CUDA(cudaSetDevice(h->device));
 		RXB_CUDA(cudaStreamSynchronize(h->stream));
-		RXB_CUDA(cudaMemcpy(&h->stats.fixup_segments, h->d_sync + 1, sizeof(int), cudaMemcpyDeviceToHost));
+		RXB_CUDA(cudaMemcpy(&h->stats.fixup_segments, h->fix_src, sizeof(int), cudaMemcpyDeviceToHost));
 	}
 	*out = h->stats;
 	return RXB200_OK;
@@ -3195,6 +3338,21 @@ extern "C" int rxb200_fm_prof_read(unsigned long long *dst, size_t n, int clear)
 		void *p = nullptr;
 		RXB_CUDA(cudaGetSymbolAddress(&p, rxb_prof));
 		RXB_CUDA(cudaMemset(p, 0, all * sizeof(unsigned long long)));
+	}
+	return RXB200_OK;
+}
+
+// the split kernel's timeline: [PROF_CALLS][PROF_CTAS][TS_N] %globaltimer stamps of the calls since the last clear
+// (clear = 1: zero them and start again at slot 0)
+extern "C" int rxb200_fm_prof_timeline(unsigned long long *dst, size_t n, int clear)
+{
+	const size_t all = (size_t)PROF_CALLS * PROF_CTAS * TS_N;
+	if (dst && n) { RXB_CUDA(cudaMemcpyFromSymbol(dst, rxb_prof_ts, (n < all ? n : all) * sizeof(unsigned long long))); }
+	if (clear) {
+		void *p = nullptr;
+		RXB_CUDA(cudaGetSymbolAddress(&p, rxb_prof_ts));
+		RXB_CUDA(cudaMemset(p, 0, all * sizeof(unsigned long long)));
+		h_prof_calls = 0;
 	}
 	return RXB200_OK;
 }

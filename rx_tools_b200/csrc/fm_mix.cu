@@ -452,6 +452,7 @@ int mix_call(rxb200_fm_mix *m, const int16_t *cs16, size_t n_int16, size_t chunk
 	RXB_CUDA(cudaEventRecord(m->ev1, st));
 	rc = ddc_carry(m, src, c, st);
 	if (rc != RXB200_OK) { return rc; }
+	rxb::fm_unchain(m->h);                       // the member's input was just written on its stream
 	if (n16) {
 		int16_t *out = device ? pcm : m->d_out;
 		const size_t stride = device ? pcm_stride : total + 8;

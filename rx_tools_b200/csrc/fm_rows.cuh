@@ -407,8 +407,8 @@ __device__ __forceinline__ void front_rows(const FmDev &c, const FmCall &k, cons
 }
 
 // ---- margin hand-over between the items of a channel.  Item w's slot in k.margin holds n_extra rows of PCM: row r of
-// the item sits at (r - (own_hi - n_extra)) * row_pcm, and only its own rows are written.  pub[4 w + 2] = 1 says the
-// slot is complete.  (PCM_PAD_ROWS is 0: the shared buffer is linear.)
+// the item sits at (r - (own_hi - n_extra)) * row_pcm, and only its own rows are written.  pub[4 w + 2] = tag | 1 says
+// the slot is complete.  (PCM_PAD_ROWS is 0: the shared buffer is linear.)
 #define BAR_PUB 3
 
 // Front end, after its own rows: the last front-end warp waits for the others' rows (the others only arrive), copies
@@ -428,7 +428,7 @@ __device__ __forceinline__ void rows_publish(const FmCall &k, const Item &it, in
 	const int n = ((own_hi - lo) << LG) / 8;
 	for (int i = lane; i < n; i += 32) { dst[i] = src[i]; }
 	__syncwarp();                                          // the lanes' copies are ordered before lane 0's release
-	if (lane == 0) { st_release_gpu(k.pub + 4 * (size_t)work + 2, 1); }
+	if (lane == 0) { st_release_gpu(k.pub + 4 * (size_t)work + 2, k.tag | 1); }
 }
 
 // Back end, before pass 1: the margin rows [buf_lo, own_lo) of this item, from the slots of the older items of the
@@ -445,7 +445,7 @@ __device__ __forceinline__ void rows_collect(const FmCall &k, const Item &it, in
 	const int first = buf_lo / k.n_own;                  // the oldest item holding a margin row
 	for (int j = first; j < it.b; j++) {
 		const int *f = k.pub + 4 * (size_t)(work - (it.b - j)) + 2;
-		while (ld_acquire_gpu(f) == 0) { __nanosleep(32); }
+		while (ld_acquire_gpu(f) != (k.tag | 1)) { __nanosleep(32); }
 	}
 	const int n = ((own_lo - buf_lo) << LG) / 8;
 	uint4 *dst = reinterpret_cast<uint4 *>(pcm_s + (((long long)buf_lo << LG) - it.m_lo));

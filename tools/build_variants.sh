@@ -12,7 +12,7 @@ for spec in "$@"; do
 	name="${spec%%=*}"; flags="${spec#*=}"
 	(
 		nvcc $ARCH -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -Xptxas -v $flags -c -o ../variants/fm_$name.o fm_kernels.cu 2> ../variants/fm_$name.ptxas.log
-		nvcc $ARCH -shared -o ../variants/librxb200_$name.so ../variants/fm_$name.o power_kernels.o sdr_kernels.o host_plan.o nccl_dyn.o -ldl
+		nvcc $ARCH -shared -o ../variants/librxb200_$name.so ../variants/fm_$name.o fm_mix.o fm_group.o power_kernels.o sdr_kernels.o host_plan.o nccl_dyn.o -ldl
 		echo "$flags" > ../variants/$name.flags
 		echo "built $name: $flags"
 	) &

@@ -5,7 +5,11 @@ Needs a scratch build with -DRXB_PROF (tools/build_variants.sh prof="-DRXB_PROF"
 then sums clock64() intervals per warp into a device array (fm_kernels.cu, PF_*).  Runs bench.py's fm2b stream (1 GiB
 CS16, chunk 131072) once to warm up and once measured, and prints per warp slot of the CTA: its %warpid % 4 over all
 CTAs (the SMSP it issues on), and per item the cycles of each phase.
-  RXB200_LIB=rx_tools_b200/variants/librxb200_prof.so python tools/fm_prof.py [--size-mib 1024]"""
+  RXB200_LIB=rx_tools_b200/variants/librxb200_prof.so python tools/fm_prof.py [--size-mib 1024]
+--timeline: instead, PROF_CALLS back-to-back calls of that stream (sync=False, one output buffer, as bench.py makes
+them) and, per call, from each CTA's %globaltimer stamps: how long the back end waits for its first item (fill), how
+long the front-end warps sit idle after the sentinel ticket (drain), how long the CTA's SM slot stays empty before the
+grid ends (tail), and the gap from the end of one call to the first CTA of the next (negative: the calls overlap)."""
 import argparse
 import collections
 import ctypes as C
@@ -23,11 +27,55 @@ PROF_CTAS, PROF_SLOTS = 1024, 16
 FE_COLS = [("rows", PF_ROWS), ("front_rows", PF_FRONT), ("ring wait", PF_RING), ("BAR_FE", PF_BAR_FE),
            ("empty", PF_EMPTY), ("publish", PF_PUBLISH)]
 BE_COLS = [("full", PF_FULL), ("collect", PF_COLLECT), ("pass 1", PF_PASS1), ("chain", PF_CHAIN), ("pass 2", PF_PASS2)]
+PROF_CALLS, TS_N = 4, 8
+TS_ENTRY, TS_FIRST_FULL, TS_SENTINEL, TS_LAST_END, TS_EXIT = range(5)
+
+
+def timeline(lib, d, x, out, cap):
+    """per-call fill / drain / tail / gap of PROF_CALLS chained calls (microseconds and shares of the call's span)"""
+    import torch
+    import bench
+    from rx_tools_b200 import _lib
+    lib.rxb200_fm_prof_timeline.argtypes = [C.c_void_p, C.c_size_t, C.c_int]
+
+    def step():
+        d.process_device(x.data_ptr(), x.numel(), bench.CHUNK, out.data_ptr(), cap, sync=False)
+    for _ in range(3):
+        step()
+    torch.cuda.synchronize()
+    _lib.check(lib.rxb200_fm_prof_timeline(None, 0, 1))
+    for _ in range(PROF_CALLS):
+        step()
+    torch.cuda.synchronize()
+    buf = np.zeros(PROF_CALLS * PROF_CTAS * TS_N, dtype=np.uint64)
+    _lib.check(lib.rxb200_fm_prof_timeline(buf.ctypes.data, buf.size, 0))
+    ts = buf.reshape(PROF_CALLS, PROF_CTAS, TS_N).astype(np.int64)
+    n = int((ts[0, :, TS_ENTRY] > 0).sum())
+    ts = (ts[:, :n] - ts[0, :n, TS_ENTRY].min()) / 1e3        # microseconds from the first call's first CTA
+    print(f"{n} CTAs per call; times in us from the first CTA of call 0")
+    print("call   start     end    span   period    gap | fill mean/max   drain mean/max   tail mean/max |"
+          "  fill%  drain%  tail%  gap%")
+    prev_end = prev_start = None
+    for c in range(PROF_CALLS):
+        t = ts[c]
+        start, end = t[:, TS_ENTRY].min(), t[:, TS_EXIT].max()
+        span = end - start
+        fill = t[:, TS_FIRST_FULL] - t[:, TS_ENTRY]
+        drain = t[:, TS_EXIT] - t[:, TS_SENTINEL]
+        tail = end - t[:, TS_EXIT]
+        gap = start - prev_end if prev_end is not None else float("nan")
+        period = start - prev_start if prev_start is not None else float("nan")
+        print(f"{c:4d} {start:7.1f} {end:7.1f} {span:7.1f} {period:8.1f} {gap:6.1f} | {fill.mean():6.1f} {fill.max():6.1f}"
+              f"    {drain.mean():6.1f} {drain.max():6.1f}   {tail.mean():6.1f} {tail.max():6.1f} |"
+              f" {100 * fill.mean() / span:6.1f} {100 * drain.mean() / span:6.1f} {100 * tail.mean() / span:6.1f}"
+              f" {100 * gap / span:5.1f}")
+        prev_end, prev_start = end, start
 
 
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--size-mib", type=int, default=1024)
+    ap.add_argument("--timeline", action="store_true")
     args = ap.parse_args()
     import torch
     import bench
@@ -43,6 +91,10 @@ def main():
     d = fm.FmDemod(bench.fm_params("fm2b"))
     cap = d.max_output(n_int16, bench.CHUNK) + 8
     out = torch.empty(cap, dtype=torch.int16, device="cuda")
+    if args.timeline:
+        timeline(lib, d, x, out, cap)
+        d.close()
+        return
     d.process_device(x.data_ptr(), n_int16, bench.CHUNK, out.data_ptr(), cap, sync=True)
     _lib.check(lib.rxb200_fm_prof_read(None, 0, 1))
     d.process_device(x.data_ptr(), n_int16, bench.CHUNK, out.data_ptr(), cap, sync=True)
