@@ -10,6 +10,11 @@
  * Several GPUs: RXB200_GPUS=n (environment, so the reference's option string stays as it is) shards the hops over
  * n GPUs of this box through rxb200_power_group_* -- every GPU transforms the hops it owns, ONE NCCL all-gather
  * collates the spectrum rows in hop order before the report loop (src/rtl_power.c:1047-1050).
+ *
+ * Capture mode: RXB200_CAPTURE_RATE=<max Hz> takes every hop of a sweep from ONE wideband capture instead of a retune
+ * and a read per hop.  The device is tuned once to the centre of the hops, at M times the hop rate, and read without
+ * pause; each pass of M * buf_len int16 goes through rxb200_power_mix_accumulate, whose NCO down-converter makes every
+ * hop's buffer on the GPU.  A pass counts as a sweep.
  */
 #include <math.h>
 #include <signal.h>
@@ -37,7 +42,9 @@ static void usage(void)
 		"\t[-w rectangle|hamming|blackman|blackman-harris|hann-poisson|youssef|kaiser|bartlett]\n"
 		"\t[-c crop_percent] [-F fir_size] [-P peak hold] [-D direct_sampling] [-O offset tuning]\n"
 		"\t[-S tuner_sleep_usec] [-R tuner_retry_max]\n"
-		"\tfilename ('-' means stdout)\n");
+		"\tfilename ('-' means stdout)\n"
+		"environment: RXB200_GPUS=n shards the hops over n GPUs; RXB200_CAPTURE_RATE=max_Hz takes every hop from one\n"
+		"\tcapture of at most max_Hz samples/s, tuned once to the centre of the sweep (one GPU)\n");
 	exit(1);
 }
 
@@ -46,6 +53,121 @@ static int window_id(const char *name)
 	static const char *names[] = {"rectangle", "hamming", "blackman", "blackman-harris", "hann-poisson", "youssef", "kaiser", "bartlett"};
 	for (int i = 0; i < 8; i++) { if (!strcmp(name, names[i])) { return i; } }
 	return -1;
+}
+
+/* ---- report (:1044-1058): csv_dbm()'s rows of every hop from the accumulators of pw, then the date/time prefix */
+static int report(FILE *out, rxb200_power *pw, const rxb200_power_plan *plan, double *db, int row_len, int *samples,
+                  char *row, size_t row_cap, const char *tstr)
+{
+	const rxb200_power_params *pp = &plan->params;
+	if (rxb200_power_read_db(pw, plan->rate, plan->crop, db, (size_t)row_len, samples) != RXB200_OK) { fprintf(stderr, "rxb200: %s\n", rxb200_last_error()); return -1; }
+	int have = 0;
+	for (int i = 0; i < pp->n_hops; i++) { have |= samples[i]; }
+	if (have) {
+		for (int i = 0; i < pp->n_hops; i++) {
+			int n = rxb200_power_format_db_row(db + (size_t)i * row_len, pp->bin_e, plan->first_freq + (int64_t)i * plan->freq_step, plan->rate,
+			                                pp->downsample, plan->crop, samples[i], row, row_cap);
+			if (n < 0) { fprintf(stderr, "rxb200: %s\n", rxb200_last_error()); break; }
+			fprintf(out, "%s, ", tstr);
+			fwrite(row, 1, (size_t)n, out);
+		}
+		fflush(out);
+	}
+	return 0;
+}
+
+static void time_string(char *tstr, size_t cap, time_t now)
+{
+	struct tm cal;
+	localtime_r(&now, &cal);
+	strftime(tstr, cap, "%Y-%m-%d, %H:%M:%S", &cal);
+	if (getenv("RXB200_FIXED_TIME")) { snprintf(tstr, cap, "%s", getenv("RXB200_FIXED_TIME")); }
+}
+
+/* Capture mode's device side and report loop: one tune to fc at R, one flush read, then passes of M * buf_len int16
+ * collected from reads of whatever length the device returns; a failed read discards the partial pass, and
+ * tuner_retry_max failed reads in a row mean the stream has run dry. */
+static int capture_mode(rxb200_power_mix *pm, const rxb200_power_plan *plan, int R, int64_t fc, int M,
+                        const char *dev_query, size_t channel, const char *gain_str, const char *antenna, const char *filename,
+                        int ppm, int direct_sampling, int offset_tuning, int tuner_sleep_usec, int tuner_retry_max,
+                        int interval, int single, time_t exit_after)
+{
+	const rxb200_power_params *pp = &plan->params;
+	const int n_hops = pp->n_hops, N = 1 << pp->bin_e;
+	rxb200_power *pw = rxb200_power_mix_member(pm);
+	SoapySDRDevice *dev = NULL; SoapySDRStream *stream = NULL;
+	if (sdr_open(dev_query, channel, &dev, &stream) != 0) { fprintf(stderr, "Failed to open sdr device matching '%s'.\n", dev_query); return 1; }
+	if (antenna && SoapySDRDevice_setAntenna(dev, SOAPY_SDR_RX, channel, antenna) != 0) { fprintf(stderr, "Failed to set antenna"); }
+	SoapySDRDevice_activateStream(dev, stream, 0, 0, 0);
+	struct sigaction sa; memset(&sa, 0, sizeof sa); sa.sa_handler = on_signal;
+	sigaction(SIGINT, &sa, NULL); sigaction(SIGTERM, &sa, NULL); sigaction(SIGQUIT, &sa, NULL);
+	signal(SIGPIPE, SIG_IGN);
+	if (direct_sampling) { SoapySDRDevice_writeSetting(dev, "direct_samp", direct_sampling == 1 ? "1" : "2"); }
+	if (offset_tuning) { SoapySDRDevice_writeSetting(dev, "offset_tune", "true"); }
+	sdr_set_gain(dev, channel, gain_str);
+	SoapySDRDevice_setFrequencyCorrection(dev, SOAPY_SDR_RX, channel, (double)ppm);
+	FILE *out = !strcmp(filename, "-") ? stdout : fopen(filename, "wb");
+	if (!out) { fprintf(stderr, "Failed to open %s\n", filename); return 1; }
+	SoapySDRDevice_setSampleRate(dev, SOAPY_SDR_RX, channel, (double)R);
+	SoapySDRKwargs none = {0, NULL, NULL};
+	if (SoapySDRDevice_setFrequency(dev, SOAPY_SDR_RX, channel, (double)fc, &none) != 0) {
+		fprintf(stderr, "Error: failed to set frequency %lli Hz\n", (long long)fc);
+	} else {
+		usleep((useconds_t)tuner_sleep_usec);
+		int16_t *dump = (int16_t *)malloc((size_t)BUFFER_DUMP * 4);
+		int r = -1, flags = 0; long long tn = 0; void *bp[] = {dump};
+		for (int a = 0; a < tuner_retry_max && r < 0; a++) { r = SoapySDRDevice_readStream(dev, stream, bp, BUFFER_DUMP, &flags, &tn, 1000000); }
+		if (r < 0) { fprintf(stderr, "Error: bad retune at %lli Hz, r=%d (try increasing -S or -R).\n", (long long)fc, r); }
+		free(dump);
+	}
+	const size_t pass16 = (size_t)M * (size_t)pp->buf_len;
+	int16_t *pass = (int16_t *)malloc(pass16 * sizeof(int16_t));
+	const int row_len = rxb200_power_row_len(pp->bin_e, plan->crop);
+	double *db = (double *)malloc((size_t)n_hops * (size_t)row_len * sizeof(double));
+	int *samples = (int *)malloc((size_t)n_hops * sizeof(int));
+	char *row = (char *)malloc(64 + 16 * ((size_t)N + 8));
+	const char *hook = getenv("RXB200_MAX_SWEEPS");       /* test hook: report after this many sweeps and exit */
+	const long max_sweeps = hook ? atol(hook) : 0;
+	long sweeps = 0;
+	time_t next_tick = time(NULL) + interval, exit_time = exit_after ? time(NULL) + exit_after : 0;
+	int done = 0, rc = 0;
+	while (!done && !g_stop) {
+		/* ---- one pass: M * buf_len int16 from as many reads as it takes */
+		size_t have = 0;
+		int fails = 0, dry = 0;
+		while (have < pass16 && !g_stop) {
+			void *bp[] = {pass + have};
+			int flags = 0; long long tn = 0;
+			const int r = SoapySDRDevice_readStream(dev, stream, bp, (pass16 - have) / 2, &flags, &tn, 1000000);
+			if (r < 0) {
+				fprintf(stderr, "Error: reading stream %d\n", r);
+				have = 0;                                         /* the partial pass is not continuous with the next read */
+				if (++fails >= tuner_retry_max) { dry = 1; break; }
+				continue;
+			}
+			fails = 0;
+			have += 2 * (size_t)r;
+		}
+		if (have == pass16) {
+			if (rxb200_power_mix_accumulate(pm, pass, pass16) != RXB200_OK) { fprintf(stderr, "rxb200: %s\n", rxb200_last_error()); rc = 1; break; }
+			sweeps++;
+		}
+		time_t now = time(NULL);
+		const int hooked = max_sweeps && sweeps >= max_sweeps;
+		if (now < next_tick && !hooked && !dry) { continue; }
+		char tstr[50];
+		time_string(tstr, sizeof tstr, now);
+		if (report(out, pw, plan, db, row_len, samples, row, 64 + 16 * ((size_t)N + 8), tstr) != 0) { rc = 1; break; }
+		rxb200_power_reset(pw);                               /* the accumulators only: the capture stream goes on */
+		while (time(NULL) >= next_tick) { next_tick += interval; }
+		if (single || hooked || dry) { done = 1; }
+		if (exit_time && time(NULL) >= exit_time) { done = 1; }
+	}
+	fprintf(stderr, g_stop ? "\nUser cancel, exiting...\n" : "\nDone, exiting...\n");
+	if (out != stdout) { fclose(out); }
+	free(pass); free(db); free(samples); free(row);
+	sdr_close(dev, stream);
+	return rc;
 }
 
 int main(int argc, char **argv)
@@ -112,6 +234,37 @@ int main(int argc, char **argv)
 	int n_gpus = getenv("RXB200_GPUS") ? atoi(getenv("RXB200_GPUS")) : 1;
 	if (n_gpus < 1) { n_gpus = 1; }
 	if (n_gpus > n_hops) { n_gpus = n_hops; }
+	const char *cap_env = getenv("RXB200_CAPTURE_RATE");
+	if (cap_env) {
+		/* capture mode: centre of the hops, each hop's offset from it, the smallest M whose capture holds them all */
+		if (n_gpus > 1) { fprintf(stderr, "Capture mode (RXB200_CAPTURE_RATE) runs on one GPU: unset RXB200_GPUS.\n"); return 1; }
+		const long long cap_max = atoll(cap_env), rate = plan.rate;
+		const int64_t fc = plan.first_freq + ((int64_t)(n_hops - 1) * plan.freq_step) / 2;
+		int *offs = (int *)malloc(sizeof(int) * (size_t)n_hops);
+		long long span = 0;
+		for (int i = 0; i < n_hops; i++) {
+			const long long f = (long long)(plan.first_freq + (int64_t)i * plan.freq_step - fc);
+			if (2 * (f < 0 ? -f : f) > span) { span = 2 * (f < 0 ? -f : f); }
+			offs[i] = (int)f;
+		}
+		const long long M = (span + rate + rate - 1) / rate, R = M * rate;
+		if (R > cap_max || R > 2147483647LL || M > 4096) {
+			fprintf(stderr, "Capture mode: the span needs a capture rate of %lld Hz, above RXB200_CAPTURE_RATE=%s.\n", R, cap_env);
+			return 1;
+		}
+		const int T = M * 32 + 1 < 8191 ? (int)M * 32 + 1 : 8191;
+		int32_t *taps = (int32_t *)malloc(sizeof(int32_t) * (size_t)T);
+		rxb200_ddc_lowpass((int)M, T, 15, taps);
+		fprintf(stderr, "Capture mode: %lld Hz centred at %lli Hz, decimation %lld, %d taps\n", R, (long long)fc, M, T);
+		const rxb200_ddc ddc = {(int)M, T, taps, 15};
+		rxb200_power_mix *pm = NULL;
+		if (rxb200_power_mix_create(pp, window_coefs, NULL, (int)R, offs, &ddc, 0, &pm) != RXB200_OK) { fprintf(stderr, "rxb200: %s\n", rxb200_last_error()); return 1; }
+		free(offs); free(taps);
+		const int rc = capture_mode(pm, &plan, (int)R, fc, (int)M, dev_query, channel, gain_str, antenna, filename, ppm,
+		                            direct_sampling, offset_tuning, tuner_sleep_usec, tuner_retry_max, interval, single, exit_after);
+		rxb200_power_mix_destroy(pm);
+		return rc;
+	}
 	rxb200_power_group *grp = NULL;
 	if (rxb200_power_group_create(pp, window_coefs, NULL, n_gpus, NULL, &grp) != RXB200_OK) { fprintf(stderr, "rxb200: %s\n", rxb200_last_error()); return 1; }
 	rxb200_power *pw = rxb200_power_group_member(grp, 0);     /* after the gather member 0 holds every row */
@@ -187,24 +340,10 @@ int main(int argc, char **argv)
 		const int hooked = max_sweeps && sweeps >= max_sweeps;
 		if (now < next_tick && !hooked && !stream_dry) { continue; }
 		/* ---- report (:1044-1058) */
-		struct tm cal; char tstr[50];
-		localtime_r(&now, &cal);
-		strftime(tstr, sizeof tstr, "%Y-%m-%d, %H:%M:%S", &cal);
-		if (getenv("RXB200_FIXED_TIME")) { snprintf(tstr, sizeof tstr, "%s", getenv("RXB200_FIXED_TIME")); }
+		char tstr[50];
+		time_string(tstr, sizeof tstr, now);
 		if (rxb200_power_group_gather(grp) != RXB200_OK) { fprintf(stderr, "rxb200: %s\n", rxb200_last_error()); break; }
-		if (rxb200_power_read_db(pw, plan.rate, plan.crop, db, (size_t)row_len, samples) != RXB200_OK) { fprintf(stderr, "rxb200: %s\n", rxb200_last_error()); break; }
-		int have = 0;
-		for (int i = 0; i < n_hops; i++) { have |= samples[i]; }
-		if (have) {
-			for (int i = 0; i < n_hops; i++) {
-				int n = rxb200_power_format_db_row(db + (size_t)i * row_len, pp->bin_e, plan.first_freq + (int64_t)i * plan.freq_step, plan.rate,
-				                                pp->downsample, plan.crop, samples[i], row, 64 + 16 * ((size_t)N + 8));
-				if (n < 0) { fprintf(stderr, "rxb200: %s\n", rxb200_last_error()); break; }
-				fprintf(out, "%s, ", tstr);
-				fwrite(row, 1, (size_t)n, out);
-			}
-			fflush(out);
-		}
+		if (report(out, pw, &plan, db, row_len, samples, row, 64 + 16 * ((size_t)N + 8), tstr) != 0) { break; }
 		rxb200_power_group_reset(grp);
 		while (time(NULL) >= next_tick) { next_tick += interval; }
 		if (single || hooked || stream_dry) { done = 1; }

@@ -550,6 +550,61 @@ int rxb200_fm_mix_group_levels(rxb200_fm_mix_group *g, int *levels, size_t cap, 
 /* every member's phases back to 0 and its chain back to the state right after create */
 int rxb200_fm_mix_group_reset(rxb200_fm_mix_group *g);
 
+/* ======================================================================== rx_power hops of one capture
+ * Every hop of a sweep from ONE wideband CS16 capture, instead of a retune and a read per hop (DESIGN.md section 4.5).
+ * A power mixing handle has a capture rate R (Hz, > 0), one integer offset f_i per hop with |f_i| < R/2, one rxb200_ddc
+ * (M, T taps h, shift S; the ranges of rxb200_fm_mix_create_ddc) and the rxb200_power_params, window and sine table of
+ * rxb200_power_create.
+ * NCO.  Frequency word w_i = floor((f_i 2^32 + floor(R/2)) / R) mod 2^32, exact in 64-bit integers (floor, also for
+ * negative f).  Capture sample n, counted from create or reset across calls, has phase theta = n w_i mod 2^32 and table
+ * index j = ((theta + 2^15) mod 2^32) >> 16.  One shared table of 2^16 entries (rxb200_nco_table) holds
+ * (c_j, s_j) = ((int)round(32768 cos t), (int)round(32768 sin t)), t = -2 pi j' / 65536 in fp64, j' the representative
+ * of j in (-32768, 32768], so the entries of j and 65536 - j are exact conjugates.  Mixing is the rx_fm mixer's rule:
+ *     I' = (int16)((I c - Q s + 2^14) >> 15),  Q' = (int16)((I s + Q c + 2^14) >> 15)   (arithmetic shift, int16 wrap).
+ * f = 0 is the identity, f = +-R/4 with 4 | R an exact quarter turn; no period limit, and the frequency error is at
+ * most R / 2^33.
+ * Filter.  z_i = mix_i(x), z_i[n] = 0 for n < 0.  Output m is emitted at e_m = m M + M - 1:
+ *     A = sum_{j<T} h[j] z_i[e_m - j] (exact);  y = S ? (A + 2^(S-1)) >> S : A;  saturated to int16
+ * (the rule of rxb200_fm_mix_create_ddc word for word).
+ * Passes.  With B = buf_len / 2, outputs [p B, (p+1) B) of hop i are hop i's buffer in pass p, counted from create or
+ * reset.  A call must cover whole passes: n_int16 a multiple of M * buf_len (else RXB200_EUNSUPPORTED, and nothing
+ * changes); n_int16 == 0 is a no-op.  A call of P passes accumulates exactly what
+ * rxb200_power_accumulate(member, bufs, P, 0, n_hops) would with bufs[p][i] = pass p of hop i.  power_ddc_kernel writes
+ * those buffers pass-major into a scratch buffer of the handle, which a long call fills in groups of passes of at most
+ * RXB200_POWER_MIX_SCRATCH_BYTES (at least one pass per group); the bytes are the same as with one group. */
+#define RXB200_POWER_MIX_SCRATCH_BYTES (64u << 20)
+typedef struct rxb200_power_mix rxb200_power_mix;
+/* Refusals, all before any device is touched: those of rxb200_power_create for the params; RXB200_EINVAL for NULL
+ * offsets, R <= 0 or any |f_i| >= R/2; those of rxb200_fm_mix_create_ddc for the ddc. */
+int rxb200_power_mix_create(const rxb200_power_params *params, const int *window_coefs, const int16_t *sinewave,
+                            int capture_rate, const int *offsets_hz /* n_hops */, const rxb200_ddc *ddc,
+                            int device, rxb200_power_mix **out);
+void rxb200_power_mix_destroy(rxb200_power_mix *m);
+/* The inner rxb200_power handle, for rxb200_power_read / _read_db / _reset / _last_path / _kernel_ms / _stream (the DDC
+ * runs on its stream).  rxb200_power_reset on it zeroes only the accumulators (csv_dbm's side effect): the phases and
+ * the filter history carry on, since a capture stream is continuous across reports. */
+rxb200_power *rxb200_power_mix_member(rxb200_power_mix *m);
+/* Back to the state right after create: phases, filter history, pass count and accumulators. */
+int rxb200_power_mix_reset(rxb200_power_mix *m);
+/* cs16: HOST pointer to n_int16 int16 of the capture. */
+int rxb200_power_mix_accumulate(rxb200_power_mix *m, const int16_t *cs16, size_t n_int16);
+/* Same with a DEVICE capture (4-byte aligned), asynchronous on the member's stream unless sync != 0. */
+int rxb200_power_mix_accumulate_device(rxb200_power_mix *m, const int16_t *d_cs16, size_t n_int16, int sync);
+/* Device time (CUDA events on the member's stream) of the DDC launches of the last call, summed, in milliseconds;
+ * synchronises. */
+int rxb200_power_mix_kernel_ms(rxb200_power_mix *m, float *ms);
+/* The NCO table: 2 * 65536 int32, (c, s) pairs. */
+int rxb200_nco_table(int32_t *table);
+/* The DDC alone on DEVICE pointers, stateless, on `stream`: the samples before d_src are zero, d_src[i] is capture
+ * sample n0 + i for the NCO of (R, f), and floor(n_complex / M) outputs go to d_dst, e_m counted from d_src.  Both
+ * pointers 4-byte aligned.  Asynchronous. */
+int rxb200_power_ddc_device(int capture_rate, int offset_hz, unsigned long long n0, const rxb200_ddc *ddc,
+                            const int16_t *d_src, size_t n_complex, int16_t *d_dst, void *stream);
+/* The channel filter the rx_power shell's capture mode uses: a Blackman-windowed sinc with cutoff 1/(2M) cycles per
+ * sample over T taps (odd, 1..8191), quantised to round(2^shift g_j / sum g) (shift 0..30) with the centre tap
+ * corrected so that sum h = 2^shift exactly.  Pure host arithmetic. */
+int rxb200_ddc_lowpass(int decim, int n_taps, int shift, int32_t *taps);
+
 /* ======================================================================== rx_sdr (SURVEY.md §8f row 4)
  * The pointwise sample-format conversions of rx_sdr's recorder loop (src/rtl_sdr.c:348-391):
  *   RXB200_CVT_CS16_CS8  : (uint8_t)(int)(x/32767.0*128.0+0.4)       per int16 (:367-370)

@@ -10,12 +10,12 @@
 #include <new>
 #include <vector>
 #include "common.cuh"
+#include "ddc.cuh"
 
 namespace rxb {
 
 #define MIX_THREADS 256
 #define MIX_UNIT 8                   // complex samples per thread and trip: 32 bytes of capture
-#define MIX_GROUP 256                // channels per grid row (blockIdx.y): the capture is read once per group
 #define MIX_SMEM_MAX (96 * 1024)     // the largest table range a CTA stages in shared memory; beyond, reads go through L1
 
 struct MixChan {
@@ -24,15 +24,6 @@ struct MixChan {
 	unsigned m;      // floor((2^32 - 1) / L): t mod L for t < 2^21 with one multiply-high and one correction
 	int pad;
 };
-
-// one complex sample through the mixer: (I + jQ)(c + js) in Q15, rounded, arithmetic shift, int16 wrap
-__device__ __forceinline__ uint32_t mix_one(uint32_t w, int2 cs)
-{
-	const int I = (int)(int16_t)(w & 0xffffu), Q = (int)(int16_t)(w >> 16);
-	const int i2 = (I * cs.x - Q * cs.y + 16384) >> 15;      // |x| |(c, s)| sqrt(2) < 2^31: no overflow
-	const int q2 = (I * cs.y + Q * cs.x + 16384) >> 15;
-	return ((uint32_t)i2 & 0xffffu) | ((uint32_t)q2 << 16);
-}
 
 // Grid-stride over units of MIX_UNIT complex samples: each thread loads its unit once, then writes it mixed with every
 // channel of its group.  Stream row c of dst is dst + c*dst_stride; sample n of the call uses entry (pos + n) mod L of
@@ -153,10 +144,6 @@ static int mix_table(int capture_rate, int offset_hz, std::vector<int32_t> &t, s
 }
 
 // ---- the decimating down-converter (rxb200_fm_mix_create_ddc, rxb200_ddc_device)
-#define DDC_THREADS 256
-#define DDC_SPAN 8192                // capture samples a CTA stages at most (T <= 8192: one output always fits)
-#define DDC_REACH (1 << 20)          // capture samples a CTA's span covers at most: table offsets stay below 2^21
-
 struct DdcArgs {
 	const uint32_t *src;             // the call's capture, one word per complex sample
 	const uint32_t *hist;            // the T - 1 raw capture samples before src
@@ -174,24 +161,6 @@ struct DdcArgs {
 	int U;                           // outputs per CTA
 	int lpo;                         // lanes per output (a power of two <= 32)
 };
-
-// staged sample s -> its offset from the CTA's first staged sample: windows of T samples, M apart, stored ws apart
-__device__ __forceinline__ int ddc_off(int s, const DdcArgs &a)
-{
-	unsigned q = __umulhi((unsigned)s, a.ws_m);
-	int r = s - (int)q * a.ws;
-	if (r >= a.ws) { q++; r -= a.ws; }
-	return (int)q * a.M + r;
-}
-
-// one output: y = S == 0 ? A : (A + 2^(S-1)) >> S (arithmetic), saturated to int16
-template <typename Acc>
-__device__ __forceinline__ int ddc_out(Acc acc, int S)
-{
-	long long y = (long long)acc;
-	if (S) { y = (y + (1ll << (S - 1))) >> S; }
-	return (int)(y < -32768 ? -32768 : (y > 32767 ? 32767 : y));
-}
 
 // One CTA: U consecutive outputs of every channel of its grid row (up to 256 channels, blockIdx.y).  It stages the
 // capture samples its outputs' windows cover once (the handle's history before the call's first sample), then per
@@ -267,24 +236,15 @@ __global__ void __launch_bounds__(DDC_THREADS) fm_ddc_kernel(const DdcArgs a)
 // Launches fm_ddc_kernel on the current device for a.n_out > 0 outputs per channel; fills a's launch shape
 static int ddc_launch(DdcArgs a, bool wide, cudaStream_t st)
 {
-	const int T = a.T, M = a.M;
-	a.ws = T >= M ? M : T;
-	a.ws_m = 0xffffffffu / (unsigned)a.ws;
-	a.lpo = 1;
-	while (a.lpo < 32 && a.lpo < T) { a.lpo <<= 1; }
 	const int groups = (a.n_ch + MIX_GROUP - 1) / MIX_GROUP;
-	int dev = 0, n_sm = 0;
-	RXB_CUDA(cudaGetDevice(&dev));
-	RXB_CUDA(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
-	// as many outputs per CTA as the staging room and the reach allow, but at least two CTAs per SM when there is work
-	long long U = std::min((long long)(DDC_SPAN - T) / a.ws, (long long)(DDC_REACH - T) / M) + 1;
-	const long long ctas = std::max(1ll, (2ll * n_sm + groups - 1) / groups);
-	U = std::max(1ll, std::min(U, (a.n_out + ctas - 1) / ctas));
-	a.U = (int)U;
-	const size_t smem = ((size_t)T + 2 * ((size_t)(a.U - 1) * a.ws + T)) * sizeof(uint32_t);
+	DdcShape sh;
+	size_t smem = 0;
+	long long bx = 0;
+	const int rc = ddc_shape(a.M, a.T, a.n_out, groups, &sh, &smem, &bx);
+	if (rc != RXB200_OK) { return rc; }
+	a.ws = sh.ws; a.ws_m = sh.ws_m; a.U = sh.U; a.lpo = sh.lpo;
 	void (*kern)(const DdcArgs) = wide ? fm_ddc_kernel<long long> : fm_ddc_kernel<int>;
 	RXB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-	const long long bx = (a.n_out + U - 1) / U;
 	kern<<<dim3((unsigned)bx, (unsigned)groups), DDC_THREADS, smem, st>>>(a);
 	RXB_CUDA(cudaGetLastError());
 	return RXB200_OK;

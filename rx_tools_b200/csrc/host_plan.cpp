@@ -8,6 +8,7 @@
 #include <stdarg.h>
 #include <stdio.h>
 #include <string.h>
+#include <vector>
 #include <cuda_runtime.h>
 #include "../../include/rxb200.h"
 
@@ -110,6 +111,37 @@ extern "C" int rxb200_fm_mix_table(int capture_rate, int offset_hz, int32_t *tab
 		table[2 * m] = (int32_t)round(32768.0 * cos(t));
 		table[2 * m + 1] = (int32_t)round(32768.0 * sin(t));
 	}
+	return RXB200_OK;
+}
+
+// The channel filter of rx_power's capture mode (include/rxb200.h, "rx_power hops of one capture"): a Blackman-windowed
+// sinc with its cutoff at 1/(2M) cycles per sample, quantised to 2^shift / sum(g) and the rounding error put on the
+// centre tap, so that the DC gain is 2^shift exactly.
+extern "C" int rxb200_ddc_lowpass(int decim, int n_taps, int shift, int32_t *taps)
+{
+	if (!taps) { set_error("null argument"); return RXB200_EINVAL; }
+	if (decim < 1 || decim > 4096 || n_taps < 1 || n_taps > 8191 || n_taps % 2 == 0 || shift < 0 || shift > 30) {
+		set_error("lowpass decim %d, n_taps %d, shift %d: need 1 <= decim <= 4096, odd 1 <= n_taps <= 8191, 0 <= shift <= 30",
+		          decim, n_taps, shift);
+		return RXB200_EINVAL;
+	}
+	const int c = (n_taps - 1) / 2;
+	double sum = 0.0;
+	std::vector<double> g((size_t)n_taps);
+	for (int j = 0; j < n_taps; j++) {
+		const double x = (double)(j - c) / (double)decim;           // 2 * cutoff * (j - c)
+		const double s = j == c ? 1.0 : sin(M_PI * x) / (M_PI * x);
+		const double a = n_taps == 1 ? 0.0 : 2.0 * M_PI * (double)j / (double)(n_taps - 1);
+		g[j] = s * (n_taps == 1 ? 1.0 : 0.42 - 0.5 * cos(a) + 0.08 * cos(2.0 * a));
+		sum += g[j];
+	}
+	const double unity = (double)(1ll << shift);
+	long long q = 0;
+	for (int j = 0; j < n_taps; j++) {
+		taps[j] = (int32_t)llround(unity * g[j] / sum);
+		q += taps[j];
+	}
+	taps[c] += (int32_t)((1ll << shift) - q);
 	return RXB200_OK;
 }
 

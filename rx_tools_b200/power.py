@@ -3,7 +3,8 @@
 ``plan_range`` is ``frequency_range()`` (:431-543), ``window_table``/``sine_table`` are the tables
 ``main()`` builds (:1028, :1034-1037), ``PowerScanner.scanner`` is n passes of ``scanner()`` (:670-772)
 over hop buffers, executed by the batched sm_90a kernel behind ``rxb200_power_accumulate``
-(include/rxb200.h); ``csv_rows`` is ``csv_dbm()`` (:774-817).
+(include/rxb200.h); ``csv_rows`` is ``csv_dbm()`` (:774-817).  ``PowerMix`` takes every hop of a sweep from one
+wideband capture through an NCO down-converter on the GPU (``rxb200_power_mix_*``).
 """
 from __future__ import annotations
 
@@ -14,6 +15,7 @@ from typing import Optional, Sequence
 import numpy as np
 
 from . import _lib
+from .fm import _ddc_c
 
 WINDOWS = {"rectangle": 0, "hamming": 1, "blackman": 2, "blackman-harris": 3, "hann-poisson": 4,
            "youssef": 5, "kaiser": 6, "bartlett": 7, "hann": 8}
@@ -186,6 +188,93 @@ def csv_rows(plan: Plan, avg: np.ndarray, samples: np.ndarray, tstr: str = "2026
                                                           int(samples[i]), buf, len(buf)))
         lines.append(tstr + ", " + buf.raw[:r].decode())
     return "".join(lines)
+
+
+class PowerMix(PowerScanner):
+    """Every hop of a sweep from ONE wideband capture (``rxb200_power_mix_*``): hop i is the capture mixed down by
+    offsets_hz[i] with a phase-accumulator NCO, filtered and decimated by ddc = (M, taps, S), and every buf_len / 2
+    outputs of it are one hop buffer of the inner rx_power handle (the member).  read, read_db, csv_rows_device and
+    last_path are the member's; reset() brings the whole handle back to create, reset_accumulators() zeroes only the
+    accumulators (the phases and the filter history carry on, as across the reports of a continuous capture)."""
+
+    def __init__(self, plan: Plan, capture_rate: int, offsets_hz: Sequence[int], ddc,
+                 window: Sequence[int] | str = "rectangle", device: int = 0, sinewave: Optional[np.ndarray] = None):
+        self.plan = plan
+        n = 1 << plan.bin_e
+        self.window = window_table(window, n) if isinstance(window, str) else np.ascontiguousarray(window, np.int32)
+        assert self.window.size == n
+        self.capture_rate, self.ddc = int(capture_rate), ddc
+        self.offsets = np.ascontiguousarray(offsets_hz, dtype=np.int32)
+        assert self.offsets.size == plan.n_hops
+        self._m = C.c_void_p()
+        pc = plan.to_c()
+        d, _t = _ddc_c(ddc)
+        sw = None if sinewave is None else np.ascontiguousarray(sinewave, np.int16).ctypes.data_as(C.POINTER(C.c_int16))
+        _lib.check(_lib.lib().rxb200_power_mix_create(C.byref(pc), self.window.ctypes.data_as(C.POINTER(C.c_int)), sw,
+                                                      self.capture_rate,
+                                                      self.offsets.ctypes.data_as(C.POINTER(C.c_int)), C.byref(d),
+                                                      device, C.byref(self._m)))
+        self._h = C.c_void_p(_lib.lib().rxb200_power_mix_member(self._m))
+
+    def close(self) -> None:
+        if _lib is not None and getattr(self, "_m", None) is not None and self._m:
+            _lib.lib().rxb200_power_mix_destroy(self._m)
+            self._m = None
+            self._h = None
+
+    __del__ = close
+
+    @property
+    def pass_int16(self) -> int:
+        """Capture int16 per pass: decim * buf_len."""
+        return int(self.ddc[0]) * self.plan.buf_len
+
+    def accumulate(self, capture: np.ndarray) -> None:
+        """capture: int16 CS16 (host), a whole number of passes."""
+        x = np.ascontiguousarray(capture, dtype=np.int16).reshape(-1)
+        _lib.check(_lib.lib().rxb200_power_mix_accumulate(self._m, x.ctypes.data, x.size))
+
+    def accumulate_device(self, d_ptr: int, n_int16: int, sync: bool = False) -> None:
+        _lib.check(_lib.lib().rxb200_power_mix_accumulate_device(self._m, d_ptr, n_int16, 1 if sync else 0))
+
+    def reset(self) -> None:
+        _lib.check(_lib.lib().rxb200_power_mix_reset(self._m))
+
+    def reset_accumulators(self) -> None:
+        _lib.check(_lib.lib().rxb200_power_reset(self._h))
+
+    def kernel_ms(self) -> float:
+        """Device time of the last call's DDC launches (ms)."""
+        ms = C.c_float(0)
+        _lib.check(_lib.lib().rxb200_power_mix_kernel_ms(self._m, C.byref(ms)))
+        return float(ms.value)
+
+    def accumulate_ms(self) -> float:
+        """Device time of the member's last accumulate kernel (ms)."""
+        return PowerScanner.kernel_ms(self)
+
+
+def nco_table() -> np.ndarray:
+    """The NCO table (``rxb200_nco_table``): int32[65536][2] of (c, s)."""
+    t = np.empty((65536, 2), dtype=np.int32)
+    _lib.check(_lib.lib().rxb200_nco_table(t.ctypes.data_as(C.POINTER(C.c_int32))))
+    return t
+
+
+def ddc_lowpass(decim: int, n_taps: int, shift: int) -> np.ndarray:
+    """The capture mode's channel filter (``rxb200_ddc_lowpass``): int32[n_taps] summing to 2^shift."""
+    t = np.empty(n_taps, dtype=np.int32)
+    _lib.check(_lib.lib().rxb200_ddc_lowpass(decim, n_taps, shift, t.ctypes.data_as(C.POINTER(C.c_int32))))
+    return t
+
+
+def power_ddc_device(capture_rate: int, offset_hz: int, n0: int, ddc, d_src_ptr: int, n_complex: int, d_dst_ptr: int,
+                     stream: int = 0) -> None:
+    """The NCO down-converter alone on device pointers (``rxb200_power_ddc_device``), asynchronous on ``stream``: zero
+    samples before d_src, d_src[i] is capture sample n0 + i, floor(n_complex / decim) outputs.  ddc: (decim, taps, S)."""
+    d, _t = _ddc_c(ddc)
+    _lib.check(_lib.lib().rxb200_power_ddc_device(capture_rate, offset_hz, n0, C.byref(d), d_src_ptr, n_complex,
+                                                  d_dst_ptr, stream or None))
 
 
 def shard(n_hops: int, n_ranks: int, rank: int):
