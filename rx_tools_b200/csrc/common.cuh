@@ -17,8 +17,8 @@ void set_error(const char *fmt, ...);
 int fm_check_host_call(rxb200_fm *h, const int16_t *cs16, size_t n_int16, size_t chunk_int16, int16_t *pcm,
                        size_t pcm_stride, int *chunk_result_len, size_t *n_pcm, bool read, size_t *total);
 // fm_mix.cu: the same for a mixing handle's call, on the shape its member will see (the decimated one for a handle of
-// rxb200_fm_mix_create_ddc), *n16 and *chunk16 receiving that shape; and the refusals of an rxb200_ddc, *wide receiving
-// whether its kernel accumulates in 64 bits
+// rxb200_fm_mix_create_ddc), *n16 and *chunk16 receiving that shape; and (ddc.cu) the refusals of an rxb200_ddc, *wide
+// receiving whether its kernel accumulates in 64 bits
 int fm_mix_check_host_call(rxb200_fm_mix *m, const int16_t *cs16, size_t n_int16, size_t chunk_int16, int16_t *pcm,
                            size_t pcm_stride, int *chunk_result_len, size_t *n_pcm, bool read, size_t *total,
                            size_t *n16, size_t *chunk16);

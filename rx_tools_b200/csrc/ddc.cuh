@@ -1,9 +1,13 @@
-// ddc.cuh — the pieces the two digital down-converters share: fm_ddc_kernel (fm_mix.cu: rx_fm channels, each mixed
+// ddc.cuh — the digital down-converter both mixing handles run: fm_ddc_kernel (fm_mix.cu: rx_fm channels, each mixed
 // with its integer table) and power_ddc_kernel (power_mix.cu: rx_power hops, each mixed with a phase-accumulator NCO).
-// Both stage the capture samples their outputs' windows cover, mix them per channel into shared memory with mix_one,
-// and run the T-tap dot product at the emission points only; they differ in the mixer index and the output address.
+// Both kernels are ddc_body with their mixer policy: it stages the capture samples its outputs' windows cover, mixes
+// them per channel into shared memory with mix_one, and runs the T-tap dot product at the emission points only; the
+// policy supplies the mixer index and the output address, the two things they differ in.  The host side they share is
+// here too (the launch, the filter state a handle carries between calls) and in ddc.cu (the argument check, the
+// stateless entries' upload).
 #pragma once
 #include <algorithm>
+#include <vector>
 #include "common.cuh"
 
 namespace rxb {
@@ -22,13 +26,22 @@ __device__ __forceinline__ uint32_t mix_one(uint32_t w, int2 cs)
 	return ((uint32_t)i2 & 0xffffu) | ((uint32_t)q2 << 16);
 }
 
-// The launch shape both kernels take: a.ws staged samples between two outputs' windows (M when T >= M, else T),
-// a.ws_m = floor((2^32 - 1) / ws), a.lpo lanes per output (a power of two <= 32) and a.U outputs per CTA.
-struct DdcShape {
-	int ws;
-	unsigned ws_m;
-	int U;
-	int lpo;
+// The arguments of one DDC launch: the fields every DDC takes, then the mixer policy's own (Mix).
+template <typename Mix>
+struct DdcArgs {
+	const uint32_t *src;             // the call's capture, one word per complex sample
+	const uint32_t *hist;            // the T - 1 raw capture samples before src
+	long long n_out;                 // outputs per channel
+	long long r0;                    // src index of the first emission point
+	unsigned long long pos;          // the mixer's position (capture sample index) of src[0]
+	uint32_t *dst;                   // one word per output, at the address Mix gives
+	const int32_t *taps;             // reversed: taps[t] = h[T - 1 - t]
+	int n_ch, M, T, S;
+	int ws;                          // staged samples between two outputs' windows: M when T >= M, else T
+	unsigned ws_m;                   // floor((2^32 - 1) / ws)
+	int U;                           // outputs per CTA
+	int lpo;                         // lanes per output (a power of two <= 32)
+	Mix mix;
 };
 
 // staged sample s -> its offset from the CTA's first staged sample: windows of T samples, M apart, stored ws apart
@@ -50,25 +63,157 @@ __device__ __forceinline__ int ddc_out(Acc acc, int S)
 	return (int)(y < -32768 ? -32768 : (y > 32767 ? 32767 : y));
 }
 
-// The shape of a launch of n_out > 0 outputs per channel over `groups` grid rows on the current device; *smem receives
-// the dynamic shared memory (the reversed taps, the staged and the mixed span) and *bx the CTAs per grid row.
-static inline int ddc_shape(int M, int T, long long n_out, int groups, DdcShape *s, size_t *smem, long long *bx)
+// One CTA: U consecutive outputs of every channel of its grid row (up to 256 channels, blockIdx.y).  It stages the
+// capture samples its outputs' windows cover once (the history before the call's first sample), then per channel mixes
+// them into shared memory and runs the T-tap dot product at the emission points only, lpo lanes per output.  Acc: int
+// when sum |h| * 32768 + 2^(S-1) < 2^31, else long long (no partial sum can overflow either way).  The mixer policy:
+//   typename Mix::Row row(a, c0, nc, u0, g0)   the grid row's set-up, g0 the first staged sample's mixer position
+//   row.chan(c)                                 takes channel c's mixer state
+//   row.entry(off)                              the channel's table entry for the staged sample at offset off
+//   row.out(u)                                  the address of the channel's call output u
+template <typename Acc, typename Mix>
+__device__ __forceinline__ void ddc_body(const DdcArgs<Mix> &a)
 {
-	s->ws = T >= M ? M : T;
-	s->ws_m = 0xffffffffu / (unsigned)s->ws;
-	s->lpo = 1;
-	while (s->lpo < 32 && s->lpo < T) { s->lpo <<= 1; }
+	extern __shared__ int4 ddc_smem[];
+	const int T = a.T;
+	const int room = (a.U - 1) * a.ws + T;
+	int32_t *s_h = reinterpret_cast<int32_t *>(ddc_smem);
+	uint32_t *s_x = reinterpret_cast<uint32_t *>(s_h + T);
+	uint32_t *s_z = s_x + room;
+	const int c0 = (int)blockIdx.y * MIX_GROUP;
+	const int nc = min(MIX_GROUP, a.n_ch - c0);
+	const long long u0 = (long long)blockIdx.x * a.U;
+	const int U = (int)min((long long)a.U, a.n_out - u0);
+	const int n = (U - 1) * a.ws + T;
+	const long long b0 = u0 * a.M + a.r0 - (T - 1);       // src index of the first staged sample, >= -(T - 1)
+	const long long g0 = (long long)a.pos + b0;            // its mixer position
+	for (int j = threadIdx.x; j < T; j += blockDim.x) { s_h[j] = a.taps[j]; }
+	typename Mix::Row row(a, c0, nc, u0, g0);
+	for (int s = threadIdx.x; s < n; s += blockDim.x) {
+		const long long i = b0 + ddc_off(s, a);
+		s_x[s] = i >= 0 ? __ldg(a.src + i) : a.hist[(T - 1) + i];
+	}
+	__syncthreads();
+	const int lane = (int)threadIdx.x & (a.lpo - 1), sub = (int)threadIdx.x / a.lpo, n_sub = (int)blockDim.x / a.lpo;
+	for (int c = 0; c < nc; c++) {
+		row.chan(c);
+		for (int s = threadIdx.x; s < n; s += blockDim.x) {
+			const int2 *e = row.entry(ddc_off(s, a));
+			s_z[s] = mix_one(s_x[s], __ldg(e));
+		}
+		__syncthreads();
+		for (int ub = 0; ub < U; ub += n_sub) {                  // the same trip count on every lane of a warp
+			const int u = ub + sub;
+			Acc ai = 0, aq = 0;
+			if (u < U) {
+				const uint32_t *z = s_z + u * a.ws;
+				for (int j = lane; j < T; j += a.lpo) {
+					const uint32_t w = z[j];
+					const Acc h = (Acc)s_h[j];
+					ai += h * (Acc)(int16_t)(w & 0xffffu);
+					aq += h * (Acc)(int16_t)(w >> 16);
+				}
+			}
+			for (int o = a.lpo >> 1; o > 0; o >>= 1) {
+				ai += __shfl_xor_sync(0xffffffffu, ai, o);
+				aq += __shfl_xor_sync(0xffffffffu, aq, o);
+			}
+			if (u < U && lane == 0) {
+				*row.out(u) = ((uint32_t)ddc_out(ai, a.S) & 0xffffu) | ((uint32_t)ddc_out(aq, a.S) << 16);
+			}
+		}
+		__syncthreads();                    // every output of this channel is made before s_z is overwritten
+	}
+}
+
+// Launches kern (a DDC kernel) on the current device for a.n_out > 0 outputs per channel, with its launch shape: a.ws,
+// a.ws_m, a.lpo, and as many outputs per CTA (a.U) as the staging room and the reach allow, but at least two CTAs per
+// SM when there is work.  The dynamic shared memory holds the reversed taps, the staged and the mixed span.
+template <typename Mix>
+int ddc_launch(DdcArgs<Mix> a, void (*kern)(DdcArgs<Mix>), cudaStream_t st)
+{
+	const int groups = (a.n_ch + MIX_GROUP - 1) / MIX_GROUP;
+	a.ws = a.T >= a.M ? a.M : a.T;
+	a.ws_m = 0xffffffffu / (unsigned)a.ws;
+	a.lpo = 1;
+	while (a.lpo < 32 && a.lpo < a.T) { a.lpo <<= 1; }
 	int dev = 0, n_sm = 0;
 	RXB_CUDA(cudaGetDevice(&dev));
 	RXB_CUDA(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
-	// as many outputs per CTA as the staging room and the reach allow, but at least two CTAs per SM when there is work
-	long long U = std::min((long long)(DDC_SPAN - T) / s->ws, (long long)(DDC_REACH - T) / M) + 1;
+	long long U = std::min((long long)(DDC_SPAN - a.T) / a.ws, (long long)(DDC_REACH - a.T) / a.M) + 1;
 	const long long ctas = std::max(1ll, (2ll * n_sm + groups - 1) / groups);
-	U = std::max(1ll, std::min(U, (n_out + ctas - 1) / ctas));
-	s->U = (int)U;
-	*smem = ((size_t)T + 2 * ((size_t)(s->U - 1) * s->ws + T)) * sizeof(uint32_t);
-	*bx = (n_out + U - 1) / U;
+	U = std::max(1ll, std::min(U, (a.n_out + ctas - 1) / ctas));
+	a.U = (int)U;
+	const size_t smem = ((size_t)a.T + 2 * ((size_t)(a.U - 1) * a.ws + a.T)) * sizeof(uint32_t);
+	const long long bx = (a.n_out + U - 1) / U;
+	RXB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+	kern<<<dim3((unsigned)bx, (unsigned)groups), DDC_THREADS, smem, st>>>(a);
+	RXB_CUDA(cudaGetLastError());
 	return RXB200_OK;
 }
+
+// The filter state a mixing handle carries between calls (the rule of include/rxb200.h's rxb200_ddc): M, T and S, the
+// reversed taps, and the raw capture's last T - 1 samples before the handle's position (zero before create or reset,
+// which is exactly the rule's z = 0 before sample 0, since a zero sample mixes to zero) in two device buffers.  A
+// handle's kernels read hist[cur]; carry then writes the next history into the other buffer behind them on the same
+// stream, and commit makes it live.  Each handle commits once no later launch of the call reads the old history:
+// rx_fm once at the end of a successful call, after the member's call, so a failed call leaves the old history live;
+// rx_power after each group's launch, since the next group of passes reads the new history.
+struct DdcFilter {
+	int M = 1, T = 1, S = 0;             // T = 1 (a plain rx_fm mixing handle): no history, carry and commit do nothing
+	bool wide = false;                   // the kernel accumulates in 64 bits
+	int32_t *taps = nullptr;
+	uint32_t *hist[2] = {nullptr, nullptr};
+	int cur = 0;
+	// the buffers hold at least one sample, so that T = 1 needs no special case
+	size_t hist_bytes() const { return std::max<size_t>(1, (size_t)T - 1) * sizeof(uint32_t); }
+	// on the current device, for a checked ddc; the caller releases the filter when it fails
+	int create(const rxb200_ddc *ddc, bool w)
+	{
+		M = ddc->decim; T = ddc->n_taps; S = ddc->shift; wide = w;
+		std::vector<int32_t> rev(ddc->taps, ddc->taps + T);
+		std::reverse(rev.begin(), rev.end());
+		RXB_CUDA(cudaMalloc(&taps, (size_t)T * sizeof(int32_t)));
+		RXB_CUDA(cudaMemcpy(taps, rev.data(), (size_t)T * sizeof(int32_t), cudaMemcpyHostToDevice));
+		for (int i = 0; i < 2; i++) {
+			RXB_CUDA(cudaMalloc(&hist[i], hist_bytes()));
+			RXB_CUDA(cudaMemset(hist[i], 0, hist_bytes()));
+		}
+		return RXB200_OK;
+	}
+	// the last T - 1 samples of (hist[cur], the c capture samples at src), into hist[cur ^ 1]
+	int carry(const uint32_t *src, size_t c, cudaStream_t st) const
+	{
+		const size_t H = (size_t)T - 1, w = sizeof(uint32_t);
+		if (H == 0) { return RXB200_OK; }
+		if (c >= H) {
+			RXB_CUDA(cudaMemcpyAsync(hist[cur ^ 1], src + (c - H), H * w, cudaMemcpyDeviceToDevice, st));
+		} else {
+			RXB_CUDA(cudaMemcpyAsync(hist[cur ^ 1], hist[cur] + c, (H - c) * w, cudaMemcpyDeviceToDevice, st));
+			RXB_CUDA(cudaMemcpyAsync(hist[cur ^ 1] + (H - c), src, c * w, cudaMemcpyDeviceToDevice, st));
+		}
+		return RXB200_OK;
+	}
+	void commit() { if (T > 1) { cur ^= 1; } }
+	// both histories zeroed behind any call still running on st, on the current device
+	int reset(cudaStream_t st)
+	{
+		RXB_CUDA(cudaMemsetAsync(hist[0], 0, hist_bytes(), st));
+		RXB_CUDA(cudaMemsetAsync(hist[1], 0, hist_bytes(), st));
+		cur = 0;
+		return RXB200_OK;
+	}
+	void release() { cudaFree(taps); cudaFree(hist[0]); cudaFree(hist[1]); }
+};
+
+// The device block of a stateless call: the mixer data at the front of h (a multiple of 16 bytes), then for a DDC the
+// reversed taps and a zero history, uploaded with one allocation and one copy on st.  The caller frees d with
+// cudaFreeAsync on st behind its launch.
+struct DdcBlock {
+	unsigned char *d = nullptr;
+	const int32_t *taps = nullptr;
+	const uint32_t *hist = nullptr;
+};
+int ddc_upload(std::vector<unsigned char> &h, const rxb200_ddc *ddc, cudaStream_t st, DdcBlock *b);
 
 }  // namespace rxb

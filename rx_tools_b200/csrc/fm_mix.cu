@@ -2,7 +2,8 @@
 // fm_mix_kernel mixes the capture to baseband once per channel with that channel's integer table, reading the capture
 // once and writing one CS16 stream per channel; a plain rxb200_fm handle with one channel per stream then runs the
 // chain on them through its device entry points.  A decimating handle (rxb200_fm_mix_create_ddc) runs fm_ddc_kernel
-// instead, which mixes, filters and decimates, and carries the capture's last T - 1 samples between calls.  Every
+// instead (ddc.cuh's down-converter with the channels' tables), which mixes, filters and decimates, and carries its
+// filter state (DdcFilter) between calls.  Every
 // process entry point of both kinds goes through mix_call, whose refusals and member shape come from
 // fm_mix_check_host_call (which the group uses too).  The chain itself is not touched here.
 #include <algorithm>
@@ -143,135 +144,47 @@ static int mix_table(int capture_rate, int offset_hz, std::vector<int32_t> &t, s
 	return rxb200_fm_mix_table(capture_rate, offset_hz, t.data(), t.size(), period);
 }
 
-// ---- the decimating down-converter (rxb200_fm_mix_create_ddc, rxb200_ddc_device)
-struct DdcArgs {
-	const uint32_t *src;             // the call's capture, one word per complex sample
-	const uint32_t *hist;            // the T - 1 raw capture samples before src
-	long long n_out;                 // outputs per channel
-	long long r0;                    // src index of the first emission point
-	unsigned long long pos;          // the mixer: src[i] uses table entry (pos + i) mod L
-	uint32_t *dst;                   // channel row c at dst + c * dst_stride, one word per output
-	long long dst_stride;
-	const int32_t *taps;             // reversed: taps[t] = h[T - 1 - t]
+// ---- the decimating down-converter (rxb200_fm_mix_create_ddc, rxb200_ddc_device): ddc_body with channel c's mixer
+// its own table (src[i] uses entry (pos + i) mod L) and its outputs in row c of dst, dst_stride words apart
+struct TabMix {
 	const int2 *tab;
 	const MixChan *chan;
-	int n_ch, M, T, S;
-	int ws;                          // staged samples between two outputs' windows: M when T >= M, else T
-	unsigned ws_m;                   // floor((2^32 - 1) / ws)
-	int U;                           // outputs per CTA
-	int lpo;                         // lanes per output (a power of two <= 32)
+	long long dst_stride;
+	struct Row {
+		const DdcArgs<TabMix> &a;
+		int c0, c;
+		long long u0;
+		MixChan *s_ch, ch;               // the grid row's channel records in shared memory, and channel c's
+		unsigned *s_base, base;          // their table entries at the CTA's first staged sample, and channel c's
+		__device__ Row(const DdcArgs<TabMix> &a, int c0, int nc, long long u0, long long g0) : a(a), c0(c0), u0(u0)
+		{
+			__shared__ MixChan sc[MIX_GROUP];
+			__shared__ unsigned sb[MIX_GROUP];
+			for (int c = threadIdx.x; c < nc; c += blockDim.x) {
+				const MixChan m = a.mix.chan[c0 + c];
+				long long q = g0 % m.L;
+				sb[c] = (unsigned)(q < 0 ? q + m.L : q);
+				sc[c] = m;
+			}
+			s_ch = sc; s_base = sb;
+		}
+		__device__ void chan(int k) { c = k; ch = s_ch[k]; base = s_base[k]; }
+		__device__ const int2 *entry(int off) const
+		{
+			const unsigned L = (unsigned)ch.L, t = base + (unsigned)off;      // < 2^20 + DDC_REACH
+			unsigned p = t - __umulhi(t, ch.m) * L;                         // the quotient is low by at most 1
+			if (p >= L) { p -= L; }
+			return a.mix.tab + ch.off + (int)p;
+		}
+		__device__ uint32_t *out(int u) const { return a.dst + (long long)(c0 + c) * a.mix.dst_stride + u0 + u; }
+	};
 };
 
-// One CTA: U consecutive outputs of every channel of its grid row (up to 256 channels, blockIdx.y).  It stages the
-// capture samples its outputs' windows cover once (the handle's history before the call's first sample), then per
-// channel mixes them into shared memory with the channel's table and runs the T-tap dot product at the emission points
-// only, lpo lanes per output.  Acc: int when sum |h| * 32768 + 2^(S-1) < 2^31, else long long (no partial sum can
-// overflow either way).
 template <typename Acc>
-__global__ void __launch_bounds__(DDC_THREADS) fm_ddc_kernel(const DdcArgs a)
-{
-	extern __shared__ int4 ddc_smem[];
-	__shared__ MixChan s_ch[MIX_GROUP];
-	__shared__ unsigned s_base[MIX_GROUP];  // each channel's table entry at the CTA's first staged sample
-	const int T = a.T;
-	const int room = (a.U - 1) * a.ws + T;
-	int32_t *s_h = reinterpret_cast<int32_t *>(ddc_smem);
-	uint32_t *s_x = reinterpret_cast<uint32_t *>(s_h + T);
-	uint32_t *s_z = s_x + room;
-	const int c0 = (int)blockIdx.y * MIX_GROUP;
-	const int nc = min(MIX_GROUP, a.n_ch - c0);
-	const long long u0 = (long long)blockIdx.x * a.U;
-	const int U = (int)min((long long)a.U, a.n_out - u0);
-	const int n = (U - 1) * a.ws + T;
-	const long long b0 = u0 * a.M + a.r0 - (T - 1);       // src index of the first staged sample, >= -(T - 1)
-	const long long g0 = (long long)a.pos + b0;            // its mixer position (< 0 only for zero history samples)
-	for (int j = threadIdx.x; j < T; j += blockDim.x) { s_h[j] = a.taps[j]; }
-	for (int c = threadIdx.x; c < nc; c += blockDim.x) {
-		const MixChan ch = a.chan[c0 + c];
-		long long q = g0 % ch.L;
-		s_base[c] = (unsigned)(q < 0 ? q + ch.L : q);
-		s_ch[c] = ch;
-	}
-	for (int s = threadIdx.x; s < n; s += blockDim.x) {
-		const long long i = b0 + ddc_off(s, a);
-		s_x[s] = i >= 0 ? __ldg(a.src + i) : a.hist[(T - 1) + i];
-	}
-	__syncthreads();
-	const int lane = (int)threadIdx.x & (a.lpo - 1), sub = (int)threadIdx.x / a.lpo, n_sub = (int)blockDim.x / a.lpo;
-	for (int c = 0; c < nc; c++) {
-		const MixChan ch = s_ch[c];
-		const unsigned L = (unsigned)ch.L, base = s_base[c];
-		for (int s = threadIdx.x; s < n; s += blockDim.x) {
-			const unsigned t = base + (unsigned)ddc_off(s, a);      // < 2^20 + DDC_REACH
-			unsigned p = t - __umulhi(t, ch.m) * L;               // the quotient is low by at most 1
-			if (p >= L) { p -= L; }
-			s_z[s] = mix_one(s_x[s], __ldg(a.tab + ch.off + (int)p));
-		}
-		__syncthreads();
-		uint32_t *row = a.dst + (long long)(c0 + c) * a.dst_stride + u0;
-		for (int ub = 0; ub < U; ub += n_sub) {                  // the same trip count on every lane of a warp
-			const int u = ub + sub;
-			Acc ai = 0, aq = 0;
-			if (u < U) {
-				const uint32_t *z = s_z + u * a.ws;
-				for (int j = lane; j < T; j += a.lpo) {
-					const uint32_t w = z[j];
-					const Acc h = (Acc)s_h[j];
-					ai += h * (Acc)(int16_t)(w & 0xffffu);
-					aq += h * (Acc)(int16_t)(w >> 16);
-				}
-			}
-			for (int o = a.lpo >> 1; o > 0; o >>= 1) {
-				ai += __shfl_xor_sync(0xffffffffu, ai, o);
-				aq += __shfl_xor_sync(0xffffffffu, aq, o);
-			}
-			if (u < U && lane == 0) {
-				row[u] = ((uint32_t)ddc_out(ai, a.S) & 0xffffu) | ((uint32_t)ddc_out(aq, a.S) << 16);
-			}
-		}
-		__syncthreads();                    // every output of this channel is made before s_z is overwritten
-	}
-}
-
-// Launches fm_ddc_kernel on the current device for a.n_out > 0 outputs per channel; fills a's launch shape
-static int ddc_launch(DdcArgs a, bool wide, cudaStream_t st)
-{
-	const int groups = (a.n_ch + MIX_GROUP - 1) / MIX_GROUP;
-	DdcShape sh;
-	size_t smem = 0;
-	long long bx = 0;
-	const int rc = ddc_shape(a.M, a.T, a.n_out, groups, &sh, &smem, &bx);
-	if (rc != RXB200_OK) { return rc; }
-	a.ws = sh.ws; a.ws_m = sh.ws_m; a.U = sh.U; a.lpo = sh.lpo;
-	void (*kern)(const DdcArgs) = wide ? fm_ddc_kernel<long long> : fm_ddc_kernel<int>;
-	RXB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-	kern<<<dim3((unsigned)bx, (unsigned)groups), DDC_THREADS, smem, st>>>(a);
-	RXB_CUDA(cudaGetLastError());
-	return RXB200_OK;
-}
+__global__ void __launch_bounds__(DDC_THREADS) fm_ddc_kernel(const DdcArgs<TabMix> a) { ddc_body<Acc>(a); }
 
 }  // namespace rxb
 
-// the DDC's arguments: M, T and S in range, taps given, and sum |h| * 32768 + 2^(S-1) < 2^63 (which these ranges
-// already bound by 2^59 + 2^61); *wide: the sum reaches 2^31, so the kernel accumulates in 64 bits
-int rxb::ddc_check(const rxb200_ddc *d, bool *wide)
-{
-	if (!d || !d->taps) { set_error("null ddc or taps"); return RXB200_EINVAL; }
-	if (d->decim < 1 || d->decim > 4096 || d->n_taps < 1 || d->n_taps > 8192 || d->shift < 0 || d->shift > 62) {
-		set_error("ddc decim %d, n_taps %d, shift %d: need 1 <= decim <= 4096, 1 <= n_taps <= 8192, 0 <= shift <= 62",
-		          d->decim, d->n_taps, d->shift);
-		return RXB200_EINVAL;
-	}
-	unsigned long long sum = 0;
-	for (int j = 0; j < d->n_taps; j++) {
-		const long long h = d->taps[j];
-		sum += (unsigned long long)(h < 0 ? -h : h);
-	}
-	const unsigned long long g = sum * 32768ull + (d->shift ? 1ull << (d->shift - 1) : 0ull);
-	if (g >= (1ull << 63)) { set_error("sum |taps| * 32768 + 2^(shift-1) >= 2^63"); return RXB200_EINVAL; }
-	if (wide) { *wide = g >= (1ull << 31); }
-	return RXB200_OK;
-}
 using namespace rxb;
 
 struct rxb200_fm_mix {
@@ -288,11 +201,8 @@ struct rxb200_fm_mix {
 	cudaEvent_t ev0 = nullptr, ev1 = nullptr;    // around the last fm_mix_kernel (fm_ddc_kernel)
 	// a decimating handle (rxb200_fm_mix_create_ddc): fm_ddc_kernel writes the decimated streams to d_mix ([n_channels]
 	// [n_dec_int16]) and the member runs on those
-	bool ddc = false, wide = false;              // wide: the kernel accumulates in 64 bits
-	int decim = 1, n_taps = 1, shift = 0;
-	int32_t *d_taps = nullptr;                   // reversed
-	int16_t *d_hist[2] = {nullptr, nullptr};     // the raw capture's last T - 1 samples before pos (zero before 0)
-	int cur_hist = 0;                            // d_hist[cur_hist] is the live one, the other the next call's
+	bool ddc = false;
+	DdcFilter f;                                 // its filter state (T = 1 for a plain handle)
 };
 
 namespace {
@@ -324,13 +234,13 @@ int rxb::fm_mix_check_host_call(rxb200_fm_mix *m, const int16_t *cs16, size_t n_
 		                               total);
 	}
 	if (!cs16 || !pcm) { set_error("null argument"); return RXB200_EINVAL; }
-	const size_t M = (size_t)m->decim;
+	const size_t M = (size_t)m->f.M;
 	if (n_int16 % 2 != 0) { set_error("n_int16=%zu must be even", n_int16); return RXB200_EUNSUPPORTED; }
 	if (!read && (chunk_int16 == 0 || chunk_int16 % (2 * M) != 0)) {
 		set_error("chunk_int16=%zu must be a multiple of 2 * decim = %zu", chunk_int16, 2 * M);
 		return RXB200_EUNSUPPORTED;
 	}
-	*n16 = ddc_len(m->pos, n_int16, m->decim);
+	*n16 = ddc_len(m->pos, n_int16, m->f.M);
 	*chunk16 = read ? *n16 : chunk_int16 / M;
 	if (read && *n16 == 0 && n_int16 > 0) {
 		return rxb::fm_check_host_call(m->h, cs16, 0, 262144, pcm, pcm_stride, nullptr, n_pcm, false, total);
@@ -346,37 +256,21 @@ int rxb::fm_mix_check_host_call(rxb200_fm_mix *m, const int16_t *cs16, size_t n_
 
 namespace {
 
-// The next history: the last T - 1 samples of (history, the call's c capture samples at src), into the spare buffer.
-// A plain handle has T = 1: no history.
-int ddc_carry(rxb200_fm_mix *m, const int16_t *src, size_t c, cudaStream_t st)
-{
-	const size_t H = (size_t)m->n_taps - 1, w = 2 * sizeof(int16_t);
-	if (H == 0) { return RXB200_OK; }
-	const int16_t *old = m->d_hist[m->cur_hist];
-	int16_t *next = m->d_hist[m->cur_hist ^ 1];
-	if (c >= H) {
-		RXB_CUDA(cudaMemcpyAsync(next, src + 2 * (c - H), H * w, cudaMemcpyDeviceToDevice, st));
-	} else {
-		RXB_CUDA(cudaMemcpyAsync(next, old + 2 * c, (H - c) * w, cudaMemcpyDeviceToDevice, st));
-		RXB_CUDA(cudaMemcpyAsync(next + 2 * (H - c), src, c * w, cudaMemcpyDeviceToDevice, st));
-	}
-	return RXB200_OK;
-}
-
 // a decimating handle's front stage: fm_ddc_kernel from the call's capture at src to n16 int16 per channel in d_mix
 int ddc_front(rxb200_fm_mix *m, const int16_t *src, size_t n16, cudaStream_t st)
 {
-	DdcArgs a{};
+	const DdcFilter &f = m->f;
+	DdcArgs<TabMix> a{};
 	a.src = reinterpret_cast<const uint32_t *>(src);
-	a.hist = reinterpret_cast<const uint32_t *>(m->d_hist[m->cur_hist]);
+	a.hist = f.hist[f.cur];
 	a.n_out = (long long)(n16 / 2);
-	a.r0 = (long long)(m->decim - 1) - (long long)(m->pos % (unsigned long long)m->decim);
+	a.r0 = (long long)(f.M - 1) - (long long)(m->pos % (unsigned long long)f.M);
 	a.pos = m->pos;
 	a.dst = reinterpret_cast<uint32_t *>(m->d_mix);
-	a.dst_stride = (long long)(n16 / 2);
-	a.taps = m->d_taps; a.tab = m->d_tab; a.chan = m->d_chan;
-	a.n_ch = m->n_channels; a.M = m->decim; a.T = m->n_taps; a.S = m->shift;
-	return ddc_launch(a, m->wide, st);
+	a.taps = f.taps;
+	a.n_ch = m->n_channels; a.M = f.M; a.T = f.T; a.S = f.S;
+	a.mix = TabMix{m->d_tab, m->d_chan, (long long)(n16 / 2)};
+	return ddc_launch(a, f.wide ? fm_ddc_kernel<long long> : fm_ddc_kernel<int>, st);
 }
 
 // One call of any process entry point.  device: cs16 and pcm are device pointers (the member's device entry point
@@ -410,7 +304,7 @@ int mix_call(rxb200_fm_mix *m, const int16_t *cs16, size_t n_int16, size_t chunk
 		if (rc != RXB200_OK) { return rc; }
 	}
 	RXB_CUDA(cudaEventRecord(m->ev1, st));
-	rc = ddc_carry(m, src, c, st);
+	rc = m->f.carry(reinterpret_cast<const uint32_t *>(src), c, st);
 	if (rc != RXB200_OK) { return rc; }
 	rxb::fm_unchain(m->h);                       // the member's input was just written on its stream
 	if (n16) {
@@ -430,45 +324,25 @@ int mix_call(rxb200_fm_mix *m, const int16_t *cs16, size_t n_int16, size_t chunk
 	} else if (sync && n16 == 0) {
 		RXB_CUDA(cudaStreamSynchronize(st));    // with output, the member's call has synchronised
 	}
-	if (m->n_taps > 1) { m->cur_hist ^= 1; }
+	m->f.commit();
 	m->pos += c;
 	if (n_pcm) { *n_pcm = total; }
 	return RXB200_OK;
 }
 
-// The device block of a one-channel call of the mixer or the DDC alone: the table, the channel record and, for a DDC,
-// the reversed taps and a zero history, uploaded with one allocation and one copy on st.  The caller frees o->d with
-// cudaFreeAsync on st behind its launch.
-struct OneChannel {
-	unsigned char *d = nullptr;
-	const int2 *tab = nullptr;
-	const MixChan *chan = nullptr;
-	const int32_t *taps = nullptr;
-	const uint32_t *hist = nullptr;
-};
-
-int upload_one(const std::vector<int32_t> &t, size_t L, const rxb200_ddc *ddc, cudaStream_t st, OneChannel *o)
+// The device block of a one-channel call of the mixer or the DDC alone: the table and the channel record, then what
+// ddc_upload adds.  *tab and *chan point into it.
+int upload_one(const std::vector<int32_t> &t, size_t L, const rxb200_ddc *ddc, cudaStream_t st, DdcBlock *b,
+               const int2 **tab, const MixChan **chan)
 {
-	const size_t T = ddc ? (size_t)ddc->n_taps : 0;
-	const size_t o_chan = L * sizeof(int2), o_taps = o_chan + sizeof(MixChan), o_hist = o_taps + T * sizeof(int32_t);
-	const size_t bytes = o_hist + (ddc ? std::max<size_t>(1, T - 1) * sizeof(uint32_t) : 0);
-	std::vector<unsigned char> h(bytes, 0);
+	std::vector<unsigned char> h(L * sizeof(int2) + sizeof(MixChan));
 	const MixChan ch = mix_chan(0, L);
-	memcpy(h.data(), t.data(), o_chan);
-	memcpy(h.data() + o_chan, &ch, sizeof(MixChan));
-	for (size_t j = 0; j < T; j++) { memcpy(h.data() + o_taps + j * sizeof(int32_t), ddc->taps + (T - 1 - j), sizeof(int32_t)); }
-	RXB_CUDA(cudaMallocAsync((void **)&o->d, bytes, st));
-	// from pageable memory: the copy has read its source when it returns
-	if (cudaMemcpyAsync(o->d, h.data(), bytes, cudaMemcpyHostToDevice, st) != cudaSuccess) {
-		set_error("%s upload failed: %s", ddc ? "ddc" : "table", cudaGetErrorString(cudaGetLastError()));
-		cudaFreeAsync(o->d, st);
-		o->d = nullptr;
-		return RXB200_ECUDA;
-	}
-	o->tab = reinterpret_cast<const int2 *>(o->d);
-	o->chan = reinterpret_cast<const MixChan *>(o->d + o_chan);
-	o->taps = reinterpret_cast<const int32_t *>(o->d + o_taps);
-	o->hist = reinterpret_cast<const uint32_t *>(o->d + o_hist);
+	memcpy(h.data(), t.data(), L * sizeof(int2));
+	memcpy(h.data() + L * sizeof(int2), &ch, sizeof(MixChan));
+	const int rc = ddc_upload(h, ddc, st, b);
+	if (rc != RXB200_OK) { return rc; }
+	*tab = reinterpret_cast<const int2 *>(b->d);
+	*chan = reinterpret_cast<const MixChan *>(b->d + L * sizeof(int2));
 	return RXB200_OK;
 }
 
@@ -484,12 +358,14 @@ extern "C" int rxb200_mix_device(int capture_rate, int offset_hz, long long phas
 	int rc = mix_table(capture_rate, offset_hz, t, &L);
 	if (rc != RXB200_OK || n_complex == 0) { return rc; }
 	const cudaStream_t st = (cudaStream_t)stream;
-	OneChannel o;
-	rc = upload_one(t, L, nullptr, st, &o);
+	DdcBlock b;
+	const int2 *tab = nullptr;
+	const MixChan *chan = nullptr;
+	rc = upload_one(t, L, nullptr, st, &b, &tab, &chan);
 	if (rc != RXB200_OK) { return rc; }
-	rc = mix_launch(d_src, (long long)n_complex, d_dst, 0, o.tab, o.chan, std::vector<MixChan>(1, mix_chan(0, L)),
+	rc = mix_launch(d_src, (long long)n_complex, d_dst, 0, tab, chan, std::vector<MixChan>(1, mix_chan(0, L)),
 	                (unsigned long long)phase % L, st);
-	cudaFreeAsync(o.d, st);
+	cudaFreeAsync(b.d, st);
 	return rc;
 }
 
@@ -499,7 +375,7 @@ extern "C" void rxb200_fm_mix_destroy(rxb200_fm_mix *m)
 	rxb200_fm_destroy(m->h);   // synchronises the stream the mixer runs on
 	cudaSetDevice(m->device);
 	cudaFree(m->d_tab); cudaFree(m->d_chan); cudaFree(m->d_cap); cudaFree(m->d_mix); cudaFree(m->d_out);
-	cudaFree(m->d_taps); cudaFree(m->d_hist[0]); cudaFree(m->d_hist[1]);
+	m->f.release();
 	if (m->ev0) { cudaEventDestroy(m->ev0); }
 	if (m->ev1) { cudaEventDestroy(m->ev1); }
 	delete m;
@@ -538,17 +414,9 @@ int mix_create(const rxb200_fm_params *params, int capture_rate, const int *offs
 	RXB_CUDA_OR(cudaEventCreate(&m->ev0), rxb200_fm_mix_destroy(m));
 	RXB_CUDA_OR(cudaEventCreate(&m->ev1), rxb200_fm_mix_destroy(m));
 	if (ddc) {
-		m->ddc = true; m->wide = wide;
-		m->decim = ddc->decim; m->n_taps = ddc->n_taps; m->shift = ddc->shift;
-		const size_t T = (size_t)ddc->n_taps, hist_bytes = std::max<size_t>(1, T - 1) * 2 * sizeof(int16_t);
-		std::vector<int32_t> rev(ddc->taps, ddc->taps + T);
-		std::reverse(rev.begin(), rev.end());
-		RXB_CUDA_OR(cudaMalloc(&m->d_taps, T * sizeof(int32_t)), rxb200_fm_mix_destroy(m));
-		RXB_CUDA_OR(cudaMemcpy(m->d_taps, rev.data(), T * sizeof(int32_t), cudaMemcpyHostToDevice), rxb200_fm_mix_destroy(m));
-		for (int i = 0; i < 2; i++) {
-			RXB_CUDA_OR(cudaMalloc(&m->d_hist[i], hist_bytes), rxb200_fm_mix_destroy(m));
-			RXB_CUDA_OR(cudaMemset(m->d_hist[i], 0, hist_bytes), rxb200_fm_mix_destroy(m));
-		}
+		m->ddc = true;
+		const int rc = m->f.create(ddc, wide);
+		if (rc != RXB200_OK) { rxb200_fm_mix_destroy(m); return rc; }
 	}
 	*out = m;
 	return RXB200_OK;
@@ -577,7 +445,7 @@ extern "C" int rxb200_fm_mix_create_ddc(const rxb200_fm_params *params, int capt
 extern "C" int rxb200_fm_mix_decimated_len(const rxb200_fm_mix *m, size_t n_int16, size_t *n_dec_int16)
 {
 	if (!m || !n_dec_int16) { set_error("null argument"); return RXB200_EINVAL; }
-	*n_dec_int16 = m->ddc ? ddc_len(m->pos, n_int16, m->decim) : n_int16;
+	*n_dec_int16 = m->ddc ? ddc_len(m->pos, n_int16, m->f.M) : n_int16;
 	return RXB200_OK;
 }
 
@@ -586,7 +454,7 @@ extern "C" size_t rxb200_fm_mix_max_output(const rxb200_fm_mix *m, size_t n_int1
 	if (!m || chunk_int16 == 0) { return 0; }
 	if (!m->ddc) { return rxb200_fm_max_output(m->h, n_int16, chunk_int16); }
 	// floor((p + c) / M) - floor(p / M) <= ceil(c / M) at any phase p
-	const size_t M = (size_t)m->decim, n16 = 2 * ((n_int16 / 2 + M - 1) / M);
+	const size_t M = (size_t)m->f.M, n16 = 2 * ((n_int16 / 2 + M - 1) / M);
 	return rxb200_fm_max_output(m->h, n16, chunk_int16 / M ? chunk_int16 / M : 2);
 }
 
@@ -604,37 +472,32 @@ extern "C" int rxb200_ddc_device(int capture_rate, int offset_hz, long long phas
 	const size_t n_out = n_complex / (size_t)ddc->decim;
 	if (rc != RXB200_OK || n_out == 0) { return rc; }
 	const cudaStream_t st = (cudaStream_t)stream;
-	OneChannel o;
-	rc = upload_one(t, L, ddc, st, &o);
+	DdcBlock b;
+	DdcArgs<TabMix> a{};
+	rc = upload_one(t, L, ddc, st, &b, &a.mix.tab, &a.mix.chan);
 	if (rc != RXB200_OK) { return rc; }
-	DdcArgs a{};
 	a.src = reinterpret_cast<const uint32_t *>(d_src);
-	a.hist = o.hist;
+	a.hist = b.hist;
 	a.n_out = (long long)n_out;
 	a.r0 = ddc->decim - 1;
 	a.pos = (unsigned long long)phase % L;
 	a.dst = reinterpret_cast<uint32_t *>(d_dst);
-	a.dst_stride = 0;
-	a.taps = o.taps; a.tab = o.tab; a.chan = o.chan;
+	a.taps = b.taps;
 	a.n_ch = 1; a.M = ddc->decim; a.T = ddc->n_taps; a.S = ddc->shift;
-	rc = ddc_launch(a, wide, st);
-	cudaFreeAsync(o.d, st);
+	rc = ddc_launch(a, wide ? fm_ddc_kernel<long long> : fm_ddc_kernel<int>, st);
+	cudaFreeAsync(b.d, st);
 	return rc;
 }
 
 extern "C" int rxb200_fm_mix_reset(rxb200_fm_mix *m)
 {
 	if (!m) { return RXB200_EINVAL; }
-	const int rc = rxb200_fm_reset(m->h);
+	int rc = rxb200_fm_reset(m->h);
 	if (rc != RXB200_OK) { return rc; }
 	if (m->ddc) {
-		// behind any call still running on the member's stream
-		const cudaStream_t st = (cudaStream_t)rxb200_fm_stream(m->h);
-		const size_t hist_bytes = std::max<size_t>(1, (size_t)m->n_taps - 1) * 2 * sizeof(int16_t);
 		RXB_CUDA(cudaSetDevice(m->device));
-		RXB_CUDA(cudaMemsetAsync(m->d_hist[0], 0, hist_bytes, st));
-		RXB_CUDA(cudaMemsetAsync(m->d_hist[1], 0, hist_bytes, st));
-		m->cur_hist = 0;
+		rc = m->f.reset((cudaStream_t)rxb200_fm_stream(m->h));   // behind any call still running on the member's stream
+		if (rc != RXB200_OK) { return rc; }
 	}
 	m->pos = 0;
 	return RXB200_OK;

@@ -4,7 +4,8 @@
 #   tools/build_variants.sh name1="-DX=1 -DY=2" name2="..."
 set -e
 cd "$(dirname "$0")/../rx_tools_b200/csrc"
-make -s -j4 >/dev/null            # the shared objects (power, sdr, host plan) come from the default build
+make -s -j4 >/dev/null            # every other object comes from the default build
+others=$(make -s print-objs | tr ' ' '\n' | grep -vx fm_kernels.o)
 ARCH="-gencode arch=compute_90a,code=sm_90a"
 mkdir -p ../variants
 pids=()
@@ -12,7 +13,7 @@ for spec in "$@"; do
 	name="${spec%%=*}"; flags="${spec#*=}"
 	(
 		nvcc $ARCH -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -Xptxas -v $flags -c -o ../variants/fm_$name.o fm_kernels.cu 2> ../variants/fm_$name.ptxas.log
-		nvcc $ARCH -shared -o ../variants/librxb200_$name.so ../variants/fm_$name.o fm_mix.o fm_group.o power_kernels.o sdr_kernels.o host_plan.o nccl_dyn.o -ldl
+		nvcc $ARCH -shared -o ../variants/librxb200_$name.so ../variants/fm_$name.o $others -ldl
 		echo "$flags" > ../variants/$name.flags
 		echo "built $name: $flags"
 	) &
