@@ -15,6 +15,11 @@
  * and a read per hop.  The device is tuned once to the centre of the hops, at M times the hop rate, and read without
  * pause; each pass of M * buf_len int16 goes through rxb200_power_mix_accumulate, whose NCO down-converter makes every
  * hop's buffer on the GPU.  A pass counts as a sweep.
+ *
+ * Tile mode: RXB200_TILE_RATE=<max Hz> takes a sweep wider than one capture in tiles of consecutive hops
+ * (rxb200_power_plan_tiles).  Per sweep, each tile is one retune to its centre, one flush read, and one burst of the
+ * filter's lead plus one pass, gathered from reads of any length and handed to rxb200_power_mix_accumulate_burst for
+ * the tile's hops.  A failed read drops that tile's burst for the sweep, as hop mode skips a hop.
  */
 #include <math.h>
 #include <signal.h>
@@ -44,7 +49,9 @@ static void usage(void)
 		"\t[-S tuner_sleep_usec] [-R tuner_retry_max]\n"
 		"\tfilename ('-' means stdout)\n"
 		"environment: RXB200_GPUS=n shards the hops over n GPUs; RXB200_CAPTURE_RATE=max_Hz takes every hop from one\n"
-		"\tcapture of at most max_Hz samples/s, tuned once to the centre of the sweep (one GPU)\n");
+		"\tcapture of at most max_Hz samples/s, tuned once to the centre of the sweep (one GPU);\n"
+		"\tRXB200_TILE_RATE=max_Hz takes a wider sweep in tiles of hops, one retune and one burst of at most max_Hz\n"
+		"\tsamples/s per tile (one GPU)\n");
 	exit(1);
 }
 
@@ -84,6 +91,113 @@ static void time_string(char *tstr, size_t cap, time_t now)
 	if (getenv("RXB200_FIXED_TIME")) { snprintf(tstr, cap, "%s", getenv("RXB200_FIXED_TIME")); }
 }
 
+/* The set-up every mode shares: the device, its stream, the signal handlers, the -D / -O / -g / -p settings, then the
+ * output file.  NULL (reported on stderr) when the device or the file cannot be opened. */
+static FILE *open_radio(const char *dev_query, size_t channel, const char *antenna, const char *gain_str, int ppm,
+                        int direct_sampling, int offset_tuning, const char *filename, SoapySDRDevice **devp,
+                        SoapySDRStream **streamp)
+{
+	if (sdr_open(dev_query, channel, devp, streamp) != 0) { fprintf(stderr, "Failed to open sdr device matching '%s'.\n", dev_query); return NULL; }
+	SoapySDRDevice *dev = *devp;
+	if (antenna && SoapySDRDevice_setAntenna(dev, SOAPY_SDR_RX, channel, antenna) != 0) { fprintf(stderr, "Failed to set antenna"); }
+	SoapySDRDevice_activateStream(dev, *streamp, 0, 0, 0);
+	struct sigaction sa; memset(&sa, 0, sizeof sa); sa.sa_handler = on_signal;
+	sigaction(SIGINT, &sa, NULL); sigaction(SIGTERM, &sa, NULL); sigaction(SIGQUIT, &sa, NULL);
+	signal(SIGPIPE, SIG_IGN);
+	if (direct_sampling) { SoapySDRDevice_writeSetting(dev, "direct_samp", direct_sampling == 1 ? "1" : "2"); }
+	if (offset_tuning) { SoapySDRDevice_writeSetting(dev, "offset_tune", "true"); }
+	sdr_set_gain(dev, channel, gain_str);
+	SoapySDRDevice_setFrequencyCorrection(dev, SOAPY_SDR_RX, channel, (double)ppm);
+	FILE *out = !strcmp(filename, "-") ? stdout : fopen(filename, "wb");
+	if (!out) { fprintf(stderr, "Failed to open %s\n", filename); }
+	return out;
+}
+
+/* retune() (:548-580): tune to f, sleep -S, then one flush read of BUFFER_DUMP elements with -R tries */
+static void retune(SoapySDRDevice *dev, SoapySDRStream *stream, size_t channel, int64_t f, int16_t *dump,
+                   int tuner_sleep_usec, int tuner_retry_max)
+{
+	SoapySDRKwargs none = {0, NULL, NULL};
+	if (SoapySDRDevice_setFrequency(dev, SOAPY_SDR_RX, channel, (double)f, &none) != 0) {
+		fprintf(stderr, "Error: failed to set frequency %lli Hz\n", (long long)f);
+		return;
+	}
+	usleep((useconds_t)tuner_sleep_usec);
+	int r = -1, flags = 0; long long tn = 0; void *bp[] = {dump};
+	for (int a = 0; a < tuner_retry_max && r < 0; a++) { r = SoapySDRDevice_readStream(dev, stream, bp, BUFFER_DUMP, &flags, &tn, 1000000); }
+	if (r < 0) { fprintf(stderr, "Error: bad retune at %lli Hz, r=%d (try increasing -S or -R).\n", (long long)f, r); }
+}
+
+/* Tile mode's device side and report loop.  Per sweep, each tile retunes to its centre when the device is elsewhere,
+ * then gathers one burst of G + M * buf_len / 2 complex samples from reads of whatever length the device returns and
+ * accumulates it for the tile's hops.  A failed read drops the burst, so the tile's hops get no pass this sweep; the
+ * stream has run dry when no tile got its burst in a sweep. */
+static int tile_mode(rxb200_power_mix *pm, const rxb200_power_plan *plan, const rxb200_power_tiling *tl,
+                     const char *dev_query, size_t channel, const char *gain_str, const char *antenna, const char *filename,
+                     int ppm, int direct_sampling, int offset_tuning, int tuner_sleep_usec, int tuner_retry_max,
+                     int interval, int single, time_t exit_after)
+{
+	const rxb200_power_params *pp = &plan->params;
+	const int n_hops = pp->n_hops, N = 1 << pp->bin_e;
+	rxb200_power *pw = rxb200_power_mix_member(pm);
+	SoapySDRDevice *dev = NULL; SoapySDRStream *stream = NULL;
+	FILE *out = open_radio(dev_query, channel, antenna, gain_str, ppm, direct_sampling, offset_tuning, filename, &dev, &stream);
+	if (!out) { return 1; }
+	SoapySDRDevice_setSampleRate(dev, SOAPY_SDR_RX, channel, (double)tl->capture_rate);
+	const size_t burst16 = 2 * (size_t)rxb200_power_mix_lead(pm) + (size_t)tl->decim * (size_t)pp->buf_len;
+	int16_t *burst = (int16_t *)malloc(burst16 * sizeof(int16_t));
+	int16_t *dump = (int16_t *)malloc((size_t)BUFFER_DUMP * 4);
+	const int row_len = rxb200_power_row_len(pp->bin_e, plan->crop);
+	double *db = (double *)malloc((size_t)n_hops * (size_t)row_len * sizeof(double));
+	int *samples = (int *)malloc((size_t)n_hops * sizeof(int));
+	char *row = (char *)malloc(64 + 16 * ((size_t)N + 8));
+	const char *hook = getenv("RXB200_MAX_SWEEPS");       /* test hook: report after this many sweeps and exit */
+	const long max_sweeps = hook ? atol(hook) : 0;
+	long sweeps = 0;
+	time_t next_tick = time(NULL) + interval, exit_time = exit_after ? time(NULL) + exit_after : 0;
+	int done = 0, rc = 0;
+	while (!done && !g_stop) {
+		/* ---- one sweep: one burst per tile */
+		int n_ok = 0;
+		for (int t = 0; t < tl->n_tiles && !g_stop && !rc; t++) {
+			int hb = 0, he = 0; int64_t fc = 0;
+			rxb200_power_tile(plan, tl, t, &hb, &he, &fc);
+			if ((int64_t)SoapySDRDevice_getFrequency(dev, SOAPY_SDR_RX, channel) != fc) {
+				retune(dev, stream, channel, fc, dump, tuner_sleep_usec, tuner_retry_max);
+			}
+			size_t have = 0;
+			while (have < burst16 && !g_stop) {
+				void *bp[] = {burst + have};
+				int flags = 0; long long tn = 0;
+				const int r = SoapySDRDevice_readStream(dev, stream, bp, (burst16 - have) / 2, &flags, &tn, 1000000);
+				if (r < 0) { fprintf(stderr, "Error: reading stream %d\n", r); break; }    /* the burst is dropped */
+				have += 2 * (size_t)r;
+			}
+			if (have < burst16) { continue; }
+			if (rxb200_power_mix_accumulate_burst(pm, hb, he, burst, burst16) != RXB200_OK) { fprintf(stderr, "rxb200: %s\n", rxb200_last_error()); rc = 1; break; }
+			n_ok++;
+		}
+		if (rc) { break; }
+		sweeps++;
+		const int dry = n_ok == 0;
+		time_t now = time(NULL);
+		const int hooked = max_sweeps && sweeps >= max_sweeps;
+		if (now < next_tick && !hooked && !dry) { continue; }
+		char tstr[50];
+		time_string(tstr, sizeof tstr, now);
+		if (report(out, pw, plan, db, row_len, samples, row, 64 + 16 * ((size_t)N + 8), tstr) != 0) { rc = 1; break; }
+		rxb200_power_reset(pw);
+		while (time(NULL) >= next_tick) { next_tick += interval; }
+		if (single || hooked || dry) { done = 1; }
+		if (exit_time && time(NULL) >= exit_time) { done = 1; }
+	}
+	fprintf(stderr, g_stop ? "\nUser cancel, exiting...\n" : "\nDone, exiting...\n");
+	if (out != stdout) { fclose(out); }
+	free(burst); free(dump); free(db); free(samples); free(row);
+	sdr_close(dev, stream);
+	return rc;
+}
+
 /* Capture mode's device side and report loop: one tune to fc at R, one flush read, then passes of M * buf_len int16
  * collected from reads of whatever length the device returns; a failed read discards the partial pass, and
  * tuner_retry_max failed reads in a row mean the stream has run dry. */
@@ -96,30 +210,12 @@ static int capture_mode(rxb200_power_mix *pm, const rxb200_power_plan *plan, int
 	const int n_hops = pp->n_hops, N = 1 << pp->bin_e;
 	rxb200_power *pw = rxb200_power_mix_member(pm);
 	SoapySDRDevice *dev = NULL; SoapySDRStream *stream = NULL;
-	if (sdr_open(dev_query, channel, &dev, &stream) != 0) { fprintf(stderr, "Failed to open sdr device matching '%s'.\n", dev_query); return 1; }
-	if (antenna && SoapySDRDevice_setAntenna(dev, SOAPY_SDR_RX, channel, antenna) != 0) { fprintf(stderr, "Failed to set antenna"); }
-	SoapySDRDevice_activateStream(dev, stream, 0, 0, 0);
-	struct sigaction sa; memset(&sa, 0, sizeof sa); sa.sa_handler = on_signal;
-	sigaction(SIGINT, &sa, NULL); sigaction(SIGTERM, &sa, NULL); sigaction(SIGQUIT, &sa, NULL);
-	signal(SIGPIPE, SIG_IGN);
-	if (direct_sampling) { SoapySDRDevice_writeSetting(dev, "direct_samp", direct_sampling == 1 ? "1" : "2"); }
-	if (offset_tuning) { SoapySDRDevice_writeSetting(dev, "offset_tune", "true"); }
-	sdr_set_gain(dev, channel, gain_str);
-	SoapySDRDevice_setFrequencyCorrection(dev, SOAPY_SDR_RX, channel, (double)ppm);
-	FILE *out = !strcmp(filename, "-") ? stdout : fopen(filename, "wb");
-	if (!out) { fprintf(stderr, "Failed to open %s\n", filename); return 1; }
+	FILE *out = open_radio(dev_query, channel, antenna, gain_str, ppm, direct_sampling, offset_tuning, filename, &dev, &stream);
+	if (!out) { return 1; }
 	SoapySDRDevice_setSampleRate(dev, SOAPY_SDR_RX, channel, (double)R);
-	SoapySDRKwargs none = {0, NULL, NULL};
-	if (SoapySDRDevice_setFrequency(dev, SOAPY_SDR_RX, channel, (double)fc, &none) != 0) {
-		fprintf(stderr, "Error: failed to set frequency %lli Hz\n", (long long)fc);
-	} else {
-		usleep((useconds_t)tuner_sleep_usec);
-		int16_t *dump = (int16_t *)malloc((size_t)BUFFER_DUMP * 4);
-		int r = -1, flags = 0; long long tn = 0; void *bp[] = {dump};
-		for (int a = 0; a < tuner_retry_max && r < 0; a++) { r = SoapySDRDevice_readStream(dev, stream, bp, BUFFER_DUMP, &flags, &tn, 1000000); }
-		if (r < 0) { fprintf(stderr, "Error: bad retune at %lli Hz, r=%d (try increasing -S or -R).\n", (long long)fc, r); }
-		free(dump);
-	}
+	int16_t *dump = (int16_t *)malloc((size_t)BUFFER_DUMP * 4);
+	retune(dev, stream, channel, fc, dump, tuner_sleep_usec, tuner_retry_max);
+	free(dump);
 	const size_t pass16 = (size_t)M * (size_t)pp->buf_len;
 	int16_t *pass = (int16_t *)malloc(pass16 * sizeof(int16_t));
 	const int row_len = rxb200_power_row_len(pp->bin_e, plan->crop);
@@ -234,7 +330,30 @@ int main(int argc, char **argv)
 	int n_gpus = getenv("RXB200_GPUS") ? atoi(getenv("RXB200_GPUS")) : 1;
 	if (n_gpus < 1) { n_gpus = 1; }
 	if (n_gpus > n_hops) { n_gpus = n_hops; }
-	const char *cap_env = getenv("RXB200_CAPTURE_RATE");
+	const char *cap_env = getenv("RXB200_CAPTURE_RATE"), *tile_env = getenv("RXB200_TILE_RATE");
+	if (tile_env) {
+		/* tile mode: the planner's tiles, each hop's offset from its tile's centre, one filter for every tile */
+		if (cap_env) { fprintf(stderr, "Tile mode (RXB200_TILE_RATE) and capture mode (RXB200_CAPTURE_RATE) exclude each other.\n"); return 1; }
+		if (n_gpus > 1) { fprintf(stderr, "Tile mode (RXB200_TILE_RATE) runs on one GPU: unset RXB200_GPUS.\n"); return 1; }
+		rxb200_power_tiling tl;
+		int *offs = (int *)malloc(sizeof(int) * (size_t)n_hops);
+		if (rxb200_power_plan_tiles(&plan, atoll(tile_env), &tl, offs) != RXB200_OK) {
+			fprintf(stderr, "Tile mode: %s (RXB200_TILE_RATE=%s).\n", rxb200_last_error(), tile_env);
+			return 1;
+		}
+		fprintf(stderr, "Tile mode: %d tiles of up to %d hops, %d Hz, decimation %d, %d taps\n", tl.n_tiles,
+		        tl.hops_per_tile, tl.capture_rate, tl.decim, tl.n_taps);
+		int32_t *taps = (int32_t *)malloc(sizeof(int32_t) * (size_t)tl.n_taps);
+		rxb200_ddc_lowpass(tl.decim, tl.n_taps, 15, taps);
+		const rxb200_ddc ddc = {tl.decim, tl.n_taps, taps, 15};
+		rxb200_power_mix *pm = NULL;
+		if (rxb200_power_mix_create(pp, window_coefs, NULL, tl.capture_rate, offs, &ddc, 0, &pm) != RXB200_OK) { fprintf(stderr, "rxb200: %s\n", rxb200_last_error()); return 1; }
+		free(offs); free(taps);
+		const int rc = tile_mode(pm, &plan, &tl, dev_query, channel, gain_str, antenna, filename, ppm, direct_sampling,
+		                         offset_tuning, tuner_sleep_usec, tuner_retry_max, interval, single, exit_after);
+		rxb200_power_mix_destroy(pm);
+		return rc;
+	}
 	if (cap_env) {
 		/* capture mode: centre of the hops, each hop's offset from it, the smallest M whose capture holds them all */
 		if (n_gpus > 1) { fprintf(stderr, "Capture mode (RXB200_CAPTURE_RATE) runs on one GPU: unset RXB200_GPUS.\n"); return 1; }
@@ -271,18 +390,8 @@ int main(int argc, char **argv)
 	if (n_gpus > 1) { fprintf(stderr, "Hops sharded over %d GPUs\n", n_gpus); }
 
 	SoapySDRDevice *dev = NULL; SoapySDRStream *stream = NULL;
-	if (sdr_open(dev_query, channel, &dev, &stream) != 0) { fprintf(stderr, "Failed to open sdr device matching '%s'.\n", dev_query); return 1; }
-	if (antenna && SoapySDRDevice_setAntenna(dev, SOAPY_SDR_RX, channel, antenna) != 0) { fprintf(stderr, "Failed to set antenna"); }
-	SoapySDRDevice_activateStream(dev, stream, 0, 0, 0);
-	struct sigaction sa; memset(&sa, 0, sizeof sa); sa.sa_handler = on_signal;
-	sigaction(SIGINT, &sa, NULL); sigaction(SIGTERM, &sa, NULL); sigaction(SIGQUIT, &sa, NULL);
-	signal(SIGPIPE, SIG_IGN);
-	if (direct_sampling) { SoapySDRDevice_writeSetting(dev, "direct_samp", direct_sampling == 1 ? "1" : "2"); }
-	if (offset_tuning) { SoapySDRDevice_writeSetting(dev, "offset_tune", "true"); }
-	sdr_set_gain(dev, channel, gain_str);
-	SoapySDRDevice_setFrequencyCorrection(dev, SOAPY_SDR_RX, channel, (double)ppm);
-	FILE *out = !strcmp(filename, "-") ? stdout : fopen(filename, "wb");
-	if (!out) { fprintf(stderr, "Failed to open %s\n", filename); return 1; }
+	FILE *out = open_radio(dev_query, channel, antenna, gain_str, ppm, direct_sampling, offset_tuning, filename, &dev, &stream);
+	if (!out) { return 1; }
 	SoapySDRDevice_setSampleRate(dev, SOAPY_SDR_RX, channel, (double)plan.rate);
 
 	/* buffers: one read of buf_len COMPLEX elements per hop (the reference asks for that many, src/rtl_power.c:694),
@@ -298,22 +407,14 @@ int main(int argc, char **argv)
 	const long max_sweeps = hook ? atol(hook) : 0;
 	long sweeps = 0;
 	time_t next_tick = time(NULL) + interval, exit_time = exit_after ? time(NULL) + exit_after : 0;
-	SoapySDRKwargs none = {0, NULL, NULL};
 	int done = 0;
 	while (!done && !g_stop) {
 		/* ---- one sweep: scanner()'s device side (:679-708) */
 		int first_ok = -1, n_ok = 0;
 		for (int i = 0; i < n_hops && g_stop < 2; i++) {
 			const int64_t f = plan.first_freq + (int64_t)i * plan.freq_step;
-			if ((int64_t)SoapySDRDevice_getFrequency(dev, SOAPY_SDR_RX, channel) != f) {       /* retune() :548-580 */
-				if (SoapySDRDevice_setFrequency(dev, SOAPY_SDR_RX, channel, (double)f, &none) != 0) {
-					fprintf(stderr, "Error: failed to set frequency %lli Hz\n", (long long)f);
-				} else {
-					usleep((useconds_t)tuner_sleep_usec);
-					int r = -1, flags = 0; long long tn = 0; void *db[] = {dump};
-					for (int a = 0; a < tuner_retry_max && r < 0; a++) { r = SoapySDRDevice_readStream(dev, stream, db, BUFFER_DUMP, &flags, &tn, 1000000); }
-					if (r < 0) { fprintf(stderr, "Error: bad retune at %lli Hz, r=%d (try increasing -S or -R).\n", (long long)f, r); }
-				}
+			if ((int64_t)SoapySDRDevice_getFrequency(dev, SOAPY_SDR_RX, channel) != f) {
+				retune(dev, stream, channel, f, dump, tuner_sleep_usec, tuner_retry_max);
 			}
 			void *buffs[] = {rd};
 			int flags = 0; long long tn = 0;

@@ -605,6 +605,52 @@ int rxb200_power_ddc_device(int capture_rate, int offset_hz, unsigned long long 
  * corrected so that sum h = 2^shift exactly.  Pure host arithmetic. */
 int rxb200_ddc_lowpass(int decim, int n_taps, int shift, int32_t *taps);
 
+/* ---- wide sweeps in tiles (DESIGN.md section 4.5, "Wide sweeps in tiles")
+ * A sweep wider than one capture is cut into tiles of consecutive hops; the radio is tuned once per tile and the tile's
+ * hops are taken from one burst, a fresh capture after the retune.  The tiling of a plan for captures of at most
+ * max_capture_rate Hz, with r = plan->rate, s = freq_step, F0 = first_freq and n = n_hops:
+ *   Mcap = min(4096, floor(min(max_capture_rate, 2^31 - 1) / r)); Mcap < 1 is refused (RXB200_EINVAL).
+ *   A run of k hops is centred at its first hop plus c(k) = floor((k - 1) s / 2) and needs
+ *   Mreq(k) = ceil((2 max(c(k), (k - 1) s - c(k)) + r) / r), the capture mode's rule for the same hops.
+ *   hmax is the largest k <= n with Mreq(k) <= Mcap (k = 1 always fits).
+ *   n_tiles = ceil(n / hmax), h = ceil(n / n_tiles): no tile is empty, since (n_tiles - 1) h <= (n_tiles - 1) hmax < n.
+ *   M = Mreq(h), R = M r, T = min(8191, 32 M + 1).
+ *   Tile t holds hops [t h, min((t+1) h, n)) and is centred at F0 + t h s + c(len_t); hop i's offset is its frequency
+ *   minus its tile's centre, so |f_i| < R/2.
+ * With one tile this is exactly the centre, offsets, M, R and T of the shell's capture mode.  Pure host arithmetic. */
+typedef struct rxb200_power_tiling {
+	int n_tiles;
+	int hops_per_tile;   /* h: tile t holds hops [t h, min((t+1) h, n_hops)) */
+	int decim;           /* M */
+	int n_taps;          /* T = min(8191, 32 M + 1), the capture mode's filter length */
+	int capture_rate;    /* R = M * plan->rate */
+} rxb200_power_tiling;
+/* offsets_hz: n_hops ints, each hop's offset from its tile's centre, or NULL.  RXB200_EINVAL for NULL plan or out, a
+ * plan with n_hops < 1, rate < 1 or freq_step < 0, and Mcap < 1. */
+int rxb200_power_plan_tiles(const rxb200_power_plan *plan, long long max_capture_rate,
+                            rxb200_power_tiling *out, int *offsets_hz /* n_hops, may be NULL */);
+/* Tile t's hop range and centre (Hz); RXB200_EINVAL for a NULL argument or t outside [0, n_tiles). */
+int rxb200_power_tile(const rxb200_power_plan *plan, const rxb200_power_tiling *tl, int t,
+                      int *hop_begin, int *hop_end, int64_t *centre_hz);
+/* Bursts.  A burst is one self-contained capture, not a continuation of the handle's stream: n_int16 = 2G + P M buf_len
+ * int16 with P >= 1, where the lead G = M ceil((T - 1) / M) complex samples (rxb200_power_mix_lead) primes the filter.
+ * Any other length is RXB200_EUNSUPPORTED; a hop range other than 0 <= hb < he <= n_hops, a NULL pointer or a device
+ * pointer that is not 4-byte aligned is RXB200_EINVAL; a refused call changes nothing.
+ * For hop i in [hb, he), n counts from the burst's first sample (the lead included) and z_i is the NCO rule above at
+ * that n.  Output m is emitted at e_m = G + m M + M - 1 with the filter rule above word for word; every index it reads
+ * is >= 0, so no zeros enter.  Outputs [p B, (p+1) B) are pass p of hop i, and the call accumulates what
+ * rxb200_power_accumulate(member, bufs, P, hb, he) would.  Equivalently they are outputs G/M + u of
+ * rxb200_power_ddc_device(R, f_i, 0, ddc, burst, n_complex).  A burst neither reads nor moves the handle's sample count
+ * or filter history: continuous rxb200_power_mix_accumulate calls before and after it see one unbroken stream.
+ * The offsets at create may be relative to different tile centres; create's rule |f_i| < R/2 is unchanged. */
+int rxb200_power_mix_lead(const rxb200_power_mix *m);   /* G, or RXB200_EINVAL for NULL */
+/* cs16: HOST pointer to the burst, staged through the handle's device buffer; synchronous. */
+int rxb200_power_mix_accumulate_burst(rxb200_power_mix *m, int hop_begin, int hop_end,
+                                      const int16_t *cs16, size_t n_int16);
+/* Same with a DEVICE burst (4-byte aligned), asynchronous on the member's stream unless sync != 0. */
+int rxb200_power_mix_accumulate_burst_device(rxb200_power_mix *m, int hop_begin, int hop_end,
+                                             const int16_t *d_cs16, size_t n_int16, int sync);
+
 /* ======================================================================== rx_sdr (SURVEY.md §8f row 4)
  * The pointwise sample-format conversions of rx_sdr's recorder loop (src/rtl_sdr.c:348-391):
  *   RXB200_CVT_CS16_CS8  : (uint8_t)(int)(x/32767.0*128.0+0.4)       per int16 (:367-370)

@@ -63,6 +63,11 @@ class PowerPlanC(C.Structure):
                 ("first_freq", C.c_int64), ("freq_step", C.c_int64), ("bin_size_hz", C.c_double)]
 
 
+class PowerTilingC(C.Structure):
+    _fields_ = [("n_tiles", C.c_int), ("hops_per_tile", C.c_int), ("decim", C.c_int), ("n_taps", C.c_int),
+                ("capture_rate", C.c_int)]
+
+
 # every symbol include/rxb200.h declares (tests/test_abi.py checks the header against this list)
 SYMBOLS = [
     "rxb200_last_error", "rxb200_abi_version", "rxb200_device_count",
@@ -93,6 +98,8 @@ SYMBOLS = [
     "rxb200_power_mix_create", "rxb200_power_mix_destroy", "rxb200_power_mix_member", "rxb200_power_mix_reset",
     "rxb200_power_mix_accumulate", "rxb200_power_mix_accumulate_device", "rxb200_power_mix_kernel_ms",
     "rxb200_nco_table", "rxb200_power_ddc_device", "rxb200_ddc_lowpass",
+    "rxb200_power_plan_tiles", "rxb200_power_tile", "rxb200_power_mix_lead", "rxb200_power_mix_accumulate_burst",
+    "rxb200_power_mix_accumulate_burst_device",
     "rxb200_sdr_convert", "rxb200_sdr_convert_device",
 ]
 
@@ -231,6 +238,12 @@ def lib() -> C.CDLL:
     L.rxb200_power_ddc_device.argtypes = [C.c_int, C.c_int, C.c_ulonglong, C.POINTER(DdcC), C.c_void_p, sz, C.c_void_p,
                                           C.c_void_p]
     L.rxb200_ddc_lowpass.argtypes = [C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int32)]
+    L.rxb200_power_plan_tiles.argtypes = [C.POINTER(PowerPlanC), C.c_longlong, C.POINTER(PowerTilingC), pint]
+    L.rxb200_power_tile.argtypes = [C.POINTER(PowerPlanC), C.POINTER(PowerTilingC), C.c_int, pint, pint,
+                                    C.POINTER(C.c_int64)]
+    L.rxb200_power_mix_lead.argtypes = [C.c_void_p]
+    L.rxb200_power_mix_accumulate_burst.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, sz]
+    L.rxb200_power_mix_accumulate_burst_device.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, sz, C.c_int]
     L.rxb200_sdr_convert.argtypes = [C.c_int, C.c_void_p, sz, C.c_void_p, C.c_int]
     L.rxb200_sdr_convert_device.argtypes = [C.c_int, C.c_void_p, sz, C.c_void_p, C.c_void_p]
     _lib = L

@@ -8,6 +8,7 @@
 #include <stdarg.h>
 #include <stdio.h>
 #include <string.h>
+#include <algorithm>
 #include <vector>
 #include <cuda_runtime.h>
 #include "../../include/rxb200.h"
@@ -142,6 +143,62 @@ extern "C" int rxb200_ddc_lowpass(int decim, int n_taps, int shift, int32_t *tap
 		q += taps[j];
 	}
 	taps[c] += (int32_t)((1ll << shift) - q);
+	return RXB200_OK;
+}
+
+// The tiling of a sweep wider than one capture (include/rxb200.h, "wide sweeps in tiles"): c(k) is the centre of a run
+// of k hops from its first hop, Mreq(k) the decimation a capture centred there needs.
+static long long tile_centre(long long k, long long s) { return (k - 1) * s / 2; }
+static long long tile_decim(long long k, long long s, long long r)
+{
+	const long long c = tile_centre(k, s), half = std::max(c, (k - 1) * s - c);
+	return (2 * half + r + r - 1) / r;
+}
+
+extern "C" int rxb200_power_plan_tiles(const rxb200_power_plan *plan, long long max_capture_rate,
+                                       rxb200_power_tiling *out, int *offsets_hz)
+{
+	if (!plan || !out) { set_error("null argument"); return RXB200_EINVAL; }
+	const long long n = plan->params.n_hops, r = plan->rate, s = plan->freq_step;
+	if (n < 1 || r < 1 || s < 0) {
+		set_error("tiling: plan with n_hops %lld, rate %lld, freq_step %lld (need n_hops, rate >= 1, freq_step >= 0)", n, r, s);
+		return RXB200_EINVAL;
+	}
+	const long long mcap = std::min(4096ll, std::min(max_capture_rate, 2147483647ll) / r);
+	if (mcap < 1) {
+		set_error("tiling: a capture rate of at most %lld Hz is below the hop rate %lld Hz", max_capture_rate, r);
+		return RXB200_EINVAL;
+	}
+	long long hmax = 1;                                  // Mreq is non-decreasing in k
+	while (hmax < n && tile_decim(hmax + 1, s, r) <= mcap) { hmax++; }
+	const long long n_tiles = (n + hmax - 1) / hmax, h = (n + n_tiles - 1) / n_tiles, M = tile_decim(h, s, r);
+	out->n_tiles = (int)n_tiles;
+	out->hops_per_tile = (int)h;
+	out->decim = (int)M;
+	out->n_taps = (int)std::min(8191ll, 32 * M + 1);
+	out->capture_rate = (int)(M * r);
+	if (offsets_hz) {
+		for (long long i = 0; i < n; i++) {
+			const long long t = i / h, len = std::min(h, n - t * h);
+			offsets_hz[i] = (int)((i - t * h) * s - tile_centre(len, s));
+		}
+	}
+	return RXB200_OK;
+}
+
+extern "C" int rxb200_power_tile(const rxb200_power_plan *plan, const rxb200_power_tiling *tl, int t,
+                                 int *hop_begin, int *hop_end, int64_t *centre_hz)
+{
+	if (!plan || !tl || !hop_begin || !hop_end || !centre_hz) { set_error("null argument"); return RXB200_EINVAL; }
+	if (t < 0 || t >= tl->n_tiles || tl->hops_per_tile < 1) {
+		set_error("tile %d outside [0, %d)", t, tl->n_tiles);
+		return RXB200_EINVAL;
+	}
+	const long long h = tl->hops_per_tile, b = (long long)t * h, e = std::min(b + h, (long long)plan->params.n_hops);
+	if (b >= e) { set_error("tile %d of %d hops is empty", t, plan->params.n_hops); return RXB200_EINVAL; }
+	*hop_begin = (int)b;
+	*hop_end = (int)e;
+	*centre_hz = plan->first_freq + (int64_t)b * plan->freq_step + (int64_t)tile_centre(e - b, plan->freq_step);
 	return RXB200_OK;
 }
 

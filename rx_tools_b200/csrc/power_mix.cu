@@ -3,7 +3,9 @@
 // decimates it, and writes each hop's outputs straight into the pass-major hop buffers ([pass][hop][buf_len]) that
 // rxb200_power_accumulate_device reads; the member rxb200_power handle then accumulates them on its own stream.  The
 // kernel is ddc.cuh's down-converter with the NCO mixer below.  The handle carries the sample count (the NCO phases)
-// and its filter state (DdcFilter) between calls.
+// and its filter state (DdcFilter) between calls.  A burst (a fresh capture after a retune, for a tile of a wide sweep)
+// runs the same kernel on a subset of the hops, with its history read from the burst's own lead and its phases counted
+// from its first sample, and leaves the carried state alone.
 #include <math.h>
 #include <algorithm>
 #include <cstring>
@@ -91,7 +93,7 @@ struct rxb200_power_mix {
 	int2 *d_nco = nullptr;                       // the shared NCO table
 	unsigned long long pos = 0;                  // capture samples since create or reset (whole passes)
 	int16_t *d_cap = nullptr; size_t cap_cap = 0;     // host calls: the capture (int16 elements)
-	int16_t *d_bufs = nullptr; size_t bufs_cap = 0;   // the hop buffers of one group of passes, [P][n_hops][buf_len]
+	int16_t *d_bufs = nullptr; size_t bufs_cap = 0;   // the hop buffers of one group of passes, [P][he - hb][buf_len]
 	std::vector<cudaEvent_t> ev;                 // pairs around each DDC launch of the last call
 	int n_ev = 0;                                // pairs recorded by the last call
 };
@@ -155,20 +157,36 @@ extern "C" int rxb200_power_mix_reset(rxb200_power_mix *m)
 
 namespace {
 
-// One call of either entry point: the capture's passes in groups of at most RXB200_POWER_MIX_SCRATCH_BYTES of hop
-// buffers, each group one DDC launch into the scratch buffer and one accumulate of the member.  device: cs16 is a device
-// pointer, else a host pointer staged through the handle's buffer.
-int power_mix_call(rxb200_power_mix *m, const int16_t *cs16, size_t n_int16, bool device, int sync)
+// G = M ceil((T - 1) / M): the lead of a burst, in complex samples
+size_t burst_lead(const DdcFilter &f) { return (size_t)f.M * (((size_t)f.T - 1 + (size_t)f.M - 1) / (size_t)f.M); }
+
+// One call of any entry point: the passes of hops [hb, he) in groups of at most RXB200_POWER_MIX_SCRATCH_BYTES of hop
+// buffers, each group one DDC launch into the scratch buffer ([P][he - hb][buf_len]) and one accumulate of the member.
+// device: cs16 is a device pointer, else a host pointer staged through the handle's buffer.  burst: cs16 is a burst
+// (its lead, then whole passes), whose groups read their history from the burst itself at positions counted from its
+// first sample; else cs16 continues the handle's stream, whose history and sample count each group carries on.
+int power_mix_call(rxb200_power_mix *m, int hb, int he, const int16_t *cs16, size_t n_int16, bool device, int sync,
+                   bool burst)
 {
 	if (!m || !cs16) { set_error("null argument"); return RXB200_EINVAL; }
+	if (hb < 0 || hb >= he || he > m->n_hops) {
+		set_error("hop range [%d, %d) needs 0 <= hop_begin < hop_end <= n_hops = %d", hb, he, m->n_hops);
+		return RXB200_EINVAL;
+	}
 	if (device && ((uintptr_t)cs16 & 3u) != 0) { set_error("d_cs16 must be 4-byte aligned"); return RXB200_EINVAL; }
 	const size_t M = (size_t)m->f.M, L = (size_t)m->buf_len, pass16 = M * L;
-	if (n_int16 % pass16 != 0) {
+	const size_t lead16 = burst ? 2 * burst_lead(m->f) : 0;
+	if (burst && (n_int16 < lead16 + pass16 || (n_int16 - lead16) % pass16 != 0)) {
+		set_error("n_int16=%zu must be the lead 2G = %zu plus a positive multiple of decim * buf_len = %zu", n_int16,
+		          lead16, pass16);
+		return RXB200_EUNSUPPORTED;
+	}
+	if (n_int16 % pass16 != 0 && !burst) {
 		set_error("n_int16=%zu must be a multiple of decim * buf_len = %zu (whole passes)", n_int16, pass16);
 		return RXB200_EUNSUPPORTED;
 	}
 	if (n_int16 == 0) { return RXB200_OK; }
-	const size_t n_pass = n_int16 / pass16, hops = (size_t)m->n_hops;
+	const size_t n_pass = (n_int16 - lead16) / pass16, hops = (size_t)(he - hb);
 	const size_t per_pass = hops * L * sizeof(int16_t);
 	const size_t group = std::max<size_t>(1, std::min<size_t>(n_pass, RXB200_POWER_MIX_SCRATCH_BYTES / per_pass));
 	RXB_CUDA(cudaSetDevice(m->device));
@@ -191,25 +209,28 @@ int power_mix_call(rxb200_power_mix *m, const int16_t *cs16, size_t n_int16, boo
 	for (size_t p0 = 0; p0 < n_pass; p0 += group) {
 		const size_t P = std::min(group, n_pass - p0);
 		DdcArgs<NcoMix> a{};
-		a.src = reinterpret_cast<const uint32_t *>(src + p0 * pass16);
-		a.hist = f.hist[f.cur];
+		a.src = reinterpret_cast<const uint32_t *>(src + lead16 + p0 * pass16);
+		// a burst's lead is at least T - 1 samples, so its history is the samples just before src in the burst
+		a.hist = burst ? a.src - (f.T - 1) : f.hist[f.cur];
 		a.n_out = (long long)(P * L / 2);
-		a.r0 = (long long)M - 1;                             // pos is a whole number of passes, so of M
-		a.pos = m->pos;
+		a.r0 = (long long)M - 1;                             // pos is the lead plus whole passes, so a multiple of M
+		a.pos = burst ? (lead16 + p0 * pass16) / 2 : m->pos;
 		a.dst = reinterpret_cast<uint32_t *>(m->d_bufs);
 		a.taps = f.taps;
-		a.n_ch = m->n_hops; a.M = f.M; a.T = f.T; a.S = f.S;
-		a.mix = NcoMix{m->d_nco, m->d_w, (int)(L / 2)};
+		a.n_ch = he - hb; a.M = f.M; a.T = f.T; a.S = f.S;
+		a.mix = NcoMix{m->d_nco, m->d_w + hb, (int)(L / 2)};
 		RXB_CUDA(cudaEventRecord(m->ev[(size_t)2 * m->n_ev], st));
 		int rc = ddc_launch(a, f.wide ? power_ddc_kernel<long long> : power_ddc_kernel<int>, st);
 		if (rc != RXB200_OK) { return rc; }
 		RXB_CUDA(cudaEventRecord(m->ev[(size_t)2 * m->n_ev + 1], st));
 		m->n_ev++;
-		rc = f.carry(a.src, P * pass16 / 2, st);
-		if (rc != RXB200_OK) { return rc; }
-		f.commit();
-		m->pos += P * pass16 / 2;
-		rc = rxb200_power_accumulate_device(m->h, m->d_bufs, (int)P, 0, m->n_hops, 0);
+		if (!burst) {
+			rc = f.carry(a.src, P * pass16 / 2, st);
+			if (rc != RXB200_OK) { return rc; }
+			f.commit();
+			m->pos += P * pass16 / 2;
+		}
+		rc = rxb200_power_accumulate_device(m->h, m->d_bufs, (int)P, hb, he, 0);
 		if (rc != RXB200_OK) { return rc; }
 	}
 	if (!device || sync) { RXB_CUDA(cudaStreamSynchronize(st)); }
@@ -220,12 +241,30 @@ int power_mix_call(rxb200_power_mix *m, const int16_t *cs16, size_t n_int16, boo
 
 extern "C" int rxb200_power_mix_accumulate(rxb200_power_mix *m, const int16_t *cs16, size_t n_int16)
 {
-	return power_mix_call(m, cs16, n_int16, false, 1);
+	return power_mix_call(m, 0, m ? m->n_hops : 1, cs16, n_int16, false, 1, false);
 }
 
 extern "C" int rxb200_power_mix_accumulate_device(rxb200_power_mix *m, const int16_t *d_cs16, size_t n_int16, int sync)
 {
-	return power_mix_call(m, d_cs16, n_int16, true, sync);
+	return power_mix_call(m, 0, m ? m->n_hops : 1, d_cs16, n_int16, true, sync, false);
+}
+
+extern "C" int rxb200_power_mix_lead(const rxb200_power_mix *m)
+{
+	if (!m) { set_error("null argument"); return RXB200_EINVAL; }
+	return (int)burst_lead(m->f);
+}
+
+extern "C" int rxb200_power_mix_accumulate_burst(rxb200_power_mix *m, int hop_begin, int hop_end, const int16_t *cs16,
+                                                 size_t n_int16)
+{
+	return power_mix_call(m, hop_begin, hop_end, cs16, n_int16, false, 1, true);
+}
+
+extern "C" int rxb200_power_mix_accumulate_burst_device(rxb200_power_mix *m, int hop_begin, int hop_end,
+                                                        const int16_t *d_cs16, size_t n_int16, int sync)
+{
+	return power_mix_call(m, hop_begin, hop_end, d_cs16, n_int16, true, sync, true);
 }
 
 extern "C" int rxb200_power_mix_kernel_ms(rxb200_power_mix *m, float *ms)

@@ -4,7 +4,8 @@
 ``main()`` builds (:1028, :1034-1037), ``PowerScanner.scanner`` is n passes of ``scanner()`` (:670-772)
 over hop buffers, executed by the batched sm_90a kernel behind ``rxb200_power_accumulate``
 (include/rxb200.h); ``csv_rows`` is ``csv_dbm()`` (:774-817).  ``PowerMix`` takes every hop of a sweep from one
-wideband capture through an NCO down-converter on the GPU (``rxb200_power_mix_*``).
+wideband capture through an NCO down-converter on the GPU (``rxb200_power_mix_*``); ``plan_tiles`` cuts a sweep wider
+than one capture into tiles, each taken from one burst (``PowerMix.accumulate_burst``).
 """
 from __future__ import annotations
 
@@ -252,6 +253,54 @@ class PowerMix(PowerScanner):
     def accumulate_ms(self) -> float:
         """Device time of the member's last accumulate kernel (ms)."""
         return PowerScanner.kernel_ms(self)
+
+    @property
+    def lead(self) -> int:
+        """G = M ceil((T - 1) / M): the complex samples at the front of a burst that prime the filter."""
+        return _lib.check(_lib.lib().rxb200_power_mix_lead(self._m))
+
+    def burst_int16(self, n_pass: int = 1) -> int:
+        """Capture int16 of a burst of n_pass passes: 2 G + n_pass M buf_len."""
+        return 2 * self.lead + n_pass * self.pass_int16
+
+    def accumulate_burst(self, hop_begin: int, hop_end: int, capture: np.ndarray) -> None:
+        """One burst (host int16 CS16: the lead, then whole passes) for hops [hop_begin, hop_end).  The handle's
+        carried phases and filter history are left as they are."""
+        x = np.ascontiguousarray(capture, dtype=np.int16).reshape(-1)
+        _lib.check(_lib.lib().rxb200_power_mix_accumulate_burst(self._m, hop_begin, hop_end, x.ctypes.data, x.size))
+
+    def accumulate_burst_device(self, hop_begin: int, hop_end: int, d_ptr: int, n_int16: int,
+                                sync: bool = False) -> None:
+        _lib.check(_lib.lib().rxb200_power_mix_accumulate_burst_device(self._m, hop_begin, hop_end, d_ptr, n_int16,
+                                                                       1 if sync else 0))
+
+
+@dataclass
+class Tiling:
+    """rxb200_power_tiling: n_tiles tiles of up to hops_per_tile hops, each taken from one capture at capture_rate
+    (decim times the hop rate) through a filter of n_taps taps."""
+    n_tiles: int
+    hops_per_tile: int
+    decim: int
+    n_taps: int
+    capture_rate: int
+
+
+def plan_tiles(plan: Plan, max_rate: int):
+    """The tiling of a sweep for captures of at most max_rate Hz (``rxb200_power_plan_tiles``): (Tiling, each tile's
+    (hop_begin, hop_end, centre_hz), each hop's offset from its tile's centre)."""
+    pc = _lib.PowerPlanC(plan.to_c(), plan.rate, plan.crop, plan.first_freq, plan.freq_step, plan.bin_size_hz)
+    tl = _lib.PowerTilingC()
+    offs = np.zeros(plan.n_hops, dtype=np.int32)
+    _lib.check(_lib.lib().rxb200_power_plan_tiles(C.byref(pc), int(max_rate), C.byref(tl),
+                                                  offs.ctypes.data_as(C.POINTER(C.c_int))))
+    tiles = []
+    for t in range(tl.n_tiles):
+        b, e, c = C.c_int(0), C.c_int(0), C.c_int64(0)
+        _lib.check(_lib.lib().rxb200_power_tile(C.byref(pc), C.byref(tl), t, C.byref(b), C.byref(e), C.byref(c)))
+        tiles.append((b.value, e.value, c.value))
+    return (Tiling(tl.n_tiles, tl.hops_per_tile, tl.decim, tl.n_taps, tl.capture_rate), tiles,
+            [int(v) for v in offs])
 
 
 def nco_table() -> np.ndarray:
