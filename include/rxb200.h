@@ -509,6 +509,41 @@ size_t rxb200_fm_mix_max_output(const rxb200_fm_mix *m, size_t n_int16, size_t c
 int rxb200_ddc_device(int capture_rate, int offset_hz, long long phase, const rxb200_ddc *ddc, const int16_t *d_src,
                       size_t n_complex, int16_t *d_dst, void *stream);
 
+/* ---- raster mixing handles: the channels of a uniform raster through a polyphase channelizer (DESIGN.md section 4.4,
+ * "Channels on a raster")
+ * A raster handle has K bins (3 <= K <= 4096) over the capture and n_channels channels, channel c being bin k_c
+ * (0 <= k_c < K; bins may repeat), centred at k_c R / K for a capture rate R (negative for k_c > K/2), plus one rxb200_ddc
+ * (M, T taps h, S) shared by every channel.  Let x[n] be the capture, n counting complex samples from create or reset
+ * across calls, x[n] = 0 for n < 0, and tw[r] = (c, s) entry r of rxb200_fm_mix_table(K, 1) (the period-K table:
+ * round(2^15 cos, sin) of -2 pi r' / K, r' the representative of r in (-K/2, K/2], so bins k and K - k are conjugates).
+ * Output m of channel c (bin k) is emitted at e_m = m*M + M - 1:
+ *     A = sum_{j<T} h[j] * x[e_m - j] * tw[(k (e_m - j)) mod K]   (complex, exact: no rounding anywhere in the sum);
+ *     y = S ? (A + 2^(S-1)) >> S : A   (arithmetic, I and Q separately);   out = y saturated to [-32768, 32767].
+ * This is the decimating handle's rule at offset k R / K without the mixer's per-sample >> 15 rounding and int16 wrap, so
+ * it is not byte for byte that handle.  Two anchors are exact: bin 0 at shift S + 15 is the decimating handle at offset 0
+ * with shift S; and bin K/4 (4 | K) at shift S + 15 is the decimating handle at offset R/4 with shift S whenever no I or
+ * Q sample is -32768 (the quarter-turn mixer wraps there).  Everything else is a decimating handle's: the decimated length, the chunk rule (multiples of 2M), a
+ * read with no output, the refusals on the decimated shape, reset, and every rxb200_fm_mix_* entry point; there is no
+ * capture rate, and rxb200_fm_mix_kernel_ms reports the two raster kernels of the last call summed.
+ * raster_branch_kernel sums each output's taps by residue rho = (e_m - j) mod K into v_rho (fp64, exact below 2^37),
+ * and raster_dft_kernel multiplies those rows by the handle's constant [2K][2C] twiddle matrix on FP64 tensor cores
+ * (DMMA); every product and partial sum is an integer below 2^53, so the result is exact in any summation order.  The
+ * branch sums of a long call go through a scratch buffer in groups of at most RXB200_RASTER_SCRATCH_BYTES of frames;
+ * the bytes are the same as with one group. */
+#define RXB200_RASTER_SCRATCH_BYTES (64u << 20)
+/* Refusals, all before any device is touched: those of rxb200_fm_mix_create_ddc for params and ddc; RXB200_EINVAL for
+ * K outside [3, 4096], NULL bins, n_channels < 1, any bin outside [0, K), or sum |h| >= 2^22 (which keeps every partial
+ * sum, |A| <= sum |h| 2^31, below 2^53). */
+int rxb200_fm_mix_create_raster(const rxb200_fm_params *params, int n_bins, const int *bins /* n_channels */,
+                                int n_channels, const rxb200_ddc *ddc, int device, rxb200_fm_mix **out);
+/* The raster down-converter alone on DEVICE pointers, stateless, on `stream`: d_src[i] is capture sample n0 + i (its
+ * twiddle uses (k (n0 + i)) mod K, n0 + i taken as an exact integer), the samples before d_src are zero, and
+ * floor(n_complex / M) outputs per channel go to d_dst, channel c's at d_dst + 2 c floor(n_complex / M), e_m counted
+ * from d_src.  Both pointers 4-byte aligned.  The refusals of rxb200_fm_mix_create_raster for K, bins and ddc.
+ * Asynchronous. */
+int rxb200_raster_device(int n_bins, const int *bins, int n_channels, unsigned long long n0, const rxb200_ddc *ddc,
+                         const int16_t *d_src, size_t n_complex, int16_t *d_dst, void *stream);
+
 /* ======================================================================== rx_fm channels of one capture on several GPUs
  * The channels of ONE capture split over GPUs: one process, n_dev rxb200_fm_mix handles, member i owning the contiguous
  * channels [b, e) that rxb200_power_shard(n_channels, n_dev, i, &b, &e) gives, with offsets offsets_hz[b..e).  A member

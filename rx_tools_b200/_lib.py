@@ -94,7 +94,7 @@ SYMBOLS = [
     "rxb200_fm_mix_group_member", "rxb200_fm_mix_group_process", "rxb200_fm_mix_group_process_read",
     "rxb200_fm_mix_group_squelch_hits", "rxb200_fm_mix_group_levels", "rxb200_fm_mix_group_reset",
     "rxb200_fm_mix_create_ddc", "rxb200_fm_mix_decimated_len", "rxb200_fm_mix_max_output", "rxb200_ddc_device",
-    "rxb200_fm_mix_group_create_ddc",
+    "rxb200_fm_mix_group_create_ddc", "rxb200_fm_mix_create_raster", "rxb200_raster_device",
     "rxb200_power_mix_create", "rxb200_power_mix_destroy", "rxb200_power_mix_member", "rxb200_power_mix_reset",
     "rxb200_power_mix_accumulate", "rxb200_power_mix_accumulate_device", "rxb200_power_mix_kernel_ms",
     "rxb200_nco_table", "rxb200_power_ddc_device", "rxb200_ddc_lowpass",
@@ -224,6 +224,10 @@ def lib() -> C.CDLL:
                                     C.c_void_p]
     L.rxb200_fm_mix_group_create_ddc.argtypes = [C.POINTER(FmParamsC), C.c_int, pint, C.c_int, C.POINTER(DdcC),
                                                  C.c_int, pint, C.POINTER(C.c_void_p)]
+    L.rxb200_fm_mix_create_raster.argtypes = [C.POINTER(FmParamsC), C.c_int, pint, C.c_int, C.POINTER(DdcC), C.c_int,
+                                              C.POINTER(C.c_void_p)]
+    L.rxb200_raster_device.argtypes = [C.c_int, pint, C.c_int, C.c_ulonglong, C.POINTER(DdcC), C.c_void_p, sz,
+                                       C.c_void_p, C.c_void_p]
     L.rxb200_power_mix_create.argtypes = [C.POINTER(PowerParamsC), pint, p16, C.c_int, pint, C.POINTER(DdcC), C.c_int,
                                           C.POINTER(C.c_void_p)]
     L.rxb200_power_mix_destroy.argtypes = [C.c_void_p]

@@ -3,15 +3,17 @@
 // once and writing one CS16 stream per channel; a plain rxb200_fm handle with one channel per stream then runs the
 // chain on them through its device entry points.  A decimating handle (rxb200_fm_mix_create_ddc) runs fm_ddc_kernel
 // instead (ddc.cuh's down-converter with the channels' tables), which mixes, filters and decimates, and carries its
-// filter state (DdcFilter) between calls.  Every
-// process entry point of both kinds goes through mix_call, whose refusals and member shape come from
-// fm_mix_check_host_call (which the group uses too).  The chain itself is not touched here.
+// filter state (DdcFilter) between calls.  A raster handle (rxb200_fm_mix_create_raster) is a decimating handle whose
+// front stage is fm_raster.cu's polyphase channelizer instead.  Every process entry point of every kind goes through
+// mix_call, whose refusals and member shape come from fm_mix_check_host_call (which the group uses too).  The chain
+// itself is not touched here.
 #include <algorithm>
 #include <cstring>
 #include <new>
 #include <vector>
 #include "common.cuh"
 #include "ddc.cuh"
+#include "raster.cuh"
 
 namespace rxb {
 
@@ -198,11 +200,16 @@ struct rxb200_fm_mix {
 	int16_t *d_cap = nullptr; size_t cap_cap = 0;   // host calls: the capture (int16 elements)
 	int16_t *d_mix = nullptr; size_t mix_cap = 0;   // the mixed streams, [n_channels][n_int16]
 	int16_t *d_out = nullptr; size_t out_cap = 0;   // host calls: the PCM rows, total + 8 apart
-	cudaEvent_t ev0 = nullptr, ev1 = nullptr;    // around the last fm_mix_kernel (fm_ddc_kernel)
+	cudaEvent_t ev0 = nullptr, ev1 = nullptr;    // around the last fm_mix_kernel (fm_ddc_kernel, the raster kernels)
 	// a decimating handle (rxb200_fm_mix_create_ddc): fm_ddc_kernel writes the decimated streams to d_mix ([n_channels]
 	// [n_dec_int16]) and the member runs on those
 	bool ddc = false;
 	DdcFilter f;                                 // its filter state (T = 1 for a plain handle)
+	// a raster handle (rxb200_fm_mix_create_raster, r.K > 0): a decimating handle with no mixer tables, whose front
+	// stage is raster_front with the twiddle matrix d_wt and the branch sums' scratch d_v
+	RasterPlan r;
+	double *d_wt = nullptr;
+	double *d_v = nullptr; size_t v_cap = 0;     // doubles
 };
 
 namespace {
@@ -273,9 +280,21 @@ int ddc_front(rxb200_fm_mix *m, const int16_t *src, size_t n16, cudaStream_t st)
 	return ddc_launch(a, f.wide ? fm_ddc_kernel<long long> : fm_ddc_kernel<int>, st);
 }
 
+// a raster handle's front stage: raster_front from the call's capture at src to n16 int16 per channel in d_mix
+int raster_call_front(rxb200_fm_mix *m, const int16_t *src, size_t n16, cudaStream_t st)
+{
+	const DdcFilter &f = m->f;
+	const long long n_out = (long long)(n16 / 2);
+	RXB_CUDA(reserve(m->d_v, m->v_cap, (size_t)std::min(n_out, m->r.group) * (size_t)m->r.Kp));
+	return raster_front(m->r, m->d_wt, m->d_v, reinterpret_cast<const uint32_t *>(src), f.hist[f.cur], f.taps, f.M, f.T,
+	                    f.S, (long long)(f.M - 1) - (long long)(m->pos % (unsigned long long)f.M),
+	                    (unsigned)(m->pos % (unsigned long long)m->r.K), n_out, reinterpret_cast<uint32_t *>(m->d_mix),
+	                    n_out, st);
+}
+
 // One call of any process entry point.  device: cs16 and pcm are device pointers (the member's device entry point
 // writes pcm), else host pointers staged through the handle's buffers.  read: one read (chunk_int16 == n_int16).  The
-// front stage (fm_mix_kernel, or fm_ddc_kernel for a decimating handle) writes the member's input to d_mix; when it has
+// front stage (fm_mix_kernel, fm_ddc_kernel for a decimating handle, the raster kernels for a raster handle) writes the member's input to d_mix; when it has
 // no output (n16 == 0) neither it nor the member runs, but the phases and the history still advance.
 int mix_call(rxb200_fm_mix *m, const int16_t *cs16, size_t n_int16, size_t chunk_int16, int16_t *pcm, size_t pcm_stride,
              size_t *n_pcm, int *chunk_result_len, bool read, bool device, int sync)
@@ -299,7 +318,8 @@ int mix_call(rxb200_fm_mix *m, const int16_t *cs16, size_t n_int16, size_t chunk
 	}
 	RXB_CUDA(cudaEventRecord(m->ev0, st));
 	if (n16) {
-		rc = m->ddc ? ddc_front(m, src, n16, st)
+		rc = m->r.K ? raster_call_front(m, src, n16, st)
+		   : m->ddc ? ddc_front(m, src, n16, st)
 		            : mix_launch(src, (long long)c, m->d_mix, (long long)n16, m->d_tab, m->d_chan, m->chan, m->pos, st);
 		if (rc != RXB200_OK) { return rc; }
 	}
@@ -375,6 +395,7 @@ extern "C" void rxb200_fm_mix_destroy(rxb200_fm_mix *m)
 	rxb200_fm_destroy(m->h);   // synchronises the stream the mixer runs on
 	cudaSetDevice(m->device);
 	cudaFree(m->d_tab); cudaFree(m->d_chan); cudaFree(m->d_cap); cudaFree(m->d_mix); cudaFree(m->d_out);
+	cudaFree(m->d_wt); cudaFree(m->d_v);
 	m->f.release();
 	if (m->ev0) { cudaEventDestroy(m->ev0); }
 	if (m->ev1) { cudaEventDestroy(m->ev1); }
@@ -383,15 +404,16 @@ extern "C" void rxb200_fm_mix_destroy(rxb200_fm_mix *m)
 
 namespace {
 
-// rxb200_fm_mix_create and rxb200_fm_mix_create_ddc (ddc != NULL, already checked)
+// rxb200_fm_mix_create, rxb200_fm_mix_create_ddc (ddc != NULL, already checked) and rxb200_fm_mix_create_raster
+// (raster != NULL, planned; no offsets and no tables)
 int mix_create(const rxb200_fm_params *params, int capture_rate, const int *offsets_hz, int n_channels,
-               const rxb200_ddc *ddc, bool wide, int device, rxb200_fm_mix **out)
+               const rxb200_ddc *ddc, bool wide, const RasterPlan *raster, int device, rxb200_fm_mix **out)
 {
 	*out = nullptr;
 	// every table first: a refused offset fails before any device work
 	std::vector<int32_t> all, t;
 	std::vector<MixChan> chan;
-	for (int k = 0; k < n_channels; k++) {
+	for (int k = 0; !raster && k < n_channels; k++) {
 		size_t L = 0;
 		const int rc = mix_table(capture_rate, offsets_hz[k], t, &L);
 		if (rc != RXB200_OK) { return rc; }
@@ -407,16 +429,25 @@ int mix_create(const rxb200_fm_params *params, int capture_rate, const int *offs
 	const int rc = rxb200_fm_create(params, device, n_channels, &m->h);
 	if (rc != RXB200_OK) { delete m; return rc; }
 	RXB_CUDA_OR(cudaSetDevice(device), rxb200_fm_mix_destroy(m));
-	RXB_CUDA_OR(cudaMalloc(&m->d_tab, all.size() * sizeof(int32_t)), rxb200_fm_mix_destroy(m));
-	RXB_CUDA_OR(cudaMalloc(&m->d_chan, chan.size() * sizeof(MixChan)), rxb200_fm_mix_destroy(m));
-	RXB_CUDA_OR(cudaMemcpy(m->d_tab, all.data(), all.size() * sizeof(int32_t), cudaMemcpyHostToDevice), rxb200_fm_mix_destroy(m));
-	RXB_CUDA_OR(cudaMemcpy(m->d_chan, chan.data(), chan.size() * sizeof(MixChan), cudaMemcpyHostToDevice), rxb200_fm_mix_destroy(m));
+	if (!raster) {
+		RXB_CUDA_OR(cudaMalloc(&m->d_tab, all.size() * sizeof(int32_t)), rxb200_fm_mix_destroy(m));
+		RXB_CUDA_OR(cudaMalloc(&m->d_chan, chan.size() * sizeof(MixChan)), rxb200_fm_mix_destroy(m));
+		RXB_CUDA_OR(cudaMemcpy(m->d_tab, all.data(), all.size() * sizeof(int32_t), cudaMemcpyHostToDevice), rxb200_fm_mix_destroy(m));
+		RXB_CUDA_OR(cudaMemcpy(m->d_chan, chan.data(), chan.size() * sizeof(MixChan), cudaMemcpyHostToDevice), rxb200_fm_mix_destroy(m));
+	}
 	RXB_CUDA_OR(cudaEventCreate(&m->ev0), rxb200_fm_mix_destroy(m));
 	RXB_CUDA_OR(cudaEventCreate(&m->ev1), rxb200_fm_mix_destroy(m));
 	if (ddc) {
 		m->ddc = true;
 		const int rc = m->f.create(ddc, wide);
 		if (rc != RXB200_OK) { rxb200_fm_mix_destroy(m); return rc; }
+	}
+	if (raster) {
+		m->r = *raster;
+		m->r.wt.clear();
+		RXB_CUDA_OR(cudaMalloc(&m->d_wt, raster->w_bytes()), rxb200_fm_mix_destroy(m));
+		RXB_CUDA_OR(cudaMemcpy(m->d_wt, raster->wt.data(), raster->w_bytes(), cudaMemcpyHostToDevice),
+		            rxb200_fm_mix_destroy(m));
 	}
 	*out = m;
 	return RXB200_OK;
@@ -428,7 +459,7 @@ extern "C" int rxb200_fm_mix_create(const rxb200_fm_params *params, int capture_
                                     int n_channels, int device, rxb200_fm_mix **out)
 {
 	if (!params || !offsets_hz || !out || n_channels < 1) { set_error("bad mix arguments (n_channels >= 1)"); return RXB200_EINVAL; }
-	return mix_create(params, capture_rate, offsets_hz, n_channels, nullptr, false, device, out);
+	return mix_create(params, capture_rate, offsets_hz, n_channels, nullptr, false, nullptr, device, out);
 }
 
 extern "C" int rxb200_fm_mix_create_ddc(const rxb200_fm_params *params, int capture_rate, const int *offsets_hz,
@@ -439,7 +470,23 @@ extern "C" int rxb200_fm_mix_create_ddc(const rxb200_fm_params *params, int capt
 	bool wide = false;
 	const int rc = rxb::ddc_check(ddc, &wide);
 	if (rc != RXB200_OK) { return rc; }
-	return mix_create(params, capture_rate, offsets_hz, n_channels, ddc, wide, device, out);
+	return mix_create(params, capture_rate, offsets_hz, n_channels, ddc, wide, nullptr, device, out);
+}
+
+extern "C" int rxb200_fm_mix_create_raster(const rxb200_fm_params *params, int n_bins, const int *bins, int n_channels,
+                                           const rxb200_ddc *ddc, int device, rxb200_fm_mix **out)
+{
+	if (!params || !out) { set_error("null argument"); return RXB200_EINVAL; }
+	*out = nullptr;
+	bool wide = false;
+	int rc = rxb::ddc_check(ddc, &wide);
+	if (rc != RXB200_OK) { return rc; }
+	rc = raster_check(n_bins, bins, n_channels, ddc);
+	if (rc != RXB200_OK) { return rc; }
+	RasterPlan p;
+	rc = p.plan(n_bins, bins, n_channels);
+	if (rc != RXB200_OK) { return rc; }
+	return mix_create(params, 0, nullptr, n_channels, ddc, wide, &p, device, out);
 }
 
 extern "C" int rxb200_fm_mix_decimated_len(const rxb200_fm_mix *m, size_t n_int16, size_t *n_dec_int16)

@@ -280,6 +280,18 @@ def ddc_device(capture_rate: int, offset_hz: int, phase: int, ddc, d_src_ptr: in
                                             stream or None))
 
 
+def raster_device(n_bins: int, bins, n0: int, ddc, d_src_ptr: int, n_complex: int, d_dst_ptr: int,
+                  stream: int = 0) -> None:
+    """The raster down-converter alone on device pointers (``rxb200_raster_device``), asynchronous on ``stream``:
+    d_src[i] is capture sample n0 + i, zero samples before d_src, floor(n_complex / decim) outputs per channel, channel
+    c's at d_dst + 2 c floor(n_complex / decim).  bins: one raster bin (0 <= bin < n_bins) per channel; ddc: (decim,
+    taps, shift)."""
+    b = np.ascontiguousarray(bins, dtype=np.int32)
+    d, _t = _ddc_c(ddc)
+    _lib.check(_lib.lib().rxb200_raster_device(n_bins, _ptr(b), int(b.size), n0, C.byref(d), d_src_ptr, n_complex,
+                                               d_dst_ptr, stream or None))
+
+
 def disc_device(form: int, quads, stream: int = 0):
     """One discriminator alone on the device (``rxb200_fm_disc_device``): quads is a contiguous int32 CUDA tensor
     [n][4] of (ar, aj, br, bj); returns the int32 [n] results, a new tensor on the same device, written asynchronously
@@ -295,21 +307,37 @@ class FmMix(_OneGpu):
     ``FmDemod`` run on the capture mixed down by ``offsets_hz[k]`` with ``mix_table``; the mixers' phases carry across
     calls.  Every call takes the one capture, int16[n_int16], and returns int16[n_channels][n_pcm].
     ddc = (decim, taps, shift): a decimating handle (``rxb200_fm_mix_create_ddc``), each channel filtered by the int32
-    taps, rounded by the shift and decimated by decim before the chain."""
+    taps, rounded by the shift and decimated by decim before the chain.
+    raster = (n_bins, bins) with ddc: a raster handle (``rxb200_fm_mix_create_raster``), channel c bin bins[c] of an
+    n_bins-bin raster over the capture, through the polyphase channelizer; capture_rate and offsets_hz are then not
+    passed (None)."""
 
     _prefix = "rxb200_fm_mix"
     _streams = False
     _m = property(lambda self: self._h)     # the handle under the name callers of earlier releases read
 
-    def __init__(self, params, capture_rate: int, offsets_hz, device: int = 0, ddc=None):
+    def __init__(self, params, capture_rate: Optional[int] = None, offsets_hz=None, device: int = 0, ddc=None,
+                 raster=None):
         self.params = FmParams.from_any(params)
         self.capture_rate = capture_rate
+        self.ddc = ddc
+        self.raster = raster
+        self._h = C.c_void_p()
+        pc = self.params.to_c()
+        if raster is not None:
+            if ddc is None or capture_rate is not None or offsets_hz is not None:
+                raise ValueError("a raster handle takes a ddc and no capture_rate or offsets_hz")
+            n_bins, bins = raster
+            b = np.ascontiguousarray(bins, dtype=np.int32).reshape(-1)
+            self.offsets_hz = None
+            self.n_channels = int(b.size)
+            d, _t = _ddc_c(ddc)
+            _lib.check(_lib.lib().rxb200_fm_mix_create_raster(C.byref(pc), n_bins, _ptr(b), self.n_channels, C.byref(d),
+                                                              device, C.byref(self._h)))
+            return
         offs = np.ascontiguousarray(offsets_hz, dtype=np.int32)
         self.offsets_hz = offs.tolist()
         self.n_channels = len(offs)
-        self.ddc = ddc
-        self._h = C.c_void_p()
-        pc = self.params.to_c()
         if ddc is None:
             _lib.check(_lib.lib().rxb200_fm_mix_create(C.byref(pc), capture_rate, _ptr(offs), self.n_channels, device,
                                                        C.byref(self._h)))
@@ -345,7 +373,8 @@ class FmMix(_OneGpu):
         return int(_lib.lib().rxb200_fm_stream(C.c_void_p(self.member())) or 0)
 
     def mix_ms(self) -> float:
-        """Device time of the last call's fm_mix_kernel (fm_ddc_kernel for a decimating handle)."""
+        """Device time of the last call's fm_mix_kernel (fm_ddc_kernel for a decimating handle, the two raster kernels
+        summed for a raster handle)."""
         ms = C.c_float(0)
         _lib.check(_lib.lib().rxb200_fm_mix_kernel_ms(self._h, C.byref(ms)))
         return float(ms.value)
