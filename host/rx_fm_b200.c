@@ -7,6 +7,12 @@
  * and a file replay is deterministic.  Every DSP stage of rtlsdr_callback()+full_demod() is one call:
  * rxb200_fm_process_read(), one stream read (<= 131072 complex) per call, like the reference's chunks
  * (a read re-blocked to the library's chunk granularity with -o N).
+ *
+ * Capture mode: RXB200_CAPTURE_RATE=<max Hz> takes every -f channel from ONE wideband capture instead of scanning.  The
+ * device is tuned once to the centre rxb200_fm_plan_capture picks, at R = M times the chain's capture rate, and read
+ * without pause; the reader gathers blocks of M * 131072 complex samples, each one rxb200_fm_mix_process_read of a
+ * decimating mixing handle, so every channel's chain sees reads of 131072 complex samples whatever lengths the device
+ * returns.  Channel k goes to <filename>.<f_k>, with its own squelch.
  */
 #include <errno.h>
 #include <math.h>
@@ -28,7 +34,7 @@ static volatile sig_atomic_t g_stop = 0;
 static void on_signal(int s) { (void)s; g_stop = 1; }
 
 /* ---- bounded queue of buffers ---- */
-typedef struct { int16_t *data; size_t n; int eof; } Slot;
+typedef struct { int16_t *data; size_t n; int eof; unsigned char silent[MAX_FREQS]; } Slot;   /* silent: capture mode */
 typedef struct {
 	Slot slot[QDEPTH];
 	int head, tail, count;
@@ -86,6 +92,11 @@ static struct {
 	int failed;                        /* a library call failed: exit status 1 */
 	rxb200_fm *fm;
 	FILE *out;
+	int offset_flag;                   /* -E offset: the device's offset_tune setting */
+	rxb200_fm_mix *mix;                /* capture mode: one decimating mixing handle, K = freq_len channels */
+	size_t block16, stride;            /* capture mode: int16 per block, PCM int16 per channel and block */
+	int decim;
+	FILE *outs[MAX_FREQS];
 	Queue q_raw, q_pcm;
 	pthread_mutex_t hop_m;
 } G;
@@ -101,7 +112,9 @@ static void usage(void)
 		"\t[-g gain] [-w bandwidth] [-l squelch_level] [-t squelch_delay] [-p ppm] [-o oversampling]\n"
 		"\t[-E edge|dc|adc|rdc|deemp|direct|no-mod|offset|agc|zero|wav] [-q rdc_block_const]\n"
 		"\t[-F fir_size] [-A std|fast|lut|ale] [-c us|eu|N] [-L N] [-v]\n"
-		"\tfilename ('-' means stdout)\n");
+		"\tfilename ('-' means stdout)\n"
+		"environment: RXB200_CAPTURE_RATE=max_Hz takes every -f channel from one capture of at most max_Hz samples/s,\n"
+		"\ttuned once to their centre (one GPU), channel f to filename.f (no scanning, no -l needed; refuses '-', -L, -o)\n");
 	exit(1);
 }
 
@@ -125,7 +138,7 @@ static uint32_t capture_freq(int idx)
 	return (uint32_t)f;
 }
 
-static void write_wav_header(void)
+static void write_wav_header(FILE *out)
 {
 	/* generate_header(), src/rtl_fm.c:1174-1206: sizes unknown (0xFFFFFFFF), PCM 16 bit */
 	const int raw = (G.der.params.mode == RXB200_MODE_RAW);
@@ -134,7 +147,35 @@ static void write_wav_header(void)
 	                       (unsigned char)(raw ? 2 : 1),0, 0,0,0,0, 0,0,0,0, (unsigned char)(raw ? 4 : 2),0,16,0,
 	                       'd','a','t','a',0xFF,0xFF,0xFF,0xFF};
 	for (int i = 0; i < 4; i++) { h[24 + i] = (unsigned char)(rate >> (8 * i)); h[28 + i] = (unsigned char)(brate >> (8 * i)); }
-	fwrite(h, 1, sizeof h, G.out);
+	fwrite(h, 1, sizeof h, out);
+}
+
+/* Capture mode's plan and handle: the channels' tuned frequencies through rxb200_fm_plan_capture, the capture mode
+ * filter of rx_power, one decimating mixing handle.  Nonzero (reported on stderr) when the plan or the handle is refused. */
+static int capture_setup(const char *cap_env, int64_t *centre, int *rate)
+{
+	int64_t t[MAX_FREQS];
+	int offs[MAX_FREQS];
+	for (int k = 0; k < G.freq_len; k++) { t[k] = capture_freq(k); }
+	rxb200_fm_capture_plan pl;
+	if (rxb200_fm_plan_capture(t, G.freq_len, G.der.capture_rate, atoll(cap_env), &pl, offs) != RXB200_OK) {
+		fprintf(stderr, "Capture mode: %s (RXB200_CAPTURE_RATE=%s).\n", rxb200_last_error(), cap_env);
+		return 1;
+	}
+	int32_t *taps = (int32_t *)malloc(sizeof(int32_t) * (size_t)pl.n_taps);
+	rxb200_ddc_lowpass(pl.decim, pl.n_taps, 15, taps);
+	const rxb200_ddc ddc = {pl.decim, pl.n_taps, taps, 15};
+	const int rc = rxb200_fm_mix_create_ddc(&G.der.params, pl.capture_rate, offs, G.freq_len, &ddc, 0, &G.mix);
+	free(taps);
+	if (rc != RXB200_OK) { fprintf(stderr, "rxb200: %s\n", rxb200_last_error()); return 1; }
+	G.decim = pl.decim;
+	G.block16 = (size_t)pl.decim * 2 * CHUNK_COMPLEX;
+	G.stride = rxb200_fm_mix_max_output(G.mix, G.block16, G.block16);
+	*centre = pl.centre_hz;
+	*rate = pl.capture_rate;
+	fprintf(stderr, "Capture mode: %d Hz centred at %lld Hz, decimation %d, %d taps, %d channels\n", pl.capture_rate,
+	        (long long)pl.centre_hz, pl.decim, pl.n_taps, G.freq_len);
+	return 0;
 }
 
 /* ---- threads ---- */
@@ -179,6 +220,37 @@ static void *reader_thread(void *arg)
 	return NULL;
 }
 
+/* Capture mode's reader: blocks of M * 131072 complex samples gathered from reads of any length, so that blocks start at
+ * multiples of M and every channel's chain sees reads of exactly 131072 complex samples.  At the end of the stream, or
+ * on a failed read, the partial block is handed on if it decimates to at least min_chunk int16, else dropped. */
+static void *block_reader_thread(void *arg)
+{
+	(void)arg;
+	SoapySDRDevice_activateStream(G.dev, G.stream, 0, 0, 0);
+	for (;;) {
+		Slot *s = q_begin_put(&G.q_raw);
+		size_t have = 0;
+		int r = 1;
+		while (have < G.block16) {
+			void *buffs[] = {s->data + have};
+			int flags = 0; long long t_ns = 0;
+			r = g_stop ? -1 : SoapySDRDevice_readStream(G.dev, G.stream, buffs, (G.block16 - have) / 2, &flags, &t_ns, 1000000);
+			if (r == SOAPY_SDR_OVERFLOW) { fprintf(stderr, "O"); fflush(stderr); continue; }
+			if (r <= 0) { break; }
+			have += (size_t)r * 2;
+		}
+		if (have == G.block16) { s->n = have; s->eof = 0; q_end_put(&G.q_raw); continue; }
+		if (!g_stop) { fprintf(stderr, "readStream read failed: %d\n", r); }
+		if (2 * (have / 2 / (size_t)G.decim) >= G.min_chunk) {
+			s->n = have; s->eof = 0; q_end_put(&G.q_raw);
+			s = q_begin_put(&G.q_raw);
+		}
+		s->n = 0; s->eof = 1; q_end_put(&G.q_raw);
+		break;
+	}
+	return NULL;
+}
+
 static void hop_to_next(void)
 {
 	/* controller_thread_fn's hop (src/rtl_fm.c:1039-1048) */
@@ -201,7 +273,8 @@ static void *demod_thread(void *arg)
 		Slot *out = q_begin_put(&G.q_pcm);
 		size_t n_pcm = 0;
 		/* a slot re-blocked for -o N is a read rxb200_fm_process(h, x, n, n) takes, and runs exactly as that call */
-		int rc = rxb200_fm_process_read(G.fm, in->data, in->n, out->data, 2 * CHUNK_COMPLEX, &n_pcm);
+		int rc = G.mix ? rxb200_fm_mix_process_read(G.mix, in->data, in->n, out->data, G.stride, &n_pcm)
+		               : rxb200_fm_process_read(G.fm, in->data, in->n, out->data, 2 * CHUNK_COMPLEX, &n_pcm);
 		q_end_get(&G.q_raw);
 		if (rc != RXB200_OK) { fprintf(stderr, "rxb200: %s\n", rxb200_last_error()); g_stop = 1; G.failed = 1; n_pcm = 0; }
 		if (G.print_levels && rc == RXB200_OK) {                                  /* :792-806, one chunk per call */
@@ -217,6 +290,18 @@ static void *demod_thread(void *arg)
 					G.level_max = 0; G.level_sum = 0;
 				}
 			}
+		}
+		if (G.mix) {                             /* capture mode: the same rule per channel, without the hop */
+			int hits_k[MAX_FREQS];
+			if (squelch && rc == RXB200_OK) { rxb200_fm_mix_squelch_hits(G.mix, hits_k); }
+			for (int k = 0; k < G.freq_len; k++) {
+				const int active = squelch && rc == RXB200_OK && hits_k[k] > G.conseq_squelch;
+				out->silent[k] = (unsigned char)(active && !G.squelch_zero);
+				if (active && G.squelch_zero) { memset(out->data + (size_t)k * G.stride, 0, n_pcm * sizeof(int16_t)); }
+			}
+			out->n = n_pcm; out->eof = 0;
+			q_end_put(&G.q_pcm);
+			continue;
 		}
 		int hits = 0;
 		if (squelch) { rxb200_fm_squelch_hits(G.fm, &hits); }
@@ -244,10 +329,18 @@ static void *writer_thread(void *arg)
 	for (;;) {
 		Slot *s = q_begin_get(&G.q_pcm);
 		if (s->eof) { q_end_get(&G.q_pcm); break; }
-		if (s->n && fwrite(s->data, 2, s->n, G.out) != s->n) { g_stop = 1; }
+		if (G.mix) {
+			for (int k = 0; k < G.freq_len; k++) {
+				if (s->n && !s->silent[k] && fwrite(s->data + (size_t)k * G.stride, 2, s->n, G.outs[k]) != s->n) { g_stop = 1; }
+			}
+		} else if (s->n && fwrite(s->data, 2, s->n, G.out) != s->n) { g_stop = 1; }
 		q_end_get(&G.q_pcm);
 	}
-	fflush(G.out);
+	if (G.mix) {
+		for (int k = 0; k < G.freq_len; k++) { fflush(G.outs[k]); }
+	} else {
+		fflush(G.out);
+	}
 	return NULL;
 }
 
@@ -285,7 +378,7 @@ int main(int argc, char **argv)
 			if (!strcmp(optarg, "deemp")) { G.cli.deemph = 1; }
 			if (!strcmp(optarg, "direct")) { G.direct_sampling = 1; }
 			if (!strcmp(optarg, "no-mod")) { G.direct_sampling = 3; }
-			if (!strcmp(optarg, "offset")) { G.cli.offset_tuning = 1; }
+			if (!strcmp(optarg, "offset")) { G.cli.offset_tuning = 1; G.offset_flag = 1; }
 			if (!strcmp(optarg, "rtlagc") || !strcmp(optarg, "agc")) { G.rtlagc = 1; }
 			if (!strcmp(optarg, "zero")) { G.squelch_zero = 1; }
 			if (!strcmp(optarg, "wav")) { G.wav = 1; }
@@ -324,12 +417,25 @@ int main(int argc, char **argv)
 		}
 	}
 	if (G.freq_len == 0) { fprintf(stderr, "Please specify a frequency.\n"); usage(); }
-	if (G.freq_len > 1 && G.cli.squelch_level == 0) {
+	const char *cap_env = getenv("RXB200_CAPTURE_RATE");
+	if (!cap_env && G.freq_len > 1 && G.cli.squelch_level == 0) {
 		fprintf(stderr, "Please specify a squelch level.  Required for scanning multiple frequencies.\n");
 		return 1;
 	}
 	if (G.freq_len > 1) { G.terminate_on_squelch = 0; }
 	G.filename = (argc <= optind) ? "-" : argv[optind];
+	if (cap_env) {
+		/* capture mode: one file per channel, one read per block; the mixer puts each channel at DC */
+		const char *bad = !strcmp(G.filename, "-") ? "'-' as the filename (it writes one file per channel)"
+		                  : G.print_levels ? "-L" : G.cli.post_downsample != 1 ? "-o" : NULL;
+		if (bad) { fprintf(stderr, "Capture mode (RXB200_CAPTURE_RATE) does not take %s.\n", bad); return 1; }
+		for (int i = 0; i < G.freq_len; i++) {
+			for (int j = 0; j < i; j++) {
+				if (G.freqs[i] == G.freqs[j]) { fprintf(stderr, "Capture mode (RXB200_CAPTURE_RATE): %u Hz is given twice.\n", G.freqs[i]); return 1; }
+			}
+		}
+		G.cli.offset_tuning = 1;
+	}
 	if (rxb200_fm_derive(&G.cli, &G.der) != RXB200_OK) { fprintf(stderr, "rxb200: %s\n", rxb200_last_error()); return 1; }
 	if (G.der.params.post_downsample <= 1) {
 		/* no -o: every read is handed on as it was read, one rxb200_fm_process_read per read, like the reference's
@@ -348,7 +454,11 @@ int main(int argc, char **argv)
 	}
 	G.der.params.report_levels = G.print_levels ? 1 : 0;
 	G.level_no = 1;
-	if (rxb200_fm_create(&G.der.params, 0, 1, &G.fm) != RXB200_OK) { fprintf(stderr, "rxb200: %s\n", rxb200_last_error()); return 1; }
+	int64_t tune_freq = capture_freq(0);
+	int tune_rate = G.der.capture_rate;
+	if (cap_env) {
+		if (capture_setup(cap_env, &tune_freq, &tune_rate) != 0) { return 1; }
+	} else if (rxb200_fm_create(&G.der.params, 0, 1, &G.fm) != RXB200_OK) { fprintf(stderr, "rxb200: %s\n", rxb200_last_error()); return 1; }
 
 	if (sdr_open(G.dev_query, G.channel, &G.dev, &G.stream) != 0) {
 		fprintf(stderr, "Failed to open sdr device matching '%s'.\n", G.dev_query);
@@ -363,29 +473,43 @@ int main(int argc, char **argv)
 	if (G.custom_ppm) { SoapySDRDevice_setFrequencyCorrection(G.dev, SOAPY_SDR_RX, G.channel, (double)G.ppm); }
 	if (G.bandwidth) { SoapySDRDevice_setBandwidth(G.dev, SOAPY_SDR_RX, G.channel, (double)G.bandwidth); }
 	if (G.direct_sampling) { SoapySDRDevice_writeSetting(G.dev, "direct_samp", G.direct_sampling == 1 ? "1" : "3"); }
-	if (G.cli.offset_tuning) { SoapySDRDevice_writeSetting(G.dev, "offset_tune", "true"); }
+	if (G.mix ? G.offset_flag : G.cli.offset_tuning) { SoapySDRDevice_writeSetting(G.dev, "offset_tune", "true"); }
 	{
 		SoapySDRKwargs none = {0, NULL, NULL};
-		SoapySDRDevice_setFrequency(G.dev, SOAPY_SDR_RX, G.channel, (double)capture_freq(0), &none);
-		SoapySDRDevice_setSampleRate(G.dev, SOAPY_SDR_RX, G.channel, (double)G.der.capture_rate);
+		SoapySDRDevice_setFrequency(G.dev, SOAPY_SDR_RX, G.channel, (double)tune_freq, &none);
+		SoapySDRDevice_setSampleRate(G.dev, SOAPY_SDR_RX, G.channel, (double)tune_rate);
 	}
 	fprintf(stderr, "Oversampling input by: %ix.\n", G.der.params.downsample);
 	fprintf(stderr, "Oversampling output by: %ix.\n", G.der.params.post_downsample);
 	fprintf(stderr, "Output at %u Hz.\n", (unsigned)G.der.params.rate_out);
 
-	if (!strcmp(G.filename, "-")) { G.out = stdout; }
-	else if (!(G.out = fopen(G.filename, "wb"))) { fprintf(stderr, "Failed to open %s\n", G.filename); return 1; }
-	if (G.wav) { write_wav_header(); }
+	if (G.mix) {
+		for (int k = 0; k < G.freq_len; k++) {                  /* channel k to <filename>.<f_k> */
+			char name[4096];
+			snprintf(name, sizeof name, "%s.%u", G.filename, G.freqs[k]);
+			if (!(G.outs[k] = fopen(name, "wb"))) { fprintf(stderr, "Failed to open %s\n", name); return 1; }
+			if (G.wav) { write_wav_header(G.outs[k]); }
+		}
+	} else {
+		if (!strcmp(G.filename, "-")) { G.out = stdout; }
+		else if (!(G.out = fopen(G.filename, "wb"))) { fprintf(stderr, "Failed to open %s\n", G.filename); return 1; }
+		if (G.wav) { write_wav_header(G.out); }
+	}
 
-	q_init(&G.q_raw, 2 * CHUNK_COMPLEX);
-	q_init(&G.q_pcm, 2 * CHUNK_COMPLEX);
+	q_init(&G.q_raw, G.mix ? G.block16 : 2 * CHUNK_COMPLEX);
+	q_init(&G.q_pcm, G.mix ? (size_t)G.freq_len * G.stride : 2 * CHUNK_COMPLEX);
 	pthread_t tr, td, tw;
 	pthread_create(&tw, NULL, writer_thread, NULL);
 	pthread_create(&td, NULL, demod_thread, NULL);
-	pthread_create(&tr, NULL, reader_thread, NULL);
+	pthread_create(&tr, NULL, G.mix ? block_reader_thread : reader_thread, NULL);
 	pthread_join(tr, NULL); pthread_join(td, NULL); pthread_join(tw, NULL);
-	if (G.out != stdout) { fclose(G.out); }
-	rxb200_fm_destroy(G.fm);
+	if (G.mix) {
+		for (int k = 0; k < G.freq_len; k++) { fclose(G.outs[k]); }
+		rxb200_fm_mix_destroy(G.mix);
+	} else {
+		if (G.out != stdout) { fclose(G.out); }
+		rxb200_fm_destroy(G.fm);
+	}
 	sdr_close(G.dev, G.stream);
 	return G.failed ? 1 : 0;
 }

@@ -509,6 +509,29 @@ size_t rxb200_fm_mix_max_output(const rxb200_fm_mix *m, size_t n_int16, size_t c
 int rxb200_ddc_device(int capture_rate, int offset_hz, long long phase, const rxb200_ddc *ddc, const int16_t *d_src,
                       size_t n_complex, int16_t *d_dst, void *stream);
 
+/* ---- rx_fm channels of one capture in the shell (DESIGN.md section 4.4, "Capture mode in the rx_fm shell")
+ * The plan the rx_fm shell's capture mode (RXB200_CAPTURE_RATE) uses to take K tuned frequencies t_k (Hz) from one
+ * capture through a decimating handle, for a chain whose capture rate is c (rxb200_fm_derived.capture_rate):
+ *   tmin, tmax = the smallest and largest t_k; g = gcd of every t_k - tmin (g = 0 when every t_k is equal);
+ *   fc = tmin when g = 0, else tmin + g floor((tmax - tmin) / (2 g)), so every offset is a multiple of the channel grid
+ *     and the mixer's period L = R / gcd(R, |o|) stays small for ordinary rasters;
+ *   o_k = t_k - fc, A = max |o_k|;  M = ceil((2 A + c) / c), so |o_k| < R / 2;  R = M c;  T = min(8191, 32 M + 1);
+ *   the filter is rxb200_ddc_lowpass(M, T, 15) at shift S = 15, the one rx_power's capture mode uses.
+ * Refusals, pure host arithmetic: RXB200_EINVAL for a NULL pointer, K < 1, c < 1, any t_k outside [0, 2^61), and R
+ * above max_capture_rate or 2^31 - 1 or M > 256 (the message names R); for an offset whose mixer table
+ * rxb200_fm_mix_table refuses, that call's code and message (RXB200_EUNSUPPORTED for a period above 2^20).  M is capped
+ * at 256 because the shell holds each block of M * 131072 complex capture samples (M * 512 KiB) on the host, four in
+ * flight. */
+typedef struct rxb200_fm_capture_plan {
+	int64_t centre_hz;   /* fc */
+	int decim;           /* M */
+	int capture_rate;    /* R = M c */
+	int n_taps;          /* T */
+} rxb200_fm_capture_plan;
+/* offsets_hz receives the K offsets o_k. */
+int rxb200_fm_plan_capture(const int64_t *tuned_hz /* n_channels */, int n_channels, int chain_rate,
+                           long long max_capture_rate, rxb200_fm_capture_plan *out, int *offsets_hz /* n_channels */);
+
 /* ---- raster mixing handles: the channels of a uniform raster through a polyphase channelizer (DESIGN.md section 4.4,
  * "Channels on a raster")
  * A raster handle has K bins (3 <= K <= 4096) over the capture and n_channels channels, channel c being bin k_c

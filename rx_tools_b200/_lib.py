@@ -58,6 +58,10 @@ class DdcC(C.Structure):
     _fields_ = [("decim", C.c_int), ("n_taps", C.c_int), ("taps", C.POINTER(C.c_int32)), ("shift", C.c_int)]
 
 
+class FmCapturePlanC(C.Structure):
+    _fields_ = [("centre_hz", C.c_int64), ("decim", C.c_int), ("capture_rate", C.c_int), ("n_taps", C.c_int)]
+
+
 class PowerPlanC(C.Structure):
     _fields_ = [("params", PowerParamsC), ("rate", C.c_int), ("crop", C.c_double),
                 ("first_freq", C.c_int64), ("freq_step", C.c_int64), ("bin_size_hz", C.c_double)]
@@ -95,6 +99,7 @@ SYMBOLS = [
     "rxb200_fm_mix_group_squelch_hits", "rxb200_fm_mix_group_levels", "rxb200_fm_mix_group_reset",
     "rxb200_fm_mix_create_ddc", "rxb200_fm_mix_decimated_len", "rxb200_fm_mix_max_output", "rxb200_ddc_device",
     "rxb200_fm_mix_group_create_ddc", "rxb200_fm_mix_create_raster", "rxb200_raster_device",
+    "rxb200_fm_plan_capture",
     "rxb200_power_mix_create", "rxb200_power_mix_destroy", "rxb200_power_mix_member", "rxb200_power_mix_reset",
     "rxb200_power_mix_accumulate", "rxb200_power_mix_accumulate_device", "rxb200_power_mix_kernel_ms",
     "rxb200_nco_table", "rxb200_power_ddc_device", "rxb200_ddc_lowpass",
@@ -228,6 +233,7 @@ def lib() -> C.CDLL:
                                               C.POINTER(C.c_void_p)]
     L.rxb200_raster_device.argtypes = [C.c_int, pint, C.c_int, C.c_ulonglong, C.POINTER(DdcC), C.c_void_p, sz,
                                        C.c_void_p, C.c_void_p]
+    L.rxb200_fm_plan_capture.argtypes = [pi64, C.c_int, C.c_int, C.c_longlong, C.POINTER(FmCapturePlanC), pint]
     L.rxb200_power_mix_create.argtypes = [C.POINTER(PowerParamsC), pint, p16, C.c_int, pint, C.POINTER(DdcC), C.c_int,
                                           C.POINTER(C.c_void_p)]
     L.rxb200_power_mix_destroy.argtypes = [C.c_void_p]

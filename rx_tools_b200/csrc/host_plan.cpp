@@ -115,6 +115,49 @@ extern "C" int rxb200_fm_mix_table(int capture_rate, int offset_hz, int32_t *tab
 	return RXB200_OK;
 }
 
+// The capture plan of the rx_fm shell's capture mode (include/rxb200.h, "rx_fm channels of one capture in the shell").
+extern "C" int rxb200_fm_plan_capture(const int64_t *tuned_hz, int n_channels, int chain_rate, long long max_capture_rate,
+                                      rxb200_fm_capture_plan *out, int *offsets_hz)
+{
+	if (!tuned_hz || !out || !offsets_hz) { set_error("null argument"); return RXB200_EINVAL; }
+	if (n_channels < 1 || chain_rate < 1) {
+		set_error("capture plan of %d channels at a chain capture rate of %d Hz (need >= 1 of each)", n_channels, chain_rate);
+		return RXB200_EINVAL;
+	}
+	const long long fmax = 1ll << 61;                   // keeps 2 A + 2 c below 2^63
+	long long tmin = tuned_hz[0], tmax = tuned_hz[0];
+	for (int k = 0; k < n_channels; k++) {
+		if (tuned_hz[k] < 0 || tuned_hz[k] >= fmax) { set_error("tuned frequency %lld Hz outside [0, 2^61)", (long long)tuned_hz[k]); return RXB200_EINVAL; }
+		tmin = std::min(tmin, (long long)tuned_hz[k]);
+		tmax = std::max(tmax, (long long)tuned_hz[k]);
+	}
+	long long g = 0;                                      // gcd of every t_k - tmin; 0 when all are equal
+	for (int k = 0; k < n_channels; k++) {
+		long long a = tuned_hz[k] - tmin, b = g;
+		while (b) { const long long t = a % b; a = b; b = t; }
+		g = a;
+	}
+	const long long fc = g ? tmin + g * ((tmax - tmin) / (2 * g)) : tmin;
+	const long long A = std::max(fc - tmin, tmax - fc), c = chain_rate;
+	const long long M = (2 * A + c + c - 1) / c, R = M * c;
+	if (R > max_capture_rate || R > 2147483647ll || M > 256) {
+		set_error("the channels need a capture rate of %lld Hz (decimation %lld), above the cap of %lld Hz, 2^31 - 1 or "
+		          "decimation 256", R, M, max_capture_rate);
+		return RXB200_EINVAL;
+	}
+	for (int k = 0; k < n_channels; k++) {
+		size_t L = 0;
+		const int rc = rxb200_fm_mix_table((int)R, (int)(tuned_hz[k] - fc), NULL, 0, &L);
+		if (rc != RXB200_ECAPACITY) { return rc; }        // the table's own refusal and message
+		offsets_hz[k] = (int)(tuned_hz[k] - fc);
+	}
+	out->centre_hz = fc;
+	out->decim = (int)M;
+	out->capture_rate = (int)R;
+	out->n_taps = (int)std::min(8191ll, 32 * M + 1);
+	return RXB200_OK;
+}
+
 // The channel filter of rx_power's capture mode (include/rxb200.h, "rx_power hops of one capture"): a Blackman-windowed
 // sinc with its cutoff at 1/(2M) cycles per sample, quantised to 2^shift / sum(g) and the rounding error put on the
 // centre tap, so that the DC gain is 2^shift exactly.

@@ -292,6 +292,27 @@ def raster_device(n_bins: int, bins, n0: int, ddc, d_src_ptr: int, n_complex: in
                                                d_dst_ptr, stream or None))
 
 
+@dataclass
+class CapturePlan:
+    """rxb200_fm_capture_plan: the capture's centre fc (Hz), decimation M, capture rate R = M c and filter length T."""
+    centre_hz: int
+    decim: int
+    capture_rate: int
+    n_taps: int
+
+
+def plan_capture(tuned_hz, chain_rate: int, max_rate: int):
+    """The rx_fm shell's capture plan for the tuned frequencies t_k (Hz) of a chain whose capture rate is chain_rate, under
+    a rate cap (``rxb200_fm_plan_capture``): (CapturePlan, each channel's offset o_k = t_k - fc).  The filter is
+    ``power.ddc_lowpass(decim, n_taps, 15)``."""
+    t = np.ascontiguousarray(tuned_hz, dtype=np.int64).reshape(-1)
+    offs = np.zeros(max(t.size, 1), dtype=np.int32)
+    out = _lib.FmCapturePlanC()
+    _lib.check(_lib.lib().rxb200_fm_plan_capture(t.ctypes.data_as(C.POINTER(C.c_int64)), int(t.size), int(chain_rate),
+                                                 int(max_rate), C.byref(out), _ptr(offs)))
+    return CapturePlan(int(out.centre_hz), out.decim, out.capture_rate, out.n_taps), [int(v) for v in offs[:t.size]]
+
+
 def disc_device(form: int, quads, stream: int = 0):
     """One discriminator alone on the device (``rxb200_fm_disc_device``): quads is a contiguous int32 CUDA tensor
     [n][4] of (ar, aj, br, bj); returns the int32 [n] results, a new tensor on the same device, written asynchronously
