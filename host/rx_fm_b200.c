@@ -12,7 +12,8 @@
  * device is tuned once to the centre rxb200_fm_plan_capture picks, at R = M times the chain's capture rate, and read
  * without pause; the reader gathers blocks of M * 131072 complex samples, each one rxb200_fm_mix_process_read of a
  * decimating mixing handle, so every channel's chain sees reads of 131072 complex samples whatever lengths the device
- * returns.  Channel k goes to <filename>.<f_k>, with its own squelch.
+ * returns.  Channel k goes to <filename>.<f_k>, with its own squelch.  With RXB200_CAPTURE_STAGES=2 as well, the plan is
+ * rxb200_fm_plan_capture_two_stage's and the handle a two-stage mixing handle (M = M1 M2); nothing else changes.
  */
 #include <errno.h>
 #include <math.h>
@@ -150,6 +151,37 @@ static void write_wav_header(FILE *out)
 	fwrite(h, 1, sizeof h, out);
 }
 
+/* Capture mode with RXB200_CAPTURE_STAGES=2: the plan of rxb200_fm_plan_capture_two_stage and one two-stage mixing
+ * handle, whose channel filters cost a coarse DFT shared by every channel plus a 129-tap fine filter per channel. */
+static int capture_setup_two_stage(const char *cap_env, const int64_t *t, int *offs, int64_t *centre, int *rate)
+{
+	rxb200_fm_two_stage_plan pl;
+	if (rxb200_fm_plan_capture_two_stage(t, G.freq_len, G.der.capture_rate, atoll(cap_env), &pl, offs) != RXB200_OK) {
+		fprintf(stderr, "Capture mode: %s (RXB200_CAPTURE_RATE=%s).\n", rxb200_last_error(), cap_env);
+		return 1;
+	}
+	int32_t *h1 = (int32_t *)malloc(sizeof(int32_t) * (size_t)pl.coarse_taps);
+	int32_t *h2 = (int32_t *)malloc(sizeof(int32_t) * (size_t)pl.fine_taps);
+	rxb200_ddc_lowpass(pl.coarse_decim, pl.coarse_taps, 15, h1);
+	rxb200_ddc_lowpass(pl.fine_decim, pl.fine_taps, 15, h2);
+	const rxb200_ddc coarse = {pl.coarse_decim, pl.coarse_taps, h1, pl.coarse_shift};
+	const rxb200_ddc fine = {pl.fine_decim, pl.fine_taps, h2, pl.fine_shift};
+	const int rc = rxb200_fm_mix_create_two_stage(&G.der.params, pl.capture_rate, pl.n_bins, offs, G.freq_len, &coarse,
+	                                              &fine, 0, &G.mix);
+	free(h1);
+	free(h2);
+	if (rc != RXB200_OK) { fprintf(stderr, "rxb200: %s\n", rxb200_last_error()); return 1; }
+	G.decim = pl.coarse_decim * pl.fine_decim;
+	G.block16 = (size_t)G.decim * 2 * CHUNK_COMPLEX;
+	G.stride = rxb200_fm_mix_max_output(G.mix, G.block16, G.block16);
+	*centre = pl.centre_hz;
+	*rate = pl.capture_rate;
+	fprintf(stderr, "Capture mode: %d Hz centred at %lld Hz in two stages: %d bins, coarse decimation %d with %d taps, "
+	        "fine decimation %d with %d taps, %d channels\n", pl.capture_rate, (long long)pl.centre_hz, pl.n_bins,
+	        pl.coarse_decim, pl.coarse_taps, pl.fine_decim, pl.fine_taps, G.freq_len);
+	return 0;
+}
+
 /* Capture mode's plan and handle: the channels' tuned frequencies through rxb200_fm_plan_capture, the capture mode
  * filter of rx_power, one decimating mixing handle.  Nonzero (reported on stderr) when the plan or the handle is refused. */
 static int capture_setup(const char *cap_env, int64_t *centre, int *rate)
@@ -157,6 +189,8 @@ static int capture_setup(const char *cap_env, int64_t *centre, int *rate)
 	int64_t t[MAX_FREQS];
 	int offs[MAX_FREQS];
 	for (int k = 0; k < G.freq_len; k++) { t[k] = capture_freq(k); }
+	const char *stages = getenv("RXB200_CAPTURE_STAGES");
+	if (stages && strcmp(stages, "2") == 0) { return capture_setup_two_stage(cap_env, t, offs, centre, rate); }
 	rxb200_fm_capture_plan pl;
 	if (rxb200_fm_plan_capture(t, G.freq_len, G.der.capture_rate, atoll(cap_env), &pl, offs) != RXB200_OK) {
 		fprintf(stderr, "Capture mode: %s (RXB200_CAPTURE_RATE=%s).\n", rxb200_last_error(), cap_env);

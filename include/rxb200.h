@@ -567,6 +567,77 @@ int rxb200_fm_mix_create_raster(const rxb200_fm_params *params, int n_bins, cons
 int rxb200_raster_device(int n_bins, const int *bins, int n_channels, unsigned long long n0, const rxb200_ddc *ddc,
                          const int16_t *d_src, size_t n_complex, int16_t *d_dst, void *stream);
 
+/* ---- two-stage mixing handles: channels at any offset through a shared polyphase stage, then a per-channel NCO stage
+ * (DESIGN.md section 4.4, "Channels at any offset in two stages")
+ * A two-stage handle has a capture rate R > 0 (Hz), one integer offset f_c per channel with |f_c| < R/2, K coarse bins
+ * (3 <= K <= 4096), a coarse rxb200_ddc d1 = (M1, T1, h1, S1) with sum |h1| < 2^22 (the raster bound) and a fine
+ * rxb200_ddc d2 = (M2, T2, h2, S2), with M = M1 M2 <= 4096.  Indices n count capture samples from create or reset across
+ * calls; every stream is 0 before index 0.
+ *   Bin and word of channel c: b_c = floor((f_c K + floor(R/2)) / R) mod K (the nearest bin centre b R / K, ties
+ *     rounded up); N_c = (f_c K - b'_c R) M1 with b'_c the representative of b_c in (-K/2, K/2]; D = K R;
+ *     w_c = floor((N_c 2^32 + floor(D/2)) / D) mod 2^32, exact (128-bit host integers): the rx_power NCO word of the
+ *     residual offset f_c - b'_c R / K at the coarse rate R / M1 (rxb200_two_stage_word).
+ *   Coarse stage: for each bin b that holds a channel, y_b[m] is output m of the raster rule above for bin b with d1:
+ *     emitted at e1_m = m M1 + M1 - 1, twiddle tw[(b n) mod K] of rxb200_fm_mix_table(K, 1), no rounding inside the
+ *     sum, then the S1 shift and int16 saturation.
+ *   Fine stage: z_c[m] = y_{b_c}[m] through the rx_power NCO mixer (rxb200_nco_table) at phase m w_c mod 2^32, with
+ *     mix_one's rounding and int16 wrap; output q is emitted at coarse index q M2 + M2 - 1:
+ *     A = sum_{j<T2} h2[j] z_c[q M2 + M2 - 1 - j] (exact), then the S2 shift and int16 saturation.
+ * Fine output q falls at capture sample q M + M - 1, so the decimated length (rxb200_fm_mix_decimated_len), the chunk
+ * rule (multiples of 2M), a read with no output, the refusals on the decimated shape, reset and every rxb200_fm_mix_*
+ * entry point behave exactly as for a decimating handle with decimation M; rxb200_fm_mix_kernel_ms reports both stages
+ * of the last call summed.  It is neither the decimating handle, the raster handle nor a single-stage filter byte for
+ * byte.  Two anchors are exact: M1 = 1, T1 = 1, h1 = {1}, S1 = 15 and a channel on bin 0 give rxb200_power_ddc_device
+ * (R, f_c, n0, d2) (the twiddle of bin 0 is 2^15, so the coarse stage is the identity, and for even R the word is the
+ * rx_power word); and M2 = 1, T2 = 1, h2 = {1}, S2 = 0 with f_c = b_c R / K exactly (so w_c = 0) give the raster
+ * handle with bins b_c.
+ * The coarse stage runs the raster kernels for the distinct bins only; the fine stage runs fine_ddc_kernel (ddc.cuh's
+ * down-converter with the NCO mixer) with the channels in bin order, each grid row staging its bin's coarse stream once.
+ * The handle carries the capture count, the coarse stage's last T1 - 1 raw samples and each bin's last T2 - 1 coarse
+ * samples, and a call's next histories become live only when it succeeds.  A long call runs in groups of coarse frames
+ * whose branch sums and coarse rows fit about RXB200_RASTER_SCRATCH_BYTES; the bytes are the same as with one group.
+ * Refusals, all before any device is touched: those of rxb200_fm_mix_create_ddc for params and d2; those of
+ * rxb200_fm_mix_create_raster for K and d1; RXB200_EINVAL for R <= 0, NULL offsets, n_channels < 1, any |f_c| >= R/2
+ * and M1 M2 > 4096. */
+int rxb200_fm_mix_create_two_stage(const rxb200_fm_params *params, int capture_rate, int n_bins,
+                                   const int *offsets_hz /* n_channels */, int n_channels, const rxb200_ddc *coarse,
+                                   const rxb200_ddc *fine, int device, rxb200_fm_mix **out);
+/* b_c into bins[c] and w_c into words[c] for M1 = coarse_decim, pure host arithmetic.  RXB200_EINVAL for a NULL pointer,
+ * n_channels < 1, R <= 0, K outside [3, 4096], M1 outside [1, 4096] or any |f_c| >= R/2. */
+int rxb200_two_stage_word(int capture_rate, int n_bins, int coarse_decim, const int *offsets_hz /* n_channels */,
+                          int n_channels, int *bins /* n_channels */, uint32_t *words /* n_channels */);
+/* The two stages alone on DEVICE pointers, stateless, on `stream`: d_src[i] is capture sample n0 + i (its twiddle uses
+ * (b (n0 + i)) mod K, n0 + i an exact integer), the samples before d_src are zero, coarse output m is emitted at d_src
+ * index m M1 + M1 - 1 and mixed at phase (floor(n0 / M1) + m) w_c, and fine output q at coarse output q M2 + M2 - 1;
+ * floor(n_complex / M) outputs per channel go to d_dst, channel c's at d_dst + 2 c floor(n_complex / M).  For M | n0
+ * this is the rule for a capture that is zero before n0.  Both pointers 4-byte aligned.  The refusals of
+ * rxb200_fm_mix_create_two_stage but the params'.  Asynchronous. */
+int rxb200_two_stage_device(int capture_rate, int n_bins, const int *offsets_hz /* n_channels */, int n_channels,
+                            unsigned long long n0, const rxb200_ddc *coarse, const rxb200_ddc *fine,
+                            const int16_t *d_src, size_t n_complex, int16_t *d_dst, void *stream);
+/* The plan the rx_fm shell's capture mode uses with RXB200_CAPTURE_STAGES=2 for K tuned frequencies t_k of a chain whose
+ * capture rate is c: fc and the offsets o_k as rxb200_fm_plan_capture gives them; M from that plan's rule,
+ * M' = 4 ceil(M / 4); R = M' c; M2 = 4, M1 = M' / 4 and K = 2 M1 (bins 2c apart, coarse rate 4c, residual at most c);
+ * the coarse filter rxb200_ddc_lowpass(M1, min(8191, 24 M1 + 1), 15) at S1 = 30 (Q15 taps times the 2^15 twiddle) and
+ * the fine filter rxb200_ddc_lowpass(4, 129, 15) at S2 = 15, so the final cutoff is c/2 as in the single-stage plan.
+ * Refusals, pure host arithmetic: RXB200_EINVAL for a NULL pointer, K < 1, c < 1, any t_k outside [0, 2^61), M' < 8, and
+ * R above max_capture_rate or 2^31 - 1 or M' > 256 (the message names R). */
+typedef struct rxb200_fm_two_stage_plan {
+	int64_t centre_hz;     /* fc */
+	int capture_rate;      /* R = M' c */
+	int n_bins;            /* K = 2 M1 */
+	int coarse_decim;      /* M1 */
+	int coarse_taps;       /* T1 */
+	int coarse_shift;      /* S1 = 30 */
+	int fine_decim;        /* M2 = 4 */
+	int fine_taps;         /* T2 = 129 */
+	int fine_shift;        /* S2 = 15 */
+} rxb200_fm_two_stage_plan;
+/* offsets_hz receives the K offsets o_k. */
+int rxb200_fm_plan_capture_two_stage(const int64_t *tuned_hz /* n_channels */, int n_channels, int chain_rate,
+                                     long long max_capture_rate, rxb200_fm_two_stage_plan *out,
+                                     int *offsets_hz /* n_channels */);
+
 /* ======================================================================== rx_fm channels of one capture on several GPUs
  * The channels of ONE capture split over GPUs: one process, n_dev rxb200_fm_mix handles, member i owning the contiguous
  * channels [b, e) that rxb200_power_shard(n_channels, n_dev, i, &b, &e) gives, with offsets offsets_hz[b..e).  A member

@@ -62,6 +62,12 @@ class FmCapturePlanC(C.Structure):
     _fields_ = [("centre_hz", C.c_int64), ("decim", C.c_int), ("capture_rate", C.c_int), ("n_taps", C.c_int)]
 
 
+class FmTwoStagePlanC(C.Structure):
+    _fields_ = [("centre_hz", C.c_int64), ("capture_rate", C.c_int), ("n_bins", C.c_int), ("coarse_decim", C.c_int),
+                ("coarse_taps", C.c_int), ("coarse_shift", C.c_int), ("fine_decim", C.c_int), ("fine_taps", C.c_int),
+                ("fine_shift", C.c_int)]
+
+
 class PowerPlanC(C.Structure):
     _fields_ = [("params", PowerParamsC), ("rate", C.c_int), ("crop", C.c_double),
                 ("first_freq", C.c_int64), ("freq_step", C.c_int64), ("bin_size_hz", C.c_double)]
@@ -99,7 +105,8 @@ SYMBOLS = [
     "rxb200_fm_mix_group_squelch_hits", "rxb200_fm_mix_group_levels", "rxb200_fm_mix_group_reset",
     "rxb200_fm_mix_create_ddc", "rxb200_fm_mix_decimated_len", "rxb200_fm_mix_max_output", "rxb200_ddc_device",
     "rxb200_fm_mix_group_create_ddc", "rxb200_fm_mix_create_raster", "rxb200_raster_device",
-    "rxb200_fm_plan_capture",
+    "rxb200_fm_plan_capture", "rxb200_fm_mix_create_two_stage", "rxb200_two_stage_word", "rxb200_two_stage_device",
+    "rxb200_fm_plan_capture_two_stage",
     "rxb200_power_mix_create", "rxb200_power_mix_destroy", "rxb200_power_mix_member", "rxb200_power_mix_reset",
     "rxb200_power_mix_accumulate", "rxb200_power_mix_accumulate_device", "rxb200_power_mix_kernel_ms",
     "rxb200_nco_table", "rxb200_power_ddc_device", "rxb200_ddc_lowpass",
@@ -234,6 +241,13 @@ def lib() -> C.CDLL:
     L.rxb200_raster_device.argtypes = [C.c_int, pint, C.c_int, C.c_ulonglong, C.POINTER(DdcC), C.c_void_p, sz,
                                        C.c_void_p, C.c_void_p]
     L.rxb200_fm_plan_capture.argtypes = [pi64, C.c_int, C.c_int, C.c_longlong, C.POINTER(FmCapturePlanC), pint]
+    L.rxb200_fm_mix_create_two_stage.argtypes = [C.POINTER(FmParamsC), C.c_int, C.c_int, pint, C.c_int, C.POINTER(DdcC),
+                                                 C.POINTER(DdcC), C.c_int, C.POINTER(C.c_void_p)]
+    L.rxb200_two_stage_word.argtypes = [C.c_int, C.c_int, C.c_int, pint, C.c_int, pint, C.POINTER(C.c_uint32)]
+    L.rxb200_two_stage_device.argtypes = [C.c_int, C.c_int, pint, C.c_int, C.c_ulonglong, C.POINTER(DdcC),
+                                          C.POINTER(DdcC), C.c_void_p, sz, C.c_void_p, C.c_void_p]
+    L.rxb200_fm_plan_capture_two_stage.argtypes = [pi64, C.c_int, C.c_int, C.c_longlong, C.POINTER(FmTwoStagePlanC),
+                                                   pint]
     L.rxb200_power_mix_create.argtypes = [C.POINTER(PowerParamsC), pint, p16, C.c_int, pint, C.POINTER(DdcC), C.c_int,
                                           C.POINTER(C.c_void_p)]
     L.rxb200_power_mix_destroy.argtypes = [C.c_void_p]

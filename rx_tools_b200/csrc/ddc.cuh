@@ -2,7 +2,9 @@
 // with its integer table) and power_ddc_kernel (power_mix.cu: rx_power hops, each mixed with a phase-accumulator NCO).
 // Both kernels are ddc_body with their mixer policy: it stages the capture samples its outputs' windows cover, mixes
 // them per channel into shared memory with mix_one, and runs the T-tap dot product at the emission points only; the
-// policy supplies the mixer index and the output address, the two things they differ in.  The host side they share is
+// policy supplies the mixer index and the output address, the two things they differ in.  fine_ddc_kernel
+// (fm_two_stage.cu) is ddc_body too, with an NCO mixer and the staging hook ddc_row giving each grid row its own
+// stream.  The host side they share is
 // here too (the launch, the filter state a handle carries between calls) and in ddc.cu (the argument check, the
 // stateless entries' upload).
 #pragma once
@@ -63,6 +65,20 @@ __device__ __forceinline__ int ddc_out(Acc acc, int S)
 	return (int)(y < -32768 ? -32768 : (y > 32767 ? 32767 : y));
 }
 
+// The staging hook: grid row blockIdx.y's channels [c0, c0 + nc) in the policy's order, and the stream it stages (src,
+// with the T - 1 samples before src[0] at hist).  By default every grid row stages the one capture and holds channels
+// [y MIX_GROUP, y MIX_GROUP + MIX_GROUP); a policy whose grid rows read different streams specialises it.
+struct DdcRow {
+	int c0, nc;
+	const uint32_t *src, *hist;
+};
+template <typename Mix>
+__device__ __forceinline__ DdcRow ddc_row(const DdcArgs<Mix> &a)
+{
+	const int c0 = (int)blockIdx.y * MIX_GROUP;
+	return DdcRow{c0, min(MIX_GROUP, a.n_ch - c0), a.src, a.hist};
+}
+
 // One CTA: U consecutive outputs of every channel of its grid row (up to 256 channels, blockIdx.y).  It stages the
 // capture samples its outputs' windows cover once (the history before the call's first sample), then per channel mixes
 // them into shared memory and runs the T-tap dot product at the emission points only, lpo lanes per output.  Acc: int
@@ -80,8 +96,8 @@ __device__ __forceinline__ void ddc_body(const DdcArgs<Mix> &a)
 	int32_t *s_h = reinterpret_cast<int32_t *>(ddc_smem);
 	uint32_t *s_x = reinterpret_cast<uint32_t *>(s_h + T);
 	uint32_t *s_z = s_x + room;
-	const int c0 = (int)blockIdx.y * MIX_GROUP;
-	const int nc = min(MIX_GROUP, a.n_ch - c0);
+	const DdcRow g = ddc_row(a);
+	const int c0 = g.c0, nc = g.nc;
 	const long long u0 = (long long)blockIdx.x * a.U;
 	const int U = (int)min((long long)a.U, a.n_out - u0);
 	const int n = (U - 1) * a.ws + T;
@@ -91,7 +107,7 @@ __device__ __forceinline__ void ddc_body(const DdcArgs<Mix> &a)
 	typename Mix::Row row(a, c0, nc, u0, g0);
 	for (int s = threadIdx.x; s < n; s += blockDim.x) {
 		const long long i = b0 + ddc_off(s, a);
-		s_x[s] = i >= 0 ? __ldg(a.src + i) : a.hist[(T - 1) + i];
+		s_x[s] = i >= 0 ? __ldg(g.src + i) : g.hist[(T - 1) + i];
 	}
 	__syncthreads();
 	const int lane = (int)threadIdx.x & (a.lpo - 1), sub = (int)threadIdx.x / a.lpo, n_sub = (int)blockDim.x / a.lpo;
@@ -128,11 +144,12 @@ __device__ __forceinline__ void ddc_body(const DdcArgs<Mix> &a)
 
 // Launches kern (a DDC kernel) on the current device for a.n_out > 0 outputs per channel, with its launch shape: a.ws,
 // a.ws_m, a.lpo, and as many outputs per CTA (a.U) as the staging room and the reach allow, but at least two CTAs per
-// SM when there is work.  The dynamic shared memory holds the reversed taps, the staged and the mixed span.
+// SM when there is work.  The dynamic shared memory holds the reversed taps, the staged and the mixed span.  rows: the
+// grid rows of a policy that specialises ddc_row (0: one per MIX_GROUP channels).
 template <typename Mix>
-int ddc_launch(DdcArgs<Mix> a, void (*kern)(DdcArgs<Mix>), cudaStream_t st)
+int ddc_launch(DdcArgs<Mix> a, void (*kern)(DdcArgs<Mix>), cudaStream_t st, int rows = 0)
 {
-	const int groups = (a.n_ch + MIX_GROUP - 1) / MIX_GROUP;
+	const int groups = rows ? rows : (a.n_ch + MIX_GROUP - 1) / MIX_GROUP;
 	a.ws = a.T >= a.M ? a.M : a.T;
 	a.ws_m = 0xffffffffu / (unsigned)a.ws;
 	a.lpo = 1;

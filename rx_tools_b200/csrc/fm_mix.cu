@@ -4,7 +4,9 @@
 // chain on them through its device entry points.  A decimating handle (rxb200_fm_mix_create_ddc) runs fm_ddc_kernel
 // instead (ddc.cuh's down-converter with the channels' tables), which mixes, filters and decimates, and carries its
 // filter state (DdcFilter) between calls.  A raster handle (rxb200_fm_mix_create_raster) is a decimating handle whose
-// front stage is fm_raster.cu's polyphase channelizer instead.  Every process entry point of every kind goes through
+// front stage is fm_raster.cu's polyphase channelizer instead, and a two-stage handle
+// (rxb200_fm_mix_create_two_stage) one whose front stage is fm_two_stage.cu's coarse and fine stages.  Every process
+// entry point of every kind goes through
 // mix_call, whose refusals and member shape come from fm_mix_check_host_call (which the group uses too).  The chain
 // itself is not touched here.
 #include <algorithm>
@@ -14,6 +16,7 @@
 #include "common.cuh"
 #include "ddc.cuh"
 #include "raster.cuh"
+#include "two_stage.cuh"
 
 namespace rxb {
 
@@ -210,9 +213,16 @@ struct rxb200_fm_mix {
 	RasterPlan r;
 	double *d_wt = nullptr;
 	double *d_v = nullptr; size_t v_cap = 0;     // doubles
+	// a two-stage handle (rxb200_fm_mix_create_two_stage, ts != NULL): a decimating handle whose DdcFilter f is the
+	// coarse stage's and whose front stage is ts->front, with the coarse rows' scratch d_y (and d_v)
+	TwoStage *ts = nullptr;
+	uint32_t *d_y = nullptr; size_t y_cap = 0;   // words
 };
 
 namespace {
+
+// the decimation of a decimating handle: M, or M1 M2 for a two-stage handle
+size_t decim(const rxb200_fm_mix *m) { return (size_t)m->f.M * (size_t)(m->ts ? m->ts->M2 : 1); }
 
 // int16 a decimating handle hands the chain from a call of n_int16 capture int16 after pos capture samples: the
 // outputs whose emission point m*M + M - 1 falls in the call
@@ -241,13 +251,13 @@ int rxb::fm_mix_check_host_call(rxb200_fm_mix *m, const int16_t *cs16, size_t n_
 		                               total);
 	}
 	if (!cs16 || !pcm) { set_error("null argument"); return RXB200_EINVAL; }
-	const size_t M = (size_t)m->f.M;
+	const size_t M = decim(m);
 	if (n_int16 % 2 != 0) { set_error("n_int16=%zu must be even", n_int16); return RXB200_EUNSUPPORTED; }
 	if (!read && (chunk_int16 == 0 || chunk_int16 % (2 * M) != 0)) {
 		set_error("chunk_int16=%zu must be a multiple of 2 * decim = %zu", chunk_int16, 2 * M);
 		return RXB200_EUNSUPPORTED;
 	}
-	*n16 = ddc_len(m->pos, n_int16, m->f.M);
+	*n16 = ddc_len(m->pos, n_int16, (int)M);
 	*chunk16 = read ? *n16 : chunk_int16 / M;
 	if (read && *n16 == 0 && n_int16 > 0) {
 		return rxb::fm_check_host_call(m->h, cs16, 0, 262144, pcm, pcm_stride, nullptr, n_pcm, false, total);
@@ -292,10 +302,28 @@ int raster_call_front(rxb200_fm_mix *m, const int16_t *src, size_t n16, cudaStre
 	                    n_out, st);
 }
 
+// a two-stage handle's front stage: the coarse outputs whose emission points fall in the call's c capture samples, and
+// the fine outputs among them to n16 int16 per channel in d_mix.  It runs whenever the call has coarse outputs, since
+// they advance the bins' histories even when no fine output falls in the call.
+int two_stage_call_front(rxb200_fm_mix *m, const int16_t *src, size_t c, size_t n16, cudaStream_t st)
+{
+	TwoStage &t = *m->ts;
+	const unsigned long long M1 = (unsigned long long)m->f.M, ma = m->pos / M1;
+	const long long n1 = (long long)((m->pos + c) / M1 - ma);
+	if (n1 == 0) { return RXB200_OK; }
+	const long long F = std::min(t.G, n1);
+	RXB_CUDA(reserve(m->d_v, m->v_cap, (size_t)F * (size_t)t.r.Kp));
+	RXB_CUDA(reserve(m->d_y, m->y_cap, t.y_words(F)));
+	return t.front(m->f, reinterpret_cast<const uint32_t *>(src), (long long)(ma * M1 + M1 - 1 - m->pos),
+	               (unsigned)(m->pos % (unsigned long long)t.r.K), n1, ma, (int)(ma % (unsigned long long)t.M2), m->d_v,
+	               m->d_y, reinterpret_cast<uint32_t *>(m->d_mix), (long long)(n16 / 2), st);
+}
+
 // One call of any process entry point.  device: cs16 and pcm are device pointers (the member's device entry point
 // writes pcm), else host pointers staged through the handle's buffers.  read: one read (chunk_int16 == n_int16).  The
-// front stage (fm_mix_kernel, fm_ddc_kernel for a decimating handle, the raster kernels for a raster handle) writes the member's input to d_mix; when it has
-// no output (n16 == 0) neither it nor the member runs, but the phases and the history still advance.
+// front stage (fm_mix_kernel, fm_ddc_kernel for a decimating handle, the raster kernels for a raster handle, both stages
+// for a two-stage handle) writes the member's input to d_mix; when it has no output (n16 == 0) the member does not run
+// (nor the front stage, but a two-stage handle's coarse stage), but the phases and the histories still advance.
 int mix_call(rxb200_fm_mix *m, const int16_t *cs16, size_t n_int16, size_t chunk_int16, int16_t *pcm, size_t pcm_stride,
              size_t *n_pcm, int *chunk_result_len, bool read, bool device, int sync)
 {
@@ -317,12 +345,14 @@ int mix_call(rxb200_fm_mix *m, const int16_t *cs16, size_t n_int16, size_t chunk
 		src = m->d_cap;
 	}
 	RXB_CUDA(cudaEventRecord(m->ev0, st));
-	if (n16) {
+	if (m->ts) {
+		rc = two_stage_call_front(m, src, c, n16, st);
+	} else if (n16) {
 		rc = m->r.K ? raster_call_front(m, src, n16, st)
 		   : m->ddc ? ddc_front(m, src, n16, st)
 		            : mix_launch(src, (long long)c, m->d_mix, (long long)n16, m->d_tab, m->d_chan, m->chan, m->pos, st);
-		if (rc != RXB200_OK) { return rc; }
 	}
+	if (rc != RXB200_OK) { return rc; }
 	RXB_CUDA(cudaEventRecord(m->ev1, st));
 	rc = m->f.carry(reinterpret_cast<const uint32_t *>(src), c, st);
 	if (rc != RXB200_OK) { return rc; }
@@ -345,6 +375,7 @@ int mix_call(rxb200_fm_mix *m, const int16_t *cs16, size_t n_int16, size_t chunk
 		RXB_CUDA(cudaStreamSynchronize(st));    // with output, the member's call has synchronised
 	}
 	m->f.commit();
+	if (m->ts) { m->ts->commit(); }
 	m->pos += c;
 	if (n_pcm) { *n_pcm = total; }
 	return RXB200_OK;
@@ -395,8 +426,9 @@ extern "C" void rxb200_fm_mix_destroy(rxb200_fm_mix *m)
 	rxb200_fm_destroy(m->h);   // synchronises the stream the mixer runs on
 	cudaSetDevice(m->device);
 	cudaFree(m->d_tab); cudaFree(m->d_chan); cudaFree(m->d_cap); cudaFree(m->d_mix); cudaFree(m->d_out);
-	cudaFree(m->d_wt); cudaFree(m->d_v);
+	cudaFree(m->d_wt); cudaFree(m->d_v); cudaFree(m->d_y);
 	m->f.release();
+	if (m->ts) { m->ts->release(0); delete m->ts; }
 	if (m->ev0) { cudaEventDestroy(m->ev0); }
 	if (m->ev1) { cudaEventDestroy(m->ev1); }
 	delete m;
@@ -404,11 +436,14 @@ extern "C" void rxb200_fm_mix_destroy(rxb200_fm_mix *m)
 
 namespace {
 
-// rxb200_fm_mix_create, rxb200_fm_mix_create_ddc (ddc != NULL, already checked) and rxb200_fm_mix_create_raster
-// (raster != NULL, planned; no offsets and no tables)
+// rxb200_fm_mix_create, rxb200_fm_mix_create_ddc (ddc != NULL, already checked), rxb200_fm_mix_create_raster
+// (raster != NULL, planned; no offsets and no tables) and rxb200_fm_mix_create_two_stage (ddc the coarse filter, ts
+// planned, fine its fine filter; no tables)
 int mix_create(const rxb200_fm_params *params, int capture_rate, const int *offsets_hz, int n_channels,
-               const rxb200_ddc *ddc, bool wide, const RasterPlan *raster, int device, rxb200_fm_mix **out)
+               const rxb200_ddc *ddc, bool wide, const RasterPlan *raster, int device, rxb200_fm_mix **out,
+               const TwoStage *ts = nullptr, const rxb200_ddc *fine = nullptr)
 {
+	if (ts) { raster = &ts->r; }
 	*out = nullptr;
 	// every table first: a refused offset fails before any device work
 	std::vector<int32_t> all, t;
@@ -442,7 +477,12 @@ int mix_create(const rxb200_fm_params *params, int capture_rate, const int *offs
 		const int rc = m->f.create(ddc, wide);
 		if (rc != RXB200_OK) { rxb200_fm_mix_destroy(m); return rc; }
 	}
-	if (raster) {
+	if (ts) {
+		m->ts = new (std::nothrow) TwoStage(*ts);
+		if (!m->ts) { rxb200_fm_mix_destroy(m); return RXB200_ENOMEM; }
+		const int rc = m->ts->upload(fine, (cudaStream_t)rxb200_fm_stream(m->h));
+		if (rc != RXB200_OK) { rxb200_fm_mix_destroy(m); return rc; }
+	} else if (raster) {
 		m->r = *raster;
 		m->r.wt.clear();
 		RXB_CUDA_OR(cudaMalloc(&m->d_wt, raster->w_bytes()), rxb200_fm_mix_destroy(m));
@@ -489,10 +529,26 @@ extern "C" int rxb200_fm_mix_create_raster(const rxb200_fm_params *params, int n
 	return mix_create(params, 0, nullptr, n_channels, ddc, wide, &p, device, out);
 }
 
+extern "C" int rxb200_fm_mix_create_two_stage(const rxb200_fm_params *params, int capture_rate, int n_bins,
+                                              const int *offsets_hz, int n_channels, const rxb200_ddc *coarse,
+                                              const rxb200_ddc *fine, int device, rxb200_fm_mix **out)
+{
+	if (!params || !out) { set_error("null argument"); return RXB200_EINVAL; }
+	*out = nullptr;
+	int rc = rxb::ddc_check(fine, nullptr);
+	if (rc != RXB200_OK) { return rc; }
+	rc = rxb::ddc_check(coarse, nullptr);
+	if (rc != RXB200_OK) { return rc; }
+	TwoStage t;
+	rc = t.plan(capture_rate, n_bins, offsets_hz, n_channels, coarse, fine);
+	if (rc != RXB200_OK) { return rc; }
+	return mix_create(params, 0, nullptr, n_channels, coarse, false, nullptr, device, out, &t, fine);
+}
+
 extern "C" int rxb200_fm_mix_decimated_len(const rxb200_fm_mix *m, size_t n_int16, size_t *n_dec_int16)
 {
 	if (!m || !n_dec_int16) { set_error("null argument"); return RXB200_EINVAL; }
-	*n_dec_int16 = m->ddc ? ddc_len(m->pos, n_int16, m->f.M) : n_int16;
+	*n_dec_int16 = m->ddc ? ddc_len(m->pos, n_int16, (int)decim(m)) : n_int16;
 	return RXB200_OK;
 }
 
@@ -501,7 +557,7 @@ extern "C" size_t rxb200_fm_mix_max_output(const rxb200_fm_mix *m, size_t n_int1
 	if (!m || chunk_int16 == 0) { return 0; }
 	if (!m->ddc) { return rxb200_fm_max_output(m->h, n_int16, chunk_int16); }
 	// floor((p + c) / M) - floor(p / M) <= ceil(c / M) at any phase p
-	const size_t M = (size_t)m->f.M, n16 = 2 * ((n_int16 / 2 + M - 1) / M);
+	const size_t M = decim(m), n16 = 2 * ((n_int16 / 2 + M - 1) / M);
 	return rxb200_fm_max_output(m->h, n16, chunk_int16 / M ? chunk_int16 / M : 2);
 }
 
@@ -544,6 +600,7 @@ extern "C" int rxb200_fm_mix_reset(rxb200_fm_mix *m)
 	if (m->ddc) {
 		RXB_CUDA(cudaSetDevice(m->device));
 		rc = m->f.reset((cudaStream_t)rxb200_fm_stream(m->h));   // behind any call still running on the member's stream
+		if (rc == RXB200_OK && m->ts) { rc = m->ts->reset((cudaStream_t)rxb200_fm_stream(m->h)); }
 		if (rc != RXB200_OK) { return rc; }
 	}
 	m->pos = 0;

@@ -116,10 +116,9 @@ extern "C" int rxb200_fm_mix_table(int capture_rate, int offset_hz, int32_t *tab
 }
 
 // The capture plan of the rx_fm shell's capture mode (include/rxb200.h, "rx_fm channels of one capture in the shell").
-extern "C" int rxb200_fm_plan_capture(const int64_t *tuned_hz, int n_channels, int chain_rate, long long max_capture_rate,
-                                      rxb200_fm_capture_plan *out, int *offsets_hz)
+// The centre fc and the decimation M of rxb200_fm_plan_capture's rule, with its refusals of the arguments
+static int capture_centre(const int64_t *tuned_hz, int n_channels, int chain_rate, long long *fc_out, long long *M_out)
 {
-	if (!tuned_hz || !out || !offsets_hz) { set_error("null argument"); return RXB200_EINVAL; }
 	if (n_channels < 1 || chain_rate < 1) {
 		set_error("capture plan of %d channels at a chain capture rate of %d Hz (need >= 1 of each)", n_channels, chain_rate);
 		return RXB200_EINVAL;
@@ -139,7 +138,19 @@ extern "C" int rxb200_fm_plan_capture(const int64_t *tuned_hz, int n_channels, i
 	}
 	const long long fc = g ? tmin + g * ((tmax - tmin) / (2 * g)) : tmin;
 	const long long A = std::max(fc - tmin, tmax - fc), c = chain_rate;
-	const long long M = (2 * A + c + c - 1) / c, R = M * c;
+	*fc_out = fc;
+	*M_out = (2 * A + c + c - 1) / c;
+	return RXB200_OK;
+}
+
+extern "C" int rxb200_fm_plan_capture(const int64_t *tuned_hz, int n_channels, int chain_rate, long long max_capture_rate,
+                                      rxb200_fm_capture_plan *out, int *offsets_hz)
+{
+	if (!tuned_hz || !out || !offsets_hz) { set_error("null argument"); return RXB200_EINVAL; }
+	long long fc = 0, M = 0;
+	int rc = capture_centre(tuned_hz, n_channels, chain_rate, &fc, &M);
+	if (rc != RXB200_OK) { return rc; }
+	const long long R = M * chain_rate;
 	if (R > max_capture_rate || R > 2147483647ll || M > 256) {
 		set_error("the channels need a capture rate of %lld Hz (decimation %lld), above the cap of %lld Hz, 2^31 - 1 or "
 		          "decimation 256", R, M, max_capture_rate);
@@ -147,7 +158,7 @@ extern "C" int rxb200_fm_plan_capture(const int64_t *tuned_hz, int n_channels, i
 	}
 	for (int k = 0; k < n_channels; k++) {
 		size_t L = 0;
-		const int rc = rxb200_fm_mix_table((int)R, (int)(tuned_hz[k] - fc), NULL, 0, &L);
+		rc = rxb200_fm_mix_table((int)R, (int)(tuned_hz[k] - fc), NULL, 0, &L);
 		if (rc != RXB200_ECAPACITY) { return rc; }        // the table's own refusal and message
 		offsets_hz[k] = (int)(tuned_hz[k] - fc);
 	}
@@ -155,6 +166,37 @@ extern "C" int rxb200_fm_plan_capture(const int64_t *tuned_hz, int n_channels, i
 	out->decim = (int)M;
 	out->capture_rate = (int)R;
 	out->n_taps = (int)std::min(8191ll, 32 * M + 1);
+	return RXB200_OK;
+}
+
+extern "C" int rxb200_fm_plan_capture_two_stage(const int64_t *tuned_hz, int n_channels, int chain_rate,
+                                                long long max_capture_rate, rxb200_fm_two_stage_plan *out, int *offsets_hz)
+{
+	if (!tuned_hz || !out || !offsets_hz) { set_error("null argument"); return RXB200_EINVAL; }
+	long long fc = 0, M = 0;
+	const int rc = capture_centre(tuned_hz, n_channels, chain_rate, &fc, &M);
+	if (rc != RXB200_OK) { return rc; }
+	const long long Mp = 4 * ((M + 3) / 4), R = Mp * chain_rate;
+	if (Mp < 8) {
+		set_error("two-stage capture plan: decimation %lld (from %lld) is below 8; the single-stage plan fits", Mp, M);
+		return RXB200_EINVAL;
+	}
+	if (R > max_capture_rate || R > 2147483647ll || Mp > 256) {
+		set_error("the channels need a capture rate of %lld Hz (two-stage decimation %lld), above the cap of %lld Hz, "
+		          "2^31 - 1 or decimation 256", R, Mp, max_capture_rate);
+		return RXB200_EINVAL;
+	}
+	for (int k = 0; k < n_channels; k++) { offsets_hz[k] = (int)(tuned_hz[k] - fc); }
+	const int M1 = (int)(Mp / 4);
+	out->centre_hz = fc;
+	out->capture_rate = (int)R;
+	out->n_bins = 2 * M1;
+	out->coarse_decim = M1;
+	out->coarse_taps = std::min(8191, 24 * M1 + 1);
+	out->coarse_shift = 30;
+	out->fine_decim = 4;
+	out->fine_taps = 129;
+	out->fine_shift = 15;
 	return RXB200_OK;
 }
 

@@ -292,6 +292,29 @@ def raster_device(n_bins: int, bins, n0: int, ddc, d_src_ptr: int, n_complex: in
                                                d_dst_ptr, stream or None))
 
 
+def two_stage_word(capture_rate: int, n_bins: int, coarse_decim: int, offsets_hz):
+    """Each channel's coarse bin b_c and fine NCO word w_c of a two-stage handle (``rxb200_two_stage_word``):
+    (list of bins, list of words)."""
+    offs = np.ascontiguousarray(offsets_hz, dtype=np.int32).reshape(-1)
+    bins = np.zeros(max(offs.size, 1), dtype=np.int32)
+    words = np.zeros(max(offs.size, 1), dtype=np.uint32)
+    _lib.check(_lib.lib().rxb200_two_stage_word(capture_rate, n_bins, coarse_decim, _ptr(offs), int(offs.size),
+                                                _ptr(bins), words.ctypes.data_as(C.POINTER(C.c_uint32))))
+    return [int(b) for b in bins[:offs.size]], [int(w) for w in words[:offs.size]]
+
+
+def two_stage_device(capture_rate: int, n_bins: int, offsets_hz, n0: int, coarse, fine, d_src_ptr: int,
+                     n_complex: int, d_dst_ptr: int, stream: int = 0) -> None:
+    """The two-stage down-converter alone on device pointers (``rxb200_two_stage_device``), asynchronous on ``stream``:
+    d_src[i] is capture sample n0 + i, zero samples before d_src, floor(n_complex / (M1 M2)) outputs per channel,
+    channel c's at d_dst + 2 c floor(n_complex / (M1 M2)).  coarse, fine: (decim, taps, shift)."""
+    offs = np.ascontiguousarray(offsets_hz, dtype=np.int32).reshape(-1)
+    d1, _t1 = _ddc_c(coarse)
+    d2, _t2 = _ddc_c(fine)
+    _lib.check(_lib.lib().rxb200_two_stage_device(capture_rate, n_bins, _ptr(offs), int(offs.size), n0, C.byref(d1),
+                                                  C.byref(d2), d_src_ptr, n_complex, d_dst_ptr, stream or None))
+
+
 @dataclass
 class CapturePlan:
     """rxb200_fm_capture_plan: the capture's centre fc (Hz), decimation M, capture rate R = M c and filter length T."""
@@ -313,6 +336,32 @@ def plan_capture(tuned_hz, chain_rate: int, max_rate: int):
     return CapturePlan(int(out.centre_hz), out.decim, out.capture_rate, out.n_taps), [int(v) for v in offs[:t.size]]
 
 
+@dataclass
+class TwoStagePlan:
+    """rxb200_fm_two_stage_plan: the capture's centre fc (Hz) and rate R, K coarse bins, and the two stages' decimation,
+    filter length and shift; the filters are ``power.ddc_lowpass(decim, n_taps, 15)``."""
+    centre_hz: int
+    capture_rate: int
+    n_bins: int
+    coarse_decim: int
+    coarse_taps: int
+    coarse_shift: int
+    fine_decim: int
+    fine_taps: int
+    fine_shift: int
+
+
+def plan_capture_two_stage(tuned_hz, chain_rate: int, max_rate: int):
+    """The rx_fm shell's two-stage capture plan (``rxb200_fm_plan_capture_two_stage``): (TwoStagePlan, each channel's
+    offset o_k = t_k - fc)."""
+    t = np.ascontiguousarray(tuned_hz, dtype=np.int64).reshape(-1)
+    offs = np.zeros(max(t.size, 1), dtype=np.int32)
+    out = _lib.FmTwoStagePlanC()
+    _lib.check(_lib.lib().rxb200_fm_plan_capture_two_stage(t.ctypes.data_as(C.POINTER(C.c_int64)), int(t.size),
+                                                           int(chain_rate), int(max_rate), C.byref(out), _ptr(offs)))
+    return TwoStagePlan(*(int(getattr(out, f[0])) for f in out._fields_)), [int(v) for v in offs[:t.size]]
+
+
 def disc_device(form: int, quads, stream: int = 0):
     """One discriminator alone on the device (``rxb200_fm_disc_device``): quads is a contiguous int32 CUDA tensor
     [n][4] of (ar, aj, br, bj); returns the int32 [n] results, a new tensor on the same device, written asynchronously
@@ -331,20 +380,37 @@ class FmMix(_OneGpu):
     taps, rounded by the shift and decimated by decim before the chain.
     raster = (n_bins, bins) with ddc: a raster handle (``rxb200_fm_mix_create_raster``), channel c bin bins[c] of an
     n_bins-bin raster over the capture, through the polyphase channelizer; capture_rate and offsets_hz are then not
-    passed (None)."""
+    passed (None).
+    two_stage = (n_bins, coarse, fine) without ddc: a two-stage handle (``rxb200_fm_mix_create_two_stage``), the
+    channels at offsets_hz through a coarse polyphase stage on n_bins bins and a fine NCO stage, coarse and fine being
+    (decim, taps, shift)."""
 
     _prefix = "rxb200_fm_mix"
     _streams = False
     _m = property(lambda self: self._h)     # the handle under the name callers of earlier releases read
 
     def __init__(self, params, capture_rate: Optional[int] = None, offsets_hz=None, device: int = 0, ddc=None,
-                 raster=None):
+                 raster=None, two_stage=None):
         self.params = FmParams.from_any(params)
         self.capture_rate = capture_rate
         self.ddc = ddc
         self.raster = raster
+        self.two_stage = two_stage
         self._h = C.c_void_p()
         pc = self.params.to_c()
+        if two_stage is not None:
+            if ddc is not None or raster is not None:
+                raise ValueError("a two-stage handle takes its own coarse and fine filters, no ddc or raster")
+            n_bins, coarse, fine = two_stage
+            offs = np.ascontiguousarray(offsets_hz, dtype=np.int32).reshape(-1)
+            self.offsets_hz = offs.tolist()
+            self.n_channels = int(offs.size)
+            d1, _t1 = _ddc_c(coarse)
+            d2, _t2 = _ddc_c(fine)
+            _lib.check(_lib.lib().rxb200_fm_mix_create_two_stage(C.byref(pc), capture_rate, n_bins, _ptr(offs),
+                                                                 self.n_channels, C.byref(d1), C.byref(d2), device,
+                                                                 C.byref(self._h)))
+            return
         if raster is not None:
             if ddc is None or capture_rate is not None or offsets_hz is not None:
                 raise ValueError("a raster handle takes a ddc and no capture_rate or offsets_hz")
@@ -395,7 +461,7 @@ class FmMix(_OneGpu):
 
     def mix_ms(self) -> float:
         """Device time of the last call's fm_mix_kernel (fm_ddc_kernel for a decimating handle, the two raster kernels
-        summed for a raster handle)."""
+        summed for a raster handle, both stages summed for a two-stage handle)."""
         ms = C.c_float(0)
         _lib.check(_lib.lib().rxb200_fm_mix_kernel_ms(self._h, C.byref(ms)))
         return float(ms.value)
