@@ -58,12 +58,13 @@ def ddc_lanes(T):
     return lanes
 
 
-def ddc_regime(n_out, M, T, n_ch, n_sm):
+def ddc_regime(n_out, M, T, n_ch, n_sm, rows=None):
     """ddc_launch's outputs per CTA for n_out > 0 outputs per channel: (U, which), which is "span" (the staging room),
-    "reach" (the table offsets) or "n_out" (the even share of the outputs) -- the term that sets U."""
+    "reach" (the table offsets) or "n_out" (the even share of the outputs) -- the term that sets U.  rows: the grid rows
+    of a policy that plans its own (ddc_launch's rows; None: one per MIX_GROUP channels)."""
     span = ddc_span(M, T)
     reach = (DDC_REACH - T) // M + 1
-    ctas = ddc_ctas(n_ch, n_sm)
+    ctas = ddc_ctas(n_ch, n_sm, rows)
     share = (n_out + ctas - 1) // ctas
     bound = min(span, reach)
     U = max(1, min(bound, share))
@@ -72,9 +73,10 @@ def ddc_regime(n_out, M, T, n_ch, n_sm):
     return U, "span" if span <= reach else "reach"
 
 
-def ddc_ctas(n_ch, n_sm):
-    """CTAs per grid row ddc_launch shares the outputs over."""
-    return max(1, (2 * n_sm + groups(n_ch) - 1) // groups(n_ch))
+def ddc_ctas(n_ch, n_sm, rows=None):
+    """CTAs per grid row ddc_launch shares the outputs over (rows as ddc_regime)."""
+    g = rows if rows else groups(n_ch)
+    return max(1, (2 * n_sm + g - 1) // g)
 
 
 def device_sms():

@@ -19,6 +19,7 @@ import fm_any_chunk as fac  # noqa: E402
 import fm_two_stage as fts  # noqa: E402
 from rx_tools_b200 import fm  # noqa: E402
 
+differs = 0
 for rate, K, offs, coarse, fine, n in (
         (4_096_000, 4096, [1000 * k - 2_000_000 + 7 for k in range(3000)], (1, np.array([3, -1, 2], np.int32), 18),
          (2, np.array([1, 2, 1], np.int32), 2), 2101),
@@ -33,7 +34,9 @@ for rate, K, offs, coarse, fine, n in (
     torch.cuda.synchronize()
     want = fts.two_stage_model(x, rate, K, offs, coarse, fine, (1 << 64) - 5)
     ok = out.cpu().numpy().tobytes() == want.tobytes()
+    differs += not ok
     mx = fm.FmMix(fac.with_(fac.RAW, downsample=1, offset_tuning=1), rate, offs, two_stage=(K, coarse, fine))
     got = np.concatenate([mx.process_read(x[:2 * (n // 2)]), mx.process_read(x[2 * (n // 2):])], axis=1)
     mx.close()
     print("two-stage K =", K, "M =", M, "exact" if ok else "DIFFERS", "handle", got.shape)
+sys.exit(1 if differs else 0)
