@@ -1,0 +1,338 @@
+/* rx_sdr_b200 — drop-in rx_sdr: records I/Q from a SoapySDR device, the format conversions on the GPU (librxb200).
+ *
+ * Plain mode: rx_sdr's command line (-d -f -g -c -a -s -b -n -p -D -S -I -F -t filename) and its output bytes.  Input
+ * and output formats: the same format in and out (written as read), CS16 in and CS8 / CU8 / CF32 out
+ * (rxb200_sdr_convert), or CS12 in and CS16 out; any other pair exits 1.  Every read of any length is converted and
+ * written.  -n N keeps rx_sdr's rule: a read longer than the count still to record is cut to it and ends the run; the
+ * count then drops by each read's length, and once it reaches 0 exactly it no longer limits the run.  The run ends when
+ * the device reports an error other than an overflow (a replay device at the end of its data).
+ *
+ * Capture mode: RXB200_CAPTURE_RATE=<max Hz> with one or more -f records every -f channel from ONE wideband capture.
+ * The plan is rxb200_sdr_plan_capture's for the channels and -s (RXB200_CAPTURE_STAGES=2: the two-stage plan of
+ * rxb200_fm_plan_capture_two_stage with chain rate -s); the device is tuned once to the centre at the plan's rate R
+ * and read as CS16 in reads of any length, and one rx_sdr I/Q down-converter handle (rxb200_sdr_mix_*) writes channel
+ * f's -F samples to <filename>.<f>, f the tuned frequency in Hz.  With -n N every file gets exactly N samples and the
+ * run stops; without it every output is written until the stream ends.  '-' as the filename, -I other than CS16, a
+ * frequency given twice and a plan above the cap (the message names the rate needed) exit 1 before the device is
+ * opened, and no file is created.
+ */
+#include <limits.h>
+#include <signal.h>
+#include <stdio.h>
+#include <stdlib.h>
+#include <string.h>
+#include <strings.h>
+#include <unistd.h>
+#include <SoapySDR/Device.h>
+#include <SoapySDR/Formats.h>
+#include "rxb200.h"
+#include "sdr_util.h"
+
+#define BLOCK_DEFAULT (16 * 16384)
+#define BLOCK_MIN 512
+#define BLOCK_MAX (256 * 16384)
+#define MAX_FREQS 1024
+
+static volatile sig_atomic_t g_stop = 0;
+static void on_signal(int s) { (void)s; g_stop = 1; }
+
+static void usage(void)
+{
+	fprintf(stderr,
+		"rx_sdr_b200, an I/Q recorder for SoapySDR devices (format conversions on the GPU)\n\n"
+		"Usage:\t -f frequency_to_tune_to [Hz]\n"
+		"\t[-s samplerate (default: 2048000 Hz)]\n"
+		"\t[-d device key/value query (ex: 0, 1, driver=rtlsdr, driver=hackrf)]\n"
+		"\t[-g tuner gain(s) (ex: 20, 40, LNA=40,VGA=20,AMP=0)]\n"
+		"\t[-c channel number (ex: 0)]\n"
+		"\t[-a antenna (ex: 'Tuner 1 50 ohm')]\n"
+		"\t[-p ppm_error (default: 0)]\n"
+		"\t[-b output_block_size (default: 16 * 16384)]\n"
+		"\t[-n number of samples to read (default: 0, infinite)]\n"
+		"\t[-I input format, CU8|CS8|CS12|CS16|CF32 (default: CS16)]\n"
+		"\t[-F output format, CU8|CS8|CS12|CS16|CF32 (default: CU8)]\n"
+		"\t[-S force sync output (default: async)]\n"
+		"\t[-D direct_sampling_mode, 0 (default/off), 1 (I), 2 (Q), 3 (no-mod)]\n"
+		"\t[-t SDR settings (ex: rfnotch_ctrl=false,dabnotch_ctrlb=true)]\n"
+		"\tfilename (a '-' dumps samples to stdout)\n\n"
+		"environment: RXB200_CAPTURE_RATE=max_Hz records every -f channel from one capture of at most max_Hz samples/s,\n"
+		"each to filename.<frequency>; RXB200_CAPTURE_STAGES=2 plans that capture in two stages.\n");
+	exit(1);
+}
+
+static const char *format_of(const char *s)
+{
+	static const char *names[] = {SOAPY_SDR_CU8, SOAPY_SDR_CS8, SOAPY_SDR_CS12, SOAPY_SDR_CS16, SOAPY_SDR_CF32};
+	for (size_t i = 0; i < sizeof names / sizeof names[0]; i++) {
+		if (s && !strcasecmp(s, names[i])) { return names[i]; }
+	}
+	return NULL;
+}
+
+static int same(const char *a, const char *b) { return !strcmp(a, b); }
+
+/* the rxb200 output format of -F (input CS16) */
+static int out_kind(const char *fmt)
+{
+	return same(fmt, SOAPY_SDR_CS8) ? RXB200_CVT_CS16_CS8 : same(fmt, SOAPY_SDR_CU8) ? RXB200_CVT_CS16_CU8
+	     : same(fmt, SOAPY_SDR_CF32) ? RXB200_CVT_CS16_CF32 : RXB200_SDR_OUT_CS16;
+}
+
+static size_t out_bytes(const char *fmt) { return same(fmt, SOAPY_SDR_CF32) ? 8 : same(fmt, SOAPY_SDR_CS16) ? 4 : 2; }
+
+/* "key=value,key=value" to the device's settings */
+static void write_settings(SoapySDRDevice *dev, const char *s)
+{
+	char *c = strdup(s), *save = NULL;
+	for (char *kv = strtok_r(c, ",", &save); kv; kv = strtok_r(NULL, ",", &save)) {
+		char *eq = strchr(kv, '=');
+		if (!eq) { fprintf(stderr, "Ignoring setting '%s' (no '=')\n", kv); continue; }
+		*eq = 0;
+		if (SoapySDRDevice_writeSetting(dev, kv, eq + 1) != 0) { fprintf(stderr, "Failed to set %s\n", kv); }
+	}
+	free(c);
+}
+
+struct opts {
+	const char *query, *gain, *antenna, *settings, *filename, *in_fmt, *out_fmt;
+	size_t channel;
+	int ppm, direct;
+	uint32_t rate, block, n_samples;
+	uint32_t freqs[MAX_FREQS];
+	int n_freqs;
+};
+
+/* device bring-up as rx_sdr does it: rate, frequency, gain, antenna, ppm, then a stream of `fmt` on the channel */
+static int open_device(const struct opts *o, const char *fmt, double rate, double freq, SoapySDRDevice **dev,
+                       SoapySDRStream **stream)
+{
+	SoapySDRKwargs none = {0, NULL, NULL};
+	size_t ch = o->channel;
+	*dev = SoapySDRDevice_makeStrArgs(o->query);
+	if (!*dev) { fprintf(stderr, "Failed to open sdr device matching '%s'.\n", o->query); return -1; }
+	if (o->direct) {
+		char v[16];
+		snprintf(v, sizeof v, "%d", o->direct);
+		SoapySDRDevice_writeSetting(*dev, "direct_samp", v);
+	}
+	SoapySDRDevice_setSampleRate(*dev, SOAPY_SDR_RX, ch, rate);
+	fprintf(stderr, "Sampling at %.0f S/s.\n", rate);
+	SoapySDRDevice_setFrequency(*dev, SOAPY_SDR_RX, ch, freq, NULL);
+	fprintf(stderr, "Tuned to %.0f Hz.\n", freq);
+	sdr_set_gain(*dev, ch, o->gain);
+	if (o->antenna && SoapySDRDevice_setAntenna(*dev, SOAPY_SDR_RX, ch, o->antenna) != 0) {
+		fprintf(stderr, "Failed to set antenna");
+	}
+	if (o->ppm) { SoapySDRDevice_setFrequencyCorrection(*dev, SOAPY_SDR_RX, ch, (double)o->ppm); }
+	*stream = SoapySDRDevice_setupStream(*dev, SOAPY_SDR_RX, fmt, &ch, 1, &none);
+	if (!*stream) { fprintf(stderr, "Failed to setup stream\n"); return -1; }
+	if (o->settings) { write_settings(*dev, o->settings); }
+	if (SoapySDRDevice_activateStream(*dev, *stream, 0, 0, 0) != 0) { fprintf(stderr, "Failed to activate stream\n"); return -1; }
+	return 0;
+}
+
+/* one read of at most `elems` complex elements; < 0 when the stream has ended (overflows are skipped) */
+static int read_some(SoapySDRDevice *dev, SoapySDRStream *stream, void *buf, size_t elems)
+{
+	while (!g_stop) {
+		void *buffs[] = {buf};
+		int flags = 0;
+		long long t_ns = 0;
+		const int r = SoapySDRDevice_readStream(dev, stream, buffs, elems, &flags, &t_ns, 1000000);
+		if (r >= 0) { return r; }
+		if (r != SOAPY_SDR_OVERFLOW) { return r; }
+		fprintf(stderr, "O");
+	}
+	return -1;
+}
+
+static int plain_mode(const struct opts *o)
+{
+	const size_t in_size = SoapySDR_formatToSize(o->in_fmt), cvt = !same(o->in_fmt, o->out_fmt);
+	void *buf = malloc((size_t)o->block * 4 > (size_t)o->block * in_size ? (size_t)o->block * 4 : (size_t)o->block * in_size);
+	void *out = malloc((size_t)o->block * 8);
+	SoapySDRDevice *dev = NULL;
+	SoapySDRStream *stream = NULL;
+	if (open_device(o, o->in_fmt, o->rate, o->n_freqs ? o->freqs[o->n_freqs - 1] : 100000000, &dev, &stream) != 0) { return 1; }
+	FILE *f = same(o->filename, "-") ? stdout : fopen(o->filename, "wb");
+	if (!f) { fprintf(stderr, "Failed to open %s\n", o->filename); return 1; }
+	fprintf(stderr, "Using output format: %s (input format %s, %d bytes per element)\n", o->out_fmt, o->in_fmt, (int)in_size);
+	uint32_t left = o->n_samples;
+	int rc = 0;
+	while (!g_stop) {
+		const int r = read_some(dev, stream, buf, o->block);
+		if (r < 0) { break; }
+		size_t n = (size_t)r;
+		int last = 0;
+		if (left > 0 && left < (uint32_t)r) { n = left; last = 1; }
+		const void *w = buf;
+		size_t bytes = n * in_size;
+		if (cvt && n) {
+			const int kind = same(o->in_fmt, SOAPY_SDR_CS12) ? RXB200_CVT_CS12_CS16 : out_kind(o->out_fmt);
+			if (rxb200_sdr_convert(kind, buf, n, out, 0) != RXB200_OK) {
+				fprintf(stderr, "rxb200_sdr_convert: %s\n", rxb200_last_error());
+				rc = 1;
+				break;
+			}
+			w = out;
+			bytes = n * (kind == RXB200_CVT_CS12_CS16 ? 4 : out_bytes(o->out_fmt));
+		}
+		if (fwrite(w, 1, bytes, f) != bytes) { fprintf(stderr, "Short write, samples lost, exiting!\n"); rc = 1; break; }
+		if (last) { break; }
+		if (left > 0) { left -= (uint32_t)r; }
+	}
+	if (f != stdout) { fclose(f); }
+	SoapySDRDevice_deactivateStream(dev, stream, 0, 0);
+	sdr_close(dev, stream);
+	free(buf);
+	free(out);
+	return rc;
+}
+
+static int capture_mode(const struct opts *o, const char *cap_env)
+{
+	const int K = o->n_freqs;
+	if (same(o->filename, "-")) { fprintf(stderr, "Capture mode (RXB200_CAPTURE_RATE) writes one file per channel, not to '-'.\n"); return 1; }
+	if (!same(o->in_fmt, SOAPY_SDR_CS16)) { fprintf(stderr, "Capture mode (RXB200_CAPTURE_RATE) reads CS16, not %s.\n", o->in_fmt); return 1; }
+	for (int i = 0; i < K; i++) {
+		for (int j = 0; j < i; j++) {
+			if (o->freqs[i] == o->freqs[j]) { fprintf(stderr, "Capture mode (RXB200_CAPTURE_RATE): %u Hz is given twice.\n", o->freqs[i]); return 1; }
+		}
+	}
+	const long long cap = atoll(cap_env);
+	const char *stages = getenv("RXB200_CAPTURE_STAGES");
+	const int two = stages && atoi(stages) == 2;
+	int64_t tuned[MAX_FREQS];
+	int offs[MAX_FREQS];
+	for (int i = 0; i < K; i++) { tuned[i] = o->freqs[i]; }
+	int64_t fc = 0;
+	int R = 0, M = 0;
+	int32_t *taps1 = NULL, *taps2 = NULL;
+	rxb200_ddc d1, d2;
+	rxb200_fm_two_stage_plan tp;
+	if (two) {
+		if (rxb200_fm_plan_capture_two_stage(tuned, K, (int)o->rate, cap, &tp, offs) != RXB200_OK) {
+			fprintf(stderr, "Capture mode: %s (RXB200_CAPTURE_RATE=%s).\n", rxb200_last_error(), cap_env);
+			return 1;
+		}
+		fc = tp.centre_hz; R = tp.capture_rate; M = tp.coarse_decim * tp.fine_decim;
+		taps1 = malloc((size_t)tp.coarse_taps * sizeof(int32_t));
+		taps2 = malloc((size_t)tp.fine_taps * sizeof(int32_t));
+		rxb200_ddc_lowpass(tp.coarse_decim, tp.coarse_taps, 15, taps1);
+		rxb200_ddc_lowpass(tp.fine_decim, tp.fine_taps, 15, taps2);
+		d1 = (rxb200_ddc){tp.coarse_decim, tp.coarse_taps, taps1, tp.coarse_shift};
+		d2 = (rxb200_ddc){tp.fine_decim, tp.fine_taps, taps2, tp.fine_shift};
+		fprintf(stderr, "Capture mode: %d Hz centred at %lld Hz in two stages: %d bins, coarse decimation %d with %d taps, "
+		        "fine decimation %d with %d taps, %d channels\n", R, (long long)fc, tp.n_bins, tp.coarse_decim,
+		        tp.coarse_taps, tp.fine_decim, tp.fine_taps, K);
+	} else {
+		rxb200_fm_capture_plan pl;
+		if (rxb200_sdr_plan_capture(tuned, K, (int)o->rate, cap, &pl, offs) != RXB200_OK) {
+			fprintf(stderr, "Capture mode: %s (RXB200_CAPTURE_RATE=%s).\n", rxb200_last_error(), cap_env);
+			return 1;
+		}
+		fc = pl.centre_hz; R = pl.capture_rate; M = pl.decim;
+		taps1 = malloc((size_t)pl.n_taps * sizeof(int32_t));
+		rxb200_ddc_lowpass(pl.decim, pl.n_taps, 15, taps1);
+		d1 = (rxb200_ddc){pl.decim, pl.n_taps, taps1, 15};
+		fprintf(stderr, "Capture mode: %d Hz centred at %lld Hz, decimation %d, %d taps, %d channels\n", R, (long long)fc,
+		        M, pl.n_taps, K);
+	}
+	SoapySDRDevice *dev = NULL;
+	SoapySDRStream *stream = NULL;
+	if (open_device(o, SOAPY_SDR_CS16, R, (double)fc, &dev, &stream) != 0) { return 1; }
+	rxb200_sdr_mix *h = NULL;
+	const int rc0 = two ? rxb200_sdr_mix_create_two_stage(R, tp.n_bins, offs, K, &d1, &d2, 0, &h)
+	                    : rxb200_sdr_mix_create(R, offs, K, &d1, 0, &h);
+	if (rc0 != RXB200_OK) { fprintf(stderr, "rxb200_sdr_mix_create: %s\n", rxb200_last_error()); return 1; }
+	FILE *files[MAX_FREQS];
+	for (int k = 0; k < K; k++) {
+		char name[4096];
+		snprintf(name, sizeof name, "%s.%u", o->filename, o->freqs[k]);
+		if (!(files[k] = fopen(name, "wb"))) { fprintf(stderr, "Failed to open %s\n", name); return 1; }
+	}
+	const int kind = out_kind(o->out_fmt);
+	const size_t E = out_bytes(o->out_fmt), stride = o->block / (size_t)M + 2;
+	int16_t *buf = malloc((size_t)o->block * 4);
+	unsigned char *out = malloc((size_t)K * stride * E);
+	unsigned long long written = 0;
+	int rc = 0;
+	while (!g_stop && !(o->n_samples && written >= o->n_samples)) {
+		const int r = read_some(dev, stream, buf, o->block);
+		if (r < 0) { break; }
+		size_t n = 0;
+		if (rxb200_sdr_mix_process(h, buf, 2 * (size_t)r, kind, out, (size_t)K * stride, stride, &n) != RXB200_OK) {
+			fprintf(stderr, "rxb200_sdr_mix_process: %s\n", rxb200_last_error());
+			rc = 1;
+			break;
+		}
+		if (o->n_samples && written + n > o->n_samples) { n = (size_t)(o->n_samples - written); }
+		for (int k = 0; k < K && n; k++) {
+			if (fwrite(out + (size_t)k * stride * E, E, n, files[k]) != n) { fprintf(stderr, "Short write, samples lost, exiting!\n"); rc = 1; }
+		}
+		written += n;
+		if (rc) { break; }
+	}
+	for (int k = 0; k < K; k++) { fclose(files[k]); }
+	rxb200_sdr_mix_destroy(h);
+	SoapySDRDevice_deactivateStream(dev, stream, 0, 0);
+	sdr_close(dev, stream);
+	free(buf); free(out); free(taps1); free(taps2);
+	return rc;
+}
+
+int main(int argc, char **argv)
+{
+	struct opts o;
+	memset(&o, 0, sizeof o);
+	o.query = "";
+	o.rate = 2048000;
+	o.block = BLOCK_DEFAULT;
+	o.in_fmt = SOAPY_SDR_CS16;
+	o.out_fmt = SOAPY_SDR_CU8;
+	int opt;
+	while ((opt = getopt(argc, argv, "d:f:g:c:a:s:b:n:p:D:SI:F:t:")) != -1) {
+		switch (opt) {
+		case 'd': o.query = optarg; break;
+		case 'f':
+			if (o.n_freqs == MAX_FREQS) { fprintf(stderr, "Too many frequencies (at most %d)\n", MAX_FREQS); return 1; }
+			o.freqs[o.n_freqs++] = (uint32_t)parse_scaled(optarg);
+			break;
+		case 'g': o.gain = optarg; break;
+		case 'c': o.channel = (size_t)atoi(optarg); break;
+		case 'a': o.antenna = optarg; break;
+		case 's': o.rate = (uint32_t)parse_scaled(optarg); break;
+		case 'p': o.ppm = atoi(optarg); break;
+		case 'b': o.block = (uint32_t)atof(optarg); break;
+		case 'n': o.n_samples = (uint32_t)parse_scaled(optarg); break;
+		case 'S': break;                            /* reads are synchronous either way */
+		case 'I':
+			if (!(o.in_fmt = format_of(optarg))) { fprintf(stderr, "Unsupported input format: %s\n", optarg); return 1; }
+			break;
+		case 'F':
+			if (!(o.out_fmt = format_of(optarg))) { fprintf(stderr, "Unsupported output format: %s\n", optarg); return 1; }
+			break;
+		case 'D': o.direct = atoi(optarg); break;
+		case 't': o.settings = optarg; break;
+		default: usage();
+		}
+	}
+	if (!same(o.in_fmt, o.out_fmt) && !same(o.in_fmt, SOAPY_SDR_CS16) &&
+	    !(same(o.in_fmt, SOAPY_SDR_CS12) && same(o.out_fmt, SOAPY_SDR_CS16))) {
+		fprintf(stderr, "Unsupported input/output conversion: %s to %s\n", o.in_fmt, o.out_fmt);
+		return 1;
+	}
+	if (argc <= optind) { usage(); }
+	o.filename = argv[optind];
+	if (o.block < BLOCK_MIN || o.block > BLOCK_MAX) {
+		fprintf(stderr, "Output block size wrong value, falling back to default\n");
+		fprintf(stderr, "Minimal length: %u\nMaximal length: %u\n", BLOCK_MIN, BLOCK_MAX);
+		o.block = BLOCK_DEFAULT;
+	}
+	signal(SIGINT, on_signal);
+	signal(SIGTERM, on_signal);
+	signal(SIGPIPE, on_signal);
+	const char *cap_env = getenv("RXB200_CAPTURE_RATE");
+	if (cap_env && *cap_env && o.n_freqs >= 1) { return capture_mode(&o, cap_env); }
+	return plain_mode(&o);
+}

@@ -798,6 +798,70 @@ int rxb200_sdr_convert(int kind, const void *src, size_t n_elems, void *dst, int
  *   RXB200_CVT_CS12_CS16                       : d_dst 4-byte aligned (one 32-bit store per element); d_src any */
 int rxb200_sdr_convert_device(int kind, const void *d_src, size_t n_elems, void *d_dst, void *stream);
 
+/* ---- rx_sdr channels of one capture (DESIGN.md section 4.6)
+ * An I/Q down-converter handle records C channels of ONE wideband CS16 capture at rate R (Hz), channel c at an integer
+ * offset f_c with |f_c| < R/2, each as its own decimated stream in a recorded format.  Indices n count capture samples
+ * from create or reset across calls.  It has one of two front stages:
+ *   Single stage (rxb200_sdr_mix_create, one rxb200_ddc (M, T, h, S)): channel c is the rx_power NCO rule of
+ *     "rx_power hops of one capture" (word w_c, rxb200_nco_table, the mixer's rounding and wrap) followed by the filter
+ *     rule: output q is output q of rxb200_power_ddc_device(R, f_c, 0, ddc, .) over the whole capture since create or
+ *     reset.  The NCO has no period limit, so any integer offset works.
+ *   Two stages (rxb200_sdr_mix_create_two_stage, K bins, coarse d1 and fine d2, M = M1 M2): channel c is the rule of
+ *     "two-stage mixing handles": output q is output q of rxb200_two_stage_device at n0 = 0 over the whole capture.
+ * The rule.  Output q of channel c is the stateless rule's output q over the concatenated capture since create or
+ * reset, so the bytes never depend on how the capture is cut into calls.  A call covering capture samples [n0, n0 + n)
+ * returns the floor((n0 + n) / M) - floor(n0 / M) outputs emitted in it (rxb200_sdr_mix_decimated_len); any even
+ * n_int16 is accepted, including calls with no output, which still advance the count and the histories.
+ * Formats.  format RXB200_SDR_OUT_CS16 writes the rule's int16 I/Q pairs (4 bytes per output); RXB200_CVT_CS16_CS8,
+ * _CU8 (2 bytes) and _CF32 (8 bytes) write rx_sdr's conversion of that int16 exactly as rxb200_sdr_convert defines it.
+ * The kernels write the format directly, with no CS16 pass in between.  Rows are channel-major: channel c's call
+ * output q is element c * out_stride + q of out, an output buffer of out_cap elements.
+ * Refusals, all before anything is enqueued, and a refused call changes nothing: RXB200_EINVAL for a NULL handle,
+ * capture or output, a bad format, odd n_int16, out_stride above RXB200_SDR_MIX_MAX_STRIDE, and (device entry) a capture
+ * that is not 4-byte aligned or an output not aligned to min(element, 4) bytes; RXB200_ECAPACITY when out_stride or
+ * out_cap is too small for the call's outputs (out_stride >= n_out, (C - 1) out_stride + n_out <= out_cap).
+ * The handle carries the capture count and the histories (the filter's last T - 1 raw samples, or the coarse stage's
+ * raw history and each bin's fine history), and a call's next histories become live only when it succeeds.  A host
+ * call stages its capture and outputs through the device in groups of at most RXB200_SDR_MIX_SCRATCH_BYTES, each group
+ * a device call of its own that commits its count and histories when it succeeds (so a CUDA failure in a later group
+ * leaves the earlier groups' outputs written and their state live; reset starts over), and a
+ * two-stage call runs its coarse frames in groups under RXB200_RASTER_SCRATCH_BYTES; the bytes are the same as with
+ * one group. */
+#define RXB200_SDR_OUT_CS16 4
+#define RXB200_SDR_MIX_SCRATCH_BYTES (64u << 20)
+#define RXB200_SDR_MIX_MAX_STRIDE (1u << 30)
+typedef struct rxb200_sdr_mix rxb200_sdr_mix;
+/* Refusals, all before any device is touched: RXB200_EINVAL for NULL offsets or out, n_channels < 1, R <= 0 or any
+ * |f_c| >= R/2; those of rxb200_fm_mix_create_ddc for the ddc. */
+int rxb200_sdr_mix_create(int capture_rate, const int *offsets_hz /* n_channels */, int n_channels,
+                          const rxb200_ddc *ddc, int device, rxb200_sdr_mix **out);
+/* Refusals, all before any device is touched: those of rxb200_fm_mix_create_two_stage but the params'. */
+int rxb200_sdr_mix_create_two_stage(int capture_rate, int n_bins, const int *offsets_hz /* n_channels */,
+                                    int n_channels, const rxb200_ddc *coarse, const rxb200_ddc *fine, int device,
+                                    rxb200_sdr_mix **out);
+void rxb200_sdr_mix_destroy(rxb200_sdr_mix *m);
+/* the count and every history back to the state right after create */
+int rxb200_sdr_mix_reset(rxb200_sdr_mix *m);
+/* *n_out: the outputs per channel the next call of n_int16 capture int16 returns */
+int rxb200_sdr_mix_decimated_len(const rxb200_sdr_mix *m, size_t n_int16, size_t *n_out);
+/* HOST capture and output; synchronous.  *n_out (may be NULL) receives the outputs per channel. */
+int rxb200_sdr_mix_process(rxb200_sdr_mix *m, const int16_t *cs16, size_t n_int16, int format, void *out,
+                           size_t out_cap, size_t out_stride, size_t *n_out);
+/* DEVICE capture and output, asynchronous on the handle's stream unless sync != 0. */
+int rxb200_sdr_mix_process_device(rxb200_sdr_mix *m, const int16_t *d_cs16, size_t n_int16, int format, void *d_out,
+                                  size_t out_cap, size_t out_stride, size_t *n_out, int sync);
+/* Device time (CUDA events on the handle's stream) of the down-converter kernels of the last call (of a host call's
+ * last group), in milliseconds; synchronises. */
+int rxb200_sdr_mix_kernel_ms(rxb200_sdr_mix *m, float *ms);
+/* the handle's cudaStream_t */
+void *rxb200_sdr_mix_stream(rxb200_sdr_mix *m);
+/* The plan of the rx_sdr shell's capture mode for K tuned frequencies t_k (Hz) and a per-channel rate s (rx_sdr's -s):
+ * the rule of rxb200_fm_plan_capture with c = s (fc, o_k, M, R = M s, T = min(8191, 32 M + 1), the filter
+ * rxb200_ddc_lowpass(M, T, 15) at S = 15) and its refusals, but no offset is refused for a mixer table's period, since
+ * the handle mixes with the NCO.  The two-stage plan is rxb200_fm_plan_capture_two_stage with chain rate s. */
+int rxb200_sdr_plan_capture(const int64_t *tuned_hz /* n_channels */, int n_channels, int sample_rate,
+                            long long max_capture_rate, rxb200_fm_capture_plan *out, int *offsets_hz /* n_channels */);
+
 #ifdef __cplusplus
 }
 #endif

@@ -113,6 +113,9 @@ SYMBOLS = [
     "rxb200_power_plan_tiles", "rxb200_power_tile", "rxb200_power_mix_lead", "rxb200_power_mix_accumulate_burst",
     "rxb200_power_mix_accumulate_burst_device",
     "rxb200_sdr_convert", "rxb200_sdr_convert_device",
+    "rxb200_sdr_mix_create", "rxb200_sdr_mix_create_two_stage", "rxb200_sdr_mix_destroy", "rxb200_sdr_mix_reset",
+    "rxb200_sdr_mix_decimated_len", "rxb200_sdr_mix_process", "rxb200_sdr_mix_process_device",
+    "rxb200_sdr_mix_kernel_ms", "rxb200_sdr_mix_stream", "rxb200_sdr_plan_capture",
 ]
 
 _lib = None
@@ -270,6 +273,20 @@ def lib() -> C.CDLL:
     L.rxb200_power_mix_accumulate_burst_device.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, sz, C.c_int]
     L.rxb200_sdr_convert.argtypes = [C.c_int, C.c_void_p, sz, C.c_void_p, C.c_int]
     L.rxb200_sdr_convert_device.argtypes = [C.c_int, C.c_void_p, sz, C.c_void_p, C.c_void_p]
+    L.rxb200_sdr_mix_create.argtypes = [C.c_int, pint, C.c_int, C.POINTER(DdcC), C.c_int, C.POINTER(C.c_void_p)]
+    L.rxb200_sdr_mix_create_two_stage.argtypes = [C.c_int, C.c_int, pint, C.c_int, C.POINTER(DdcC), C.POINTER(DdcC),
+                                                  C.c_int, C.POINTER(C.c_void_p)]
+    L.rxb200_sdr_mix_destroy.argtypes = [C.c_void_p]
+    L.rxb200_sdr_mix_destroy.restype = None
+    L.rxb200_sdr_mix_reset.argtypes = [C.c_void_p]
+    L.rxb200_sdr_mix_decimated_len.argtypes = [C.c_void_p, sz, C.POINTER(sz)]
+    L.rxb200_sdr_mix_process.argtypes = [C.c_void_p, C.c_void_p, sz, C.c_int, C.c_void_p, sz, sz, C.POINTER(sz)]
+    L.rxb200_sdr_mix_process_device.argtypes = [C.c_void_p, C.c_void_p, sz, C.c_int, C.c_void_p, sz, sz, C.POINTER(sz),
+                                                C.c_int]
+    L.rxb200_sdr_mix_kernel_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float)]
+    L.rxb200_sdr_mix_stream.argtypes = [C.c_void_p]
+    L.rxb200_sdr_mix_stream.restype = C.c_void_p
+    L.rxb200_sdr_plan_capture.argtypes = [pi64, C.c_int, C.c_int, C.c_longlong, C.POINTER(FmCapturePlanC), pint]
     _lib = L
     return L
 

@@ -4,13 +4,15 @@
 // them per channel into shared memory with mix_one, and runs the T-tap dot product at the emission points only; the
 // policy supplies the mixer index and the output address, the two things they differ in.  fine_ddc_kernel
 // (fm_two_stage.cu) is ddc_body too, with an NCO mixer and the staging hook ddc_row giving each grid row its own
-// stream.  The host side they share is
+// stream.  sdr_nco_kernel (sdr_mix.cu) is ddc_body with the NCO mixer and the output hook ddc_store writing an rx_sdr
+// format (SdrOut), and fine_ddc_kernel has such instances too.  The host side they share is
 // here too (the launch, the filter state a handle carries between calls) and in ddc.cu (the argument check, the
 // stateless entries' upload).
 #pragma once
 #include <algorithm>
 #include <vector>
 #include "common.cuh"
+#include "sdr_cvt.cuh"
 
 namespace rxb {
 
@@ -79,6 +81,14 @@ __device__ __forceinline__ DdcRow ddc_row(const DdcArgs<Mix> &a)
 	return DdcRow{c0, min(MIX_GROUP, a.n_ch - c0), a.src, a.hist};
 }
 
+// The output hook: the store of the current channel's call output u, w its int16 pair (I low, Q high).  By default w
+// goes to the word row.out(u); a policy that writes another format overloads it (SdrOut below).
+template <typename Mix, typename Row>
+__device__ __forceinline__ void ddc_store(const DdcArgs<Mix> &, const Row &row, int u, uint32_t w)
+{
+	*row.out(u) = w;
+}
+
 // One CTA: U consecutive outputs of every channel of its grid row (up to 256 channels, blockIdx.y).  It stages the
 // capture samples its outputs' windows cover once (the history before the call's first sample), then per channel mixes
 // them into shared memory and runs the T-tap dot product at the emission points only, lpo lanes per output.  Acc: int
@@ -86,7 +96,7 @@ __device__ __forceinline__ DdcRow ddc_row(const DdcArgs<Mix> &a)
 //   typename Mix::Row row(a, c0, nc, u0, g0)   the grid row's set-up, g0 the first staged sample's mixer position
 //   row.chan(c)                                 takes channel c's mixer state
 //   row.entry(off)                              the channel's table entry for the staged sample at offset off
-//   row.out(u)                                  the address of the channel's call output u
+//   row.out(u)                                  the address of the channel's call output u (ddc_store writes it)
 template <typename Acc, typename Mix>
 __device__ __forceinline__ void ddc_body(const DdcArgs<Mix> &a)
 {
@@ -135,12 +145,71 @@ __device__ __forceinline__ void ddc_body(const DdcArgs<Mix> &a)
 				aq += __shfl_xor_sync(0xffffffffu, aq, o);
 			}
 			if (u < U && lane == 0) {
-				*row.out(u) = ((uint32_t)ddc_out(ai, a.S) & 0xffffu) | ((uint32_t)ddc_out(aq, a.S) << 16);
+				ddc_store(a, row, u, ((uint32_t)ddc_out(ai, a.S) & 0xffffu) | ((uint32_t)ddc_out(aq, a.S) << 16));
 			}
 		}
 		__syncthreads();                    // every output of this channel is made before s_z is overwritten
 	}
 }
+
+// A mixer policy Base whose outputs are written in rx_sdr format F (RXB200_SDR_OUT_CS16 or a RXB200_CVT_CS16_* kind)
+// instead of as int16 pair words: Base's row.out(u) names the output's complex element, counted in elements from
+// a.dst, and the store converts the word there (sdr_put).  Base's Row is its RowOf template on these arguments.
+template <typename Base, int F>
+struct SdrOut : Base {
+	using Row = typename Base::template RowOf<DdcArgs<SdrOut>>;
+};
+template <typename Base, int F, typename Row>
+__device__ __forceinline__ void ddc_store(const DdcArgs<SdrOut<Base, F>> &a, const Row &row, int u, uint32_t w)
+{
+	sdr_put<F>(a.dst, row.out(u) - a.dst, w);
+}
+
+// the arguments b with the mixer policy Mix, built from b's (a base of Mix), for a launch of another instance
+template <typename Mix, typename Base>
+DdcArgs<Mix> ddc_args_as(const DdcArgs<Base> &b)
+{
+	DdcArgs<Mix> a{};
+	a.src = b.src; a.hist = b.hist; a.n_out = b.n_out; a.r0 = b.r0; a.pos = b.pos; a.dst = b.dst; a.taps = b.taps;
+	a.n_ch = b.n_ch; a.M = b.M; a.T = b.T; a.S = b.S;
+	static_cast<Base &>(a.mix) = b.mix;
+	return a;
+}
+
+// ddc_body's rx_power NCO mixer policy (power_ddc_kernel, sdr_nco_kernel): channel c's capture sample n mixed by NCO
+// entry ((n w_c + 2^15) mod 2^32) >> 16, the phase taken per CTA and channel as (uint32)g0 * w_c (g0 < 0 only for the
+// zero samples before create or reset, which mix to zero at any phase) and stepped by off * w_c in uint32 arithmetic;
+// and channel c's call output u at (u / B) * n_ch * B + c * B + u mod B, in the pass-major hop buffers of rx_power
+// (with B >= n_out, one pass: channel-major rows B apart)
+#define NCO_ENTRIES 65536            // the shared table: index j = ((theta + 2^15) mod 2^32) >> 16
+struct NcoMix {
+	const int2 *nco;                 // NCO_ENTRIES (c, s) pairs
+	const uint32_t *w;               // each hop's frequency word
+	int B;                           // outputs per hop buffer (buf_len / 2)
+	template <typename Args>
+	struct RowOf {
+		const Args &a;
+		int c0, c;
+		uint32_t g0, w, th0;             // hop c's word and its phase at the CTA's first staged sample
+		long long q0, pass_words;        // the pass of the CTA's first output, and the words of one pass
+		int rb;                          // the first output's place in its pass
+		__device__ RowOf(const Args &a, int c0, int, long long u0, long long g0)
+		    : a(a), c0(c0), g0((uint32_t)(unsigned long long)g0), q0(u0 / a.mix.B), pass_words((long long)a.n_ch * a.mix.B),
+		      rb((int)(u0 - q0 * a.mix.B)) {}
+		__device__ void chan(int k) { c = k; w = __ldg(a.mix.w + c0 + k); th0 = g0 * w; }
+		__device__ const int2 *entry(int off) const { return a.mix.nco + ((th0 + (uint32_t)off * w + 32768u) >> 16); }
+		__device__ uint32_t *out(int u) const
+		{
+			const int r = rb + u, q = r / a.mix.B;               // rb + u < B + DDC_SPAN
+			return a.dst + q0 * pass_words + (long long)(c0 + c) * a.mix.B + (q * pass_words + (r - q * a.mix.B));
+		}
+	};
+	using Row = RowOf<DdcArgs<NcoMix>>;
+};
+
+// w = floor((f 2^32 + floor(R/2)) / R) mod 2^32 for each of the n offsets, exactly, with the refusals of R <= 0 and
+// |f| >= R/2 (power_mix.cu)
+int nco_words(int capture_rate, const int *offsets_hz, int n, std::vector<uint32_t> &w);
 
 // Launches kern (a DDC kernel) on the current device for a.n_out > 0 outputs per channel, with its launch shape: a.ws,
 // a.ws_m, a.lpo, and as many outputs per CTA (a.U) as the staging room and the reach allow, but at least two CTAs per

@@ -3,7 +3,8 @@
 // stage is the raster down-converter (fm_raster.cu: raster_branch_kernel, raster_dft_kernel) run for the distinct bins
 // of the channels, writing each bin's coarse stream to a scratch row after that bin's last T2 - 1 coarse samples.  The
 // fine stage is ddc.cuh's down-converter with the rx_power NCO mixer (as power_ddc_kernel) whose grid rows each stage
-// one bin's coarse stream (the ddc_row hook below) and whose channels write to their own rows of the output.
+// one bin's coarse stream (the ddc_row hook below) and whose channels write to their own rows of the output, as int16
+// pair words or, for the rx_sdr two-stage handle (sdr_mix.cu), in a recorded format (SdrOut).
 #include <algorithm>
 #include <cstring>
 #include <numeric>
@@ -22,13 +23,14 @@ struct BinMix {
 	const int *row;                  // each channel's row of dst, channels in bin order
 	const int4 *rows;                // each grid row: (its bin's slot, its first channel, its channel count, 0)
 	long long src_stride;            // words between two slots' rows of the coarse scratch
-	long long dst_stride;            // words between two rows of dst
-	struct Row {
-		const DdcArgs<BinMix> &a;
+	long long dst_stride;            // words (elements, for SdrOut) between two rows of dst
+	template <typename Args>
+	struct RowOf {
+		const Args &a;
 		int c0, c;
 		uint32_t g0, w, th0;             // channel c's word and its phase at the CTA's first staged sample
 		long long u0;
-		__device__ Row(const DdcArgs<BinMix> &a, int c0, int, long long u0, long long g0)
+		__device__ RowOf(const Args &a, int c0, int, long long u0, long long g0)
 		    : a(a), c0(c0), g0((uint32_t)(unsigned long long)g0), u0(u0) {}
 		__device__ void chan(int k) { c = k; w = __ldg(a.mix.w + c0 + k); th0 = g0 * w; }
 		__device__ const int2 *entry(int off) const { return a.mix.nco + ((th0 + (uint32_t)off * w + 32768u) >> 16); }
@@ -37,20 +39,28 @@ struct BinMix {
 			return a.dst + (long long)__ldg(a.mix.row + c0 + c) * a.mix.dst_stride + u0 + u;
 		}
 	};
+	using Row = RowOf<DdcArgs<BinMix>>;
 };
 
 // the staging hook: grid row y stages its bin's row of the coarse scratch, whose T - 1 samples before a.src's column are
 // that bin's fine history, so the history is contiguous with the stream
-template <>
-__device__ __forceinline__ DdcRow ddc_row(const DdcArgs<BinMix> &a)
+template <typename Args>
+__device__ __forceinline__ DdcRow bin_row(const Args &a)
 {
 	const int4 g = a.mix.rows[blockIdx.y];
 	const uint32_t *src = a.src + g.x * a.mix.src_stride;
 	return DdcRow{g.y, g.z, src, src - (a.T - 1)};
 }
+template <>
+__device__ __forceinline__ DdcRow ddc_row(const DdcArgs<BinMix> &a) { return bin_row(a); }
+template <int F>
+__device__ __forceinline__ DdcRow ddc_row(const DdcArgs<SdrOut<BinMix, F>> &a) { return bin_row(a); }
 
 template <typename Acc>
 __global__ void __launch_bounds__(DDC_THREADS) fine_ddc_kernel(const DdcArgs<BinMix> a) { ddc_body<Acc>(a); }
+// the same writing rx_sdr format F (the rx_sdr two-stage handle; CS16 is the instance above)
+template <typename Acc, int F>
+__global__ void __launch_bounds__(DDC_THREADS) fine_ddc_kernel(const DdcArgs<SdrOut<BinMix, F>> a) { ddc_body<Acc>(a); }
 
 namespace {
 
@@ -67,6 +77,13 @@ __int128 floor_div(__int128 a, __int128 b)
 }
 
 size_t align16(size_t n) { return (n + 15) / 16 * 16; }
+
+template <int F>
+int fine_launch(const DdcArgs<BinMix> &b, bool wide, cudaStream_t st, int rows)
+{
+	const DdcArgs<SdrOut<BinMix, F>> a = ddc_args_as<SdrOut<BinMix, F>>(b);
+	return ddc_launch(a, wide ? fine_ddc_kernel<long long, F> : fine_ddc_kernel<int, F>, st, rows);
+}
 
 }  // namespace
 
@@ -139,7 +156,7 @@ int TwoStage::upload(const rxb200_ddc *fine, cudaStream_t st)
 
 int TwoStage::front(const DdcFilter &f, const uint32_t *src, long long r0, unsigned p0, long long n1,
                     unsigned long long nco0, int ph2, double *d_v, uint32_t *d_y, uint32_t *dst, long long stride,
-                    cudaStream_t st)
+                    cudaStream_t st, int fmt)
 {
 	if (n1 <= 0) { return RXB200_OK; }
 	const long long H = this->H(), F_max = std::min(G, n1), ys = H + F_max;
@@ -162,8 +179,11 @@ int TwoStage::front(const DdcFilter &f, const uint32_t *src, long long r0, unsig
 			a.n_out = qb - qa;
 			a.r0 = (M2 - 1) - (ph2 + l) % M2;
 			a.pos = nco0 + (unsigned long long)l;
-			a.dst = dst + qa;
-			rc = ddc_launch(a, wide2 ? fine_ddc_kernel<long long> : fine_ddc_kernel<int>, st, n_rows);
+			a.dst = reinterpret_cast<uint32_t *>(reinterpret_cast<unsigned char *>(dst) + qa * sdr_elem_bytes(fmt));
+			rc = fmt == RXB200_CVT_CS16_CS8  ? fine_launch<RXB200_CVT_CS16_CS8>(a, wide2, st, n_rows)
+			   : fmt == RXB200_CVT_CS16_CU8  ? fine_launch<RXB200_CVT_CS16_CU8>(a, wide2, st, n_rows)
+			   : fmt == RXB200_CVT_CS16_CF32 ? fine_launch<RXB200_CVT_CS16_CF32>(a, wide2, st, n_rows)
+			                                 : ddc_launch(a, wide2 ? fine_ddc_kernel<long long> : fine_ddc_kernel<int>, st, n_rows);
 			if (rc != RXB200_OK) { return rc; }
 		}
 		// each slot's last H coarse samples: the row's words [F, F + H) of (history, the group's outputs)

@@ -143,8 +143,10 @@ static int capture_centre(const int64_t *tuned_hz, int n_channels, int chain_rat
 	return RXB200_OK;
 }
 
-extern "C" int rxb200_fm_plan_capture(const int64_t *tuned_hz, int n_channels, int chain_rate, long long max_capture_rate,
-                                      rxb200_fm_capture_plan *out, int *offsets_hz)
+// rxb200_fm_plan_capture's rule; table: refuse offsets whose mixer table rxb200_fm_mix_table refuses (the rx_fm shell's
+// table mixer), else take any offset (the rx_sdr shell's NCO, rxb200_sdr_plan_capture)
+static int capture_plan(const int64_t *tuned_hz, int n_channels, int chain_rate, long long max_capture_rate,
+                        rxb200_fm_capture_plan *out, int *offsets_hz, bool table)
 {
 	if (!tuned_hz || !out || !offsets_hz) { set_error("null argument"); return RXB200_EINVAL; }
 	long long fc = 0, M = 0;
@@ -158,7 +160,7 @@ extern "C" int rxb200_fm_plan_capture(const int64_t *tuned_hz, int n_channels, i
 	}
 	for (int k = 0; k < n_channels; k++) {
 		size_t L = 0;
-		rc = rxb200_fm_mix_table((int)R, (int)(tuned_hz[k] - fc), NULL, 0, &L);
+		rc = table ? rxb200_fm_mix_table((int)R, (int)(tuned_hz[k] - fc), NULL, 0, &L) : RXB200_ECAPACITY;
 		if (rc != RXB200_ECAPACITY) { return rc; }        // the table's own refusal and message
 		offsets_hz[k] = (int)(tuned_hz[k] - fc);
 	}
@@ -167,6 +169,18 @@ extern "C" int rxb200_fm_plan_capture(const int64_t *tuned_hz, int n_channels, i
 	out->capture_rate = (int)R;
 	out->n_taps = (int)std::min(8191ll, 32 * M + 1);
 	return RXB200_OK;
+}
+
+extern "C" int rxb200_fm_plan_capture(const int64_t *tuned_hz, int n_channels, int chain_rate, long long max_capture_rate,
+                                      rxb200_fm_capture_plan *out, int *offsets_hz)
+{
+	return capture_plan(tuned_hz, n_channels, chain_rate, max_capture_rate, out, offsets_hz, true);
+}
+
+extern "C" int rxb200_sdr_plan_capture(const int64_t *tuned_hz, int n_channels, int sample_rate,
+                                       long long max_capture_rate, rxb200_fm_capture_plan *out, int *offsets_hz)
+{
+	return capture_plan(tuned_hz, n_channels, sample_rate, max_capture_rate, out, offsets_hz, false);
 }
 
 extern "C" int rxb200_fm_plan_capture_two_stage(const int64_t *tuned_hz, int n_channels, int chain_rate,

@@ -2,7 +2,7 @@
 // capture").  power_ddc_kernel mixes the capture to baseband once per hop with a phase-accumulator NCO, filters and
 // decimates it, and writes each hop's outputs straight into the pass-major hop buffers ([pass][hop][buf_len]) that
 // rxb200_power_accumulate_device reads; the member rxb200_power handle then accumulates them on its own stream.  The
-// kernel is ddc.cuh's down-converter with the NCO mixer below.  The handle carries the sample count (the NCO phases)
+// kernel is ddc.cuh's down-converter with its NCO mixer (NcoMix).  The handle carries the sample count (the NCO phases)
 // and its filter state (DdcFilter) between calls.  A burst (a fresh capture after a retune, for a tile of a wide sweep)
 // runs the same kernel on a subset of the hops, with its history read from the burst's own lead and its phases counted
 // from its first sample, and leaves the carried state alone.
@@ -16,40 +16,11 @@
 
 namespace rxb {
 
-#define NCO_ENTRIES 65536            // the shared table: index j = ((theta + 2^15) mod 2^32) >> 16
-
-// ddc_body with hop c's capture sample n mixed by NCO entry ((n w_c + 2^15) mod 2^32) >> 16, the phase taken per CTA
-// and hop as (uint32)g0 * w_c (g0 < 0 only for the zero samples before create or reset, which mix to zero at any phase)
-// and stepped by off * w_c in uint32 arithmetic; and hop c's call output u at (u / B) * n_ch * B + c * B + u mod B, in
-// the pass-major hop buffers
-struct NcoMix {
-	const int2 *nco;                 // NCO_ENTRIES (c, s) pairs
-	const uint32_t *w;               // each hop's frequency word
-	int B;                           // outputs per hop buffer (buf_len / 2)
-	struct Row {
-		const DdcArgs<NcoMix> &a;
-		int c0, c;
-		uint32_t g0, w, th0;             // hop c's word and its phase at the CTA's first staged sample
-		long long q0, pass_words;        // the pass of the CTA's first output, and the words of one pass
-		int rb;                          // the first output's place in its pass
-		__device__ Row(const DdcArgs<NcoMix> &a, int c0, int, long long u0, long long g0)
-		    : a(a), c0(c0), g0((uint32_t)(unsigned long long)g0), q0(u0 / a.mix.B), pass_words((long long)a.n_ch * a.mix.B),
-		      rb((int)(u0 - q0 * a.mix.B)) {}
-		__device__ void chan(int k) { c = k; w = __ldg(a.mix.w + c0 + k); th0 = g0 * w; }
-		__device__ const int2 *entry(int off) const { return a.mix.nco + ((th0 + (uint32_t)off * w + 32768u) >> 16); }
-		__device__ uint32_t *out(int u) const
-		{
-			const int r = rb + u, q = r / a.mix.B;               // rb + u < B + DDC_SPAN
-			return a.dst + q0 * pass_words + (long long)(c0 + c) * a.mix.B + (q * pass_words + (r - q * a.mix.B));
-		}
-	};
-};
-
 template <typename Acc>
 __global__ void __launch_bounds__(DDC_THREADS) power_ddc_kernel(const DdcArgs<NcoMix> a) { ddc_body<Acc>(a); }
 
 // w = floor((f 2^32 + floor(R/2)) / R) mod 2^32, exactly: |f| < R/2 <= 2^30, so the numerator fits 63 bits
-static int nco_words(int capture_rate, const int *offsets_hz, int n, std::vector<uint32_t> &w)
+int nco_words(int capture_rate, const int *offsets_hz, int n, std::vector<uint32_t> &w)
 {
 	const long long R = capture_rate;
 	if (R <= 0) { set_error("capture_rate %d must be > 0", capture_rate); return RXB200_EINVAL; }

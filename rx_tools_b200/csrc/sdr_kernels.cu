@@ -1,16 +1,10 @@
 // sdr_kernels.cu — rx_sdr's pointwise sample-format conversions (src/rtl_sdr.c:348-391) as one
-// bandwidth-bound kernel: 128-bit loads, grid-stride, nothing but the input read and the output written.
+// bandwidth-bound kernel: 128-bit loads, grid-stride, nothing but the input read and the output written.  The
+// per-int16 arithmetic is sdr_cvt.cuh's, shared with the I/Q down-converter's output store.
 #include "common.cuh"
+#include "sdr_cvt.cuh"
 
 namespace rxb {
-
-// (x/32767.0*128.0 + 127.4) truncated: same identity as scale_cs16 with the bias moved by 127
-// (checked for all 65 536 inputs against the oracle in tests/test_sdr_gpu.py); result 0..255.
-__device__ __forceinline__ int scale_cu8(int x)
-{
-	int t = x * 32769 + 3355366 + 127 * 8388608;     // negative only for x <= -32614: truncation gives 0 there
-	return (t >> 23) - (t >> 31);
-}
 
 __global__ void __launch_bounds__(256) sdr_convert_kernel(int kind, const uint8_t *__restrict__ src, size_t n_elems,
                                                           uint8_t *__restrict__ dst)
@@ -34,10 +28,10 @@ __global__ void __launch_bounds__(256) sdr_convert_kernel(int kind, const uint8_
 		uint32_t w[4] = {v.x, v.y, v.z, v.w};
 		if (kind == RXB200_CVT_CS16_CF32) {
 			float4 o0, o1;
-			o0.x = __fdiv_rn((float)(int16_t)(w[0] & 0xffffu), 32767.0f); o0.y = __fdiv_rn((float)(int16_t)(w[0] >> 16), 32767.0f);
-			o0.z = __fdiv_rn((float)(int16_t)(w[1] & 0xffffu), 32767.0f); o0.w = __fdiv_rn((float)(int16_t)(w[1] >> 16), 32767.0f);
-			o1.x = __fdiv_rn((float)(int16_t)(w[2] & 0xffffu), 32767.0f); o1.y = __fdiv_rn((float)(int16_t)(w[2] >> 16), 32767.0f);
-			o1.z = __fdiv_rn((float)(int16_t)(w[3] & 0xffffu), 32767.0f); o1.w = __fdiv_rn((float)(int16_t)(w[3] >> 16), 32767.0f);
+			o0.x = sdr_f32((int16_t)(w[0] & 0xffffu)); o0.y = sdr_f32((int16_t)(w[0] >> 16));
+			o0.z = sdr_f32((int16_t)(w[1] & 0xffffu)); o0.w = sdr_f32((int16_t)(w[1] >> 16));
+			o1.x = sdr_f32((int16_t)(w[2] & 0xffffu)); o1.y = sdr_f32((int16_t)(w[2] >> 16));
+			o1.z = sdr_f32((int16_t)(w[3] & 0xffffu)); o1.w = sdr_f32((int16_t)(w[3] >> 16));
 			reinterpret_cast<float4 *>(dst)[2 * i] = o0;
 			reinterpret_cast<float4 *>(dst)[2 * i + 1] = o1;
 		} else {
@@ -45,8 +39,8 @@ __global__ void __launch_bounds__(256) sdr_convert_kernel(int kind, const uint8_
 #pragma unroll
 			for (int q = 0; q < 4; q++) {
 				int a = (int)(int16_t)(w[q] & 0xffffu), b = (int)(int16_t)(w[q] >> 16);
-				int ya = kind == RXB200_CVT_CS16_CS8 ? scale_cs16(a) : scale_cu8(a);
-				int yb = kind == RXB200_CVT_CS16_CS8 ? scale_cs16(b) : scale_cu8(b);
+				int ya = kind == RXB200_CVT_CS16_CS8 ? sdr_byte<RXB200_CVT_CS16_CS8>(a) : sdr_byte<RXB200_CVT_CS16_CU8>(a);
+				int yb = kind == RXB200_CVT_CS16_CS8 ? sdr_byte<RXB200_CVT_CS16_CS8>(b) : sdr_byte<RXB200_CVT_CS16_CU8>(b);
 				o[q >> 1] |= ((uint32_t)(ya & 0xff) | ((uint32_t)(yb & 0xff) << 8)) << (16 * (q & 1));
 			}
 			reinterpret_cast<uint2 *>(dst)[i] = make_uint2(o[0], o[1]);
@@ -58,10 +52,10 @@ __global__ void __launch_bounds__(256) sdr_convert_kernel(int kind, const uint8_
 		uint32_t w = reinterpret_cast<const uint32_t *>(src)[e];
 		int a = (int)(int16_t)(w & 0xffffu), b = (int)(int16_t)(w >> 16);
 		if (kind == RXB200_CVT_CS16_CF32) {
-			reinterpret_cast<float2 *>(dst)[e] = make_float2(__fdiv_rn((float)a, 32767.0f), __fdiv_rn((float)b, 32767.0f));
+			reinterpret_cast<float2 *>(dst)[e] = make_float2(sdr_f32(a), sdr_f32(b));
 		} else {
-			int ya = kind == RXB200_CVT_CS16_CS8 ? scale_cs16(a) : scale_cu8(a);
-			int yb = kind == RXB200_CVT_CS16_CS8 ? scale_cs16(b) : scale_cu8(b);
+			int ya = kind == RXB200_CVT_CS16_CS8 ? sdr_byte<RXB200_CVT_CS16_CS8>(a) : sdr_byte<RXB200_CVT_CS16_CU8>(a);
+			int yb = kind == RXB200_CVT_CS16_CS8 ? sdr_byte<RXB200_CVT_CS16_CS8>(b) : sdr_byte<RXB200_CVT_CS16_CU8>(b);
 			dst[2 * e] = (uint8_t)ya; dst[2 * e + 1] = (uint8_t)yb;
 		}
 	}

@@ -1,7 +1,7 @@
 // two_stage.cuh — the two-stage down-converter of rx_fm two-stage mixing handles (include/rxb200.h, "two-stage mixing
 // handles"): the host side fm_mix.cu needs from fm_two_stage.cu.  A two-stage handle is a decimating handle (DdcFilter,
 // mix_call) whose DdcFilter is the coarse stage's (M1, T1, h1, S1 and the raw capture history) and whose front stage
-// runs TwoStage::front.
+// runs TwoStage::front; so is an rx_sdr two-stage handle (sdr_mix.cu), which has it write a recorded format.
 #pragma once
 #include <vector>
 #include "ddc.cuh"
@@ -39,10 +39,11 @@ struct TwoStage {
 	// One call's two stages: the n1 coarse outputs whose emission points fall in the call (the first at src index r0,
 	// with coarse index nco0 for the fine mixer, and (ph2 + l) mod M2 = M2 - 1 marking a fine emission at local coarse
 	// output l), in groups of at most G frames through d_v (G frames of branch sums) and d_y ([slots][T2 - 1 + G]);
-	// fine output q of channel c to dst + c * stride + q.  f: the coarse filter; p0: the residue mod K of src[0]'s index.
+	// fine output q of channel c to element c * stride + q of dst in format fmt (RXB200_SDR_OUT_CS16: the int16 pair
+	// word).  f: the coarse filter; p0: the residue mod K of src[0]'s index.
 	int front(const DdcFilter &f, const uint32_t *src, long long r0, unsigned p0, long long n1,
 	          unsigned long long nco0, int ph2, double *d_v, uint32_t *d_y, uint32_t *dst, long long stride,
-	          cudaStream_t st);
+	          cudaStream_t st, int fmt = RXB200_SDR_OUT_CS16);
 	void commit() { if (pending && T2 > 1) { cur ^= 1; } pending = false; }
 	int reset(cudaStream_t st);
 	void release(cudaStream_t st);
