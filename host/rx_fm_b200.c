@@ -13,7 +13,9 @@
  * without pause; the reader gathers blocks of M * 131072 complex samples, each one rxb200_fm_mix_process_read of a
  * decimating mixing handle, so every channel's chain sees reads of 131072 complex samples whatever lengths the device
  * returns.  Channel k goes to <filename>.<f_k>, with its own squelch.  With RXB200_CAPTURE_STAGES=2 as well, the plan is
- * rxb200_fm_plan_capture_two_stage's and the handle a two-stage mixing handle (M = M1 M2); nothing else changes.
+ * rxb200_fm_plan_capture_two_stage's and the handle a two-stage mixing handle (M = M1 M2); with
+ * RXB200_CAPTURE_STAGES=raster, the plan is rxb200_fm_plan_capture_raster's (channels on a common grid, at most 4096
+ * bins) and the handle a raster mixing handle; nothing else changes.
  */
 #include <errno.h>
 #include <math.h>
@@ -115,7 +117,9 @@ static void usage(void)
 		"\t[-F fir_size] [-A std|fast|lut|ale] [-c us|eu|N] [-L N] [-v]\n"
 		"\tfilename ('-' means stdout)\n"
 		"environment: RXB200_CAPTURE_RATE=max_Hz takes every -f channel from one capture of at most max_Hz samples/s,\n"
-		"\ttuned once to their centre (one GPU), channel f to filename.f (no scanning, no -l needed; refuses '-', -L, -o)\n");
+		"\ttuned once to their centre (one GPU), channel f to filename.f (no scanning, no -l needed; refuses '-', -L, -o);\n"
+		"\tRXB200_CAPTURE_STAGES=2 plans that capture in two stages, RXB200_CAPTURE_STAGES=raster as one raster of bins\n"
+		"\t(channels on a common grid, at most 4096 bins)\n");
 	exit(1);
 }
 
@@ -182,6 +186,32 @@ static int capture_setup_two_stage(const char *cap_env, const int64_t *t, int *o
 	return 0;
 }
 
+/* Capture mode with RXB200_CAPTURE_STAGES=raster: the plan of rxb200_fm_plan_capture_raster and one raster mixing handle,
+ * whose channels share one polyphase branch sum per output and one DFT. */
+static int capture_setup_raster(const char *cap_env, const int64_t *t, int64_t *centre, int *rate)
+{
+	rxb200_fm_raster_plan pl;
+	int bins[MAX_FREQS];
+	if (rxb200_fm_plan_capture_raster(t, G.freq_len, G.der.capture_rate, atoll(cap_env), &pl, bins) != RXB200_OK) {
+		fprintf(stderr, "Capture mode: %s (RXB200_CAPTURE_RATE=%s).\n", rxb200_last_error(), cap_env);
+		return 1;
+	}
+	int32_t *taps = (int32_t *)malloc(sizeof(int32_t) * (size_t)pl.n_taps);
+	rxb200_ddc_lowpass(pl.decim, pl.n_taps, 15, taps);
+	const rxb200_ddc ddc = {pl.decim, pl.n_taps, taps, pl.shift};
+	const int rc = rxb200_fm_mix_create_raster(&G.der.params, pl.n_bins, bins, G.freq_len, &ddc, 0, &G.mix);
+	free(taps);
+	if (rc != RXB200_OK) { fprintf(stderr, "rxb200: %s\n", rxb200_last_error()); return 1; }
+	G.decim = pl.decim;
+	G.block16 = (size_t)pl.decim * 2 * CHUNK_COMPLEX;
+	G.stride = rxb200_fm_mix_max_output(G.mix, G.block16, G.block16);
+	*centre = pl.centre_hz;
+	*rate = pl.capture_rate;
+	fprintf(stderr, "Capture mode: %d Hz centred at %lld Hz as a raster: %d bins, decimation %d, %d taps, %d channels\n",
+	        pl.capture_rate, (long long)pl.centre_hz, pl.n_bins, pl.decim, pl.n_taps, G.freq_len);
+	return 0;
+}
+
 /* Capture mode's plan and handle: the channels' tuned frequencies through rxb200_fm_plan_capture, the capture mode
  * filter of rx_power, one decimating mixing handle.  Nonzero (reported on stderr) when the plan or the handle is refused. */
 static int capture_setup(const char *cap_env, int64_t *centre, int *rate)
@@ -191,6 +221,7 @@ static int capture_setup(const char *cap_env, int64_t *centre, int *rate)
 	for (int k = 0; k < G.freq_len; k++) { t[k] = capture_freq(k); }
 	const char *stages = getenv("RXB200_CAPTURE_STAGES");
 	if (stages && strcmp(stages, "2") == 0) { return capture_setup_two_stage(cap_env, t, offs, centre, rate); }
+	if (stages && strcmp(stages, "raster") == 0) { return capture_setup_raster(cap_env, t, centre, rate); }
 	rxb200_fm_capture_plan pl;
 	if (rxb200_fm_plan_capture(t, G.freq_len, G.der.capture_rate, atoll(cap_env), &pl, offs) != RXB200_OK) {
 		fprintf(stderr, "Capture mode: %s (RXB200_CAPTURE_RATE=%s).\n", rxb200_last_error(), cap_env);

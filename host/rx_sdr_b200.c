@@ -9,12 +9,13 @@
  *
  * Capture mode: RXB200_CAPTURE_RATE=<max Hz> with one or more -f records every -f channel from ONE wideband capture.
  * The plan is rxb200_sdr_plan_capture's for the channels and -s (RXB200_CAPTURE_STAGES=2: the two-stage plan of
- * rxb200_fm_plan_capture_two_stage with chain rate -s); the device is tuned once to the centre at the plan's rate R
+ * rxb200_fm_plan_capture_two_stage with chain rate -s; RXB200_CAPTURE_STAGES=raster: the raster plan of
+ * rxb200_fm_plan_capture_raster, for channels on a common grid); the device is tuned once to the centre at the plan's rate R
  * and read as CS16 in reads of any length, and one rx_sdr I/Q down-converter handle (rxb200_sdr_mix_*) writes channel
  * f's -F samples to <filename>.<f>, f the tuned frequency in Hz.  With -n N every file gets exactly N samples and the
  * run stops; without it every output is written until the stream ends.  '-' as the filename, -I other than CS16, a
- * frequency given twice and a plan above the cap (the message names the rate needed) exit 1 before the device is
- * opened, and no file is created.
+ * frequency given twice and a plan above the cap (the message names the rate needed) or, for the raster, above 4096 bins
+ * exit 1 before the device is opened, and no file is created.
  */
 #include <limits.h>
 #include <signal.h>
@@ -56,7 +57,8 @@ static void usage(void)
 		"\t[-t SDR settings (ex: rfnotch_ctrl=false,dabnotch_ctrlb=true)]\n"
 		"\tfilename (a '-' dumps samples to stdout)\n\n"
 		"environment: RXB200_CAPTURE_RATE=max_Hz records every -f channel from one capture of at most max_Hz samples/s,\n"
-		"each to filename.<frequency>; RXB200_CAPTURE_STAGES=2 plans that capture in two stages.\n");
+		"each to filename.<frequency>; RXB200_CAPTURE_STAGES=2 plans that capture in two stages, and\n"
+		"RXB200_CAPTURE_STAGES=raster as one raster of bins (channels on a common grid, at most 4096 bins).\n");
 	exit(1);
 }
 
@@ -201,16 +203,29 @@ static int capture_mode(const struct opts *o, const char *cap_env)
 	}
 	const long long cap = atoll(cap_env);
 	const char *stages = getenv("RXB200_CAPTURE_STAGES");
-	const int two = stages && atoi(stages) == 2;
+	const int raster = stages && !strcmp(stages, "raster");
+	const int two = !raster && stages && atoi(stages) == 2;
 	int64_t tuned[MAX_FREQS];
-	int offs[MAX_FREQS];
+	int offs[MAX_FREQS], bins[MAX_FREQS];
 	for (int i = 0; i < K; i++) { tuned[i] = o->freqs[i]; }
 	int64_t fc = 0;
 	int R = 0, M = 0;
 	int32_t *taps1 = NULL, *taps2 = NULL;
 	rxb200_ddc d1, d2;
 	rxb200_fm_two_stage_plan tp;
-	if (two) {
+	rxb200_fm_raster_plan rp;
+	if (raster) {
+		if (rxb200_fm_plan_capture_raster(tuned, K, (int)o->rate, cap, &rp, bins) != RXB200_OK) {
+			fprintf(stderr, "Capture mode: %s (RXB200_CAPTURE_RATE=%s).\n", rxb200_last_error(), cap_env);
+			return 1;
+		}
+		fc = rp.centre_hz; R = rp.capture_rate; M = rp.decim;
+		taps1 = malloc((size_t)rp.n_taps * sizeof(int32_t));
+		rxb200_ddc_lowpass(rp.decim, rp.n_taps, 15, taps1);
+		d1 = (rxb200_ddc){rp.decim, rp.n_taps, taps1, rp.shift};
+		fprintf(stderr, "Capture mode: %d Hz centred at %lld Hz as a raster: %d bins, decimation %d, %d taps, %d channels\n",
+		        R, (long long)fc, rp.n_bins, M, rp.n_taps, K);
+	} else if (two) {
 		if (rxb200_fm_plan_capture_two_stage(tuned, K, (int)o->rate, cap, &tp, offs) != RXB200_OK) {
 			fprintf(stderr, "Capture mode: %s (RXB200_CAPTURE_RATE=%s).\n", rxb200_last_error(), cap_env);
 			return 1;
@@ -242,8 +257,9 @@ static int capture_mode(const struct opts *o, const char *cap_env)
 	SoapySDRStream *stream = NULL;
 	if (open_device(o, SOAPY_SDR_CS16, R, (double)fc, &dev, &stream) != 0) { return 1; }
 	rxb200_sdr_mix *h = NULL;
-	const int rc0 = two ? rxb200_sdr_mix_create_two_stage(R, tp.n_bins, offs, K, &d1, &d2, 0, &h)
-	                    : rxb200_sdr_mix_create(R, offs, K, &d1, 0, &h);
+	const int rc0 = raster ? rxb200_sdr_mix_create_raster(rp.n_bins, bins, K, &d1, 0, &h)
+	              : two    ? rxb200_sdr_mix_create_two_stage(R, tp.n_bins, offs, K, &d1, &d2, 0, &h)
+	                       : rxb200_sdr_mix_create(R, offs, K, &d1, 0, &h);
 	if (rc0 != RXB200_OK) { fprintf(stderr, "rxb200_sdr_mix_create: %s\n", rxb200_last_error()); return 1; }
 	FILE *files[MAX_FREQS];
 	for (int k = 0; k < K; k++) {

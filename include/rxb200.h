@@ -637,6 +637,35 @@ typedef struct rxb200_fm_two_stage_plan {
 int rxb200_fm_plan_capture_two_stage(const int64_t *tuned_hz /* n_channels */, int n_channels, int chain_rate,
                                      long long max_capture_rate, rxb200_fm_two_stage_plan *out,
                                      int *offsets_hz /* n_channels */);
+/* The plan the rx_fm and rx_sdr shells' capture modes use with RXB200_CAPTURE_STAGES=raster, for K tuned frequencies t_k
+ * on a common grid and a chain capture rate c (rx_sdr: its -s): the channels as bins of one raster handle.
+ *   fc, M, R = M c and T = min(8191, 32 M + 1) are exactly those of rxb200_fm_plan_capture, and g is its grid (the gcd
+ *     of every t_k - tmin, 0 when every t_k is equal), so every o_k = t_k - fc is a multiple of g;
+ *   K0 = R / gcd(R, g) (K0 = 1 for g = 0); K = K0 when K0 >= 3, else 3 (then every o_k is 0);
+ *   bin of channel k: b_k = (o_k K / R) mod K, exact since R / K divides every o_k; so a channel at fc is bin 0;
+ *   the filter is rxb200_ddc_lowpass(M, T, 15) at shift S = 30 (Q15 taps times the 2^15 twiddle).
+ * By the raster anchor (bin 0 at shift S + 15 is the decimating handle at offset 0 with shift S), the stream of a channel
+ * at fc is byte for byte the one the default capture mode gives it; every other channel's differs from it.
+ * Worked examples (the FM broadcast band is one -f per station):
+ *   -f set                                 chain rate c          fc            M   R           T     K
+ *   88.1-107.9 MHz, 200 kHz grid (100 ch)  250 kHz (rx_sdr -s)   97.9 MHz      81  20 250 000  2593  405
+ *   162.400-162.550 MHz, 25 kHz (7 ch)     25 kHz (rx_sdr -s)    162.475 MHz   7   175 000     225   7
+ *   162.400-162.550 MHz, 25 kHz (7 ch)     1 008 000 (-s 24k)    162.475 MHz   2   2 016 000   65    2016
+ *   162.400, 162.400001, 162.550 MHz       25 kHz                refused: g = 1 Hz, M = 7, K = 175 000
+ * Refusals, pure host arithmetic: those of rxb200_fm_plan_capture for the arguments, the cap, 2^31 - 1 and M > 256 (no
+ * mixer-table refusal: there is no table mixer); RXB200_EINVAL for K > 4096 (the message names K and the grid, and
+ * RXB200_CAPTURE_STAGES=2 for channels off a grid). */
+typedef struct rxb200_fm_raster_plan {
+	int64_t centre_hz;     /* fc */
+	int capture_rate;      /* R = M c */
+	int n_bins;            /* K */
+	int decim;             /* M */
+	int n_taps;            /* T */
+	int shift;             /* S = 30 */
+} rxb200_fm_raster_plan;
+/* bins receives the K bins b_k. */
+int rxb200_fm_plan_capture_raster(const int64_t *tuned_hz /* n_channels */, int n_channels, int chain_rate,
+                                  long long max_capture_rate, rxb200_fm_raster_plan *out, int *bins /* n_channels */);
 
 /* ======================================================================== rx_fm channels of one capture on several GPUs
  * The channels of ONE capture split over GPUs: one process, n_dev rxb200_fm_mix handles, member i owning the contiguous
@@ -801,13 +830,17 @@ int rxb200_sdr_convert_device(int kind, const void *d_src, size_t n_elems, void 
 /* ---- rx_sdr channels of one capture (DESIGN.md section 4.6)
  * An I/Q down-converter handle records C channels of ONE wideband CS16 capture at rate R (Hz), channel c at an integer
  * offset f_c with |f_c| < R/2, each as its own decimated stream in a recorded format.  Indices n count capture samples
- * from create or reset across calls.  It has one of two front stages:
+ * from create or reset across calls.  It has one of three front stages:
  *   Single stage (rxb200_sdr_mix_create, one rxb200_ddc (M, T, h, S)): channel c is the rx_power NCO rule of
  *     "rx_power hops of one capture" (word w_c, rxb200_nco_table, the mixer's rounding and wrap) followed by the filter
  *     rule: output q is output q of rxb200_power_ddc_device(R, f_c, 0, ddc, .) over the whole capture since create or
  *     reset.  The NCO has no period limit, so any integer offset works.
  *   Two stages (rxb200_sdr_mix_create_two_stage, K bins, coarse d1 and fine d2, M = M1 M2): channel c is the rule of
  *     "two-stage mixing handles": output q is output q of rxb200_two_stage_device at n0 = 0 over the whole capture.
+ *   Raster (rxb200_sdr_mix_create_raster, K bins, channel c bin k_c, one rxb200_ddc (M, T, h, S)): channel c is the rule
+ *     of "raster mixing handles": output q is output q of rxb200_raster_device(K, bins, 0, ddc, .) over the whole
+ *     capture.  Channel c sits at k_c R / K for whatever capture rate R the capture has; the handle needs none.  Its
+ *     DFT's epilogue (raster_dft_kernel) writes the format.
  * The rule.  Output q of channel c is the stateless rule's output q over the concatenated capture since create or
  * reset, so the bytes never depend on how the capture is cut into calls.  A call covering capture samples [n0, n0 + n)
  * returns the floor((n0 + n) / M) - floor(n0 / M) outputs emitted in it (rxb200_sdr_mix_decimated_len); any even
@@ -825,8 +858,8 @@ int rxb200_sdr_convert_device(int kind, const void *d_src, size_t n_elems, void 
  * call stages its capture and outputs through the device in groups of at most RXB200_SDR_MIX_SCRATCH_BYTES, each group
  * a device call of its own that commits its count and histories when it succeeds (so a CUDA failure in a later group
  * leaves the earlier groups' outputs written and their state live; reset starts over), and a
- * two-stage call runs its coarse frames in groups under RXB200_RASTER_SCRATCH_BYTES; the bytes are the same as with
- * one group. */
+ * two-stage or raster call runs its (coarse) frames in groups under RXB200_RASTER_SCRATCH_BYTES; the bytes are the
+ * same as with one group. */
 #define RXB200_SDR_OUT_CS16 4
 #define RXB200_SDR_MIX_SCRATCH_BYTES (64u << 20)
 #define RXB200_SDR_MIX_MAX_STRIDE (1u << 30)
@@ -839,6 +872,10 @@ int rxb200_sdr_mix_create(int capture_rate, const int *offsets_hz /* n_channels 
 int rxb200_sdr_mix_create_two_stage(int capture_rate, int n_bins, const int *offsets_hz /* n_channels */,
                                     int n_channels, const rxb200_ddc *coarse, const rxb200_ddc *fine, int device,
                                     rxb200_sdr_mix **out);
+/* Refusals, all before any device is touched: RXB200_EINVAL for NULL out; those of rxb200_raster_device for K, bins
+ * and the ddc (K outside [3, 4096], NULL bins, n_channels < 1, a bin outside [0, K), the ddc's own, sum |h| >= 2^22). */
+int rxb200_sdr_mix_create_raster(int n_bins, const int *bins /* n_channels */, int n_channels, const rxb200_ddc *ddc,
+                                 int device, rxb200_sdr_mix **out);
 void rxb200_sdr_mix_destroy(rxb200_sdr_mix *m);
 /* the count and every history back to the state right after create */
 int rxb200_sdr_mix_reset(rxb200_sdr_mix *m);
@@ -858,7 +895,8 @@ void *rxb200_sdr_mix_stream(rxb200_sdr_mix *m);
 /* The plan of the rx_sdr shell's capture mode for K tuned frequencies t_k (Hz) and a per-channel rate s (rx_sdr's -s):
  * the rule of rxb200_fm_plan_capture with c = s (fc, o_k, M, R = M s, T = min(8191, 32 M + 1), the filter
  * rxb200_ddc_lowpass(M, T, 15) at S = 15) and its refusals, but no offset is refused for a mixer table's period, since
- * the handle mixes with the NCO.  The two-stage plan is rxb200_fm_plan_capture_two_stage with chain rate s. */
+ * the handle mixes with the NCO.  The two-stage plan is rxb200_fm_plan_capture_two_stage and the raster plan
+ * rxb200_fm_plan_capture_raster, each with chain rate s. */
 int rxb200_sdr_plan_capture(const int64_t *tuned_hz /* n_channels */, int n_channels, int sample_rate,
                             long long max_capture_rate, rxb200_fm_capture_plan *out, int *offsets_hz /* n_channels */);
 

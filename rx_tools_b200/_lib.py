@@ -68,6 +68,11 @@ class FmTwoStagePlanC(C.Structure):
                 ("fine_shift", C.c_int)]
 
 
+class FmRasterPlanC(C.Structure):
+    _fields_ = [("centre_hz", C.c_int64), ("capture_rate", C.c_int), ("n_bins", C.c_int), ("decim", C.c_int),
+                ("n_taps", C.c_int), ("shift", C.c_int)]
+
+
 class PowerPlanC(C.Structure):
     _fields_ = [("params", PowerParamsC), ("rate", C.c_int), ("crop", C.c_double),
                 ("first_freq", C.c_int64), ("freq_step", C.c_int64), ("bin_size_hz", C.c_double)]
@@ -106,14 +111,15 @@ SYMBOLS = [
     "rxb200_fm_mix_create_ddc", "rxb200_fm_mix_decimated_len", "rxb200_fm_mix_max_output", "rxb200_ddc_device",
     "rxb200_fm_mix_group_create_ddc", "rxb200_fm_mix_create_raster", "rxb200_raster_device",
     "rxb200_fm_plan_capture", "rxb200_fm_mix_create_two_stage", "rxb200_two_stage_word", "rxb200_two_stage_device",
-    "rxb200_fm_plan_capture_two_stage",
+    "rxb200_fm_plan_capture_two_stage", "rxb200_fm_plan_capture_raster",
     "rxb200_power_mix_create", "rxb200_power_mix_destroy", "rxb200_power_mix_member", "rxb200_power_mix_reset",
     "rxb200_power_mix_accumulate", "rxb200_power_mix_accumulate_device", "rxb200_power_mix_kernel_ms",
     "rxb200_nco_table", "rxb200_power_ddc_device", "rxb200_ddc_lowpass",
     "rxb200_power_plan_tiles", "rxb200_power_tile", "rxb200_power_mix_lead", "rxb200_power_mix_accumulate_burst",
     "rxb200_power_mix_accumulate_burst_device",
     "rxb200_sdr_convert", "rxb200_sdr_convert_device",
-    "rxb200_sdr_mix_create", "rxb200_sdr_mix_create_two_stage", "rxb200_sdr_mix_destroy", "rxb200_sdr_mix_reset",
+    "rxb200_sdr_mix_create", "rxb200_sdr_mix_create_two_stage", "rxb200_sdr_mix_create_raster",
+    "rxb200_sdr_mix_destroy", "rxb200_sdr_mix_reset",
     "rxb200_sdr_mix_decimated_len", "rxb200_sdr_mix_process", "rxb200_sdr_mix_process_device",
     "rxb200_sdr_mix_kernel_ms", "rxb200_sdr_mix_stream", "rxb200_sdr_plan_capture",
 ]
@@ -251,6 +257,7 @@ def lib() -> C.CDLL:
                                           C.POINTER(DdcC), C.c_void_p, sz, C.c_void_p, C.c_void_p]
     L.rxb200_fm_plan_capture_two_stage.argtypes = [pi64, C.c_int, C.c_int, C.c_longlong, C.POINTER(FmTwoStagePlanC),
                                                    pint]
+    L.rxb200_fm_plan_capture_raster.argtypes = [pi64, C.c_int, C.c_int, C.c_longlong, C.POINTER(FmRasterPlanC), pint]
     L.rxb200_power_mix_create.argtypes = [C.POINTER(PowerParamsC), pint, p16, C.c_int, pint, C.POINTER(DdcC), C.c_int,
                                           C.POINTER(C.c_void_p)]
     L.rxb200_power_mix_destroy.argtypes = [C.c_void_p]
@@ -276,6 +283,7 @@ def lib() -> C.CDLL:
     L.rxb200_sdr_mix_create.argtypes = [C.c_int, pint, C.c_int, C.POINTER(DdcC), C.c_int, C.POINTER(C.c_void_p)]
     L.rxb200_sdr_mix_create_two_stage.argtypes = [C.c_int, C.c_int, pint, C.c_int, C.POINTER(DdcC), C.POINTER(DdcC),
                                                   C.c_int, C.POINTER(C.c_void_p)]
+    L.rxb200_sdr_mix_create_raster.argtypes = [C.c_int, pint, C.c_int, C.POINTER(DdcC), C.c_int, C.POINTER(C.c_void_p)]
     L.rxb200_sdr_mix_destroy.argtypes = [C.c_void_p]
     L.rxb200_sdr_mix_destroy.restype = None
     L.rxb200_sdr_mix_reset.argtypes = [C.c_void_p]

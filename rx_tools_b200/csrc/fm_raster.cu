@@ -4,9 +4,10 @@
 //     v_rho[m] = sum_{j<T, (e_m - j) mod K = rho} h[j] x[e_m - j],     A_k[m] = sum_rho tw[(k rho) mod K] v_rho[m].
 // raster_branch_kernel makes the rows v[m] (2K doubles) of a group of frames, shared by every channel; raster_dft_kernel
 // multiplies them by the handle's constant real [2K][2C] twiddle matrix with DMMA (mma.sync m8n8k4 f64) and rounds,
-// saturates and writes each channel's outputs.  Every value is an integer: |v| <= sum |h| 2^15 < 2^37, every product
-// |v| 2^15 < 2^52 and every partial sum at most sum |h| 2^31 < 2^53, so fp64 holds them all exactly and the result does
-// not depend on the order the tensor cores sum in.
+// saturates and writes each channel's outputs, as int16 pair words or in an rx_sdr format (sdr_mix.cu's raster kind).
+// Every value is an integer: |v| <= sum |h| 2^15 < 2^37, every product |v| 2^15 < 2^52 and every partial sum at most
+// sum |h| 2^31 < 2^53, so fp64 holds them all exactly and the result does not depend on the order the tensor cores sum
+// in.
 #include <algorithm>
 #include <cstring>
 #include "ddc.cuh"
@@ -83,7 +84,7 @@ struct DftArgs {
 	const double *Wt;                 // [Np][Kp]
 	long long F;
 	int Kp, n_col, S;                 // n_col = 2C
-	uint32_t *dst;                    // channel c's output u at dst[c * stride + u]
+	void *dst;                        // channel c's output u is complex element c * stride + u of the format's row at dst
 	long long stride;
 };
 
@@ -96,7 +97,10 @@ __device__ __forceinline__ void cp_async16(void *smem, const void *gmem, int byt
 // Y = V Wt^T for one 64 x 64 tile (64 frames, 32 channels): eight warps of 32 x 16, each a 4 x 2 grid of DMMA 8 x 8
 // tiles over k steps of 4; the operands stream through shared memory in stages of 16 input columns with cp.async,
 // two stages in flight.  Frames past F load as zeros and store nothing.  The epilogue converts each (I, Q) pair to
-// int64 (exact), rounds by S and saturates with ddc_out, and writes one word per channel and frame.
+// int64 (exact), rounds by S and saturates with ddc_out, and writes one element per channel and frame in rx_sdr format
+// F (sdr_put): the int16 pair word for RXB200_SDR_OUT_CS16 (rx_fm's raster and two-stage handles), a CS16 conversion
+// for the rx_sdr raster handle.
+template <int F>
 __global__ void __launch_bounds__(RAS_THREADS) raster_dft_kernel(const DftArgs a)
 {
 	__shared__ __align__(16) double s_a[2][RAS_BM][RAS_LD];
@@ -161,7 +165,7 @@ __global__ void __launch_bounds__(RAS_THREADS) raster_dft_kernel(const DftArgs a
 			const int col = n0 + wn + j * 8 + 2 * t4;
 			if (f < a.F && col < a.n_col) {
 				const int yi = ddc_out((long long)acc[i][j][0], a.S), yq = ddc_out((long long)acc[i][j][1], a.S);
-				a.dst[(long long)(col >> 1) * a.stride + f] = ((uint32_t)yi & 0xffffu) | ((uint32_t)yq << 16);
+				sdr_put<F>(a.dst, (long long)(col >> 1) * a.stride + f, ((uint32_t)yi & 0xffffu) | ((uint32_t)yq << 16));
 			}
 		}
 	}
@@ -210,9 +214,13 @@ int RasterPlan::plan(int n_bins, const int *bins, int n_channels)
 }
 
 int raster_front(const RasterPlan &p, const double *d_wt, double *V, const uint32_t *src, const uint32_t *hist,
-                 const int32_t *taps, int M, int T, int S, long long r0, unsigned p0, long long n_out, uint32_t *dst,
-                 long long stride, cudaStream_t st)
+                 const int32_t *taps, int M, int T, int S, long long r0, unsigned p0, long long n_out, void *dst,
+                 long long stride, cudaStream_t st, int fmt)
 {
+	void (*const dft)(DftArgs) = fmt == RXB200_CVT_CS16_CS8  ? raster_dft_kernel<RXB200_CVT_CS16_CS8>
+	                           : fmt == RXB200_CVT_CS16_CU8  ? raster_dft_kernel<RXB200_CVT_CS16_CU8>
+	                           : fmt == RXB200_CVT_CS16_CF32 ? raster_dft_kernel<RXB200_CVT_CS16_CF32>
+	                                                         : raster_dft_kernel<RXB200_SDR_OUT_CS16>;
 	int dev = 0, n_sm = 0;
 	RXB_CUDA(cudaGetDevice(&dev));
 	RXB_CUDA(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
@@ -235,8 +243,8 @@ int raster_front(const RasterPlan &p, const double *d_wt, double *V, const uint3
 		raster_branch_kernel<<<(unsigned)((F + U - 1) / U), RAS_THREADS, smem, st>>>(b);
 		RXB_CUDA(cudaGetLastError());
 		d.F = F;
-		d.dst = dst + f0;
-		raster_dft_kernel<<<dim3((unsigned)((F + RAS_BM - 1) / RAS_BM), (unsigned)(p.Np / RAS_BN)), RAS_THREADS, 0, st>>>(d);
+		d.dst = static_cast<unsigned char *>(dst) + f0 * sdr_elem_bytes(fmt);
+		dft<<<dim3((unsigned)((F + RAS_BM - 1) / RAS_BM), (unsigned)(p.Np / RAS_BN)), RAS_THREADS, 0, st>>>(d);
 		RXB_CUDA(cudaGetLastError());
 	}
 	return RXB200_OK;

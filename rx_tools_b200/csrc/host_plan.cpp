@@ -116,8 +116,10 @@ extern "C" int rxb200_fm_mix_table(int capture_rate, int offset_hz, int32_t *tab
 }
 
 // The capture plan of the rx_fm shell's capture mode (include/rxb200.h, "rx_fm channels of one capture in the shell").
-// The centre fc and the decimation M of rxb200_fm_plan_capture's rule, with its refusals of the arguments
-static int capture_centre(const int64_t *tuned_hz, int n_channels, int chain_rate, long long *fc_out, long long *M_out)
+// The centre fc, the decimation M and the channel grid g of rxb200_fm_plan_capture's rule, with its refusals of the
+// arguments (g_out may be NULL)
+static int capture_centre(const int64_t *tuned_hz, int n_channels, int chain_rate, long long *fc_out, long long *M_out,
+                          long long *g_out = NULL)
 {
 	if (n_channels < 1 || chain_rate < 1) {
 		set_error("capture plan of %d channels at a chain capture rate of %d Hz (need >= 1 of each)", n_channels, chain_rate);
@@ -140,6 +142,18 @@ static int capture_centre(const int64_t *tuned_hz, int n_channels, int chain_rat
 	const long long A = std::max(fc - tmin, tmax - fc), c = chain_rate;
 	*fc_out = fc;
 	*M_out = (2 * A + c + c - 1) / c;
+	if (g_out) { *g_out = g; }
+	return RXB200_OK;
+}
+
+// the single-stage plan's refusal of its capture rate R = M c
+static int rate_check(long long R, long long M, long long max_capture_rate)
+{
+	if (R > max_capture_rate || R > 2147483647ll || M > 256) {
+		set_error("the channels need a capture rate of %lld Hz (decimation %lld), above the cap of %lld Hz, 2^31 - 1 or "
+		          "decimation 256", R, M, max_capture_rate);
+		return RXB200_EINVAL;
+	}
 	return RXB200_OK;
 }
 
@@ -153,11 +167,8 @@ static int capture_plan(const int64_t *tuned_hz, int n_channels, int chain_rate,
 	int rc = capture_centre(tuned_hz, n_channels, chain_rate, &fc, &M);
 	if (rc != RXB200_OK) { return rc; }
 	const long long R = M * chain_rate;
-	if (R > max_capture_rate || R > 2147483647ll || M > 256) {
-		set_error("the channels need a capture rate of %lld Hz (decimation %lld), above the cap of %lld Hz, 2^31 - 1 or "
-		          "decimation 256", R, M, max_capture_rate);
-		return RXB200_EINVAL;
-	}
+	rc = rate_check(R, M, max_capture_rate);
+	if (rc != RXB200_OK) { return rc; }
 	for (int k = 0; k < n_channels; k++) {
 		size_t L = 0;
 		rc = table ? rxb200_fm_mix_table((int)R, (int)(tuned_hz[k] - fc), NULL, 0, &L) : RXB200_ECAPACITY;
@@ -211,6 +222,37 @@ extern "C" int rxb200_fm_plan_capture_two_stage(const int64_t *tuned_hz, int n_c
 	out->fine_decim = 4;
 	out->fine_taps = 129;
 	out->fine_shift = 15;
+	return RXB200_OK;
+}
+
+extern "C" int rxb200_fm_plan_capture_raster(const int64_t *tuned_hz, int n_channels, int chain_rate,
+                                             long long max_capture_rate, rxb200_fm_raster_plan *out, int *bins)
+{
+	if (!tuned_hz || !out || !bins) { set_error("null argument"); return RXB200_EINVAL; }
+	long long fc = 0, M = 0, g = 0;
+	int rc = capture_centre(tuned_hz, n_channels, chain_rate, &fc, &M, &g);
+	if (rc != RXB200_OK) { return rc; }
+	const long long R = M * chain_rate;
+	rc = rate_check(R, M, max_capture_rate);
+	if (rc != RXB200_OK) { return rc; }
+	long long a = R, b = g;                              // K0 = R / gcd(R, g), 1 for g = 0
+	while (b) { const long long t = a % b; a = b; b = t; }
+	const long long K = std::max(3ll, R / a);
+	if (K > 4096) {
+		set_error("raster capture plan: the channels' %lld Hz grid at a capture rate of %lld Hz needs %lld bins, above "
+		          "4096; RXB200_CAPTURE_STAGES=2 takes channels off a grid", g, R, K);
+		return RXB200_EINVAL;
+	}
+	for (int k = 0; k < n_channels; k++) {
+		const long long o = tuned_hz[k] - fc;             // a multiple of R / K: o K / R is exact
+		bins[k] = (int)((o * K / R % K + K) % K);
+	}
+	out->centre_hz = fc;
+	out->capture_rate = (int)R;
+	out->n_bins = (int)K;
+	out->decim = (int)M;
+	out->n_taps = (int)std::min(8191ll, 32 * M + 1);
+	out->shift = 30;
 	return RXB200_OK;
 }
 

@@ -23,9 +23,10 @@ struct RasterPlan {
 
 // One call's raster front stage on the current device: n_out outputs per channel from the capture at src (hist: the
 // T - 1 samples before it; r0: src index of the first emission point; p0: the residue mod K of src[0]'s sample index)
-// to dst, channel c's output u at word c * stride + u, through V (room for min(n_out, plan.group) frames).
+// to dst, channel c's output u at complex element c * stride + u of rx_sdr format fmt (RXB200_SDR_OUT_CS16: the int16
+// pair word), through V (room for min(n_out, plan.group) frames).
 int raster_front(const RasterPlan &p, const double *d_wt, double *V, const uint32_t *src, const uint32_t *hist,
-                 const int32_t *taps, int M, int T, int S, long long r0, unsigned p0, long long n_out, uint32_t *dst,
-                 long long stride, cudaStream_t st);
+                 const int32_t *taps, int M, int T, int S, long long r0, unsigned p0, long long n_out, void *dst,
+                 long long stride, cudaStream_t st, int fmt = RXB200_SDR_OUT_CS16);
 
 }  // namespace rxb

@@ -4,6 +4,7 @@
 // A single-stage handle runs sdr_nco_kernel, ddc.cuh's down-converter with power_mix.cu's NCO mixer (NcoMix, its pass
 // length set to the row stride so that every channel's outputs form one row) and the rx_sdr output store (SdrOut).  A
 // two-stage handle runs fm_two_stage.cu's coarse and fine stages (TwoStage::front), the fine stage writing the format.
+// A raster handle runs fm_raster.cu's polyphase channelizer (raster_front), its DFT epilogue writing the format.
 #include <algorithm>
 #include <new>
 #include <vector>
@@ -39,7 +40,9 @@ struct rxb200_sdr_mix {
 	uint32_t *d_w = nullptr;                     // single stage: each channel's NCO word
 	int2 *d_nco = nullptr;                       // single stage: the shared NCO table
 	TwoStage *ts = nullptr;                      // two stages: the plan, the fine stage and the bins' histories
-	double *d_v = nullptr; size_t v_cap = 0;     // two stages: the coarse branch sums (doubles)
+	RasterPlan r;                                // raster (r.K > 0): the raster's shape, its twiddle matrix at d_wt
+	double *d_wt = nullptr;
+	double *d_v = nullptr; size_t v_cap = 0;     // two stages, raster: the (coarse) branch sums (doubles)
 	uint32_t *d_y = nullptr; size_t y_cap = 0;   // two stages: the coarse rows (words)
 	unsigned long long pos = 0;                  // capture samples since create or reset
 	int16_t *d_cap = nullptr; size_t cap_cap = 0;         // host calls: the capture (int16 elements)
@@ -108,6 +111,13 @@ int device_call(rxb200_sdr_mix *m, const int16_t *src, size_t c, int fmt, void *
 			                       (long long)stride, st, fmt);
 			if (rc != RXB200_OK) { return rc; }
 		}
+	} else if (m->r.K && n) {
+		RXB_CUDA(reserve(m->d_v, m->v_cap, (size_t)std::min((long long)n, m->r.group) * (size_t)m->r.Kp));
+		const int rc = raster_front(m->r, m->d_wt, m->d_v, reinterpret_cast<const uint32_t *>(src), f.hist[f.cur], f.taps,
+		                            f.M, f.T, f.S, (long long)(f.M - 1) - (long long)(m->pos % (unsigned long long)f.M),
+		                            (unsigned)(m->pos % (unsigned long long)m->r.K), (long long)n, dst, (long long)stride,
+		                            st, fmt);
+		if (rc != RXB200_OK) { return rc; }
 	} else if (n) {
 		DdcArgs<NcoMix> a{};
 		a.src = reinterpret_cast<const uint32_t *>(src);
@@ -144,10 +154,11 @@ size_t host_group(const rxb200_sdr_mix *m, int fmt)
 	return M * std::max<size_t>(1, (size_t)RXB200_SDR_MIX_SCRATCH_BYTES / per);
 }
 
-// rxb200_sdr_mix_create (w the channels' NCO words, ddc the filter) and rxb200_sdr_mix_create_two_stage (ts planned,
-// ddc the coarse filter, fine the fine one), after every refusal
+// rxb200_sdr_mix_create (w the channels' NCO words, ddc the filter), rxb200_sdr_mix_create_two_stage (ts planned,
+// ddc the coarse filter, fine the fine one) and rxb200_sdr_mix_create_raster (raster planned, ddc the filter), after
+// every refusal
 int mix_create(const std::vector<uint32_t> &w, int n_channels, const rxb200_ddc *ddc, bool wide, const TwoStage *ts,
-               const rxb200_ddc *fine, int device, rxb200_sdr_mix **out)
+               const rxb200_ddc *fine, const RasterPlan *raster, int device, rxb200_sdr_mix **out)
 {
 	rxb200_sdr_mix *m = new (std::nothrow) rxb200_sdr_mix();
 	if (!m) { return RXB200_ENOMEM; }
@@ -165,6 +176,12 @@ int mix_create(const std::vector<uint32_t> &w, int n_channels, const rxb200_ddc 
 		rc = m->ts->upload(fine, m->st);
 		if (rc != RXB200_OK) { rxb200_sdr_mix_destroy(m); return rc; }
 		RXB_CUDA_OR(cudaStreamSynchronize(m->st), rxb200_sdr_mix_destroy(m));
+	} else if (raster) {
+		m->r = *raster;
+		m->r.wt.clear();
+		RXB_CUDA_OR(cudaMalloc(&m->d_wt, raster->w_bytes()), rxb200_sdr_mix_destroy(m));
+		RXB_CUDA_OR(cudaMemcpy(m->d_wt, raster->wt.data(), raster->w_bytes(), cudaMemcpyHostToDevice),
+		            rxb200_sdr_mix_destroy(m));
 	} else {
 		std::vector<int32_t> nco(2 * NCO_ENTRIES);
 		rxb200_nco_table(nco.data());
@@ -187,7 +204,7 @@ extern "C" void rxb200_sdr_mix_destroy(rxb200_sdr_mix *m)
 	if (m->ts) { m->ts->release(m->st); delete m->ts; }
 	if (m->st) { cudaStreamSynchronize(m->st); }
 	m->f.release();
-	cudaFree(m->d_w); cudaFree(m->d_nco); cudaFree(m->d_v); cudaFree(m->d_y); cudaFree(m->d_cap); cudaFree(m->d_out);
+	cudaFree(m->d_w); cudaFree(m->d_nco); cudaFree(m->d_wt); cudaFree(m->d_v); cudaFree(m->d_y); cudaFree(m->d_cap); cudaFree(m->d_out);
 	if (m->ev0) { cudaEventDestroy(m->ev0); }
 	if (m->ev1) { cudaEventDestroy(m->ev1); }
 	if (m->st) { cudaStreamDestroy(m->st); }
@@ -205,7 +222,7 @@ extern "C" int rxb200_sdr_mix_create(int capture_rate, const int *offsets_hz, in
 	bool wide = false;
 	rc = ddc_check(ddc, &wide);
 	if (rc != RXB200_OK) { return rc; }
-	return mix_create(w, n_channels, ddc, wide, nullptr, nullptr, device, out);
+	return mix_create(w, n_channels, ddc, wide, nullptr, nullptr, nullptr, device, out);
 }
 
 extern "C" int rxb200_sdr_mix_create_two_stage(int capture_rate, int n_bins, const int *offsets_hz, int n_channels,
@@ -221,7 +238,23 @@ extern "C" int rxb200_sdr_mix_create_two_stage(int capture_rate, int n_bins, con
 	TwoStage t;
 	rc = t.plan(capture_rate, n_bins, offsets_hz, n_channels, coarse, fine);
 	if (rc != RXB200_OK) { return rc; }
-	return mix_create({}, n_channels, coarse, false, &t, fine, device, out);
+	return mix_create({}, n_channels, coarse, false, &t, fine, nullptr, device, out);
+}
+
+extern "C" int rxb200_sdr_mix_create_raster(int n_bins, const int *bins, int n_channels, const rxb200_ddc *ddc,
+                                            int device, rxb200_sdr_mix **out)
+{
+	if (!out) { set_error("null argument"); return RXB200_EINVAL; }
+	*out = nullptr;
+	bool wide = false;
+	int rc = ddc_check(ddc, &wide);
+	if (rc != RXB200_OK) { return rc; }
+	rc = raster_check(n_bins, bins, n_channels, ddc);
+	if (rc != RXB200_OK) { return rc; }
+	RasterPlan p;
+	rc = p.plan(n_bins, bins, n_channels);
+	if (rc != RXB200_OK) { return rc; }
+	return mix_create({}, n_channels, ddc, wide, nullptr, nullptr, &p, device, out);
 }
 
 extern "C" int rxb200_sdr_mix_reset(rxb200_sdr_mix *m)

@@ -362,6 +362,29 @@ def plan_capture_two_stage(tuned_hz, chain_rate: int, max_rate: int):
     return TwoStagePlan(*(int(getattr(out, f[0])) for f in out._fields_)), [int(v) for v in offs[:t.size]]
 
 
+@dataclass
+class RasterCapturePlan:
+    """rxb200_fm_raster_plan: the capture's centre fc (Hz) and rate R, K raster bins, and the filter's decimation M,
+    length T and shift S; the filter is ``power.ddc_lowpass(decim, n_taps, 15)``."""
+    centre_hz: int
+    capture_rate: int
+    n_bins: int
+    decim: int
+    n_taps: int
+    shift: int
+
+
+def plan_capture_raster(tuned_hz, chain_rate: int, max_rate: int):
+    """The capture plan of the shells' raster mode (``rxb200_fm_plan_capture_raster``) for tuned frequencies on a common
+    grid: (RasterCapturePlan, each channel's raster bin b_k).  rx_fm passes its chain capture rate, rx_sdr its -s."""
+    t = np.ascontiguousarray(tuned_hz, dtype=np.int64).reshape(-1)
+    bins = np.zeros(max(t.size, 1), dtype=np.int32)
+    out = _lib.FmRasterPlanC()
+    _lib.check(_lib.lib().rxb200_fm_plan_capture_raster(t.ctypes.data_as(C.POINTER(C.c_int64)), int(t.size),
+                                                        int(chain_rate), int(max_rate), C.byref(out), _ptr(bins)))
+    return RasterCapturePlan(*(int(getattr(out, f[0])) for f in out._fields_)), [int(v) for v in bins[:t.size]]
+
+
 def disc_device(form: int, quads, stream: int = 0):
     """One discriminator alone on the device (``rxb200_fm_disc_device``): quads is a contiguous int32 CUDA tensor
     [n][4] of (ar, aj, br, bj); returns the int32 [n] results, a new tensor on the same device, written asynchronously

@@ -32,18 +32,31 @@ def plan_sdr_capture(tuned_hz, sample_rate: int, max_rate: int):
 class SdrMix:
     """``len(offsets_hz)`` channels of ONE CS16 capture at ``capture_rate``.  ddc = (decim, taps, shift): the single
     stage (``rxb200_sdr_mix_create``), channel c the rx_power NCO rule then the filter.  two_stage = (n_bins, coarse,
-    fine) instead: the two-stage rule (``rxb200_sdr_mix_create_two_stage``).  Every call takes the capture, int16
-    [n_int16], and returns the call's outputs in format fmt (``FORMATS``) as a [n_channels][2 n_out] array of the
-    format's component type."""
+    fine) instead: the two-stage rule (``rxb200_sdr_mix_create_two_stage``).  raster = (n_bins, bins) with ddc: the
+    raster rule (``rxb200_sdr_mix_create_raster``), channel c bin bins[c] of an n_bins-bin raster over the capture;
+    capture_rate and offsets_hz are then None.  Every call takes the capture, int16 [n_int16], and returns the call's
+    outputs in format fmt (``FORMATS``) as a [n_channels][2 n_out] array of the format's component type."""
 
-    def __init__(self, capture_rate: int, offsets_hz, ddc=None, two_stage=None, device: int = 0):
+    def __init__(self, capture_rate: Optional[int] = None, offsets_hz=None, ddc=None, two_stage=None, device: int = 0,
+                 raster=None):
         if (ddc is None) == (two_stage is None):
             raise ValueError("give exactly one of ddc and two_stage")
-        offs = np.ascontiguousarray(offsets_hz, dtype=np.int32).reshape(-1)
-        self.capture_rate, self.offsets_hz, self.n_channels = capture_rate, offs.tolist(), int(offs.size)
         self.device = device
         self._h = C.c_void_p()
         L = _lib.lib()
+        if raster is not None:
+            if ddc is None or capture_rate is not None or offsets_hz is not None:
+                raise ValueError("a raster handle takes a ddc and bins, no capture_rate or offsets_hz")
+            n_bins, bins = raster
+            b = np.ascontiguousarray(bins, dtype=np.int32).reshape(-1)
+            self.capture_rate, self.offsets_hz, self.n_channels = None, None, int(b.size)
+            d, _t = _ddc_c(ddc)
+            self.decim = int(ddc[0])
+            _lib.check(L.rxb200_sdr_mix_create_raster(n_bins, _ptr(b), self.n_channels, C.byref(d), device,
+                                                      C.byref(self._h)))
+            return
+        offs = np.ascontiguousarray(offsets_hz, dtype=np.int32).reshape(-1)
+        self.capture_rate, self.offsets_hz, self.n_channels = capture_rate, offs.tolist(), int(offs.size)
         if ddc is not None:
             d, _t = _ddc_c(ddc)
             self.decim = int(ddc[0])
