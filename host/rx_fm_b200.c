@@ -155,91 +155,36 @@ static void write_wav_header(FILE *out)
 	fwrite(h, 1, sizeof h, out);
 }
 
-/* Capture mode with RXB200_CAPTURE_STAGES=2: the plan of rxb200_fm_plan_capture_two_stage and one two-stage mixing
- * handle, whose channel filters cost a coarse DFT shared by every channel plus a 129-tap fine filter per channel. */
-static int capture_setup_two_stage(const char *cap_env, const int64_t *t, int *offs, int64_t *centre, int *rate)
-{
-	rxb200_fm_two_stage_plan pl;
-	if (rxb200_fm_plan_capture_two_stage(t, G.freq_len, G.der.capture_rate, atoll(cap_env), &pl, offs) != RXB200_OK) {
-		fprintf(stderr, "Capture mode: %s (RXB200_CAPTURE_RATE=%s).\n", rxb200_last_error(), cap_env);
-		return 1;
-	}
-	int32_t *h1 = (int32_t *)malloc(sizeof(int32_t) * (size_t)pl.coarse_taps);
-	int32_t *h2 = (int32_t *)malloc(sizeof(int32_t) * (size_t)pl.fine_taps);
-	rxb200_ddc_lowpass(pl.coarse_decim, pl.coarse_taps, 15, h1);
-	rxb200_ddc_lowpass(pl.fine_decim, pl.fine_taps, 15, h2);
-	const rxb200_ddc coarse = {pl.coarse_decim, pl.coarse_taps, h1, pl.coarse_shift};
-	const rxb200_ddc fine = {pl.fine_decim, pl.fine_taps, h2, pl.fine_shift};
-	const int rc = rxb200_fm_mix_create_two_stage(&G.der.params, pl.capture_rate, pl.n_bins, offs, G.freq_len, &coarse,
-	                                              &fine, 0, &G.mix);
-	free(h1);
-	free(h2);
-	if (rc != RXB200_OK) { fprintf(stderr, "rxb200: %s\n", rxb200_last_error()); return 1; }
-	G.decim = pl.coarse_decim * pl.fine_decim;
-	G.block16 = (size_t)G.decim * 2 * CHUNK_COMPLEX;
-	G.stride = rxb200_fm_mix_max_output(G.mix, G.block16, G.block16);
-	*centre = pl.centre_hz;
-	*rate = pl.capture_rate;
-	fprintf(stderr, "Capture mode: %d Hz centred at %lld Hz in two stages: %d bins, coarse decimation %d with %d taps, "
-	        "fine decimation %d with %d taps, %d channels\n", pl.capture_rate, (long long)pl.centre_hz, pl.n_bins,
-	        pl.coarse_decim, pl.coarse_taps, pl.fine_decim, pl.fine_taps, G.freq_len);
-	return 0;
-}
-
-/* Capture mode with RXB200_CAPTURE_STAGES=raster: the plan of rxb200_fm_plan_capture_raster and one raster mixing handle,
- * whose channels share one polyphase branch sum per output and one DFT. */
-static int capture_setup_raster(const char *cap_env, const int64_t *t, int64_t *centre, int *rate)
-{
-	rxb200_fm_raster_plan pl;
-	int bins[MAX_FREQS];
-	if (rxb200_fm_plan_capture_raster(t, G.freq_len, G.der.capture_rate, atoll(cap_env), &pl, bins) != RXB200_OK) {
-		fprintf(stderr, "Capture mode: %s (RXB200_CAPTURE_RATE=%s).\n", rxb200_last_error(), cap_env);
-		return 1;
-	}
-	int32_t *taps = (int32_t *)malloc(sizeof(int32_t) * (size_t)pl.n_taps);
-	rxb200_ddc_lowpass(pl.decim, pl.n_taps, 15, taps);
-	const rxb200_ddc ddc = {pl.decim, pl.n_taps, taps, pl.shift};
-	const int rc = rxb200_fm_mix_create_raster(&G.der.params, pl.n_bins, bins, G.freq_len, &ddc, 0, &G.mix);
-	free(taps);
-	if (rc != RXB200_OK) { fprintf(stderr, "rxb200: %s\n", rxb200_last_error()); return 1; }
-	G.decim = pl.decim;
-	G.block16 = (size_t)pl.decim * 2 * CHUNK_COMPLEX;
-	G.stride = rxb200_fm_mix_max_output(G.mix, G.block16, G.block16);
-	*centre = pl.centre_hz;
-	*rate = pl.capture_rate;
-	fprintf(stderr, "Capture mode: %d Hz centred at %lld Hz as a raster: %d bins, decimation %d, %d taps, %d channels\n",
-	        pl.capture_rate, (long long)pl.centre_hz, pl.n_bins, pl.decim, pl.n_taps, G.freq_len);
-	return 0;
-}
-
 /* Capture mode's plan and handle: the channels' tuned frequencies through rxb200_fm_plan_capture, the capture mode
- * filter of rx_power, one decimating mixing handle.  Nonzero (reported on stderr) when the plan or the handle is refused. */
+ * filter of rx_power, one decimating mixing handle; with RXB200_CAPTURE_STAGES=2, the two-stage plan and a two-stage
+ * mixing handle, whose channel filters cost a coarse DFT shared by every channel plus a 129-tap fine filter per channel;
+ * with RXB200_CAPTURE_STAGES=raster, the raster plan and a raster mixing handle, whose channels share one polyphase
+ * branch sum per output and one DFT.  Nonzero (reported on stderr) when the plan or the handle is refused. */
 static int capture_setup(const char *cap_env, int64_t *centre, int *rate)
 {
 	int64_t t[MAX_FREQS];
-	int offs[MAX_FREQS];
+	int chans[MAX_FREQS];
 	for (int k = 0; k < G.freq_len; k++) { t[k] = capture_freq(k); }
 	const char *stages = getenv("RXB200_CAPTURE_STAGES");
-	if (stages && strcmp(stages, "2") == 0) { return capture_setup_two_stage(cap_env, t, offs, centre, rate); }
-	if (stages && strcmp(stages, "raster") == 0) { return capture_setup_raster(cap_env, t, centre, rate); }
-	rxb200_fm_capture_plan pl;
-	if (rxb200_fm_plan_capture(t, G.freq_len, G.der.capture_rate, atoll(cap_env), &pl, offs) != RXB200_OK) {
-		fprintf(stderr, "Capture mode: %s (RXB200_CAPTURE_RATE=%s).\n", rxb200_last_error(), cap_env);
-		return 1;
-	}
-	int32_t *taps = (int32_t *)malloc(sizeof(int32_t) * (size_t)pl.n_taps);
-	rxb200_ddc_lowpass(pl.decim, pl.n_taps, 15, taps);
-	const rxb200_ddc ddc = {pl.decim, pl.n_taps, taps, 15};
-	const int rc = rxb200_fm_mix_create_ddc(&G.der.params, pl.capture_rate, offs, G.freq_len, &ddc, 0, &G.mix);
-	free(taps);
+	const enum capture_kind kind = stages && strcmp(stages, "2") == 0        ? CAPTURE_TWO_STAGE
+	                             : stages && strcmp(stages, "raster") == 0 ? CAPTURE_RASTER
+	                                                                       : CAPTURE_SINGLE;
+	struct capture_plan pl;
+	if (capture_plan(kind, t, G.freq_len, G.der.capture_rate, cap_env, rxb200_fm_plan_capture, &pl, chans) != 0) { return 1; }
+	const int rc = kind == CAPTURE_TWO_STAGE ? rxb200_fm_mix_create_two_stage(&G.der.params, pl.capture_rate, pl.n_bins, chans,
+	                                                                          G.freq_len, &pl.ddc, &pl.fine, 0, &G.mix)
+	             : kind == CAPTURE_RASTER ? rxb200_fm_mix_create_raster(&G.der.params, pl.n_bins, chans, G.freq_len, &pl.ddc, 0,
+	                                                                    &G.mix)
+	                                      : rxb200_fm_mix_create_ddc(&G.der.params, pl.capture_rate, chans, G.freq_len,
+	                                                                 &pl.ddc, 0, &G.mix);
+	capture_plan_release(&pl);
 	if (rc != RXB200_OK) { fprintf(stderr, "rxb200: %s\n", rxb200_last_error()); return 1; }
 	G.decim = pl.decim;
 	G.block16 = (size_t)pl.decim * 2 * CHUNK_COMPLEX;
 	G.stride = rxb200_fm_mix_max_output(G.mix, G.block16, G.block16);
 	*centre = pl.centre_hz;
 	*rate = pl.capture_rate;
-	fprintf(stderr, "Capture mode: %d Hz centred at %lld Hz, decimation %d, %d taps, %d channels\n", pl.capture_rate,
-	        (long long)pl.centre_hz, pl.decim, pl.n_taps, G.freq_len);
+	fputs(pl.banner, stderr);
 	return 0;
 }
 

@@ -201,65 +201,24 @@ static int capture_mode(const struct opts *o, const char *cap_env)
 			if (o->freqs[i] == o->freqs[j]) { fprintf(stderr, "Capture mode (RXB200_CAPTURE_RATE): %u Hz is given twice.\n", o->freqs[i]); return 1; }
 		}
 	}
-	const long long cap = atoll(cap_env);
 	const char *stages = getenv("RXB200_CAPTURE_STAGES");
-	const int raster = stages && !strcmp(stages, "raster");
-	const int two = !raster && stages && atoi(stages) == 2;
+	const enum capture_kind kind = stages && !strcmp(stages, "raster") ? CAPTURE_RASTER
+	                             : stages && atoi(stages) == 2         ? CAPTURE_TWO_STAGE
+	                                                                   : CAPTURE_SINGLE;
 	int64_t tuned[MAX_FREQS];
-	int offs[MAX_FREQS], bins[MAX_FREQS];
+	int chans[MAX_FREQS];
 	for (int i = 0; i < K; i++) { tuned[i] = o->freqs[i]; }
-	int64_t fc = 0;
-	int R = 0, M = 0;
-	int32_t *taps1 = NULL, *taps2 = NULL;
-	rxb200_ddc d1, d2;
-	rxb200_fm_two_stage_plan tp;
-	rxb200_fm_raster_plan rp;
-	if (raster) {
-		if (rxb200_fm_plan_capture_raster(tuned, K, (int)o->rate, cap, &rp, bins) != RXB200_OK) {
-			fprintf(stderr, "Capture mode: %s (RXB200_CAPTURE_RATE=%s).\n", rxb200_last_error(), cap_env);
-			return 1;
-		}
-		fc = rp.centre_hz; R = rp.capture_rate; M = rp.decim;
-		taps1 = malloc((size_t)rp.n_taps * sizeof(int32_t));
-		rxb200_ddc_lowpass(rp.decim, rp.n_taps, 15, taps1);
-		d1 = (rxb200_ddc){rp.decim, rp.n_taps, taps1, rp.shift};
-		fprintf(stderr, "Capture mode: %d Hz centred at %lld Hz as a raster: %d bins, decimation %d, %d taps, %d channels\n",
-		        R, (long long)fc, rp.n_bins, M, rp.n_taps, K);
-	} else if (two) {
-		if (rxb200_fm_plan_capture_two_stage(tuned, K, (int)o->rate, cap, &tp, offs) != RXB200_OK) {
-			fprintf(stderr, "Capture mode: %s (RXB200_CAPTURE_RATE=%s).\n", rxb200_last_error(), cap_env);
-			return 1;
-		}
-		fc = tp.centre_hz; R = tp.capture_rate; M = tp.coarse_decim * tp.fine_decim;
-		taps1 = malloc((size_t)tp.coarse_taps * sizeof(int32_t));
-		taps2 = malloc((size_t)tp.fine_taps * sizeof(int32_t));
-		rxb200_ddc_lowpass(tp.coarse_decim, tp.coarse_taps, 15, taps1);
-		rxb200_ddc_lowpass(tp.fine_decim, tp.fine_taps, 15, taps2);
-		d1 = (rxb200_ddc){tp.coarse_decim, tp.coarse_taps, taps1, tp.coarse_shift};
-		d2 = (rxb200_ddc){tp.fine_decim, tp.fine_taps, taps2, tp.fine_shift};
-		fprintf(stderr, "Capture mode: %d Hz centred at %lld Hz in two stages: %d bins, coarse decimation %d with %d taps, "
-		        "fine decimation %d with %d taps, %d channels\n", R, (long long)fc, tp.n_bins, tp.coarse_decim,
-		        tp.coarse_taps, tp.fine_decim, tp.fine_taps, K);
-	} else {
-		rxb200_fm_capture_plan pl;
-		if (rxb200_sdr_plan_capture(tuned, K, (int)o->rate, cap, &pl, offs) != RXB200_OK) {
-			fprintf(stderr, "Capture mode: %s (RXB200_CAPTURE_RATE=%s).\n", rxb200_last_error(), cap_env);
-			return 1;
-		}
-		fc = pl.centre_hz; R = pl.capture_rate; M = pl.decim;
-		taps1 = malloc((size_t)pl.n_taps * sizeof(int32_t));
-		rxb200_ddc_lowpass(pl.decim, pl.n_taps, 15, taps1);
-		d1 = (rxb200_ddc){pl.decim, pl.n_taps, taps1, 15};
-		fprintf(stderr, "Capture mode: %d Hz centred at %lld Hz, decimation %d, %d taps, %d channels\n", R, (long long)fc,
-		        M, pl.n_taps, K);
-	}
+	struct capture_plan pl;
+	if (capture_plan(kind, tuned, K, (int)o->rate, cap_env, rxb200_sdr_plan_capture, &pl, chans) != 0) { return 1; }
+	fputs(pl.banner, stderr);
 	SoapySDRDevice *dev = NULL;
 	SoapySDRStream *stream = NULL;
-	if (open_device(o, SOAPY_SDR_CS16, R, (double)fc, &dev, &stream) != 0) { return 1; }
+	if (open_device(o, SOAPY_SDR_CS16, pl.capture_rate, (double)pl.centre_hz, &dev, &stream) != 0) { return 1; }
 	rxb200_sdr_mix *h = NULL;
-	const int rc0 = raster ? rxb200_sdr_mix_create_raster(rp.n_bins, bins, K, &d1, 0, &h)
-	              : two    ? rxb200_sdr_mix_create_two_stage(R, tp.n_bins, offs, K, &d1, &d2, 0, &h)
-	                       : rxb200_sdr_mix_create(R, offs, K, &d1, 0, &h);
+	const int rc0 = kind == CAPTURE_RASTER ? rxb200_sdr_mix_create_raster(pl.n_bins, chans, K, &pl.ddc, 0, &h)
+	              : kind == CAPTURE_TWO_STAGE
+	                  ? rxb200_sdr_mix_create_two_stage(pl.capture_rate, pl.n_bins, chans, K, &pl.ddc, &pl.fine, 0, &h)
+	                  : rxb200_sdr_mix_create(pl.capture_rate, chans, K, &pl.ddc, 0, &h);
 	if (rc0 != RXB200_OK) { fprintf(stderr, "rxb200_sdr_mix_create: %s\n", rxb200_last_error()); return 1; }
 	FILE *files[MAX_FREQS];
 	for (int k = 0; k < K; k++) {
@@ -267,8 +226,8 @@ static int capture_mode(const struct opts *o, const char *cap_env)
 		snprintf(name, sizeof name, "%s.%u", o->filename, o->freqs[k]);
 		if (!(files[k] = fopen(name, "wb"))) { fprintf(stderr, "Failed to open %s\n", name); return 1; }
 	}
-	const int kind = out_kind(o->out_fmt);
-	const size_t E = out_bytes(o->out_fmt), stride = o->block / (size_t)M + 2;
+	const int fmt = out_kind(o->out_fmt);
+	const size_t E = out_bytes(o->out_fmt), stride = o->block / (size_t)pl.decim + 2;
 	int16_t *buf = malloc((size_t)o->block * 4);
 	unsigned char *out = malloc((size_t)K * stride * E);
 	unsigned long long written = 0;
@@ -277,7 +236,7 @@ static int capture_mode(const struct opts *o, const char *cap_env)
 		const int r = read_some(dev, stream, buf, o->block);
 		if (r < 0) { break; }
 		size_t n = 0;
-		if (rxb200_sdr_mix_process(h, buf, 2 * (size_t)r, kind, out, (size_t)K * stride, stride, &n) != RXB200_OK) {
+		if (rxb200_sdr_mix_process(h, buf, 2 * (size_t)r, fmt, out, (size_t)K * stride, stride, &n) != RXB200_OK) {
 			fprintf(stderr, "rxb200_sdr_mix_process: %s\n", rxb200_last_error());
 			rc = 1;
 			break;
@@ -293,7 +252,8 @@ static int capture_mode(const struct opts *o, const char *cap_env)
 	rxb200_sdr_mix_destroy(h);
 	SoapySDRDevice_deactivateStream(dev, stream, 0, 0);
 	sdr_close(dev, stream);
-	free(buf); free(out); free(taps1); free(taps2);
+	free(buf); free(out);
+	capture_plan_release(&pl);
 	return rc;
 }
 

@@ -74,3 +74,61 @@ void sdr_set_gain(SoapySDRDevice *dev, size_t channel, const char *gain_str)
 		fprintf(stderr, "WARNING: Failed to set tuner gain: %s\n", SoapySDRDevice_lastError());
 	}
 }
+
+/* rxb200_ddc_lowpass(M, T) as a filter at shift S, its taps on the heap */
+static rxb200_ddc lowpass(int M, int T, int S)
+{
+	int32_t *taps = (int32_t *)malloc(sizeof(int32_t) * (size_t)T);
+	rxb200_ddc_lowpass(M, T, 15, taps);
+	return (rxb200_ddc){M, T, taps, S};
+}
+
+int capture_plan(enum capture_kind kind, const int64_t *tuned, int n, int chain_rate, const char *cap_env,
+                 capture_planner single, struct capture_plan *p, int *chans)
+{
+	const long long cap = atoll(cap_env);
+	int rc;
+	memset(p, 0, sizeof *p);
+	if (kind == CAPTURE_TWO_STAGE) {
+		rxb200_fm_two_stage_plan t;
+		rc = rxb200_fm_plan_capture_two_stage(tuned, n, chain_rate, cap, &t, chans);
+		if (rc == RXB200_OK) {
+			p->centre_hz = t.centre_hz; p->capture_rate = t.capture_rate; p->decim = t.coarse_decim * t.fine_decim;
+			p->n_bins = t.n_bins;
+			p->ddc = lowpass(t.coarse_decim, t.coarse_taps, t.coarse_shift);
+			p->fine = lowpass(t.fine_decim, t.fine_taps, t.fine_shift);
+			snprintf(p->banner, sizeof p->banner, "Capture mode: %d Hz centred at %lld Hz in two stages: %d bins, coarse "
+			         "decimation %d with %d taps, fine decimation %d with %d taps, %d channels\n", t.capture_rate,
+			         (long long)t.centre_hz, t.n_bins, t.coarse_decim, t.coarse_taps, t.fine_decim, t.fine_taps, n);
+		}
+	} else if (kind == CAPTURE_RASTER) {
+		rxb200_fm_raster_plan r;
+		rc = rxb200_fm_plan_capture_raster(tuned, n, chain_rate, cap, &r, chans);
+		if (rc == RXB200_OK) {
+			p->centre_hz = r.centre_hz; p->capture_rate = r.capture_rate; p->decim = r.decim; p->n_bins = r.n_bins;
+			p->ddc = lowpass(r.decim, r.n_taps, r.shift);
+			snprintf(p->banner, sizeof p->banner, "Capture mode: %d Hz centred at %lld Hz as a raster: %d bins, decimation "
+			         "%d, %d taps, %d channels\n", r.capture_rate, (long long)r.centre_hz, r.n_bins, r.decim, r.n_taps, n);
+		}
+	} else {
+		rxb200_fm_capture_plan s;
+		rc = single(tuned, n, chain_rate, cap, &s, chans);
+		if (rc == RXB200_OK) {
+			p->centre_hz = s.centre_hz; p->capture_rate = s.capture_rate; p->decim = s.decim;
+			p->ddc = lowpass(s.decim, s.n_taps, 15);
+			snprintf(p->banner, sizeof p->banner, "Capture mode: %d Hz centred at %lld Hz, decimation %d, %d taps, %d "
+			         "channels\n", s.capture_rate, (long long)s.centre_hz, s.decim, s.n_taps, n);
+		}
+	}
+	if (rc != RXB200_OK) {
+		fprintf(stderr, "Capture mode: %s (RXB200_CAPTURE_RATE=%s).\n", rxb200_last_error(), cap_env);
+		return 1;
+	}
+	return 0;
+}
+
+void capture_plan_release(struct capture_plan *p)
+{
+	free((void *)p->ddc.taps);
+	free((void *)p->fine.taps);
+}

@@ -1,12 +1,13 @@
-/* sdr_util.h — small host helpers shared by the drop-in shells rx_fm_b200 / rx_power_b200.
+/* sdr_util.h — small host helpers shared by the drop-in shells rx_fm_b200 / rx_power_b200 / rx_sdr_b200.
  * Own implementation of what rx_tools keeps in src/convenience/ (suffix parsing, device/stream
- * bring-up); behaviourally equivalent, not copied. */
+ * bring-up); behaviourally equivalent, not copied.  And the capture-mode plan of rx_fm_b200 and rx_sdr_b200. */
 #ifndef RXB_SDR_UTIL_H
 #define RXB_SDR_UTIL_H
 #include <stddef.h>
 #include <stdint.h>
 #include <SoapySDR/Device.h>
 #include <SoapySDR/Formats.h>
+#include "rxb200.h"
 
 double parse_scaled(const char *s);    /* 100M, 24k, 1.2G   (convenience.c:65-90)  */
 double parse_seconds(const char *s);   /* 10s, 5m, 1h       (convenience.c:92-117) */
@@ -17,4 +18,25 @@ int sdr_open(const char *query, size_t channel, SoapySDRDevice **dev, SoapySDRSt
 void sdr_close(SoapySDRDevice *dev, SoapySDRStream *stream);
 /* gain: NULL = automatic, "30" overall, or "LNA=20,VGA=10" per element */
 void sdr_set_gain(SoapySDRDevice *dev, size_t channel, const char *gain_str);
+
+/* Capture mode (RXB200_CAPTURE_RATE): every channel from one capture, through a front stage of one of three kinds. */
+enum capture_kind { CAPTURE_SINGLE, CAPTURE_RASTER, CAPTURE_TWO_STAGE };
+typedef int (*capture_planner)(const int64_t *, int, int, long long, rxb200_fm_capture_plan *, int *);
+struct capture_plan {
+	int64_t centre_hz;     /* fc */
+	int capture_rate;      /* R */
+	int decim;             /* the total decimation: M, or M1 M2 for two stages */
+	int n_bins;            /* K (raster, two stages) */
+	rxb200_ddc ddc;        /* the filter, the coarse one for two stages */
+	rxb200_ddc fine;       /* two stages: the fine filter */
+	char banner[256];      /* the "Capture mode: ..." line the shell prints */
+};
+/* The plan of kind for the n tuned frequencies at chain rate chain_rate under the cap cap_env (RXB200_CAPTURE_RATE's
+ * value): single, the plan of `single` (rxb200_fm_plan_capture or rxb200_sdr_plan_capture); raster,
+ * rxb200_fm_plan_capture_raster's; two stages, rxb200_fm_plan_capture_two_stage's.  chans receives the n offsets (the
+ * bins for a raster).  The filters' taps are rxb200_ddc_lowpass's, freed by capture_plan_release.  A refused plan is
+ * reported on stderr and returns nonzero, with nothing to release. */
+int capture_plan(enum capture_kind kind, const int64_t *tuned, int n, int chain_rate, const char *cap_env,
+                 capture_planner single, struct capture_plan *p, int *chans);
+void capture_plan_release(struct capture_plan *p);
 #endif

@@ -1,13 +1,13 @@
-// ddc.cuh — the digital down-converter both mixing handles run: fm_ddc_kernel (fm_mix.cu: rx_fm channels, each mixed
+// ddc.cuh — the digital down-converter the mixing handles run: fm_ddc_kernel (fm_mix.cu: rx_fm channels, each mixed
 // with its integer table) and power_ddc_kernel (power_mix.cu: rx_power hops, each mixed with a phase-accumulator NCO).
 // Both kernels are ddc_body with their mixer policy: it stages the capture samples its outputs' windows cover, mixes
 // them per channel into shared memory with mix_one, and runs the T-tap dot product at the emission points only; the
 // policy supplies the mixer index and the output address, the two things they differ in.  fine_ddc_kernel
 // (fm_two_stage.cu) is ddc_body too, with an NCO mixer and the staging hook ddc_row giving each grid row its own
 // stream.  sdr_nco_kernel (sdr_mix.cu) is ddc_body with the NCO mixer and the output hook ddc_store writing an rx_sdr
-// format (SdrOut), and fine_ddc_kernel has such instances too.  The host side they share is
-// here too (the launch, the filter state a handle carries between calls) and in ddc.cu (the argument check, the
-// stateless entries' upload).
+// format (SdrOut), and fine_ddc_kernel has such instances too.  The host side they share is here too (the launch, the
+// filter state a handle carries between calls, the NCO bank) and in ddc.cu (the argument check, the stateless entries'
+// upload).  The front stage a handle runs on one capture, of whichever kind, is capture_front.cuh's.
 #pragma once
 #include <algorithm>
 #include <vector>
@@ -205,6 +205,14 @@ struct NcoMix {
 		}
 	};
 	using Row = RowOf<DdcArgs<NcoMix>>;
+};
+
+// NcoMix's device data on the current device: the shared table (rxb200_nco_table) and each channel's word
+struct NcoBank {
+	int2 *nco = nullptr;
+	uint32_t *w = nullptr;
+	int upload(const std::vector<uint32_t> &words);   // the caller releases the bank when it fails
+	void release() { cudaFree(w); cudaFree(nco); }
 };
 
 // w = floor((f 2^32 + floor(R/2)) / R) mod 2^32 for each of the n offsets, exactly, with the refusals of R <= 0 and

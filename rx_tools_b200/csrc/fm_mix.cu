@@ -2,21 +2,19 @@
 // fm_mix_kernel mixes the capture to baseband once per channel with that channel's integer table, reading the capture
 // once and writing one CS16 stream per channel; a plain rxb200_fm handle with one channel per stream then runs the
 // chain on them through its device entry points.  A decimating handle (rxb200_fm_mix_create_ddc) runs fm_ddc_kernel
-// instead (ddc.cuh's down-converter with the channels' tables), which mixes, filters and decimates, and carries its
-// filter state (DdcFilter) between calls.  A raster handle (rxb200_fm_mix_create_raster) is a decimating handle whose
-// front stage is fm_raster.cu's polyphase channelizer instead, and a two-stage handle
-// (rxb200_fm_mix_create_two_stage) one whose front stage is fm_two_stage.cu's coarse and fine stages.  Every process
-// entry point of every kind goes through
-// mix_call, whose refusals and member shape come from fm_mix_check_host_call (which the group uses too).  The chain
-// itself is not touched here.
+// instead (ddc.cuh's down-converter with the channels' tables), which mixes, filters and decimates.  A raster handle
+// (rxb200_fm_mix_create_raster) is a decimating handle whose front stage is fm_raster.cu's polyphase channelizer
+// instead, and a two-stage handle (rxb200_fm_mix_create_two_stage) one whose front stage is fm_two_stage.cu's coarse and
+// fine stages.  The front stage of every kind, with the capture count and the filter state it carries between calls,
+// is a CaptureFront (capture_front.cuh); the two mixers it calls back are here.  Every process entry point of every
+// kind goes through mix_call, whose refusals and member shape come from fm_mix_check_host_call (which the group uses
+// too).  The chain itself is not touched here.
 #include <algorithm>
 #include <cstring>
 #include <new>
 #include <vector>
 #include "common.cuh"
-#include "ddc.cuh"
-#include "raster.cuh"
-#include "two_stage.cuh"
+#include "capture_front.cuh"
 
 namespace rxb {
 
@@ -199,40 +197,14 @@ struct rxb200_fm_mix {
 	std::vector<MixChan> chan;                   // host copy of d_chan
 	int2 *d_tab = nullptr;                       // every channel's table, concatenated
 	MixChan *d_chan = nullptr;
-	unsigned long long pos = 0;                  // complex samples since create or reset: channel k's phase is pos mod L_k
 	int16_t *d_cap = nullptr; size_t cap_cap = 0;   // host calls: the capture (int16 elements)
 	int16_t *d_mix = nullptr; size_t mix_cap = 0;   // the mixed streams, [n_channels][n_int16]
 	int16_t *d_out = nullptr; size_t out_cap = 0;   // host calls: the PCM rows, total + 8 apart
-	cudaEvent_t ev0 = nullptr, ev1 = nullptr;    // around the last fm_mix_kernel (fm_ddc_kernel, the raster kernels)
-	// a decimating handle (rxb200_fm_mix_create_ddc): fm_ddc_kernel writes the decimated streams to d_mix ([n_channels]
-	// [n_dec_int16]) and the member runs on those
-	bool ddc = false;
-	DdcFilter f;                                 // its filter state (T = 1 for a plain handle)
-	// a raster handle (rxb200_fm_mix_create_raster, r.K > 0): a decimating handle with no mixer tables, whose front
-	// stage is raster_front with the twiddle matrix d_wt and the branch sums' scratch d_v
-	RasterPlan r;
-	double *d_wt = nullptr;
-	double *d_v = nullptr; size_t v_cap = 0;     // doubles
-	// a two-stage handle (rxb200_fm_mix_create_two_stage, ts != NULL): a decimating handle whose DdcFilter f is the
-	// coarse stage's and whose front stage is ts->front, with the coarse rows' scratch d_y (and d_v)
-	TwoStage *ts = nullptr;
-	uint32_t *d_y = nullptr; size_t y_cap = 0;   // words
+	// the front stage: a plain handle's has no filter, and channel k's mixer phase is fr.pos mod L_k; a decimating
+	// handle's (any with a filter) writes the decimated streams to d_mix ([n_channels][n_dec_int16]) and the member runs
+	// on those
+	CaptureFront fr;
 };
-
-namespace {
-
-// the decimation of a decimating handle: M, or M1 M2 for a two-stage handle
-size_t decim(const rxb200_fm_mix *m) { return (size_t)m->f.M * (size_t)(m->ts ? m->ts->M2 : 1); }
-
-// int16 a decimating handle hands the chain from a call of n_int16 capture int16 after pos capture samples: the
-// outputs whose emission point m*M + M - 1 falls in the call
-size_t ddc_len(unsigned long long pos, size_t n_int16, int decim)
-{
-	const unsigned long long M = (unsigned long long)decim;
-	return 2 * (size_t)((pos + n_int16 / 2) / M - pos / M);
-}
-
-}  // namespace
 
 // Every refusal of a mixing handle's call, in the order the call reports them, without enqueuing anything; *total
 // receives the PCM count per channel, *n16 and *chunk16 the member's call (n16 == 0: no member call).  A plain handle's
@@ -244,20 +216,20 @@ int rxb::fm_mix_check_host_call(rxb200_fm_mix *m, const int16_t *cs16, size_t n_
                                 size_t *n16, size_t *chunk16)
 {
 	if (!m) { set_error("null argument"); return RXB200_EINVAL; }
-	if (!m->ddc) {
+	if (!m->fr.filtered()) {
 		*n16 = n_int16;
 		*chunk16 = chunk_int16;
 		return rxb::fm_check_host_call(m->h, cs16, n_int16, chunk_int16, pcm, pcm_stride, chunk_result_len, n_pcm, read,
 		                               total);
 	}
 	if (!cs16 || !pcm) { set_error("null argument"); return RXB200_EINVAL; }
-	const size_t M = decim(m);
+	const size_t M = m->fr.decim();
 	if (n_int16 % 2 != 0) { set_error("n_int16=%zu must be even", n_int16); return RXB200_EUNSUPPORTED; }
 	if (!read && (chunk_int16 == 0 || chunk_int16 % (2 * M) != 0)) {
 		set_error("chunk_int16=%zu must be a multiple of 2 * decim = %zu", chunk_int16, 2 * M);
 		return RXB200_EUNSUPPORTED;
 	}
-	*n16 = ddc_len(m->pos, n_int16, (int)M);
+	*n16 = 2 * m->fr.out_len(n_int16 / 2);
 	*chunk16 = read ? *n16 : chunk_int16 / M;
 	if (read && *n16 == 0 && n_int16 > 0) {
 		return rxb::fm_check_host_call(m->h, cs16, 0, 262144, pcm, pcm_stride, nullptr, n_pcm, false, total);
@@ -273,57 +245,12 @@ int rxb::fm_mix_check_host_call(rxb200_fm_mix *m, const int16_t *cs16, size_t n_
 
 namespace {
 
-// a decimating handle's front stage: fm_ddc_kernel from the call's capture at src to n16 int16 per channel in d_mix
-int ddc_front(rxb200_fm_mix *m, const int16_t *src, size_t n16, cudaStream_t st)
-{
-	const DdcFilter &f = m->f;
-	DdcArgs<TabMix> a{};
-	a.src = reinterpret_cast<const uint32_t *>(src);
-	a.hist = f.hist[f.cur];
-	a.n_out = (long long)(n16 / 2);
-	a.r0 = (long long)(f.M - 1) - (long long)(m->pos % (unsigned long long)f.M);
-	a.pos = m->pos;
-	a.dst = reinterpret_cast<uint32_t *>(m->d_mix);
-	a.taps = f.taps;
-	a.n_ch = m->n_channels; a.M = f.M; a.T = f.T; a.S = f.S;
-	a.mix = TabMix{m->d_tab, m->d_chan, (long long)(n16 / 2)};
-	return ddc_launch(a, f.wide ? fm_ddc_kernel<long long> : fm_ddc_kernel<int>, st);
-}
-
-// a raster handle's front stage: raster_front from the call's capture at src to n16 int16 per channel in d_mix
-int raster_call_front(rxb200_fm_mix *m, const int16_t *src, size_t n16, cudaStream_t st)
-{
-	const DdcFilter &f = m->f;
-	const long long n_out = (long long)(n16 / 2);
-	RXB_CUDA(reserve(m->d_v, m->v_cap, (size_t)std::min(n_out, m->r.group) * (size_t)m->r.Kp));
-	return raster_front(m->r, m->d_wt, m->d_v, reinterpret_cast<const uint32_t *>(src), f.hist[f.cur], f.taps, f.M, f.T,
-	                    f.S, (long long)(f.M - 1) - (long long)(m->pos % (unsigned long long)f.M),
-	                    (unsigned)(m->pos % (unsigned long long)m->r.K), n_out, reinterpret_cast<uint32_t *>(m->d_mix),
-	                    n_out, st);
-}
-
-// a two-stage handle's front stage: the coarse outputs whose emission points fall in the call's c capture samples, and
-// the fine outputs among them to n16 int16 per channel in d_mix.  It runs whenever the call has coarse outputs, since
-// they advance the bins' histories even when no fine output falls in the call.
-int two_stage_call_front(rxb200_fm_mix *m, const int16_t *src, size_t c, size_t n16, cudaStream_t st)
-{
-	TwoStage &t = *m->ts;
-	const unsigned long long M1 = (unsigned long long)m->f.M, ma = m->pos / M1;
-	const long long n1 = (long long)((m->pos + c) / M1 - ma);
-	if (n1 == 0) { return RXB200_OK; }
-	const long long F = std::min(t.G, n1);
-	RXB_CUDA(reserve(m->d_v, m->v_cap, (size_t)F * (size_t)t.r.Kp));
-	RXB_CUDA(reserve(m->d_y, m->y_cap, t.y_words(F)));
-	return t.front(m->f, reinterpret_cast<const uint32_t *>(src), (long long)(ma * M1 + M1 - 1 - m->pos),
-	               (unsigned)(m->pos % (unsigned long long)t.r.K), n1, ma, (int)(ma % (unsigned long long)t.M2), m->d_v,
-	               m->d_y, reinterpret_cast<uint32_t *>(m->d_mix), (long long)(n16 / 2), st);
-}
-
 // One call of any process entry point.  device: cs16 and pcm are device pointers (the member's device entry point
 // writes pcm), else host pointers staged through the handle's buffers.  read: one read (chunk_int16 == n_int16).  The
-// front stage (fm_mix_kernel, fm_ddc_kernel for a decimating handle, the raster kernels for a raster handle, both stages
-// for a two-stage handle) writes the member's input to d_mix; when it has no output (n16 == 0) the member does not run
-// (nor the front stage, but a two-stage handle's coarse stage), but the phases and the histories still advance.
+// front stage (fm_mix_kernel for a plain handle, fm_ddc_kernel for a decimating one, the raster kernels for a raster
+// handle, both stages for a two-stage handle) writes the member's input to d_mix; when it has no output (n16 == 0) the
+// member does not run, but the phases and the histories still advance.  The front commits once, after the member's
+// call, so a failed call leaves the old histories live.
 int mix_call(rxb200_fm_mix *m, const int16_t *cs16, size_t n_int16, size_t chunk_int16, int16_t *pcm, size_t pcm_stride,
              size_t *n_pcm, int *chunk_result_len, bool read, bool device, int sync)
 {
@@ -344,17 +271,14 @@ int mix_call(rxb200_fm_mix *m, const int16_t *cs16, size_t n_int16, size_t chunk
 		RXB_CUDA(cudaMemcpyAsync(m->d_cap, cs16, n_int16 * sizeof(int16_t), cudaMemcpyHostToDevice, st));
 		src = m->d_cap;
 	}
-	RXB_CUDA(cudaEventRecord(m->ev0, st));
-	if (m->ts) {
-		rc = two_stage_call_front(m, src, c, n16, st);
-	} else if (n16) {
-		rc = m->r.K ? raster_call_front(m, src, n16, st)
-		   : m->ddc ? ddc_front(m, src, n16, st)
-		            : mix_launch(src, (long long)c, m->d_mix, (long long)n16, m->d_tab, m->d_chan, m->chan, m->pos, st);
-	}
-	if (rc != RXB200_OK) { return rc; }
-	RXB_CUDA(cudaEventRecord(m->ev1, st));
-	rc = m->f.carry(reinterpret_cast<const uint32_t *>(src), c, st);
+	rc = m->fr.call<TabMix>(src, c, m->d_mix, (long long)(n16 / 2), RXB200_SDR_OUT_CS16, m->n_channels, st,
+	                        [&](DdcArgs<TabMix> &a) {
+		if (!m->fr.filtered()) {
+			return mix_launch(src, (long long)c, m->d_mix, (long long)n16, m->d_tab, m->d_chan, m->chan, m->fr.pos, st);
+		}
+		a.mix = TabMix{m->d_tab, m->d_chan, (long long)(n16 / 2)};
+		return ddc_launch(a, m->fr.f.wide ? fm_ddc_kernel<long long> : fm_ddc_kernel<int>, st);
+	});
 	if (rc != RXB200_OK) { return rc; }
 	rxb::fm_unchain(m->h);                       // the member's input was just written on its stream
 	if (n16) {
@@ -374,9 +298,7 @@ int mix_call(rxb200_fm_mix *m, const int16_t *cs16, size_t n_int16, size_t chunk
 	} else if (sync && n16 == 0) {
 		RXB_CUDA(cudaStreamSynchronize(st));    // with output, the member's call has synchronised
 	}
-	m->f.commit();
-	if (m->ts) { m->ts->commit(); }
-	m->pos += c;
+	m->fr.commit(c);
 	if (n_pcm) { *n_pcm = total; }
 	return RXB200_OK;
 }
@@ -426,29 +348,24 @@ extern "C" void rxb200_fm_mix_destroy(rxb200_fm_mix *m)
 	rxb200_fm_destroy(m->h);   // synchronises the stream the mixer runs on
 	cudaSetDevice(m->device);
 	cudaFree(m->d_tab); cudaFree(m->d_chan); cudaFree(m->d_cap); cudaFree(m->d_mix); cudaFree(m->d_out);
-	cudaFree(m->d_wt); cudaFree(m->d_v); cudaFree(m->d_y);
-	m->f.release();
-	if (m->ts) { m->ts->release(0); delete m->ts; }
-	if (m->ev0) { cudaEventDestroy(m->ev0); }
-	if (m->ev1) { cudaEventDestroy(m->ev1); }
+	m->fr.release(0);
 	delete m;
 }
 
 namespace {
 
-// rxb200_fm_mix_create, rxb200_fm_mix_create_ddc (ddc != NULL, already checked), rxb200_fm_mix_create_raster
-// (raster != NULL, planned; no offsets and no tables) and rxb200_fm_mix_create_two_stage (ddc the coarse filter, ts
-// planned, fine its fine filter; no tables)
-int mix_create(const rxb200_fm_params *params, int capture_rate, const int *offsets_hz, int n_channels,
-               const rxb200_ddc *ddc, bool wide, const RasterPlan *raster, int device, rxb200_fm_mix **out,
-               const TwoStage *ts = nullptr, const rxb200_ddc *fine = nullptr)
+// rxb200_fm_mix_create (fr not planned: no filter), rxb200_fm_mix_create_ddc (ddc its filter, already checked),
+// rxb200_fm_mix_create_raster and rxb200_fm_mix_create_two_stage (ddc the coarse filter, fine the fine one), with fr
+// planned; a single stage has offsets and tables, a raster or two stages none
+int mix_create(const rxb200_fm_params *params, int capture_rate, const int *offsets_hz, int n_channels, CaptureFront &fr,
+               const rxb200_ddc *ddc, const rxb200_ddc *fine, int device, rxb200_fm_mix **out)
 {
-	if (ts) { raster = &ts->r; }
+	const bool tables = fr.kind == CaptureFront::SINGLE;
 	*out = nullptr;
 	// every table first: a refused offset fails before any device work
 	std::vector<int32_t> all, t;
 	std::vector<MixChan> chan;
-	for (int k = 0; !raster && k < n_channels; k++) {
+	for (int k = 0; tables && k < n_channels; k++) {
 		size_t L = 0;
 		const int rc = mix_table(capture_rate, offsets_hz[k], t, &L);
 		if (rc != RXB200_OK) { return rc; }
@@ -461,34 +378,18 @@ int mix_create(const rxb200_fm_params *params, int capture_rate, const int *offs
 	m->device = device;
 	m->n_channels = n_channels;
 	m->chan = chan;
-	const int rc = rxb200_fm_create(params, device, n_channels, &m->h);
+	m->fr = std::move(fr);
+	int rc = rxb200_fm_create(params, device, n_channels, &m->h);
 	if (rc != RXB200_OK) { delete m; return rc; }
 	RXB_CUDA_OR(cudaSetDevice(device), rxb200_fm_mix_destroy(m));
-	if (!raster) {
+	if (tables) {
 		RXB_CUDA_OR(cudaMalloc(&m->d_tab, all.size() * sizeof(int32_t)), rxb200_fm_mix_destroy(m));
 		RXB_CUDA_OR(cudaMalloc(&m->d_chan, chan.size() * sizeof(MixChan)), rxb200_fm_mix_destroy(m));
 		RXB_CUDA_OR(cudaMemcpy(m->d_tab, all.data(), all.size() * sizeof(int32_t), cudaMemcpyHostToDevice), rxb200_fm_mix_destroy(m));
 		RXB_CUDA_OR(cudaMemcpy(m->d_chan, chan.data(), chan.size() * sizeof(MixChan), cudaMemcpyHostToDevice), rxb200_fm_mix_destroy(m));
 	}
-	RXB_CUDA_OR(cudaEventCreate(&m->ev0), rxb200_fm_mix_destroy(m));
-	RXB_CUDA_OR(cudaEventCreate(&m->ev1), rxb200_fm_mix_destroy(m));
-	if (ddc) {
-		m->ddc = true;
-		const int rc = m->f.create(ddc, wide);
-		if (rc != RXB200_OK) { rxb200_fm_mix_destroy(m); return rc; }
-	}
-	if (ts) {
-		m->ts = new (std::nothrow) TwoStage(*ts);
-		if (!m->ts) { rxb200_fm_mix_destroy(m); return RXB200_ENOMEM; }
-		const int rc = m->ts->upload(fine, (cudaStream_t)rxb200_fm_stream(m->h));
-		if (rc != RXB200_OK) { rxb200_fm_mix_destroy(m); return rc; }
-	} else if (raster) {
-		m->r = *raster;
-		m->r.wt.clear();
-		RXB_CUDA_OR(cudaMalloc(&m->d_wt, raster->w_bytes()), rxb200_fm_mix_destroy(m));
-		RXB_CUDA_OR(cudaMemcpy(m->d_wt, raster->wt.data(), raster->w_bytes(), cudaMemcpyHostToDevice),
-		            rxb200_fm_mix_destroy(m));
-	}
+	rc = m->fr.create(ddc, fine, (cudaStream_t)rxb200_fm_stream(m->h));
+	if (rc != RXB200_OK) { rxb200_fm_mix_destroy(m); return rc; }
 	*out = m;
 	return RXB200_OK;
 }
@@ -499,7 +400,8 @@ extern "C" int rxb200_fm_mix_create(const rxb200_fm_params *params, int capture_
                                     int n_channels, int device, rxb200_fm_mix **out)
 {
 	if (!params || !offsets_hz || !out || n_channels < 1) { set_error("bad mix arguments (n_channels >= 1)"); return RXB200_EINVAL; }
-	return mix_create(params, capture_rate, offsets_hz, n_channels, nullptr, false, nullptr, device, out);
+	CaptureFront fr;
+	return mix_create(params, capture_rate, offsets_hz, n_channels, fr, nullptr, nullptr, device, out);
 }
 
 extern "C" int rxb200_fm_mix_create_ddc(const rxb200_fm_params *params, int capture_rate, const int *offsets_hz,
@@ -507,10 +409,10 @@ extern "C" int rxb200_fm_mix_create_ddc(const rxb200_fm_params *params, int capt
 {
 	if (!params || !offsets_hz || !out || n_channels < 1) { set_error("bad mix arguments (n_channels >= 1)"); return RXB200_EINVAL; }
 	*out = nullptr;
-	bool wide = false;
-	const int rc = rxb::ddc_check(ddc, &wide);
+	CaptureFront fr;
+	const int rc = fr.plan_single(ddc);
 	if (rc != RXB200_OK) { return rc; }
-	return mix_create(params, capture_rate, offsets_hz, n_channels, ddc, wide, nullptr, device, out);
+	return mix_create(params, capture_rate, offsets_hz, n_channels, fr, ddc, nullptr, device, out);
 }
 
 extern "C" int rxb200_fm_mix_create_raster(const rxb200_fm_params *params, int n_bins, const int *bins, int n_channels,
@@ -518,15 +420,10 @@ extern "C" int rxb200_fm_mix_create_raster(const rxb200_fm_params *params, int n
 {
 	if (!params || !out) { set_error("null argument"); return RXB200_EINVAL; }
 	*out = nullptr;
-	bool wide = false;
-	int rc = rxb::ddc_check(ddc, &wide);
+	CaptureFront fr;
+	const int rc = fr.plan_raster(n_bins, bins, n_channels, ddc);
 	if (rc != RXB200_OK) { return rc; }
-	rc = raster_check(n_bins, bins, n_channels, ddc);
-	if (rc != RXB200_OK) { return rc; }
-	RasterPlan p;
-	rc = p.plan(n_bins, bins, n_channels);
-	if (rc != RXB200_OK) { return rc; }
-	return mix_create(params, 0, nullptr, n_channels, ddc, wide, &p, device, out);
+	return mix_create(params, 0, nullptr, n_channels, fr, ddc, nullptr, device, out);
 }
 
 extern "C" int rxb200_fm_mix_create_two_stage(const rxb200_fm_params *params, int capture_rate, int n_bins,
@@ -535,29 +432,25 @@ extern "C" int rxb200_fm_mix_create_two_stage(const rxb200_fm_params *params, in
 {
 	if (!params || !out) { set_error("null argument"); return RXB200_EINVAL; }
 	*out = nullptr;
-	int rc = rxb::ddc_check(fine, nullptr);
+	CaptureFront fr;
+	const int rc = fr.plan_two_stage(capture_rate, n_bins, offsets_hz, n_channels, coarse, fine);
 	if (rc != RXB200_OK) { return rc; }
-	rc = rxb::ddc_check(coarse, nullptr);
-	if (rc != RXB200_OK) { return rc; }
-	TwoStage t;
-	rc = t.plan(capture_rate, n_bins, offsets_hz, n_channels, coarse, fine);
-	if (rc != RXB200_OK) { return rc; }
-	return mix_create(params, 0, nullptr, n_channels, coarse, false, nullptr, device, out, &t, fine);
+	return mix_create(params, 0, nullptr, n_channels, fr, coarse, fine, device, out);
 }
 
 extern "C" int rxb200_fm_mix_decimated_len(const rxb200_fm_mix *m, size_t n_int16, size_t *n_dec_int16)
 {
 	if (!m || !n_dec_int16) { set_error("null argument"); return RXB200_EINVAL; }
-	*n_dec_int16 = m->ddc ? ddc_len(m->pos, n_int16, (int)decim(m)) : n_int16;
+	*n_dec_int16 = m->fr.filtered() ? 2 * m->fr.out_len(n_int16 / 2) : n_int16;
 	return RXB200_OK;
 }
 
 extern "C" size_t rxb200_fm_mix_max_output(const rxb200_fm_mix *m, size_t n_int16, size_t chunk_int16)
 {
 	if (!m || chunk_int16 == 0) { return 0; }
-	if (!m->ddc) { return rxb200_fm_max_output(m->h, n_int16, chunk_int16); }
+	if (!m->fr.filtered()) { return rxb200_fm_max_output(m->h, n_int16, chunk_int16); }
 	// floor((p + c) / M) - floor(p / M) <= ceil(c / M) at any phase p
-	const size_t M = decim(m), n16 = 2 * ((n_int16 / 2 + M - 1) / M);
+	const size_t M = m->fr.decim(), n16 = 2 * ((n_int16 / 2 + M - 1) / M);
 	return rxb200_fm_max_output(m->h, n16, chunk_int16 / M ? chunk_int16 / M : 2);
 }
 
@@ -595,16 +488,10 @@ extern "C" int rxb200_ddc_device(int capture_rate, int offset_hz, long long phas
 extern "C" int rxb200_fm_mix_reset(rxb200_fm_mix *m)
 {
 	if (!m) { return RXB200_EINVAL; }
-	int rc = rxb200_fm_reset(m->h);
+	const int rc = rxb200_fm_reset(m->h);
 	if (rc != RXB200_OK) { return rc; }
-	if (m->ddc) {
-		RXB_CUDA(cudaSetDevice(m->device));
-		rc = m->f.reset((cudaStream_t)rxb200_fm_stream(m->h));   // behind any call still running on the member's stream
-		if (rc == RXB200_OK && m->ts) { rc = m->ts->reset((cudaStream_t)rxb200_fm_stream(m->h)); }
-		if (rc != RXB200_OK) { return rc; }
-	}
-	m->pos = 0;
-	return RXB200_OK;
+	RXB_CUDA(cudaSetDevice(m->device));
+	return m->fr.reset((cudaStream_t)rxb200_fm_stream(m->h));   // behind any call still running on the member's stream
 }
 
 extern "C" rxb200_fm *rxb200_fm_mix_member(rxb200_fm_mix *m) { return m ? m->h : nullptr; }
@@ -647,7 +534,5 @@ extern "C" int rxb200_fm_mix_kernel_ms(rxb200_fm_mix *m, float *ms)
 {
 	if (!m || !ms) { return RXB200_EINVAL; }
 	RXB_CUDA(cudaSetDevice(m->device));
-	RXB_CUDA(cudaEventSynchronize(m->ev1));
-	RXB_CUDA(cudaEventElapsedTime(ms, m->ev0, m->ev1));
-	return RXB200_OK;
+	return m->fr.kernel_ms(ms);
 }

@@ -12,13 +12,11 @@
 
 namespace rxb {
 
-#define TS_NCO_ENTRIES 65536         // rxb200_nco_table: index j = ((theta + 2^15) mod 2^32) >> 16
-
 // ddc_body's mixer policy for the fine stage: channel k (in bin order) of the grid row mixes coarse sample m of its bin
 // by NCO entry ((m w_k + 2^15) mod 2^32) >> 16, the phase taken per CTA as (uint32)g0 * w_k and stepped by off * w_k in
 // uint32 arithmetic (as NcoMix), and writes its call output u to word u of its own row of dst.
 struct BinMix {
-	const int2 *nco;                 // TS_NCO_ENTRIES (c, s) pairs
+	const int2 *nco;                 // NCO_ENTRIES (c, s) pairs
 	const uint32_t *w;               // each channel's fine word, channels in bin order
 	const int *row;                  // each channel's row of dst, channels in bin order
 	const int4 *rows;                // each grid row: (its bin's slot, its first channel, its channel count, 0)
@@ -125,7 +123,7 @@ int TwoStage::plan(int capture_rate, int n_bins, const int *offsets_hz, int n_ch
 	const long long per = (long long)r.Kp * (long long)sizeof(double) + (long long)r.C * (long long)sizeof(uint32_t);
 	G = std::max<long long>(64, ((long long)RXB200_RASTER_SCRATCH_BYTES - fixed) / per / 64 * 64);
 	o_nco = align16(r.w_bytes());
-	o_rows = o_nco + align16((size_t)TS_NCO_ENTRIES * sizeof(int2));
+	o_rows = o_nco + align16((size_t)NCO_ENTRIES * sizeof(int2));
 	o_w = o_rows + align16((size_t)n_rows * sizeof(int4));
 	o_row = o_w + align16((size_t)n_ch * sizeof(uint32_t));
 	blk.assign(o_row + align16((size_t)n_ch * sizeof(int)), 0);

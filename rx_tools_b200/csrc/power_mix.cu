@@ -60,8 +60,7 @@ struct rxb200_power_mix {
 	int device = 0;
 	int n_hops = 0, buf_len = 0;
 	DdcFilter f;                                 // M, T, S and the filter history
-	uint32_t *d_w = nullptr;                     // each hop's frequency word
-	int2 *d_nco = nullptr;                       // the shared NCO table
+	NcoBank nco;                                 // the shared NCO table and each hop's frequency word
 	unsigned long long pos = 0;                  // capture samples since create or reset (whole passes)
 	int16_t *d_cap = nullptr; size_t cap_cap = 0;     // host calls: the capture (int16 elements)
 	int16_t *d_bufs = nullptr; size_t bufs_cap = 0;   // the hop buffers of one group of passes, [P][he - hb][buf_len]
@@ -75,7 +74,7 @@ extern "C" void rxb200_power_mix_destroy(rxb200_power_mix *m)
 	rxb200_power_destroy(m->h);                  // synchronises the stream the DDC runs on
 	cudaSetDevice(m->device);
 	m->f.release();
-	cudaFree(m->d_w); cudaFree(m->d_nco);
+	m->nco.release();
 	cudaFree(m->d_cap); cudaFree(m->d_bufs);
 	for (cudaEvent_t e : m->ev) { cudaEventDestroy(e); }
 	delete m;
@@ -99,14 +98,9 @@ extern "C" int rxb200_power_mix_create(const rxb200_power_params *params, const 
 	if (rc != RXB200_OK) { delete m; return rc; }
 	m->device = device;
 	m->n_hops = params->n_hops; m->buf_len = params->buf_len;
-	std::vector<int32_t> nco(2 * NCO_ENTRIES);
-	rxb200_nco_table(nco.data());
 	RXB_CUDA_OR(cudaSetDevice(device), rxb200_power_mix_destroy(m));
-	RXB_CUDA_OR(cudaMalloc(&m->d_w, w.size() * sizeof(uint32_t)), rxb200_power_mix_destroy(m));
-	RXB_CUDA_OR(cudaMalloc(&m->d_nco, nco.size() * sizeof(int32_t)), rxb200_power_mix_destroy(m));
-	RXB_CUDA_OR(cudaMemcpy(m->d_w, w.data(), w.size() * sizeof(uint32_t), cudaMemcpyHostToDevice), rxb200_power_mix_destroy(m));
-	RXB_CUDA_OR(cudaMemcpy(m->d_nco, nco.data(), nco.size() * sizeof(int32_t), cudaMemcpyHostToDevice), rxb200_power_mix_destroy(m));
-	rc = m->f.create(ddc, wide);
+	rc = m->nco.upload(w);
+	if (rc == RXB200_OK) { rc = m->f.create(ddc, wide); }
 	if (rc != RXB200_OK) { rxb200_power_mix_destroy(m); return rc; }
 	*out = m;
 	return RXB200_OK;
@@ -189,7 +183,7 @@ int power_mix_call(rxb200_power_mix *m, int hb, int he, const int16_t *cs16, siz
 		a.dst = reinterpret_cast<uint32_t *>(m->d_bufs);
 		a.taps = f.taps;
 		a.n_ch = he - hb; a.M = f.M; a.T = f.T; a.S = f.S;
-		a.mix = NcoMix{m->d_nco, m->d_w + hb, (int)(L / 2)};
+		a.mix = NcoMix{m->nco.nco, m->nco.w + hb, (int)(L / 2)};
 		RXB_CUDA(cudaEventRecord(m->ev[(size_t)2 * m->n_ev], st));
 		int rc = ddc_launch(a, f.wide ? power_ddc_kernel<long long> : power_ddc_kernel<int>, st);
 		if (rc != RXB200_OK) { return rc; }

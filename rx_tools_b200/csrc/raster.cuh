@@ -1,6 +1,6 @@
-// raster.cuh — the raster down-converter of rx_fm raster mixing handles (include/rxb200.h, "raster mixing handles"):
-// the host side fm_mix.cu needs from fm_raster.cu.  A raster handle is a decimating handle (DdcFilter, mix_call) whose
-// front stage runs raster_front instead of fm_ddc_kernel.
+// raster.cuh — the raster down-converter of raster mixing handles (include/rxb200.h, "raster mixing handles"): the host
+// side the capture front (capture_front.cuh) needs from fm_raster.cu.  A raster handle, rx_fm's or rx_sdr's, is one whose
+// CaptureFront runs raster_front instead of a single-stage down-converter.
 #pragma once
 #include <vector>
 #include "common.cuh"

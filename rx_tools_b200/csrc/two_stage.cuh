@@ -1,7 +1,7 @@
-// two_stage.cuh — the two-stage down-converter of rx_fm two-stage mixing handles (include/rxb200.h, "two-stage mixing
-// handles"): the host side fm_mix.cu needs from fm_two_stage.cu.  A two-stage handle is a decimating handle (DdcFilter,
-// mix_call) whose DdcFilter is the coarse stage's (M1, T1, h1, S1 and the raw capture history) and whose front stage
-// runs TwoStage::front; so is an rx_sdr two-stage handle (sdr_mix.cu), which has it write a recorded format.
+// two_stage.cuh — the two-stage down-converter of two-stage mixing handles (include/rxb200.h, "two-stage mixing
+// handles"): the host side the capture front (capture_front.cuh) needs from fm_two_stage.cu.  A two-stage handle, rx_fm's
+// or rx_sdr's, is one whose CaptureFront's DdcFilter is the coarse stage's (M1, T1, h1, S1 and the raw capture history)
+// and which runs TwoStage::front; rx_sdr's has it write a recorded format.
 #pragma once
 #include <vector>
 #include "ddc.cuh"
