@@ -900,6 +900,95 @@ void *rxb200_sdr_mix_stream(rxb200_sdr_mix *m);
 int rxb200_sdr_plan_capture(const int64_t *tuned_hz /* n_channels */, int n_channels, int sample_rate,
                             long long max_capture_rate, rxb200_fm_capture_plan *out, int *offsets_hz /* n_channels */);
 
+/* ======================================================================== capture from a device at its own rate
+ * (DESIGN.md section 4.7)  Every capture plan above asks the device for exactly R = M c.  Many receivers run only at a
+ * few fixed rates, or round what they are asked for; a device that delivers R' != R moves every channel by
+ * o (1 - R'/R) and scales the chain rate by R'/R.  A rational resampler takes the device's stream at the rate it really
+ * runs at, R_dev, to the plan's R exactly, so every front stage above runs unchanged on its output.
+ * The rule.  A resampler has an up factor L and a down factor N (R / R_dev = L / N, 1 <= L, N), J taps per phase
+ * (1..1024, J L <= 2^22), a prototype h of J L int32 taps and a rounding shift S (0..62).  Let x[n] be the device's
+ * CS16 samples, n counted from create or reset across calls, x[n] = 0 for n < 0.  For output m >= 0:
+ *     t = m N,  q = floor(t / L),  p = t mod L;
+ *     A = sum_{j<J} h[p + j L] x[q - j]   (exact, I and Q separately);
+ *     y = S ? (A + 2^(S-1)) >> S : A   (arithmetic), saturated to [-32768, 32767].
+ * Output m is emitted by device sample q.  A call over device samples [n0, n0 + c) returns the
+ * ceil((n0 + c) L / N) - ceil(n0 L / N) outputs whose q falls in it (computed in 128-bit integers: no count wraps), so
+ * the bytes never depend on how the stream is cut into calls.
+ * Anchors.  L = N = 1, J = 1, h = {2^15}, S = 15 is the identity.  L = 1, N = M: output m is output m of
+ * rxb200_ddc_device at offset 0 with the same M, taps and shift over the stream with M - 1 zeros prepended (the DDC
+ * emits at m M + M - 1, this rule at m M).
+ * resample_kernel accumulates in int32 when max_p sum_j |h[p + j L]| * 32768 + 2^(S-1) < 2^31, else in int64.  A CTA
+ * owns consecutive outputs, stages the device samples they read once in shared memory, and holds the taps phase-major
+ * ([L][J]) in shared memory when they fit (J L <= 12288), else reads them through the caches. */
+typedef struct rxb200_resampler {
+	int up;                /* L */
+	int down;              /* N */
+	int taps_per_phase;    /* J */
+	const int32_t *taps;   /* h[0..J L), the prototype at rate L R_dev: phase p is h[p], h[p + L], ..., h[p + (J-1) L] */
+	int shift;             /* S */
+} rxb200_resampler;
+/* The prototype filter: a Blackman-windowed sinc of J L taps at the prototype rate L R_dev, cutoff 1 / (2 max(L, N))
+ * cycles per prototype sample (min(R, R_dev) / 2 Hz), scaled so that each phase sums to about 2^15 and rounded; then
+ * each phase's sum is corrected to exactly 2^15 on that phase's largest-magnitude tap (the first of equals), so at
+ * S = 15 a constant input comes out exactly constant once q >= J - 1.  Window w_i = 0.42 - 0.5 cos a + 0.08 cos 2a,
+ * a = 2 pi (i + 1) / (J L + 1).  RXB200_EINVAL for NULL taps, L or N < 1, J outside [1, 1024] or J L > 2^22.  Pure host
+ * arithmetic. */
+int rxb200_resample_lowpass(int up, int down, int taps_per_phase, int32_t *taps /* J L */);
+/* The resampler from a device rate R_dev to a plan's rate R for channels spanning `span` Hz around the centre (2A + c,
+ * A the largest |offset|, c the chain rate):
+ *   G = ceil(R_dev / 32), the guard band the transition needs; D = min(R, R_dev) - span, refused when D < G
+ *     (RXB200_EINVAL; the message names the span, R_dev and the largest span that fits, min(R, R_dev) - G);
+ *   L = R / gcd(R, R_dev), N = R_dev / gcd(R, R_dev);  J = 8 ceil(ceil(6 R_dev / D) / 8), so 8 <= J <= 192;
+ *   J L > 2^22 is refused (RXB200_EUNSUPPORTED, the message names L/N);  S = 15, taps rxb200_resample_lowpass(L, N, J).
+ * out->taps is set to NULL: the caller designs the J L taps.  L = N = 1 means no resampler is needed.  Also
+ * RXB200_EINVAL for a NULL out, a rate outside [1, 2^31 - 1] or a negative span.  Pure host arithmetic.
+ * Worked examples.  span = 2A + c, and R = M c with M = ceil((2A + c + G) / c): the decimation a capture plan needs so
+ * that the guard band fits (the capture planners above choose M = ceil((2A + c) / c), which leaves no room for it on
+ * these sets; DESIGN.md section 4.7):
+ *   set                                          R_dev        M, R             L/N          J     J L
+ *   7 NOAA channels, rx_fm NBFM (c = 1.008 M)    2.4 M        2, 2.016 M       21/25        24    504
+ *   the same                                     2.5 M        2, 2.016 M       504/625      24    12 096
+ *   100 FM stations, wbfm (c = 1.02 M)           30.72 M      22, 22.44 M      187/256      136   25 432
+ *   the same                                     20 M         refused: span 21.02 MHz > 20 M - 625 k
+ *   4 rx_sdr channels 100-100.95 MHz, -s 250k    2.4 M        6, 1.5 M         5/8          48    240
+ *   100 FM stations, rx_sdr raster, -s 250k      30.72 M      85, 21.25 M      2125/3072    192   408 000 */
+int rxb200_plan_resample(long long device_rate, long long rate, long long span, rxb200_resampler *out);
+/* A resampler handle carries the device-sample count and the last J - 1 raw samples between calls; a call's next
+ * history and count become live only when it succeeds, and a refused call changes nothing.  Refusals of create, all
+ * before any device is touched: RXB200_EINVAL for a NULL resampler, taps or out, L or N < 1, J outside [1, 1024],
+ * J L > 2^22, S outside [0, 62] and max_p sum |h_p| * 32768 + 2^(S-1) >= 2^63 (which the other bounds already keep
+ * below 2^62).  The taps are copied. */
+#define RXB200_RESAMPLE_SCRATCH_BYTES (64u << 20)
+typedef struct rxb200_resample rxb200_resample;
+int rxb200_resample_create(const rxb200_resampler *rs, int device, rxb200_resample **out);
+void rxb200_resample_destroy(rxb200_resample *r);
+/* the count and the history back to the state right after create */
+int rxb200_resample_reset(rxb200_resample *r);
+/* *n_out: the outputs the next call of n_int16 device int16 returns */
+int rxb200_resample_out_len(const rxb200_resample *r, size_t n_int16, size_t *n_out);
+/* HOST stream and output, synchronous: n_int16 int16 (even) in, *n_out (may be NULL) complex outputs to out, which
+ * holds out_cap complex outputs.  RXB200_EINVAL for a NULL handle, stream or output or an odd n_int16;
+ * RXB200_ECAPACITY when out_cap is below the call's outputs.  The call stages the stream through the device in groups
+ * of at most RXB200_RESAMPLE_SCRATCH_BYTES, each a device call that commits its count and history when it succeeds;
+ * the bytes are those of one group. */
+int rxb200_resample_process(rxb200_resample *r, const int16_t *cs16, size_t n_int16, int16_t *out, size_t out_cap,
+                            size_t *n_out);
+/* The same on DEVICE pointers (both 4-byte aligned, else RXB200_EINVAL), asynchronous on the handle's stream unless
+ * sync != 0. */
+int rxb200_resample_process_device(rxb200_resample *r, const int16_t *d_cs16, size_t n_int16, int16_t *d_out,
+                                   size_t out_cap, size_t *n_out, int sync);
+/* the handle's cudaStream_t */
+void *rxb200_resample_stream(rxb200_resample *r);
+/* Device time (CUDA events on the handle's stream) of the resample_kernel launches of the last call (of a host call's
+ * last group), in milliseconds; synchronises. */
+int rxb200_resample_kernel_ms(rxb200_resample *r, float *ms);
+/* The resampler alone on DEVICE pointers, stateless, on `stream`: d_src[i] is device sample n0 + i, the samples before
+ * d_src are zero, and the ceil((n0 + n_complex) L / N) - ceil(n0 L / N) outputs whose q falls in
+ * [n0, n0 + n_complex) go to d_dst.  Both pointers 4-byte aligned.  The refusals of rxb200_resample_create.
+ * Asynchronous. */
+int rxb200_resample_device(const rxb200_resampler *rs, unsigned long long n0, const int16_t *d_src, size_t n_complex,
+                           int16_t *d_dst, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -73,6 +73,11 @@ class FmRasterPlanC(C.Structure):
                 ("n_taps", C.c_int), ("shift", C.c_int)]
 
 
+class ResamplerC(C.Structure):
+    _fields_ = [("up", C.c_int), ("down", C.c_int), ("taps_per_phase", C.c_int), ("taps", C.POINTER(C.c_int32)),
+                ("shift", C.c_int)]
+
+
 class PowerPlanC(C.Structure):
     _fields_ = [("params", PowerParamsC), ("rate", C.c_int), ("crop", C.c_double),
                 ("first_freq", C.c_int64), ("freq_step", C.c_int64), ("bin_size_hz", C.c_double)]
@@ -122,6 +127,9 @@ SYMBOLS = [
     "rxb200_sdr_mix_destroy", "rxb200_sdr_mix_reset",
     "rxb200_sdr_mix_decimated_len", "rxb200_sdr_mix_process", "rxb200_sdr_mix_process_device",
     "rxb200_sdr_mix_kernel_ms", "rxb200_sdr_mix_stream", "rxb200_sdr_plan_capture",
+    "rxb200_resample_lowpass", "rxb200_plan_resample", "rxb200_resample_create", "rxb200_resample_destroy",
+    "rxb200_resample_reset", "rxb200_resample_out_len", "rxb200_resample_process", "rxb200_resample_process_device",
+    "rxb200_resample_stream", "rxb200_resample_kernel_ms", "rxb200_resample_device",
 ]
 
 _lib = None
@@ -295,6 +303,20 @@ def lib() -> C.CDLL:
     L.rxb200_sdr_mix_stream.argtypes = [C.c_void_p]
     L.rxb200_sdr_mix_stream.restype = C.c_void_p
     L.rxb200_sdr_plan_capture.argtypes = [pi64, C.c_int, C.c_int, C.c_longlong, C.POINTER(FmCapturePlanC), pint]
+    pr = C.POINTER(ResamplerC)
+    L.rxb200_resample_lowpass.argtypes = [C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int32)]
+    L.rxb200_plan_resample.argtypes = [C.c_longlong, C.c_longlong, C.c_longlong, pr]
+    L.rxb200_resample_create.argtypes = [pr, C.c_int, C.POINTER(C.c_void_p)]
+    L.rxb200_resample_destroy.argtypes = [C.c_void_p]
+    L.rxb200_resample_destroy.restype = None
+    L.rxb200_resample_reset.argtypes = [C.c_void_p]
+    L.rxb200_resample_out_len.argtypes = [C.c_void_p, sz, C.POINTER(sz)]
+    L.rxb200_resample_process.argtypes = [C.c_void_p, C.c_void_p, sz, C.c_void_p, sz, C.POINTER(sz)]
+    L.rxb200_resample_process_device.argtypes = [C.c_void_p, C.c_void_p, sz, C.c_void_p, sz, C.POINTER(sz), C.c_int]
+    L.rxb200_resample_stream.argtypes = [C.c_void_p]
+    L.rxb200_resample_stream.restype = C.c_void_p
+    L.rxb200_resample_kernel_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float)]
+    L.rxb200_resample_device.argtypes = [pr, C.c_ulonglong, C.c_void_p, sz, C.c_void_p, C.c_void_p]
     _lib = L
     return L
 

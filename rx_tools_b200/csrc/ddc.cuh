@@ -269,6 +269,11 @@ struct DdcFilter {
 		std::reverse(rev.begin(), rev.end());
 		RXB_CUDA(cudaMalloc(&taps, (size_t)T * sizeof(int32_t)));
 		RXB_CUDA(cudaMemcpy(taps, rev.data(), (size_t)T * sizeof(int32_t), cudaMemcpyHostToDevice));
+		return alloc_hist();
+	}
+	// the two zeroed histories of T - 1 samples (create; the resampler, whose taps are its own, sets T and calls it)
+	int alloc_hist()
+	{
 		for (int i = 0; i < 2; i++) {
 			RXB_CUDA(cudaMalloc(&hist[i], hist_bytes()));
 			RXB_CUDA(cudaMemset(hist[i], 0, hist_bytes()));

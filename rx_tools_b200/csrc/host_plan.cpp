@@ -7,6 +7,7 @@
 #include <math.h>
 #include <stdarg.h>
 #include <stdio.h>
+#include <stdlib.h>
 #include <string.h>
 #include <algorithm>
 #include <vector>
@@ -284,6 +285,70 @@ extern "C" int rxb200_ddc_lowpass(int decim, int n_taps, int shift, int32_t *tap
 		q += taps[j];
 	}
 	taps[c] += (int32_t)((1ll << shift) - q);
+	return RXB200_OK;
+}
+
+// The resampler's prototype filter (include/rxb200.h, "capture from a device at its own rate"): a Blackman-windowed
+// sinc over J L taps with its cutoff at 1/(2 max(L, N)) cycles per prototype sample, scaled so that each of the L
+// phases sums to about 2^15, rounded, then each phase's sum made exactly 2^15 on its largest-magnitude tap.
+extern "C" int rxb200_resample_lowpass(int up, int down, int taps_per_phase, int32_t *taps)
+{
+	if (!taps) { set_error("null argument"); return RXB200_EINVAL; }
+	if (up < 1 || down < 1 || taps_per_phase < 1 || taps_per_phase > 1024 || (long long)taps_per_phase * up > (1ll << 22)) {
+		set_error("resampler lowpass up %d, down %d, taps_per_phase %d: need up, down >= 1, 1 <= taps_per_phase <= 1024 "
+		          "and taps_per_phase * up <= 2^22", up, down, taps_per_phase);
+		return RXB200_EINVAL;
+	}
+	const long long L = up, J = taps_per_phase, n = J * L;
+	const double c = (double)(n - 1) / 2.0, fc = 1.0 / (2.0 * (double)std::max(up, down));
+	std::vector<double> g((size_t)n);
+	double sum = 0.0;
+	for (long long i = 0; i < n; i++) {
+		const double x = 2.0 * fc * ((double)i - c);
+		const double s = x == 0.0 ? 1.0 : sin(M_PI * x) / (M_PI * x);
+		const double a = 2.0 * M_PI * (double)(i + 1) / (double)(n + 1);
+		g[i] = s * (0.42 - 0.5 * cos(a) + 0.08 * cos(2.0 * a));
+		sum += g[i];
+	}
+	const double scale = 32768.0 * (double)L / sum;
+	for (long long i = 0; i < n; i++) { taps[i] = (int32_t)llround(g[i] * scale); }
+	for (long long p = 0; p < L; p++) {
+		long long s = 0, k = p;
+		for (long long i = p; i < n; i += L) {
+			s += taps[i];
+			if (std::llabs(taps[i]) > std::llabs(taps[k])) { k = i; }
+		}
+		taps[k] += (int32_t)(32768 - s);
+	}
+	return RXB200_OK;
+}
+
+extern "C" int rxb200_plan_resample(long long device_rate, long long rate, long long span, rxb200_resampler *out)
+{
+	if (!out) { set_error("null argument"); return RXB200_EINVAL; }
+	if (device_rate < 1 || device_rate > 2147483647ll || rate < 1 || rate > 2147483647ll || span < 0) {
+		set_error("resampler plan: device rate %lld Hz, rate %lld Hz, span %lld Hz (need rates in [1, 2^31 - 1] and a "
+		          "span >= 0)", device_rate, rate, span);
+		return RXB200_EINVAL;
+	}
+	const long long G = (device_rate + 31) / 32, D = std::min(rate, device_rate) - span;
+	if (D < G) {
+		set_error("the channels span %lld Hz, too wide for a device at %lld Hz resampled to %lld Hz: the largest span "
+		          "that fits is %lld Hz", span, device_rate, rate, std::min(rate, device_rate) - G);
+		return RXB200_EINVAL;
+	}
+	long long a = rate, b = device_rate;
+	while (b) { const long long t = a % b; a = b; b = t; }
+	const long long L = rate / a, N = device_rate / a, J = 8 * (((6 * device_rate + D - 1) / D + 7) / 8);
+	if (J * L > (1ll << 22)) {
+		set_error("resampling by %lld/%lld needs %lld taps (%lld per phase), above 2^22", L, N, J * L, J);
+		return RXB200_EUNSUPPORTED;
+	}
+	out->up = (int)L;
+	out->down = (int)N;
+	out->taps_per_phase = (int)J;
+	out->taps = NULL;
+	out->shift = 15;
 	return RXB200_OK;
 }
 
