@@ -988,6 +988,69 @@ int rxb200_resample_kernel_ms(rxb200_resample *r, float *ms);
  * Asynchronous. */
 int rxb200_resample_device(const rxb200_resampler *rs, unsigned long long n0, const int16_t *d_src, size_t n_complex,
                            int16_t *d_dst, void *stream);
+/* The fewest device samples c that a call starting at device sample n0 needs for n_out outputs: the least c with
+ * ceil((n0 + c) L / N) - ceil(n0 L / N) >= n_out (0 for n_out = 0), computed in 128-bit integers.  Output m is emitted
+ * by device sample floor(m N / L), so c = floor((m0 + n_out - 1) N / L) + 1 - n0 with m0 = ceil(n0 L / N).  When L <= N
+ * each device sample emits at most one output, so the call's count is exactly n_out: a reader that needs one block of
+ * n_out capture samples reads exactly c device samples.  RXB200_EINVAL for NULL n_in, L or N < 1, or c >= 2^64.  Pure
+ * host arithmetic. */
+int rxb200_resample_in_len(int up, int down, unsigned long long n0, size_t n_out, size_t *n_in);
+
+/* ---- capture handles at a device rate (DESIGN.md section 4.7)
+ * rxb200_fm_mix_set_device_rate, rxb200_sdr_mix_set_device_rate and rxb200_power_mix_set_device_rate attach a resampler
+ * (the rule above) to a capture handle of any kind, ahead of its front stage.  After the call every host and device
+ * entry of the handle takes device-rate CS16: the handle's capture is the resampler's output over the device stream
+ * since create or reset, and a call over device samples [n0, n0 + c) hands the front the ceil((n0 + c) L / N) -
+ * ceil(n0 L / N) capture samples those device samples emit.  So a handle's bytes are exactly those of an
+ * rxb200_resample handle followed by the same handle without a resampler on its output, however the device stream is
+ * cut into calls.  What follows the device-sample count:
+ *   rxb200_fm_mix: a call's shape is that of its capture samples (a read is one read of them; a chunked call's
+ *     chunk_int16 counts capture int16 as before); _decimated_len and _max_output take device int16;
+ *   rxb200_sdr_mix: _decimated_len takes device int16; a host call stages device samples in groups whose device-rate
+ *     upload, resampled capture and output rows together fit RXB200_SDR_MIX_SCRATCH_BYTES;
+ *   rxb200_power_mix: a call must resample to whole passes (else RXB200_EUNSUPPORTED, and nothing changes); bursts,
+ *     capture-rate captures of their own, are refused (RXB200_EUNSUPPORTED);
+ *   every handle: reset clears the resampler's count and history and keeps it attached; a refused call changes nothing;
+ *     _kernel_ms includes resample_kernel; an odd n_int16 gets the code the handle gives it without a resampler
+ *     (RXB200_EUNSUPPORTED for rx_fm and rx_power, RXB200_EINVAL for rx_sdr).
+ * The resampler runs on the handle's stream into a capture-rate scratch buffer in device memory (4 bytes per capture
+ * sample of a call, or of a host call's group).  rx_fm and rx_sdr commit its history and count with the front's, per
+ * call or per host group.  rx_power resamples a whole call ahead of its pass groups and commits the resampler once
+ * that is enqueued, before the groups commit theirs; a CUDA failure in a later group (RXB200_ECUDA) therefore leaves
+ * the resampler's count ahead of the passes taken, and rxb200_power_mix_reset starts over, as after any failed call.
+ * Refusals: RXB200_EINVAL for a NULL handle, or a handle that has taken any sample since create or reset or already has
+ * a resampler; then those of rxb200_resample_create.  All come before any device work.  The taps are copied. */
+int rxb200_fm_mix_set_device_rate(rxb200_fm_mix *m, const rxb200_resampler *rs);
+int rxb200_sdr_mix_set_device_rate(rxb200_sdr_mix *m, const rxb200_resampler *rs);
+int rxb200_power_mix_set_device_rate(rxb200_power_mix *m, const rxb200_resampler *rs);
+
+/* ---- capture plans at a device rate
+ * The capture planners above with one more argument, the device rate R_dev (Hz) the shell's resampler starts from.
+ * Each follows its own planner's rule, with one change: G = ceil(R_dev / 32), the guard band rxb200_plan_resample needs,
+ * and the decimation floor leaves it, M = ceil((2 A + c + G) / c) instead of ceil((2 A + c) / c).  The centre, the
+ * offsets, T, the raster's K and bins and the two-stage split M' = 4 ceil(M / 4) follow from that M as before, so
+ * rxb200_plan_resample(R_dev, R, 2 A + c) fits whenever R <= R_dev.
+ * Refusals, pure host arithmetic: RXB200_EINVAL for R_dev outside [1, 2^31 - 1], first; then every refusal of the
+ * planner in its order (the arguments, the cap, 2^31 - 1 and the decimation bound, the two-stage M' < 8, the raster's
+ * K > 4096, the mixer table's); and RXB200_EUNSUPPORTED for R > R_dev, right after the cap's refusal (the message names
+ * R and R_dev): the shells only resample down.
+ * Worked examples (each also in rxb200_plan_resample's table):
+ *   set                                          planner    R_dev     M    R           resampler L/N
+ *   7 NOAA channels, rx_fm NBFM (c = 1.008 M)    fm         2.4 M     2    2 016 000   21/25
+ *   4 rx_sdr channels 100-100.95 MHz, -s 250k    sdr        2.4 M     6    1 500 000   5/8
+ *   100 FM stations, wbfm (c = 1.02 M)           fm         30.72 M   22   22 440 000  187/256 */
+int rxb200_fm_plan_capture_at(const int64_t *tuned_hz /* n_channels */, int n_channels, int chain_rate,
+                              long long max_capture_rate, long long device_rate, rxb200_fm_capture_plan *out,
+                              int *offsets_hz /* n_channels */);
+int rxb200_fm_plan_capture_two_stage_at(const int64_t *tuned_hz /* n_channels */, int n_channels, int chain_rate,
+                                        long long max_capture_rate, long long device_rate,
+                                        rxb200_fm_two_stage_plan *out, int *offsets_hz /* n_channels */);
+int rxb200_fm_plan_capture_raster_at(const int64_t *tuned_hz /* n_channels */, int n_channels, int chain_rate,
+                                     long long max_capture_rate, long long device_rate, rxb200_fm_raster_plan *out,
+                                     int *bins /* n_channels */);
+int rxb200_sdr_plan_capture_at(const int64_t *tuned_hz /* n_channels */, int n_channels, int sample_rate,
+                               long long max_capture_rate, long long device_rate, rxb200_fm_capture_plan *out,
+                               int *offsets_hz /* n_channels */);
 
 #ifdef __cplusplus
 }

@@ -130,6 +130,9 @@ SYMBOLS = [
     "rxb200_resample_lowpass", "rxb200_plan_resample", "rxb200_resample_create", "rxb200_resample_destroy",
     "rxb200_resample_reset", "rxb200_resample_out_len", "rxb200_resample_process", "rxb200_resample_process_device",
     "rxb200_resample_stream", "rxb200_resample_kernel_ms", "rxb200_resample_device",
+    "rxb200_resample_in_len", "rxb200_fm_plan_capture_at", "rxb200_fm_plan_capture_two_stage_at",
+    "rxb200_fm_plan_capture_raster_at", "rxb200_sdr_plan_capture_at",
+    "rxb200_fm_mix_set_device_rate", "rxb200_sdr_mix_set_device_rate", "rxb200_power_mix_set_device_rate",
 ]
 
 _lib = None
@@ -317,6 +320,18 @@ def lib() -> C.CDLL:
     L.rxb200_resample_stream.restype = C.c_void_p
     L.rxb200_resample_kernel_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float)]
     L.rxb200_resample_device.argtypes = [pr, C.c_ulonglong, C.c_void_p, sz, C.c_void_p, C.c_void_p]
+    L.rxb200_resample_in_len.argtypes = [C.c_int, C.c_int, C.c_ulonglong, sz, C.POINTER(sz)]
+    L.rxb200_fm_plan_capture_at.argtypes = [pi64, C.c_int, C.c_int, C.c_longlong, C.c_longlong,
+                                            C.POINTER(FmCapturePlanC), pint]
+    L.rxb200_fm_plan_capture_two_stage_at.argtypes = [pi64, C.c_int, C.c_int, C.c_longlong, C.c_longlong,
+                                                      C.POINTER(FmTwoStagePlanC), pint]
+    L.rxb200_fm_plan_capture_raster_at.argtypes = [pi64, C.c_int, C.c_int, C.c_longlong, C.c_longlong,
+                                                   C.POINTER(FmRasterPlanC), pint]
+    L.rxb200_sdr_plan_capture_at.argtypes = [pi64, C.c_int, C.c_int, C.c_longlong, C.c_longlong,
+                                             C.POINTER(FmCapturePlanC), pint]
+    L.rxb200_fm_mix_set_device_rate.argtypes = [C.c_void_p, pr]
+    L.rxb200_sdr_mix_set_device_rate.argtypes = [C.c_void_p, pr]
+    L.rxb200_power_mix_set_device_rate.argtypes = [C.c_void_p, pr]
     _lib = L
     return L
 

@@ -4,11 +4,14 @@
 // handle's own mixer (the handle launches it); a raster is fm_raster.cu's polyphase channelizer (raster_front); two
 // stages are fm_two_stage.cu's coarse raster then per-channel NCO stage (TwoStage::front).  The front owns the capture
 // count, and so the rule that makes a recording's bytes independent of how the capture is cut into calls: each call's
-// kernels start at the count's phases, and commit advances the count and the histories.  Its host code is in ddc.cu.
+// kernels start at the count's phases, and commit advances the count and the histories.  A front with a resampler
+// attached (resample_stage.cuh) takes device-rate samples: each call resamples them to the capture first, and every
+// count below that takes a call's length counts device samples.  Its host code is in ddc.cu.
 #pragma once
 #include <algorithm>
 #include "ddc.cuh"
 #include "raster.cuh"
+#include "resample_stage.cuh"
 #include "two_stage.cuh"
 
 namespace rxb {
@@ -24,6 +27,7 @@ struct CaptureFront {
 	TwoStage ts;                                 // two stages: the plan, the fine stage and the bins' histories
 	uint32_t *d_y = nullptr; size_t y_cap = 0;   // two stages: the coarse rows (words)
 	cudaEvent_t ev0 = nullptr, ev1 = nullptr;    // around the front's kernels of the last call
+	ResampleStage rs;                            // from the device rate, once attached
 
 	// The refusals of each kind, in the order the handles report them, then its host plan; no device work.  A single
 	// stage is its filter's check alone.
@@ -39,29 +43,37 @@ struct CaptureFront {
 
 	// M, or M1 M2 for two stages
 	size_t decim() const { return (size_t)f.M * (size_t)(kind == TWO_STAGE ? ts.M2 : 1); }
-	// the outputs per channel of a call of c capture samples: those whose emission points m M + M - 1 fall in it
-	size_t out_len(size_t c) const
+	// the outputs per channel of c capture samples at the current count: those whose emission points m M + M - 1 fall
+	// in them
+	size_t dec_len(size_t c) const
 	{
 		const unsigned long long M = decim();
 		return (size_t)((pos + c) / M - pos / M);
 	}
+	// the outputs per channel of a call of c device samples (capture samples without a resampler)
+	size_t out_len(size_t c) const { return dec_len(rs.out_len(c)); }
+	// Attaches the resampler, which only a front that has taken no sample since create or reset accepts (and only
+	// once); its refusals precede any device work
+	int set_device_rate(const rxb200_resampler *r);
 
-	// One call's front stage on the current device, ordered on st: the c capture samples at src (a device pointer) to
-	// the out_len(c) outputs per channel of the n_ch channels at dst, channel k's output u at element k * stride + u in
-	// rx_sdr format fmt (RXB200_SDR_OUT_CS16: the int16 pair word); then the carry of the raw history.  ev0 and ev1
-	// bracket the kernels.  Two stages run whenever the call has coarse outputs, since those advance the bins'
+	// One call's front stage on the current device, ordered on st: the c device samples at src (a device pointer),
+	// resampled to the capture when a resampler is attached, to the out_len(c) outputs per channel of the n_ch channels
+	// at dst, channel k's output u at element k * stride + u in rx_sdr format fmt (RXB200_SDR_OUT_CS16: the int16
+	// pair word); then the carry of the raw history.  ev0 and ev1 bracket the kernels.  Two stages run whenever the call has coarse outputs, since those advance the bins'
 	// histories even when no fine output falls in the call; the other kinds run when the call has outputs.  single
-	// launches a single stage from the DdcArgs<Mix> it is given, every field but mix filled.  Nothing becomes live
-	// before commit(c).
+	// launches a single stage from the DdcArgs<Mix> it is given, every field but mix filled (src, n_out and pos
+	// describe the capture).  ev0 and ev1 also bracket the resampler.  Nothing becomes live before commit(c).
 	template <typename Mix, typename Single>
-	int call(const int16_t *src, size_t c, void *dst, long long stride, int fmt, int n_ch, cudaStream_t st,
+	int call(const int16_t *src, size_t c_dev, void *dst, long long stride, int fmt, int n_ch, cudaStream_t st,
 	         Single single)
 	{
-		const uint32_t *x = reinterpret_cast<const uint32_t *>(src);
-		const long long n = (long long)out_len(c);
+		const size_t c = rs.out_len(c_dev);
+		const long long n = (long long)dec_len(c);
 		const long long r0 = (long long)(f.M - 1) - (long long)(pos % (unsigned long long)f.M);
 		RXB_CUDA(cudaEventRecord(ev0, st));
-		int rc = RXB200_OK;
+		const uint32_t *x = nullptr;
+		int rc = rs.run(reinterpret_cast<const uint32_t *>(src), c_dev, st, &x);
+		if (rc != RXB200_OK) { return rc; }
 		if (kind == TWO_STAGE) {
 			const unsigned long long M1 = (unsigned long long)f.M, ma = pos / M1;
 			const long long n1 = (long long)((pos + c) / M1 - ma);
@@ -93,14 +105,15 @@ struct CaptureFront {
 		RXB_CUDA(cudaEventRecord(ev1, st));
 		return f.carry(x, c, st);
 	}
-	// the histories a call of c capture samples wrote become live, and the count advances past it
+	// the histories a call of c device samples wrote become live, and the counts advance past it
 	void commit(size_t c)
 	{
+		pos += rs.out_len(c);
+		rs.commit(c);
 		f.commit();
 		ts.commit();
-		pos += c;
 	}
-	// every history zeroed behind any call still running on st, and the count cleared
+	// every history zeroed behind any call still running on st, and the counts cleared (a resampler stays attached)
 	int reset(cudaStream_t st);
 	// frees the device state, once no kernel of the front's is in flight: the caller has synchronised st, the stream
 	// they ran on (or destroyed it, st = 0)

@@ -102,6 +102,15 @@ int CaptureFront::create(const rxb200_ddc *ddc, const rxb200_ddc *fine, cudaStre
 	return RXB200_OK;
 }
 
+int CaptureFront::set_device_rate(const rxb200_resampler *r)
+{
+	if (pos != 0 || rs.pos != 0 || rs.on()) {
+		set_error("a device rate is set once, right after create or reset, before any sample");
+		return RXB200_EINVAL;
+	}
+	return rs.attach(r);
+}
+
 int CaptureFront::reset(cudaStream_t st)
 {
 	if (filtered()) {
@@ -109,12 +118,15 @@ int CaptureFront::reset(cudaStream_t st)
 		if (rc == RXB200_OK && kind == TWO_STAGE) { rc = ts.reset(st); }
 		if (rc != RXB200_OK) { return rc; }
 	}
+	const int rc = rs.reset(st);
+	if (rc != RXB200_OK) { return rc; }
 	pos = 0;
 	return RXB200_OK;
 }
 
 void CaptureFront::release(cudaStream_t st)
 {
+	rs.release();
 	f.release();
 	ts.release(st);
 	cudaFree(d_wt); cudaFree(d_v); cudaFree(d_y);

@@ -206,7 +206,8 @@ struct rxb200_fm_mix {
 	CaptureFront fr;
 };
 
-// Every refusal of a mixing handle's call, in the order the call reports them, without enqueuing anything; *total
+// Every refusal of a mixing handle's call of n_int16 capture int16 (with a resampler, those its device samples emit), in
+// the order the call reports them, without enqueuing anything; *total
 // receives the PCM count per channel, *n16 and *chunk16 the member's call (n16 == 0: no member call).  A plain handle's
 // member sees the call's own shape.  A decimating handle's member sees the decimated one: a read with no output reports
 // what an empty call of the member reports (no PCM, no level chunks), and chunk_result_len entries of capture chunks
@@ -229,7 +230,7 @@ int rxb::fm_mix_check_host_call(rxb200_fm_mix *m, const int16_t *cs16, size_t n_
 		set_error("chunk_int16=%zu must be a multiple of 2 * decim = %zu", chunk_int16, 2 * M);
 		return RXB200_EUNSUPPORTED;
 	}
-	*n16 = 2 * m->fr.out_len(n_int16 / 2);
+	*n16 = 2 * m->fr.dec_len(n_int16 / 2);
 	*chunk16 = read ? *n16 : chunk_int16 / M;
 	if (read && *n16 == 0 && n_int16 > 0) {
 		return rxb::fm_check_host_call(m->h, cs16, 0, 262144, pcm, pcm_stride, nullptr, n_pcm, false, total);
@@ -256,9 +257,16 @@ int mix_call(rxb200_fm_mix *m, const int16_t *cs16, size_t n_int16, size_t chunk
 {
 	if (!m) { set_error("null argument"); return RXB200_EINVAL; }
 	if (device && ((uintptr_t)cs16 & 3u) != 0) { set_error("d_cs16 must be 4-byte aligned"); return RXB200_EINVAL; }
+	// with a resampler, the call's shape is that of its capture-rate output: one read of those samples, or its chunks
+	const bool rs = m->fr.rs.on();
+	if (rs && n_int16 % 2 != 0) { set_error("n_int16=%zu must be even", n_int16); return RXB200_EUNSUPPORTED; }
+	const size_t cap16 = rs ? 2 * m->fr.rs.out_len(n_int16 / 2) : n_int16;
 	size_t total = 0, n16 = 0, chunk16 = 0;
-	int rc = rxb::fm_mix_check_host_call(m, cs16, n_int16, chunk_int16, pcm, pcm_stride, chunk_result_len, n_pcm, read,
-	                                     &total, &n16, &chunk16);
+	// a call whose device samples emit no capture sample reports what an empty call of the member reports
+	int rc = rs && cap16 == 0 && n_int16 > 0
+	             ? rxb::fm_check_host_call(m->h, cs16, 0, 262144, pcm, pcm_stride, nullptr, n_pcm, false, &total)
+	             : rxb::fm_mix_check_host_call(m, cs16, cap16, read ? cap16 : chunk_int16, pcm, pcm_stride,
+	                                           chunk_result_len, n_pcm, read, &total, &n16, &chunk16);
 	if (rc != RXB200_OK || n_int16 == 0) { return rc; }
 	RXB_CUDA(cudaSetDevice(m->device));
 	const cudaStream_t st = (cudaStream_t)rxb200_fm_stream(m->h);
@@ -274,7 +282,8 @@ int mix_call(rxb200_fm_mix *m, const int16_t *cs16, size_t n_int16, size_t chunk
 	rc = m->fr.call<TabMix>(src, c, m->d_mix, (long long)(n16 / 2), RXB200_SDR_OUT_CS16, m->n_channels, st,
 	                        [&](DdcArgs<TabMix> &a) {
 		if (!m->fr.filtered()) {
-			return mix_launch(src, (long long)c, m->d_mix, (long long)n16, m->d_tab, m->d_chan, m->chan, m->fr.pos, st);
+			return mix_launch(reinterpret_cast<const int16_t *>(a.src), a.n_out, m->d_mix, (long long)n16, m->d_tab,
+			                  m->d_chan, m->chan, a.pos, st);
 		}
 		a.mix = TabMix{m->d_tab, m->d_chan, (long long)(n16 / 2)};
 		return ddc_launch(a, m->fr.f.wide ? fm_ddc_kernel<long long> : fm_ddc_kernel<int>, st);
@@ -438,19 +447,27 @@ extern "C" int rxb200_fm_mix_create_two_stage(const rxb200_fm_params *params, in
 	return mix_create(params, 0, nullptr, n_channels, fr, coarse, fine, device, out);
 }
 
+extern "C" int rxb200_fm_mix_set_device_rate(rxb200_fm_mix *m, const rxb200_resampler *rs)
+{
+	if (!m) { set_error("null argument"); return RXB200_EINVAL; }
+	RXB_CUDA(cudaSetDevice(m->device));
+	return m->fr.set_device_rate(rs);
+}
+
 extern "C" int rxb200_fm_mix_decimated_len(const rxb200_fm_mix *m, size_t n_int16, size_t *n_dec_int16)
 {
 	if (!m || !n_dec_int16) { set_error("null argument"); return RXB200_EINVAL; }
-	*n_dec_int16 = m->fr.filtered() ? 2 * m->fr.out_len(n_int16 / 2) : n_int16;
+	*n_dec_int16 = m->fr.filtered() || m->fr.rs.on() ? 2 * m->fr.out_len(n_int16 / 2) : n_int16;
 	return RXB200_OK;
 }
 
 extern "C" size_t rxb200_fm_mix_max_output(const rxb200_fm_mix *m, size_t n_int16, size_t chunk_int16)
 {
 	if (!m || chunk_int16 == 0) { return 0; }
-	if (!m->fr.filtered()) { return rxb200_fm_max_output(m->h, n_int16, chunk_int16); }
+	const size_t c = m->fr.rs.max_out(n_int16 / 2);             // the capture samples at any resampler count
+	if (!m->fr.filtered()) { return rxb200_fm_max_output(m->h, m->fr.rs.on() ? 2 * c : n_int16, chunk_int16); }
 	// floor((p + c) / M) - floor(p / M) <= ceil(c / M) at any phase p
-	const size_t M = m->fr.decim(), n16 = 2 * ((n_int16 / 2 + M - 1) / M);
+	const size_t M = m->fr.decim(), n16 = 2 * ((c + M - 1) / M);
 	return rxb200_fm_max_output(m->h, n16, chunk_int16 / M ? chunk_int16 / M : 2);
 }
 

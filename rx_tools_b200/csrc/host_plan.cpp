@@ -118,9 +118,10 @@ extern "C" int rxb200_fm_mix_table(int capture_rate, int offset_hz, int32_t *tab
 
 // The capture plan of the rx_fm shell's capture mode (include/rxb200.h, "rx_fm channels of one capture in the shell").
 // The centre fc, the decimation M and the channel grid g of rxb200_fm_plan_capture's rule, with its refusals of the
-// arguments (g_out may be NULL)
-static int capture_centre(const int64_t *tuned_hz, int n_channels, int chain_rate, long long *fc_out, long long *M_out,
-                          long long *g_out = NULL)
+// arguments (g_out may be NULL).  G: the guard band a resampler from a device rate needs (rxb200_plan_resample), which
+// the decimation floor leaves, M = ceil((2 A + c + G) / c); 0 without a device rate, today's rule.
+static int capture_centre(const int64_t *tuned_hz, int n_channels, int chain_rate, long long G, long long *fc_out,
+                          long long *M_out, long long *g_out = NULL)
 {
 	if (n_channels < 1 || chain_rate < 1) {
 		set_error("capture plan of %d channels at a chain capture rate of %d Hz (need >= 1 of each)", n_channels, chain_rate);
@@ -142,7 +143,7 @@ static int capture_centre(const int64_t *tuned_hz, int n_channels, int chain_rat
 	const long long fc = g ? tmin + g * ((tmax - tmin) / (2 * g)) : tmin;
 	const long long A = std::max(fc - tmin, tmax - fc), c = chain_rate;
 	*fc_out = fc;
-	*M_out = (2 * A + c + c - 1) / c;
+	*M_out = (2 * A + c + G + c - 1) / c;
 	if (g_out) { *g_out = g; }
 	return RXB200_OK;
 }
@@ -158,17 +159,41 @@ static int rate_check(long long R, long long M, long long max_capture_rate)
 	return RXB200_OK;
 }
 
+// The guard band G = ceil(R_dev / 32) of the _at planners' device rate (rxb200_plan_resample's), with its refusal
+static int device_guard(long long device_rate, long long *G)
+{
+	if (device_rate < 1 || device_rate > 2147483647ll) {
+		set_error("device rate %lld Hz outside [1, 2^31 - 1]", device_rate);
+		return RXB200_EINVAL;
+	}
+	*G = (device_rate + 31) / 32;
+	return RXB200_OK;
+}
+
+// the _at planners' refusal of a capture rate R above the device rate (device_rate 0: no device rate): the shells only
+// resample down
+static int device_check(long long R, long long device_rate)
+{
+	if (device_rate && R > device_rate) {
+		set_error("the channels need a capture rate of %lld Hz, above the device rate of %lld Hz", R, device_rate);
+		return RXB200_EUNSUPPORTED;
+	}
+	return RXB200_OK;
+}
+
 // rxb200_fm_plan_capture's rule; table: refuse offsets whose mixer table rxb200_fm_mix_table refuses (the rx_fm shell's
-// table mixer), else take any offset (the rx_sdr shell's NCO, rxb200_sdr_plan_capture)
+// table mixer), else take any offset (the rx_sdr shell's NCO, rxb200_sdr_plan_capture).  device_rate: 0, or the _at
+// planners' checked device rate, whose guard band G the decimation floor leaves
 static int capture_plan(const int64_t *tuned_hz, int n_channels, int chain_rate, long long max_capture_rate,
-                        rxb200_fm_capture_plan *out, int *offsets_hz, bool table)
+                        long long device_rate, long long G, rxb200_fm_capture_plan *out, int *offsets_hz, bool table)
 {
 	if (!tuned_hz || !out || !offsets_hz) { set_error("null argument"); return RXB200_EINVAL; }
 	long long fc = 0, M = 0;
-	int rc = capture_centre(tuned_hz, n_channels, chain_rate, &fc, &M);
+	int rc = capture_centre(tuned_hz, n_channels, chain_rate, G, &fc, &M);
 	if (rc != RXB200_OK) { return rc; }
 	const long long R = M * chain_rate;
 	rc = rate_check(R, M, max_capture_rate);
+	if (rc == RXB200_OK) { rc = device_check(R, device_rate); }
 	if (rc != RXB200_OK) { return rc; }
 	for (int k = 0; k < n_channels; k++) {
 		size_t L = 0;
@@ -186,21 +211,42 @@ static int capture_plan(const int64_t *tuned_hz, int n_channels, int chain_rate,
 extern "C" int rxb200_fm_plan_capture(const int64_t *tuned_hz, int n_channels, int chain_rate, long long max_capture_rate,
                                       rxb200_fm_capture_plan *out, int *offsets_hz)
 {
-	return capture_plan(tuned_hz, n_channels, chain_rate, max_capture_rate, out, offsets_hz, true);
+	return capture_plan(tuned_hz, n_channels, chain_rate, max_capture_rate, 0, 0, out, offsets_hz, true);
+}
+
+extern "C" int rxb200_fm_plan_capture_at(const int64_t *tuned_hz, int n_channels, int chain_rate,
+                                         long long max_capture_rate, long long device_rate, rxb200_fm_capture_plan *out,
+                                         int *offsets_hz)
+{
+	long long G = 0;
+	const int rc = device_guard(device_rate, &G);
+	if (rc != RXB200_OK) { return rc; }
+	return capture_plan(tuned_hz, n_channels, chain_rate, max_capture_rate, device_rate, G, out, offsets_hz, true);
 }
 
 extern "C" int rxb200_sdr_plan_capture(const int64_t *tuned_hz, int n_channels, int sample_rate,
                                        long long max_capture_rate, rxb200_fm_capture_plan *out, int *offsets_hz)
 {
-	return capture_plan(tuned_hz, n_channels, sample_rate, max_capture_rate, out, offsets_hz, false);
+	return capture_plan(tuned_hz, n_channels, sample_rate, max_capture_rate, 0, 0, out, offsets_hz, false);
 }
 
-extern "C" int rxb200_fm_plan_capture_two_stage(const int64_t *tuned_hz, int n_channels, int chain_rate,
-                                                long long max_capture_rate, rxb200_fm_two_stage_plan *out, int *offsets_hz)
+extern "C" int rxb200_sdr_plan_capture_at(const int64_t *tuned_hz, int n_channels, int sample_rate,
+                                          long long max_capture_rate, long long device_rate, rxb200_fm_capture_plan *out,
+                                          int *offsets_hz)
+{
+	long long G = 0;
+	const int rc = device_guard(device_rate, &G);
+	if (rc != RXB200_OK) { return rc; }
+	return capture_plan(tuned_hz, n_channels, sample_rate, max_capture_rate, device_rate, G, out, offsets_hz, false);
+}
+
+// rxb200_fm_plan_capture_two_stage's rule; device_rate and G as for capture_plan
+static int two_stage_plan(const int64_t *tuned_hz, int n_channels, int chain_rate, long long max_capture_rate,
+                          long long device_rate, long long G, rxb200_fm_two_stage_plan *out, int *offsets_hz)
 {
 	if (!tuned_hz || !out || !offsets_hz) { set_error("null argument"); return RXB200_EINVAL; }
 	long long fc = 0, M = 0;
-	const int rc = capture_centre(tuned_hz, n_channels, chain_rate, &fc, &M);
+	int rc = capture_centre(tuned_hz, n_channels, chain_rate, G, &fc, &M);
 	if (rc != RXB200_OK) { return rc; }
 	const long long Mp = 4 * ((M + 3) / 4), R = Mp * chain_rate;
 	if (Mp < 8) {
@@ -212,6 +258,8 @@ extern "C" int rxb200_fm_plan_capture_two_stage(const int64_t *tuned_hz, int n_c
 		          "2^31 - 1 or decimation 256", R, Mp, max_capture_rate);
 		return RXB200_EINVAL;
 	}
+	rc = device_check(R, device_rate);
+	if (rc != RXB200_OK) { return rc; }
 	for (int k = 0; k < n_channels; k++) { offsets_hz[k] = (int)(tuned_hz[k] - fc); }
 	const int M1 = (int)(Mp / 4);
 	out->centre_hz = fc;
@@ -226,15 +274,33 @@ extern "C" int rxb200_fm_plan_capture_two_stage(const int64_t *tuned_hz, int n_c
 	return RXB200_OK;
 }
 
-extern "C" int rxb200_fm_plan_capture_raster(const int64_t *tuned_hz, int n_channels, int chain_rate,
-                                             long long max_capture_rate, rxb200_fm_raster_plan *out, int *bins)
+extern "C" int rxb200_fm_plan_capture_two_stage(const int64_t *tuned_hz, int n_channels, int chain_rate,
+                                                long long max_capture_rate, rxb200_fm_two_stage_plan *out, int *offsets_hz)
+{
+	return two_stage_plan(tuned_hz, n_channels, chain_rate, max_capture_rate, 0, 0, out, offsets_hz);
+}
+
+extern "C" int rxb200_fm_plan_capture_two_stage_at(const int64_t *tuned_hz, int n_channels, int chain_rate,
+                                                   long long max_capture_rate, long long device_rate,
+                                                   rxb200_fm_two_stage_plan *out, int *offsets_hz)
+{
+	long long G = 0;
+	const int rc = device_guard(device_rate, &G);
+	if (rc != RXB200_OK) { return rc; }
+	return two_stage_plan(tuned_hz, n_channels, chain_rate, max_capture_rate, device_rate, G, out, offsets_hz);
+}
+
+// rxb200_fm_plan_capture_raster's rule; device_rate and G as for capture_plan
+static int raster_plan(const int64_t *tuned_hz, int n_channels, int chain_rate, long long max_capture_rate,
+                       long long device_rate, long long G, rxb200_fm_raster_plan *out, int *bins)
 {
 	if (!tuned_hz || !out || !bins) { set_error("null argument"); return RXB200_EINVAL; }
 	long long fc = 0, M = 0, g = 0;
-	int rc = capture_centre(tuned_hz, n_channels, chain_rate, &fc, &M, &g);
+	int rc = capture_centre(tuned_hz, n_channels, chain_rate, G, &fc, &M, &g);
 	if (rc != RXB200_OK) { return rc; }
 	const long long R = M * chain_rate;
 	rc = rate_check(R, M, max_capture_rate);
+	if (rc == RXB200_OK) { rc = device_check(R, device_rate); }
 	if (rc != RXB200_OK) { return rc; }
 	long long a = R, b = g;                              // K0 = R / gcd(R, g), 1 for g = 0
 	while (b) { const long long t = a % b; a = b; b = t; }
@@ -255,6 +321,22 @@ extern "C" int rxb200_fm_plan_capture_raster(const int64_t *tuned_hz, int n_chan
 	out->n_taps = (int)std::min(8191ll, 32 * M + 1);
 	out->shift = 30;
 	return RXB200_OK;
+}
+
+extern "C" int rxb200_fm_plan_capture_raster(const int64_t *tuned_hz, int n_channels, int chain_rate,
+                                             long long max_capture_rate, rxb200_fm_raster_plan *out, int *bins)
+{
+	return raster_plan(tuned_hz, n_channels, chain_rate, max_capture_rate, 0, 0, out, bins);
+}
+
+extern "C" int rxb200_fm_plan_capture_raster_at(const int64_t *tuned_hz, int n_channels, int chain_rate,
+                                                long long max_capture_rate, long long device_rate,
+                                                rxb200_fm_raster_plan *out, int *bins)
+{
+	long long G = 0;
+	const int rc = device_guard(device_rate, &G);
+	if (rc != RXB200_OK) { return rc; }
+	return raster_plan(tuned_hz, n_channels, chain_rate, max_capture_rate, device_rate, G, out, bins);
 }
 
 // The channel filter of rx_power's capture mode (include/rxb200.h, "rx_power hops of one capture"): a Blackman-windowed
@@ -349,6 +431,19 @@ extern "C" int rxb200_plan_resample(long long device_rate, long long rate, long 
 	out->taps_per_phase = (int)J;
 	out->taps = NULL;
 	out->shift = 15;
+	return RXB200_OK;
+}
+
+extern "C" int rxb200_resample_in_len(int up, int down, unsigned long long n0, size_t n_out, size_t *n_in)
+{
+	if (!n_in || up < 1 || down < 1) { set_error("resample_in_len: need up, down >= 1 and n_in"); return RXB200_EINVAL; }
+	typedef unsigned __int128 u128;
+	if (n_out == 0) { *n_in = 0; return RXB200_OK; }
+	// output m is emitted by device sample floor(m N / L): the call must reach the last output's, m0 + n_out - 1
+	const u128 L = (u128)up, N = (u128)down, m0 = ((u128)n0 * L + N - 1) / N;
+	const u128 c = ((m0 + (u128)n_out - 1) * N) / L + 1 - (u128)n0;
+	if (c > (u128)SIZE_MAX) { set_error("resample_in_len: %zu outputs need more than 2^64 device samples", n_out); return RXB200_EINVAL; }
+	*n_in = (size_t)c;
 	return RXB200_OK;
 }
 

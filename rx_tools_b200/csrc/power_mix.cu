@@ -12,7 +12,7 @@
 #include <new>
 #include <vector>
 #include "common.cuh"
-#include "ddc.cuh"
+#include "resample_stage.cuh"
 
 namespace rxb {
 
@@ -62,6 +62,7 @@ struct rxb200_power_mix {
 	DdcFilter f;                                 // M, T, S and the filter history
 	NcoBank nco;                                 // the shared NCO table and each hop's frequency word
 	unsigned long long pos = 0;                  // capture samples since create or reset (whole passes)
+	ResampleStage rs;                            // from the device rate, once attached
 	int16_t *d_cap = nullptr; size_t cap_cap = 0;     // host calls: the capture (int16 elements)
 	int16_t *d_bufs = nullptr; size_t bufs_cap = 0;   // the hop buffers of one group of passes, [P][he - hb][buf_len]
 	std::vector<cudaEvent_t> ev;                 // pairs around each DDC launch of the last call
@@ -74,6 +75,7 @@ extern "C" void rxb200_power_mix_destroy(rxb200_power_mix *m)
 	rxb200_power_destroy(m->h);                  // synchronises the stream the DDC runs on
 	cudaSetDevice(m->device);
 	m->f.release();
+	m->rs.release();
 	m->nco.release();
 	cudaFree(m->d_cap); cudaFree(m->d_bufs);
 	for (cudaEvent_t e : m->ev) { cudaEventDestroy(e); }
@@ -115,9 +117,21 @@ extern "C" int rxb200_power_mix_reset(rxb200_power_mix *m)
 	if (rc != RXB200_OK) { return rc; }
 	RXB_CUDA(cudaSetDevice(m->device));
 	rc = m->f.reset((cudaStream_t)rxb200_power_stream(m->h));   // behind any call still running on the member's stream
+	if (rc == RXB200_OK) { rc = m->rs.reset((cudaStream_t)rxb200_power_stream(m->h)); }
 	if (rc != RXB200_OK) { return rc; }
 	m->pos = 0;
 	return RXB200_OK;
+}
+
+extern "C" int rxb200_power_mix_set_device_rate(rxb200_power_mix *m, const rxb200_resampler *rs)
+{
+	if (!m) { set_error("null argument"); return RXB200_EINVAL; }
+	if (m->pos != 0 || m->rs.pos != 0 || m->rs.on()) {
+		set_error("a device rate is set once, right after create or reset, before any sample");
+		return RXB200_EINVAL;
+	}
+	RXB_CUDA(cudaSetDevice(m->device));
+	return m->rs.attach(rs);
 }
 
 namespace {
@@ -139,6 +153,11 @@ int power_mix_call(rxb200_power_mix *m, int hb, int he, const int16_t *cs16, siz
 		return RXB200_EINVAL;
 	}
 	if (device && ((uintptr_t)cs16 & 3u) != 0) { set_error("d_cs16 must be 4-byte aligned"); return RXB200_EINVAL; }
+	const bool rs = m->rs.on();
+	if (rs && burst) { set_error("a burst is a capture-rate capture: a handle with a device rate takes none"); return RXB200_EUNSUPPORTED; }
+	if (rs && n_int16 % 2 != 0) { set_error("n_int16=%zu must be even", n_int16); return RXB200_EUNSUPPORTED; }
+	const size_t dev16 = n_int16;                  // with a resampler, the call's device int16; n_int16 its capture's
+	if (rs) { n_int16 = 2 * m->rs.out_len(dev16 / 2); }
 	const size_t M = (size_t)m->f.M, L = (size_t)m->buf_len, pass16 = M * L;
 	const size_t lead16 = burst ? 2 * burst_lead(m->f) : 0;
 	if (burst && (n_int16 < lead16 + pass16 || (n_int16 - lead16) % pass16 != 0)) {
@@ -150,14 +169,14 @@ int power_mix_call(rxb200_power_mix *m, int hb, int he, const int16_t *cs16, siz
 		set_error("n_int16=%zu must be a multiple of decim * buf_len = %zu (whole passes)", n_int16, pass16);
 		return RXB200_EUNSUPPORTED;
 	}
-	if (n_int16 == 0) { return RXB200_OK; }
+	if (dev16 == 0) { return RXB200_OK; }
 	const size_t n_pass = (n_int16 - lead16) / pass16, hops = (size_t)(he - hb);
 	const size_t per_pass = hops * L * sizeof(int16_t);
 	const size_t group = std::max<size_t>(1, std::min<size_t>(n_pass, RXB200_POWER_MIX_SCRATCH_BYTES / per_pass));
 	RXB_CUDA(cudaSetDevice(m->device));
 	const cudaStream_t st = (cudaStream_t)rxb200_power_stream(m->h);
 	RXB_CUDA(reserve(m->d_bufs, m->bufs_cap, group * hops * L));
-	const size_t n_groups = (n_pass + group - 1) / group;
+	const size_t n_groups = (n_pass + group - 1) / group + (rs ? 1 : 0);   // and a pair around the resampler
 	while (m->ev.size() < 2 * n_groups) {
 		cudaEvent_t e = nullptr;
 		RXB_CUDA(cudaEventCreate(&e));
@@ -165,11 +184,21 @@ int power_mix_call(rxb200_power_mix *m, int hb, int he, const int16_t *cs16, siz
 	}
 	const int16_t *src = cs16;
 	if (!device) {
-		RXB_CUDA(reserve(m->d_cap, m->cap_cap, n_int16));
-		RXB_CUDA(cudaMemcpyAsync(m->d_cap, cs16, n_int16 * sizeof(int16_t), cudaMemcpyHostToDevice, st));
+		RXB_CUDA(reserve(m->d_cap, m->cap_cap, dev16));
+		RXB_CUDA(cudaMemcpyAsync(m->d_cap, cs16, dev16 * sizeof(int16_t), cudaMemcpyHostToDevice, st));
 		src = m->d_cap;
 	}
 	m->n_ev = 0;
+	if (rs) {                                      // the whole call to the capture, ahead of the groups that read it
+		const uint32_t *x = nullptr;
+		RXB_CUDA(cudaEventRecord(m->ev[0], st));
+		int rc = m->rs.run(reinterpret_cast<const uint32_t *>(src), dev16 / 2, st, &x);
+		if (rc != RXB200_OK) { return rc; }
+		RXB_CUDA(cudaEventRecord(m->ev[1], st));
+		m->n_ev++;
+		m->rs.commit(dev16 / 2);
+		src = reinterpret_cast<const int16_t *>(x);
+	}
 	DdcFilter &f = m->f;
 	for (size_t p0 = 0; p0 < n_pass; p0 += group) {
 		const size_t P = std::min(group, n_pass - p0);

@@ -7,7 +7,7 @@
 #include <new>
 #include <vector>
 #include "common.cuh"
-#include "ddc.cuh"
+#include "resample_stage.cuh"
 
 namespace rxb {
 
@@ -93,10 +93,7 @@ __global__ void __launch_bounds__(RS_THREADS) resample_kernel(const ResampleArgs
 	}
 }
 
-namespace {
-
-// the resampler's arguments: every refusal of rxb200_resample_create but the out pointer; *wide: the kernel
-// accumulates in 64 bits
+// (resample_stage.cuh)
 int resample_check(const rxb200_resampler *rs, bool *wide)
 {
 	if (!rs || !rs->taps) { set_error("null resampler or taps"); return RXB200_EINVAL; }
@@ -124,6 +121,8 @@ int resample_check(const rxb200_resampler *rs, bool *wide)
 	return RXB200_OK;
 }
 
+namespace {
+
 // the prototype phase-major: pm[p J + j] = h[p + j L]
 std::vector<int32_t> phase_major(const rxb200_resampler *rs)
 {
@@ -138,14 +137,15 @@ std::vector<int32_t> phase_major(const rxb200_resampler *rs)
 // ceil(n L / N), exactly
 u128 first_out(u128 n, long long L, long long N) { return (n * (u128)L + (u128)(N - 1)) / (u128)N; }
 
-// the outputs of a call over device samples [n0, n0 + c)
+}  // namespace
+
+// (resample_stage.cuh)
 size_t out_count(unsigned long long n0, size_t c, long long L, long long N)
 {
 	return (size_t)(first_out((u128)n0 + c, L, N) - first_out(n0, L, N));
 }
 
-// Launches resample_kernel on st for the outputs of a call over device samples [n0, n0 + c) at src (hist: the J - 1
-// samples before it), to dst; nothing when the call has no output.
+// (resample_stage.cuh)
 int resample_launch(long long L, long long N, int J, int S, bool wide, const int32_t *taps, const uint32_t *src,
                     const uint32_t *hist, unsigned long long n0, size_t c, uint32_t *dst, cudaStream_t st)
 {
@@ -179,7 +179,58 @@ int resample_launch(long long L, long long N, int J, int S, bool wide, const int
 	return RXB200_OK;
 }
 
-}  // namespace
+size_t ResampleStage::max_out(size_t c) const
+{
+	return on() ? (size_t)(((u128)c * (u128)L + (u128)(N - 1)) / (u128)N) : c;
+}
+
+int ResampleStage::attach(const rxb200_resampler *rs)
+{
+	bool wide = false;
+	const int rc = resample_check(rs, &wide);
+	if (rc != RXB200_OK) { return rc; }
+	const std::vector<int32_t> pm = phase_major(rs);
+	DdcFilter g;
+	g.M = 1; g.T = rs->taps_per_phase; g.S = rs->shift; g.wide = wide;
+	cudaError_t e = cudaMalloc(&g.taps, pm.size() * sizeof(int32_t));
+	if (e == cudaSuccess) { e = cudaMemcpy(g.taps, pm.data(), pm.size() * sizeof(int32_t), cudaMemcpyHostToDevice); }
+	const int hc = e == cudaSuccess ? g.alloc_hist() : RXB200_ECUDA;
+	if (hc != RXB200_OK) {
+		if (e != cudaSuccess) { set_error("resampler upload failed: %s", cudaGetErrorString(e)); }
+		g.release();
+		return hc;
+	}
+	L = rs->up; N = rs->down;
+	f = g;
+	pos = 0;
+	return RXB200_OK;
+}
+
+int ResampleStage::run(const uint32_t *src, size_t c, cudaStream_t st, const uint32_t **out)
+{
+	if (!on()) { *out = src; return RXB200_OK; }
+	RXB_CUDA(reserve(d_y, y_cap, std::max<size_t>(1, out_len(c))));   // at least one word: the front's carry reads it
+	const int rc = resample_launch(L, N, f.T, f.S, f.wide, f.taps, src, f.hist[f.cur], pos, c, d_y, st);
+	if (rc != RXB200_OK) { return rc; }
+	*out = d_y;
+	return f.carry(src, c, st);
+}
+
+int ResampleStage::reset(cudaStream_t st)
+{
+	if (on()) {
+		const int rc = f.reset(st);
+		if (rc != RXB200_OK) { return rc; }
+	}
+	pos = 0;
+	return RXB200_OK;
+}
+
+void ResampleStage::release()
+{
+	if (on()) { f.release(); }
+	cudaFree(d_y);
+}
 
 }  // namespace rxb
 

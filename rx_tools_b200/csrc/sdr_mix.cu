@@ -89,13 +89,25 @@ int device_call(rxb200_sdr_mix *m, const int16_t *src, size_t c, int fmt, void *
 	return RXB200_OK;
 }
 
-// capture samples per group of a host call: the staged capture and output of a group fit RXB200_SDR_MIX_SCRATCH_BYTES,
-// a multiple of M and at least M.  Each group is a device_call, which commits when it succeeds, as rx_power's groups do
-// (DdcFilter): the next group reads the history the last one left.
-size_t host_group(const rxb200_sdr_mix *m, int fmt)
+// device samples per group of a host call: what a group stages fits RXB200_SDR_MIX_SCRATCH_BYTES.  Without a
+// resampler that is the capture and the output rows, a multiple of M and at least M; with one, the device-rate upload
+// (4 bytes per device sample), the resampled capture (4 bytes per capture sample, L/N of them) and the output rows, at
+// least one device sample.  Each group is a device_call, which commits when it succeeds, as rx_power's groups do
+// (DdcFilter): the next group reads the history the last one left.  *gn: a bound on a group's outputs per channel at
+// any phase.
+size_t host_group(const rxb200_sdr_mix *m, int fmt, size_t *gn)
 {
-	const size_t M = m->fr.decim(), per = 4 * M + (size_t)m->n_ch * (size_t)sdr_elem_bytes(fmt);   // bytes per M samples
-	return M * std::max<size_t>(1, (size_t)RXB200_SDR_MIX_SCRATCH_BYTES / per);
+	const size_t M = m->fr.decim(), rows = (size_t)m->n_ch * (size_t)sdr_elem_bytes(fmt);   // row bytes per M samples
+	const ResampleStage &rs = m->fr.rs;
+	size_t g = M * std::max<size_t>(1, (size_t)RXB200_SDR_MIX_SCRATCH_BYTES / (4 * M + rows));
+	if (rs.on()) {
+		// gd device samples take gd (4 + (4 M + rows) L / (N M)) bytes
+		typedef unsigned __int128 u128;
+		const u128 S = RXB200_SDR_MIX_SCRATCH_BYTES, L = (u128)rs.L, N = (u128)rs.N, Mw = (u128)M;
+		g = std::max<size_t>(1, (size_t)(S * N * Mw / (4 * N * Mw + (4 * Mw + (u128)rows) * L)));
+	}
+	*gn = rs.max_out(g) / M + 1;
+	return g;
 }
 
 // rxb200_sdr_mix_create (w the channels' NCO words, ddc the filter), rxb200_sdr_mix_create_two_stage (fine the fine
@@ -178,6 +190,13 @@ extern "C" int rxb200_sdr_mix_reset(rxb200_sdr_mix *m)
 	return m->fr.reset(m->st);                   // behind any call still running on the handle's stream
 }
 
+extern "C" int rxb200_sdr_mix_set_device_rate(rxb200_sdr_mix *m, const rxb200_resampler *rs)
+{
+	if (!m) { set_error("null argument"); return RXB200_EINVAL; }
+	RXB_CUDA(cudaSetDevice(m->device));
+	return m->fr.set_device_rate(rs);
+}
+
 extern "C" int rxb200_sdr_mix_decimated_len(const rxb200_sdr_mix *m, size_t n_int16, size_t *n_out)
 {
 	if (!m || !n_out) { set_error("null argument"); return RXB200_EINVAL; }
@@ -209,8 +228,8 @@ extern "C" int rxb200_sdr_mix_process(rxb200_sdr_mix *m, const int16_t *cs16, si
 	if (rc != RXB200_OK) { return rc; }
 	if (n_int16 > 0) {
 		RXB_CUDA(cudaSetDevice(m->device));
-		const size_t E = (size_t)sdr_elem_bytes(format), g = host_group(m, format), c = n_int16 / 2;
-		const size_t gn = g / m->fr.decim() + 1;                   // outputs per channel of a group at any phase
+		size_t gn = 0;                                             // outputs per channel of a group at any phase
+		const size_t E = (size_t)sdr_elem_bytes(format), g = host_group(m, format, &gn), c = n_int16 / 2;
 		RXB_CUDA(reserve(m->d_cap, m->cap_cap, 2 * std::min(g, c)));
 		RXB_CUDA(reserve(m->d_out, m->out_cap, (size_t)m->n_ch * gn * E));
 		size_t done = 0;                                      // outputs per channel written so far

@@ -97,6 +97,10 @@ class _Handle:
     def reset(self) -> None:
         _lib.check(self._fn("reset")(self._h))
 
+    def _capture_int16(self, n_int16: int) -> int:
+        """A bound on the capture int16 a call of n_int16 input int16 hands the front (itself but with a resampler)."""
+        return n_int16
+
     def _input(self, cs16):
         """(the input as one C array, n_int16, whether a 1-D input of a one-channel stream handle returns 1-D)"""
         x = np.ascontiguousarray(cs16, dtype=np.int16)
@@ -114,7 +118,7 @@ class _Handle:
         x, n_int16, single = self._input(cs16)
         cap = self._bound(n_int16, chunk_int16) + 8
         out = np.empty((self.n_channels, cap), dtype=np.int16)
-        lens = np.zeros(max(1, -(-n_int16 // chunk_int16)), dtype=np.int32)
+        lens = np.zeros(max(1, -(-self._capture_int16(n_int16) // chunk_int16)), dtype=np.int32)
         n_pcm = C.c_size_t(0)
         _lib.check(self._fn("process")(self._h, x.ctypes.data, n_int16, chunk_int16, out.ctypes.data, cap,
                                        C.byref(n_pcm), lens.ctypes.data_as(C.POINTER(C.c_int))))
@@ -126,7 +130,7 @@ class _Handle:
         """One device read: ``rtlsdr_callback`` + ``full_demod`` once on the whole of it, whatever its length
         (``<prefix>_process_read``).  Shapes as ``full_demod``."""
         x, n_int16, single = self._input(cs16)
-        cap = self._bound(n_int16, max(n_int16, 1)) + 8
+        cap = self._bound(n_int16, max(self._capture_int16(n_int16), 1)) + 8
         out = np.empty((self.n_channels, cap), dtype=np.int16)
         n_pcm = C.c_size_t(0)
         _lib.check(self._fn("process_read")(self._h, x.ctypes.data, n_int16, out.ctypes.data, cap, C.byref(n_pcm)))
@@ -324,15 +328,25 @@ class CapturePlan:
     n_taps: int
 
 
-def plan_capture(tuned_hz, chain_rate: int, max_rate: int):
+def _plan_call(name: str, t, chain_rate: int, max_rate: int, device_rate: Optional[int], out, dst) -> None:
+    """One capture planner: ``name`` without a device rate, ``name_at`` (the decimation floor leaves the resampler's
+    guard band, and R above the device rate is refused) with one."""
+    args = [t.ctypes.data_as(C.POINTER(C.c_int64)), int(t.size), int(chain_rate), int(max_rate)]
+    if device_rate is not None:
+        name += "_at"
+        args.append(int(device_rate))
+    _lib.check(getattr(_lib.lib(), name)(*args, C.byref(out), _ptr(dst)))
+
+
+def plan_capture(tuned_hz, chain_rate: int, max_rate: int, device_rate: Optional[int] = None):
     """The rx_fm shell's capture plan for the tuned frequencies t_k (Hz) of a chain whose capture rate is chain_rate, under
     a rate cap (``rxb200_fm_plan_capture``): (CapturePlan, each channel's offset o_k = t_k - fc).  The filter is
-    ``power.ddc_lowpass(decim, n_taps, 15)``."""
+    ``power.ddc_lowpass(decim, n_taps, 15)``.  device_rate: the plan for a device at that rate
+    (``rxb200_fm_plan_capture_at``)."""
     t = np.ascontiguousarray(tuned_hz, dtype=np.int64).reshape(-1)
     offs = np.zeros(max(t.size, 1), dtype=np.int32)
     out = _lib.FmCapturePlanC()
-    _lib.check(_lib.lib().rxb200_fm_plan_capture(t.ctypes.data_as(C.POINTER(C.c_int64)), int(t.size), int(chain_rate),
-                                                 int(max_rate), C.byref(out), _ptr(offs)))
+    _plan_call("rxb200_fm_plan_capture", t, chain_rate, max_rate, device_rate, out, offs)
     return CapturePlan(int(out.centre_hz), out.decim, out.capture_rate, out.n_taps), [int(v) for v in offs[:t.size]]
 
 
@@ -351,14 +365,13 @@ class TwoStagePlan:
     fine_shift: int
 
 
-def plan_capture_two_stage(tuned_hz, chain_rate: int, max_rate: int):
-    """The rx_fm shell's two-stage capture plan (``rxb200_fm_plan_capture_two_stage``): (TwoStagePlan, each channel's
-    offset o_k = t_k - fc)."""
+def plan_capture_two_stage(tuned_hz, chain_rate: int, max_rate: int, device_rate: Optional[int] = None):
+    """The rx_fm shell's two-stage capture plan (``rxb200_fm_plan_capture_two_stage``, or ``_at`` with a device_rate):
+    (TwoStagePlan, each channel's offset o_k = t_k - fc)."""
     t = np.ascontiguousarray(tuned_hz, dtype=np.int64).reshape(-1)
     offs = np.zeros(max(t.size, 1), dtype=np.int32)
     out = _lib.FmTwoStagePlanC()
-    _lib.check(_lib.lib().rxb200_fm_plan_capture_two_stage(t.ctypes.data_as(C.POINTER(C.c_int64)), int(t.size),
-                                                           int(chain_rate), int(max_rate), C.byref(out), _ptr(offs)))
+    _plan_call("rxb200_fm_plan_capture_two_stage", t, chain_rate, max_rate, device_rate, out, offs)
     return TwoStagePlan(*(int(getattr(out, f[0])) for f in out._fields_)), [int(v) for v in offs[:t.size]]
 
 
@@ -374,14 +387,14 @@ class RasterCapturePlan:
     shift: int
 
 
-def plan_capture_raster(tuned_hz, chain_rate: int, max_rate: int):
-    """The capture plan of the shells' raster mode (``rxb200_fm_plan_capture_raster``) for tuned frequencies on a common
-    grid: (RasterCapturePlan, each channel's raster bin b_k).  rx_fm passes its chain capture rate, rx_sdr its -s."""
+def plan_capture_raster(tuned_hz, chain_rate: int, max_rate: int, device_rate: Optional[int] = None):
+    """The capture plan of the shells' raster mode (``rxb200_fm_plan_capture_raster``, or ``_at`` with a device_rate)
+    for tuned frequencies on a common grid: (RasterCapturePlan, each channel's raster bin b_k).  rx_fm passes its chain
+    capture rate, rx_sdr its -s."""
     t = np.ascontiguousarray(tuned_hz, dtype=np.int64).reshape(-1)
     bins = np.zeros(max(t.size, 1), dtype=np.int32)
     out = _lib.FmRasterPlanC()
-    _lib.check(_lib.lib().rxb200_fm_plan_capture_raster(t.ctypes.data_as(C.POINTER(C.c_int64)), int(t.size),
-                                                        int(chain_rate), int(max_rate), C.byref(out), _ptr(bins)))
+    _plan_call("rxb200_fm_plan_capture_raster", t, chain_rate, max_rate, device_rate, out, bins)
     return RasterCapturePlan(*(int(getattr(out, f[0])) for f in out._fields_)), [int(v) for v in bins[:t.size]]
 
 
@@ -455,6 +468,18 @@ class FmMix(_OneGpu):
             d, _t = _ddc_c(ddc)
             _lib.check(_lib.lib().rxb200_fm_mix_create_ddc(C.byref(pc), capture_rate, _ptr(offs), self.n_channels,
                                                            C.byref(d), device, C.byref(self._h)))
+
+    def set_device_rate(self, up: int, down: int, taps, shift: int = 15) -> None:
+        """Attach a resampler right after create or reset (``rxb200_fm_mix_set_device_rate``): from then on every call
+        takes device-rate CS16, resampled by up/down with the prototype taps before the front stage."""
+        from .resample import _rs_c
+        rs, _t = _rs_c(up, down, taps, shift)
+        _lib.check(_lib.lib().rxb200_fm_mix_set_device_rate(self._h, C.byref(rs)))
+        self._up_down = (int(up), int(down))
+
+    def _capture_int16(self, n_int16: int) -> int:
+        L, N = getattr(self, "_up_down", (1, 1))
+        return 2 * -(-(n_int16 // 2) * L // N)
 
     def member(self) -> int:
         """The inner rxb200_fm handle (one channel per mixed stream) as an integer."""

@@ -244,6 +244,13 @@ class PowerMix(PowerScanner):
     def reset_accumulators(self) -> None:
         _lib.check(_lib.lib().rxb200_power_reset(self._h))
 
+    def set_device_rate(self, up: int, down: int, taps, shift: int = 15) -> None:
+        """Attach a resampler right after create or reset (``rxb200_power_mix_set_device_rate``): from then on every
+        accumulate takes device-rate CS16 that resamples to whole passes."""
+        from .resample import _rs_c
+        rs, _t = _rs_c(up, down, taps, shift)
+        _lib.check(_lib.lib().rxb200_power_mix_set_device_rate(self._m, C.byref(rs)))
+
     def kernel_ms(self) -> float:
         """Device time of the last call's DDC launches (ms)."""
         ms = C.c_float(0)

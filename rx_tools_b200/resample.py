@@ -39,6 +39,13 @@ def out_count(n0: int, n_complex: int, up: int, down: int) -> int:
     return -(-(n0 + n_complex) * up // down) + (-(n0 * up) // down)
 
 
+def in_len(up: int, down: int, n0: int, n_out: int) -> int:
+    """``rxb200_resample_in_len``: the fewest device samples from n0 that emit at least n_out outputs."""
+    n = C.c_size_t(0)
+    _lib.check(_lib.lib().rxb200_resample_in_len(int(up), int(down), int(n0), int(n_out), C.byref(n)))
+    return int(n.value)
+
+
 def _rs_c(up, down, taps, shift):
     t = np.ascontiguousarray(taps, dtype=np.int32).reshape(-1)
     J = t.size // int(up) if int(up) > 0 else 0

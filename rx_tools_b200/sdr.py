@@ -9,7 +9,7 @@ from typing import Optional
 import numpy as np
 
 from . import _lib
-from .fm import CVT_CS16_CF32, CVT_CS16_CS8, CVT_CS16_CU8, CapturePlan, _ddc_c, _ptr
+from .fm import CVT_CS16_CF32, CVT_CS16_CS8, CVT_CS16_CU8, CapturePlan, _ddc_c, _plan_call, _ptr
 
 OUT_CS16 = 4
 FORMATS = {"CS16": OUT_CS16, "CS8": CVT_CS16_CS8, "CU8": CVT_CS16_CU8, "CF32": CVT_CS16_CF32}
@@ -18,14 +18,14 @@ ELEM_BYTES = {OUT_CS16: 4, CVT_CS16_CS8: 2, CVT_CS16_CU8: 2, CVT_CS16_CF32: 8}
 DTYPES = {OUT_CS16: np.int16, CVT_CS16_CS8: np.uint8, CVT_CS16_CU8: np.uint8, CVT_CS16_CF32: np.float32}
 
 
-def plan_sdr_capture(tuned_hz, sample_rate: int, max_rate: int):
-    """The rx_sdr shell's capture plan (``rxb200_sdr_plan_capture``): (CapturePlan, each channel's offset).  It is
-    ``fm.plan_capture`` with chain rate sample_rate, but takes any offset (the handle mixes with the NCO)."""
+def plan_sdr_capture(tuned_hz, sample_rate: int, max_rate: int, device_rate: Optional[int] = None):
+    """The rx_sdr shell's capture plan (``rxb200_sdr_plan_capture``, or ``_at`` with a device_rate): (CapturePlan, each
+    channel's offset).  It is ``fm.plan_capture`` with chain rate sample_rate, but takes any offset (the handle mixes
+    with the NCO)."""
     t = np.ascontiguousarray(tuned_hz, dtype=np.int64).reshape(-1)
     offs = np.zeros(max(t.size, 1), dtype=np.int32)
     out = _lib.FmCapturePlanC()
-    _lib.check(_lib.lib().rxb200_sdr_plan_capture(t.ctypes.data_as(C.POINTER(C.c_int64)), int(t.size), int(sample_rate),
-                                                  int(max_rate), C.byref(out), _ptr(offs)))
+    _plan_call("rxb200_sdr_plan_capture", t, sample_rate, max_rate, device_rate, out, offs)
     return CapturePlan(int(out.centre_hz), out.decim, out.capture_rate, out.n_taps), [int(v) for v in offs[:t.size]]
 
 
@@ -89,6 +89,13 @@ class SdrMix:
 
     def reset(self) -> None:
         _lib.check(_lib.lib().rxb200_sdr_mix_reset(self._h))
+
+    def set_device_rate(self, up: int, down: int, taps, shift: int = 15) -> None:
+        """Attach a resampler right after create or reset (``rxb200_sdr_mix_set_device_rate``): from then on every call
+        takes device-rate CS16."""
+        from .resample import _rs_c
+        rs, _t = _rs_c(up, down, taps, shift)
+        _lib.check(_lib.lib().rxb200_sdr_mix_set_device_rate(self._h, C.byref(rs)))
 
     def decimated_len(self, n_int16: int) -> int:
         n = C.c_size_t(0)
