@@ -16,6 +16,12 @@
  * rxb200_fm_plan_capture_two_stage's and the handle a two-stage mixing handle (M = M1 M2); with
  * RXB200_CAPTURE_STAGES=raster, the plan is rxb200_fm_plan_capture_raster's (channels on a common grid, at most 4096
  * bins) and the handle a raster mixing handle; nothing else changes.
+ *
+ * RXB200_DEVICE_RATE=<Hz> with capture mode: the device runs at that rate instead of R.  The plan is the _at planner's
+ * (its decimation leaves the resampler's guard band; a plan above the device rate exits 1 before the device is
+ * opened), the device is asked for R_dev, and the rate it reports is what the plan and the resampler start from
+ * (rxb200_plan_resample, rxb200_fm_mix_set_device_rate).  The reader then gathers blocks of exactly the device samples
+ * that emit M * 131072 capture samples (rxb200_resample_in_len), so every chain read is still 131072 samples.
  */
 #include <errno.h>
 #include <math.h>
@@ -99,6 +105,9 @@ static struct {
 	rxb200_fm_mix *mix;                /* capture mode: one decimating mixing handle, K = freq_len channels */
 	size_t block16, stride;            /* capture mode: int16 per block, PCM int16 per channel and block */
 	int decim;
+	int rs_up, rs_down;                /* capture mode at a device rate: the resampler's L/N (0: none attached) */
+	size_t slot16;                     /* capture mode: int16 a raw slot holds, the most device int16 of a block */
+	unsigned long long dev_pos;        /* capture mode at a device rate: device samples handed on so far */
 	FILE *outs[MAX_FREQS];
 	Queue q_raw, q_pcm;
 	pthread_mutex_t hop_m;
@@ -119,7 +128,8 @@ static void usage(void)
 		"environment: RXB200_CAPTURE_RATE=max_Hz takes every -f channel from one capture of at most max_Hz samples/s,\n"
 		"\ttuned once to their centre (one GPU), channel f to filename.f (no scanning, no -l needed; refuses '-', -L, -o);\n"
 		"\tRXB200_CAPTURE_STAGES=2 plans that capture in two stages, RXB200_CAPTURE_STAGES=raster as one raster of bins\n"
-		"\t(channels on a common grid, at most 4096 bins)\n");
+		"\t(channels on a common grid, at most 4096 bins); RXB200_DEVICE_RATE=Hz runs the device at that rate and\n"
+		"\tresamples its stream to the capture's rate on the GPU\n");
 	exit(1);
 }
 
@@ -160,7 +170,7 @@ static void write_wav_header(FILE *out)
  * mixing handle, whose channel filters cost a coarse DFT shared by every channel plus a 129-tap fine filter per channel;
  * with RXB200_CAPTURE_STAGES=raster, the raster plan and a raster mixing handle, whose channels share one polyphase
  * branch sum per output and one DFT.  Nonzero (reported on stderr) when the plan or the handle is refused. */
-static int capture_setup(const char *cap_env, int64_t *centre, int *rate)
+static int capture_setup(const char *cap_env, long long dev_rate, int64_t *centre, int *rate)
 {
 	int64_t t[MAX_FREQS];
 	int chans[MAX_FREQS];
@@ -170,8 +180,9 @@ static int capture_setup(const char *cap_env, int64_t *centre, int *rate)
 	                             : stages && strcmp(stages, "raster") == 0 ? CAPTURE_RASTER
 	                                                                       : CAPTURE_SINGLE;
 	struct capture_plan pl;
-	if (capture_plan(kind, t, G.freq_len, G.der.capture_rate, cap_env, rxb200_fm_plan_capture, &pl, chans) != 0) { return 1; }
-	const int rc = kind == CAPTURE_TWO_STAGE ? rxb200_fm_mix_create_two_stage(&G.der.params, pl.capture_rate, pl.n_bins, chans,
+	rxb200_resampler rs = {1, 1, 0, NULL, 15};
+	if (capture_plan(kind, t, G.freq_len, G.der.capture_rate, cap_env, 0, dev_rate, &pl, chans) != 0) { return 1; }
+	int rc = kind == CAPTURE_TWO_STAGE ? rxb200_fm_mix_create_two_stage(&G.der.params, pl.capture_rate, pl.n_bins, chans,
 	                                                                          G.freq_len, &pl.ddc, &pl.fine, 0, &G.mix)
 	             : kind == CAPTURE_RASTER ? rxb200_fm_mix_create_raster(&G.der.params, pl.n_bins, chans, G.freq_len, &pl.ddc, 0,
 	                                                                    &G.mix)
@@ -179,12 +190,22 @@ static int capture_setup(const char *cap_env, int64_t *centre, int *rate)
 	                                                                 &pl.ddc, 0, &G.mix);
 	capture_plan_release(&pl);
 	if (rc != RXB200_OK) { fprintf(stderr, "rxb200: %s\n", rxb200_last_error()); return 1; }
+	fputs(pl.banner, stderr);
+	/* the _at plan leaves the guard band, so the resampler's plan is not refused here */
+	if (dev_rate && device_resampler(dev_rate, pl.capture_rate, pl.span, &rs) != 0) { return 1; }
+	if (rs.taps) { rc = rxb200_fm_mix_set_device_rate(G.mix, &rs); }
+	free((void *)rs.taps);
+	if (rc != RXB200_OK) { fprintf(stderr, "rxb200: %s\n", rxb200_last_error()); return 1; }
 	G.decim = pl.decim;
 	G.block16 = (size_t)pl.decim * 2 * CHUNK_COMPLEX;
-	G.stride = rxb200_fm_mix_max_output(G.mix, G.block16, G.block16);
+	G.rs_up = rs.taps ? rs.up : 0;
+	G.rs_down = rs.taps ? rs.down : 0;
+	/* a block of M * 131072 capture samples takes at most ceil(M * 131072 N / L) + 1 device samples */
+	G.slot16 = G.rs_up ? 2 * (((size_t)pl.decim * CHUNK_COMPLEX * (size_t)G.rs_down + (size_t)G.rs_up - 1) / (size_t)G.rs_up + 1)
+	                   : G.block16;
+	G.stride = rxb200_fm_mix_max_output(G.mix, G.slot16, G.block16);
 	*centre = pl.centre_hz;
 	*rate = pl.capture_rate;
-	fputs(pl.banner, stderr);
 	return 0;
 }
 
@@ -232,26 +253,35 @@ static void *reader_thread(void *arg)
 
 /* Capture mode's reader: blocks of M * 131072 complex samples gathered from reads of any length, so that blocks start at
  * multiples of M and every channel's chain sees reads of exactly 131072 complex samples.  At the end of the stream, or
- * on a failed read, the partial block is handed on if it decimates to at least min_chunk int16, else dropped. */
+ * on a failed read, the partial block is handed on if it decimates to at least min_chunk int16, else dropped.  With a
+ * resampler a block is the device samples that emit M * 131072 capture samples from the device count so far, and the
+ * partial block's rule counts the capture samples it emits. */
 static void *block_reader_thread(void *arg)
 {
 	(void)arg;
 	SoapySDRDevice_activateStream(G.dev, G.stream, 0, 0, 0);
 	for (;;) {
 		Slot *s = q_begin_put(&G.q_raw);
+		size_t want16 = G.block16;
+		if (G.rs_up) {
+			size_t c = 0;
+			rxb200_resample_in_len(G.rs_up, G.rs_down, G.dev_pos, G.block16 / 2, &c);
+			want16 = 2 * c;
+		}
 		size_t have = 0;
 		int r = 1;
-		while (have < G.block16) {
+		while (have < want16) {
 			void *buffs[] = {s->data + have};
 			int flags = 0; long long t_ns = 0;
-			r = g_stop ? -1 : SoapySDRDevice_readStream(G.dev, G.stream, buffs, (G.block16 - have) / 2, &flags, &t_ns, 1000000);
+			r = g_stop ? -1 : SoapySDRDevice_readStream(G.dev, G.stream, buffs, (want16 - have) / 2, &flags, &t_ns, 1000000);
 			if (r == SOAPY_SDR_OVERFLOW) { fprintf(stderr, "O"); fflush(stderr); continue; }
 			if (r <= 0) { break; }
 			have += (size_t)r * 2;
 		}
-		if (have == G.block16) { s->n = have; s->eof = 0; q_end_put(&G.q_raw); continue; }
+		if (have == want16) { s->n = have; s->eof = 0; G.dev_pos += have / 2; q_end_put(&G.q_raw); continue; }
 		if (!g_stop) { fprintf(stderr, "readStream read failed: %d\n", r); }
-		if (2 * (have / 2 / (size_t)G.decim) >= G.min_chunk) {
+		const size_t emitted = G.rs_up ? resample_out_count(G.rs_up, G.rs_down, G.dev_pos, have / 2) : have / 2;
+		if (2 * (emitted / (size_t)G.decim) >= G.min_chunk) {
 			s->n = have; s->eof = 0; q_end_put(&G.q_raw);
 			s = q_begin_put(&G.q_raw);
 		}
@@ -434,6 +464,8 @@ int main(int argc, char **argv)
 	}
 	if (G.freq_len > 1) { G.terminate_on_squelch = 0; }
 	G.filename = (argc <= optind) ? "-" : argv[optind];
+	const long long dev_rate = device_rate_env(cap_env != NULL, "capture mode (RXB200_CAPTURE_RATE)");
+	if (dev_rate < 0) { return 1; }
 	if (cap_env) {
 		/* capture mode: one file per channel, one read per block; the mixer puts each channel at DC */
 		const char *bad = !strcmp(G.filename, "-") ? "'-' as the filename (it writes one file per channel)"
@@ -467,7 +499,7 @@ int main(int argc, char **argv)
 	int64_t tune_freq = capture_freq(0);
 	int tune_rate = G.der.capture_rate;
 	if (cap_env) {
-		if (capture_setup(cap_env, &tune_freq, &tune_rate) != 0) { return 1; }
+		if (capture_setup(cap_env, dev_rate, &tune_freq, &tune_rate) != 0) { return 1; }
 	} else if (rxb200_fm_create(&G.der.params, 0, 1, &G.fm) != RXB200_OK) { fprintf(stderr, "rxb200: %s\n", rxb200_last_error()); return 1; }
 
 	if (sdr_open(G.dev_query, G.channel, &G.dev, &G.stream) != 0) {
@@ -487,7 +519,20 @@ int main(int argc, char **argv)
 	{
 		SoapySDRKwargs none = {0, NULL, NULL};
 		SoapySDRDevice_setFrequency(G.dev, SOAPY_SDR_RX, G.channel, (double)tune_freq, &none);
-		SoapySDRDevice_setSampleRate(G.dev, SOAPY_SDR_RX, G.channel, (double)tune_rate);
+		if (!dev_rate) {
+			SoapySDRDevice_setSampleRate(G.dev, SOAPY_SDR_RX, G.channel, (double)tune_rate);
+		} else {
+			const long long got = sdr_device_rate(G.dev, G.channel, dev_rate);
+			if (got < 0) { sdr_close(G.dev, G.stream); return 1; }
+			if (got != dev_rate) {
+				/* the device runs at another rate than it was asked for: plan and resample from the rate it reports
+				 * (the centre does not depend on the rate, so the tuning stands) */
+				fprintf(stderr, "The device reports %lld Hz, not RXB200_DEVICE_RATE=%lld Hz: planning again.\n", got, dev_rate);
+				rxb200_fm_mix_destroy(G.mix);
+				G.mix = NULL;
+				if (capture_setup(cap_env, got, &tune_freq, &tune_rate) != 0) { sdr_close(G.dev, G.stream); return 1; }
+			}
+		}
 	}
 	fprintf(stderr, "Oversampling input by: %ix.\n", G.der.params.downsample);
 	fprintf(stderr, "Oversampling output by: %ix.\n", G.der.params.post_downsample);
@@ -506,7 +551,7 @@ int main(int argc, char **argv)
 		if (G.wav) { write_wav_header(G.out); }
 	}
 
-	q_init(&G.q_raw, G.mix ? G.block16 : 2 * CHUNK_COMPLEX);
+	q_init(&G.q_raw, G.mix ? G.slot16 : 2 * CHUNK_COMPLEX);
 	q_init(&G.q_pcm, G.mix ? (size_t)G.freq_len * G.stride : 2 * CHUNK_COMPLEX);
 	pthread_t tr, td, tw;
 	pthread_create(&tw, NULL, writer_thread, NULL);

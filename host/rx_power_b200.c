@@ -20,6 +20,14 @@
  * (rxb200_power_plan_tiles).  Per sweep, each tile is one retune to its centre, one flush read, and one burst of the
  * filter's lead plus one pass, gathered from reads of any length and handed to rxb200_power_mix_accumulate_burst for
  * the tile's hops.  A failed read drops that tile's burst for the sweep, as hop mode skips a hop.
+ *
+ * RXB200_DEVICE_RATE=<Hz> with capture or tile mode: the device runs at that rate instead of R.  The plan is
+ * rxb200_power_plan_capture_at's or rxb200_power_plan_tiles_at's (the decimation leaves the resampler's guard band;
+ * tiles shrink to fit the device; a capture plan above the device rate exits 1 before the device is opened).  The
+ * device is asked for R_dev, and the rate it reports is what the plan and the resampler start from.  Capture mode reads
+ * passes of the device samples that emit one pass of M * buf_len int16 (rxb200_resample_in_len) into a handle with
+ * rxb200_power_mix_set_device_rate; tile mode reads bursts of rxb200_power_mix_burst_in_len device int16 into a handle
+ * with rxb200_power_mix_set_burst_device_rate.
  */
 #include <math.h>
 #include <signal.h>
@@ -51,7 +59,8 @@ static void usage(void)
 		"environment: RXB200_GPUS=n shards the hops over n GPUs; RXB200_CAPTURE_RATE=max_Hz takes every hop from one\n"
 		"\tcapture of at most max_Hz samples/s, tuned once to the centre of the sweep (one GPU);\n"
 		"\tRXB200_TILE_RATE=max_Hz takes a wider sweep in tiles of hops, one retune and one burst of at most max_Hz\n"
-		"\tsamples/s per tile (one GPU)\n");
+		"\tsamples/s per tile (one GPU); RXB200_DEVICE_RATE=Hz (with either) runs the device at that rate and resamples\n"
+		"\tits stream to the capture's rate on the GPU\n");
 	exit(1);
 }
 
@@ -128,23 +137,108 @@ static void retune(SoapySDRDevice *dev, SoapySDRStream *stream, size_t channel, 
 	if (r < 0) { fprintf(stderr, "Error: bad retune at %lli Hz, r=%d (try increasing -S or -R).\n", (long long)f, r); }
 }
 
+/* Capture or tile mode's plan and handle.  tiles: tile mode, its plan rxb200_power_plan_tiles's, else capture mode's
+ * rxb200_power_plan_capture's; each the _at planner's when dev_rate is not 0, with the resampler from that rate
+ * attached to the handle (to its bursts in tile mode).  limit is the mode's variable, RXB200_TILE_RATE's or
+ * RXB200_CAPTURE_RATE's value.  Prints the mode's banner and the device rate's line; nonzero, reported on stderr, when
+ * a plan or the handle is refused. */
+struct power_setup {
+	rxb200_power_mix *pm;
+	rxb200_power_tiling tl;      /* tile mode */
+	int64_t fc;                  /* capture mode: the centre */
+	int decim, rate;             /* M and R = M plan->rate */
+	int rs_up, rs_down;          /* capture mode at a device rate: the resampler's L/N (0: none attached) */
+};
+static int power_setup(int tiles, const rxb200_power_plan *plan, const int *window_coefs, const char *limit,
+                       long long dev_rate, struct power_setup *ps)
+{
+	const rxb200_power_params *pp = &plan->params;
+	const char *mode = tiles ? "Tile mode" : "Capture mode", *var = tiles ? "RXB200_TILE_RATE" : "RXB200_CAPTURE_RATE";
+	memset(ps, 0, sizeof *ps);
+	int *offs = (int *)malloc(sizeof(int) * (size_t)pp->n_hops);
+	rxb200_fm_capture_plan cp;
+	int rc, T;
+	if (tiles) {
+		rc = dev_rate ? rxb200_power_plan_tiles_at(plan, atoll(limit), dev_rate, &ps->tl, offs)
+		              : rxb200_power_plan_tiles(plan, atoll(limit), &ps->tl, offs);
+		ps->decim = ps->tl.decim; ps->rate = ps->tl.capture_rate; T = ps->tl.n_taps;
+	} else {
+		rc = dev_rate ? rxb200_power_plan_capture_at(plan, atoll(limit), dev_rate, &cp, offs)
+		              : rxb200_power_plan_capture(plan, atoll(limit), &cp, offs);
+		ps->fc = cp.centre_hz; ps->decim = cp.decim; ps->rate = cp.capture_rate; T = cp.n_taps;
+	}
+	if (rc == RXB200_EINVAL && !tiles) {         /* the rate the span needs is above the cap (the message names it) */
+		fprintf(stderr, "Capture mode: %s, above RXB200_CAPTURE_RATE=%s.\n", rxb200_last_error(), limit);
+		free(offs);
+		return 1;
+	}
+	if (rc != RXB200_OK) { fprintf(stderr, "%s: %s (%s=%s).\n", mode, rxb200_last_error(), var, limit); free(offs); return 1; }
+	if (tiles) {
+		fprintf(stderr, "Tile mode: %d tiles of up to %d hops, %d Hz, decimation %d, %d taps\n", ps->tl.n_tiles,
+		        ps->tl.hops_per_tile, ps->tl.capture_rate, ps->tl.decim, ps->tl.n_taps);
+	} else {
+		fprintf(stderr, "Capture mode: %lld Hz centred at %lli Hz, decimation %lld, %d taps\n", (long long)ps->rate,
+		        (long long)ps->fc, (long long)ps->decim, T);
+	}
+	/* the resampler spans the widest tile (each offset is from its own tile's centre), or every hop */
+	long long span = 0;
+	for (int i = 0; i < pp->n_hops; i++) { span = 2 * (long long)abs(offs[i]) > span ? 2 * (long long)abs(offs[i]) : span; }
+	rxb200_resampler rs = {1, 1, 0, NULL, 15};
+	if (dev_rate && device_resampler(dev_rate, ps->rate, span + plan->rate, &rs) != 0) { free(offs); return 1; }
+	int32_t *taps = (int32_t *)malloc(sizeof(int32_t) * (size_t)T);
+	rxb200_ddc_lowpass(ps->decim, T, 15, taps);
+	const rxb200_ddc ddc = {ps->decim, T, taps, 15};
+	rc = rxb200_power_mix_create(pp, window_coefs, NULL, ps->rate, offs, &ddc, 0, &ps->pm);
+	free(offs); free(taps);
+	if (rc == RXB200_OK && rs.taps) {
+		rc = tiles ? rxb200_power_mix_set_burst_device_rate(ps->pm, &rs) : rxb200_power_mix_set_device_rate(ps->pm, &rs);
+		if (!tiles) { ps->rs_up = rs.up; ps->rs_down = rs.down; }
+	}
+	free((void *)rs.taps);
+	if (rc != RXB200_OK) { fprintf(stderr, "rxb200: %s\n", rxb200_last_error()); return 1; }
+	return 0;
+}
+
+/* The mode's sample rate on the device: R, or at a device rate R_dev the rate the device reports, planning again (a
+ * new handle in *ps) when that is not R_dev.  The centres do not depend on the rate, so a tuning stands.  Nonzero,
+ * reported on stderr, when the device reports no valid rate or the new plan is refused. */
+static int device_side_rate(SoapySDRDevice *dev, size_t channel, int tiles, const rxb200_power_plan *plan,
+                            const int *window_coefs, const char *limit, long long dev_rate, struct power_setup *ps)
+{
+	if (!dev_rate) { SoapySDRDevice_setSampleRate(dev, SOAPY_SDR_RX, channel, (double)ps->rate); return 0; }
+	const long long got = sdr_device_rate(dev, channel, dev_rate);
+	if (got < 0) { return 1; }
+	if (got == dev_rate) { return 0; }
+	fprintf(stderr, "The device reports %lld Hz, not RXB200_DEVICE_RATE=%lld Hz: planning again.\n", got, dev_rate);
+	rxb200_power_mix_destroy(ps->pm);
+	return power_setup(tiles, plan, window_coefs, limit, got, ps);
+}
+
 /* Tile mode's device side and report loop.  Per sweep, each tile retunes to its centre when the device is elsewhere,
- * then gathers one burst of G + M * buf_len / 2 complex samples from reads of whatever length the device returns and
- * accumulates it for the tile's hops.  A failed read drops the burst, so the tile's hops get no pass this sweep; the
+ * then gathers one burst of rxb200_power_mix_burst_in_len int16 (G + M * buf_len / 2 complex samples, or at a device
+ * rate the device samples that emit E more) from reads of whatever length the device returns and accumulates it for
+ * the tile's hops.  A failed read drops the burst, so the tile's hops get no pass this sweep; the
  * stream has run dry when no tile got its burst in a sweep. */
-static int tile_mode(rxb200_power_mix *pm, const rxb200_power_plan *plan, const rxb200_power_tiling *tl,
-                     const char *dev_query, size_t channel, const char *gain_str, const char *antenna, const char *filename,
-                     int ppm, int direct_sampling, int offset_tuning, int tuner_sleep_usec, int tuner_retry_max,
-                     int interval, int single, time_t exit_after)
+static int tile_mode(struct power_setup *ps, const rxb200_power_plan *plan, const int *window_coefs, const char *limit,
+                     long long dev_rate, const char *dev_query, size_t channel, const char *gain_str, const char *antenna,
+                     const char *filename, int ppm, int direct_sampling, int offset_tuning, int tuner_sleep_usec,
+                     int tuner_retry_max, int interval, int single, time_t exit_after)
 {
 	const rxb200_power_params *pp = &plan->params;
 	const int n_hops = pp->n_hops, N = 1 << pp->bin_e;
-	rxb200_power *pw = rxb200_power_mix_member(pm);
 	SoapySDRDevice *dev = NULL; SoapySDRStream *stream = NULL;
 	FILE *out = open_radio(dev_query, channel, antenna, gain_str, ppm, direct_sampling, offset_tuning, filename, &dev, &stream);
 	if (!out) { return 1; }
-	SoapySDRDevice_setSampleRate(dev, SOAPY_SDR_RX, channel, (double)tl->capture_rate);
-	const size_t burst16 = 2 * (size_t)rxb200_power_mix_lead(pm) + (size_t)tl->decim * (size_t)pp->buf_len;
+	if (device_side_rate(dev, channel, 1, plan, window_coefs, limit, dev_rate, ps) != 0) {
+		if (out != stdout) { fclose(out); }
+		sdr_close(dev, stream);
+		return 1;
+	}
+	rxb200_power_mix *pm = ps->pm;
+	const rxb200_power_tiling *tl = &ps->tl;
+	rxb200_power *pw = rxb200_power_mix_member(pm);
+	size_t burst16 = 0;                                  /* the lead plus one pass, device int16 at a device rate */
+	rxb200_power_mix_burst_in_len(pm, 1, &burst16);
 	int16_t *burst = (int16_t *)malloc(burst16 * sizeof(int16_t));
 	int16_t *dump = (int16_t *)malloc((size_t)BUFFER_DUMP * 4);
 	const int row_len = rxb200_power_row_len(pp->bin_e, plan->crop);
@@ -201,23 +295,31 @@ static int tile_mode(rxb200_power_mix *pm, const rxb200_power_plan *plan, const 
 /* Capture mode's device side and report loop: one tune to fc at R, one flush read, then passes of M * buf_len int16
  * collected from reads of whatever length the device returns; a failed read discards the partial pass, and
  * tuner_retry_max failed reads in a row mean the stream has run dry. */
-static int capture_mode(rxb200_power_mix *pm, const rxb200_power_plan *plan, int R, int64_t fc, int M,
-                        const char *dev_query, size_t channel, const char *gain_str, const char *antenna, const char *filename,
-                        int ppm, int direct_sampling, int offset_tuning, int tuner_sleep_usec, int tuner_retry_max,
-                        int interval, int single, time_t exit_after)
+static int capture_mode(struct power_setup *ps, const rxb200_power_plan *plan, const int *window_coefs,
+                        const char *limit, long long dev_rate, const char *dev_query, size_t channel, const char *gain_str,
+                        const char *antenna, const char *filename, int ppm, int direct_sampling, int offset_tuning,
+                        int tuner_sleep_usec, int tuner_retry_max, int interval, int single, time_t exit_after)
 {
 	const rxb200_power_params *pp = &plan->params;
 	const int n_hops = pp->n_hops, N = 1 << pp->bin_e;
-	rxb200_power *pw = rxb200_power_mix_member(pm);
 	SoapySDRDevice *dev = NULL; SoapySDRStream *stream = NULL;
 	FILE *out = open_radio(dev_query, channel, antenna, gain_str, ppm, direct_sampling, offset_tuning, filename, &dev, &stream);
 	if (!out) { return 1; }
-	SoapySDRDevice_setSampleRate(dev, SOAPY_SDR_RX, channel, (double)R);
+	if (device_side_rate(dev, channel, 0, plan, window_coefs, limit, dev_rate, ps) != 0) {
+		if (out != stdout) { fclose(out); }
+		sdr_close(dev, stream);
+		return 1;
+	}
+	rxb200_power_mix *pm = ps->pm;
+	rxb200_power *pw = rxb200_power_mix_member(pm);
 	int16_t *dump = (int16_t *)malloc((size_t)BUFFER_DUMP * 4);
-	retune(dev, stream, channel, fc, dump, tuner_sleep_usec, tuner_retry_max);
+	retune(dev, stream, channel, ps->fc, dump, tuner_sleep_usec, tuner_retry_max);
 	free(dump);
-	const size_t pass16 = (size_t)M * (size_t)pp->buf_len;
-	int16_t *pass = (int16_t *)malloc(pass16 * sizeof(int16_t));
+	/* a pass: M * buf_len capture int16; at a device rate, the device samples that emit them from the count so far */
+	const size_t cap16 = (size_t)ps->decim * (size_t)pp->buf_len;
+	const size_t max16 = ps->rs_up ? 2 * ((cap16 / 2 * (size_t)ps->rs_down + (size_t)ps->rs_up - 1) / (size_t)ps->rs_up + 1) : cap16;
+	unsigned long long dev_pos = 0;                       /* device samples of the passes taken */
+	int16_t *pass = (int16_t *)malloc(max16 * sizeof(int16_t));
 	const int row_len = rxb200_power_row_len(pp->bin_e, plan->crop);
 	double *db = (double *)malloc((size_t)n_hops * (size_t)row_len * sizeof(double));
 	int *samples = (int *)malloc((size_t)n_hops * sizeof(int));
@@ -228,7 +330,13 @@ static int capture_mode(rxb200_power_mix *pm, const rxb200_power_plan *plan, int
 	time_t next_tick = time(NULL) + interval, exit_time = exit_after ? time(NULL) + exit_after : 0;
 	int done = 0, rc = 0;
 	while (!done && !g_stop) {
-		/* ---- one pass: M * buf_len int16 from as many reads as it takes */
+		/* ---- one pass: M * buf_len int16 (or the device int16 that emit them) from as many reads as it takes */
+		size_t pass16 = cap16;
+		if (ps->rs_up) {
+			size_t c = 0;
+			rxb200_resample_in_len(ps->rs_up, ps->rs_down, dev_pos, cap16 / 2, &c);
+			pass16 = 2 * c;
+		}
 		size_t have = 0;
 		int fails = 0, dry = 0;
 		while (have < pass16 && !g_stop) {
@@ -246,6 +354,7 @@ static int capture_mode(rxb200_power_mix *pm, const rxb200_power_plan *plan, int
 		}
 		if (have == pass16) {
 			if (rxb200_power_mix_accumulate(pm, pass, pass16) != RXB200_OK) { fprintf(stderr, "rxb200: %s\n", rxb200_last_error()); rc = 1; break; }
+			dev_pos += pass16 / 2;
 			sweeps++;
 		}
 		time_t now = time(NULL);
@@ -331,57 +440,29 @@ int main(int argc, char **argv)
 	if (n_gpus < 1) { n_gpus = 1; }
 	if (n_gpus > n_hops) { n_gpus = n_hops; }
 	const char *cap_env = getenv("RXB200_CAPTURE_RATE"), *tile_env = getenv("RXB200_TILE_RATE");
+	const long long dev_rate = device_rate_env(cap_env || tile_env, "capture or tile mode (RXB200_CAPTURE_RATE or RXB200_TILE_RATE)");
+	if (dev_rate < 0) { return 1; }
 	if (tile_env) {
 		/* tile mode: the planner's tiles, each hop's offset from its tile's centre, one filter for every tile */
 		if (cap_env) { fprintf(stderr, "Tile mode (RXB200_TILE_RATE) and capture mode (RXB200_CAPTURE_RATE) exclude each other.\n"); return 1; }
 		if (n_gpus > 1) { fprintf(stderr, "Tile mode (RXB200_TILE_RATE) runs on one GPU: unset RXB200_GPUS.\n"); return 1; }
-		rxb200_power_tiling tl;
-		int *offs = (int *)malloc(sizeof(int) * (size_t)n_hops);
-		if (rxb200_power_plan_tiles(&plan, atoll(tile_env), &tl, offs) != RXB200_OK) {
-			fprintf(stderr, "Tile mode: %s (RXB200_TILE_RATE=%s).\n", rxb200_last_error(), tile_env);
-			return 1;
-		}
-		fprintf(stderr, "Tile mode: %d tiles of up to %d hops, %d Hz, decimation %d, %d taps\n", tl.n_tiles,
-		        tl.hops_per_tile, tl.capture_rate, tl.decim, tl.n_taps);
-		int32_t *taps = (int32_t *)malloc(sizeof(int32_t) * (size_t)tl.n_taps);
-		rxb200_ddc_lowpass(tl.decim, tl.n_taps, 15, taps);
-		const rxb200_ddc ddc = {tl.decim, tl.n_taps, taps, 15};
-		rxb200_power_mix *pm = NULL;
-		if (rxb200_power_mix_create(pp, window_coefs, NULL, tl.capture_rate, offs, &ddc, 0, &pm) != RXB200_OK) { fprintf(stderr, "rxb200: %s\n", rxb200_last_error()); return 1; }
-		free(offs); free(taps);
-		const int rc = tile_mode(pm, &plan, &tl, dev_query, channel, gain_str, antenna, filename, ppm, direct_sampling,
-		                         offset_tuning, tuner_sleep_usec, tuner_retry_max, interval, single, exit_after);
-		rxb200_power_mix_destroy(pm);
+		struct power_setup ps;
+		if (power_setup(1, &plan, window_coefs, tile_env, dev_rate, &ps) != 0) { return 1; }
+		const int rc = tile_mode(&ps, &plan, window_coefs, tile_env, dev_rate, dev_query, channel, gain_str, antenna, filename,
+		                         ppm, direct_sampling, offset_tuning, tuner_sleep_usec, tuner_retry_max, interval, single,
+		                         exit_after);
+		rxb200_power_mix_destroy(ps.pm);
 		return rc;
 	}
 	if (cap_env) {
 		/* capture mode: centre of the hops, each hop's offset from it, the smallest M whose capture holds them all */
 		if (n_gpus > 1) { fprintf(stderr, "Capture mode (RXB200_CAPTURE_RATE) runs on one GPU: unset RXB200_GPUS.\n"); return 1; }
-		const long long cap_max = atoll(cap_env), rate = plan.rate;
-		const int64_t fc = plan.first_freq + ((int64_t)(n_hops - 1) * plan.freq_step) / 2;
-		int *offs = (int *)malloc(sizeof(int) * (size_t)n_hops);
-		long long span = 0;
-		for (int i = 0; i < n_hops; i++) {
-			const long long f = (long long)(plan.first_freq + (int64_t)i * plan.freq_step - fc);
-			if (2 * (f < 0 ? -f : f) > span) { span = 2 * (f < 0 ? -f : f); }
-			offs[i] = (int)f;
-		}
-		const long long M = (span + rate + rate - 1) / rate, R = M * rate;
-		if (R > cap_max || R > 2147483647LL || M > 4096) {
-			fprintf(stderr, "Capture mode: the span needs a capture rate of %lld Hz, above RXB200_CAPTURE_RATE=%s.\n", R, cap_env);
-			return 1;
-		}
-		const int T = M * 32 + 1 < 8191 ? (int)M * 32 + 1 : 8191;
-		int32_t *taps = (int32_t *)malloc(sizeof(int32_t) * (size_t)T);
-		rxb200_ddc_lowpass((int)M, T, 15, taps);
-		fprintf(stderr, "Capture mode: %lld Hz centred at %lli Hz, decimation %lld, %d taps\n", R, (long long)fc, M, T);
-		const rxb200_ddc ddc = {(int)M, T, taps, 15};
-		rxb200_power_mix *pm = NULL;
-		if (rxb200_power_mix_create(pp, window_coefs, NULL, (int)R, offs, &ddc, 0, &pm) != RXB200_OK) { fprintf(stderr, "rxb200: %s\n", rxb200_last_error()); return 1; }
-		free(offs); free(taps);
-		const int rc = capture_mode(pm, &plan, (int)R, fc, (int)M, dev_query, channel, gain_str, antenna, filename, ppm,
-		                            direct_sampling, offset_tuning, tuner_sleep_usec, tuner_retry_max, interval, single, exit_after);
-		rxb200_power_mix_destroy(pm);
+		struct power_setup ps;
+		if (power_setup(0, &plan, window_coefs, cap_env, dev_rate, &ps) != 0) { return 1; }
+		const int rc = capture_mode(&ps, &plan, window_coefs, cap_env, dev_rate, dev_query, channel, gain_str, antenna,
+		                            filename, ppm, direct_sampling, offset_tuning, tuner_sleep_usec, tuner_retry_max,
+		                            interval, single, exit_after);
+		rxb200_power_mix_destroy(ps.pm);
 		return rc;
 	}
 	rxb200_power_group *grp = NULL;

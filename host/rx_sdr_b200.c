@@ -16,6 +16,12 @@
  * run stops; without it every output is written until the stream ends.  '-' as the filename, -I other than CS16, a
  * frequency given twice and a plan above the cap (the message names the rate needed) or, for the raster, above 4096 bins
  * exit 1 before the device is opened, and no file is created.
+ *
+ * RXB200_DEVICE_RATE=<Hz> with capture mode: the device runs at that rate instead of R.  The plan is the _at planner's
+ * (its decimation leaves the resampler's guard band, and a plan above the device rate exits 1 before the device is
+ * opened); the device is asked for R_dev, and the rate it reports is what the plan and the resampler
+ * (rxb200_plan_resample, rxb200_sdr_mix_set_device_rate) start from, so every read goes to the handle at the device's
+ * rate and the files hold the same channels, resampled to R on the GPU.
  */
 #include <limits.h>
 #include <signal.h>
@@ -58,7 +64,9 @@ static void usage(void)
 		"\tfilename (a '-' dumps samples to stdout)\n\n"
 		"environment: RXB200_CAPTURE_RATE=max_Hz records every -f channel from one capture of at most max_Hz samples/s,\n"
 		"each to filename.<frequency>; RXB200_CAPTURE_STAGES=2 plans that capture in two stages, and\n"
-		"RXB200_CAPTURE_STAGES=raster as one raster of bins (channels on a common grid, at most 4096 bins).\n");
+		"RXB200_CAPTURE_STAGES=raster as one raster of bins (channels on a common grid, at most 4096 bins);\n"
+		"RXB200_DEVICE_RATE=Hz (with capture mode) runs the device at that rate and resamples its stream to the\n"
+		"capture's rate on the GPU.\n");
 	exit(1);
 }
 
@@ -191,7 +199,7 @@ static int plain_mode(const struct opts *o)
 	return rc;
 }
 
-static int capture_mode(const struct opts *o, const char *cap_env)
+static int capture_mode(const struct opts *o, const char *cap_env, long long dev_rate)
 {
 	const int K = o->n_freqs;
 	if (same(o->filename, "-")) { fprintf(stderr, "Capture mode (RXB200_CAPTURE_RATE) writes one file per channel, not to '-'.\n"); return 1; }
@@ -209,17 +217,33 @@ static int capture_mode(const struct opts *o, const char *cap_env)
 	int chans[MAX_FREQS];
 	for (int i = 0; i < K; i++) { tuned[i] = o->freqs[i]; }
 	struct capture_plan pl;
-	if (capture_plan(kind, tuned, K, (int)o->rate, cap_env, rxb200_sdr_plan_capture, &pl, chans) != 0) { return 1; }
+	rxb200_resampler rs = {1, 1, 0, NULL, 15};
+	if (capture_plan(kind, tuned, K, (int)o->rate, cap_env, 1, dev_rate, &pl, chans) != 0) { return 1; }
 	fputs(pl.banner, stderr);
+	if (dev_rate && device_resampler(dev_rate, pl.capture_rate, pl.span, &rs) != 0) { return 1; }
 	SoapySDRDevice *dev = NULL;
 	SoapySDRStream *stream = NULL;
-	if (open_device(o, SOAPY_SDR_CS16, pl.capture_rate, (double)pl.centre_hz, &dev, &stream) != 0) { return 1; }
+	if (open_device(o, SOAPY_SDR_CS16, dev_rate ? dev_rate : pl.capture_rate, (double)pl.centre_hz, &dev, &stream) != 0) { return 1; }
+	const long long got = dev_rate ? sdr_device_rate(dev, o->channel, dev_rate) : 0;
+	if (got < 0) { sdr_close(dev, stream); return 1; }
+	if (got != dev_rate) {
+		/* the device runs at another rate than it was asked for: plan and resample from the rate it reports */
+		fprintf(stderr, "The device reports %lld Hz, not RXB200_DEVICE_RATE=%lld Hz: planning again.\n", got, dev_rate);
+		capture_plan_release(&pl);
+		free((void *)rs.taps);
+		rs.taps = NULL;
+		if (capture_plan(kind, tuned, K, (int)o->rate, cap_env, 1, got, &pl, chans) != 0) { sdr_close(dev, stream); return 1; }
+		fputs(pl.banner, stderr);
+		if (device_resampler(got, pl.capture_rate, pl.span, &rs) != 0) { sdr_close(dev, stream); return 1; }
+	}
 	rxb200_sdr_mix *h = NULL;
 	const int rc0 = kind == CAPTURE_RASTER ? rxb200_sdr_mix_create_raster(pl.n_bins, chans, K, &pl.ddc, 0, &h)
 	              : kind == CAPTURE_TWO_STAGE
 	                  ? rxb200_sdr_mix_create_two_stage(pl.capture_rate, pl.n_bins, chans, K, &pl.ddc, &pl.fine, 0, &h)
 	                  : rxb200_sdr_mix_create(pl.capture_rate, chans, K, &pl.ddc, 0, &h);
 	if (rc0 != RXB200_OK) { fprintf(stderr, "rxb200_sdr_mix_create: %s\n", rxb200_last_error()); return 1; }
+	if (rs.taps && rxb200_sdr_mix_set_device_rate(h, &rs) != RXB200_OK) { fprintf(stderr, "rxb200: %s\n", rxb200_last_error()); return 1; }
+	free((void *)rs.taps);
 	FILE *files[MAX_FREQS];
 	for (int k = 0; k < K; k++) {
 		char name[4096];
@@ -227,7 +251,10 @@ static int capture_mode(const struct opts *o, const char *cap_env)
 		if (!(files[k] = fopen(name, "wb"))) { fprintf(stderr, "Failed to open %s\n", name); return 1; }
 	}
 	const int fmt = out_kind(o->out_fmt);
-	const size_t E = out_bytes(o->out_fmt), stride = o->block / (size_t)pl.decim + 2;
+	/* each read's outputs per channel come from the handle (rxb200_sdr_mix_decimated_len counts device int16 once a
+	 * resampler is attached), and the output buffer grows to hold them */
+	const size_t E = out_bytes(o->out_fmt);
+	size_t stride = o->block / (size_t)pl.decim + 2;
 	int16_t *buf = malloc((size_t)o->block * 4);
 	unsigned char *out = malloc((size_t)K * stride * E);
 	unsigned long long written = 0;
@@ -235,7 +262,14 @@ static int capture_mode(const struct opts *o, const char *cap_env)
 	while (!g_stop && !(o->n_samples && written >= o->n_samples)) {
 		const int r = read_some(dev, stream, buf, o->block);
 		if (r < 0) { break; }
-		size_t n = 0;
+		size_t n = 0, need = 0;
+		rxb200_sdr_mix_decimated_len(h, 2 * (size_t)r, &need);
+		if (need > stride) {
+			unsigned char *grown = realloc(out, (size_t)K * need * E);
+			if (!grown) { fprintf(stderr, "Out of memory for %zu outputs per channel\n", need); rc = 1; break; }
+			out = grown;
+			stride = need;
+		}
 		if (rxb200_sdr_mix_process(h, buf, 2 * (size_t)r, fmt, out, (size_t)K * stride, stride, &n) != RXB200_OK) {
 			fprintf(stderr, "rxb200_sdr_mix_process: %s\n", rxb200_last_error());
 			rc = 1;
@@ -309,6 +343,9 @@ int main(int argc, char **argv)
 	signal(SIGTERM, on_signal);
 	signal(SIGPIPE, on_signal);
 	const char *cap_env = getenv("RXB200_CAPTURE_RATE");
-	if (cap_env && *cap_env && o.n_freqs >= 1) { return capture_mode(&o, cap_env); }
+	const int capture = cap_env && *cap_env && o.n_freqs >= 1;
+	const long long dev_rate = device_rate_env(capture, "capture mode (RXB200_CAPTURE_RATE with -f)");
+	if (dev_rate < 0) { return 1; }
+	if (capture) { return capture_mode(&o, cap_env, dev_rate); }
 	return plain_mode(&o);
 }

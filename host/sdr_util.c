@@ -1,4 +1,5 @@
 #include "sdr_util.h"
+#include <math.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -83,15 +84,16 @@ static rxb200_ddc lowpass(int M, int T, int S)
 	return (rxb200_ddc){M, T, taps, S};
 }
 
-int capture_plan(enum capture_kind kind, const int64_t *tuned, int n, int chain_rate, const char *cap_env,
-                 capture_planner single, struct capture_plan *p, int *chans)
+int capture_plan(enum capture_kind kind, const int64_t *tuned, int n, int chain_rate, const char *cap_env, int nco,
+                 long long device_rate, struct capture_plan *p, int *chans)
 {
-	const long long cap = atoll(cap_env);
+	const long long cap = atoll(cap_env), R_dev = device_rate;
 	int rc;
 	memset(p, 0, sizeof *p);
 	if (kind == CAPTURE_TWO_STAGE) {
 		rxb200_fm_two_stage_plan t;
-		rc = rxb200_fm_plan_capture_two_stage(tuned, n, chain_rate, cap, &t, chans);
+		rc = R_dev ? rxb200_fm_plan_capture_two_stage_at(tuned, n, chain_rate, cap, R_dev, &t, chans)
+		           : rxb200_fm_plan_capture_two_stage(tuned, n, chain_rate, cap, &t, chans);
 		if (rc == RXB200_OK) {
 			p->centre_hz = t.centre_hz; p->capture_rate = t.capture_rate; p->decim = t.coarse_decim * t.fine_decim;
 			p->n_bins = t.n_bins;
@@ -103,7 +105,8 @@ int capture_plan(enum capture_kind kind, const int64_t *tuned, int n, int chain_
 		}
 	} else if (kind == CAPTURE_RASTER) {
 		rxb200_fm_raster_plan r;
-		rc = rxb200_fm_plan_capture_raster(tuned, n, chain_rate, cap, &r, chans);
+		rc = R_dev ? rxb200_fm_plan_capture_raster_at(tuned, n, chain_rate, cap, R_dev, &r, chans)
+		           : rxb200_fm_plan_capture_raster(tuned, n, chain_rate, cap, &r, chans);
 		if (rc == RXB200_OK) {
 			p->centre_hz = r.centre_hz; p->capture_rate = r.capture_rate; p->decim = r.decim; p->n_bins = r.n_bins;
 			p->ddc = lowpass(r.decim, r.n_taps, r.shift);
@@ -112,7 +115,10 @@ int capture_plan(enum capture_kind kind, const int64_t *tuned, int n, int chain_
 		}
 	} else {
 		rxb200_fm_capture_plan s;
-		rc = single(tuned, n, chain_rate, cap, &s, chans);
+		rc = nco ? (R_dev ? rxb200_sdr_plan_capture_at(tuned, n, chain_rate, cap, R_dev, &s, chans)
+		                  : rxb200_sdr_plan_capture(tuned, n, chain_rate, cap, &s, chans))
+		         : (R_dev ? rxb200_fm_plan_capture_at(tuned, n, chain_rate, cap, R_dev, &s, chans)
+		                  : rxb200_fm_plan_capture(tuned, n, chain_rate, cap, &s, chans));
 		if (rc == RXB200_OK) {
 			p->centre_hz = s.centre_hz; p->capture_rate = s.capture_rate; p->decim = s.decim;
 			p->ddc = lowpass(s.decim, s.n_taps, 15);
@@ -124,6 +130,12 @@ int capture_plan(enum capture_kind kind, const int64_t *tuned, int n, int chain_
 		fprintf(stderr, "Capture mode: %s (RXB200_CAPTURE_RATE=%s).\n", rxb200_last_error(), cap_env);
 		return 1;
 	}
+	long long A = 0;
+	for (int k = 0; k < n; k++) {
+		const long long o = (long long)(tuned[k] - p->centre_hz);
+		if ((o < 0 ? -o : o) > A) { A = o < 0 ? -o : o; }
+	}
+	p->span = 2 * A + chain_rate;
 	return 0;
 }
 
@@ -131,4 +143,55 @@ void capture_plan_release(struct capture_plan *p)
 {
 	free((void *)p->ddc.taps);
 	free((void *)p->fine.taps);
+}
+
+long long device_rate_env(int allowed, const char *needs)
+{
+	const char *v = getenv("RXB200_DEVICE_RATE");
+	if (!v) { return 0; }
+	if (!allowed) { fprintf(stderr, "RXB200_DEVICE_RATE needs %s.\n", needs); return -1; }
+	char *e = NULL;
+	const long long r = strtoll(v, &e, 10);
+	if (e == v || *e || r < 1 || r > 2147483647LL) {
+		fprintf(stderr, "RXB200_DEVICE_RATE=%s is not a rate in [1, 2^31 - 1] Hz.\n", v);
+		return -1;
+	}
+	return r;
+}
+
+long long sdr_device_rate(SoapySDRDevice *dev, size_t channel, long long rate)
+{
+	SoapySDRDevice_setSampleRate(dev, SOAPY_SDR_RX, channel, (double)rate);
+	const double got = SoapySDRDevice_getSampleRate(dev, SOAPY_SDR_RX, channel);
+	if (!(got >= 0.5 && got < 2147483647.5)) {
+		fprintf(stderr, "The device reports a sample rate of %.0f Hz after RXB200_DEVICE_RATE=%lld asked for it: not a "
+		        "rate in [1, 2^31 - 1] Hz, so its samples cannot be resampled.\n", got, rate);
+		return -1;
+	}
+	return llround(got);
+}
+
+int device_resampler(long long device_rate, long long rate, long long span, rxb200_resampler *rs)
+{
+	if (rxb200_plan_resample(device_rate, rate, span, rs) != RXB200_OK) {
+		fprintf(stderr, "Device rate: %s (RXB200_DEVICE_RATE=%lld).\n", rxb200_last_error(), device_rate);
+		return 1;
+	}
+	if (rs->up == 1 && rs->down == 1) {
+		fprintf(stderr, "Device rate: %lld Hz, the capture rate: no resampling needed\n", device_rate);
+		return 0;
+	}
+	int32_t *taps = (int32_t *)malloc(sizeof(int32_t) * (size_t)rs->up * (size_t)rs->taps_per_phase);
+	rxb200_resample_lowpass(rs->up, rs->down, rs->taps_per_phase, taps);
+	rs->taps = taps;
+	fprintf(stderr, "Device rate: %lld Hz, resampled by %d/%d with %d taps per phase to %lld Hz\n", device_rate, rs->up,
+	        rs->down, rs->taps_per_phase, rate);
+	return 0;
+}
+
+size_t resample_out_count(int up, int down, unsigned long long n0, size_t c)
+{
+	typedef unsigned __int128 u128;
+	const u128 L = (u128)up, N = (u128)down;
+	return (size_t)((((u128)n0 + c) * L + N - 1) / N - ((u128)n0 * L + N - 1) / N);
 }

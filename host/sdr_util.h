@@ -21,22 +21,37 @@ void sdr_set_gain(SoapySDRDevice *dev, size_t channel, const char *gain_str);
 
 /* Capture mode (RXB200_CAPTURE_RATE): every channel from one capture, through a front stage of one of three kinds. */
 enum capture_kind { CAPTURE_SINGLE, CAPTURE_RASTER, CAPTURE_TWO_STAGE };
-typedef int (*capture_planner)(const int64_t *, int, int, long long, rxb200_fm_capture_plan *, int *);
 struct capture_plan {
 	int64_t centre_hz;     /* fc */
 	int capture_rate;      /* R */
 	int decim;             /* the total decimation: M, or M1 M2 for two stages */
 	int n_bins;            /* K (raster, two stages) */
+	long long span;        /* 2 A + c: the channels' span around the centre, A the largest |t_k - fc| */
 	rxb200_ddc ddc;        /* the filter, the coarse one for two stages */
 	rxb200_ddc fine;       /* two stages: the fine filter */
 	char banner[256];      /* the "Capture mode: ..." line the shell prints */
 };
 /* The plan of kind for the n tuned frequencies at chain rate chain_rate under the cap cap_env (RXB200_CAPTURE_RATE's
- * value): single, the plan of `single` (rxb200_fm_plan_capture or rxb200_sdr_plan_capture); raster,
- * rxb200_fm_plan_capture_raster's; two stages, rxb200_fm_plan_capture_two_stage's.  chans receives the n offsets (the
- * bins for a raster).  The filters' taps are rxb200_ddc_lowpass's, freed by capture_plan_release.  A refused plan is
- * reported on stderr and returns nonzero, with nothing to release. */
-int capture_plan(enum capture_kind kind, const int64_t *tuned, int n, int chain_rate, const char *cap_env,
-                 capture_planner single, struct capture_plan *p, int *chans);
+ * value): single, rxb200_sdr_plan_capture's when nco (rx_sdr mixes with the NCO) else rxb200_fm_plan_capture's;
+ * raster, rxb200_fm_plan_capture_raster's; two stages, rxb200_fm_plan_capture_two_stage's; each through its _at
+ * planner when device_rate is not 0.  chans receives the n offsets (the bins for a raster).  The filters' taps are
+ * rxb200_ddc_lowpass's, freed by capture_plan_release.  A refused plan is reported on stderr and returns nonzero, with
+ * nothing to release. */
+int capture_plan(enum capture_kind kind, const int64_t *tuned, int n, int chain_rate, const char *cap_env, int nco,
+                 long long device_rate, struct capture_plan *p, int *chans);
 void capture_plan_release(struct capture_plan *p);
+
+/* Capture at the device's own rate (RXB200_DEVICE_RATE, DESIGN.md section 4.7).
+ * device_rate_env: the variable's value, 0 when it is unset; -1, reported on stderr, when it is set but `allowed` is 0
+ * (none of the variables named by `needs` is set) or it is not a whole number of Hz in [1, 2^31 - 1]. */
+long long device_rate_env(int allowed, const char *needs);
+/* setSampleRate(rate), then the rate the device reports, rounded to whole Hz; -1, reported on stderr, when that is not
+ * a rate in [1, 2^31 - 1] Hz (a driver that does not report its rate returns 0) */
+long long sdr_device_rate(SoapySDRDevice *dev, size_t channel, long long rate);
+/* The resampler from device_rate to a plan's rate for channels spanning span Hz (rxb200_plan_resample), its taps
+ * rxb200_resample_lowpass's on the heap (free rs->taps; NULL when L = N = 1, no resampler needed), and the banner line
+ * "Device rate: ...".  Nonzero, reported on stderr, when the span leaves no room for the resampler. */
+int device_resampler(long long device_rate, long long rate, long long span, rxb200_resampler *rs);
+/* the capture samples the device samples [n0, n0 + c) emit through an L/N resampler */
+size_t resample_out_count(int up, int down, unsigned long long n0, size_t c);
 #endif

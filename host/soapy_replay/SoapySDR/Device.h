@@ -78,6 +78,7 @@ int SoapySDRDevice_setFrequency(SoapySDRDevice *device, const int direction, con
 double SoapySDRDevice_getFrequency(const SoapySDRDevice *device, const int direction, const size_t channel);
 int SoapySDRDevice_setFrequencyCorrection(SoapySDRDevice *device, const int direction, const size_t channel, const double value);
 int SoapySDRDevice_setSampleRate(SoapySDRDevice *device, const int direction, const size_t channel, const double rate);
+double SoapySDRDevice_getSampleRate(const SoapySDRDevice *device, const int direction, const size_t channel);
 int SoapySDRDevice_setBandwidth(SoapySDRDevice *device, const int direction, const size_t channel, const double bw);
 double SoapySDRDevice_getBandwidth(const SoapySDRDevice *device, const int direction, const size_t channel);
 

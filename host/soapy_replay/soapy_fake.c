@@ -7,13 +7,15 @@
  *      compiled against host/soapy_replay and linked with this file so every symbol
  *      resolves; the harness feeds samples from memory (soapy_fake_set_memory).
  *   2. the drop-in host shells (host/rx_fm_b200, host/rx_power_b200) run hardware-free
- *      with `-d driver=file,path=capture.cs16[,loop=1][,reads=a:b:c]`; reads= caps successive reads at a, b, c, a, ...
- *      complex elements, the way a device that reads in packets returns them.
+ *      with `-d driver=file,path=capture.cs16[,loop=1][,reads=a:b:c][,rate=Hz]`; reads= caps successive reads at a, b, c, a, ...
+ *      complex elements, the way a device that reads in packets returns them; rate=<Hz> models a device that runs only
+ *      at that rate: setSampleRate records the request, getSampleRate returns rate and listSampleRates {rate}.  Without
+ *      it getSampleRate returns the last request (a device that honours any rate).
  *
  * Behaviour that matters: readStream (copies the next numElems CS16 complex elements,
  * returns the count, SOAPY_SDR_TIMEOUT... never; returns -2 STREAM_ERROR at end of data so
  * the reference's dongle thread terminates), set/getFrequency (remembers the last value so
- * rx_power's retune() logic runs as on hardware), formatToSize, getNumChannels.
+ * rx_power's retune() logic runs as on hardware), set/getSampleRate, formatToSize, getNumChannels.
  * Everything else is a successful no-op.
  */
 #include <stdio.h>
@@ -32,7 +34,8 @@ struct SoapySDRDevice {
 	int loop;
 	int owns_mem;
 	double freq;
-	double rate;
+	double rate;            /* the last setSampleRate request */
+	double fixed_rate;      /* rate=: the only rate the device runs at; 0: any rate it is asked for */
 	double bw;
 	long long reads;        /* number of readStream calls served */
 	size_t read_len[64];    /* reads=a:b:c: a read returns at most these many complex elements, in turn (a device reading in packets) */
@@ -141,6 +144,12 @@ SoapySDRDevice *SoapySDRDevice_makeStrArgs(const char *args)
 {
 	char v[1024];
 	g_dev.freq = 0; g_dev.rate = 0; g_dev.bw = 0;
+	g_dev.fixed_rate = 0.0;
+	if (args && kw_find(args, "rate", v, sizeof v)) {
+		char *e = NULL;
+		g_dev.fixed_rate = strtod(v, &e);
+		if (e == v || *e || !(g_dev.fixed_rate > 0)) { g_err = "fake: rate= takes a positive rate in Hz"; return NULL; }
+	}
 	if (args && kw_find(args, "path", v, sizeof v)) {
 		if (load_file(v) != 0) { return NULL; }
 	}
@@ -215,7 +224,15 @@ static char **empty_list(size_t *length) { if (length) { *length = 0; } return N
 char **SoapySDRDevice_listAntennas(const SoapySDRDevice *d, const int dir, const size_t ch, size_t *length) { (void)d; (void)dir; (void)ch; return empty_list(length); }
 char **SoapySDRDevice_listGains(const SoapySDRDevice *d, const int dir, const size_t ch, size_t *length) { (void)d; (void)dir; (void)ch; return empty_list(length); }
 char **SoapySDRDevice_listFrequencies(const SoapySDRDevice *d, const int dir, const size_t ch, size_t *length) { (void)d; (void)dir; (void)ch; return empty_list(length); }
-double *SoapySDRDevice_listSampleRates(const SoapySDRDevice *d, const int dir, const size_t ch, size_t *length) { (void)d; (void)dir; (void)ch; if (length) { *length = 0; } return NULL; }
+double *SoapySDRDevice_listSampleRates(const SoapySDRDevice *d, const int dir, const size_t ch, size_t *length)
+{
+	(void)dir; (void)ch;
+	if (!d || d->fixed_rate <= 0) { if (length) { *length = 0; } return NULL; }
+	double *r = (double *)malloc(sizeof(double));
+	r[0] = d->fixed_rate;
+	if (length) { *length = 1; }
+	return r;
+}
 double *SoapySDRDevice_listBandwidths(const SoapySDRDevice *d, const int dir, const size_t ch, size_t *length) { (void)d; (void)dir; (void)ch; if (length) { *length = 0; } return NULL; }
 
 int SoapySDRDevice_setGainMode(SoapySDRDevice *d, const int dir, const size_t ch, const bool a) { (void)d; (void)dir; (void)ch; (void)a; return 0; }
@@ -227,6 +244,8 @@ int SoapySDRDevice_setFrequency(SoapySDRDevice *d, const int dir, const size_t c
 double SoapySDRDevice_getFrequency(const SoapySDRDevice *d, const int dir, const size_t ch) { (void)dir; (void)ch; return d ? d->freq : 0.0; }
 int SoapySDRDevice_setFrequencyCorrection(SoapySDRDevice *d, const int dir, const size_t ch, const double v) { (void)d; (void)dir; (void)ch; (void)v; return 0; }
 int SoapySDRDevice_setSampleRate(SoapySDRDevice *d, const int dir, const size_t ch, const double r) { (void)dir; (void)ch; if (d) { d->rate = r; } return 0; }
+double SoapySDRDevice_getSampleRate(const SoapySDRDevice *d, const int dir, const size_t ch)
+{ (void)dir; (void)ch; return !d ? 0.0 : d->fixed_rate > 0 ? d->fixed_rate : d->rate; }
 int SoapySDRDevice_setBandwidth(SoapySDRDevice *d, const int dir, const size_t ch, const double bw) { (void)dir; (void)ch; if (d) { d->bw = bw; } return 0; }
 double SoapySDRDevice_getBandwidth(const SoapySDRDevice *d, const int dir, const size_t ch) { (void)dir; (void)ch; return d ? d->bw : 0.0; }
 

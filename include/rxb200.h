@@ -1009,7 +1009,8 @@ int rxb200_resample_in_len(int up, int down, unsigned long long n0, size_t n_out
  *   rxb200_sdr_mix: _decimated_len takes device int16; a host call stages device samples in groups whose device-rate
  *     upload, resampled capture and output rows together fit RXB200_SDR_MIX_SCRATCH_BYTES;
  *   rxb200_power_mix: a call must resample to whole passes (else RXB200_EUNSUPPORTED, and nothing changes); bursts,
- *     capture-rate captures of their own, are refused (RXB200_EUNSUPPORTED);
+ *     capture-rate captures of their own, are refused (RXB200_EUNSUPPORTED): device-rate bursts take
+ *     rxb200_power_mix_set_burst_device_rate instead;
  *   every handle: reset clears the resampler's count and history and keeps it attached; a refused call changes nothing;
  *     _kernel_ms includes resample_kernel; an odd n_int16 gets the code the handle gives it without a resampler
  *     (RXB200_EUNSUPPORTED for rx_fm and rx_power, RXB200_EINVAL for rx_sdr).
@@ -1051,6 +1052,44 @@ int rxb200_fm_plan_capture_raster_at(const int64_t *tuned_hz /* n_channels */, i
 int rxb200_sdr_plan_capture_at(const int64_t *tuned_hz /* n_channels */, int n_channels, int sample_rate,
                                long long max_capture_rate, long long device_rate, rxb200_fm_capture_plan *out,
                                int *offsets_hz /* n_channels */);
+
+/* ---- rx_power plans at a device rate (DESIGN.md section 4.7)
+ * The capture mode's plan, with r = plan->rate, s = freq_step, F0 = first_freq and n = n_hops: the centre
+ * fc = F0 + floor((n - 1) s / 2), hop i's offset f_i = F0 + i s - fc, span = 2 max |f_i|, M = ceil((span + r) / r),
+ * R = M r and T = min(32 M + 1, 8191), in out (centre_hz, decim, capture_rate, n_taps).  Refused (RXB200_EINVAL):
+ * R > max_capture_rate, R > 2^31 - 1 or M > 4096, the message "the span needs a capture rate of R Hz"; a NULL plan or
+ * out, n_hops < 1, rate < 1 or freq_step < 0.  offsets_hz (n_hops ints) may be NULL.  Pure host arithmetic. */
+int rxb200_power_plan_capture(const rxb200_power_plan *plan, long long max_capture_rate, rxb200_fm_capture_plan *out,
+                              int *offsets_hz /* n_hops, may be NULL */);
+/* The same at a device rate R_dev, with the guard band G = ceil(R_dev / 32) of rxb200_plan_resample in the decimation
+ * floor, M = ceil((span + r + G) / r), so rxb200_plan_resample(R_dev, R, span + r) fits whenever R <= R_dev.
+ * Refusals: RXB200_EINVAL for R_dev outside [1, 2^31 - 1], first; then those of rxb200_power_plan_capture; then
+ * RXB200_EUNSUPPORTED for R > R_dev (the message names R and R_dev). */
+int rxb200_power_plan_capture_at(const rxb200_power_plan *plan, long long max_capture_rate, long long device_rate,
+                                 rxb200_fm_capture_plan *out, int *offsets_hz /* n_hops, may be NULL */);
+/* The tiling of rxb200_power_plan_tiles at a device rate R_dev: Mcap = min(4096, floor(min(max_capture_rate, R_dev,
+ * 2^31 - 1) / r)) and Mreq(k) = ceil((2 max(c(k), (k - 1) s - c(k)) + r + G) / r), G = ceil(R_dev / 32); the rest of
+ * that rule unchanged.  Tiles shrink until each fits: no tile runs above R_dev, and rxb200_plan_resample(R_dev, R,
+ * 2 max(c, (len - 1) s - c) + r) fits every tile of len hops.  Refusals (RXB200_EINVAL): R_dev outside [1, 2^31 - 1],
+ * first; those of rxb200_power_plan_tiles; and Mreq(1) > Mcap, a device too slow for a tile of one hop. */
+int rxb200_power_plan_tiles_at(const rxb200_power_plan *plan, long long max_capture_rate, long long device_rate,
+                               rxb200_power_tiling *out, int *offsets_hz /* n_hops, may be NULL */);
+/* Bursts at a device rate.  rxb200_power_mix_set_burst_device_rate attaches a resampler (L, N, J taps per phase) for
+ * bursts only, right after create or reset, on a handle without rxb200_power_mix_set_device_rate's resampler (the two
+ * exclude each other; RXB200_EINVAL otherwise, then the refusals of rxb200_resample_create; the taps are copied).
+ * After it, rxb200_power_mix_accumulate_burst and _accumulate_burst_device take DEVICE-rate bursts; the stream entries
+ * (_accumulate, _accumulate_device) still take capture-rate samples, as before.
+ * The burst rule.  A burst's capture is the stateless resampler rule over the burst's device samples, n0 = 0 with zeros
+ * before the burst.  Its first E = ceil((J - 1) L / N) outputs, those whose window reaches before the burst, are
+ * dropped, so no zeros enter; the remaining outputs must be exactly a capture-rate burst of the rule above, the lead G
+ * plus P >= 1 whole passes (E + G + P M buf_len / 2 outputs), else RXB200_EUNSUPPORTED and nothing changes.  So the
+ * call accumulates what rxb200_resample_device(rs, 0, burst) followed, from output E on, by the capture-rate burst
+ * call would.  A burst still neither reads nor moves the handle's sample count or filter history. */
+int rxb200_power_mix_set_burst_device_rate(rxb200_power_mix *m, const rxb200_resampler *rs);
+/* *n_int16: the device int16 of one burst of `passes` passes: 2 rxb200_resample_in_len(L, N, 0, E + G + passes M
+ * buf_len / 2), exact when L <= N (the planners only make such resamplers); on a handle without a burst device rate,
+ * the capture-rate burst 2 G + passes M buf_len.  RXB200_EINVAL for a NULL argument or passes < 1. */
+int rxb200_power_mix_burst_in_len(const rxb200_power_mix *m, int passes, size_t *n_int16);
 
 #ifdef __cplusplus
 }

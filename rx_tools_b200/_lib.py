@@ -133,6 +133,8 @@ SYMBOLS = [
     "rxb200_resample_in_len", "rxb200_fm_plan_capture_at", "rxb200_fm_plan_capture_two_stage_at",
     "rxb200_fm_plan_capture_raster_at", "rxb200_sdr_plan_capture_at",
     "rxb200_fm_mix_set_device_rate", "rxb200_sdr_mix_set_device_rate", "rxb200_power_mix_set_device_rate",
+    "rxb200_power_plan_capture", "rxb200_power_plan_capture_at", "rxb200_power_plan_tiles_at",
+    "rxb200_power_mix_set_burst_device_rate", "rxb200_power_mix_burst_in_len",
 ]
 
 _lib = None
@@ -332,6 +334,13 @@ def lib() -> C.CDLL:
     L.rxb200_fm_mix_set_device_rate.argtypes = [C.c_void_p, pr]
     L.rxb200_sdr_mix_set_device_rate.argtypes = [C.c_void_p, pr]
     L.rxb200_power_mix_set_device_rate.argtypes = [C.c_void_p, pr]
+    L.rxb200_power_plan_capture.argtypes = [C.POINTER(PowerPlanC), C.c_longlong, C.POINTER(FmCapturePlanC), pint]
+    L.rxb200_power_plan_capture_at.argtypes = [C.POINTER(PowerPlanC), C.c_longlong, C.c_longlong,
+                                               C.POINTER(FmCapturePlanC), pint]
+    L.rxb200_power_plan_tiles_at.argtypes = [C.POINTER(PowerPlanC), C.c_longlong, C.c_longlong,
+                                             C.POINTER(PowerTilingC), pint]
+    L.rxb200_power_mix_set_burst_device_rate.argtypes = [C.c_void_p, pr]
+    L.rxb200_power_mix_burst_in_len.argtypes = [C.c_void_p, C.c_int, C.POINTER(sz)]
     _lib = L
     return L
 

@@ -450,29 +450,46 @@ extern "C" int rxb200_resample_in_len(int up, int down, unsigned long long n0, s
 // The tiling of a sweep wider than one capture (include/rxb200.h, "wide sweeps in tiles"): c(k) is the centre of a run
 // of k hops from its first hop, Mreq(k) the decimation a capture centred there needs.
 static long long tile_centre(long long k, long long s) { return (k - 1) * s / 2; }
-static long long tile_decim(long long k, long long s, long long r)
+// G: the guard band of a device rate (0 without one), which the decimation floor leaves
+static long long tile_decim(long long k, long long s, long long r, long long G)
 {
 	const long long c = tile_centre(k, s), half = std::max(c, (k - 1) * s - c);
-	return (2 * half + r + r - 1) / r;
+	return (2 * half + r + G + r - 1) / r;
 }
 
-extern "C" int rxb200_power_plan_tiles(const rxb200_power_plan *plan, long long max_capture_rate,
-                                       rxb200_power_tiling *out, int *offsets_hz)
+// a plan the rx_power planners take
+static int power_plan_check(const rxb200_power_plan *plan, const char *what)
 {
-	if (!plan || !out) { set_error("null argument"); return RXB200_EINVAL; }
 	const long long n = plan->params.n_hops, r = plan->rate, s = plan->freq_step;
 	if (n < 1 || r < 1 || s < 0) {
-		set_error("tiling: plan with n_hops %lld, rate %lld, freq_step %lld (need n_hops, rate >= 1, freq_step >= 0)", n, r, s);
+		set_error("%s: plan with n_hops %lld, rate %lld, freq_step %lld (need n_hops, rate >= 1, freq_step >= 0)", what, n, r, s);
 		return RXB200_EINVAL;
 	}
-	const long long mcap = std::min(4096ll, std::min(max_capture_rate, 2147483647ll) / r);
+	return RXB200_OK;
+}
+
+// rxb200_power_plan_tiles's rule; device_rate: 0, or the _at planner's checked device rate with its guard band G
+static int power_tiles(const rxb200_power_plan *plan, long long max_capture_rate, long long device_rate, long long G,
+                       rxb200_power_tiling *out, int *offsets_hz)
+{
+	if (!plan || !out) { set_error("null argument"); return RXB200_EINVAL; }
+	int rc = power_plan_check(plan, "tiling");
+	if (rc != RXB200_OK) { return rc; }
+	const long long n = plan->params.n_hops, r = plan->rate, s = plan->freq_step;
+	const long long top = device_rate ? std::min(max_capture_rate, device_rate) : max_capture_rate;
+	const long long mcap = std::min(4096ll, std::min(top, 2147483647ll) / r);
 	if (mcap < 1) {
-		set_error("tiling: a capture rate of at most %lld Hz is below the hop rate %lld Hz", max_capture_rate, r);
+		set_error("tiling: a capture rate of at most %lld Hz is below the hop rate %lld Hz", top, r);
+		return RXB200_EINVAL;
+	}
+	if (tile_decim(1, s, r, G) > mcap) {
+		set_error("tiling: one hop at %lld Hz with the guard band of a device at %lld Hz needs %lld Hz, above %lld Hz", r,
+		          device_rate, tile_decim(1, s, r, G) * r, mcap * r);
 		return RXB200_EINVAL;
 	}
 	long long hmax = 1;                                  // Mreq is non-decreasing in k
-	while (hmax < n && tile_decim(hmax + 1, s, r) <= mcap) { hmax++; }
-	const long long n_tiles = (n + hmax - 1) / hmax, h = (n + n_tiles - 1) / n_tiles, M = tile_decim(h, s, r);
+	while (hmax < n && tile_decim(hmax + 1, s, r, G) <= mcap) { hmax++; }
+	const long long n_tiles = (n + hmax - 1) / hmax, h = (n + n_tiles - 1) / n_tiles, M = tile_decim(h, s, r, G);
 	out->n_tiles = (int)n_tiles;
 	out->hops_per_tile = (int)h;
 	out->decim = (int)M;
@@ -485,6 +502,71 @@ extern "C" int rxb200_power_plan_tiles(const rxb200_power_plan *plan, long long 
 		}
 	}
 	return RXB200_OK;
+}
+
+extern "C" int rxb200_power_plan_tiles(const rxb200_power_plan *plan, long long max_capture_rate,
+                                       rxb200_power_tiling *out, int *offsets_hz)
+{
+	return power_tiles(plan, max_capture_rate, 0, 0, out, offsets_hz);
+}
+
+extern "C" int rxb200_power_plan_tiles_at(const rxb200_power_plan *plan, long long max_capture_rate,
+                                          long long device_rate, rxb200_power_tiling *out, int *offsets_hz)
+{
+	long long G = 0;
+	const int rc = device_guard(device_rate, &G);
+	if (rc != RXB200_OK) { return rc; }
+	return power_tiles(plan, max_capture_rate, device_rate, G, out, offsets_hz);
+}
+
+// The rx_power shell's capture mode (include/rxb200.h, "rx_power plans at a device rate"): the centre of the hops, each
+// hop's offset from it and the smallest M whose capture holds them all, with the guard band G of a device rate
+static int power_capture(const rxb200_power_plan *plan, long long max_capture_rate, long long device_rate, long long G,
+                         rxb200_fm_capture_plan *out, int *offsets_hz)
+{
+	if (!plan || !out) { set_error("null argument"); return RXB200_EINVAL; }
+	int rc = power_plan_check(plan, "capture plan");
+	if (rc != RXB200_OK) { return rc; }
+	const long long n = plan->params.n_hops, r = plan->rate, s = plan->freq_step;
+	const long long fc = plan->first_freq + (n - 1) * s / 2;
+	long long span = 0;
+	for (long long i = 0; i < n; i++) {
+		const long long f = plan->first_freq + i * s - fc;
+		span = std::max(span, 2 * std::llabs(f));
+	}
+	const long long M = (span + r + G + r - 1) / r, R = M * r;
+	if (R > max_capture_rate || R > 2147483647ll || M > 4096) {
+		// the rx_power shell appends ", above RXB200_CAPTURE_RATE=<cap>", its refusal since before this planner
+		set_error("the span needs a capture rate of %lld Hz", R);
+		return RXB200_EINVAL;
+	}
+	if (device_rate && R > device_rate) {
+		set_error("the hops need a capture rate of %lld Hz, above the device rate of %lld Hz", R, device_rate);
+		return RXB200_EUNSUPPORTED;
+	}
+	if (offsets_hz) {
+		for (long long i = 0; i < n; i++) { offsets_hz[i] = (int)(plan->first_freq + i * s - fc); }
+	}
+	out->centre_hz = fc;
+	out->decim = (int)M;
+	out->capture_rate = (int)R;
+	out->n_taps = (int)std::min(8191ll, 32 * M + 1);
+	return RXB200_OK;
+}
+
+extern "C" int rxb200_power_plan_capture(const rxb200_power_plan *plan, long long max_capture_rate,
+                                         rxb200_fm_capture_plan *out, int *offsets_hz)
+{
+	return power_capture(plan, max_capture_rate, 0, 0, out, offsets_hz);
+}
+
+extern "C" int rxb200_power_plan_capture_at(const rxb200_power_plan *plan, long long max_capture_rate,
+                                            long long device_rate, rxb200_fm_capture_plan *out, int *offsets_hz)
+{
+	long long G = 0;
+	const int rc = device_guard(device_rate, &G);
+	if (rc != RXB200_OK) { return rc; }
+	return power_capture(plan, max_capture_rate, device_rate, G, out, offsets_hz);
 }
 
 extern "C" int rxb200_power_tile(const rxb200_power_plan *plan, const rxb200_power_tiling *tl, int t,

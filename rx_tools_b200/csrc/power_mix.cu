@@ -63,6 +63,7 @@ struct rxb200_power_mix {
 	NcoBank nco;                                 // the shared NCO table and each hop's frequency word
 	unsigned long long pos = 0;                  // capture samples since create or reset (whole passes)
 	ResampleStage rs;                            // from the device rate, once attached
+	bool burst_rate = false;                     // rs resamples bursts only (set_burst_device_rate), statelessly
 	int16_t *d_cap = nullptr; size_t cap_cap = 0;     // host calls: the capture (int16 elements)
 	int16_t *d_bufs = nullptr; size_t bufs_cap = 0;   // the hop buffers of one group of passes, [P][he - hb][buf_len]
 	std::vector<cudaEvent_t> ev;                 // pairs around each DDC launch of the last call
@@ -134,10 +135,26 @@ extern "C" int rxb200_power_mix_set_device_rate(rxb200_power_mix *m, const rxb20
 	return m->rs.attach(rs);
 }
 
+extern "C" int rxb200_power_mix_set_burst_device_rate(rxb200_power_mix *m, const rxb200_resampler *rs)
+{
+	if (!m) { set_error("null argument"); return RXB200_EINVAL; }
+	if (m->pos != 0 || m->rs.on()) {
+		set_error("a burst device rate is set once, right after create or reset, on a handle without a device rate");
+		return RXB200_EINVAL;
+	}
+	RXB_CUDA(cudaSetDevice(m->device));
+	const int rc = m->rs.attach(rs);
+	if (rc == RXB200_OK) { m->burst_rate = true; }
+	return rc;
+}
+
 namespace {
 
 // G = M ceil((T - 1) / M): the lead of a burst, in complex samples
 size_t burst_lead(const DdcFilter &f) { return (size_t)f.M * (((size_t)f.T - 1 + (size_t)f.M - 1) / (size_t)f.M); }
+
+// E = ceil((J - 1) L / N): the outputs of a device-rate burst whose resampler window reaches before the burst
+size_t burst_skip(const ResampleStage &rs) { return (size_t)((rs.f.T - 1) * rs.L + rs.N - 1) / (size_t)rs.N; }
 
 // One call of any entry point: the passes of hops [hb, he) in groups of at most RXB200_POWER_MIX_SCRATCH_BYTES of hop
 // buffers, each group one DDC launch into the scratch buffer ([P][he - hb][buf_len]) and one accumulate of the member.
@@ -153,11 +170,17 @@ int power_mix_call(rxb200_power_mix *m, int hb, int he, const int16_t *cs16, siz
 		return RXB200_EINVAL;
 	}
 	if (device && ((uintptr_t)cs16 & 3u) != 0) { set_error("d_cs16 must be 4-byte aligned"); return RXB200_EINVAL; }
-	const bool rs = m->rs.on();
-	if (rs && burst) { set_error("a burst is a capture-rate capture: a handle with a device rate takes none"); return RXB200_EUNSUPPORTED; }
+	// rs: this call is resampled, a stream call on a handle with a device rate or a burst on one with a burst device
+	// rate; a burst is resampled statelessly, so its first `skip` outputs (E) are dropped
+	const bool rs = m->rs.on() && burst == m->burst_rate;
+	if (m->rs.on() && burst && !rs) { set_error("a burst is a capture-rate capture: a handle with a device rate takes none"); return RXB200_EUNSUPPORTED; }
 	if (rs && n_int16 % 2 != 0) { set_error("n_int16=%zu must be even", n_int16); return RXB200_EUNSUPPORTED; }
 	const size_t dev16 = n_int16;                  // with a resampler, the call's device int16; n_int16 its capture's
-	if (rs) { n_int16 = 2 * m->rs.out_len(dev16 / 2); }
+	const size_t skip = rs && burst ? burst_skip(m->rs) : 0;
+	if (rs) {
+		const size_t n_out = m->rs.out_len(dev16 / 2);
+		n_int16 = n_out > skip ? 2 * (n_out - skip) : 0;
+	}
 	const size_t M = (size_t)m->f.M, L = (size_t)m->buf_len, pass16 = M * L;
 	const size_t lead16 = burst ? 2 * burst_lead(m->f) : 0;
 	if (burst && (n_int16 < lead16 + pass16 || (n_int16 - lead16) % pass16 != 0)) {
@@ -196,8 +219,8 @@ int power_mix_call(rxb200_power_mix *m, int hb, int he, const int16_t *cs16, siz
 		if (rc != RXB200_OK) { return rc; }
 		RXB_CUDA(cudaEventRecord(m->ev[1], st));
 		m->n_ev++;
-		m->rs.commit(dev16 / 2);
-		src = reinterpret_cast<const int16_t *>(x);
+		if (!burst) { m->rs.commit(dev16 / 2); }    // a burst leaves the stage at count 0 with its zero history
+		src = reinterpret_cast<const int16_t *>(x + skip);
 	}
 	DdcFilter &f = m->f;
 	for (size_t p0 = 0; p0 < n_pass; p0 += group) {
@@ -259,6 +282,18 @@ extern "C" int rxb200_power_mix_accumulate_burst_device(rxb200_power_mix *m, int
                                                         const int16_t *d_cs16, size_t n_int16, int sync)
 {
 	return power_mix_call(m, hop_begin, hop_end, d_cs16, n_int16, true, sync, true);
+}
+
+extern "C" int rxb200_power_mix_burst_in_len(const rxb200_power_mix *m, int passes, size_t *n_int16)
+{
+	if (!m || !n_int16 || passes < 1) { set_error("burst_in_len needs a handle, n_int16 and passes >= 1"); return RXB200_EINVAL; }
+	const size_t capture = burst_lead(m->f) + (size_t)passes * (size_t)m->f.M * (size_t)m->buf_len / 2;
+	if (!m->burst_rate) { *n_int16 = 2 * capture; return RXB200_OK; }
+	size_t c = 0;
+	const int rc = rxb200_resample_in_len((int)m->rs.L, (int)m->rs.N, 0, burst_skip(m->rs) + capture, &c);
+	if (rc != RXB200_OK) { return rc; }
+	*n_int16 = 2 * c;
+	return RXB200_OK;
 }
 
 extern "C" int rxb200_power_mix_kernel_ms(rxb200_power_mix *m, float *ms)

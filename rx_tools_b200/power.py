@@ -251,6 +251,21 @@ class PowerMix(PowerScanner):
         rs, _t = _rs_c(up, down, taps, shift)
         _lib.check(_lib.lib().rxb200_power_mix_set_device_rate(self._m, C.byref(rs)))
 
+    def set_burst_device_rate(self, up: int, down: int, taps, shift: int = 15) -> None:
+        """Attach a resampler for bursts only, right after create or reset (``rxb200_power_mix_set_burst_device_rate``):
+        from then on every burst is device-rate CS16 (``burst_in_len``), resampled statelessly with its first
+        ceil((J - 1) L / N) outputs dropped; accumulate still takes capture-rate samples."""
+        from .resample import _rs_c
+        rs, _t = _rs_c(up, down, taps, shift)
+        _lib.check(_lib.lib().rxb200_power_mix_set_burst_device_rate(self._m, C.byref(rs)))
+
+    def burst_in_len(self, n_pass: int = 1) -> int:
+        """int16 of one burst of n_pass passes as the handle takes it (``rxb200_power_mix_burst_in_len``): device int16
+        with a burst device rate, else burst_int16(n_pass)."""
+        n = C.c_size_t(0)
+        _lib.check(_lib.lib().rxb200_power_mix_burst_in_len(self._m, int(n_pass), C.byref(n)))
+        return int(n.value)
+
     def kernel_ms(self) -> float:
         """Device time of the last call's DDC launches (ms)."""
         ms = C.c_float(0)
@@ -293,14 +308,37 @@ class Tiling:
     capture_rate: int
 
 
-def plan_tiles(plan: Plan, max_rate: int):
-    """The tiling of a sweep for captures of at most max_rate Hz (``rxb200_power_plan_tiles``): (Tiling, each tile's
-    (hop_begin, hop_end, centre_hz), each hop's offset from its tile's centre)."""
-    pc = _lib.PowerPlanC(plan.to_c(), plan.rate, plan.crop, plan.first_freq, plan.freq_step, plan.bin_size_hz)
+def _plan_c(plan: Plan) -> _lib.PowerPlanC:
+    return _lib.PowerPlanC(plan.to_c(), plan.rate, plan.crop, plan.first_freq, plan.freq_step, plan.bin_size_hz)
+
+
+def _power_plan_call(name: str, pc, max_rate: int, device_rate: Optional[int], out, offs) -> None:
+    """``name`` without a device rate, ``name_at`` (the guard band in the decimation floor) with one."""
+    args = [C.byref(pc), int(max_rate)]
+    if device_rate is not None:
+        name += "_at"
+        args.append(int(device_rate))
+    _lib.check(getattr(_lib.lib(), name)(*args, C.byref(out), offs.ctypes.data_as(C.POINTER(C.c_int))))
+
+
+def plan_capture(plan: Plan, max_rate: int, device_rate: Optional[int] = None):
+    """The rx_power shell's capture-mode plan (``rxb200_power_plan_capture``, or ``_at`` with a device_rate):
+    (fm.CapturePlan of the centre, M, R = M rate and T, each hop's offset from the centre)."""
+    from .fm import CapturePlan
+    out = _lib.FmCapturePlanC()
+    offs = np.zeros(plan.n_hops, dtype=np.int32)
+    _power_plan_call("rxb200_power_plan_capture", _plan_c(plan), max_rate, device_rate, out, offs)
+    return CapturePlan(int(out.centre_hz), out.decim, out.capture_rate, out.n_taps), [int(v) for v in offs]
+
+
+def plan_tiles(plan: Plan, max_rate: int, device_rate: Optional[int] = None):
+    """The tiling of a sweep for captures of at most max_rate Hz (``rxb200_power_plan_tiles``, or ``_at`` with a
+    device_rate, whose tiles shrink to fit it): (Tiling, each tile's (hop_begin, hop_end, centre_hz), each hop's offset
+    from its tile's centre)."""
+    pc = _plan_c(plan)
     tl = _lib.PowerTilingC()
     offs = np.zeros(plan.n_hops, dtype=np.int32)
-    _lib.check(_lib.lib().rxb200_power_plan_tiles(C.byref(pc), int(max_rate), C.byref(tl),
-                                                  offs.ctypes.data_as(C.POINTER(C.c_int))))
+    _power_plan_call("rxb200_power_plan_tiles", pc, max_rate, device_rate, tl, offs)
     tiles = []
     for t in range(tl.n_tiles):
         b, e, c = C.c_int(0), C.c_int(0), C.c_int64(0)
