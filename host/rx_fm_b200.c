@@ -22,6 +22,11 @@
  * opened), the device is asked for R_dev, and the rate it reports is what the plan and the resampler start from
  * (rxb200_plan_resample, rxb200_fm_mix_set_device_rate).  The reader then gathers blocks of exactly the device samples
  * that emit M * 131072 capture samples (rxb200_resample_in_len), so every chain read is still 131072 samples.
+ *
+ * RXB200_DEVICE_FORMAT=CS16|CS8|CU8|CS12 with capture mode: the stream is opened in that format, the reader gathers the
+ * same blocks of elements in it, and the handle widens each block to CS16 on the GPU (rxb200_fm_mix_set_input_format),
+ * so the files are those of the same run on the widened CS16 stream.  An unknown value, or the variable without capture
+ * mode, exits 1 before the device is opened.
  */
 #include <errno.h>
 #include <math.h>
@@ -108,6 +113,8 @@ static struct {
 	int rs_up, rs_down;                /* capture mode at a device rate: the resampler's L/N (0: none attached) */
 	size_t slot16;                     /* capture mode: int16 a raw slot holds, the most device int16 of a block */
 	unsigned long long dev_pos;        /* capture mode at a device rate: device samples handed on so far */
+	int in_fmt;                        /* capture mode: the device's format (RXB200_IN_*, RXB200_DEVICE_FORMAT) */
+	const char *in_name;               /* its SoapySDR name, the stream's format */
 	FILE *outs[MAX_FREQS];
 	Queue q_raw, q_pcm;
 	pthread_mutex_t hop_m;
@@ -129,7 +136,8 @@ static void usage(void)
 		"\ttuned once to their centre (one GPU), channel f to filename.f (no scanning, no -l needed; refuses '-', -L, -o);\n"
 		"\tRXB200_CAPTURE_STAGES=2 plans that capture in two stages, RXB200_CAPTURE_STAGES=raster as one raster of bins\n"
 		"\t(channels on a common grid, at most 4096 bins); RXB200_DEVICE_RATE=Hz runs the device at that rate and\n"
-		"\tresamples its stream to the capture's rate on the GPU\n");
+		"\tresamples its stream to the capture's rate on the GPU; RXB200_DEVICE_FORMAT=CS16|CS8|CU8|CS12 reads the\n"
+		"\tdevice in that format and widens it to CS16 on the GPU\n");
 	exit(1);
 }
 
@@ -195,12 +203,14 @@ static int capture_setup(const char *cap_env, long long dev_rate, int64_t *centr
 	if (dev_rate && device_resampler(dev_rate, pl.capture_rate, pl.span, &rs) != 0) { return 1; }
 	if (rs.taps) { rc = rxb200_fm_mix_set_device_rate(G.mix, &rs); }
 	free((void *)rs.taps);
+	if (rc == RXB200_OK && G.in_fmt != RXB200_IN_CS16) { rc = rxb200_fm_mix_set_input_format(G.mix, G.in_fmt); }
 	if (rc != RXB200_OK) { fprintf(stderr, "rxb200: %s\n", rxb200_last_error()); return 1; }
 	G.decim = pl.decim;
 	G.block16 = (size_t)pl.decim * 2 * CHUNK_COMPLEX;
 	G.rs_up = rs.taps ? rs.up : 0;
 	G.rs_down = rs.taps ? rs.down : 0;
 	/* a block of M * 131072 capture samples takes at most ceil(M * 131072 N / L) + 1 device samples */
+	/* (a slot holds slot16 int16, so at least that many elements of a narrower format) */
 	G.slot16 = G.rs_up ? 2 * (((size_t)pl.decim * CHUNK_COMPLEX * (size_t)G.rs_down + (size_t)G.rs_up - 1) / (size_t)G.rs_up + 1)
 	                   : G.block16;
 	G.stride = rxb200_fm_mix_max_output(G.mix, G.slot16, G.block16);
@@ -271,7 +281,7 @@ static void *block_reader_thread(void *arg)
 		size_t have = 0;
 		int r = 1;
 		while (have < want16) {
-			void *buffs[] = {s->data + have};
+			void *buffs[] = {(unsigned char *)s->data + have / 2 * device_format_bytes(G.in_fmt)};   /* have: int16 */
 			int flags = 0; long long t_ns = 0;
 			r = g_stop ? -1 : SoapySDRDevice_readStream(G.dev, G.stream, buffs, (want16 - have) / 2, &flags, &t_ns, 1000000);
 			if (r == SOAPY_SDR_OVERFLOW) { fprintf(stderr, "O"); fflush(stderr); continue; }
@@ -466,6 +476,8 @@ int main(int argc, char **argv)
 	G.filename = (argc <= optind) ? "-" : argv[optind];
 	const long long dev_rate = device_rate_env(cap_env != NULL, "capture mode (RXB200_CAPTURE_RATE)");
 	if (dev_rate < 0) { return 1; }
+	G.in_fmt = device_format_env(cap_env != NULL, "capture mode (RXB200_CAPTURE_RATE)", &G.in_name);
+	if (G.in_fmt < 0) { return 1; }
 	if (cap_env) {
 		/* capture mode: one file per channel, one read per block; the mixer puts each channel at DC */
 		const char *bad = !strcmp(G.filename, "-") ? "'-' as the filename (it writes one file per channel)"
@@ -502,7 +514,7 @@ int main(int argc, char **argv)
 		if (capture_setup(cap_env, dev_rate, &tune_freq, &tune_rate) != 0) { return 1; }
 	} else if (rxb200_fm_create(&G.der.params, 0, 1, &G.fm) != RXB200_OK) { fprintf(stderr, "rxb200: %s\n", rxb200_last_error()); return 1; }
 
-	if (sdr_open(G.dev_query, G.channel, &G.dev, &G.stream) != 0) {
+	if (sdr_open(G.dev_query, G.channel, G.in_name, &G.dev, &G.stream) != 0) {
 		fprintf(stderr, "Failed to open sdr device matching '%s'.\n", G.dev_query);
 		return 1;
 	}

@@ -28,6 +28,11 @@
  * passes of the device samples that emit one pass of M * buf_len int16 (rxb200_resample_in_len) into a handle with
  * rxb200_power_mix_set_device_rate; tile mode reads bursts of rxb200_power_mix_burst_in_len device int16 into a handle
  * with rxb200_power_mix_set_burst_device_rate.
+ *
+ * RXB200_DEVICE_FORMAT=CS16|CS8|CU8|CS12 with capture or tile mode: the stream is opened in that format, passes and
+ * bursts are gathered as the same counts of elements in it, and the handle widens them to CS16 on the GPU
+ * (rxb200_power_mix_set_input_format), so the CSV is that of the same run on the widened CS16 stream.  An unknown
+ * value, or the variable without capture or tile mode, exits 1 before the device is opened.
  */
 #include <math.h>
 #include <signal.h>
@@ -42,6 +47,8 @@
 #define BUFFER_DUMP 16384            /* elements flushed after a retune, src/rtl_power.c:71-72, :568 */
 
 static volatile sig_atomic_t g_stop = 0;
+static int g_in_fmt = RXB200_IN_CS16;            /* the device's format (RXB200_DEVICE_FORMAT), capture and tile mode */
+static const char *g_in_name = SOAPY_SDR_CS16;   /* its SoapySDR name, the stream's format */
 static void on_signal(int s) { (void)s; g_stop++; }
 
 static void usage(void)
@@ -60,7 +67,8 @@ static void usage(void)
 		"\tcapture of at most max_Hz samples/s, tuned once to the centre of the sweep (one GPU);\n"
 		"\tRXB200_TILE_RATE=max_Hz takes a wider sweep in tiles of hops, one retune and one burst of at most max_Hz\n"
 		"\tsamples/s per tile (one GPU); RXB200_DEVICE_RATE=Hz (with either) runs the device at that rate and resamples\n"
-		"\tits stream to the capture's rate on the GPU\n");
+		"\tits stream to the capture's rate on the GPU; RXB200_DEVICE_FORMAT=CS16|CS8|CU8|CS12 (with either) reads the\n"
+		"\tdevice in that format and widens it to CS16 on the GPU\n");
 	exit(1);
 }
 
@@ -106,7 +114,7 @@ static FILE *open_radio(const char *dev_query, size_t channel, const char *anten
                         int direct_sampling, int offset_tuning, const char *filename, SoapySDRDevice **devp,
                         SoapySDRStream **streamp)
 {
-	if (sdr_open(dev_query, channel, devp, streamp) != 0) { fprintf(stderr, "Failed to open sdr device matching '%s'.\n", dev_query); return NULL; }
+	if (sdr_open(dev_query, channel, g_in_name, devp, streamp) != 0) { fprintf(stderr, "Failed to open sdr device matching '%s'.\n", dev_query); return NULL; }
 	SoapySDRDevice *dev = *devp;
 	if (antenna && SoapySDRDevice_setAntenna(dev, SOAPY_SDR_RX, channel, antenna) != 0) { fprintf(stderr, "Failed to set antenna"); }
 	SoapySDRDevice_activateStream(dev, *streamp, 0, 0, 0);
@@ -195,6 +203,7 @@ static int power_setup(int tiles, const rxb200_power_plan *plan, const int *wind
 		if (!tiles) { ps->rs_up = rs.up; ps->rs_down = rs.down; }
 	}
 	free((void *)rs.taps);
+	if (rc == RXB200_OK && g_in_fmt != RXB200_IN_CS16) { rc = rxb200_power_mix_set_input_format(ps->pm, g_in_fmt); }
 	if (rc != RXB200_OK) { fprintf(stderr, "rxb200: %s\n", rxb200_last_error()); return 1; }
 	return 0;
 }
@@ -261,7 +270,7 @@ static int tile_mode(struct power_setup *ps, const rxb200_power_plan *plan, cons
 			}
 			size_t have = 0;
 			while (have < burst16 && !g_stop) {
-				void *bp[] = {burst + have};
+				void *bp[] = {(unsigned char *)burst + have / 2 * device_format_bytes(g_in_fmt)};   /* have: int16 */
 				int flags = 0; long long tn = 0;
 				const int r = SoapySDRDevice_readStream(dev, stream, bp, (burst16 - have) / 2, &flags, &tn, 1000000);
 				if (r < 0) { fprintf(stderr, "Error: reading stream %d\n", r); break; }    /* the burst is dropped */
@@ -340,7 +349,7 @@ static int capture_mode(struct power_setup *ps, const rxb200_power_plan *plan, c
 		size_t have = 0;
 		int fails = 0, dry = 0;
 		while (have < pass16 && !g_stop) {
-			void *bp[] = {pass + have};
+			void *bp[] = {(unsigned char *)pass + have / 2 * device_format_bytes(g_in_fmt)};   /* have: int16 */
 			int flags = 0; long long tn = 0;
 			const int r = SoapySDRDevice_readStream(dev, stream, bp, (pass16 - have) / 2, &flags, &tn, 1000000);
 			if (r < 0) {
@@ -442,6 +451,9 @@ int main(int argc, char **argv)
 	const char *cap_env = getenv("RXB200_CAPTURE_RATE"), *tile_env = getenv("RXB200_TILE_RATE");
 	const long long dev_rate = device_rate_env(cap_env || tile_env, "capture or tile mode (RXB200_CAPTURE_RATE or RXB200_TILE_RATE)");
 	if (dev_rate < 0) { return 1; }
+	g_in_fmt = device_format_env(cap_env || tile_env, "capture or tile mode (RXB200_CAPTURE_RATE or RXB200_TILE_RATE)",
+	                             &g_in_name);
+	if (g_in_fmt < 0) { return 1; }
 	if (tile_env) {
 		/* tile mode: the planner's tiles, each hop's offset from its tile's centre, one filter for every tile */
 		if (cap_env) { fprintf(stderr, "Tile mode (RXB200_TILE_RATE) and capture mode (RXB200_CAPTURE_RATE) exclude each other.\n"); return 1; }

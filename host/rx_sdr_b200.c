@@ -22,6 +22,12 @@
  * opened); the device is asked for R_dev, and the rate it reports is what the plan and the resampler
  * (rxb200_plan_resample, rxb200_sdr_mix_set_device_rate) start from, so every read goes to the handle at the device's
  * rate and the files hold the same channels, resampled to R on the GPU.
+ *
+ * RXB200_DEVICE_FORMAT=CS16|CS8|CU8|CS12 with capture mode: the stream is opened in that format, the read buffer holds
+ * -b elements of it, and the handle widens each read to CS16 on the GPU (rxb200_sdr_mix_set_input_format), so the
+ * files are those of the same run on the widened CS16 stream.  -I may be left out or name the same format; any other -I
+ * exits 1.  An unknown value, or the variable without capture mode, exits 1 before the device is opened.  Without the
+ * variable, -I other than CS16 keeps capture mode's refusal.
  */
 #include <limits.h>
 #include <signal.h>
@@ -66,7 +72,8 @@ static void usage(void)
 		"each to filename.<frequency>; RXB200_CAPTURE_STAGES=2 plans that capture in two stages, and\n"
 		"RXB200_CAPTURE_STAGES=raster as one raster of bins (channels on a common grid, at most 4096 bins);\n"
 		"RXB200_DEVICE_RATE=Hz (with capture mode) runs the device at that rate and resamples its stream to the\n"
-		"capture's rate on the GPU.\n");
+		"capture's rate on the GPU; RXB200_DEVICE_FORMAT=CS16|CS8|CU8|CS12 (with capture mode) reads the device in\n"
+		"that format and widens it to CS16 on the GPU.\n");
 	exit(1);
 }
 
@@ -105,6 +112,7 @@ static void write_settings(SoapySDRDevice *dev, const char *s)
 
 struct opts {
 	const char *query, *gain, *antenna, *settings, *filename, *in_fmt, *out_fmt;
+	int in_given;          /* -I was on the command line */
 	size_t channel;
 	int ppm, direct;
 	uint32_t rate, block, n_samples;
@@ -199,11 +207,16 @@ static int plain_mode(const struct opts *o)
 	return rc;
 }
 
-static int capture_mode(const struct opts *o, const char *cap_env, long long dev_rate)
+static int capture_mode(const struct opts *o, const char *cap_env, long long dev_rate, int dev_fmt, const char *dev_fmt_name)
 {
 	const int K = o->n_freqs;
 	if (same(o->filename, "-")) { fprintf(stderr, "Capture mode (RXB200_CAPTURE_RATE) writes one file per channel, not to '-'.\n"); return 1; }
-	if (!same(o->in_fmt, SOAPY_SDR_CS16)) { fprintf(stderr, "Capture mode (RXB200_CAPTURE_RATE) reads CS16, not %s.\n", o->in_fmt); return 1; }
+	if (!getenv("RXB200_DEVICE_FORMAT")) {
+		if (!same(o->in_fmt, SOAPY_SDR_CS16)) { fprintf(stderr, "Capture mode (RXB200_CAPTURE_RATE) reads CS16, not %s.\n", o->in_fmt); return 1; }
+	} else if (o->in_given && !same(o->in_fmt, dev_fmt_name)) {
+		fprintf(stderr, "Capture mode reads the device in RXB200_DEVICE_FORMAT=%s, not -I %s.\n", dev_fmt_name, o->in_fmt);
+		return 1;
+	}
 	for (int i = 0; i < K; i++) {
 		for (int j = 0; j < i; j++) {
 			if (o->freqs[i] == o->freqs[j]) { fprintf(stderr, "Capture mode (RXB200_CAPTURE_RATE): %u Hz is given twice.\n", o->freqs[i]); return 1; }
@@ -223,7 +236,7 @@ static int capture_mode(const struct opts *o, const char *cap_env, long long dev
 	if (dev_rate && device_resampler(dev_rate, pl.capture_rate, pl.span, &rs) != 0) { return 1; }
 	SoapySDRDevice *dev = NULL;
 	SoapySDRStream *stream = NULL;
-	if (open_device(o, SOAPY_SDR_CS16, dev_rate ? dev_rate : pl.capture_rate, (double)pl.centre_hz, &dev, &stream) != 0) { return 1; }
+	if (open_device(o, dev_fmt_name, dev_rate ? dev_rate : pl.capture_rate, (double)pl.centre_hz, &dev, &stream) != 0) { return 1; }
 	const long long got = dev_rate ? sdr_device_rate(dev, o->channel, dev_rate) : 0;
 	if (got < 0) { sdr_close(dev, stream); return 1; }
 	if (got != dev_rate) {
@@ -243,6 +256,7 @@ static int capture_mode(const struct opts *o, const char *cap_env, long long dev
 	                  : rxb200_sdr_mix_create(pl.capture_rate, chans, K, &pl.ddc, 0, &h);
 	if (rc0 != RXB200_OK) { fprintf(stderr, "rxb200_sdr_mix_create: %s\n", rxb200_last_error()); return 1; }
 	if (rs.taps && rxb200_sdr_mix_set_device_rate(h, &rs) != RXB200_OK) { fprintf(stderr, "rxb200: %s\n", rxb200_last_error()); return 1; }
+	if (dev_fmt != RXB200_IN_CS16 && rxb200_sdr_mix_set_input_format(h, dev_fmt) != RXB200_OK) { fprintf(stderr, "rxb200: %s\n", rxb200_last_error()); return 1; }
 	free((void *)rs.taps);
 	FILE *files[MAX_FREQS];
 	for (int k = 0; k < K; k++) {
@@ -255,7 +269,7 @@ static int capture_mode(const struct opts *o, const char *cap_env, long long dev
 	 * resampler is attached), and the output buffer grows to hold them */
 	const size_t E = out_bytes(o->out_fmt);
 	size_t stride = o->block / (size_t)pl.decim + 2;
-	int16_t *buf = malloc((size_t)o->block * 4);
+	int16_t *buf = malloc((size_t)o->block * device_format_bytes(dev_fmt));   /* -b elements of the device's format */
 	unsigned char *out = malloc((size_t)K * stride * E);
 	unsigned long long written = 0;
 	int rc = 0;
@@ -318,6 +332,7 @@ int main(int argc, char **argv)
 		case 'S': break;                            /* reads are synchronous either way */
 		case 'I':
 			if (!(o.in_fmt = format_of(optarg))) { fprintf(stderr, "Unsupported input format: %s\n", optarg); return 1; }
+			o.in_given = 1;
 			break;
 		case 'F':
 			if (!(o.out_fmt = format_of(optarg))) { fprintf(stderr, "Unsupported output format: %s\n", optarg); return 1; }
@@ -327,7 +342,10 @@ int main(int argc, char **argv)
 		default: usage();
 		}
 	}
-	if (!same(o.in_fmt, o.out_fmt) && !same(o.in_fmt, SOAPY_SDR_CS16) &&
+	/* capture mode with RXB200_DEVICE_FORMAT widens any -I on the GPU and checks -I against the variable itself */
+	const char *cap_env = getenv("RXB200_CAPTURE_RATE");
+	const int capture = cap_env && *cap_env && o.n_freqs >= 1;
+	if (!(capture && getenv("RXB200_DEVICE_FORMAT")) && !same(o.in_fmt, o.out_fmt) && !same(o.in_fmt, SOAPY_SDR_CS16) &&
 	    !(same(o.in_fmt, SOAPY_SDR_CS12) && same(o.out_fmt, SOAPY_SDR_CS16))) {
 		fprintf(stderr, "Unsupported input/output conversion: %s to %s\n", o.in_fmt, o.out_fmt);
 		return 1;
@@ -342,10 +360,11 @@ int main(int argc, char **argv)
 	signal(SIGINT, on_signal);
 	signal(SIGTERM, on_signal);
 	signal(SIGPIPE, on_signal);
-	const char *cap_env = getenv("RXB200_CAPTURE_RATE");
-	const int capture = cap_env && *cap_env && o.n_freqs >= 1;
 	const long long dev_rate = device_rate_env(capture, "capture mode (RXB200_CAPTURE_RATE with -f)");
 	if (dev_rate < 0) { return 1; }
-	if (capture) { return capture_mode(&o, cap_env, dev_rate); }
+	const char *dev_fmt_name = NULL;
+	const int dev_fmt = device_format_env(capture, "capture mode (RXB200_CAPTURE_RATE with -f)", &dev_fmt_name);
+	if (dev_fmt < 0) { return 1; }
+	if (capture) { return capture_mode(&o, cap_env, dev_rate, dev_fmt, dev_fmt_name); }
 	return plain_mode(&o);
 }

@@ -34,7 +34,7 @@ double parse_fraction(const char *s)
 	return with_suffix(s, "%", m);
 }
 
-int sdr_open(const char *query, size_t channel, SoapySDRDevice **dev, SoapySDRStream **stream)
+int sdr_open(const char *query, size_t channel, const char *format, SoapySDRDevice **dev, SoapySDRStream **stream)
 {
 	SoapySDRKwargs none = {0, NULL, NULL};
 	*dev = SoapySDRDevice_makeStrArgs(query ? query : "");
@@ -46,7 +46,7 @@ int sdr_open(const char *query, size_t channel, SoapySDRDevice **dev, SoapySDRSt
 		fprintf(stderr, "Invalid channel %d selected\n", (int)channel);
 		return -3;
 	}
-	*stream = SoapySDRDevice_setupStream(*dev, SOAPY_SDR_RX, SOAPY_SDR_CS16, &channel, 1, &none);
+	*stream = SoapySDRDevice_setupStream(*dev, SOAPY_SDR_RX, format, &channel, 1, &none);
 	if (!*stream) { fprintf(stderr, "SoapySDRDevice_setupStream failed: %s\n", SoapySDRDevice_lastError()); return -3; }
 	return 0;
 }
@@ -195,3 +195,19 @@ size_t resample_out_count(int up, int down, unsigned long long n0, size_t c)
 	const u128 L = (u128)up, N = (u128)down;
 	return (size_t)((((u128)n0 + c) * L + N - 1) / N - ((u128)n0 * L + N - 1) / N);
 }
+
+int device_format_env(int allowed, const char *needs, const char **name)
+{
+	static const char *names[] = {SOAPY_SDR_CS16, SOAPY_SDR_CS8, SOAPY_SDR_CU8, SOAPY_SDR_CS12};   /* RXB200_IN_* order */
+	const char *v = getenv("RXB200_DEVICE_FORMAT");
+	*name = SOAPY_SDR_CS16;
+	if (!v) { return RXB200_IN_CS16; }
+	if (!allowed) { fprintf(stderr, "RXB200_DEVICE_FORMAT needs %s.\n", needs); return -1; }
+	for (int f = RXB200_IN_CS16; f <= RXB200_IN_CS12; f++) {
+		if (!strcmp(v, names[f])) { *name = names[f]; return f; }
+	}
+	fprintf(stderr, "RXB200_DEVICE_FORMAT=%s is not one of CS16, CS8, CU8, CS12.\n", v);
+	return -1;
+}
+
+size_t device_format_bytes(int in_fmt) { return in_fmt == RXB200_IN_CS16 ? 4 : in_fmt == RXB200_IN_CS12 ? 3 : 2; }

@@ -13,8 +13,9 @@ double parse_scaled(const char *s);    /* 100M, 24k, 1.2G   (convenience.c:65-90
 double parse_seconds(const char *s);   /* 10s, 5m, 1h       (convenience.c:92-117) */
 double parse_fraction(const char *s);  /* 28.5% -> 0.285    (convenience.c:119-136) */
 
-/* makeStrArgs + CS16 RX stream on `channel`; prints like the reference's verbose_* helpers. Returns 0 on success. */
-int sdr_open(const char *query, size_t channel, SoapySDRDevice **dev, SoapySDRStream **stream);
+/* makeStrArgs + an RX stream of `format` (SOAPY_SDR_CS16 unless RXB200_DEVICE_FORMAT says otherwise) on `channel`;
+ * prints like the reference's verbose_* helpers. Returns 0 on success. */
+int sdr_open(const char *query, size_t channel, const char *format, SoapySDRDevice **dev, SoapySDRStream **stream);
 void sdr_close(SoapySDRDevice *dev, SoapySDRStream *stream);
 /* gain: NULL = automatic, "30" overall, or "LNA=20,VGA=10" per element */
 void sdr_set_gain(SoapySDRDevice *dev, size_t channel, const char *gain_str);
@@ -54,4 +55,12 @@ long long sdr_device_rate(SoapySDRDevice *dev, size_t channel, long long rate);
 int device_resampler(long long device_rate, long long rate, long long span, rxb200_resampler *rs);
 /* the capture samples the device samples [n0, n0 + c) emit through an L/N resampler */
 size_t resample_out_count(int up, int down, unsigned long long n0, size_t c);
+
+/* Capture in the device's own sample format (RXB200_DEVICE_FORMAT, DESIGN.md section 4.8).
+ * device_format_env: the variable's value as RXB200_IN_CS16, _CS8, _CU8 or _CS12, with its SoapySDR format name at
+ * *name; RXB200_IN_CS16 and SOAPY_SDR_CS16 when it is unset; -1, reported on stderr, when it is set but `allowed` is 0
+ * (none of the variables named by `needs` is set) or it is not one of CS16, CS8, CU8, CS12. */
+int device_format_env(int allowed, const char *needs, const char **name);
+/* bytes per complex element of an RXB200_IN_* format */
+size_t device_format_bytes(int in_fmt);
 #endif

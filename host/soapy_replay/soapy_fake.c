@@ -12,7 +12,7 @@
  *      at that rate: setSampleRate records the request, getSampleRate returns rate and listSampleRates {rate}.  Without
  *      it getSampleRate returns the last request (a device that honours any rate).
  *
- * Behaviour that matters: readStream (copies the next numElems CS16 complex elements,
+ * Behaviour that matters: readStream (copies the next numElems complex elements of the stream's format,
  * returns the count, SOAPY_SDR_TIMEOUT... never; returns -2 STREAM_ERROR at end of data so
  * the reference's dongle thread terminates), set/getFrequency (remembers the last value so
  * rx_power's retune() logic runs as on hardware), set/getSampleRate, formatToSize, getNumChannels.
@@ -29,7 +29,7 @@ struct SoapySDRDevice {
 	const int16_t *mem;     /* the capture: interleaved CS16 (or raw bytes of another element format, see elem_size) */
 	size_t n_complex;       /* total complex elements available */
 	size_t n_bytes;         /* the same capture in bytes (file replay) */
-	size_t elem_size;       /* bytes per complex element of the stream format: 4 (CS16) unless setupStream said CS12 (3) */
+	size_t elem_size;       /* bytes per complex element of the stream format: 4 (CS16), 3 (CS12), 2 (CS8, CU8) */
 	size_t pos;             /* next complex element */
 	int loop;
 	int owns_mem;
@@ -181,10 +181,12 @@ SoapySDRStream *SoapySDRDevice_setupStream(SoapySDRDevice *d, const int dir, con
 {
 	(void)d; (void)dir; (void)channels; (void)numChans; (void)args;
 	/* CS16 is what rx_fm / rx_power ask for; rx_sdr may also ask for the packed 12-bit format (-I CS12,
-	 * src/rtl_sdr.c:352-362): the capture file is then taken as 3-byte elements */
+	 * src/rtl_sdr.c:352-362), and any shell for a device's own CS8, CU8 or CS12 (RXB200_DEVICE_FORMAT): the capture
+	 * file is then taken as raw 3-byte (CS12) or 2-byte (CS8, CU8) elements */
 	if (format && strcmp(format, SOAPY_SDR_CS12) == 0) { g_dev.elem_size = 3; }
 	else if (format && strcmp(format, SOAPY_SDR_CS16) == 0) { g_dev.elem_size = 4; }
-	else { g_err = "fake: only CS16 and CS12"; return NULL; }
+	else if (format && (strcmp(format, SOAPY_SDR_CS8) == 0 || strcmp(format, SOAPY_SDR_CU8) == 0)) { g_dev.elem_size = 2; }
+	else { g_err = "fake: only CS16, CS12, CS8 and CU8"; return NULL; }
 	if (g_dev.n_bytes) { g_dev.n_complex = g_dev.n_bytes / g_dev.elem_size; }
 	return &g_stream;
 }

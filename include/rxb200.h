@@ -815,16 +815,24 @@ int rxb200_power_mix_accumulate_burst_device(rxb200_power_mix *m, int hop_begin,
  *   RXB200_CVT_CS16_CU8  : (uint8_t)(x/32767.0*128.0+127.4)           per int16 (:375-378)
  *   RXB200_CVT_CS16_CF32 : x * 1.0f / SHRT_MAX                        per int16 (:383-386)
  *   RXB200_CVT_CS12_CS16 : 3 packed bytes -> (I, Q) int16             per complex element (:354-362)
+ * and the widening of a device's 8-bit formats, the input stage of the capture handles ("capture handles in a device's
+ * own format" below), exact, per byte b:
+ *   RXB200_CVT_CS8_CS16  : (int16)((int8)b << 8)
+ *   RXB200_CVT_CU8_CS16  : (int16)(((int)b - 128) << 8)
+ * (4 is RXB200_SDR_OUT_CS16, an rx_sdr output format, and no conversion.)
  * n_elems counts COMPLEX elements.  Host pointers; bandwidth-bound, one kernel. */
 #define RXB200_CVT_CS16_CS8  0
 #define RXB200_CVT_CS16_CU8  1
 #define RXB200_CVT_CS16_CF32 2
 #define RXB200_CVT_CS12_CS16 3
+#define RXB200_CVT_CS8_CS16  5
+#define RXB200_CVT_CU8_CS16  6
 int rxb200_sdr_convert(int kind, const void *src, size_t n_elems, void *dst, int device);
 /* Same with device pointers on `stream` (a cudaStream_t, may be NULL).  Asynchronous.  Alignment, else RXB200_EINVAL
  * before any CUDA call:
  *   RXB200_CVT_CS16_CS8, _CS16_CU8, _CS16_CF32 : d_src and d_dst 16-byte aligned
- *   RXB200_CVT_CS12_CS16                       : d_dst 4-byte aligned (one 32-bit store per element); d_src any */
+ *   RXB200_CVT_CS12_CS16, _CS8_CS16, _CU8_CS16 : d_dst 4-byte aligned (one 32-bit store per element); d_src any (16-byte
+ *                                                vectors when both are 16-byte aligned) */
 int rxb200_sdr_convert_device(int kind, const void *d_src, size_t n_elems, void *d_dst, void *stream);
 
 /* ---- rx_sdr channels of one capture (DESIGN.md section 4.6)
@@ -1024,6 +1032,39 @@ int rxb200_resample_in_len(int up, int down, unsigned long long n0, size_t n_out
 int rxb200_fm_mix_set_device_rate(rxb200_fm_mix *m, const rxb200_resampler *rs);
 int rxb200_sdr_mix_set_device_rate(rxb200_sdr_mix *m, const rxb200_resampler *rs);
 int rxb200_power_mix_set_device_rate(rxb200_power_mix *m, const rxb200_resampler *rs);
+
+/* ---- capture handles in a device's own format (DESIGN.md section 4.8)
+ * Many receivers deliver narrower samples than CS16: 8-bit signed I/Q (CS8), 8-bit unsigned (CU8) or packed 12-bit
+ * (CS12).  rxb200_fm_mix_set_input_format, rxb200_sdr_mix_set_input_format and rxb200_power_mix_set_input_format make
+ * every host and device entry of a capture handle of any kind (stream calls and bursts alike) take that format.  Each
+ * element is widened to one CS16 pair exactly, with no rounding:
+ *   RXB200_IN_CS16 : 4 bytes, unchanged (the default)
+ *   RXB200_IN_CS8  : 2 bytes, I and Q = (int16)((int8)b << 8)          (RXB200_CVT_CS8_CS16)
+ *   RXB200_IN_CU8  : 2 bytes, I and Q = (int16)(((int)b - 128) << 8)   (RXB200_CVT_CU8_CS16)
+ *   RXB200_IN_CS12 : 3 bytes b0 b1 b2, I = (int16)((b1 << 12) | (b0 << 4)), Q = (int16)((b2 << 8) | (b1 & 0xf0))
+ *                    (RXB200_CVT_CS12_CS16)
+ * A handle fed bytes b in format F gives exactly the bytes it gives when fed the widening of b as CS16, however the
+ * stream is cut into calls: the widening runs on the handle's stream into a CS16 scratch buffer in device memory (4
+ * bytes per sample of a call, or of a host call's group), ahead of everything else, and the resampler (when attached)
+ * and the front stage run on it unchanged.  A driver's own CS16 conversion (an RTL driver's lookup table, say) may
+ * differ from this rule; the handle matches the widened stream, not any driver.
+ * Lengths keep their meaning: n_int16 counts I and Q components, two per complex element, so a call's buffer holds
+ * n_int16 / 2 elements of the format (n_int16 bytes for CS8 and CU8, 3 n_int16 / 2 bytes for CS12), passed as the same
+ * const int16_t * (callers cast).  Every length helper (_max_output, _decimated_len, _burst_in_len,
+ * rxb200_resample_in_len) gives what it gives for CS16.  Device entries take a CS8, CU8 or CS12 capture at any byte
+ * address (CS16 keeps its 4-byte rule).  Host entries copy only the format's bytes to the device; the groups of a host
+ * call (RXB200_SDR_MIX_SCRATCH_BYTES, counting the upload and the widened samples) are cut at element boundaries, and
+ * the bytes are the same as with one group.  Reset keeps the format.  The format and the resampler are independent:
+ * set either first.  _kernel_ms includes the widening.
+ * Refusals, before any device work: RXB200_EINVAL for a NULL handle or an unknown format, and RXB200_EINVAL for a
+ * handle that has taken any sample since create or reset (as _set_device_rate).  A refused call changes nothing. */
+#define RXB200_IN_CS16 0
+#define RXB200_IN_CS8  1
+#define RXB200_IN_CU8  2
+#define RXB200_IN_CS12 3
+int rxb200_fm_mix_set_input_format(rxb200_fm_mix *m, int fmt);
+int rxb200_sdr_mix_set_input_format(rxb200_sdr_mix *m, int fmt);
+int rxb200_power_mix_set_input_format(rxb200_power_mix *m, int fmt);
 
 /* ---- capture plans at a device rate
  * The capture planners above with one more argument, the device rate R_dev (Hz) the shell's resampler starts from.

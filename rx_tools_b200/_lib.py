@@ -5,12 +5,33 @@ from __future__ import annotations
 import ctypes as C
 import os
 
+import numpy as np
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("RXB200_LIB", os.path.join(HERE, "librxb200.so"))   # override: A/B builds of the same ABI
 
 OK, EINVAL, ENODEV, ECUDA, ENOMEM, EUNSUPPORTED, ECAPACITY = 0, -1, -2, -3, -4, -5, -6
 ERR_NAMES = {EINVAL: "EINVAL", ENODEV: "ENODEV", ECUDA: "ECUDA", ENOMEM: "ENOMEM",
              EUNSUPPORTED: "EUNSUPPORTED", ECAPACITY: "ECAPACITY"}
+
+
+# the capture handles' input formats (rxb200_*_mix_set_input_format): bytes per complex element of each
+IN_CS16, IN_CS8, IN_CU8, IN_CS12 = 0, 1, 2, 3
+IN_FORMATS = {"CS16": IN_CS16, "CS8": IN_CS8, "CU8": IN_CU8, "CS12": IN_CS12}
+IN_ELEM_BYTES = {IN_CS16: 4, IN_CS8: 2, IN_CU8: 2, IN_CS12: 3}
+
+
+def in_array(x, fmt: int):
+    """A capture call's host buffer in input format fmt as one C array, and its n_int16 (two per complex element):
+    int16 for CS16, else the format's raw bytes (uint8)."""
+    if fmt == IN_CS16:
+        a = np.ascontiguousarray(x, dtype=np.int16).reshape(-1)
+        return a, a.size
+    a = np.ascontiguousarray(x, dtype=np.uint8).reshape(-1)
+    e = IN_ELEM_BYTES[fmt]
+    if a.size % e:
+        raise ValueError(f"{a.size} bytes are not whole {e}-byte elements")
+    return a, 2 * (a.size // e)
 
 
 class Rxb200Error(RuntimeError):
@@ -135,6 +156,7 @@ SYMBOLS = [
     "rxb200_fm_mix_set_device_rate", "rxb200_sdr_mix_set_device_rate", "rxb200_power_mix_set_device_rate",
     "rxb200_power_plan_capture", "rxb200_power_plan_capture_at", "rxb200_power_plan_tiles_at",
     "rxb200_power_mix_set_burst_device_rate", "rxb200_power_mix_burst_in_len",
+    "rxb200_fm_mix_set_input_format", "rxb200_sdr_mix_set_input_format", "rxb200_power_mix_set_input_format",
 ]
 
 _lib = None
@@ -334,6 +356,9 @@ def lib() -> C.CDLL:
     L.rxb200_fm_mix_set_device_rate.argtypes = [C.c_void_p, pr]
     L.rxb200_sdr_mix_set_device_rate.argtypes = [C.c_void_p, pr]
     L.rxb200_power_mix_set_device_rate.argtypes = [C.c_void_p, pr]
+    L.rxb200_fm_mix_set_input_format.argtypes = [C.c_void_p, C.c_int]
+    L.rxb200_sdr_mix_set_input_format.argtypes = [C.c_void_p, C.c_int]
+    L.rxb200_power_mix_set_input_format.argtypes = [C.c_void_p, C.c_int]
     L.rxb200_power_plan_capture.argtypes = [C.POINTER(PowerPlanC), C.c_longlong, C.POINTER(FmCapturePlanC), pint]
     L.rxb200_power_plan_capture_at.argtypes = [C.POINTER(PowerPlanC), C.c_longlong, C.c_longlong,
                                                C.POINTER(FmCapturePlanC), pint]

@@ -6,10 +6,12 @@
 // count, and so the rule that makes a recording's bytes independent of how the capture is cut into calls: each call's
 // kernels start at the count's phases, and commit advances the count and the histories.  A front with a resampler
 // attached (resample_stage.cuh) takes device-rate samples: each call resamples them to the capture first, and every
-// count below that takes a call's length counts device samples.  Its host code is in ddc.cu.
+// count below that takes a call's length counts device samples.  A front whose input format is not CS16
+// (input_stage.cuh) widens each call's elements to CS16 first, ahead of the resampler.  Its host code is in ddc.cu.
 #pragma once
 #include <algorithm>
 #include "ddc.cuh"
+#include "input_stage.cuh"
 #include "raster.cuh"
 #include "resample_stage.cuh"
 #include "two_stage.cuh"
@@ -28,6 +30,7 @@ struct CaptureFront {
 	uint32_t *d_y = nullptr; size_t y_cap = 0;   // two stages: the coarse rows (words)
 	cudaEvent_t ev0 = nullptr, ev1 = nullptr;    // around the front's kernels of the last call
 	ResampleStage rs;                            // from the device rate, once attached
+	InputStage in;                               // the input format, widened to CS16 ahead of rs
 
 	// The refusals of each kind, in the order the handles report them, then its host plan; no device work.  A single
 	// stage is its filter's check alone.
@@ -55,14 +58,18 @@ struct CaptureFront {
 	// Attaches the resampler, which only a front that has taken no sample since create or reset accepts (and only
 	// once); its refusals precede any device work
 	int set_device_rate(const rxb200_resampler *r);
+	// The input format (RXB200_IN_*), which only a front that has taken no sample since create or reset accepts; its
+	// refusals precede any device work
+	int set_input_format(int fmt);
 
-	// One call's front stage on the current device, ordered on st: the c device samples at src (a device pointer),
-	// resampled to the capture when a resampler is attached, to the out_len(c) outputs per channel of the n_ch channels
+	// One call's front stage on the current device, ordered on st: the c device samples at src (a device pointer, in
+	// the input format), widened to CS16 unless that is CS16, resampled to the capture when a resampler is attached, to the out_len(c) outputs per channel of the n_ch channels
 	// at dst, channel k's output u at element k * stride + u in rx_sdr format fmt (RXB200_SDR_OUT_CS16: the int16
 	// pair word); then the carry of the raw history.  ev0 and ev1 bracket the kernels.  Two stages run whenever the call has coarse outputs, since those advance the bins'
 	// histories even when no fine output falls in the call; the other kinds run when the call has outputs.  single
 	// launches a single stage from the DdcArgs<Mix> it is given, every field but mix filled (src, n_out and pos
-	// describe the capture).  ev0 and ev1 also bracket the resampler.  Nothing becomes live before commit(c).
+	// describe the capture).  ev0 and ev1 also bracket the widening and the resampler.  Nothing becomes live before
+	// commit(c).
 	template <typename Mix, typename Single>
 	int call(const int16_t *src, size_t c_dev, void *dst, long long stride, int fmt, int n_ch, cudaStream_t st,
 	         Single single)
@@ -71,8 +78,10 @@ struct CaptureFront {
 		const long long n = (long long)dec_len(c);
 		const long long r0 = (long long)(f.M - 1) - (long long)(pos % (unsigned long long)f.M);
 		RXB_CUDA(cudaEventRecord(ev0, st));
-		const uint32_t *x = nullptr;
-		int rc = rs.run(reinterpret_cast<const uint32_t *>(src), c_dev, st, &x);
+		const uint32_t *w = nullptr, *x = nullptr;
+		int rc = in.run(src, c_dev, st, &w);
+		if (rc != RXB200_OK) { return rc; }
+		rc = rs.run(w, c_dev, st, &x);
 		if (rc != RXB200_OK) { return rc; }
 		if (kind == TWO_STAGE) {
 			const unsigned long long M1 = (unsigned long long)f.M, ma = pos / M1;

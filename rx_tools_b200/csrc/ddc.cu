@@ -111,6 +111,15 @@ int CaptureFront::set_device_rate(const rxb200_resampler *r)
 	return rs.attach(r);
 }
 
+int CaptureFront::set_input_format(int fmt)
+{
+	if (pos != 0 || rs.pos != 0) {
+		set_error("an input format is set right after create or reset, before any sample");
+		return RXB200_EINVAL;
+	}
+	return in.set(fmt);
+}
+
 int CaptureFront::reset(cudaStream_t st)
 {
 	if (filtered()) {
@@ -120,12 +129,13 @@ int CaptureFront::reset(cudaStream_t st)
 	}
 	const int rc = rs.reset(st);
 	if (rc != RXB200_OK) { return rc; }
-	pos = 0;
+	pos = 0;                                     // the input format stays
 	return RXB200_OK;
 }
 
 void CaptureFront::release(cudaStream_t st)
 {
+	in.release();
 	rs.release();
 	f.release();
 	ts.release(st);

@@ -256,7 +256,8 @@ int mix_call(rxb200_fm_mix *m, const int16_t *cs16, size_t n_int16, size_t chunk
              size_t *n_pcm, int *chunk_result_len, bool read, bool device, int sync)
 {
 	if (!m) { set_error("null argument"); return RXB200_EINVAL; }
-	if (device && ((uintptr_t)cs16 & 3u) != 0) { set_error("d_cs16 must be 4-byte aligned"); return RXB200_EINVAL; }
+	// a CS8, CU8 or CS12 capture may sit at any byte address
+	if (device && ((uintptr_t)cs16 & 3u) != 0 && !m->fr.in.on()) { set_error("d_cs16 must be 4-byte aligned"); return RXB200_EINVAL; }
 	// with a resampler, the call's shape is that of its capture-rate output: one read of those samples, or its chunks
 	const bool rs = m->fr.rs.on();
 	if (rs && n_int16 % 2 != 0) { set_error("n_int16=%zu must be even", n_int16); return RXB200_EUNSUPPORTED; }
@@ -276,7 +277,8 @@ int mix_call(rxb200_fm_mix *m, const int16_t *cs16, size_t n_int16, size_t chunk
 	if (!device) {
 		RXB_CUDA(reserve(m->d_cap, m->cap_cap, n_int16));
 		if (n16) { RXB_CUDA(reserve(m->d_out, m->out_cap, (total + 8) * K)); }
-		RXB_CUDA(cudaMemcpyAsync(m->d_cap, cs16, n_int16 * sizeof(int16_t), cudaMemcpyHostToDevice, st));
+		const size_t bytes = m->fr.in.on() ? m->fr.in.bytes(c) : n_int16 * sizeof(int16_t);   // the format's bytes
+		RXB_CUDA(cudaMemcpyAsync(m->d_cap, cs16, bytes, cudaMemcpyHostToDevice, st));
 		src = m->d_cap;
 	}
 	rc = m->fr.call<TabMix>(src, c, m->d_mix, (long long)(n16 / 2), RXB200_SDR_OUT_CS16, m->n_channels, st,
@@ -452,6 +454,12 @@ extern "C" int rxb200_fm_mix_set_device_rate(rxb200_fm_mix *m, const rxb200_resa
 	if (!m) { set_error("null argument"); return RXB200_EINVAL; }
 	RXB_CUDA(cudaSetDevice(m->device));
 	return m->fr.set_device_rate(rs);
+}
+
+extern "C" int rxb200_fm_mix_set_input_format(rxb200_fm_mix *m, int fmt)
+{
+	if (!m) { set_error("null argument"); return RXB200_EINVAL; }
+	return m->fr.set_input_format(fmt);
 }
 
 extern "C" int rxb200_fm_mix_decimated_len(const rxb200_fm_mix *m, size_t n_int16, size_t *n_dec_int16)

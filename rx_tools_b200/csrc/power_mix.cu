@@ -5,13 +5,15 @@
 // kernel is ddc.cuh's down-converter with its NCO mixer (NcoMix).  The handle carries the sample count (the NCO phases)
 // and its filter state (DdcFilter) between calls.  A burst (a fresh capture after a retune, for a tile of a wide sweep)
 // runs the same kernel on a subset of the hops, with its history read from the burst's own lead and its phases counted
-// from its first sample, and leaves the carried state alone.
+// from its first sample, and leaves the carried state alone.  A handle whose input format is not CS16 (input_stage.cuh)
+// widens each call's elements, stream or burst, to CS16 first.
 #include <math.h>
 #include <algorithm>
 #include <cstring>
 #include <new>
 #include <vector>
 #include "common.cuh"
+#include "input_stage.cuh"
 #include "resample_stage.cuh"
 
 namespace rxb {
@@ -64,6 +66,8 @@ struct rxb200_power_mix {
 	unsigned long long pos = 0;                  // capture samples since create or reset (whole passes)
 	ResampleStage rs;                            // from the device rate, once attached
 	bool burst_rate = false;                     // rs resamples bursts only (set_burst_device_rate), statelessly
+	InputStage in;                               // the input format, widened to CS16 ahead of rs
+	bool taken = false;                          // a call (stream or burst) has taken samples since create or reset
 	int16_t *d_cap = nullptr; size_t cap_cap = 0;     // host calls: the capture (int16 elements)
 	int16_t *d_bufs = nullptr; size_t bufs_cap = 0;   // the hop buffers of one group of passes, [P][he - hb][buf_len]
 	std::vector<cudaEvent_t> ev;                 // pairs around each DDC launch of the last call
@@ -77,6 +81,7 @@ extern "C" void rxb200_power_mix_destroy(rxb200_power_mix *m)
 	cudaSetDevice(m->device);
 	m->f.release();
 	m->rs.release();
+	m->in.release();
 	m->nco.release();
 	cudaFree(m->d_cap); cudaFree(m->d_bufs);
 	for (cudaEvent_t e : m->ev) { cudaEventDestroy(e); }
@@ -121,6 +126,7 @@ extern "C" int rxb200_power_mix_reset(rxb200_power_mix *m)
 	if (rc == RXB200_OK) { rc = m->rs.reset((cudaStream_t)rxb200_power_stream(m->h)); }
 	if (rc != RXB200_OK) { return rc; }
 	m->pos = 0;
+	m->taken = false;                            // the input format stays
 	return RXB200_OK;
 }
 
@@ -133,6 +139,13 @@ extern "C" int rxb200_power_mix_set_device_rate(rxb200_power_mix *m, const rxb20
 	}
 	RXB_CUDA(cudaSetDevice(m->device));
 	return m->rs.attach(rs);
+}
+
+extern "C" int rxb200_power_mix_set_input_format(rxb200_power_mix *m, int fmt)
+{
+	if (!m) { set_error("null argument"); return RXB200_EINVAL; }
+	if (m->taken) { set_error("an input format is set right after create or reset, before any sample"); return RXB200_EINVAL; }
+	return m->in.set(fmt);
 }
 
 extern "C" int rxb200_power_mix_set_burst_device_rate(rxb200_power_mix *m, const rxb200_resampler *rs)
@@ -169,12 +182,13 @@ int power_mix_call(rxb200_power_mix *m, int hb, int he, const int16_t *cs16, siz
 		set_error("hop range [%d, %d) needs 0 <= hop_begin < hop_end <= n_hops = %d", hb, he, m->n_hops);
 		return RXB200_EINVAL;
 	}
-	if (device && ((uintptr_t)cs16 & 3u) != 0) { set_error("d_cs16 must be 4-byte aligned"); return RXB200_EINVAL; }
+	// a CS8, CU8 or CS12 capture may sit at any byte address
+	if (device && ((uintptr_t)cs16 & 3u) != 0 && !m->in.on()) { set_error("d_cs16 must be 4-byte aligned"); return RXB200_EINVAL; }
 	// rs: this call is resampled, a stream call on a handle with a device rate or a burst on one with a burst device
 	// rate; a burst is resampled statelessly, so its first `skip` outputs (E) are dropped
 	const bool rs = m->rs.on() && burst == m->burst_rate;
 	if (m->rs.on() && burst && !rs) { set_error("a burst is a capture-rate capture: a handle with a device rate takes none"); return RXB200_EUNSUPPORTED; }
-	if (rs && n_int16 % 2 != 0) { set_error("n_int16=%zu must be even", n_int16); return RXB200_EUNSUPPORTED; }
+	if ((rs || m->in.on()) && n_int16 % 2 != 0) { set_error("n_int16=%zu must be even", n_int16); return RXB200_EUNSUPPORTED; }
 	const size_t dev16 = n_int16;                  // with a resampler, the call's device int16; n_int16 its capture's
 	const size_t skip = rs && burst ? burst_skip(m->rs) : 0;
 	if (rs) {
@@ -199,7 +213,8 @@ int power_mix_call(rxb200_power_mix *m, int hb, int he, const int16_t *cs16, siz
 	RXB_CUDA(cudaSetDevice(m->device));
 	const cudaStream_t st = (cudaStream_t)rxb200_power_stream(m->h);
 	RXB_CUDA(reserve(m->d_bufs, m->bufs_cap, group * hops * L));
-	const size_t n_groups = (n_pass + group - 1) / group + (rs ? 1 : 0);   // and a pair around the resampler
+	// and a pair around the widening and one around the resampler
+	const size_t n_groups = (n_pass + group - 1) / group + (m->in.on() ? 1 : 0) + (rs ? 1 : 0);
 	while (m->ev.size() < 2 * n_groups) {
 		cudaEvent_t e = nullptr;
 		RXB_CUDA(cudaEventCreate(&e));
@@ -208,16 +223,27 @@ int power_mix_call(rxb200_power_mix *m, int hb, int he, const int16_t *cs16, siz
 	const int16_t *src = cs16;
 	if (!device) {
 		RXB_CUDA(reserve(m->d_cap, m->cap_cap, dev16));
-		RXB_CUDA(cudaMemcpyAsync(m->d_cap, cs16, dev16 * sizeof(int16_t), cudaMemcpyHostToDevice, st));
+		const size_t bytes = m->in.on() ? m->in.bytes(dev16 / 2) : dev16 * sizeof(int16_t);   // the format's bytes
+		RXB_CUDA(cudaMemcpyAsync(m->d_cap, cs16, bytes, cudaMemcpyHostToDevice, st));
 		src = m->d_cap;
 	}
 	m->n_ev = 0;
-	if (rs) {                                      // the whole call to the capture, ahead of the groups that read it
-		const uint32_t *x = nullptr;
+	m->taken = true;
+	if (m->in.on()) {                              // the whole call to CS16, ahead of everything that reads it
+		const uint32_t *w = nullptr;
 		RXB_CUDA(cudaEventRecord(m->ev[0], st));
-		int rc = m->rs.run(reinterpret_cast<const uint32_t *>(src), dev16 / 2, st, &x);
+		int rc = m->in.run(src, dev16 / 2, st, &w);
 		if (rc != RXB200_OK) { return rc; }
 		RXB_CUDA(cudaEventRecord(m->ev[1], st));
+		m->n_ev++;
+		src = reinterpret_cast<const int16_t *>(w);
+	}
+	if (rs) {                                      // the whole call to the capture, ahead of the groups that read it
+		const uint32_t *x = nullptr;
+		RXB_CUDA(cudaEventRecord(m->ev[(size_t)2 * m->n_ev], st));
+		int rc = m->rs.run(reinterpret_cast<const uint32_t *>(src), dev16 / 2, st, &x);
+		if (rc != RXB200_OK) { return rc; }
+		RXB_CUDA(cudaEventRecord(m->ev[(size_t)2 * m->n_ev + 1], st));
 		m->n_ev++;
 		if (!burst) { m->rs.commit(dev16 / 2); }    // a burst leaves the stage at count 0 with its zero history
 		src = reinterpret_cast<const int16_t *>(x + skip);

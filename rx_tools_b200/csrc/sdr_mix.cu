@@ -37,7 +37,7 @@ struct rxb200_sdr_mix {
 	cudaStream_t st = nullptr;                   // every launch and copy of the handle
 	CaptureFront fr;                             // the front stage (its events: around the kernels of the last group)
 	NcoBank nco;                                 // single stage: the NCO table and each channel's word
-	int16_t *d_cap = nullptr; size_t cap_cap = 0;         // host calls: the capture (int16 elements)
+	int16_t *d_cap = nullptr; size_t cap_cap = 0;         // host calls: the capture in its format (int16 elements)
 	unsigned char *d_out = nullptr; size_t out_cap = 0;   // host calls: the output rows (bytes)
 };
 
@@ -53,7 +53,8 @@ int check_call(const rxb200_sdr_mix *m, const int16_t *cs16, size_t n_int16, int
 	if (!good_format(fmt)) { set_error("output format %d: need RXB200_SDR_OUT_CS16 or RXB200_CVT_CS16_CS8/CU8/CF32", fmt); return RXB200_EINVAL; }
 	if (n_int16 % 2 != 0) { set_error("n_int16=%zu must be even", n_int16); return RXB200_EINVAL; }
 	const size_t E = (size_t)sdr_elem_bytes(fmt), align = std::min<size_t>(E, 4);
-	if (device && (((uintptr_t)cs16 & 3u) || ((uintptr_t)out & (align - 1)))) {
+	// a CS8, CU8 or CS12 capture may sit at any byte address
+	if (device && ((((uintptr_t)cs16 & 3u) && !m->fr.in.on()) || ((uintptr_t)out & (align - 1)))) {
 		set_error("d_cs16 must be 4-byte aligned and d_out %zu-byte aligned", align);
 		return RXB200_EINVAL;
 	}
@@ -90,21 +91,23 @@ int device_call(rxb200_sdr_mix *m, const int16_t *src, size_t c, int fmt, void *
 }
 
 // device samples per group of a host call: what a group stages fits RXB200_SDR_MIX_SCRATCH_BYTES.  Without a
-// resampler that is the capture and the output rows, a multiple of M and at least M; with one, the device-rate upload
-// (4 bytes per device sample), the resampled capture (4 bytes per capture sample, L/N of them) and the output rows, at
-// least one device sample.  Each group is a device_call, which commits when it succeeds, as rx_power's groups do
+// resampler that is the capture and the output rows, a multiple of M and at least M; with one, the device-rate upload,
+// the resampled capture (4 bytes per capture sample, L/N of them) and the output rows, at least one device sample.  The
+// upload is b bytes per device sample: 4 for CS16, else the format's bytes and the 4 of its widening.  Each group is a
+// device_call, which commits when it succeeds, as rx_power's groups do
 // (DdcFilter): the next group reads the history the last one left.  *gn: a bound on a group's outputs per channel at
 // any phase.
 size_t host_group(const rxb200_sdr_mix *m, int fmt, size_t *gn)
 {
 	const size_t M = m->fr.decim(), rows = (size_t)m->n_ch * (size_t)sdr_elem_bytes(fmt);   // row bytes per M samples
 	const ResampleStage &rs = m->fr.rs;
-	size_t g = M * std::max<size_t>(1, (size_t)RXB200_SDR_MIX_SCRATCH_BYTES / (4 * M + rows));
+	const size_t b = m->fr.in.on() ? m->fr.in.bytes(1) + 4 : 4;
+	size_t g = M * std::max<size_t>(1, (size_t)RXB200_SDR_MIX_SCRATCH_BYTES / (b * M + rows));
 	if (rs.on()) {
-		// gd device samples take gd (4 + (4 M + rows) L / (N M)) bytes
+		// gd device samples take gd (b + (4 M + rows) L / (N M)) bytes
 		typedef unsigned __int128 u128;
 		const u128 S = RXB200_SDR_MIX_SCRATCH_BYTES, L = (u128)rs.L, N = (u128)rs.N, Mw = (u128)M;
-		g = std::max<size_t>(1, (size_t)(S * N * Mw / (4 * N * Mw + (4 * Mw + (u128)rows) * L)));
+		g = std::max<size_t>(1, (size_t)(S * N * Mw / ((u128)b * N * Mw + (4 * Mw + (u128)rows) * L)));
 	}
 	*gn = rs.max_out(g) / M + 1;
 	return g;
@@ -197,6 +200,12 @@ extern "C" int rxb200_sdr_mix_set_device_rate(rxb200_sdr_mix *m, const rxb200_re
 	return m->fr.set_device_rate(rs);
 }
 
+extern "C" int rxb200_sdr_mix_set_input_format(rxb200_sdr_mix *m, int fmt)
+{
+	if (!m) { set_error("null argument"); return RXB200_EINVAL; }
+	return m->fr.set_input_format(fmt);
+}
+
 extern "C" int rxb200_sdr_mix_decimated_len(const rxb200_sdr_mix *m, size_t n_int16, size_t *n_out)
 {
 	if (!m || !n_out) { set_error("null argument"); return RXB200_EINVAL; }
@@ -230,12 +239,14 @@ extern "C" int rxb200_sdr_mix_process(rxb200_sdr_mix *m, const int16_t *cs16, si
 		RXB_CUDA(cudaSetDevice(m->device));
 		size_t gn = 0;                                             // outputs per channel of a group at any phase
 		const size_t E = (size_t)sdr_elem_bytes(format), g = host_group(m, format, &gn), c = n_int16 / 2;
-		RXB_CUDA(reserve(m->d_cap, m->cap_cap, 2 * std::min(g, c)));
+		const InputStage &in = m->fr.in;
+		RXB_CUDA(reserve(m->d_cap, m->cap_cap, (in.bytes(std::min(g, c)) + 1) / 2));
 		RXB_CUDA(reserve(m->d_out, m->out_cap, (size_t)m->n_ch * gn * E));
 		size_t done = 0;                                      // outputs per channel written so far
 		for (size_t s = 0; s < c; s += g) {
 			const size_t cg = std::min(g, c - s), ng = m->fr.out_len(cg);
-			RXB_CUDA(cudaMemcpyAsync(m->d_cap, cs16 + 2 * s, cg * 2 * sizeof(int16_t), cudaMemcpyHostToDevice, m->st));
+			RXB_CUDA(cudaMemcpyAsync(m->d_cap, reinterpret_cast<const unsigned char *>(cs16) + in.bytes(s), in.bytes(cg),
+			                         cudaMemcpyHostToDevice, m->st));
 			rc = device_call(m, m->d_cap, cg, format, m->d_out, gn);
 			if (rc != RXB200_OK) { return rc; }
 			if (ng) {

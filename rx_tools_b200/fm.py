@@ -477,6 +477,18 @@ class FmMix(_OneGpu):
         _lib.check(_lib.lib().rxb200_fm_mix_set_device_rate(self._h, C.byref(rs)))
         self._up_down = (int(up), int(down))
 
+    def set_input_format(self, fmt) -> None:
+        """The capture's format right after create or reset (``rxb200_fm_mix_set_input_format``): ``_lib.IN_*`` or its
+        name.  From then on every call takes the format's raw bytes (uint8) for CS8, CU8 and CS12, widened to CS16 on
+        the GPU; n_int16 still counts two per complex element."""
+        fmt = _lib.IN_FORMATS.get(fmt, fmt)
+        _lib.check(_lib.lib().rxb200_fm_mix_set_input_format(self._h, fmt))
+        self._in_fmt = fmt
+
+    def _input(self, cs16):
+        x, n_int16 = _lib.in_array(cs16, getattr(self, "_in_fmt", _lib.IN_CS16))
+        return x, n_int16, False
+
     def _capture_int16(self, n_int16: int) -> int:
         L, N = getattr(self, "_up_down", (1, 1))
         return 2 * -(-(n_int16 // 2) * L // N)

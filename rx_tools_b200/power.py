@@ -231,9 +231,9 @@ class PowerMix(PowerScanner):
         return int(self.ddc[0]) * self.plan.buf_len
 
     def accumulate(self, capture: np.ndarray) -> None:
-        """capture: int16 CS16 (host), a whole number of passes."""
-        x = np.ascontiguousarray(capture, dtype=np.int16).reshape(-1)
-        _lib.check(_lib.lib().rxb200_power_mix_accumulate(self._m, x.ctypes.data, x.size))
+        """capture: int16 CS16 (host), a whole number of passes; uint8 bytes after set_input_format(CS8, CU8, CS12)."""
+        x, n_int16 = _lib.in_array(capture, getattr(self, "_in_fmt", _lib.IN_CS16))
+        _lib.check(_lib.lib().rxb200_power_mix_accumulate(self._m, x.ctypes.data, n_int16))
 
     def accumulate_device(self, d_ptr: int, n_int16: int, sync: bool = False) -> None:
         _lib.check(_lib.lib().rxb200_power_mix_accumulate_device(self._m, d_ptr, n_int16, 1 if sync else 0))
@@ -250,6 +250,14 @@ class PowerMix(PowerScanner):
         from .resample import _rs_c
         rs, _t = _rs_c(up, down, taps, shift)
         _lib.check(_lib.lib().rxb200_power_mix_set_device_rate(self._m, C.byref(rs)))
+
+    def set_input_format(self, fmt) -> None:
+        """The capture's format right after create or reset (``rxb200_power_mix_set_input_format``): ``_lib.IN_*`` or
+        its name.  From then on every accumulate and burst takes the format's raw bytes (uint8) for CS8, CU8 and CS12,
+        widened to CS16 on the GPU; n_int16 still counts two per complex element."""
+        fmt = _lib.IN_FORMATS.get(fmt, fmt)
+        _lib.check(_lib.lib().rxb200_power_mix_set_input_format(self._m, fmt))
+        self._in_fmt = fmt
 
     def set_burst_device_rate(self, up: int, down: int, taps, shift: int = 15) -> None:
         """Attach a resampler for bursts only, right after create or reset (``rxb200_power_mix_set_burst_device_rate``):
@@ -288,8 +296,8 @@ class PowerMix(PowerScanner):
     def accumulate_burst(self, hop_begin: int, hop_end: int, capture: np.ndarray) -> None:
         """One burst (host int16 CS16: the lead, then whole passes) for hops [hop_begin, hop_end).  The handle's
         carried phases and filter history are left as they are."""
-        x = np.ascontiguousarray(capture, dtype=np.int16).reshape(-1)
-        _lib.check(_lib.lib().rxb200_power_mix_accumulate_burst(self._m, hop_begin, hop_end, x.ctypes.data, x.size))
+        x, n_int16 = _lib.in_array(capture, getattr(self, "_in_fmt", _lib.IN_CS16))
+        _lib.check(_lib.lib().rxb200_power_mix_accumulate_burst(self._m, hop_begin, hop_end, x.ctypes.data, n_int16))
 
     def accumulate_burst_device(self, hop_begin: int, hop_end: int, d_ptr: int, n_int16: int,
                                 sync: bool = False) -> None:

@@ -97,6 +97,14 @@ class SdrMix:
         rs, _t = _rs_c(up, down, taps, shift)
         _lib.check(_lib.lib().rxb200_sdr_mix_set_device_rate(self._h, C.byref(rs)))
 
+    def set_input_format(self, fmt) -> None:
+        """The capture's format right after create or reset (``rxb200_sdr_mix_set_input_format``): ``_lib.IN_*`` or its
+        name.  From then on every call takes the format's raw bytes (uint8) for CS8, CU8 and CS12, widened to CS16 on
+        the GPU; n_int16 still counts two per complex element."""
+        fmt = _lib.IN_FORMATS.get(fmt, fmt)
+        _lib.check(_lib.lib().rxb200_sdr_mix_set_input_format(self._h, fmt))
+        self._in_fmt = fmt
+
     def decimated_len(self, n_int16: int) -> int:
         n = C.c_size_t(0)
         _lib.check(_lib.lib().rxb200_sdr_mix_decimated_len(self._h, n_int16, C.byref(n)))
@@ -105,11 +113,11 @@ class SdrMix:
     def process(self, cs16: np.ndarray, fmt=OUT_CS16) -> np.ndarray:
         """One host call: the capture's outputs, [n_channels][2 n_out] of the format's component type."""
         fmt = FORMATS.get(fmt, fmt)
-        x = np.ascontiguousarray(cs16, dtype=np.int16).reshape(-1)
-        n = self.decimated_len(x.size)
+        x, n_int16 = _lib.in_array(cs16, getattr(self, "_in_fmt", _lib.IN_CS16))
+        n = self.decimated_len(n_int16)
         out = np.zeros((self.n_channels, 2 * max(n, 1)), dtype=DTYPES[fmt])
         got = C.c_size_t(0)
-        _lib.check(_lib.lib().rxb200_sdr_mix_process(self._h, x.ctypes.data, x.size, fmt, out.ctypes.data, out.size // 2,
+        _lib.check(_lib.lib().rxb200_sdr_mix_process(self._h, x.ctypes.data, n_int16, fmt, out.ctypes.data, out.size // 2,
                                                      out.shape[1] // 2, C.byref(got)))
         assert got.value == n
         return out[:, :2 * n]
